@@ -1,5 +1,5 @@
 /*
- * ctcb200.h -- C ABI of libctcb200.so, the B200 (sm_100a) compute backend for the
+ * ctcb200.h -- C ABI of libctcb200.so, the H100 (sm_90a) compute backend for the
  * stanford-ctc training hot path (BRNN forward/backward + CTC alpha/beta + Nesterov SGD).
  *
  * Every entry point takes plain pointers and sizes (no torch types).  Unless a parameter is
@@ -7,10 +7,10 @@
  * the caller-supplied cudaStream_t (passed as void*).  Return value: 0 on success, a negative
  * CTCB_E* code otherwise, with a message retrievable from ctcb_last_error().  Numerical
  * infeasibility of one utterance (the reference's `skip=True`) is NOT an error: it is reported
- * per utterance in `skip_out`, as /root/reference/ctc_fast/ctc-loss/ctc_fast.pyx:147-149 does.
+ * per utterance in `skip_out`, as ctc_fast/ctc-loss/ctc_fast.pyx:147-149 does.
  *
  * The reference interface each entry point replaces is cited as (file:line) relative to
- * /root/reference/.
+ * the original stanford-ctc checkout.
  */
 #ifndef CTCB200_H
 #define CTCB200_H
@@ -179,7 +179,8 @@ int ctcb_brnn_apply_l2_f32(ctcb_brnn *h, const float *params, float *grads, void
  * nnets/rnnet.py:112-116 [mode 0] and :162-177 [mode 1].
  * scratch: 256-byte aligned device memory, >= 4096 bytes (word 0 = error flag, cleared by the call); the tensor-core
  * kernel (H >= 1024, sweep_tc.cu) additionally needs room for the (hi, lo) stacks of the recurrent matrices and the
- * ring of state low halves: ctcb_brnn_sweep_workspace_bytes(H, B) in total, else the FFMA kernels run. */
+ * ring of state low halves: ctcb_brnn_sweep_workspace_bytes(H, B) in total; where that kernel applies
+ * (ctcb_sweep_uses_tensor_cores) a smaller scratch is an error (CTCB_ENOMEM), never a slower kernel. */
 size_t ctcb_brnn_sweep_workspace_bytes(int H, int B);
 int ctcb_brnn_sweep_f32(int mode, int T, int B, int H, const int32_t *T_per_utt, const float *pre,
                         const float *Wf, const float *Wb, float *outF, float *outB, const float *actF,

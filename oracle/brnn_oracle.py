@@ -1,23 +1,23 @@
 """oracle/brnn_oracle.py -- TEST INFRASTRUCTURE ONLY (checker + CPU baseline "port").
 
 NumPy restatement of the reference BRNN training step, per utterance, following line by line
-  /root/reference/ctc_fast/nnets/brnnet.py:10-32   (ctor; temporalLayer rule; maxAct = 20)
-  /root/reference/ctc_fast/nnets/brnnet.py:34-86   (initParams: shapes and np.random draw order)
-  /root/reference/ctc_fast/nnets/brnnet.py:117-173 (forward; clipped-ReLU recurrences; softmax)
-  /root/reference/ctc_fast/nnets/brnnet.py:175-249 (CTC, L2 cost, back-prop / BPTT, L2 grad)
-  /root/reference/ctc_fast/nnets/brnnet.py:251-256 (updateParams)
-  /root/reference/ctc_fast/sgd.py:57-167           (Nesterov step, global-norm clip)
+  ctc_fast/nnets/brnnet.py:10-32   (ctor; temporalLayer rule; maxAct = 20)
+  ctc_fast/nnets/brnnet.py:34-86   (initParams: shapes and np.random draw order)
+  ctc_fast/nnets/brnnet.py:117-173 (forward; clipped-ReLU recurrences; softmax)
+  ctc_fast/nnets/brnnet.py:175-249 (CTC, L2 cost, back-prop / BPTT, L2 grad)
+  ctc_fast/nnets/brnnet.py:251-256 (updateParams)
+  ctc_fast/sgd.py:57-167           (Nesterov step, global-norm clip)
 cross-checked against the reference's own NumPy BRNN
-  /root/reference/ctc_fast/debug-utils/rnnetcpu.py:54-150 (same math without the 20-clip / L2).
+  ctc_fast/debug-utils/rnnetcpu.py:54-150 (same math without the 20-clip / L2).
 
 PINNED (round 2): tests/golden/rnnetcpu_ref.npz holds inputs/outputs of the reference's own
 rnnetcpu.RNNet.costAndGrad executed in the authoring container (tests/golden/gen_rnnetcpu_ref.py: the file as
-it lies in /root/reference, print/xrange/tabs converted mechanically, CTC = oracle/_ref); configured as that file
+it lies in the reference checkout, print/xrange/tabs converted mechanically, CTC = oracle/_ref); configured as that file
 computes (float64, no clip, no float32 hand-offs, no L2) this restatement reproduces cost and all gradients of
 5 shapes to 1e-12 (tests/test_oracle.py::test_brnn_restatement_pinned_to_reference_rnnetcpu).
 What brnnet.py adds on top of rnnetcpu.py -- the 20.0 clip / within() mask, the float32 hand-offs and L2 -- runs
 inside cudamat in the reference (fork github.com/awni/cudamat, no pinned version, source absent from
-/root/reference); for those three additions the restatement follows the call sites and is checked by finite
+the reference checkout); for those three additions the restatement follows the call sites and is checked by finite
 differences only.
 Semantics adopted from the call sites and rnnetcpu.py:
   mvdot_col_slice(W,src,i,dst,j,beta=1): dst[:,j] = beta*dst[:,j] + W.dot(src[:,i])

@@ -2,16 +2,18 @@
 
 TEST INFRASTRUCTURE ONLY (checker / CPU baseline) -- never imported by the product path.
 
-Compiles /root/reference/ctc_fast/ctc-loss/ctc_fast.pyx (ctc_loss :13-152, decode_best_path
-:154-187) and ctc_fast_blankforce.pyx (ctc_loss :13-113, decode_best_path :115-142) from where they lie; outputs (generated .c and the extension .so) go only into
-oracle/_ref/, which is git-ignored but ships to the GPU box with gpurun.
+Compiles <reference>/ctc_fast/ctc-loss/ctc_fast.pyx (ctc_loss :13-152, decode_best_path
+:154-187) and ctc_fast_blankforce.pyx (ctc_loss :13-113, decode_best_path :115-142) from where they lie, <reference>
+being the checkout of the original stanford-ctc project named by $CTC_REFERENCE_DIR; outputs (generated .c and the
+extension .so) go only into oracle/_ref/, which is git-ignored.  The tests do not need it (what they compare with is
+stored under tests/golden/); the golden generators and bench.py's CPU baseline do.
 
 The reference's own setup.py (ctc-loss/setup.py:1-8) uses the removed distutils/Cython.Distutils
 API, so this is the modern equivalent.  language_level=2 is required: the source uses xrange,
 a print statement, and C integer division in `l = (s-1)/2`.
 
-Usage:  python oracle/build_ref.py [--force]
-If /root/reference is absent (GPU box) this is a no-op: the prebuilt .so is used.
+Usage:  CTC_REFERENCE_DIR=<checkout> python oracle/build_ref.py [--force]
+Without the reference sources this is a no-op: an already built .so is used.
 """
 import os
 import subprocess
@@ -19,7 +21,7 @@ import sys
 import sysconfig
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REF_DIR = "/root/reference/ctc_fast/ctc-loss"
+REF_DIR = os.path.join(os.environ.get("CTC_REFERENCE_DIR", ""), "ctc_fast", "ctc-loss")
 REF_PYX = os.path.join(REF_DIR, "ctc_fast.pyx")
 MODULES = ("ctc_fast", "ctc_fast_blankforce")
 OUT_DIR = os.path.join(HERE, "_ref")
@@ -32,10 +34,14 @@ def so_path(name="ctc_fast"):
 def _build_one(name, force):
     so = so_path(name)
     pyx = os.path.join(REF_DIR, name + ".pyx")
-    if not os.path.exists(pyx):
+    if not os.environ.get("CTC_REFERENCE_DIR") or not os.path.exists(pyx):
         return so if os.path.exists(so) else None
     if os.path.exists(so) and not force and os.path.getmtime(so) >= os.path.getmtime(pyx):
         return so
+    import importlib.util
+    if importlib.util.find_spec("Cython") is None:
+        print("oracle/build_ref.py: Cython is not installed; %s not built" % name, file=sys.stderr)
+        return so if os.path.exists(so) else None
     import numpy as np
     c_file = os.path.join(OUT_DIR, name + ".c")
     subprocess.check_call([sys.executable, "-m", "cython", "-2", pyx, "-o", c_file])

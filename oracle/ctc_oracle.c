@@ -2,8 +2,8 @@
  * oracle/ctc_oracle.c -- TEST INFRASTRUCTURE ONLY (checker + CPU baseline "port").
  *
  * Plain-C float64 restatement of the reference CTC forward-backward,
- *   /root/reference/ctc_fast/ctc-loss/ctc_fast.pyx:13-152  (ctc_loss)
- *   /root/reference/ctc_fast/ctc-loss/ctc_fast.pyx:154-187 (decode_best_path)
+ *   ctc_fast/ctc-loss/ctc_fast.pyx:13-152  (ctc_loss)
+ *   ctc_fast/ctc-loss/ctc_fast.pyx:154-187 (decode_best_path)
  * Parity pinned: validated against the unmodified .pyx compiled into oracle/_ref/
  * (tests/test_oracle.py) and the known-answer value of ctc/time_trials.py:13-25
  * (NLL 1710.233966660).  Never linked or called by the product library.
@@ -145,7 +145,7 @@ int ctc_oracle_best_path(const double *probs, int K, int T, int blank, int *hyp,
 }
 
 /*
- * Blank-forced variant: /root/reference/ctc_fast/ctc-loss/ctc_fast_blankforce.pyx:13-113.
+ * Blank-forced variant: ctc_fast/ctc-loss/ctc_fast_blankforce.pyx:13-113.
  * `seq` already contains the blanks (:24-26): L = seqLen states, transitions s -> s and s -> s+1
  * only (:51-52), a single start state (:43) and a single end state (:64); every state enters the
  * per-frame normaliser (:55-59), so -llForward is the log of the total mass of ALL states at T-1.

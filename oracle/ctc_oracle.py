@@ -1,7 +1,7 @@
 """oracle/ctc_oracle.py -- TEST INFRASTRUCTURE ONLY.
 
 ctypes front-end of oracle/ctc_oracle.c (the float64 C restatement of
-/root/reference/ctc_fast/ctc-loss/ctc_fast.pyx:13-187 and ctc_fast_blankforce.pyx:13-142) plus a loader for oracle/_ref (the
+ctc_fast/ctc-loss/ctc_fast.pyx:13-187 and ctc_fast_blankforce.pyx:13-142) plus a loader for oracle/_ref (the
 reference's own .pyx compiled unmodified by oracle/build_ref.py).
 
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs may
@@ -23,7 +23,7 @@ def lib_path():
 
 
 def build(force=False):
-    """gcc the C restatement into oracle/_build/ (git-ignored, ships with gpurun)."""
+    """gcc the C restatement into oracle/_build/ (git-ignored)."""
     src = os.path.join(HERE, "ctc_oracle.c")
     out = lib_path()
     os.makedirs(os.path.dirname(out), exist_ok=True)
@@ -131,7 +131,7 @@ def ref_ctc_loss_blankforce(params, seq):
     """The unmodified ctc_fast_blankforce.ctc_loss; failure path mapped as in ref_ctc_loss."""
     mod = ref_module("ctc_fast_blankforce")
     if mod is None:
-        raise RuntimeError("oracle/_ref not built (run oracle/build_ref.py where /root/reference exists)")
+        raise RuntimeError("oracle/_ref not built (run oracle/build_ref.py with CTC_REFERENCE_DIR set)")
     try:
         nll, grad, skip = mod.ctc_loss(params, np.ascontiguousarray(seq, dtype=np.int32))
         return float(nll), grad, bool(skip)
@@ -145,7 +145,7 @@ def ref_ctc_loss(params, seq, blank=0):
     returning skip=True -- map that (and a bare ZeroDivisionError) to skip=True with zero grad."""
     mod = ref_module()
     if mod is None:
-        raise RuntimeError("oracle/_ref not built (run oracle/build_ref.py where /root/reference exists)")
+        raise RuntimeError("oracle/_ref not built (run oracle/build_ref.py with CTC_REFERENCE_DIR set)")
     try:
         nll, grad, skip = mod.ctc_loss(params, np.ascontiguousarray(seq, dtype=np.int32), blank)
         return float(nll), grad, bool(skip)

@@ -118,5 +118,5 @@ def current_stream():
 def require_cuda():
     import torch
     if not torch.cuda.is_available():
-        raise RuntimeError("stanford-ctc_b200 needs a CUDA device (B200, sm_100a); no CPU fallback exists")
+        raise RuntimeError("stanford-ctc_b200 needs a CUDA device (H100, sm_90a); no CPU fallback exists")
     return torch

@@ -1,6 +1,6 @@
 // brnn.cu -- batched costAndGrad of the bi-directional recurrent network, orchestrated on one stream.
 //
-// Replaces nnets.brnnet.NNet.costAndGrad (/root/reference/ctc_fast/nnets/brnnet.py:117-249), which
+// Replaces nnets.brnnet.NNet.costAndGrad (ctc_fast/nnets/brnnet.py:117-249), which
 // runs one utterance at a time as ~8(T-1)+12N+40 cudamat launches with a blocking D2H/H2D round
 // trip through the CPU CTC in the middle.  Here a whole minibatch of utterances is one pass:
 //
@@ -50,7 +50,6 @@ __global__ void colsum_stage1(const float *__restrict__ x, int64_t R, int N, flo
 }
 // the same for row pitches that are a multiple of 4 floats: a block walks FULL-WIDTH row segments (each thread a float4
 // column group), so consecutive warps read consecutive 512-byte pieces of a row instead of 128-byte strips 8 KB apart
-// (the strip version ran at 0.3 TB/s on the 3 GB delta arrays of C4: 51 ms per step; this one streams them)
 constexpr int CS_ROWS_MIN = 128;
 __global__ void colsum_stage1_wide(const float4 *__restrict__ x, int64_t R, int N4, int rows_per_block, float4 *__restrict__ partial) {
     const int c4 = blockIdx.x * blockDim.x + threadIdx.x;

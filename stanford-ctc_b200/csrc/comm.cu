@@ -1,8 +1,8 @@
 // comm.cu -- the data-parallel exchange step behind the C ABI: one communicator per process (one process per
-// GPU), the flat gradient (+ its 4-float statistics tail) summed over ranks with NCCL over NVLink 5 / NVSwitch.
+// GPU), the flat gradient (+ its 4-float statistics tail) summed over ranks with NCCL over NVLink / NVSwitch.
 //
 // The reference has no multi-GPU path at all: its only device hook is the CUDA_DEVICE variable
-// (/root/reference/ctc_fast/runNNet.py:117-120), and every utterance is a complete optimisation step
+// (ctc_fast/runNNet.py:117-120), and every utterance is a complete optimisation step
 // (sgd.py:70-161).  Utterances are independent until the update, so a step's minibatch is sharded over ranks and
 // this is the single exchange of the step (SURVEY.md 8b/8e: ctcb_allreduce_grads).
 //

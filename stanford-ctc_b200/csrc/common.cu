@@ -23,8 +23,8 @@ int num_sms() {
     static int n = 0;
     if (n == 0) {
         int dev = 0;
-        if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) n = 148;
+        if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) n = 132;
     }
     return n;
 }

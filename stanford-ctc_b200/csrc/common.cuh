@@ -1,4 +1,4 @@
-// common.cuh -- shared helpers for libctcb200 (sm_100a only).
+// common.cuh -- shared helpers for libctcb200 (H100, sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -1,5 +1,5 @@
 // ctc_blankforce.cu -- the blank-forced CTC loss/gradient of the reference as an option of the CTC path
-// (/root/reference/ctc_fast/ctc-loss/ctc_fast_blankforce.pyx:13-113).
+// (ctc_fast/ctc-loss/ctc_fast_blankforce.pyx:13-113).
 //
 // Differences from ctc.cu (ctc_fast.pyx): the label sequence arrives WITH its blanks, so the trellis has
 // L = len(seq) states, transitions s -> s and s -> s+1 only (:51-52, :73-74), one start state (:43) and one

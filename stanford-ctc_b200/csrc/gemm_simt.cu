@@ -284,7 +284,7 @@ extern "C" int ctcb_gemm_f32(int transA, int transB, int M, int N, int K, float 
                              int relu, const float *mask_src, void *workspace, size_t ws_bytes, void *stream) {
     if (M <= 0 || N <= 0) return CTCB_OK;
     if (!A || !B || !C || K < 0) return set_error(CTCB_EINVAL, "ctcb_gemm_f32: bad argument");
-    // large contractions: 3xTF32 on the tcgen05 tensor cores (gemm_tc.cu); small or odd ones: exact FFMA below
+    // large contractions: 3xTF32 on the wgmma tensor cores (gemm_tc.cu); small or odd ones: exact FFMA below
     if (gemm_tc_eligible(M, N, K) && workspace && ws_bytes >= gemm_tc_workspace_bytes(M, N, K))
         return run_gemm_tc(transA, transB, M, N, K, alpha, A, lda, B, ldb, beta, C, ldc, bias, relu, mask_src, workspace,
                            ws_bytes, (cudaStream_t)stream);

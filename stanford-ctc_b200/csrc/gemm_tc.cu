@@ -1,30 +1,24 @@
-// gemm_tc.cu -- fp32-faithful dense contraction on the 5th-generation tensor cores (tcgen05 + TMEM + TMA).
+// gemm_tc.cu -- fp32-faithful dense contraction on the Hopper tensor cores (wgmma + TMA + mbarrier).
 //
 // The reference multiplies in float32 (cudamat cm.dot -> legacy cuBLAS sgemm; call sites
-// ctc_fast/nnets/brnnet.py:140,196,204,227-230).  tcgen05 has no fp32 MMA, and a single TF32 pass
+// ctc_fast/nnets/brnnet.py:140,196,204,227-230).  The tensor cores have no fp32 MMA, and a single TF32 pass
 // (10-bit mantissa) would be a reduced-precision run, so every operand is split into two TF32 parts
-//     x = hi + lo,   hi = x with the low 13 mantissa bits cleared (what kind::tf32 reads from an fp32 word),
+//     x = hi + lo,   hi = x with the low 13 mantissa bits cleared (what a .tf32 MMA reads from an fp32 word),
 //                    lo = x - hi (exact in fp32; itself read as TF32)
-// and a product is three MMAs accumulated in fp32 in tensor memory:  lo.hi + hi.lo + hi.hi
+// and a product is three MMAs accumulated in fp32:  lo.hi + hi.lo + hi.hi
 // (the dropped lo.lo term is ~2^-20 relative) -- "3xTF32", ~1e-6 relative error per product.
 //
-// Kernel shape: C[M x N] = A[M x K] . B[N x K]^T.  One CTA (12 warps) per 128 x BN output tile and K split (gridDim.z):
-//   warp 0          : TMA producer -- per k-block of 32 floats the A and B tiles into a STAGES-deep shared-memory ring
-//                     (one box per K-major operand, boxes of {32 m, 32 k} for an MN-major one), mbarrier complete_tx;
-//   warps 4..7      : A splitters -- read each row of the landed A tile once and tcgen05.st its value and its low half
-//                     (lo = x - trunc_tf32(x)) into TENSOR MEMORY next to the accumulator;
-//   warps 8..11     : B splitters -- write B's low half in shared memory (element-wise, oblivious to the swizzle);
-//   warp 1          : MMA issuer  -- 4 k-steps x 3 tcgen05.mma.kind::tf32 (M=128, N=BN, K=8) per k-block, A from tensor
-//                     memory (.ts form), B by shared-memory descriptor; tcgen05.commit releases the ring slot;
-//   warps 0..3      : epilogue -- tcgen05.ld 32 lanes x 32 columns per warp, fused alpha/beta/bias/ReLU/mask (or split-K
-//                     partial), row stores.
-//   Producer and MMA warps run warp-uniform and issue from the elect.sync lane (see tc_elect_one).
-// The default tile is 128 wide with two CTAs per SM (2 x 256 tensor-memory columns, 2 x 96 KB of shared memory), so one
-// CTA's epilogue and pipeline fill run under the other's main loop.  CTCB_GEMM_TS=0 selects the round-1 form (both
-// operands and both low halves in shared memory, eight splitter warps).
-// Operands that are contracted over their ROW index (weight gradients, delta propagation) are fed MN-major as they lie;
-// only operands whose row pitch is not a multiple of 16 bytes are re-laid-out by a prep kernel.
+// Kernel shape: C[M x N] = A[M x K] . B[N x K]^T, both operands K-major (wgmma reads .tf32 operands K-major only; an
+// operand stored the other way round is transposed by a prep kernel first).  One CTA (3 warpgroups) per 128 x BN output
+// tile and K split (gridDim.z):
+//   warpgroup 0 : producer -- one elected thread TMA-loads the A and B tiles of each k-block of 32 floats into a
+//                 STAGES-deep ring (mbarrier complete_tx); the 128 threads then write the low halves of both tiles
+//                 next to them (element-wise, oblivious to the swizzle) and signal the consumers;
+//   warpgroups 1, 2 : consumers -- rows 0..63 / 64..127 of the tile: 4 k-steps x 3 wgmma (m64 x BN x k8) per k-block
+//                 with the accumulator in registers, one k-block in flight while the previous slot is released; then
+//                 the fused alpha/beta/bias/ReLU/mask epilogue (or the split-K partial) straight from registers.
 #include "common.cuh"
+#include "wgmma.cuh"
 #include <cuda.h>
 #include <stdlib.h>
 
@@ -32,11 +26,7 @@ namespace ctcb {
 
 constexpr int TC_BM = 128;
 constexpr int TC_BK = 32;   // 32 fp32 = 128 bytes = one swizzle span
-// Measured (tools/micro/umma_rate.cu + the per-phase trace of the recurrent sweep): a kind::tf32 MMA costs max(45, N/2)
-// cycles, i.e. 12 x 128 = 1536 cycles per k-block at BN = 256, while ONE warpgroup of splitters needed ~3000: the tensor
-// pipe sat at 25-50 %.  Two warpgroups, loads hoisted above the stores, bring the split under the MMA time.
-constexpr int TC_SPLIT_WARPS = 8;
-constexpr int TC_THREADS = 128 + 32 * TC_SPLIT_WARPS;
+constexpr int TC_THREADS = 384;
 
 static unsigned long long *g_gemm_trace = nullptr;     // CTCB_GEMM_TRACE: stamps of the LAST tensor-core GEMM launched
 
@@ -47,12 +37,6 @@ struct GemmTcArgs {
     const float *bias; int relu; const float *mask;
     float *partial;      // split-K partials [splits][M][N] or nullptr
     int kb_per_split;    // k-blocks per gridDim.z slice
-    int nmma;            // debug (CTCB_GEMM_MMAS): 3 = full 3xTF32, 1 = hi.hi only (plain TF32, for rate experiments)
-    int a_mn, b_mn;      // operand is MN-major in memory (stored K x M / K x N): fed to the tensor cores as it lies
-    int ts;              // 1: the A tile goes to the tensor cores THROUGH TENSOR MEMORY: four splitter warps read each row of
-                         //    the landed tile once and tcgen05.st its value and its low half next to the accumulator; the MMAs
-                         //    take A from there (.ts form).  Shared-memory traffic per k-block of a 256-wide tile falls from
-                         //    288 KB (the bound the round-2 trace showed, profiles/gemm_tc_trace_r2.txt) to 224 KB.
     unsigned long long *trace;   // optional (CTCB_GEMM_TRACE): [64 k-blocks][8] SM clock stamps of CTA (0,0,0)
 };
 #define TC_STAMP(i, slot)                                                                                       \
@@ -68,6 +52,9 @@ __device__ __forceinline__ void tc_mbar_init(uint32_t bar, uint32_t count) {
 }
 __device__ __forceinline__ void tc_mbar_expect_tx(uint32_t bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void tc_mbar_arrive(uint32_t bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
 __device__ __forceinline__ bool tc_mbar_try_wait(uint32_t bar, uint32_t parity) {
     uint32_t ok;
@@ -90,79 +77,6 @@ __device__ __forceinline__ void tc_tma_load_2d(uint32_t dst, const CUtensorMap *
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
                  ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1) : "memory");
 }
-__device__ __forceinline__ void tc_mma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tc_mma_tf32_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// 32 consecutive columns of the calling thread's tensor-memory lane
-__device__ __forceinline__ void tc_tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-        ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-          "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]),
-          "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]),
-          "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31]) : "memory");
-}
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// One lane of a converged warp: the producer and MMA loops run warp-uniform and only ISSUE from the elected lane.  Inside a
-// `lane == 0` branch the compiler wraps every UTCHMMA / UTMALDG / UTCBAR in an ELECT + R2UR.BROADCAST loop (69 cycles per
-// MMA issue, measured in sweep_tc.cu) -- slower than the 48-64 cycles an MMA of a 64- or 128-wide tile takes to execute.
-__device__ __forceinline__ bool tc_elect_one() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.b32 %0, 1, 0, P;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// UMMA shared-memory descriptor, K-major, SWIZZLE_128B: 8-row x 128-byte atoms 1024 bytes apart
-// (cute/arch/mma_sm100_desc.hpp SmemDescriptor: start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46),
-//  version=1 [46,48), layout_type=2 (SWIZZLE_128B) [61,64)).
-__device__ __forceinline__ uint64_t tc_smem_desc(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3ffff) >> 4);
-    d |= (uint64_t)1 << 16;                  // LBO (unused for swizzled K-major)
-    d |= (uint64_t)(1024 >> 4) << 32;        // SBO
-    d |= (uint64_t)1 << 46;                  // descriptor version (sm_100)
-    d |= (uint64_t)2 << 61;                  // SWIZZLE_128B
-    return d;
-}
-// MN-major operand (the M / N index is the contiguous one in memory).  For 32-bit operands the tensor cores accept
-// exactly one swizzled MN-major layout, SWIZZLE_128B_BASE32B (layout type 1; every other type makes the MMA read zeros --
-// probed with tools/micro/umma_layout_probe.cu, which also gave the address map): rows of 128 bytes hold 32 consecutive
-// M (N) values of one k; 4 k-rows form a 512-byte atom in which the 32-byte chunks are XOR-ed with the row index
-// (Swizzle<2,5,2>); the next 4 k are SBO bytes further, the next 32 M (N) values LBO bytes.  TMA's
-// CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B writes exactly this pattern, so a box of {32 m, 32 k} floats is four K = 8 MMA
-// steps 1024 bytes apart (SBO = 512 inside a step) and the boxes of a tile lie 4096 bytes apart (LBO).
-__device__ __forceinline__ uint64_t tc_smem_desc_mn(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3ffff) >> 4);
-    d |= (uint64_t)(4096 >> 4) << 16;        // LBO: next group of 32 along M / N
-    d |= (uint64_t)(512 >> 4) << 32;         // SBO: next group of 4 along K
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)1 << 61;                  // SWIZZLE_128B_BASE32B
-    return d;
-}
-// Instruction descriptor for kind::tf32 (InstrDescriptor): D=F32 [4,6)=1, A=TF32 [7,10)=2, B=TF32 [10,13)=2,
-// a_major [15] / b_major [16] (0 = K-major, 1 = MN-major), N>>3 at [17,23), M>>4 at [24,29).
-__host__ __device__ constexpr uint32_t tc_idesc(int m, int n, int a_mn = 0, int b_mn = 0) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(a_mn & 1) << 15) | ((uint32_t)(b_mn & 1) << 16) |
-           ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
-}
 
 __device__ __forceinline__ float tc_epilogue(const GemmTcArgs &g, float acc, int m, int n) {
     float v = g.alpha * acc;
@@ -173,26 +87,30 @@ __device__ __forceinline__ float tc_epilogue(const GemmTcArgs &g, float acc, int
     return v;
 }
 
-// TS = true: the A tile reaches the tensor cores through tensor memory, so a stage holds A once and B twice (value + low
-// half); TS = false: both operands from shared memory, A and B twice each.
-template <int BN, int STAGES, bool TS>
-__global__ void __launch_bounds__(TC_THREADS, (TS && BN == 128 && STAGES == 2) ? 2 : 1)     // 128-wide: two CTAs per SM
+__device__ __forceinline__ float4 tc_lo4(float4 v) {
+    float4 r;
+    r.x = v.x - __uint_as_float(__float_as_uint(v.x) & 0xffffe000u);
+    r.y = v.y - __uint_as_float(__float_as_uint(v.y) & 0xffffe000u);
+    r.z = v.z - __uint_as_float(__float_as_uint(v.z) & 0xffffe000u);
+    r.w = v.w - __uint_as_float(__float_as_uint(v.w) & 0xffffe000u);
+    return r;
+}
+
+// A stage holds [A value | A low half | B value | B low half], each tile 1024-byte aligned.
+template <int BN, int STAGES>
+__global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmTcArgs g) {
     constexpr uint32_t A_BYTES = TC_BM * TC_BK * 4, B_BYTES = BN * TC_BK * 4;
-    constexpr uint32_t B_OFF = TS ? A_BYTES : 2 * A_BYTES;                 // where B's value tile sits inside a stage
+    constexpr uint32_t B_OFF = 2 * A_BYTES;
     constexpr uint32_t STAGE_BYTES = B_OFF + 2 * B_BYTES;
-    // tensor-memory columns: the accumulator, then per stage 32 + 32 columns for the A tile (power of two)
-    constexpr uint32_t TMEM_COLS = !TS ? (uint32_t)BN : ((BN + 64 * STAGES) <= 128 ? 128u : ((BN + 64 * STAGES) <= 256 ? 256u : 512u));
-    static_assert(!TS || BN + 64 * STAGES <= 512, "accumulator + A stages exceed the tensor memory");
     extern __shared__ __align__(1024) uint8_t tc_smem[];
     // 1024-byte alignment is required by SWIZZLE_128B: align manually (dynamic smem base is only 16B-aligned by contract)
     uint8_t *base = (uint8_t *)(((uintptr_t)tc_smem + 1023) & ~(uintptr_t)1023);
-    // full[STAGES] (TMA landed), empty[STAGES] (MMAs done with the slot), done, ready[STAGES] (lo tiles written)
-    uint64_t *bars = reinterpret_cast<uint64_t *>(base + STAGES * STAGE_BYTES);
-    uint64_t *ready = bars + 2 * STAGES + 1;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(ready + STAGES);
+    // full[STAGES] (TMA landed), empty[STAGES] (consumers done with the slot), ready[STAGES] (low halves written)
+    uint64_t *full = reinterpret_cast<uint64_t *>(base + STAGES * STAGE_BYTES);
+    uint64_t *empty = full + STAGES, *ready = full + 2 * STAGES;
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int m0 = blockIdx.y * TC_BM, n0 = blockIdx.x * BN;
     const int nkb_total = (g.K + TC_BK - 1) / TC_BK;
     const int kb0 = blockIdx.z * g.kb_per_split;
@@ -201,235 +119,121 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < STAGES; ++s) {
-            tc_mbar_init(tc_smem_u32(&bars[s]), 1);
-            tc_mbar_init(tc_smem_u32(&bars[STAGES + s]), 1);
-            tc_mbar_init(tc_smem_u32(&ready[s]), TC_SPLIT_WARPS);   // one arrival per splitter warp
+            tc_mbar_init(tc_smem_u32(&full[s]), 1);
+            tc_mbar_init(tc_smem_u32(&empty[s]), 8);    // one arrival per consumer warp
+            tc_mbar_init(tc_smem_u32(&ready[s]), 4);    // one arrival per producer warp
         }
-        tc_mbar_init(tc_smem_u32(&bars[2 * STAGES]), 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {   // TMEM: BN fp32 accumulator columns (power of two >= 32)
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tc_smem_u32(tmem_slot)), "r"(TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_d = *tmem_slot;
 
-    if (nkb > 0) {
-        if (warp == 0) {
-            // ------------------------------------------------------------ TMA producer (whole warp, elected issue)
-            const bool leader = tc_elect_one();
-            for (int i = 0; i < nkb; ++i) {
-                const int s = i % STAGES, use = i / STAGES;
-                if (use > 0) tc_mbar_wait(tc_smem_u32(&bars[STAGES + s]), (uint32_t)((use - 1) & 1));
-                const uint32_t full = tc_smem_u32(&bars[s]);
-                const uint32_t sa = tc_smem_u32(base + s * STAGE_BYTES), sb = sa + B_OFF;
-                const int k = (kb0 + i) * TC_BK;
-                if (leader) {
-                    TC_STAMP(i, 0);
-                    tc_mbar_expect_tx(full, A_BYTES + B_BYTES);
-                    if (g.a_mn) {      // four boxes of {32 m, 32 k}
+    if (wg == 0) {
+        // ---------------------------------------------------------------- producer: TMA issue runs STAGES - 1 k-blocks
+        // ahead of the split.  Split first, then issue: the slot of block i is freed by the consumers once they have
+        // started on block i - STAGES + 1, whose low halves this very iteration provides.
+        if (threadIdx.x == 0) {
+            asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
+            asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
+        }
+        constexpr int LA = STAGES - 1;
+        constexpr int NQ = (int)((A_BYTES + B_BYTES) / 16) / 128;
+        for (int i = 0; i < nkb + LA; ++i) {
+            const int j = i - LA;
+            if (j >= 0) {
+                const int s = j % STAGES, use = j / STAGES;
+                tc_mbar_wait(tc_smem_u32(&full[s]), (uint32_t)(use & 1));
+                if (threadIdx.x == 0) TC_STAMP(j, 1);
+                uint8_t *st = base + s * STAGE_BYTES;
+                float4 v[NQ];       // every load first, then every store
 #pragma unroll
-                        for (int j = 0; j < TC_BM / 32; ++j) tc_tma_load_2d(sa + j * 4096, &tmA, full, m0 + 32 * j, k);
-                    } else {
-                        tc_tma_load_2d(sa, &tmA, full, k, m0);
-                    }
-                    if (g.b_mn) {
-#pragma unroll
-                        for (int j = 0; j < BN / 32; ++j) tc_tma_load_2d(sb + j * 4096, &tmB, full, n0 + 32 * j, k);
-                    } else {
-                        tc_tma_load_2d(sb, &tmB, full, k, n0);
-                    }
+                for (int q = 0; q < NQ; ++q) {
+                    const int idx = threadIdx.x + 128 * q;                  // float4 index over A then B
+                    const int aq = (int)(A_BYTES / 16);
+                    v[q] = idx < aq ? reinterpret_cast<const float4 *>(st)[idx]
+                                    : reinterpret_cast<const float4 *>(st + B_OFF)[idx - aq];
                 }
-                __syncwarp();
-            }
-        } else if (warp == 1) {
-            // ------------------------------------------------------------ MMA issuer (whole warp, elected issue)
-            const bool leader = tc_elect_one();
-            const uint32_t idesc = tc_idesc(TC_BM, BN, g.a_mn, g.b_mn);
-            const uint32_t idesc_ts = tc_idesc(TC_BM, BN, 0, g.b_mn);     // A from tensor memory: rows = lanes, k = columns
-            // per k-step (8 floats of K): 32 bytes along the swizzled row (K-major) or one whole 1 KB atom (MN-major)
-            const uint64_t stepA = (uint64_t)((g.a_mn ? 1024 : 32) >> 4), stepB = (uint64_t)((g.b_mn ? 1024 : 32) >> 4);
-            for (int i = 0; i < nkb; ++i) {
-                const int s = i % STAGES, use = i / STAGES;
-                tc_mbar_wait(tc_smem_u32(&ready[s]), (uint32_t)(use & 1));      // hi landed and lo written
-                if (i == 0) tc_fence_after();   // once: a fence per k-block drains the MMAs already issued (sweep_tc.cu)
-                const uint32_t a = tc_smem_u32(base + s * STAGE_BYTES);
-                const uint64_t dA = g.a_mn ? tc_smem_desc_mn(a) : tc_smem_desc(a);
-                const uint64_t dAl = g.a_mn ? tc_smem_desc_mn(a + A_BYTES) : tc_smem_desc(a + A_BYTES);
-                const uint64_t dB = g.b_mn ? tc_smem_desc_mn(a + B_OFF) : tc_smem_desc(a + B_OFF);
-                const uint64_t dBl = g.b_mn ? tc_smem_desc_mn(a + B_OFF + B_BYTES) : tc_smem_desc(a + B_OFF + B_BYTES);
-                const uint32_t eb = tc_smem_u32(&bars[STAGES + s]);
-                if (TS) tc_fence_after();       // the splitters' tensor-memory stores of this stage
-                if (leader && TS) {
-                    TC_STAMP(i, 3);
-                    const uint32_t ta = tmem_d + (uint32_t)BN + (uint32_t)(64 * s);      // value at +0, low half at +32
 #pragma unroll
-                    for (int k8 = 0; k8 < TC_BK / 8; ++k8) {
-                        const uint64_t ab = (uint64_t)k8 * stepB;
-                        tc_mma_tf32_ts(tmem_d, ta + 32 + 8 * k8, dB + ab, idesc_ts, (i > 0 || k8 > 0) ? 1u : 0u);   // lo . hi
-                        tc_mma_tf32_ts(tmem_d, ta + 8 * k8, dBl + ab, idesc_ts, 1u);                                // hi . lo
-                        tc_mma_tf32_ts(tmem_d, ta + 8 * k8, dB + ab, idesc_ts, 1u);                                 // hi . hi
-                    }
-                    TC_STAMP(i, 4);
-                    tc_commit(eb);
-                } else if (leader) {
-                    TC_STAMP(i, 3);
-#pragma unroll
-                    for (int k8 = 0; k8 < TC_BK / 8; ++k8) {
-                        const uint64_t aa = (uint64_t)k8 * stepA, ab = (uint64_t)k8 * stepB;
-                        if (g.nmma >= 3) {
-                            tc_mma_tf32(tmem_d, dAl + aa, dB + ab, idesc, (i > 0 || k8 > 0) ? 1u : 0u);   // lo . hi
-                            tc_mma_tf32(tmem_d, dA + aa, dBl + ab, idesc, 1u);                              // hi . lo
-                            tc_mma_tf32(tmem_d, dA + aa, dB + ab, idesc, 1u);                               // hi . hi
-                        } else {
-                            tc_mma_tf32(tmem_d, dA + aa, dB + ab, idesc, (i > 0 || k8 > 0) ? 1u : 0u);
-                        }
-                    }
-                    TC_STAMP(i, 4);
-                    tc_commit(eb);                                 // slot free once these MMAs have read it
+                for (int q = 0; q < NQ; ++q) {
+                    const int idx = threadIdx.x + 128 * q;
+                    const int aq = (int)(A_BYTES / 16);
+                    if (idx < aq) reinterpret_cast<float4 *>(st + A_BYTES)[idx] = tc_lo4(v[q]);
+                    else reinterpret_cast<float4 *>(st + B_OFF + B_BYTES)[idx - aq] = tc_lo4(v[q]);
                 }
-                __syncwarp();
-            }
-            if (leader) tc_commit(tc_smem_u32(&bars[2 * STAGES])); // accumulator complete
-            __syncwarp();
-        } else if (warp >= 4) {
-            // ------------------------------------------------------------ splitters (TC_SPLIT_WARPS warps)
-            constexpr int NSPLIT = 32 * TC_SPLIT_WARPS;
-            constexpr int NA = (int)(A_BYTES / 16) / NSPLIT, NB = (int)(B_BYTES / 16) / NSPLIT;
-            static_assert(NA * NSPLIT * 16 == (int)A_BYTES && NB * NSPLIT * 16 == (int)B_BYTES, "tile not divisible over the splitters");
-            const int tid = threadIdx.x - 128;
-            auto lo4 = [](float4 v) {
-                float4 r;
-                r.x = v.x - __uint_as_float(__float_as_uint(v.x) & 0xffffe000u);
-                r.y = v.y - __uint_as_float(__float_as_uint(v.y) & 0xffffe000u);
-                r.z = v.z - __uint_as_float(__float_as_uint(v.z) & 0xffffe000u);
-                r.w = v.w - __uint_as_float(__float_as_uint(v.w) & 0xffffe000u);
-                return r;
-            };
-            if (TS) {
-                // warps 4..7: the A tile, row by row, into tensor memory (warp w owns lanes 32 (w % 4) ..); warps 8..11: B's low half
-                const bool a_warp = (warp < 8);
-                const int q = warp & 3, row = 32 * q + lane;
-                const int tb = threadIdx.x - 256;                     // 0..127 within the B warps
-                constexpr int NB2 = (int)(B_BYTES / 16) / 128;
-                for (int i = 0; i < nkb; ++i) {
-                    const int s = i % STAGES, use = i / STAGES;
-                    tc_mbar_wait(tc_smem_u32(&bars[s]), (uint32_t)(use & 1));       // TMA bytes have landed
-                    if (tid == 0) TC_STAMP(i, 1);
-                    const uint8_t *sA = base + s * STAGE_BYTES;
-                    if (a_warp) {
-                        uint32_t r[32];
-                        if (g.a_mn) {     // boxes of {32 m, 32 k}: box q holds this warp's rows; 32-byte chunks XOR-ed with k % 4
-#pragma unroll
-                            for (int k = 0; k < 32; ++k)
-                                r[k] = *reinterpret_cast<const uint32_t *>(sA + q * 4096 + k * 128 + ((((lane >> 3) ^ (k & 3)) << 5) | ((lane & 7) << 2)));
-                        } else {          // K-major rows of 128 bytes, 16-byte chunks XOR-ed with row % 8
-#pragma unroll
-                            for (int c = 0; c < 8; ++c) {
-                                const uint4 v = *reinterpret_cast<const uint4 *>(sA + row * 128 + ((c ^ (row & 7)) << 4));
-                                r[4 * c] = v.x; r[4 * c + 1] = v.y; r[4 * c + 2] = v.z; r[4 * c + 3] = v.w;
-                            }
-                        }
-                        const uint32_t ta = tmem_d + ((uint32_t)(32 * q) << 16) + (uint32_t)BN + (uint32_t)(64 * s);
-                        tc_tmem_st32(ta, r);
-#pragma unroll
-                        for (int k = 0; k < 32; ++k) {
-                            const float x = __uint_as_float(r[k]);
-                            r[k] = __float_as_uint(x - __uint_as_float(r[k] & 0xffffe000u));
-                        }
-                        tc_tmem_st32(ta + 32, r);
-                        asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-                        tc_fence_before();
-                    } else {
-                        const float4 *hiB = reinterpret_cast<const float4 *>(sA + B_OFF);
-                        float4 *loB = reinterpret_cast<float4 *>(base + s * STAGE_BYTES + B_OFF + B_BYTES);
-                        float4 vb[NB2];
-#pragma unroll
-                        for (int j = 0; j < NB2; ++j) vb[j] = hiB[tb + j * 128];
-#pragma unroll
-                        for (int j = 0; j < NB2; ++j) loB[tb + j * 128] = lo4(vb[j]);
-                        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                    }
-                    __syncwarp();
-                    if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(tc_smem_u32(&ready[s])) : "memory");
-                    if (tid == 0) TC_STAMP(i, 2);
-                }
-            } else
-            for (int i = 0; i < nkb && !TS; ++i) {
-                const int s = i % STAGES, use = i / STAGES;
-                tc_mbar_wait(tc_smem_u32(&bars[s]), (uint32_t)(use & 1));       // TMA bytes have landed
-                if (tid == 0) TC_STAMP(i, 1);
-                const float4 *hiA = reinterpret_cast<const float4 *>(base + s * STAGE_BYTES);
-                float4 *loA = reinterpret_cast<float4 *>(base + s * STAGE_BYTES + A_BYTES);
-                const float4 *hiB = reinterpret_cast<const float4 *>(base + s * STAGE_BYTES + 2 * A_BYTES);
-                float4 *loB = reinterpret_cast<float4 *>(base + s * STAGE_BYTES + 2 * A_BYTES + B_BYTES);
-                float4 va[NA], vb[NB];       // every load first, then every store: the two never alias
-#pragma unroll
-                for (int q = 0; q < NA; ++q) va[q] = hiA[tid + q * NSPLIT];
-#pragma unroll
-                for (int q = 0; q < NB; ++q) vb[q] = hiB[tid + q * NSPLIT];
-#pragma unroll
-                for (int q = 0; q < NA; ++q) loA[tid + q * NSPLIT] = lo4(va[q]);
-#pragma unroll
-                for (int q = 0; q < NB; ++q) loB[tid + q * NSPLIT] = lo4(vb[q]);
                 asm volatile("fence.proxy.async.shared::cta;" ::: "memory");    // generic writes -> tensor-core (async) proxy
                 __syncwarp();
-                if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(tc_smem_u32(&ready[s])) : "memory");
-                if (tid == 0) TC_STAMP(i, 2);
+                if (lane == 0) tc_mbar_arrive(tc_smem_u32(&ready[s]));
+                if (threadIdx.x == 0) TC_STAMP(j, 2);
+            }
+            if (i < nkb && threadIdx.x == 0) {
+                const int s = i % STAGES, use = i / STAGES;
+                if (use > 0) tc_mbar_wait(tc_smem_u32(&empty[s]), (uint32_t)((use - 1) & 1));
+                const uint32_t fb = tc_smem_u32(&full[s]);
+                const uint32_t sa = tc_smem_u32(base + s * STAGE_BYTES);
+                const int k = (kb0 + i) * TC_BK;
+                TC_STAMP(i, 0);
+                tc_mbar_expect_tx(fb, A_BYTES + B_BYTES);
+                tc_tma_load_2d(sa, &tmA, fb, k, m0);
+                tc_tma_load_2d(sa + B_OFF, &tmB, fb, k, n0);
             }
         }
-        __syncwarp();
-        // ---------------------------------------------------------------- epilogue (all 4 warps)
-        tc_mbar_wait(tc_smem_u32(&bars[2 * STAGES]), 0);
-        tc_fence_after();
+        return;
     }
-    const int m = m0 + warp * 32 + lane;
-#pragma unroll 1
-    for (int c = 0; c < BN && warp < 4; c += 32) {
-        uint32_t r[32];
-        if (nkb > 0) {
-            const uint32_t taddr = tmem_d + ((uint32_t)(warp * 32) << 16) + (uint32_t)c;
-            asm volatile(
-                "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                  "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-                  "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-                  "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                : "r"(taddr) : "memory");
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        } else {
+
+    // -------------------------------------------------------------------- consumers
+    const int cw = wg - 1;                                        // rows 64 cw .. 64 cw + 63 of the tile
+    float acc[BN / 2];
 #pragma unroll
-            for (int j = 0; j < 32; ++j) r[j] = 0u;
+    for (int r = 0; r < BN / 2; ++r) acc[r] = 0.f;
+    for (int i = 0; i < nkb; ++i) {
+        const int s = i % STAGES, use = i / STAGES;
+        tc_mbar_wait(tc_smem_u32(&ready[s]), (uint32_t)(use & 1));      // hi landed and lo written
+        if (threadIdx.x == 128) TC_STAMP(i, 3);
+        const uint32_t sa = tc_smem_u32(base + s * STAGE_BYTES) + (uint32_t)cw * (64 * 128);
+        const uint32_t sb = tc_smem_u32(base + s * STAGE_BYTES) + B_OFF;
+        const uint64_t dA = wg_desc(sa), dAl = wg_desc(sa + A_BYTES), dB = wg_desc(sb), dBl = wg_desc(sb + B_BYTES);
+        wg_fence();
+#pragma unroll
+        for (int k8 = 0; k8 < TC_BK / 8; ++k8) {
+            const uint64_t adv = (uint64_t)((k8 * 32) >> 4);
+            WgmmaTf32<BN>::mma(acc, dAl + adv, dB + adv, (i > 0 || k8 > 0) ? 1u : 0u);   // lo . hi
+            WgmmaTf32<BN>::mma(acc, dA + adv, dBl + adv, 1u);                            // hi . lo
+            WgmmaTf32<BN>::mma(acc, dA + adv, dB + adv, 1u);                             // hi . hi
         }
-        if (m < g.M) {
-            float *drow = g.partial ? g.partial + ((int64_t)blockIdx.z * g.M + m) * g.N + n0 + c
-                                    : g.C + (int64_t)m * g.ldc + n0 + c;
-            float v[32];
+        wg_commit();
+        if (threadIdx.x == 128) TC_STAMP(i, 4);
+        // the previous k-block's MMAs are complete once at most this one is outstanding: release its slot
+        wg_wait<1>();
+        if (i > 0) {
+            __syncwarp();
+            if (lane == 0) tc_mbar_arrive(tc_smem_u32(&empty[(i - 1) % STAGES]));
+        }
+    }
+    wg_wait<0>();
+    // (the last slot is never waited for again: nothing is loaded after it)
+
+    // -------------------------------------------------------------------- epilogue straight from the accumulator
+    const int q = warp & 3;
+    const int rbase = m0 + 64 * cw + 16 * q + (lane >> 2);
 #pragma unroll
-            for (int j = 0; j < 32; ++j)
-                v[j] = g.partial ? __uint_as_float(r[j])
-                                 : ((n0 + c + j < g.N) ? tc_epilogue(g, __uint_as_float(r[j]), m, n0 + c + j) : 0.f);
-            if (n0 + c + 32 <= g.N && (((uintptr_t)drow) & 15) == 0) {
+    for (int h = 0; h < 2; ++h) {
+        const int m = rbase + 8 * h;
+        if (m >= g.M) continue;
+        float *drow = g.partial ? g.partial + ((int64_t)blockIdx.z * g.M + m) * g.N : g.C + (int64_t)m * g.ldc;
 #pragma unroll
-                for (int j = 0; j < 32; j += 4)
-                    *reinterpret_cast<float4 *>(drow + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
+        for (int j = 0; j < BN / 8; ++j) {
+            const int n = n0 + 8 * j + 2 * (lane & 3);
+            float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+            if (!g.partial) {
+                if (n < g.N) v0 = tc_epilogue(g, v0, m, n);
+                if (n + 1 < g.N) v1 = tc_epilogue(g, v1, m, n + 1);
+            }
+            if (n + 1 < g.N && (((uintptr_t)(drow + n)) & 7) == 0) {
+                *reinterpret_cast<float2 *>(drow + n) = make_float2(v0, v1);
             } else {
-#pragma unroll
-                for (int j = 0; j < 32; ++j)
-                    if (n0 + c + j < g.N) drow[j] = v[j];
+                if (n < g.N) drow[n] = v0;
+                if (n + 1 < g.N) drow[n + 1] = v1;
             }
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d), "r"(TMEM_COLS) : "memory");
     }
 }
 
@@ -512,47 +316,14 @@ static int make_map(CUtensorMap *m, const float *ptr, int rows, int K, int64_t l
     return CTCB_OK;
 }
 
-// MN-major operand: stored K x MN (MN contiguous, pitch ld elements); box = {32 along MN, 32 along K}, 128B swizzle with 32-byte atoms
-static int make_map_mn(CUtensorMap *m, const float *ptr, int mn, int K, int64_t ld) {
-    EncodeTiledFn enc = get_encode();
-    if (!enc) return set_error(CTCB_ECUDA, "cuTensorMapEncodeTiled is not available from this driver");
-    cuuint64_t dims[2] = {(cuuint64_t)mn, (cuuint64_t)K};
-    cuuint64_t strides[1] = {(cuuint64_t)ld * sizeof(float)};
-    cuuint32_t box[2] = {32, (cuuint32_t)TC_BK};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void *)ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return set_error(CTCB_ECUDA, "cuTensorMapEncodeTiled (MN-major) failed (%d) mn=%d K=%d ld=%lld", (int)r, mn, K, (long long)ld);
-    return CTCB_OK;
-}
-
 static inline int64_t pad4(int64_t x) { return (x + 3) / 4 * 4; }
 
-static int tc_pick_bn(int M, int N, int K) {
-    static int force = -1;
-    if (force < 0) { const char *e = getenv("CTCB_GEMM_BN"); force = e ? atoi(e) : 0; }
-    if (force == 64 || force == 128 || force == 256) return force;
-    if (N <= 64) return 64;
-    {   // A through tensor memory (default): the 128-wide tile runs two CTAs per SM -- one's epilogue and pipeline fill under
-        // the other's main loop -- and beats the 256-wide one everywhere (48000x2048x2048: 228 vs 185 TFLOP/s; 25600x1024x1024:
-        // 172 vs 136; weight gradients 2048x2048x192000: 205 vs 203)
-        static int ts_env = -1;
-        if (ts_env < 0) { const char *e = getenv("CTCB_GEMM_TS"); ts_env = e ? atoi(e) : 1; }
-        if (ts_env) return 128;
-    }
-    // both operands from shared memory (CTCB_GEMM_TS=0), measured in round 1: 256-wide tiles win once they still fill >= 2 waves of CTAs (16384x2048x2048:
-    // 192 vs 163 TFLOP/s fp32-equivalent) and lose on small problems (6400x512x512: 0.062 vs 0.048 ms)
-    if (N >= 256 && (int64_t)((M + TC_BM - 1) / TC_BM) * ((N + 255) / 256) >= 2 * num_sms()) return 256;
-    // reduction-heavy shapes (the weight gradients: 512 x 512 outputs over K = T*B rows) are split over K anyway;
-    // wide tiles halve the B-operand traffic per CTA (C2 step: 0.16 -> 0.14 ms for the two recurrent gradients)
-    if (N >= 256 && M <= 1024 && K >= 4096) return 256;
-    return 128;
-}
+// 64-wide tiles for narrow outputs (the accumulator then takes 32 registers per thread instead of 64)
+static int tc_pick_bn(int N) { return N <= 64 ? 64 : 128; }
 
-// The tensor cores accumulate in fp32 with truncation, not rounding: measured (tools/gemm_check.py big), the relative
-// error of one accumulator chain grows linearly with its length -- 4e-6 at K = 512, 1.5e-5 at K = 2048, 3.4e-4 at
-// K = 48 000, 1.3e-3 at K = 192 000 (a weight gradient over T*B rows).  So no chain is allowed to be longer than
-// TC_CHAIN_KB k-blocks (K = 2048): longer contractions are split over K and the partial sums are added in fp32 with
+// The tensor cores' fp32 accumulation does not round to nearest, so the relative error of one accumulator chain grows
+// linearly with its length (tools/gemm_check.py big shows it).  No chain is allowed to be longer than TC_CHAIN_KB
+// k-blocks (K = 2048): longer contractions are split over K and the partial sums are added in fp32 with
 // round-to-nearest by the reduce kernel (deterministic order).
 constexpr int TC_CHAIN_KB = 64;
 
@@ -582,8 +353,8 @@ bool gemm_tc_enabled() {
     return on == 1;
 }
 
-// measured on B200 (tools/gemm_check.py): below these sizes the exact FFMA kernel is as fast or faster (K = 41 / 62 with
-// re-pitched copies: slower on the tensor cores; M = 62, K = 6400 -- the output layer's weight gradient: 44 -> 24 us on them)
+// Below these sizes the exact FFMA kernel is used: short contractions (K = 41 / 62) would need re-pitched copies and
+// cannot amortise the tensor-core pipeline.  The thresholds have not been re-tuned on H100.
 bool gemm_tc_eligible(int M, int N, int K) {
     static int min_k = -1, min_m = -1;      // CTCB_GEMM_MINK / _MINM: smallest contraction length / row count that goes to the tensor cores
     if (min_k < 0) { const char *e = getenv("CTCB_GEMM_MINK"); min_k = e ? atoi(e) : 128; }
@@ -594,18 +365,19 @@ bool gemm_tc_eligible(int M, int N, int K) {
 size_t gemm_tc_workspace_bytes(int M, int N, int K) {
     const int64_t Kp = pad4(K);
     size_t prep = ((size_t)M * Kp + (size_t)N * Kp) * sizeof(float);     // re-laid-out copies of A and B (when needed)
-    const int BN = tc_pick_bn(M, N, K);
+    const int BN = tc_pick_bn(N);
     const int splits = tc_choose_splits(M, N, K, BN);
     size_t part = splits > 1 ? (size_t)splits * M * N * sizeof(float) : 0;
     return align_up(prep, 256) + align_up(part, 256) + 1024;
 }
 
-template <int BN, int STAGES, bool TS>
+template <int BN, int STAGES>
 static int launch_tc(const CUtensorMap &tA, const CUtensorMap &tB, const GemmTcArgs &g, int splits, cudaStream_t st) {
-    constexpr size_t smem = (size_t)STAGES * ((TS ? 1 : 2) * TC_BM * TC_BK * 4 + 2 * BN * TC_BK * 4) + (3 * STAGES + 1) * 8 + 16 + 1024;
-    CTCB_CUDA_CHECK(cudaFuncSetAttribute((gemm_tc_kernel<BN, STAGES, TS>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    constexpr size_t smem = (size_t)STAGES * (2 * TC_BM * TC_BK * 4 + 2 * BN * TC_BK * 4) + 3 * STAGES * 8 + 1024;
+    static_assert(smem <= 227 * 1024, "stage ring exceeds the shared memory of a block");
+    CTCB_CUDA_CHECK(cudaFuncSetAttribute((gemm_tc_kernel<BN, STAGES>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     dim3 grid((g.N + BN - 1) / BN, (g.M + TC_BM - 1) / TC_BM, splits);
-    gemm_tc_kernel<BN, STAGES, TS><<<grid, TC_THREADS, smem, st>>>(tA, tB, g);
+    gemm_tc_kernel<BN, STAGES><<<grid, TC_THREADS, smem, st>>>(tA, tB, g);
     CTCB_LAUNCH_CHECK();
     return CTCB_OK;
 }
@@ -621,17 +393,10 @@ int run_gemm_tc(int transA, int transB, int M, int N, int K, float alpha, const 
     float *Bhi = p; p += (size_t)N * Kp;
     float *part = (float *)((char *)ws + align_up(((size_t)M * Kp + (size_t)N * Kp) * sizeof(float), 256));
 
-    // ---- operand A as M x K, K-major: stored M x K (transA=0) or K x M (transA=1)
+    // ---- operand A as M x K, K-major: stored M x K (transA=0) or K x M (transA=1, transposed into a copy)
     const float *Ause; int64_t lda_use;
     auto ew_grid = [](int64_t n) { int64_t b = (n + 255) / 256; const int cap = 16 * num_sms(); return (int)(b > cap ? cap : (b < 1 ? 1 : b)); };
-    static int mn_env = -1;     // CTCB_GEMM_MN=0: always transpose into K-major copies (the round-1 path)
-    if (mn_env < 0) { const char *e = getenv("CTCB_GEMM_MN"); mn_env = e ? atoi(e) : 1; }
-    auto tma_ok = [](const float *p_, int64_t ld_) { return (ld_ % 4 == 0) && (((uintptr_t)p_) % 16 == 0); };
-    const int a_mn = (transA && mn_env && tma_ok(A, lda)) ? 1 : 0;
-    const int b_mn = (!transB && mn_env && tma_ok(B, ldb)) ? 1 : 0;
-    if (a_mn) {
-        Ause = A; lda_use = lda;                       // stored K x M: MN-major A, no copy
-    } else if (transA) {
+    if (transA) {
         tc_split_transpose_kernel<<<dim3((M + 31) / 32, (K + 31) / 32), dim3(32, 8), 0, st>>>(A, lda, K, M, Ahi, nullptr, Kp);
         CTCB_LAUNCH_CHECK();
         Ause = Ahi; lda_use = Kp;
@@ -642,11 +407,9 @@ int run_gemm_tc(int transA, int transB, int M, int N, int K, float alpha, const 
         CTCB_LAUNCH_CHECK();
         Ause = Ahi; lda_use = Kp;
     }
-    // ---- operand B as N x K, K-major: stored N x K (transB=1) or K x N (transB=0)
+    // ---- operand B as N x K, K-major: stored N x K (transB=1) or K x N (transB=0, transposed into a copy)
     const float *Buse; int64_t ldb_use;
-    if (b_mn) {
-        Buse = B; ldb_use = ldb;                       // stored K x N: MN-major B, no copy
-    } else if (!transB) {
+    if (!transB) {
         tc_split_transpose_kernel<<<dim3((N + 31) / 32, (K + 31) / 32), dim3(32, 8), 0, st>>>(B, ldb, K, N, Bhi, nullptr, Kp);
         CTCB_LAUNCH_CHECK();
         Buse = Bhi; ldb_use = Kp;
@@ -658,22 +421,11 @@ int run_gemm_tc(int transA, int transB, int M, int N, int K, float alpha, const 
         Buse = Bhi; ldb_use = Kp;
     }
 
-    const int BN = tc_pick_bn(M, N, K);
+    const int BN = tc_pick_bn(N);
     int splits = tc_choose_splits(M, N, K, BN);
     const int nkb = (K + TC_BK - 1) / TC_BK;
     GemmTcArgs g;
-    g.a_mn = a_mn; g.b_mn = b_mn;
-    {
-        static int ts_env = -1;     // CTCB_GEMM_TS=0: both operands from shared memory (the round-1 form)
-        if (ts_env < 0) { const char *e = getenv("CTCB_GEMM_TS"); ts_env = e ? atoi(e) : 1; }
-        g.ts = ts_env;
-    }
     g.M = M; g.N = N; g.K = K; g.C = C; g.ldc = ldc; g.alpha = alpha; g.beta = beta; g.bias = bias; g.relu = relu; g.mask = mask_src;
-    {
-        static int nmma_env = -1;
-        if (nmma_env < 0) { const char *e = getenv("CTCB_GEMM_MMAS"); nmma_env = e ? atoi(e) : 3; }
-        g.nmma = nmma_env;
-    }
     g.trace = nullptr;
     {
         static int tr_env = -1;
@@ -689,23 +441,10 @@ int run_gemm_tc(int transA, int transB, int M, int N, int K, float alpha, const 
 
     CUtensorMap tA, tB;
     int rc;
-    if ((rc = a_mn ? make_map_mn(&tA, Ause, M, K, lda_use) : make_map(&tA, Ause, M, K, lda_use, TC_BM)) != CTCB_OK) return rc;
-    if ((rc = b_mn ? make_map_mn(&tB, Buse, N, K, ldb_use) : make_map(&tB, Buse, N, K, ldb_use, BN)) != CTCB_OK) return rc;
-    static int stages_env = -1;   // CTCB_GEMM_STAGES=2 with BN=64: 96 KB/CTA -> two CTAs per SM overlap prologue/epilogue
-    if (stages_env < 0) { const char *e = getenv("CTCB_GEMM_STAGES"); stages_env = e ? atoi(e) : 0; }
-    // Tile shapes.  TS (default): 256-wide, 2 stages of 80 KB, one CTA per SM; 128-wide with 2 stages of 48 KB so that TWO
-    // CTAs share an SM (2 x 256 tensor-memory columns) and one's epilogue runs under the other's main loop; 64-wide, 4 stages.
-    if (!g.ts) {
-        if (BN == 64 && stages_env == 2) rc = launch_tc<64, 2, false>(tA, tB, g, splits, st);
-        else if (BN == 64) rc = launch_tc<64, 4, false>(tA, tB, g, splits, st);
-        else if (BN == 256) rc = launch_tc<256, 2, false>(tA, tB, g, splits, st);
-        else rc = launch_tc<128, 3, false>(tA, tB, g, splits, st);
-    } else {
-        if (BN == 64) rc = launch_tc<64, 4, true>(tA, tB, g, splits, st);
-        else if (BN == 256) rc = launch_tc<256, 2, true>(tA, tB, g, splits, st);
-        else if (stages_env == 3) rc = launch_tc<128, 3, true>(tA, tB, g, splits, st);
-        else rc = launch_tc<128, 2, true>(tA, tB, g, splits, st);
-    }
+    if ((rc = make_map(&tA, Ause, M, K, lda_use, TC_BM)) != CTCB_OK) return rc;
+    if ((rc = make_map(&tB, Buse, N, K, ldb_use, BN)) != CTCB_OK) return rc;
+    // 192 KB of ring either way: 4 stages of 48 KB (64-wide) or 3 of 64 KB (128-wide)
+    rc = (BN == 64) ? launch_tc<64, 4>(tA, tB, g, splits, st) : launch_tc<128, 3>(tA, tB, g, splits, st);
     if (rc != CTCB_OK) return rc;
     if (splits > 1) {
         const int64_t total = (int64_t)M * N;
@@ -720,7 +459,7 @@ int run_gemm_tc(int transA, int transB, int M, int N, int K, float alpha, const 
 }  // namespace ctcb
 
 // Diagnostic: the per-k-block clock stamps of CTA (0,0,0) of the last tensor-core GEMM (CTCB_GEMM_TRACE=1):
-// [64][8] = {TMA issued, tile landed, lo written, MMA thread saw it, MMAs issued}.  Returns 0 when tracing is off.
+// [64][8] = {TMA issued, tile landed, lo written, consumers saw it, MMAs issued}.  Returns 0 when tracing is off.
 extern "C" int ctcb_debug_gemm_trace(unsigned long long *host_out) {
     if (!ctcb::g_gemm_trace || !host_out) return 0;
     if (cudaMemcpy(host_out, ctcb::g_gemm_trace, 64 * 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost) != cudaSuccess) return 0;

@@ -1,10 +1,10 @@
 // sgd.cu -- optimiser arithmetic on the flat parameter vector.
 //
 // Replaces, per step, the ~16(N+3) cudamat launches and 2(N+3) blocking euclid_norm() reads of
-//   /root/reference/ctc_fast/sgd.py:91-100   (Nesterov look-ahead / undo via NNet.updateParams)
-//   /root/reference/ctc_fast/sgd.py:103-107  (global gradient norm)
-//   /root/reference/ctc_fast/sgd.py:130-140  (clip scale, velocity update)
-//   /root/reference/ctc_fast/sgd.py:161 and nnets/brnnet.py:251-256 (w += v)
+//   ctc_fast/sgd.py:91-100   (Nesterov look-ahead / undo via NNet.updateParams)
+//   ctc_fast/sgd.py:103-107  (global gradient norm)
+//   ctc_fast/sgd.py:130-140  (clip scale, velocity update)
+//   ctc_fast/sgd.py:161 and nnets/brnnet.py:251-256 (w += v)
 // with one axpy, one two-stage sum of squares and one fused update kernel; the clip scale is
 // computed on the device from the reduced norm, so the step never synchronises with the host.
 #include "common.cuh"

@@ -2,20 +2,20 @@
 //
 // Replaces the 4(T-1) cudamat launches per utterance of the reference's hot loops
 //   forward : For[:,t]  = clip(pre[:,t] + Wtf.For[:,t-1], 0, 20),  Back mirrored
-//             (/root/reference/ctc_fast/nnets/brnnet.py:144-152: mvdot_col_slice + minmax)
+//             (ctc_fast/nnets/brnnet.py:144-152: mvdot_col_slice + minmax)
 //   BPTT    : dFor[:,t] = within(For[:,t]) * (d[:,t] + Wtf^T.dFor[:,t+1]),  dBack mirrored
 //             (brnnet.py:208-224: mvdot_col_slice on W.T + mult_slice)
 // with a batch of utterances as the second matrix dimension.
 //
 // Three kernels share this design point (run_sweep below picks one):
-//   * sweep_tc.cu (layerSize >= 1024, round 2): the step as a tcgen05 tensor-core contraction spread over the device,
+//   * sweep_tc.cu (layerSize >= 1024, round 2): the step as a wgmma tensor-core contraction spread over the device,
 //     split-K partials reduced through DSMEM, one counter barrier per step.
 //   * sweep_cluster.cu (H = 128/256/512): one thread-block cluster per (direction, 8 utterances); the
 //     hidden state is exchanged CTA-to-CTA through distributed shared memory with bulk async copies
 //     that complete on the consumer's mbarrier -- no global-memory round trip on the serial chain.
 //   * this file (any H): the general fallback below, exchanging through L2 with a counter barrier.
 //
-// Design (B200): the H x H recurrent matrix never leaves the register file.  A CTA of 8 warps owns
+// Design: the H x H recurrent matrix never leaves the register file.  A CTA of 8 warps owns
 // 32 output units; lane l of warp w keeps W[j][l + 32 i] for its 4 rows j in registers for the
 // whole sweep (H/32 * 4 registers), so a time step only moves the previous hidden state
 // (8 utterances x H floats, read from L2 into shared memory) and the 32 x 8 new outputs.  Both

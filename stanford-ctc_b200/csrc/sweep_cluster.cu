@@ -61,38 +61,23 @@ __device__ __forceinline__ void st_async_f32(uint32_t dst_cluster, float v, uint
                  ::"r"(dst_cluster), "r"(__float_as_uint(v)), "r"(bar_cluster) : "memory");
 }
 
-// packed two-lane fp32 arithmetic (FFMA2)
-__device__ __forceinline__ unsigned long long pack2(float lo, float hi) {
-    unsigned long long r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-    return r;
-}
-__device__ __forceinline__ float sum2(unsigned long long v) {
-    float lo, hi;
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-    return lo + hi;
-}
-__device__ __forceinline__ void ffma2(unsigned long long &d, unsigned long long a, unsigned long long b) {
-    asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(d) : "l"(a), "l"(b));
+// a pair of output units times one scalar state value: two FFMAs (each rounded exactly as fma.rn)
+__device__ __forceinline__ void ffma_pair(float2 &d, float2 w, float h) {
+    d.x = fmaf(w.x, h, d.x);
+    d.y = fmaf(w.y, h, d.y);
 }
 
 // ---------------------------------------------------------------------------------------------------
 // The kernel: 16 warps per CTA, 64 output units per CTA, CS = H/64 CTAs per cluster, NB
 // utterances per cluster.  The INPUT dimension is split over the warps, not over the lanes: warp w owns input
 // units [w*H/16, (w+1)*H/16) of all 64 output units; lane l owns output units 2l, 2l+1 (H/8 weights per thread
-// in registers, one 64-bit register pair per input unit: the FFMA2 form (pair of units) x (scalar state)).
+// in registers, one register pair per input unit: (pair of units) x (scalar state)).
 // Per warp and step at H = 512, NB = 5:
 //   * every lane needs the same slice of the previous state: 40 broadcast LDS.128;
 //   * no shuffle reduction: a lane's accumulators are complete over its warp's slice; the 16 per-warp partial
 //     sums of an output meet in shared memory (the one CTA barrier of the step), where thread (utterance, unit)
 //     adds them, applies clip/mask, stores the state to HBM and sends it to the CS peers with st.async.
 //   state layout in every CTA: [buffer 2][source CTA][utterance][unit 64]
-// Measured (tools/sweep_time.py, T = 200, B = 32): 1.76 us/step at H = 512 (lane-split predecessor with a
-// 31-shuffle butterfly: 2.3; this kernel with a cp.async.bulk push and a second barrier: 1.85), 0.65 at H = 256,
-// 0.43 at H = 128.  Cost model from B = 4..32 at H = 512: 0.4 us fixed (wait, barrier, reduction, exchange) +
-// 0.27 us per utterance of the cluster, of which 0.2 us is 32768 FMA per SM at the measured FFMA2 rate (2.8
-// cycles per warp instruction and sub-partition, tools/micro/mma_rate.cu).  ncu (profiles/): FMA pipe 41 % of
-// active cycles, issue slots 39 %; stall samples mostly math-pipe throttle and the mbarrier wait.
 // ---------------------------------------------------------------------------------------------------
 template <int KI, int NB>
 __global__ void __launch_bounds__(512, 1) sweep_cluster_kernel(SweepClusterArgs a) {
@@ -120,14 +105,13 @@ __global__ void __launch_bounds__(512, 1) sweep_cluster_kernel(SweepClusterArgs 
     const int j0 = rank * 64;
     const int k0 = warp * KW;
 
-    // w2[k] = weights of output units (2*lane, 2*lane + 1) for input unit k0 + k: the FFMA2 form
-    // (pair of units) x (scalar state value), whose b operand is a plain 32-bit register
-    unsigned long long w2[KW];
+    // w2[k] = weights of output units (2*lane, 2*lane + 1) for input unit k0 + k
+    float2 w2[KW];
 #pragma unroll
     for (int k = 0; k < KW; ++k) {
         const int j = j0 + 2 * lane, kk = k0 + k;
-        w2[k] = bptt ? pack2(W[(int64_t)kk * H + j], W[(int64_t)kk * H + j + 1])
-                     : pack2(W[(int64_t)j * H + kk], W[(int64_t)(j + 1) * H + kk]);
+        w2[k] = bptt ? make_float2(W[(int64_t)kk * H + j], W[(int64_t)kk * H + j + 1])
+                     : make_float2(W[(int64_t)j * H + kk], W[(int64_t)(j + 1) * H + kk]);
     }
 
     const uint32_t bar0 = smem_u32(&mbar[0]), bar1 = smem_u32(&mbar[1]);
@@ -173,22 +157,22 @@ __global__ void __launch_bounds__(512, 1) sweep_cluster_kernel(SweepClusterArgs 
                 }
             }
             const float *hs = &hbuf[s & 1][hoff];
-            unsigned long long acc2[NB];
+            float2 acc2[NB];
 #pragma unroll
             for (int u = 0; u < NB; ++u) {
 #pragma unroll
                 for (int q = 0; q < KW / 4; ++q) {
                     const float4 hv = *reinterpret_cast<const float4 *>(hs + u * 64 + 4 * q);   // broadcast
-                    if (q == 0) acc2[u] = 0ull;
-                    ffma2(acc2[u], w2[4 * q], pack2(hv.x, hv.x));
-                    ffma2(acc2[u], w2[4 * q + 1], pack2(hv.y, hv.y));
-                    ffma2(acc2[u], w2[4 * q + 2], pack2(hv.z, hv.z));
-                    ffma2(acc2[u], w2[4 * q + 3], pack2(hv.w, hv.w));
+                    if (q == 0) acc2[u] = make_float2(0.f, 0.f);
+                    ffma_pair(acc2[u], w2[4 * q], hv.x);
+                    ffma_pair(acc2[u], w2[4 * q + 1], hv.y);
+                    ffma_pair(acc2[u], w2[4 * q + 2], hv.z);
+                    ffma_pair(acc2[u], w2[4 * q + 3], hv.w);
                 }
             }
 #pragma unroll
             for (int u = 0; u < NB; ++u)
-                *reinterpret_cast<unsigned long long *>(&red[s & 1][warp][u * 64 + 2 * lane]) = acc2[u];
+                *reinterpret_cast<float2 *>(&red[s & 1][warp][u * 64 + 2 * lane]) = acc2[u];
             __syncthreads();            // the only CTA barrier of the step (red is double-buffered)
             // every warp is past its wait on this step's barrier: arm it for step s + 2
             if (tid == 0 && s + 2 < T) mbar_arrive_expect_tx(bar, CS * BLK_BYTES);

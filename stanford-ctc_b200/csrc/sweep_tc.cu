@@ -1,4 +1,4 @@
-// sweep_tc.cu -- the temporal-layer recurrences on the 5th-generation tensor cores (H >= 1024: C3 / C4).
+// sweep_tc.cu -- the temporal-layer recurrences on the Hopper tensor cores (H >= 1024: C3 / C4).
 //
 // Same arithmetic as sweep.cu / sweep_cluster.cu (reference loops ctc_fast/nnets/brnnet.py:144-152 forward,
 // :208-224 BPTT): per time step and direction  S_t = f(pre_t + S_{t-1} . W^T)  over ALL utterances of the batch.
@@ -6,33 +6,30 @@
 // (sweep.cu) re-reads it per 8-utterance tile; here a step is one fp32-faithful (3xTF32, as gemm_tc.cu) tensor-core
 // contraction  D[units x utterances] = W[units x H] . S_{t-1}[utterances x H]^T  spread over the device:
 //
-//   * work split: M tiles of 128 output units x 4 K-slices (H/4 inputs each) x NS utterance splits x 2 directions
-//     = 128 CTAs at H = 1024 (NS = 2) and H = 2048 (NS = 1); one persistent CTA per SM for the whole sweep;
-//   * the 4 K-slices of an (M tile, utterance split, direction) form a CLUSTER: each CTA accumulates its partial
-//     product in tensor memory (tcgen05.mma.kind::tf32; hi AND lo halves of both operands arrive by TMA in a
-//     128B-swizzled ring: W's are prepared once per launch, the state's are written by the previous step's epilogue,
-//     so no thread touches the operands), copies it to its own shared memory, and after one cluster barrier CTA r
-//     sums the four partials of ITS quarter of the utterances through distributed shared memory
+//   * work split: M tiles of 128 output units x CS K-slices (H/CS inputs each) x NS utterance splits x 2 directions;
+//     one persistent CTA per SM for the whole sweep, so every CTA must be co-resident: CS = 4, 2 or 1, the largest
+//     whose clusters the device can hold at once (at H = 2048 two directions need 32 clusters of 4, which a 132-SM
+//     H100 cannot place; 64 clusters of 2 it can);
+//   * the CS K-slices of an (M tile, utterance split, direction) form a CLUSTER: each CTA accumulates its partial
+//     product in registers (two warpgroups, 64 units each, wgmma .tf32; hi AND lo halves of both operands arrive by
+//     TMA in a 128B-swizzled ring: W's are prepared once per launch, the state's are written by the previous step's
+//     epilogue, so no thread touches the operands), copies it to its own shared memory, and after one cluster barrier
+//     CTA r sums the four partials of ITS quarter of the utterances through distributed shared memory
 //     (ld.shared::cluster), adds pre_t, applies clip / mask and writes S_t -- a deterministic split-K reduction
 //     that never touches global memory;
 //   * S_t goes to HBM/L2 anyway (the layer's output); the next step's B operand is TMA-loaded from there, so the only
-//     device-wide synchronisation is ONE counter barrier per step and (direction, utterance split) -- 32 or 64 CTAs;
-//   * W is streamed from L2 every step (8.4 / 33.5 MB for both directions: resident in the 126 MB L2); at H = 2048
-//     hi + lo halves of both directions (67 MB) exceed the 33 MB of shared memory on the device, so residency is
-//     not an option there, and the stream is hidden behind the MMAs whenever the batch is large enough.
-//
-// Measured on B200 (tools/micro/umma_rate.cu): a kind::tf32 MMA costs max(45, N/2) cycles whatever M is, so the
-// recurrent matrix is the M = 128 operand and the utterances are N; a first version that produced the low halves with
-// splitter warps spent ~1300 cycles per k-block there (2.4x the 12 MMAs) -- hence the TMA-only operand path.
+//     device-wide synchronisation is ONE counter barrier per step and (direction, utterance split);
+//   * W is streamed from L2 every step (hi + lo of both directions: 16 MB at H = 1024, 64 MB at H = 2048, against the
+//     50 MB L2 of an H100); the stream is hidden behind the MMAs whenever the batch is large enough.
 // Scratch: the (hi, lo) stacks of W (W^T for BPTT) for both directions and the two-slot ring of state low halves.
 #include "common.cuh"
+#include "wgmma.cuh"
 #include <cuda.h>
 #include <stdlib.h>
 
 namespace ctcb {
 
-constexpr int STC_THREADS = 256;
-constexpr int STC_CS = 4;            // K-slices = cluster size
+constexpr int STC_THREADS = 288;     // warps 0-7: two consumer warpgroups; warp 8: TMA producer
 constexpr int STC_BM = 128;          // output units per CTA
 constexpr int STC_BK = 32;           // floats per k-block (one 128-byte swizzle span)
 constexpr uint32_t STC_A_BYTES = STC_BM * STC_BK * 4;
@@ -47,18 +44,12 @@ struct SweepTcArgs {
     float maxAct;
     unsigned int *err;        // [0]: set to 3 when a wait timed out (results invalid, never a hang)
     unsigned int *counters;   // [ndir * NS] step counters, zeroed before launch
-    int ndir, MT, NS, Npad;   // Npad: utterances per split, multiple of 16, <= 256
-    int nkb;                  // k-blocks per K-slice = H / 4 / 32
+    int ndir, MT, NS;
+    int cs;                   // K-slices = cluster size (4, 2 or 1)
+    int nkb;                  // k-blocks per K-slice = H / cs / 32
     int stages;
-    uint32_t stage_bytes;     // 2 * STC_A_BYTES + 2 * Npad * 128
-    uint32_t tmem_cols;
+    uint32_t stage_bytes;     // 2 * STC_A_BYTES + 2 * NP * 128
     int partial_own;          // 1: the partial product has its own shared-memory region (W prefetch across steps)
-    int wfence;               // experiment: writer-side proxy fence before the counter arrival
-    int rotate;               // experiment (CTCB_SWEEP_TC_ROTATE=1): M-tile CTAs walk the k-blocks in rotated orders; measured: no effect
-    int nomma;                // experiment (CTCB_SWEEP_TC_NOMMA=1): issue no MMA -- how fast does the operand stream alone run?
-    int resident;             // 1: this CTA's W slice never leaves the SM: hi half in TENSOR MEMORY (A operand of the
-                              //    .ts MMA form), lo half in shared memory; only the state is streamed (H <= 1024)
-    const float *whi[2];      // resident mode: the hi plane of the prepared (hi, lo) stack, row-major H x H
     unsigned long long *trace;   // optional (CTCB_SWEEP_TRACE): [64 steps][16] SM clock stamps of CTA (0,0,0)
 };
 constexpr int STC_TRACE_STEPS = 64;
@@ -99,19 +90,11 @@ __device__ __forceinline__ void stc_mbar_wait(uint32_t bar, uint32_t parity, vol
         }
     }
 }
-// One lane of a CONVERGED warp.  The producer and MMA roles run their loops with the whole warp (warp-uniform control
-// flow and operands) and only ISSUE from the elected lane: inside a `lane == 0` branch the compiler must assume
-// divergent descriptors and wraps every UTCHMMA / UTMALDG / UTCBAR in an ELECT + R2UR.BROADCAST waterfall loop --
-// measured 69 cycles per MMA issue and ~400 per commit instead of the tensor core's 48 per MMA
-// (profiles/sweep_tc_trace_r2.txt, ncu source page).
+// One lane of a converged warp: the producer warp runs its loop warp-uniform and issues from the elected lane.
 __device__ __forceinline__ bool stc_elect_one() {
     uint32_t pred;
     asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.b32 %0, 1, 0, P;\n\t}" : "=r"(pred));
     return pred != 0;
-}
-__device__ __forceinline__ void stc_tma_2d(uint32_t dst, const CUtensorMap *map, uint32_t bar, int c0, int c1) {
-    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-                 ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1) : "memory");
 }
 __device__ __forceinline__ void stc_tma_3d(uint32_t dst, const CUtensorMap *map, uint32_t bar, int c0, int c1, int c2) {
     asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
@@ -124,26 +107,6 @@ __device__ __forceinline__ void stc_tma_4d(uint32_t dst, const CUtensorMap *map,
 __device__ __forceinline__ void stc_prefetch_map(const CUtensorMap *map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
-__device__ __forceinline__ void stc_mma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// A operand from tensor memory (128 lanes = rows, one 32-bit column per k), B from shared memory
-__device__ __forceinline__ void stc_mma_tf32_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void stc_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void stc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void stc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void stc_cluster_sync() {
     asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
     asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
@@ -158,30 +121,20 @@ __device__ __forceinline__ float4 stc_ld_cluster_f4(uint32_t addr) {
     asm volatile("ld.shared::cluster.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
     return v;
 }
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (8-row x 128-byte atoms 1024 bytes apart), as gemm_tc.cu
-__device__ __forceinline__ uint64_t stc_smem_desc(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3ffff) >> 4);
-    d |= (uint64_t)1 << 16;
-    d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
-__device__ __forceinline__ uint32_t stc_idesc(int m, int n) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
-}
+// named barrier of the 256 consumer threads (barrier 0 is __syncthreads)
+__device__ __forceinline__ void stc_consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
 // ---------------------------------------------------------------------------------------------------
-// grid = (4 K-slices [cluster], MT * NS, ndir); 8 warps:
-//   warp 0 lane 0 : TMA producer -- W (hi+lo stack, one 3-D box) as soon as a ring slot is free, even across the step
-//                   boundary; the state tiles (hi from the output array, lo from the ring) once the counter barrier
-//                   of the previous step has been seen;
-//   warp 1 lane 0 : MMA issuer (owns the tensor-memory allocation): 4 k-steps x 3 products per k-block;
-//   all 8 warps   : tensor memory -> shared partial, cluster barrier, split-K reduction over DSMEM, epilogue
-//                   (state, its low half for the next step, one counter arrival per CTA).
+// grid = (cs K-slices [cluster], MT * NS, ndir); NP = utterances per split (the wgmma N, a multiple of 32); 9 warps:
+//   warp 8 (elected lane) : TMA producer -- W (hi+lo stack, one 3-D box) as soon as a ring slot is free, even across
+//                   the step boundary; the state tiles (hi and lo, one 4-D box) once the counter barrier of the
+//                   previous step has been seen;
+//   warps 0-7     : two warpgroups, units 0..63 / 64..127 of the tile: 4 k-steps x 3 wgmma per k-block, the
+//                   accumulator in registers; then registers -> shared partial, cluster barrier, split-K reduction over
+//                   DSMEM, epilogue (state, its low half for the next step, one counter arrival per CTA).
 // There is no generic-proxy write into the operand ring: both halves of both operands arrive by TMA.
 // ---------------------------------------------------------------------------------------------------
+template <int NP>
 __global__ void __launch_bounds__(STC_THREADS, 1)
 sweep_tc_kernel(const __grid_constant__ CUtensorMap tmW0, const __grid_constant__ CUtensorMap tmW1,
                 const __grid_constant__ CUtensorMap tmR0, const __grid_constant__ CUtensorMap tmR1, SweepTcArgs a) {
@@ -189,144 +142,90 @@ sweep_tc_kernel(const __grid_constant__ CUtensorMap tmW0, const __grid_constant_
     uint8_t *base = (uint8_t *)(((uintptr_t)stc_smem + 1023) & ~(uintptr_t)1023);
     const int STAGES = a.stages;
     const uint32_t stage_bytes = a.stage_bytes;
-    const uint32_t B_BYTES = (uint32_t)a.Npad * 128u;
-    // resident mode: [W lo: nkb x 16 KB][state ring]; streaming mode: [ring of (W hi, W lo, S hi, S lo)]
-    uint8_t *wres = base;
-    if (a.resident) base += (size_t)a.nkb * STC_A_BYTES;
-    const uint32_t s_off = a.resident ? 0u : 2 * STC_A_BYTES;         // where the state tiles sit inside a stage
+    constexpr uint32_t B_BYTES = (uint32_t)NP * 128u;
+    constexpr uint32_t s_off = 2 * STC_A_BYTES;                      // where the state tiles sit inside a stage
     uint8_t *after_ring = base + (size_t)STAGES * stage_bytes;
-    // the partial product [Npad][128] has a region of its own when it fits (then W tiles of the NEXT step may land in
+    // the partial product [NP][128] has a region of its own when it fits (then W tiles of the NEXT step may land in
     // the ring while peers still read this CTA's partial); otherwise it aliases the ring and nothing is prefetched
     float *partial = reinterpret_cast<float *>(a.partial_own ? after_ring : base);
-    uint64_t *bars = reinterpret_cast<uint64_t *>(after_ring + (a.partial_own ? (size_t)a.Npad * 512 : 0));
-    uint64_t *fullW = bars, *fullS = bars + 8, *empty = bars + 16, *done = bars + 24, *resbar = bars + 26;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bars + 25);
-    volatile int *dead = reinterpret_cast<volatile int *>(tmem_slot + 1);
+    uint64_t *bars = reinterpret_cast<uint64_t *>(after_ring + (a.partial_own ? (size_t)NP * 512 : 0));
+    uint64_t *fullW = bars, *fullS = bars + 8, *empty = bars + 16;
+    volatile int *dead = reinterpret_cast<volatile int *>(bars + 24);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int rank = blockIdx.x;                                      // K-slice = rank in cluster
     const int mt = blockIdx.y % a.MT, ns = blockIdx.y / a.MT;
     const int dir = blockIdx.z;
-    const int B = a.B, T = a.T, H = a.H, Npad = a.Npad, nkb = a.nkb;
+    const int B = a.B, T = a.T, H = a.H, nkb = a.nkb;
     const int m0 = mt * STC_BM;
-    const int b_lo = ns * Npad;
-    const int Nc = Npad / STC_CS;                                     // utterance columns this CTA finalises
+    const int b_lo = ns * NP;
+    const int Nc = NP / a.cs;                                         // utterance columns this CTA finalises (<= 64)
     const bool bptt = (a.mode == 1);
     const bool ascending = (dir == 0) != bptt;
     const CUtensorMap *tmW = dir ? &tmW1 : &tmW0;
     // the state as the next step reads it: ring[parity][plane: 0 = value, 1 = low half][B][H]; ONE 4-D box fetches both
-    // planes of a k-block.  (Measured: two alternating tensor maps per k-block -- the output array for the values, a
-    // ring for the low halves -- made the TMA unit deliver one k-block per ~1250 cycles whatever its size; a single
-    // map per operand removes the descriptor switches.)
+    // planes of a k-block
     const CUtensorMap *tmR = dir ? &tmR1 : &tmR0;
     float *out = a.out[dir];
     float *ring = a.ring[dir];                                        // [2 parities][2 planes][B][H]
     const float *act = a.act[dir];
     unsigned int *ctr = a.counters + (dir * a.NS + ns);
-    const unsigned int domain = (unsigned int)(STC_CS * a.MT);        // CTAs that share this counter
+    const unsigned int domain = (unsigned int)(a.cs * a.MT);          // CTAs that share this counter
 
     if (tid == 0) {
         for (int s = 0; s < STAGES; ++s) {
             stc_mbar_init(stc_smem_u32(&fullW[s]), 1);
             stc_mbar_init(stc_smem_u32(&fullS[s]), 1);
-            stc_mbar_init(stc_smem_u32(&empty[s]), 1);
+            stc_mbar_init(stc_smem_u32(&empty[s]), 8);                // one arrival per consumer warp
         }
-        stc_mbar_init(stc_smem_u32(done), 1);
-        stc_mbar_init(stc_smem_u32(resbar), 1);
         *dead = 0;
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         stc_prefetch_map(tmW);
         stc_prefetch_map(tmR);
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(stc_smem_u32(tmem_slot)), "r"(a.tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    stc_fence_before();
     __syncthreads();
-    stc_fence_after();
-    const uint32_t tmem_a = *tmem_slot;                               // resident mode: W hi in columns [0, 32 nkb)
-    const uint32_t tmem_d = tmem_a + (a.resident ? (uint32_t)(32 * a.nkb) : 0u);
-    if (a.resident) {
-        // ---- one-time load of this CTA's 128 x (H/4) slice of W: lo half by TMA into shared memory ...
-        if (tid == 0) {
-            const uint32_t rb = stc_smem_u32(resbar);
-            stc_mbar_expect_tx(rb, (uint32_t)a.nkb * STC_A_BYTES);
-            for (int i = 0; i < a.nkb; ++i)
-                stc_tma_3d(stc_smem_u32(wres + (size_t)i * STC_A_BYTES), dir ? &tmW1 : &tmW0, rb, (blockIdx.x * a.nkb + i) * STC_BK, (blockIdx.y % a.MT) * STC_BM, 1);
-        }
-        // ---- ... hi half into tensor memory: warp w owns lanes 32 (w % 4) .. +31 (rows), warps 0-3 / 4-7 the two
-        //      halves of the columns; a thread stores 32 consecutive k of its row per tcgen05.st
-        const int row = (blockIdx.y % a.MT) * STC_BM + 32 * (warp & 3) + lane;
-        const float *wrow = a.whi[dir] + (int64_t)row * a.H + (int64_t)blockIdx.x * a.nkb * STC_BK;
-        const int ncols = 32 * a.nkb, chalf = ncols / 2;
-        for (int c0 = (warp >> 2) * chalf; c0 < (warp >> 2) * chalf + chalf; c0 += 32) {
-            uint32_t r[32];
-#pragma unroll
-            for (int q = 0; q < 8; ++q) {
-                const float4 v = __ldg(reinterpret_cast<const float4 *>(wrow + c0) + q);
-                r[4 * q] = __float_as_uint(v.x); r[4 * q + 1] = __float_as_uint(v.y);
-                r[4 * q + 2] = __float_as_uint(v.z); r[4 * q + 3] = __float_as_uint(v.w);
-            }
-            const uint32_t taddr = tmem_a + ((uint32_t)(32 * (warp & 3)) << 16) + (uint32_t)c0;
-            asm volatile(
-                "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-                "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-                "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-                ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-                  "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]),
-                  "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]),
-                  "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31]) : "memory");
-        }
-        asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-        stc_mbar_wait(stc_smem_u32(resbar), 0, dead, a.err);
-        stc_fence_before();
-        __syncthreads();
-        stc_fence_after();
-    }
     stc_cluster_sync();
 
-    // epilogue role: warp w takes columns c = w, w + 8, ... < Nc of this CTA's quarter; lane l owns units 4l..4l+3
+    // epilogue role (warps 0-7): warp w takes columns c = w, w + 8, ... < Nc of this CTA's quarter; lane l owns units 4l..4l+3
     const int j4 = m0 + 4 * lane;
     // ring bookkeeping in units of k-block jobs g = (s - 1) * nkb + i (s = 1 .. T-1): stage g % STAGES, use g / STAGES
     uint32_t gW = 0;              // producer: next job whose W tiles have not been requested yet
 
-    // The 8 (16) M-tile CTAs of a (direction, split, K-slice) all need the SAME state tiles: each starts its walk over the
-    // k-blocks at a different one, so that they do not ask L2 for the same lines at the same moment.
-    const int kb_rot = a.rotate ? mt : 0;
-    auto kb_of = [&](uint32_t g) { return (int)((g % (uint32_t)nkb + (uint32_t)kb_rot) % (uint32_t)nkb); };
     // issue the W tiles (hi + lo in one 3-D box) of job g; the caller guarantees the slot is free
     auto issue_W = [&](uint32_t g) {
         const int st = (int)(g % (uint32_t)STAGES);
         const uint32_t fb = stc_smem_u32(&fullW[st]);
         stc_mbar_expect_tx(fb, 2 * STC_A_BYTES);
-        const int i = kb_of(g);
+        const int i = (int)(g % (uint32_t)nkb);
         stc_tma_3d(stc_smem_u32(base + (size_t)st * stage_bytes), tmW, fb, (rank * nkb + i) * STC_BK, m0, 0);   // both planes
     };
 
     for (int s = 0; s < T; ++s) {
         const int t = ascending ? s : T - 1 - s;
-        const int tprev = ascending ? t - 1 : t + 1;
-        // operands of the epilogue that do not depend on the recurrence: issued before the waits
+        // operands of the epilogue that do not depend on the recurrence: loaded once the MMAs of the step are done (they
+        // would otherwise hold 72 registers across the MMA loop), so that they travel during the cluster barrier
         float4 pre_v[8], act_v[8];
         int Tb[8];
+        auto load_epilogue_operands = [&]() {
 #pragma unroll
-        for (int ci = 0; ci < 8; ++ci) {
-            const int c = warp + 8 * ci;
-            const int b = b_lo + rank * Nc + c;
-            pre_v[ci] = make_float4(0.f, 0.f, 0.f, 0.f);
-            act_v[ci] = pre_v[ci];
-            Tb[ci] = 0;
-            if (c < Nc && b < B) {
-                const int64_t o = ((int64_t)t * B + b) * H + j4;
-                pre_v[ci] = __ldg(reinterpret_cast<const float4 *>(a.pre + o));
-                if (bptt) act_v[ci] = __ldg(reinterpret_cast<const float4 *>(act + o));
-                Tb[ci] = __ldg(a.Tlen + b);
+            for (int ci = 0; ci < 8; ++ci) {
+                const int c = warp + 8 * ci;
+                const int b = b_lo + rank * Nc + c;
+                pre_v[ci] = make_float4(0.f, 0.f, 0.f, 0.f);
+                act_v[ci] = pre_v[ci];
+                Tb[ci] = 0;
+                if (warp < 8 && c < Nc && b < B) {
+                    const int64_t o = ((int64_t)t * B + b) * H + j4;
+                    pre_v[ci] = __ldg(reinterpret_cast<const float4 *>(a.pre + o));
+                    if (bptt) act_v[ci] = __ldg(reinterpret_cast<const float4 *>(act + o));
+                    Tb[ci] = __ldg(a.Tlen + b);
+                }
             }
-        }
+        };
+        if (s == 0) load_epilogue_operands();
         if (s > 0) {
             const uint32_t g0 = (uint32_t)(s - 1) * (uint32_t)nkb, g1 = g0 + (uint32_t)nkb;
-            if (warp == 0) {
+            if (warp == 8) {
                 // ---------------------------------------------------- TMA producer (whole warp, elected issue)
                 const bool leader = stc_elect_one();
                 if (leader) STC_STAMP(0);
@@ -346,101 +245,80 @@ sweep_tc_kernel(const __grid_constant__ CUtensorMap tmW0, const __grid_constant_
                 for (uint32_t g = g0; g < g1; ++g) {
                     const int st = (int)(g % (uint32_t)STAGES);
                     const uint32_t use = g / (uint32_t)STAGES;
-                    const bool need_w = !a.resident && g >= gW;
-                    if ((a.resident || need_w) && use > 0) stc_mbar_wait(stc_smem_u32(&empty[st]), (use - 1) & 1, dead, a.err);
+                    const bool need_w = g >= gW;
+                    if (need_w && use > 0) stc_mbar_wait(stc_smem_u32(&empty[st]), (use - 1) & 1, dead, a.err);
                     if (need_w) gW = g + 1;
                     const uint32_t fb = stc_smem_u32(&fullS[st]);
                     const uint32_t sdst = stc_smem_u32(base + (size_t)st * stage_bytes + s_off);
-                    const int kc = (rank * nkb + kb_of(g)) * STC_BK;
-                    if (leader && a.nomma != 2) {
+                    const int kc = (rank * nkb + (int)(g % (uint32_t)nkb)) * STC_BK;
+                    if (leader) {
                         if (need_w) issue_W(g);
                         stc_mbar_expect_tx(fb, 2 * B_BYTES);
                         stc_tma_4d(sdst, tmR, fb, kc, b_lo, 0, (s - 1) & 1);
                     }
+                    __syncwarp();
                 }
                 if (leader) STC_STAMP(2);
+                if (a.partial_own && s + 1 < T) {
+                    // request the first W tiles of the NEXT step as their slots come free -- they travel while this
+                    // CTA finishes its MMAs, reduces, stores and waits at the counter barrier
+                    const uint32_t gend = g1 + (uint32_t)((nkb < STAGES) ? nkb : STAGES);
+                    for (uint32_t g = g1; g < gend; ++g) {
+                        const int st = (int)(g % (uint32_t)STAGES);
+                        const uint32_t use = g / (uint32_t)STAGES;
+                        if (use > 0) stc_mbar_wait(stc_smem_u32(&empty[st]), (use - 1) & 1, dead, a.err);
+                        if (leader) issue_W(g);
+                        __syncwarp();
+                    }
+                    gW = gend;
+                }
                 __syncwarp();
-            } else if (warp == 1) {
-                // ---------------------------------------------------- MMA issuer (whole warp, elected issue)
-                const bool leader = stc_elect_one();
-                const uint32_t idesc = stc_idesc(STC_BM, Npad);
+            } else {
+                // ---------------------------------------------------- consumers: warpgroup cw, units 64 cw .. 64 cw + 63
+                const int cw = warp >> 2;
+                float acc[NP / 2];        // per step: dead once the partial is written
+#pragma unroll
+                for (int i = 0; i < NP / 2; ++i) acc[i] = 0.f;
                 for (uint32_t g = g0; g < g1; ++g) {
                     const int st = (int)(g % (uint32_t)STAGES);
                     const uint32_t use = g / (uint32_t)STAGES;
-                    if (!a.resident && a.nomma != 2) stc_mbar_wait(stc_smem_u32(&fullW[st]), use & 1, dead, a.err);
-                    if (a.nomma != 2) stc_mbar_wait(stc_smem_u32(&fullS[st]), use & 1, dead, a.err);
-                    // ONE tcgen05 fence per step (it orders this step's MMAs behind the epilogue's tensor-memory reads of
-                    // the previous one)
-                    if (g == g0) stc_fence_after();
+                    stc_mbar_wait(stc_smem_u32(&fullW[st]), use & 1, dead, a.err);
+                    stc_mbar_wait(stc_smem_u32(&fullS[st]), use & 1, dead, a.err);
+                    if (tid == 0 && g == g0) STC_STAMP(3);
                     const uint32_t sa = stc_smem_u32(base + (size_t)st * stage_bytes);
-                    const uint64_t dB = stc_smem_desc(sa + s_off), dBl = stc_smem_desc(sa + s_off + B_BYTES);
-                    const int i = kb_of(g);
-                    const uint64_t dAlr = stc_smem_desc(stc_smem_u32(wres + (size_t)i * STC_A_BYTES));
-                    const uint64_t dA = stc_smem_desc(sa), dAl = stc_smem_desc(sa + STC_A_BYTES);
-                    const uint32_t ta = tmem_a + (uint32_t)(32 * i);
-                    const uint32_t eb = stc_smem_u32(&empty[st]);
-                    if (leader) {
-                        if (g == g0) STC_STAMP(3);
-                        if (g == g0 + 1) STC_STAMP(14);
-                        if (g == g0 + 4) STC_STAMP(15);
-                        if (a.nomma == 1) {
-                        } else if (a.resident) {
+                    const uint64_t dA = wg_desc(sa + (uint32_t)cw * (64 * 128)), dAl = wg_desc(sa + STC_A_BYTES + (uint32_t)cw * (64 * 128));
+                    const uint64_t dB = wg_desc(sa + s_off), dBl = wg_desc(sa + s_off + B_BYTES);
+                    wg_fence();
 #pragma unroll
-                            for (int k8 = 0; k8 < STC_BK / 8; ++k8) {
-                                const uint64_t adv = (uint64_t)((k8 * 32) >> 4);
-                                stc_mma_tf32(tmem_d, dAlr + adv, dB + adv, idesc, (g > g0 || k8 > 0) ? 1u : 0u);     // lo . hi
-                                stc_mma_tf32_ts(tmem_d, ta + 8 * k8, dBl + adv, idesc, 1u);                         // hi . lo
-                                stc_mma_tf32_ts(tmem_d, ta + 8 * k8, dB + adv, idesc, 1u);                          // hi . hi
-                            }
-                        } else {
-#pragma unroll
-                            for (int k8 = 0; k8 < STC_BK / 8; ++k8) {
-                                const uint64_t adv = (uint64_t)((k8 * 32) >> 4);
-                                stc_mma_tf32(tmem_d, dAl + adv, dB + adv, idesc, (g > g0 || k8 > 0) ? 1u : 0u);   // lo . hi
-                                stc_mma_tf32(tmem_d, dA + adv, dBl + adv, idesc, 1u);                               // hi . lo
-                                stc_mma_tf32(tmem_d, dA + adv, dB + adv, idesc, 1u);                                // hi . hi
-                            }
-                        }
-                        if (g == g0) STC_STAMP(13);
-                        stc_commit(eb);
+                    for (int k8 = 0; k8 < STC_BK / 8; ++k8) {
+                        const uint64_t adv = (uint64_t)((k8 * 32) >> 4);
+                        WgmmaTf32<NP>::mma(acc, dAl + adv, dB + adv, (g > g0 || k8 > 0) ? 1u : 0u);   // lo . hi
+                        WgmmaTf32<NP>::mma(acc, dA + adv, dBl + adv, 1u);                           // hi . lo
+                        WgmmaTf32<NP>::mma(acc, dA + adv, dB + adv, 1u);                            // hi . hi
                     }
-                    __syncwarp();
+                    wg_commit();
+                    // the previous job's MMAs are complete once at most this one is outstanding: release its slot
+                    wg_wait<1>();
+                    if (g > g0) {
+                        __syncwarp();
+                        if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(stc_smem_u32(&empty[(g - 1) % (uint32_t)STAGES])) : "memory");
+                    }
                 }
-                if (leader) {
-                    stc_commit(stc_smem_u32(done));
-                    STC_STAMP(4);
-                }
+                wg_wait<0>();
                 __syncwarp();
-            }
-            __syncwarp();
-            // -------------------------------------------------------- partial product: tensor memory -> shared
-            stc_mbar_wait(stc_smem_u32(done), (uint32_t)((s - 1) & 1), dead, a.err);
-            stc_fence_after();
-            if (tid == 64) STC_STAMP(5);
-            if (warp == 0 && a.partial_own && !a.resident && s + 1 < T) {
-                // every MMA of this step is complete, so every ring slot is free: request the first W tiles of the NEXT
-                // step now -- they travel while this CTA reduces, stores and waits at the counter barrier
-                const uint32_t gend = g1 + (uint32_t)((nkb < STAGES) ? nkb : STAGES);
-                if (stc_elect_one() && a.nomma != 2)
-                    for (uint32_t g = g1; g < gend; ++g) issue_W(g);
-                gW = gend;
-                __syncwarp();
-            }
-            {
-                const int q = warp & 3, half = warp >> 2;
-                const int cbeg = half * (Npad / 2), cend = cbeg + Npad / 2;
-                for (int c0 = cbeg; c0 < cend; c0 += 8) {
-                    uint32_t r[8];
-                    const uint32_t taddr = tmem_d + ((uint32_t)(q * 32) << 16) + (uint32_t)c0;
-                    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-                                 : "r"(taddr) : "memory");
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+                if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(stc_smem_u32(&empty[(g1 - 1) % (uint32_t)STAGES])) : "memory");
+                if (tid == 0) STC_STAMP(4);
+                // ---------------------------------------------------- partial product: registers -> shared
+                if (!a.partial_own) stc_consumer_sync();     // the partial aliases the ring: both warpgroups are done with it
+                const int q = warp & 3;
+                const int u0 = 64 * cw + 16 * q + (lane >> 2);
 #pragma unroll
-                    for (int i = 0; i < 8; ++i) partial[(c0 + i) * STC_BM + q * 32 + lane] = __uint_as_float(r[i]);
+                for (int i = 0; i < NP / 2; ++i) {
+                    const int unit = u0 + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+                    partial[col * STC_BM + unit] = acc[i];
                 }
             }
-            stc_fence_before();
+            load_epilogue_operands();
             if (tid == 64) STC_STAMP(6);
             __syncthreads();         // implied by the cluster barrier below; stated for tools that only model CTA barriers
             stc_cluster_sync();      // all four partials of this (M tile, split) are in shared memory
@@ -451,13 +329,12 @@ sweep_tc_kernel(const __grid_constant__ CUtensorMap tmW0, const __grid_constant_
 #pragma unroll
         for (int ci = 0; ci < 8; ++ci) {
             const int c = warp + 8 * ci;
-            if (c >= Nc) continue;
+            if (warp >= 8 || c >= Nc) continue;
             const int b = b_lo + rank * Nc + c;
             float4 sum = make_float4(0.f, 0.f, 0.f, 0.f);
             if (s > 0) {
                 const uint32_t local = stc_smem_u32(partial + (rank * Nc + c) * STC_BM + 4 * lane);
-#pragma unroll
-                for (int q = 0; q < STC_CS; ++q) {
+                for (int q = 0; q < a.cs; ++q) {
                     const float4 p = stc_ld_cluster_f4(stc_map_to_cta(local, (uint32_t)q));
                     sum.x += p.x; sum.y += p.y; sum.z += p.z; sum.w += p.w;
                 }
@@ -495,21 +372,14 @@ sweep_tc_kernel(const __grid_constant__ CUtensorMap tmW0, const __grid_constant_
                 STC_STAMP(9);
                 // release: the CTA's state stores (ordered before this thread by the barrier above) become visible at
                 // device scope before the count does.  The generic->async proxy fence belongs to the READER (after its
-                // acquire, before its TMA loads); a second one here only cost ~500 cycles per step (CTCB_SWEEP_TC_WFENCE=1
-                // brings it back).
-                if (a.wfence) asm volatile("fence.proxy.async;" ::: "memory");
+                // acquire, before its TMA loads).
                 asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(ctr), "r"(1u) : "memory");
                 STC_STAMP(10);
             }
         }
     }
     // no CTA may exit while a peer can still read its shared memory
-    stc_fence_before();
     stc_cluster_sync();
-    if (warp == 1) {
-        stc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_a), "r"(a.tmem_cols) : "memory");
-    }
 }
 
 // Operand preparation, once per launch: out[0] = W (or W^T for BPTT), out[1] = its low half x - tf32(x); both H x H
@@ -556,84 +426,76 @@ static StcEncodeFn stc_encode() {
     return fn;
 }
 
-struct StcPlan { int NS, Npad, stages, tmem_cols, partial_own, resident; uint32_t stage_bytes; size_t smem; };
+struct StcPlan { int cs, NS, Npad, stages, partial_own; uint32_t stage_bytes; size_t smem; };
 
-static int stc_max_clusters(size_t smem) {
-    static int cached = -1;
-    if (cached >= 0) return cached;
+static constexpr size_t STC_SMEM_MAX = 208 * 1024;      // ring + partial budget (+ barriers) within the 227 KB per CTA
+
+// co-resident clusters of cs CTAs (the kernel's shared memory does not depend on NP for this question: every plan
+// uses about STC_SMEM_MAX, so one CTA per SM)
+static int stc_max_clusters(int cs) {
+    static int cached[5] = {-1, -1, -1, -1, -1};
+    if (cached[cs] >= 0) return cached[cs];
+    const size_t smem = STC_SMEM_MAX + 2048;
     cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(STC_CS, 64, 2);
+    cfg.gridDim = dim3(cs, 64, 2);
     cfg.blockDim = dim3(STC_THREADS);
     cfg.dynamicSmemBytes = smem;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = STC_CS; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+    attr[0].val.clusterDim.x = cs; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr; cfg.numAttrs = 1;
     int n = 0;
-    if (cudaFuncSetAttribute(sweep_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess ||
-        cudaOccupancyMaxActiveClusters(&n, sweep_tc_kernel, &cfg) != cudaSuccess) {
+    if (cudaFuncSetAttribute(sweep_tc_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess ||
+        cudaOccupancyMaxActiveClusters(&n, sweep_tc_kernel<256>, &cfg) != cudaSuccess) {
         cudaGetLastError();
         n = 0;
     }
-    cached = n;
-    if (getenv("CTCB_DEBUG")) fprintf(stderr, "[ctcb] tensor-core sweep: max active clusters of %d CTAs = %d\n", STC_CS, n);
-    return cached;
+    cached[cs] = n;
+    if (getenv("CTCB_DEBUG")) fprintf(stderr, "[ctcb] tensor-core sweep: max active clusters of %d CTAs = %d\n", cs, n);
+    return n;
 }
 
-static constexpr size_t STC_SMEM_MAX = 208 * 1024;      // ring + partial budget (+ barriers) within the 227 KB per CTA
-
-static bool stc_plan(int H, int B, int ndir, StcPlan *p) {
-    if (H % 128 != 0 || H < 512 || B < 1) return false;
+// Per cluster size, largest first: every CTA of the grid must be co-resident (they meet at the counter barrier), and a
+// CTA finalises at most 64 utterance columns (NP / cs <= 64).
+static bool stc_plan_cs(int H, int B, int ndir, int cs, StcPlan *p) {
     const int MT = H / STC_BM;
-    const int maxc = stc_max_clusters(STC_SMEM_MAX + 2048);
+    if ((H / cs) % STC_BK != 0) return false;
+    const int maxc = stc_max_clusters(cs);
     if (maxc < ndir * MT) return false;
     int ns_cap = maxc / (ndir * MT);
     static int ns_env = -1;
     if (ns_env < 0) { const char *e = getenv("CTCB_SWEEP_TC_NS"); ns_env = e ? atoi(e) : 0; }
     if (ns_env > 0 && ns_env < ns_cap) ns_cap = ns_env;
-    int NS = (B + 15) / 16;                  // never more splits than 16-utterance MMA tiles
+    int NS = (B + 15) / 16;                  // never more splits than 16-utterance groups
     if (NS > ns_cap) NS = ns_cap;
     if (NS < 1) NS = 1;
-    int Npad = ((B + NS - 1) / NS + 15) / 16 * 16;
-    if (Npad > 256) return false;            // would need a second utterance group per CTA and step
-    NS = (B + Npad - 1) / Npad;              // drop splits that would be empty
-    p->NS = NS; p->Npad = Npad;
+    const int Npad = ((B + NS - 1) / NS + 31) / 32 * 32;   // the wgmma N of the kernel: a multiple of 32 up to 256
+    if (Npad > 256 || Npad > 64 * cs) return false;
+    p->cs = cs;
+    p->NS = (B + Npad - 1) / Npad;           // drop splits that would be empty
+    p->Npad = Npad;
     const size_t partial_bytes = (size_t)Npad * 512;
-    {   // resident W: hi in tensor memory (H/4 columns beside the Npad accumulator columns), lo in shared memory
-        static int res_env = -1;   // CTCB_SWEEP_TC_RESIDENT=0 forces the streaming kernel
-        if (res_env < 0) { const char *e = getenv("CTCB_SWEEP_TC_RESIDENT"); res_env = e ? atoi(e) : 1; }
-        const int nkb = H / STC_CS / STC_BK;
-        const size_t wlo = (size_t)nkb * STC_A_BYTES;
-        const uint32_t sstage = 2 * (uint32_t)Npad * 128u;
-        if (res_env && 32 * nkb + Npad <= 512 && wlo + 2 * (size_t)sstage <= STC_SMEM_MAX && wlo + partial_bytes <= STC_SMEM_MAX) {
-            p->resident = 1;
-            p->partial_own = 0;                    // the partial aliases the state ring (nothing is prefetched into it)
-            p->stage_bytes = sstage;
-            int stages = (int)((STC_SMEM_MAX - wlo) / sstage);
-            if (stages > 6) stages = 6;
-            while ((size_t)stages * sstage < partial_bytes) ++stages;     // the ring must hold the aliased partial
-            if (wlo + (size_t)stages * sstage > STC_SMEM_MAX + 8192) return false;
-            p->stages = stages;
-            p->tmem_cols = 512;
-            p->smem = wlo + (size_t)stages * sstage + 512 + 1024;
-            return true;
-        }
-    }
-    p->resident = 0;
     p->stage_bytes = 2 * STC_A_BYTES + 2 * (uint32_t)Npad * 128u;
-    static int pf_env = -1;   // CTCB_SWEEP_TC_PREFETCH=0: never give the partial its own region (no W prefetch across steps)
-    if (pf_env < 0) { const char *e = getenv("CTCB_SWEEP_TC_PREFETCH"); pf_env = e ? atoi(e) : 1; }
     // own region for the partial when at least two ring stages still fit beside it
-    p->partial_own = (pf_env && STC_SMEM_MAX >= partial_bytes + 2 * (size_t)p->stage_bytes) ? 1 : 0;
+    p->partial_own = (STC_SMEM_MAX >= partial_bytes + 2 * (size_t)p->stage_bytes) ? 1 : 0;
     int stages = (int)((STC_SMEM_MAX - (p->partial_own ? partial_bytes : 0)) / p->stage_bytes);
     if (stages > 6) stages = 6;
     if (stages < 2) return false;
+    if (!p->partial_own && (size_t)stages * p->stage_bytes < partial_bytes) return false;    // the ring must hold the aliased partial
     p->stages = stages;
-    int cols = 32;
-    while (cols < Npad) cols <<= 1;
-    p->tmem_cols = cols;
-    p->smem = (size_t)stages * p->stage_bytes + (p->partial_own ? partial_bytes : 0) + 512 + 1024;
+    p->smem = (size_t)stages * p->stage_bytes + (p->partial_own ? partial_bytes : 0) + 256 + 1024;
     return true;
+}
+
+static bool stc_plan(int H, int B, int ndir, StcPlan *p) {
+    if (H % 128 != 0 || H < 512 || B < 1) return false;
+    for (int cs = 4; cs >= 1; cs >>= 1)
+        if (stc_plan_cs(H, B, ndir, cs, p)) {
+            if (getenv("CTCB_DEBUG"))
+                fprintf(stderr, "[ctcb] tensor-core sweep H=%d B=%d: clusters of %d, %d utterance split(s) of %d\n", H, B, cs, p->NS, p->Npad);
+            return true;
+        }
+    return false;
 }
 
 static bool stc_enabled(int H) {
@@ -650,6 +512,25 @@ size_t sweep_tc_workspace_bytes(int H, int B) {
     return stc_ws_stack_bytes(H) + stc_ws_ring_bytes(H, B) + STC_TRACE_STEPS * 16 * 8 + 1024;
 }
 
+template <int NP>
+static cudaError_t stc_launch(cudaLaunchConfig_t *cfg, const CUtensorMap *tmW, const CUtensorMap *tmR, const SweepTcArgs &a) {
+    cudaError_t e = cudaFuncSetAttribute(sweep_tc_kernel<NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg->dynamicSmemBytes);
+    if (e != cudaSuccess) return e;
+    return cudaLaunchKernelEx(cfg, sweep_tc_kernel<NP>, tmW[0], tmW[1], tmR[0], tmR[1], a);
+}
+static cudaError_t stc_launch_np(int np, cudaLaunchConfig_t *cfg, const CUtensorMap *tmW, const CUtensorMap *tmR, const SweepTcArgs &a) {
+    switch (np) {
+        case 32: return stc_launch<32>(cfg, tmW, tmR, a);
+        case 64: return stc_launch<64>(cfg, tmW, tmR, a);
+        case 96: return stc_launch<96>(cfg, tmW, tmR, a);
+        case 128: return stc_launch<128>(cfg, tmW, tmR, a);
+        case 160: return stc_launch<160>(cfg, tmW, tmR, a);
+        case 192: return stc_launch<192>(cfg, tmW, tmR, a);
+        case 224: return stc_launch<224>(cfg, tmW, tmR, a);
+        default: return stc_launch<256>(cfg, tmW, tmR, a);
+    }
+}
+
 int run_sweep_tc(int mode, int T, int B, int H, const int32_t *Tlen, const float *pre, const float *Wf, const float *Wb,
                  float *outF, float *outB, const float *actF, const float *actB, float maxAct, unsigned int *counters,
                  void *ws, size_t ws_bytes, cudaStream_t st, bool *handled) {
@@ -657,7 +538,10 @@ int run_sweep_tc(int mode, int T, int B, int H, const int32_t *Tlen, const float
     const int ndir = Wb ? 2 : 1;
     StcPlan p;
     if (!stc_enabled(H) || !stc_plan(H, B, ndir, &p)) return CTCB_OK;
-    if (!ws || ws_bytes < sweep_tc_workspace_bytes(H, B) || (((uintptr_t)ws) & 255)) return CTCB_OK;   // no scratch: other kernels
+    // the plan applies, so the generic kernel is no substitute: a scratch that cannot hold the operand stacks is an error
+    if (!ws || ws_bytes < sweep_tc_workspace_bytes(H, B) || (((uintptr_t)ws) & 255))
+        return set_error(CTCB_ENOMEM, "tensor-core sweep (H=%d, B=%d) needs %zu bytes of 256-byte aligned scratch, got %zu%s",
+                         H, B, sweep_tc_workspace_bytes(H, B), ws_bytes, ws ? "" : " (none)");
     StcEncodeFn enc = stc_encode();
     float *stack = (float *)ws;
     float *ring = (float *)((char *)ws + stc_ws_stack_bytes(H));
@@ -673,7 +557,7 @@ int run_sweep_tc(int mode, int T, int B, int H, const int32_t *Tlen, const float
         {
             cuuint64_t dims[3] = {(cuuint64_t)H, (cuuint64_t)H, 2};
             cuuint64_t strides[2] = {(cuuint64_t)H * sizeof(float), (cuuint64_t)H * H * sizeof(float)};
-            cuuint32_t box[3] = {(cuuint32_t)STC_BK, (cuuint32_t)STC_BM, (cuuint32_t)(p.resident ? 1 : 2)};   // resident: lo plane only
+            cuuint32_t box[3] = {(cuuint32_t)STC_BK, (cuuint32_t)STC_BM, 2};
             cuuint32_t es[3] = {1, 1, 1};
             CUresult r = enc(&tmW[d], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, (void *)(stack + (size_t)dd * 2 * H * H), dims, strides, box, es,
                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -696,13 +580,8 @@ int run_sweep_tc(int mode, int T, int B, int H, const int32_t *Tlen, const float
     a.out[0] = outs[0]; a.out[1] = outs[1]; a.act[0] = actF; a.act[1] = Wb ? actB : actF; a.maxAct = maxAct;
     a.ring[0] = ring; a.ring[1] = ring + (size_t)(ndir - 1) * 4 * B * H;
     a.err = counters; a.counters = counters + 16;
-    a.ndir = ndir; a.MT = H / STC_BM; a.NS = p.NS; a.Npad = p.Npad; a.nkb = H / STC_CS / STC_BK;
-    a.stages = p.stages; a.stage_bytes = p.stage_bytes; a.tmem_cols = (uint32_t)p.tmem_cols; a.partial_own = p.partial_own;
-    a.resident = p.resident;
-    { static int wf = -1; if (wf < 0) { const char *e = getenv("CTCB_SWEEP_TC_WFENCE"); wf = e ? atoi(e) : 0; } a.wfence = wf; }
-    { static int ro = -1; if (ro < 0) { const char *e = getenv("CTCB_SWEEP_TC_ROTATE"); ro = e ? atoi(e) : 0; } a.rotate = ro; }
-    { static int nm = -1; if (nm < 0) { const char *e = getenv("CTCB_SWEEP_TC_NOMMA"); nm = e ? atoi(e) : 0; } a.nomma = nm; }
-    a.whi[0] = stack; a.whi[1] = stack + (size_t)(ndir - 1) * 2 * H * H;
+    a.ndir = ndir; a.MT = H / STC_BM; a.NS = p.NS; a.cs = p.cs; a.nkb = H / p.cs / STC_BK;
+    a.stages = p.stages; a.stage_bytes = p.stage_bytes; a.partial_own = p.partial_own;
     a.trace = nullptr;
     {
         static int trace_env = -1;
@@ -710,15 +589,14 @@ int run_sweep_tc(int mode, int T, int B, int H, const int32_t *Tlen, const float
         if (trace_env) a.trace = (unsigned long long *)((char *)ws + stc_ws_stack_bytes(H) + stc_ws_ring_bytes(H, B));
     }
     CTCB_CUDA_CHECK(cudaMemsetAsync(a.counters, 0, sizeof(unsigned int) * (size_t)(ndir * p.NS), st));
-    CTCB_CUDA_CHECK(cudaFuncSetAttribute(sweep_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
     cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(STC_CS, a.MT * p.NS, ndir);
+    cfg.gridDim = dim3(p.cs, a.MT * p.NS, ndir);
     cfg.blockDim = dim3(STC_THREADS);
     cfg.dynamicSmemBytes = p.smem;
     cfg.stream = st;
     cudaLaunchAttribute attr[2];
     attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = STC_CS; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+    attr[0].val.clusterDim.x = p.cs; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
     attr[1].id = cudaLaunchAttributeCooperative;       // co-residency of all CTAs (they meet at the counter barrier)
     attr[1].val.cooperative = 1;
     cfg.attrs = attr;
@@ -726,7 +604,7 @@ int run_sweep_tc(int mode, int T, int B, int H, const int32_t *Tlen, const float
     if (coop < 0) { const char *e = getenv("CTCB_SWEEP_TC_COOP"); if (e && atoi(e) == 0) coop = 0; }
     if (coop != 0) {
         cfg.numAttrs = 2;
-        cudaError_t e = cudaLaunchKernelEx(&cfg, sweep_tc_kernel, tmW[0], tmW[1], tmR[0], tmR[1], a);
+        cudaError_t e = stc_launch_np(p.Npad, &cfg, tmW, tmR, a);
         if (e == cudaSuccess) { coop = 1; count_launch(); *handled = true; return CTCB_OK; }
         cudaGetLastError();
         if (coop == 1) return set_error(CTCB_ECUDA, "sweep_tc: launch failed: %s", cudaGetErrorString(e));
@@ -734,7 +612,7 @@ int run_sweep_tc(int mode, int T, int B, int H, const int32_t *Tlen, const float
         if (getenv("CTCB_DEBUG")) fprintf(stderr, "[ctcb] tensor-core sweep: cooperative+cluster launch refused (%s), plain cluster launch\n", cudaGetErrorString(e));
     }
     cfg.numAttrs = 1;         // grid <= one wave of clusters by construction (stc_plan)
-    CTCB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, sweep_tc_kernel, tmW[0], tmW[1], tmR[0], tmR[1], a));
+    CTCB_CUDA_CHECK(stc_launch_np(p.Npad, &cfg, tmW, tmR, a));
     count_launch();
     *handled = true;
     return CTCB_OK;

@@ -1,5 +1,5 @@
 """ctc_fast -- drop-in for the reference's Cython module of the same name
-(/root/reference/ctc_fast/ctc-loss/ctc_fast.pyx), computed on the B200 by libctcb200.
+(ctc_fast/ctc-loss/ctc_fast.pyx), computed on the H100 by libctcb200.
 
     ctc_loss(params, seq, blank=0)        -> (nll, grad, skip)      ctc_fast.pyx:13-152
     decode_best_path(probs, blank=0)      -> (hyp, align)           ctc_fast.pyx:154-187

@@ -1,5 +1,5 @@
 """ctc_fast_blankforce -- drop-in for the reference's second Cython CTC module
-(/root/reference/ctc_fast/ctc-loss/ctc_fast_blankforce.pyx), computed on the B200 by libctcb200.
+(ctc_fast/ctc-loss/ctc_fast_blankforce.pyx), computed on the H100 by libctcb200.
 
     ctc_loss(params, seq)                 -> (nll, grad, skip)      ctc_fast_blankforce.pyx:13-113
     decode_best_path(probs, blank=0)      -> hyp                    ctc_fast_blankforce.pyx:115-142

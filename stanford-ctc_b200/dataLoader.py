@@ -1,5 +1,5 @@
 """dataLoader -- reader of the reference's Kaldi-derived training files.  Class and method names follow
-/root/reference/ctc_fast/dataLoader.py:6-95 (DataLoader, loadDataFile, loadDataFileDict,
+ctc_fast/dataLoader.py:6-95 (DataLoader, loadDataFile, loadDataFileDict,
 loadDataFileAsynch, getDataAsynch) because sgd/runNNet and the reference's own tools call them.
 
 File triple number n in a directory:

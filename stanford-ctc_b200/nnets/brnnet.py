@@ -1,5 +1,5 @@
-"""nnets.brnnet -- drop-in for /root/reference/ctc_fast/nnets/brnnet.py (class NNet), computed by
-libctcb200 on a B200.
+"""nnets.brnnet -- drop-in for ctc_fast/nnets/brnnet.py (class NNet), computed by
+libctcb200 on an H100.
 
 Same constructor, attributes and methods as the reference (brnnet.py:10-11, :34, :88, :117, :251,
 :258, :269, :279):

@@ -1,5 +1,5 @@
-"""nnets.nnet -- drop-in for /root/reference/ctc_fast/nnets/nnet.py (class NNet): the feed-forward net
-trained with CTC, computed by libctcb200 on a B200.
+"""nnets.nnet -- drop-in for ctc_fast/nnets/nnet.py (class NNet): the feed-forward net
+trained with CTC, computed by libctcb200 on an H100.
 
     NNet(inputDim, outputDim, layerSize, numLayers, maxBatch, train=True)     nnet.py:7
     costAndGrad(data, labels) -> (cost, grad, skip)                           nnet.py:57-113

@@ -1,5 +1,5 @@
-"""nnets.rnnet -- drop-in for /root/reference/ctc_fast/nnets/rnnet.py (class NNet): the uni-directional
-recurrent net, computed by libctcb200 on a B200.
+"""nnets.rnnet -- drop-in for ctc_fast/nnets/rnnet.py (class NNet): the uni-directional
+recurrent net, computed by libctcb200 on an H100.
 
     NNet(inputDim, outputDim, layerSize, numLayers, maxBatch, train=True, temporalLayer=-1)   rnnet.py:8-9
     costAndGrad(data, labels=None) -> (cost, grad, skip)      training                        rnnet.py:91-191

@@ -1,7 +1,7 @@
 """parallel -- host-side logic of the data-parallel step (pure Python, no CUDA).
 
 The reference has no multi-GPU training (one process, one GPU, one utterance per step:
-/root/reference/ctc_fast/runNNet.py:117-120, sgd.py:70-95).  Utterances are independent until the
+ctc_fast/runNNet.py:117-120, sgd.py:70-95).  Utterances are independent until the
 parameter update, so a step's minibatch is sharded over ranks and the flat gradient (with its
 4-float statistics tail) is summed by ONE all-reduce; every rank then applies the identical update.
 """

@@ -1,6 +1,6 @@
-"""runNNet -- training / likelihood-dump driver for the B200 backend.
+"""runNNet -- training / likelihood-dump driver for the H100 backend.
 
-Call surface kept from the reference driver (/root/reference/ctc_fast/runNNet.py:23-237): `run(args)` and
+Call surface kept from the reference driver (ctc_fast/runNNet.py:23-237): `run(args)` and
 `test(opts)`, every command-line flag of runNNet.py:27-69 with its default, the run-directory protocol
 (cfg.json, params.pk = SGD pickle followed by the stack pickle, params.pk.epochNN, epoch, num_files,
 last_cost, sentinel, train.log), resume through --cfg_file with the step size re-annealed

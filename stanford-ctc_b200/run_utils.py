@@ -1,5 +1,5 @@
 """run_utils -- small helpers of the driver.  Same public names as the reference module
-(/root/reference/ctc_fast/run_utils.py:10-91: dump_config, load_config, CfgStruct, get_git_revision,
+(ctc_fast/run_utils.py:10-91: dump_config, load_config, CfgStruct, get_git_revision,
 get_hostname, touch_file, TimeString) because runNNet and the reference's run-management tools import them."""
 import json
 import pathlib

@@ -1,4 +1,4 @@
-"""sgd -- drop-in for /root/reference/ctc_fast/sgd.py (class SGD), computed by libctcb200.
+"""sgd -- drop-in for ctc_fast/sgd.py (class SGD), computed by libctcb200.
 
 Same constructor, attributes and methods as the reference (sgd.py:10-11, :36, :44, :57):
 

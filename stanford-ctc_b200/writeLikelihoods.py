@@ -1,5 +1,5 @@
 """writeLikelihoods -- forward-only log-likelihood dump, same function names and on-disk formats as
-/root/reference/ctc_fast/analysis-utils/writeLikelihoods.py:8-55 (Kaldi binary "BFM" float matrix ark
+ctc_fast/analysis-utils/writeLikelihoods.py:8-55 (Kaldi binary "BFM" float matrix ark
 + a pickle of {key: log-prob K x T})."""
 import pickle
 import struct

@@ -1,11 +1,11 @@
 """Generates tests/golden/*.npz by running the REFERENCE ITSELF in the authoring container:
-  * CTC cases through oracle/_ref = the unmodified /root/reference/ctc_fast/ctc-loss/ctc_fast.pyx
+  * CTC cases through oracle/_ref = the unmodified ctc_fast/ctc-loss/ctc_fast.pyx
     and ctc_fast_blankforce.pyx (compiled by oracle/build_ref.py), fed probs.astype(float64) in Fortran
     order as brnnet.py:175 does;
   * BRNN cases through oracle/brnn_oracle.py (float64 restatement of brnnet.py; the cudamat half of
     the reference is not runnable here) with the CTC inside it again served by oracle/_ref.
 
-Run from the repo root:  python tests/golden/gen_golden.py      (needs /root/reference)
+Run from the repo root:  python tests/golden/gen_golden.py      (needs CTC_REFERENCE_DIR)
 """
 import os
 import sys
@@ -23,7 +23,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 
 
 def main():
-    assert build_ref.build() is not None, "oracle/_ref could not be built (no /root/reference?)"
+    assert build_ref.build() is not None, "oracle/_ref could not be built (CTC_REFERENCE_DIR unset or Cython missing?)"
     out = {}
     for name in recipes.ALL_CTC:
         probs, seq = recipes.ctc_case(name)

@@ -1,9 +1,9 @@
 """Pins the BRNN half of the oracle to the REFERENCE ITSELF: runs the reference's own NumPy BRNN,
-/root/reference/ctc_fast/debug-utils/rnnetcpu.py (class RNNet, costAndGrad :54-150, self-test recipe
+ctc_fast/debug-utils/rnnetcpu.py (class RNNet, costAndGrad :54-150, self-test recipe
 :180-193), in the authoring container and stores its inputs and outputs as tests/golden/rnnetcpu_ref.npz.
 
 The file is Python 2 (print statements, xrange, tabs mixed with spaces), so it cannot be imported as it
-lies.  It is read from /root/reference, converted MECHANICALLY IN MEMORY -- tabs expanded, `print x` ->
+lies.  It is read from the original project's checkout ($CTC_REFERENCE_DIR), converted MECHANICALLY IN MEMORY -- tabs expanded, `print x` ->
 `print(x)`, `xrange` -> `range`; no arithmetic line is touched -- written to a temporary directory
 (never into this repository) and imported from there with `ctc_fast` resolving to oracle/_ref, the
 reference's own unmodified ctc_fast.pyx compiled by oracle/build_ref.py.
@@ -12,7 +12,7 @@ Cases: the reference's self-test recipe (seed 33, D=20, T=10, K=6, H=30, N=3, te
 [0,1,2]; prints "COST ...") plus further shapes, incl. a net without a temporal layer and repeated labels.
 tests/test_oracle.py asserts that oracle/brnn_oracle.py reproduces cost and every gradient to 1e-12.
 
-Run from the repo root:  python tests/golden/gen_rnnetcpu_ref.py      (needs /root/reference)
+Run from the repo root:  python tests/golden/gen_rnnetcpu_ref.py      (needs CTC_REFERENCE_DIR)
 """
 import importlib.util
 import os
@@ -25,7 +25,7 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
 HERE = os.path.dirname(os.path.abspath(__file__))
-REF = "/root/reference/ctc_fast/debug-utils/rnnetcpu.py"
+REF = os.path.join(os.environ.get("CTC_REFERENCE_DIR", ""), "ctc_fast", "debug-utils", "rnnetcpu.py")
 
 # name: (seed, inputDim, T, outputDim, layerSize, numLayers, temporalLayer, labels or None for the recipe's arange(3))
 CASES = {
@@ -39,7 +39,7 @@ CASES = {
 
 def load_reference_module():
     from oracle import build_ref
-    assert build_ref.build() is not None, "oracle/_ref could not be built (no /root/reference?)"
+    assert build_ref.build() is not None, "oracle/_ref could not be built (CTC_REFERENCE_DIR unset or Cython missing?)"
     src = open(REF).read().expandtabs(8)
     src = re.sub(r"^(\s*)print (.+)$", r"\1print(\2)", src, flags=re.M)
     src = src.replace("xrange(", "range(")

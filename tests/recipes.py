@@ -1,10 +1,10 @@
 """Deterministic input recipes shared by the golden generator and the tests.
 
 All follow the reference's own eyeball tests (seed 33, legacy np.random streams):
-  time_trials : /root/reference/ctc/time_trials.py:13-25  (K=40, |l|=125, T=1200, peaked probs)
-  ctc_py      : /root/reference/ctc/ctc.py:143-152        (K=62, |l|=54, T=453, logits ~ N(0,1))
+  time_trials : ctc/time_trials.py:13-25  (K=40, |l|=125, T=1200, peaked probs)
+  ctc_py      : ctc/ctc.py:143-152        (K=62, |l|=54, T=453, logits ~ N(0,1))
   c1          : BASELINE.json configs[0]                  (T=200, K=62, |l|=30)
-  rnnetcpu    : /root/reference/ctc_fast/debug-utils/rnnetcpu.py:181-193 (D=20,T=10,K=6,H=30,N=3,tl=2)
+  rnnetcpu    : ctc_fast/debug-utils/rnnetcpu.py:181-193 (D=20,T=10,K=6,H=30,N=3,tl=2)
 """
 import numpy as np
 
@@ -154,3 +154,43 @@ def rnn_variant_perturb(stack, tag):
     if tag == "uni":
         stack[1][1] += 4.0          # some units reach the 20.0 clip (rnnet.py:32,113-116)
         stack[-1][0] *= 1.2
+
+
+# ---- randomised shapes on which the C restatements are pinned to the compiled reference modules ----------------
+def random_ctc_cases():
+    """300 random (K, T, |l|) cases incl. T = 1, T = |l|, T < |l|, heavy label repetition and peaked distributions."""
+    rng = np.random.RandomState(2024)
+    for case in range(300):
+        K = int(rng.randint(2, 40))
+        T = int(rng.choice([1, 2, 3, 5, 8, 17, 40, 90]))
+        nlab = int(rng.randint(1, max(2, min(T + 3, 25))))
+        scale = float(rng.choice([0.5, 1.0, 4.0, 12.0]))
+        probs = softmax_cols(rng.randn(K, T) * scale).astype(np.float32).astype(np.float64)
+        if rng.rand() < 0.3:
+            seq = np.full(nlab, 1 + rng.randint(K - 1), dtype=np.int32)           # one label repeated
+        else:
+            seq = (1 + rng.randint(0, K - 1, size=nlab)).astype(np.int32)
+        yield np.asfortranarray(probs), seq
+
+
+def random_bf_cases():
+    """200 random blank-forced cases, most with the usual interleaved blanks."""
+    rng = np.random.RandomState(77)
+    for case in range(200):
+        K = int(rng.randint(2, 30))
+        T = int(rng.choice([1, 2, 4, 9, 33, 70]))
+        L = int(rng.randint(1, 20))
+        probs = softmax_cols(rng.randn(K, T) * float(rng.choice([1.0, 5.0]))).astype(np.float32).astype(np.float64)
+        seq = rng.randint(0, K, size=L).astype(np.int32)
+        if rng.rand() < 0.7:
+            seq[::2] = 0                                                           # the usual interleaved blanks
+        yield np.asfortranarray(probs), seq
+
+
+def digest(a):
+    """SHA-256 of a float64 array's values (row-major, every NaN canonical) as 32 uint8: a stored stand-in for a
+    bit-exact comparison with an array that is too large to keep."""
+    import hashlib
+    a = np.ascontiguousarray(a, dtype=np.float64)
+    a = np.where(np.isnan(a), np.nan, a)
+    return np.frombuffer(hashlib.sha256(a.tobytes()).digest(), dtype=np.uint8)

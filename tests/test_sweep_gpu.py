@@ -46,6 +46,8 @@ def test_sweep_forward_and_bptt(H, B, T, cuda):
     import _ctcb
     from _ctcb import lib, check, ptr
     torch = cuda
+    if H >= 1024:     # these sizes must run on the tensor-core kernel, not on the generic one
+        assert lib.ctcb_sweep_uses_tensor_cores(H, B) == 1, (H, B)
     rng = np.random.RandomState(H + B)
     s = 0.9 / np.sqrt(H / 3.0)                        # spectral radius ~0.9: well conditioned
     Wf = rng.uniform(-s, s, (H, H)); Wb = rng.uniform(-s, s, (H, H))

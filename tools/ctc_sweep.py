@@ -1,12 +1,14 @@
 """BASELINE.json configs[4]: CTC-kernel isolation sweep T x |l| x K -> algorithmic GB/s vs the HBM roofline.
-Batch sizes are chosen so that the activations exceed L2 (126 MB) where the alpha spill workspace allows."""
+Batch sizes are chosen so that the activations exceed L2 (50 MB on H100) where the alpha spill workspace allows.
+
+Usage:  python tools/ctc_sweep.py [OUT.json]      (default: ctc_sweep.json in the current directory)"""
 import json, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path[:0] = [ROOT, os.path.join(ROOT, "stanford-ctc_b200")]
 import numpy as np, torch
 import ctc_fast
 from _ctcb import lib
-peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))) if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else {"hbm_gbs": 6650.0}
+peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))) if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else {"hbm_gbs": 3350.0}   # H100 SXM data sheet
 rows = []
 for T in (100, 500, 2000, 5000):
     for L in (10, 100, 300):
@@ -43,4 +45,4 @@ for T in (100, 500, 2000, 5000):
             print(rows[-1], flush=True)
             del acts, grad, ws
             torch.cuda.empty_cache()
-json.dump(dict(peak_hbm_gbs=peaks["hbm_gbs"], rows=rows), open(os.path.join(ROOT, "gpurun_out", "ctc_sweep_r1.json"), "w"), indent=1)
+json.dump(dict(peak_hbm_gbs=peaks["hbm_gbs"], rows=rows), open(sys.argv[1] if len(sys.argv) > 1 else "ctc_sweep.json", "w"), indent=1)

@@ -1,4 +1,4 @@
-"""Check + time ctcb_gemm_f32 (tcgen05 3xTF32 path unless CTCB_GEMM=simt) against float64 NumPy."""
+"""Check + time ctcb_gemm_f32 (wgmma 3xTF32 path unless CTCB_GEMM=simt) against float64 NumPy."""
 import os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path[:0] = [ROOT, os.path.join(ROOT, "stanford-ctc_b200")]

@@ -1,5 +1,5 @@
 import sys, time
-sys.path[:0]=['/root/repo','/root/repo/tests']
+import os; sys.path[:0] = [os.path.dirname(os.path.dirname(os.path.abspath(__file__))), os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'tests')]
 import numpy as np, recipes
 from oracle import brnn_oracle
 D,K,H,N,tl,T,L,B = 41,32,1024,3,2,800,100,2

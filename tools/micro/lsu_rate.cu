@@ -1,18 +1,22 @@
 // Microbenchmark for the open question of the cluster sweep (DESIGN.md section 6): what does a warp-uniform
 // (broadcast) LDS.128, a full-width LDS.128 and a SHFL cost per SM when 16 warps issue them back to back, alone
-// and interleaved with FFMA2?  Prints cycles per instruction per SM sub-partition.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o lsu_rate lsu_rate.cu ; run: ./lsu_rate
+// and interleaved with the FFMA pairs of the sweep?  Prints cycles per instruction per SM sub-partition.
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o lsu_rate lsu_rate.cu ; run: ./lsu_rate
 #include <cstdio>
 #include <cuda_runtime.h>
 
+// a pair of output units times one scalar, as sweep_cluster.cu computes it: two FFMA
 __device__ __forceinline__ void ffma2(unsigned long long &d, unsigned long long a, float h) {
-    unsigned long long hh;
-    asm("mov.b64 %0, {%1, %1};" : "=l"(hh) : "f"(h));
-    asm volatile("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(d) : "l"(a), "l"(hh));
+    float dl, dh, al, ah;
+    asm("mov.b64 {%0, %1}, %2;" : "=f"(dl), "=f"(dh) : "l"(d));
+    asm("mov.b64 {%0, %1}, %2;" : "=f"(al), "=f"(ah) : "l"(a));
+    dl = fmaf(al, h, dl);
+    dh = fmaf(ah, h, dh);
+    asm("mov.b64 %0, {%1, %2};" : "=l"(d) : "f"(dl), "f"(dh));
 }
 
 // MODE 0: broadcast LDS.128 (all lanes one address)   1: full-width LDS.128 (lane-consecutive 16 B)
-// MODE 2: SHFL.BFLY                                   3: broadcast LDS.128 + 4 FFMA2 each (the sweep's inner loop)
+// MODE 2: SHFL.BFLY                                   3: broadcast LDS.128 + 4 FFMA pairs each (the sweep's inner loop)
 template <int MODE>
 __global__ void k(float *out, long long *cycles, int iters) {
     __shared__ __align__(16) float sm[32 * 4 * 16 + 64];
@@ -44,12 +48,18 @@ __global__ void k(float *out, long long *cycles, int iters) {
     if (threadIdx.x == 0) cycles[blockIdx.x] = t1 - t0;
 }
 
+static int nsm() {
+    int n = 0;
+    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, 0);
+    return n;
+}
+
 template <int MODE>
 static void run(const char *name, float *out, long long *cyc) {
     const int iters = 500;
     for (int warps : {4, 16}) {
-        long long h[148];
-        k<MODE><<<148, warps * 32>>>(out, cyc, iters);
+        long long h[1];
+        k<MODE><<<nsm(), warps * 32>>>(out, cyc, iters);
         cudaMemcpy(h, cyc, sizeof(h), cudaMemcpyDeviceToHost);
         const double per_sm = (double)h[0] / (iters * 16.0 * warps);          // cycles per instruction, whole SM
         printf("%-34s %2d warps/SM: %.2f cycles per warp instruction per SM (%.2f per sub-partition)\n", name, warps,
@@ -59,12 +69,12 @@ static void run(const char *name, float *out, long long *cyc) {
 
 int main() {
     float *out; long long *cyc;
-    cudaMalloc(&out, 148 * 512 * sizeof(float));
-    cudaMalloc(&cyc, 148 * sizeof(long long));
+    cudaMalloc(&out, nsm() * 512 * sizeof(float));
+    cudaMalloc(&cyc, nsm() * sizeof(long long));
     run<0>("broadcast LDS.128", out, cyc);
     run<1>("full-width LDS.128", out, cyc);
     run<2>("SHFL.BFLY", out, cyc);
-    run<3>("broadcast LDS.128 + 4 FFMA2", out, cyc);
+    run<3>("broadcast LDS.128 + 4 FFMA pairs", out, cyc);
     printf("%s\n", cudaGetErrorString(cudaDeviceSynchronize()));
     return 0;
 }
