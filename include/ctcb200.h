@@ -163,6 +163,27 @@ int ctcb_brnn_cost_and_grad(ctcb_brnn *h, const float *feats, const int32_t *T_p
                             float *regcost_out, float *probs_out, float *stats_out,
                             void *workspace, size_t ws_bytes, void *stream);
 
+/* Gradient accumulation: one step computed as several calls, each on a micro-batch of at most maxB utterances
+ * (gradients SUMMED over all of them, so the result equals one call on the whole step up to fp32 summation order).
+ * Same arguments as ctcb_brnn_cost_and_grad plus `flags`:
+ *   CTCB_PART_FIRST : overwrite every gradient tensor and stats_out (their earlier contents are ignored, NaN
+ *                     included; the alignment gaps between tensors of the flat vector are never written);
+ *                     without it every gradient tensor and the statistics tail are ADDED into (the error flag
+ *                     only grows, so it stays non-zero once any micro-batch set it);
+ *   CTCB_PART_LAST  : finish the step: the data-parallel exchange (ctcb_brnn_set_comm), the reg*W gradient
+ *                     (unless deferred, ctcb_brnn_set_deferred_l2) and *regcost_out, each once per step; other
+ *                     calls leave regcost_out untouched.
+ * cost_out / skip_out are per call (pass pointers offset to the micro-batch's utterances).  Every rank of a
+ * data-parallel step must make exactly one LAST call (or ctcb_brnn_exchange_only); it may make any number of
+ * calls before it.  ctcb_brnn_cost_and_grad == ctcb_brnn_cost_and_grad_part(..., CTCB_PART_FIRST | CTCB_PART_LAST). */
+#define CTCB_PART_FIRST 1
+#define CTCB_PART_LAST 2
+int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, const int32_t *T_per_utt,
+                                 const int32_t *labels, const int32_t *label_off, int B, int Tmax,
+                                 const float *params, float *grads, float *cost_out, int32_t *skip_out,
+                                 float *regcost_out, float *probs_out, float *stats_out, int flags,
+                                 void *workspace, size_t ws_bytes, void *stream);
+
 /* L2 regularisation under data parallelism.  By default ctcb_brnn_cost_and_grad adds reg*W to the weight
  * gradients itself (brnnet.py:197-198,244-247).  A data-parallel caller SUMS the gradient over ranks and must
  * add reg*W exactly once: it switches the handle to deferred mode (the call then only reports the L2 cost) and

@@ -20,6 +20,9 @@ lib = ctypes.CDLL(LIB_PATH)
 c_int, c_i64, c_f32, c_vp, c_sz = ctypes.c_int, ctypes.c_int64, ctypes.c_float, ctypes.c_void_p, ctypes.c_size_t
 
 
+PART_FIRST, PART_LAST = 1, 2      # CTCB_PART_FIRST / CTCB_PART_LAST (ctcb_brnn_cost_and_grad_part)
+
+
 class BrnnConfig(ctypes.Structure):
     _fields_ = [("inputDim", ctypes.c_int32), ("outputDim", ctypes.c_int32), ("layerSize", ctypes.c_int32),
                 ("numLayers", ctypes.c_int32), ("temporalLayer", ctypes.c_int32), ("maxT", ctypes.c_int32),
@@ -58,6 +61,8 @@ _PROTOS = {
     "ctcb_brnn_destroy": (None, [c_vp]),
     "ctcb_brnn_cost_and_grad": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp,
                                         c_vp, c_vp, c_vp, c_sz, c_vp]),
+    "ctcb_brnn_cost_and_grad_part": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_vp,
+                                             c_vp, c_vp, c_vp, c_int, c_vp, c_sz, c_vp]),
     "ctcb_brnn_sweep_f32": (c_int, [c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_f32,
                                     c_vp, c_sz, c_vp]),
     "ctcb_brnn_sweep_workspace_bytes": (c_sz, [c_int, c_int]),

@@ -73,11 +73,14 @@ __global__ void colsum_stage1_wide(const float4 *__restrict__ x, int64_t R, int 
     partial[(int64_t)blockIdx.y * N4 + c4] = make_float4((a0.x + a1.x) + (a2.x + a3.x), (a0.y + a1.y) + (a2.y + a3.y),
                                                         (a0.z + a1.z) + (a2.z + a3.z), (a0.w + a1.w) + (a2.w + a3.w));
 }
+// ACC: add the column sums into `out` (a later micro-batch of a step) instead of overwriting it
+template <bool ACC>
 __global__ void colsum_stage2(const float *__restrict__ partial, int nblk, int N, float *__restrict__ out) {
     const int n = blockIdx.x * blockDim.x + threadIdx.x;
     if (n >= N) return;
     float s = 0.f;
     for (int i = 0; i < nblk; ++i) s += partial[(int64_t)i * N + n];
+    if (ACC) s += out[n];
     out[n] = s;
 }
 
@@ -101,6 +104,8 @@ __global__ void set_scalar_kernel(float *p, float v) { *p = v; }
 
 // stats = {#non-skipped, sum of their nll, #skipped, sweep error flag}; one warp.  The flag rides in the data-parallel
 // all-reduce with the rest of the tail, so a wait timeout on one rank is seen (non-zero) by every rank.
+// ACC: add into the tail of the earlier micro-batches of the step; the flag only grows, so it stays non-zero.
+template <bool ACC>
 __global__ void batch_stats_kernel(const float *__restrict__ cost, const int32_t *__restrict__ skip, int B, float *stats,
                                    const unsigned int *__restrict__ errflag) {
     float nv = 0.f, cs = 0.f, ns = 0.f;
@@ -109,7 +114,11 @@ __global__ void batch_stats_kernel(const float *__restrict__ cost, const int32_t
         else { nv += 1.f; cs += cost[u]; }
     }
     nv = warp_sum(nv); cs = warp_sum(cs); ns = warp_sum(ns);
-    if (threadIdx.x == 0) { stats[0] = nv; stats[1] = cs; stats[2] = ns; stats[3] = (float)errflag[0]; }
+    if (threadIdx.x == 0) {
+        float ef = (float)errflag[0];
+        if (ACC) { nv += stats[0]; cs += stats[1]; ns += stats[2]; ef += stats[3]; }
+        stats[0] = nv; stats[1] = cs; stats[2] = ns; stats[3] = ef;
+    }
 }
 
 }  // namespace ctcb
@@ -335,13 +344,21 @@ static int brnn_reduce_rest(ctcb_brnn *h, float *grads, float *stats, bool early
     return comm_allreduce_ranges(h->comm, ptrs, cnt, k, st);
 }
 
-extern "C" int ctcb_brnn_cost_and_grad(ctcb_brnn *h, const float *feats, const int32_t *T_per_utt,
-                                       const int32_t *labels, const int32_t *label_off, int B, int Tmax,
-                                       const float *params, float *grads, float *cost_out, int32_t *skip_out,
-                                       float *regcost_out, float *probs_out, float *stats_out, void *workspace,
-                                       size_t ws_bytes, void *stream) {
+// One micro-batch of a step whose gradient is the sum over several calls (include/ctcb200.h): without
+// CTCB_PART_FIRST every gradient tensor and the statistics tail are added into, with it overwritten; only the
+// CTCB_PART_LAST call exchanges over the ranks and adds the L2 term, so each happens once per step.
+// ctcb_brnn_cost_and_grad is this with both flags.
+extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, const int32_t *T_per_utt,
+                                            const int32_t *labels, const int32_t *label_off, int B, int Tmax,
+                                            const float *params, float *grads, float *cost_out, int32_t *skip_out,
+                                            float *regcost_out, float *probs_out, float *stats_out, int flags,
+                                            void *workspace, size_t ws_bytes, void *stream) {
     if (!h || !feats || !T_per_utt || !params)
         return set_error(CTCB_EINVAL, "ctcb_brnn_cost_and_grad: null pointer argument");
+    if (flags & ~(CTCB_PART_FIRST | CTCB_PART_LAST))
+        return set_error(CTCB_EINVAL, "ctcb_brnn_cost_and_grad_part: unknown flags 0x%x", flags);
+    const bool first = (flags & CTCB_PART_FIRST) != 0, last = (flags & CTCB_PART_LAST) != 0;
+    const float beta_g = first ? 0.f : 1.f;      // weight-gradient contractions: C = dW (+ C)
     const ctcb_brnn_config &c = h->cfg;
     if (B <= 0 || B > c.maxB || Tmax <= 0 || Tmax > c.maxT)
         return set_error(CTCB_EINVAL, "ctcb_brnn_cost_and_grad: batch %d x %d frames exceeds the configured %d x %d",
@@ -436,7 +453,7 @@ extern "C" int ctcb_brnn_cost_and_grad(ctcb_brnn *h, const float *feats, const i
         // dW = delta^T . X_i   (brnnet.py:196)
         {
         ProfScope ps("gemm_dw", sw);
-        TRY(ctcb_gemm_f32(1, 0, n_out, n_in, (int)R, 1.f, dcur, n_out, Xi, n_in, 0.f, G(2 * i), n_in, nullptr, 0,
+        TRY(ctcb_gemm_f32(1, 0, n_out, n_in, (int)R, 1.f, dcur, n_out, Xi, n_in, beta_g, G(2 * i), n_in, nullptr, 0,
                           nullptr, on_side ? gws2 : gws, on_side ? gws2_bytes : gws_bytes, sw));
         }
         // db = row sums of delta   (brnnet.py:200)
@@ -458,10 +475,11 @@ extern "C" int ctcb_brnn_cost_and_grad(ctcb_brnn *h, const float *feats, const i
                 colsum_stage1<<<dim3((n_out + 31) / 32, nblk), dim3(32, 8), 0, sw>>>(dcur, R, n_out, part);
             }
             CTCB_LAUNCH_CHECK();
-            colsum_stage2<<<(n_out + 127) / 128, 128, 0, sw>>>(part, nblk, n_out, G(2 * i + 1));
+            if (first) colsum_stage2<false><<<(n_out + 127) / 128, 128, 0, sw>>>(part, nblk, n_out, G(2 * i + 1));
+            else colsum_stage2<true><<<(n_out + 127) / 128, 128, 0, sw>>>(part, nblk, n_out, G(2 * i + 1));
             CTCB_LAUNCH_CHECK();
         }
-        if (dp && on_side && i == tl) {
+        if (dp && last && on_side && i == tl) {
             // every gradient tensor of the layers >= tl is now queued on the side stream: sum that contiguous range over
             // the ranks there, next to the BPTT sweep on the main stream
             float *pa = G(2 * tl);
@@ -491,12 +509,12 @@ extern "C" int ctcb_brnn_cost_and_grad(ctcb_brnn *h, const float *feats, const i
                 ProfScope ps("gemm_dw_rec", h->side);
                 if (Tmax > 1) {
                     const int64_t Rm = R - B;
-                    TRY(ctcb_gemm_f32(1, 0, H, H, (int)Rm, 1.f, dFor + (int64_t)B * H, H, For, H, 0.f, G(iWtf), H,
+                    TRY(ctcb_gemm_f32(1, 0, H, H, (int)Rm, 1.f, dFor + (int64_t)B * H, H, For, H, beta_g, G(iWtf), H,
                                       nullptr, 0, nullptr, gws2, gws2_bytes, h->side));
                     if (!uni)
-                        TRY(ctcb_gemm_f32(1, 0, H, H, (int)Rm, 1.f, dBack, H, Back + (int64_t)B * H, H, 0.f, G(iWtb), H,
-                                          nullptr, 0, nullptr, gws2, gws2_bytes, h->side));
-                } else {
+                        TRY(ctcb_gemm_f32(1, 0, H, H, (int)Rm, 1.f, dBack, H, Back + (int64_t)B * H, H, beta_g, G(iWtb),
+                                          H, nullptr, 0, nullptr, gws2, gws2_bytes, h->side));
+                } else if (first) {     // one frame: no recurrence, nothing to add to earlier micro-batches
                     CTCB_CUDA_CHECK(cudaMemsetAsync(G(iWtf), 0, sizeof(float) * H * H, h->side));
                     if (!uni) CTCB_CUDA_CHECK(cudaMemsetAsync(G(iWtb), 0, sizeof(float) * H * H, h->side));
                 }
@@ -515,9 +533,12 @@ extern "C" int ctcb_brnn_cost_and_grad(ctcb_brnn *h, const float *feats, const i
     }
 
     if (stats_out) {     // after both sweeps, so that the tail carries the error flag of either
-        batch_stats_kernel<<<1, 32, 0, st>>>(cost_out, skip_out, B, stats_out, counters);
+        if (first) batch_stats_kernel<false><<<1, 32, 0, st>>>(cost_out, skip_out, B, stats_out, counters);
+        else batch_stats_kernel<true><<<1, 32, 0, st>>>(cost_out, skip_out, B, stats_out, counters);
         CTCB_LAUNCH_CHECK();
     }
+    // an earlier micro-batch of the step: the exchange and the L2 term wait for the sum of all of them
+    if (!last) return CTCB_OK;
 
     if (dp) TRY(brnn_reduce_rest(h, grads, stats_out, overlap, st));
 
@@ -537,6 +558,16 @@ extern "C" int ctcb_brnn_cost_and_grad(ctcb_brnn *h, const float *feats, const i
         }
     }
     return CTCB_OK;
+}
+
+extern "C" int ctcb_brnn_cost_and_grad(ctcb_brnn *h, const float *feats, const int32_t *T_per_utt,
+                                       const int32_t *labels, const int32_t *label_off, int B, int Tmax,
+                                       const float *params, float *grads, float *cost_out, int32_t *skip_out,
+                                       float *regcost_out, float *probs_out, float *stats_out, void *workspace,
+                                       size_t ws_bytes, void *stream) {
+    return ctcb_brnn_cost_and_grad_part(h, feats, T_per_utt, labels, label_off, B, Tmax, params, grads, cost_out,
+                                        skip_out, regcost_out, probs_out, stats_out,
+                                        CTCB_PART_FIRST | CTCB_PART_LAST, workspace, ws_bytes, stream);
 }
 
 extern "C" int ctcb_brnn_set_deferred_l2(ctcb_brnn *h, int deferred) {

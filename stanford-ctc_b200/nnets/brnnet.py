@@ -13,9 +13,10 @@ Same constructor, attributes and methods as the reference (brnnet.py:10-11, :34,
 flat fp32 device buffer (`params` / `grads`), so the optimiser and the NCCL all-reduce touch a
 single contiguous vector.  New, additive surface for the minibatch/data-parallel path:
 
-    NNet(..., maxUtts=B, maxLabels=L)        capacity for B utterances per step
-    costAndGradBatch(datas, labelss)         -> (costs[B], grad, skips[B])   host arrays in
-    costAndGradDevice(batch)                 -> no host sync; see DeviceBatch
+    NNet(..., maxUtts=B, maxLabels=L)        capacity for B utterances per call (micro-batch)
+    costAndGradBatch(datas, labelss)         -> (costs[B], grad, skips[B])   host arrays in; more than maxUtts
+                                                utterances are accumulated over micro-batches
+    costAndGradDevice(batch, first, last)    -> no host sync; see DeviceBatch
 
 torch tensors are buffer handles only; all arithmetic is in the C ABI (include/ctcb200.h).
 """
@@ -25,6 +26,7 @@ import pickle
 import numpy as np
 
 import _ctcb
+import parallel
 from _ctcb import lib, check, ptr, BrnnConfig
 
 CTC_MAX_LABELS = 511      # CTCB_CTC_MAX_LABELS
@@ -48,6 +50,8 @@ class DeviceBatch(object):
         self.B = 0
         self.Tmax = 0
         self.h2d_bytes = 0
+        self._torch = torch
+        self._copied = None     # event behind the last upload: the pinned buffers are free again once it completed
 
     def pack(self, datas, labelss):
         """datas: list of (inputDim x T_u) float32 arrays (the reference's per-utterance layout,
@@ -56,6 +60,10 @@ class DeviceBatch(object):
         Tmax = max(d.shape[1] for d in datas)
         assert B <= self.maxB, "Batch size exceeds max utterances"
         assert Tmax <= self.maxT, "Batch size exceeds max batch"      # brnnet.py:100
+        if self._copied is not None:
+            # an asynchronous copy out of these pinned buffers may still be queued (a step of several micro-batches
+            # cycles through the two staging buffers faster than the device consumes them)
+            self._copied.synchronize()
         D = self.D
         f = self.h_feats.numpy()[:Tmax * B * D].reshape(Tmax, B, D)
         lens = self.h_lens.numpy()
@@ -91,6 +99,9 @@ class DeviceBatch(object):
         self.d_off[:self.B + 1].copy_(self.h_off[:self.B + 1], non_blocking=True)
         if nl:
             self.d_labels[:nl].copy_(self.h_labels[:nl], non_blocking=True)
+        if self._copied is None:
+            self._copied = self._torch.cuda.Event()
+        self._copied.record()
         self.h2d_bytes = 4 * (n + self.B + self.B + 1 + nl)
         return self
 
@@ -118,7 +129,7 @@ class NNet:
         self.numLayers = numLayers
         self.layerSizes = [layerSize] * numLayers
         self.maxBatch = maxBatch           # frames per utterance, as in the reference
-        self.maxUtts = maxUtts             # utterances per step (new)
+        self.maxUtts = maxUtts             # utterances per call, i.e. per micro-batch of a step (new)
         # the CTC kernel holds at most CTC_MAX_LABELS labels per utterance (include/ctcb200.h); a reference-style
         # constructor call (no maxLabels) gets the largest capacity that exists
         self.maxLabels = min(maxBatch, CTC_MAX_LABELS) if maxLabels is None else maxLabels
@@ -214,6 +225,7 @@ class NNet:
         else:
             self._regcost = torch.zeros(1, dtype=torch.float32, device=self.dev)
         self._out_host = torch.zeros(2 * self.maxUtts, dtype=torch.float32).pin_memory()
+        self._out_all = None        # costs and skips of a step of more than maxUtts utterances (costAndGradBatch)
         self._rec_host = torch.zeros(8, dtype=torch.float32).pin_memory()
         self._probs = None
         self._comm = None
@@ -235,9 +247,14 @@ class NNet:
         assert batchSize <= self.maxBatch, "Batch size exceeds max batch"
 
     # ------------------------------------------------------------------ compute
-    def costAndGradDevice(self, batch, want_probs=False):
+    def costAndGradDevice(self, batch, want_probs=False, first=True, last=True, out=None):
         """Enqueue forward/CTC/backward for a staged DeviceBatch on the current stream.  Returns device
-        tensors (cost[B], skip[B]) -- or probs [Tmax][B][K] when train=False -- without synchronising."""
+        tensors (cost[B], skip[B]) -- or probs [Tmax][B][K] when train=False -- without synchronising.
+
+        Gradient accumulation over the micro-batches of one step (ctcb_brnn_cost_and_grad_part): first=False adds
+        the gradient and the statistics tail into what the earlier calls left; only the last=True call exchanges
+        over the ranks and adds the L2 term.  `out` optionally names the (cost[B], skip[B]) device tensors to write
+        (default: the net's own per-utterance buffers)."""
         torch = self._torch
         B, Tmax = batch.B, batch.Tmax
         probs = None
@@ -247,34 +264,72 @@ class NNet:
                 self._probs = torch.empty(self.maxBatch * self.maxUtts * self.outputDim, dtype=torch.float32,
                                           device=self.dev)
             probs = self._probs[:n].view(Tmax, B, self.outputDim)
-        check(lib.ctcb_brnn_cost_and_grad(
+        cost, skip = out if out is not None else (self._cost[:B], self._skip[:B])
+        flags = (_ctcb.PART_FIRST if first else 0) | (_ctcb.PART_LAST if last else 0)
+        check(lib.ctcb_brnn_cost_and_grad_part(
             self._h, ptr(batch.d_feats), ptr(batch.d_lens), ptr(batch.d_labels), ptr(batch.d_off), B, Tmax,
             ptr(self.params), ptr(self.grads) if self.train else None,
-            ptr(self._cost) if self.train else None, ptr(self._skip) if self.train else None,
-            ptr(self._regcost) if self.train else None, ptr(probs), ptr(self.stats), ptr(self._ws),
+            ptr(cost) if self.train else None, ptr(skip) if self.train else None,
+            ptr(self._regcost) if self.train else None, ptr(probs), ptr(self.stats), flags, ptr(self._ws),
             self._ws.numel(),
             _ctcb.current_stream()))
         if not self.train:
             return probs
-        return self._cost[:B], self._skip[:B]
+        return cost, skip
 
     def costAndGradBatch(self, datas, labelss):
         """Minibatch costAndGrad from host arrays: gradients of the utterances are summed.
-        Returns (costs float64[B], self.grad, skips bool[B]); the L2 term is in self.regcost."""
+        Returns (costs float64[B], self.grad, skips bool[B]); the L2 term is in self.regcost.
+        More than maxUtts utterances are computed as consecutive micro-batches of at most maxUtts that add into the
+        same gradient (parallel.micro_batches); costs and skips still cover every utterance, in input order."""
+        B = len(datas)
+        if B > self.maxUtts and self.train:
+            return self._cost_and_grad_accumulated(datas, labelss)
         self._batch.pack(datas, labelss).upload()
         self.costAndGradDevice(self._batch)
         # two pinned D2H copies on the stream (no kernels, no allocation), one synchronisation
         self._out_host.copy_(self._out, non_blocking=True)
         self._rec_host.copy_(self.record, non_blocking=True)
         self._torch.cuda.current_stream().synchronize()
-        B = len(datas)
+        self._read_record()
+        out = self._out_host.numpy()
+        costs = out[:B].astype(np.float64)
+        skips = out[self.maxUtts:self.maxUtts + B].view(np.int32) != 0
+        return costs, self.grad, skips
+
+    def _read_record(self):
         rec = self._rec_host.numpy()
         if rec[3] != 0:
             raise RuntimeError("recurrent sweep: inter-CTA wait timed out (flag %d); results are invalid" % int(rec[3]))
         self.regcost = float(rec[5])
-        out = self._out_host.numpy()
+
+    def _cost_and_grad_accumulated(self, datas, labelss):
+        torch = self._torch
+        B = len(datas)
+        # per-utterance outputs of the whole step, apart from the net's own buffers (captured CUDA graphs of
+        # sgd.SGD hold pointers into those)
+        if self._out_all is None or self._out_all.numel() < 2 * B:
+            self._out_all = torch.zeros(2 * B, dtype=torch.float32, device=self.dev)
+            self._out_all_host = torch.zeros(2 * B, dtype=torch.float32).pin_memory()
+        cost_all = self._out_all[:B]
+        skip_all = self._out_all[B:2 * B].view(torch.int32)
+        pieces = parallel.micro_batches(range(B), self.maxUtts)
+        u0 = 0
+        for k, idx in enumerate(pieces):
+            batch = self.swap_batches().pack([datas[i] for i in idx],
+                                             None if labelss is None else [labelss[i] for i in idx]).upload()
+            n = len(idx)
+            self.costAndGradDevice(batch, first=(k == 0), last=(k == len(pieces) - 1),
+                                   out=(cost_all[u0:u0 + n], skip_all[u0:u0 + n]))
+            u0 += n
+        host = self._out_all_host[:2 * B]
+        host.copy_(self._out_all[:2 * B], non_blocking=True)
+        self._rec_host.copy_(self.record, non_blocking=True)
+        torch.cuda.current_stream().synchronize()
+        self._read_record()
+        out = host.numpy()
         costs = out[:B].astype(np.float64)
-        skips = out[self.maxUtts:self.maxUtts + B].view(np.int32) != 0
+        skips = out[B:2 * B].view(np.int32) != 0
         return costs, self.grad, skips
 
     def costAndGrad(self, data, labels=None, sentence=None):

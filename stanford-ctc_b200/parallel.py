@@ -73,6 +73,23 @@ def per_rank_capacity(batch_size, world):
     return (batch_size + world - 1) // max(world, 1)
 
 
+def micro_batch_capacity(max_utts, batch_size, world):
+    """Utterances per micro-batch each rank allocates buffers for: max_utts when it is positive (never more than a
+    rank's shard can hold), else the whole shard of a step (one call per step)."""
+    shard_cap = per_rank_capacity(batch_size, world)
+    return min(max_utts, shard_cap) if max_utts > 0 else shard_cap
+
+
+def micro_batches(utts, cap):
+    """One rank's shard of a step cut into consecutive pieces of at most cap utterances, in order: the gradient of
+    the step is accumulated over them.  The shard is already length-bucketed, so consecutive pieces keep the
+    padding low.  An empty shard gives []."""
+    if cap < 1:
+        raise ValueError("micro-batch capacity must be at least 1, got %r" % (cap,))
+    utts = list(utts)
+    return [utts[i:i + cap] for i in range(0, len(utts), cap)]
+
+
 def world_info():
     """(dist module or None, rank, world) from torch.distributed if it is initialised."""
     try:

@@ -7,7 +7,7 @@ last_cost, sentinel, train.log), resume through --cfg_file with the step size re
 (runNNet.py:143-166), the fixed seeds 33 (:113-115) and CUDA_DEVICE device selection (:117-120).
 The implementation is organised differently: a declarative flag table, one RunDir helper that owns the
 side files, and separate train/evaluate phases.  Site paths of run_cfg.py / decoder_config.py became
-flags (--runDir, --outDir); new flags: --batchSize, --maxLabels, --quiet.  Under torchrun the same
+flags (--runDir, --outDir); new flags: --batchSize, --maxUtts, --maxLabels, --quiet.  Under torchrun the same
 script trains data-parallel (one process per GPU, one NCCL all-reduce per step).
 """
 import argparse
@@ -44,6 +44,8 @@ FLAGS = [
     ("run_desc", str, "", "free-text description stored in cfg.json"),
     # additions
     ("batchSize", int, 1, "utterances per optimisation step (1 = the reference schedule)"),
+    ("maxUtts", int, 0, "utterances per micro-batch per GPU: a larger shard accumulates its gradient over several "
+                        "micro-batches (0 = the whole shard, batchSize / number of GPUs rounded up)"),
     ("maxLabels", int, 511, "longest label sequence the buffers are sized for"),
     ("runDir", str, "./runs", "parent of the time-stamped run directory"),
     ("outDir", str, None, "--test: directory for the likelihood arks"),
@@ -59,6 +61,21 @@ def _parse(argv):
         else:
             ap.add_argument("--" + name, dest=name, type=typ, default=default, help=hlp)
     return ap.parse_args(argv)
+
+
+def run_config(cli):
+    """The run's configuration: the command line of a new run, or the cfg.json of the run being resumed (its flags
+    win, so a resumed run keeps e.g. its batchSize and maxUtts), with the defaults of keys an older run did not
+    record."""
+    cfg = load_config(cli.cfg_file) if cli.cfg_file is not None else dict(vars(cli))
+    for name, _, default, _ in FLAGS:                 # configs written by older runs lack the new keys
+        cfg.setdefault(name, default)
+    return cfg
+
+
+def utterance_capacity(opts, world):
+    """Utterances per micro-batch this process's net is built for (--maxUtts, default the whole shard)."""
+    return parallel.micro_batch_capacity(opts.maxUtts, opts.batchSize, world)
 
 
 def _select_device():
@@ -116,9 +133,7 @@ def run(args=None):
     cli = _parse(args)
     rank, world = _select_device()
     resumed = cli.cfg_file is not None
-    cfg = load_config(cli.cfg_file) if resumed else dict(vars(cli))
-    for name, _, default, _ in FLAGS:                 # configs written by older runs lack the new keys
-        cfg.setdefault(name, default)
+    cfg = run_config(cli)
     cfg.update(host=get_hostname(), git_rev=get_git_revision(), pid=os.getpid(), test=cli.test)
 
     if resumed:
@@ -161,7 +176,7 @@ def _train(opts, cfg, run_dir, log, rank, world):
     loader = dl.DataLoader(opts.dataDir, opts.rawDim, opts.inputDim, opts.alisDir or opts.dataDir)
     net = rnnet.NNet(opts.inputDim, opts.outputDim, opts.layerSize, opts.numLayers, opts.maxUttLen,
                      temporalLayer=opts.temporalLayer, reg=opts.reg,
-                     maxUtts=parallel.per_rank_capacity(opts.batchSize, world),
+                     maxUtts=utterance_capacity(opts, world),
                      maxLabels=min(opts.maxLabels, opts.maxUttLen))
     net.initParams()
     optimizer = sgd.SGD(net, opts.maxUttLen, alpha=opts.step, momentum=opts.momentum, batchSize=opts.batchSize,

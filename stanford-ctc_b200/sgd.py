@@ -10,7 +10,9 @@ New, additive: `batchSize` utterances per optimisation step (1 reproduces the re
 per-utterance schedule exactly) and data parallelism -- when torch.distributed is initialised the
 `batchSize` utterances of a step are sharded over the ranks and the flat gradient is summed with ONE
 all-reduce (NCCL over NVLink) before the identical, redundant update on every rank.  The clip
-threshold `maxGradNorm` applies to the norm of the summed (reduced) gradient.
+threshold `maxGradNorm` applies to the norm of the summed (reduced) gradient.  A rank whose shard of a step
+holds more utterances than the net's buffers (`model.maxUtts`) accumulates the gradient over micro-batches of at
+most that many and then updates once (step_device_parts), so the batch size is not limited by device memory.
 """
 import logging
 import pickle
@@ -140,6 +142,24 @@ class SGD:
                                              float(self.alpha), float(self.maxGNorm), ptr(self._gnorm2),
                                              ptr(m.stats), stream))
 
+    def step_device_parts(self, pieces, mom):
+        """One Nesterov step whose shard holds more utterances than the net's buffers (model.maxUtts): the gradient is
+        accumulated over consecutive micro-batches (`pieces`: lists of (data, labels) pairs, each at most maxUtts
+        long), then the norm and the update run once.  Each micro-batch is packed into the staging buffer the
+        device is not reading while the previous one computes; the step runs eagerly (not as a CUDA graph).  With a
+        communicator attached, only the last micro-batch's call exchanges, so every rank issues the same
+        collectives whatever its number of micro-batches."""
+        m = self.model
+        stream = _ctcb.current_stream()
+        check(lib.ctcb_axpy_f32(ptr(m.params), ptr(self._vflat), float(mom), m.nparams, stream))
+        for k, piece in enumerate(pieces):
+            batch = m.swap_batches().pack([d for d, _ in piece], [l for _, l in piece]).upload()
+            m.costAndGradDevice(batch, first=(k == 0), last=(k == len(pieces) - 1))
+        check(lib.ctcb_sumsq_f32(ptr(m.grads), m.nparams, ptr(self._gnorm2), ptr(self._scratch), stream))
+        check(lib.ctcb_sgd_nesterov_step_f32(ptr(m.params), ptr(self._vflat), ptr(m.grads), m.nparams, float(mom),
+                                             float(self.alpha), float(self.maxGNorm), ptr(self._gnorm2),
+                                             ptr(m.stats), stream))
+
     def ensure_comm(self):
         """Data parallelism: create this process's ctcb communicator (once per model) and attach it to the net.  The
         NCCL id travels over torch.distributed, which is used for nothing else on the training path."""
@@ -169,10 +189,13 @@ class SGD:
                                                max_labels=m.maxLabels)
         datas = [data_dict[k] for k in used]
         labels = [np.array(alis[k], dtype=np.int32) for k in used]     # only this rank's utterances are converted
-        batch = None
-        if datas:
+        batch, pieces = None, None
+        if len(datas) > m.maxUtts:
+            # more than the buffers hold: micro-batches, packed one by one when the step is launched
+            pieces = parallel.micro_batches(list(zip(datas, labels)), m.maxUtts)
+        elif datas:
             batch = m.swap_batches().pack(datas, labels).upload()
-        return dict(batch=batch, used=used, nlab=sum(l.shape[0] for l in labels),
+        return dict(batch=batch, pieces=pieces, used=used, nlab=sum(l.shape[0] for l in labels),
                     nframes=sum(d.shape[1] for d in datas))
 
     def _launch(self, prep, dist):
@@ -184,6 +207,8 @@ class SGD:
         mom = self._momentum_now()
         if prep["batch"] is not None:
             self.step_device(prep["batch"], mom)
+        elif prep["pieces"]:
+            self.step_device_parts(prep["pieces"], mom)
         else:                  # this rank has no utterance this step: contribute zeros to the exchange
             st = _ctcb.current_stream()
             m.grads_ext.zero_()
@@ -271,7 +296,7 @@ class SGD:
         pending = None
         for i in range(len(chunks)):
             prep = self._prepare(data_dict, alis, chunks[i], rank, world)
-            active = (prep["batch"] is not None) or world > 1
+            active = (prep["batch"] is not None) or bool(prep["pieces"]) or world > 1
             if active:
                 self._launch(prep, dist)
             else:
