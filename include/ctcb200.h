@@ -208,6 +208,15 @@ int ctcb_brnn_sweep_f32(int mode, int T, int B, int H, const int32_t *T_per_utt,
                         const float *actB, float maxAct, void *scratch, size_t scratch_bytes, void *stream);
 /* 1 when the recurrences of a (layerSize H, B utterances, bi-directional) step run on the tensor-core kernel. */
 int ctcb_sweep_uses_tensor_cores(int H, int B);
+/* The plan ctcb_brnn_sweep_f32 launches for (H, B, ndir = 2 bi-directional / 1 forward in time only) on the current
+ * device, under the environment knobs in effect (INTEGRATION.md section 4).  out (HOST, 8 int32):
+ *   {kernel: 0 generic / 1 cluster / 2 tensor-core, KI (H / 32 with register-resident weights, else 0),
+ *    CS (tensor-core: K-slices per cluster; cluster: CTAs per cluster; generic: 0),
+ *    NB (cluster: utterances per cluster) or NS (tensor-core: utterance splits) or the generic kernel's partitions,
+ *    NP (tensor-core: utterances per split), ring stages, partial_own (tensor-core: 1 when the split-K partial has its
+ *    own shared memory), 0}.
+ * Returns the error the launch itself would return for a plan the device cannot hold. */
+int ctcb_debug_sweep_plan(int H, int B, int ndir, int32_t *out);
 
 /* ---- optimiser (replaces sgd.SGD.run arithmetic, ctc_fast/sgd.py:91-161, and
  *      NNet.updateParams, brnnet.py:251-256) --------------------------------------------------- */

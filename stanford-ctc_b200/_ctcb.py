@@ -67,6 +67,7 @@ _PROTOS = {
                                     c_vp, c_sz, c_vp]),
     "ctcb_brnn_sweep_workspace_bytes": (c_sz, [c_int, c_int]),
     "ctcb_sweep_uses_tensor_cores": (c_int, [c_int, c_int]),
+    "ctcb_debug_sweep_plan": (c_int, [c_int, c_int, c_int, ctypes.POINTER(ctypes.c_int32)]),
     "ctcb_brnn_set_deferred_l2": (c_int, [c_vp, c_int]),
     "ctcb_brnn_apply_l2_f32": (c_int, [c_vp, c_vp, c_vp, c_vp]),
     "ctcb_comm_get_unique_id": (c_int, [c_vp]),

@@ -56,4 +56,20 @@ __device__ __forceinline__ float warp_max(float v) {
 
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
+// What run_sweep launches for (H, B, ndir) under the environment knobs in effect.  One function, select_sweep (sweep.cu),
+// makes the choice for the launch, ctcb_debug_sweep_plan and ctcb_sweep_uses_tensor_cores alike.
+enum { SWEEP_GENERIC = 0, SWEEP_CLUSTER = 1, SWEEP_TC = 2 };
+struct SweepPlan {
+    int kernel;             // SWEEP_GENERIC (sweep.cu), SWEEP_CLUSTER (sweep_cluster.cu), SWEEP_TC (sweep_tc.cu)
+    int KI;                 // generic / cluster: H / 32 with the weights in registers; 0: weights re-read (generic)
+    int cs;                 // tensor-core: K-slices per cluster; cluster: CTAs per cluster (H / 64); generic: 0
+    int groups;             // tensor-core: utterance splits (NS); cluster: utterances per cluster (NB); generic: partitions
+    int np;                 // tensor-core: utterances per split, the wgmma N
+    int stages;             // tensor-core: operand ring stages
+    int partial_own;        // tensor-core: 1 when the partial product has a shared-memory region of its own
+    uint32_t stage_bytes;   // tensor-core: bytes per ring stage
+    size_t smem;            // dynamic shared memory per CTA
+};
+int select_sweep(int H, int B, int ndir, SweepPlan *p);
+
 }  // namespace ctcb

@@ -199,81 +199,103 @@ __global__ void add2_kernel(const float *__restrict__ x, const float *__restrict
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) z[i] = x[i] + y[i];
 }
 
+// co-resident CTAs of the generic kernel with this much dynamic shared memory
 template <int KI>
-static int launch_sweep(SweepArgs &a, int slices, size_t smem, cudaStream_t st) {
-    int dev = 0, per_sm = 0;
-    CTCB_CUDA_CHECK(cudaGetDevice(&dev));
+static int sweep_capacity(size_t smem, int *capacity) {
+    int per_sm = 0;
     CTCB_CUDA_CHECK(cudaFuncSetAttribute(sweep_kernel<KI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     CTCB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sweep_kernel<KI>, SW_THREADS, smem));
-    const int capacity = per_sm * num_sms();
-    if (a.ndir * slices > capacity)
-        return set_error(CTCB_EINVAL, "recurrent sweep: layerSize %d needs %d co-resident CTAs, device holds %d",
-                         a.H, a.ndir * slices, capacity);
-    const int ntiles = (a.B + SW_NB - 1) / SW_NB;
-    int parts = capacity / (a.ndir * slices);
-    if (parts > ntiles) parts = ntiles;
-    if (parts > 500) parts = 500;   // counters region holds 1024 words
-    if (parts < 1) parts = 1;
-    a.parts = parts;
+    *capacity = per_sm * num_sms();
+    return CTCB_OK;
+}
+
+template <int KI>
+static int launch_sweep(SweepArgs &a, int slices, const SweepPlan &p, cudaStream_t st) {
+    a.parts = p.groups;
     a.counters += 16;     // words [0..15] are reserved for error flags, which the CALLER clears (once per step)
-    CTCB_CUDA_CHECK(cudaMemsetAsync(a.counters, 0, sizeof(unsigned int) * (a.ndir * parts), st));
-    dim3 grid(slices, parts, a.ndir);
+    CTCB_CUDA_CHECK(cudaMemsetAsync(a.counters, 0, sizeof(unsigned int) * (a.ndir * a.parts), st));
+    dim3 grid(slices, a.parts, a.ndir);
     void *params[] = {&a};
-    CTCB_CUDA_CHECK(cudaLaunchCooperativeKernel((void *)sweep_kernel<KI>, grid, dim3(SW_THREADS), params, smem, st));
+    CTCB_CUDA_CHECK(cudaLaunchCooperativeKernel((void *)sweep_kernel<KI>, grid, dim3(SW_THREADS), params, p.smem, st));
     count_launch();
     return CTCB_OK;
 }
 
-int run_sweep_cluster(int mode, int T, int B, int H, const int32_t *Tlen, const float *pre, const float *Wf,
-                      const float *Wb, float *outF, float *outB, const float *actF, const float *actB, float maxAct,
-                      unsigned int *err, cudaStream_t st, bool *handled);
-int run_sweep_tc(int mode, int T, int B, int H, const int32_t *Tlen, const float *pre, const float *Wf, const float *Wb,
-                 float *outF, float *outB, const float *actF, const float *actB, float maxAct, unsigned int *counters,
-                 void *ws, size_t ws_bytes, cudaStream_t st, bool *handled);
+bool sweep_tc_plan(int H, int B, int ndir, SweepPlan *p);
+bool sweep_cluster_plan(int H, int B, int ndir, SweepPlan *p);
+int run_sweep_cluster(const SweepPlan &p, int mode, int T, int B, int H, const int32_t *Tlen, const float *pre,
+                      const float *Wf, const float *Wb, float *outF, float *outB, const float *actF, const float *actB,
+                      float maxAct, unsigned int *err, cudaStream_t st);
+int run_sweep_tc(const SweepPlan &p, int mode, int T, int B, int H, const int32_t *Tlen, const float *pre, const float *Wf,
+                 const float *Wb, float *outF, float *outB, const float *actF, const float *actB, float maxAct,
+                 unsigned int *counters, void *ws, size_t ws_bytes, cudaStream_t st);
+
+// The one place that decides which kernel runs a sweep of (H, B, ndir): the tensor-core kernel where it applies
+// (H >= 1024, CTCB_SWEEP_TC), else the cluster kernel (H = 128/256/512; CTCB_SWEEP=barrier skips it), else the generic
+// kernel, whose CTAs must all be co-resident.
+int select_sweep(int H, int B, int ndir, SweepPlan *p) {
+    if (H <= 0 || B <= 0 || (ndir != 1 && ndir != 2))
+        return set_error(CTCB_EINVAL, "recurrent sweep: bad sizes (H=%d, B=%d, ndir=%d)", H, B, ndir);
+    if (sweep_tc_plan(H, B, ndir, p)) return CTCB_OK;
+    static int force_barrier = -1;
+    if (force_barrier < 0) {
+        const char *e = getenv("CTCB_SWEEP");
+        force_barrier = (e && e[0] == 'b') ? 1 : 0;
+    }
+    if (!force_barrier && sweep_cluster_plan(H, B, ndir, p)) return CTCB_OK;
+    *p = SweepPlan{};
+    p->kernel = SWEEP_GENERIC;
+    p->KI = (H == 128 || H == 256 || H == 512 || H == 1024) ? H / 32 : 0;
+    const int Hp = (H + 3) / 4 * 4 + 4;
+    p->smem = (size_t)SW_NB * Hp * sizeof(float);
+    int capacity = 0, rc;
+    switch (p->KI) {
+        case 4: rc = sweep_capacity<4>(p->smem, &capacity); break;
+        case 8: rc = sweep_capacity<8>(p->smem, &capacity); break;
+        case 16: rc = sweep_capacity<16>(p->smem, &capacity); break;
+        case 32: rc = sweep_capacity<32>(p->smem, &capacity); break;
+        default: rc = sweep_capacity<0>(p->smem, &capacity); break;
+    }
+    if (rc != CTCB_OK) return rc;
+    const int slices = (H + SW_ROWS - 1) / SW_ROWS;
+    if (ndir * slices > capacity)
+        return set_error(CTCB_EINVAL, "recurrent sweep: layerSize %d needs %d co-resident CTAs, device holds %d",
+                         H, ndir * slices, capacity);
+    const int ntiles = (B + SW_NB - 1) / SW_NB;
+    int parts = capacity / (ndir * slices);
+    if (parts > ntiles) parts = ntiles;
+    if (parts > 500) parts = 500;   // counters region holds 1024 words
+    if (parts < 1) parts = 1;
+    p->groups = parts;
+    return CTCB_OK;
+}
 
 // counters: 4096 bytes of device scratch (word 0 = error flag, cleared by the caller); ws: optional further scratch
 // (sweep_tc_workspace_bytes(H)) that lets the tensor-core kernel run the BPTT mode as well
 int run_sweep(int mode, int T, int B, int H, const int32_t *Tlen, const float *pre, const float *Wf,
               const float *Wb, float *outF, float *outB, const float *actF, const float *actB, float maxAct,
               unsigned int *counters, void *ws, size_t ws_bytes, cudaStream_t st) {
-    {   // tensor-core path (H >= 1024)
-        bool handled = false;
-        const int rc = run_sweep_tc(mode, T, B, H, Tlen, pre, Wf, Wb, outF, outB, actF, actB, maxAct, counters, ws, ws_bytes, st, &handled);
-        if (rc != CTCB_OK) return rc;
-        if (handled) return CTCB_OK;
-    }
+    SweepPlan p;
+    const int rc = select_sweep(H, B, Wb ? 2 : 1, &p);
+    if (rc != CTCB_OK) return rc;
+    if (p.kernel == SWEEP_TC)
+        return run_sweep_tc(p, mode, T, B, H, Tlen, pre, Wf, Wb, outF, outB, actF, actB, maxAct, counters, ws, ws_bytes, st);
+    if (p.kernel == SWEEP_CLUSTER)
+        return run_sweep_cluster(p, mode, T, B, H, Tlen, pre, Wf, Wb, outF, outB, actF, actB, maxAct, counters, st);
     SweepArgs a;
     a.mode = mode; a.T = T; a.B = B; a.H = H; a.Tlen = Tlen; a.pre = pre;
     a.W[0] = Wf; a.W[1] = Wb; a.out[0] = outF; a.out[1] = outB; a.act[0] = actF; a.act[1] = actB;
     a.maxAct = maxAct; a.counters = counters; a.parts = 1;
     a.ndir = Wb ? 2 : 1;
     if (!Wb) { a.W[1] = Wf; a.out[1] = outF; a.act[1] = actF; }   // never dereferenced: gridDim.z == 1
-    {   // cluster/DSMEM fast path (H = 128, 256, 512); CTCB_SWEEP=barrier forces the general kernel
-        static int force_barrier = -1;
-        if (force_barrier < 0) {
-            const char *e = getenv("CTCB_SWEEP");
-            force_barrier = (e && e[0] == 'b') ? 1 : 0;
-        }
-        if (!force_barrier) {
-            bool handled = false;
-            const int rc = run_sweep_cluster(mode, T, B, H, Tlen, pre, Wf, Wb, outF, outB, actF, actB, maxAct, counters, st, &handled);
-            if (rc == CTCB_OK && handled) return CTCB_OK;
-            if (rc != CTCB_OK) cudaGetLastError();   // cluster launch refused: fall through to the general kernel
-        }
-    }
     const int slices = (H + SW_ROWS - 1) / SW_ROWS;
-    const int Hp = (H + 3) / 4 * 4 + 4;
-    const size_t smem = (size_t)SW_NB * Hp * sizeof(float);
-    if (H % 32 == 0) {
-        switch (H / 32) {
-            case 4: return launch_sweep<4>(a, slices, smem, st);
-            case 8: return launch_sweep<8>(a, slices, smem, st);
-            case 16: return launch_sweep<16>(a, slices, smem, st);
-            case 32: return launch_sweep<32>(a, slices, smem, st);
-            default: break;
-        }
+    switch (p.KI) {
+        case 4: return launch_sweep<4>(a, slices, p, st);
+        case 8: return launch_sweep<8>(a, slices, p, st);
+        case 16: return launch_sweep<16>(a, slices, p, st);
+        case 32: return launch_sweep<32>(a, slices, p, st);
+        default: return launch_sweep<0>(a, slices, p, st);
     }
-    return launch_sweep<0>(a, slices, smem, st);
 }
 
 int run_add2(const float *x, const float *y, float *z, int64_t n, cudaStream_t st) {
@@ -286,3 +308,18 @@ int run_add2(const float *x, const float *y, float *z, int64_t n, cudaStream_t s
 }
 
 }  // namespace ctcb
+
+extern "C" int ctcb_debug_sweep_plan(int H, int B, int ndir, int32_t *out) {
+    if (!out) return ctcb::set_error(CTCB_EINVAL, "ctcb_debug_sweep_plan: null output");
+    ctcb::SweepPlan p;
+    const int rc = ctcb::select_sweep(H, B, ndir, &p);
+    if (rc != CTCB_OK) return rc;
+    const int32_t v[8] = {p.kernel, p.KI, p.cs, p.groups, p.np, p.stages, p.partial_own, 0};
+    for (int i = 0; i < 8; ++i) out[i] = v[i];
+    return CTCB_OK;
+}
+
+extern "C" int ctcb_sweep_uses_tensor_cores(int H, int B) {
+    ctcb::SweepPlan p;
+    return (ctcb::select_sweep(H, B, 2, &p) == CTCB_OK && p.kernel == ctcb::SWEEP_TC) ? 1 : 0;
+}

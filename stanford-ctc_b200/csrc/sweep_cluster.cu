@@ -235,8 +235,9 @@ static int launch_cluster_nb(const SweepClusterArgs &a, int ntiles, cudaStream_t
     return CTCB_OK;
 }
 
+// co-resident clusters of the (KI, 8) kernel, the largest of its shared-memory footprints
 template <int KI>
-static int launch_cluster(const SweepClusterArgs &a, cudaStream_t st, bool *handled) {
+static int cluster_max_active() {
     constexpr int CS = KI / 2;
     static int max_clusters = -1;
     if (max_clusters < 0) {
@@ -254,47 +255,65 @@ static int launch_cluster(const SweepClusterArgs &a, cudaStream_t st, bool *hand
         max_clusters = n;
         if (getenv("CTCB_DEBUG")) fprintf(stderr, "[ctcb] cluster sweep H=%d: cluster=%d CTAs, max active clusters=%d\n", 32 * KI, CS, n);
     }
-    *handled = false;
-    if (max_clusters < 1) return CTCB_OK;
+    return max_clusters;
+}
+
+// The cluster plan for (H, B, ndir): false where the kernel does not apply (H not 128/256/512, or one wave of clusters
+// cannot hold the batch and CTCB_SWEEP_NB does not force a group size)
+bool sweep_cluster_plan(int H, int B, int ndir, SweepPlan *p) {
+    int max_clusters;
+    switch (H) {
+        case 128: max_clusters = cluster_max_active<4>(); break;
+        case 256: max_clusters = cluster_max_active<8>(); break;
+        case 512: max_clusters = cluster_max_active<16>(); break;
+        default: return false;
+    }
+    if (max_clusters < 1) return false;
     static int nb_env = -1;   // CTCB_SWEEP_NB=1..8 forces the group size
     if (nb_env < 0) { const char *e = getenv("CTCB_SWEEP_NB"); nb_env = e ? atoi(e) : 0; }
     // fewest utterances per cluster (= least arithmetic per SM and step) that still fits one wave of clusters
     int nb = 0;
     for (int c = 1; c <= 8; ++c)
-        if (a.ndir * ((a.B + c - 1) / c) <= max_clusters) { nb = c; break; }
+        if (ndir * ((B + c - 1) / c) <= max_clusters) { nb = c; break; }
     if (nb_env >= 1 && nb_env <= 8) nb = nb_env;
-    if (nb == 0) return CTCB_OK;          // would need a second wave of clusters: the general kernel is faster
-    const int ntiles = (a.B + nb - 1) / nb;
-    int rc;
-    switch (nb) {
-        case 1: rc = launch_cluster_nb<KI, 1>(a, ntiles, st); break;
-        case 2: rc = launch_cluster_nb<KI, 2>(a, ntiles, st); break;
-        case 3: rc = launch_cluster_nb<KI, 3>(a, ntiles, st); break;
-        case 4: rc = launch_cluster_nb<KI, 4>(a, ntiles, st); break;
-        case 5: rc = launch_cluster_nb<KI, 5>(a, ntiles, st); break;
-        case 6: rc = launch_cluster_nb<KI, 6>(a, ntiles, st); break;
-        case 7: rc = launch_cluster_nb<KI, 7>(a, ntiles, st); break;
-        default: rc = launch_cluster_nb<KI, 8>(a, ntiles, st); break;
-    }
-    if (rc == CTCB_OK) *handled = true;
-    return rc;
+    if (nb == 0) return false;          // would need a second wave of clusters: the general kernel is faster
+    *p = SweepPlan{};
+    p->kernel = SWEEP_CLUSTER;
+    p->KI = H / 32;
+    p->cs = H / 64;
+    p->groups = nb;
+    p->smem = cluster_smem_bytes(H / 32, nb);
+    return true;
 }
 
-int run_sweep_cluster(int mode, int T, int B, int H, const int32_t *Tlen, const float *pre, const float *Wf,
-                      const float *Wb, float *outF, float *outB, const float *actF, const float *actB, float maxAct,
-                      unsigned int *err, cudaStream_t st, bool *handled) {
-    *handled = false;
-    if (H != 128 && H != 256 && H != 512) return CTCB_OK;
+template <int KI>
+static int launch_cluster(const SweepClusterArgs &a, int nb, cudaStream_t st) {
+    const int ntiles = (a.B + nb - 1) / nb;
+    switch (nb) {
+        case 1: return launch_cluster_nb<KI, 1>(a, ntiles, st);
+        case 2: return launch_cluster_nb<KI, 2>(a, ntiles, st);
+        case 3: return launch_cluster_nb<KI, 3>(a, ntiles, st);
+        case 4: return launch_cluster_nb<KI, 4>(a, ntiles, st);
+        case 5: return launch_cluster_nb<KI, 5>(a, ntiles, st);
+        case 6: return launch_cluster_nb<KI, 6>(a, ntiles, st);
+        case 7: return launch_cluster_nb<KI, 7>(a, ntiles, st);
+        default: return launch_cluster_nb<KI, 8>(a, ntiles, st);
+    }
+}
+
+int run_sweep_cluster(const SweepPlan &p, int mode, int T, int B, int H, const int32_t *Tlen, const float *pre,
+                      const float *Wf, const float *Wb, float *outF, float *outB, const float *actF, const float *actB,
+                      float maxAct, unsigned int *err, cudaStream_t st) {
     SweepClusterArgs a;
     a.mode = mode; a.T = T; a.B = B; a.H = H; a.Tlen = Tlen; a.pre = pre;
     a.W[0] = Wf; a.W[1] = Wb; a.out[0] = outF; a.out[1] = outB; a.act[0] = actF; a.act[1] = actB; a.maxAct = maxAct; a.err = err;
     a.ndir = Wb ? 2 : 1;
     if (!Wb) { a.W[1] = Wf; a.out[1] = outF; a.act[1] = actF; }
-    switch (H / 32) {
-        case 4: return launch_cluster<4>(a, st, handled);
-        case 8: return launch_cluster<8>(a, st, handled);
-        case 16: return launch_cluster<16>(a, st, handled);
-        default: return CTCB_OK;
+    switch (H) {
+        case 128: return launch_cluster<4>(a, p.groups, st);
+        case 256: return launch_cluster<8>(a, p.groups, st);
+        case 512: return launch_cluster<16>(a, p.groups, st);
+        default: return set_error(CTCB_EINVAL, "cluster sweep: layerSize %d is not 128, 256 or 512", H);
     }
 }
 

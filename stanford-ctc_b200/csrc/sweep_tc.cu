@@ -426,8 +426,6 @@ static StcEncodeFn stc_encode() {
     return fn;
 }
 
-struct StcPlan { int cs, NS, Npad, stages, partial_own; uint32_t stage_bytes; size_t smem; };
-
 static constexpr size_t STC_SMEM_MAX = 208 * 1024;      // ring + partial budget (+ barriers) within the 227 KB per CTA
 
 // co-resident clusters of cs CTAs (the kernel's shared memory does not depend on NP for this question: every plan
@@ -457,7 +455,7 @@ static int stc_max_clusters(int cs) {
 
 // Per cluster size, largest first: every CTA of the grid must be co-resident (they meet at the counter barrier), and a
 // CTA finalises at most 64 utterance columns (NP / cs <= 64).
-static bool stc_plan_cs(int H, int B, int ndir, int cs, StcPlan *p) {
+static bool stc_plan_cs(int H, int B, int ndir, int cs, SweepPlan *p) {
     const int MT = H / STC_BM;
     if ((H / cs) % STC_BK != 0) return false;
     const int maxc = stc_max_clusters(cs);
@@ -471,9 +469,11 @@ static bool stc_plan_cs(int H, int B, int ndir, int cs, StcPlan *p) {
     if (NS < 1) NS = 1;
     const int Npad = ((B + NS - 1) / NS + 31) / 32 * 32;   // the wgmma N of the kernel: a multiple of 32 up to 256
     if (Npad > 256 || Npad > 64 * cs) return false;
+    p->kernel = SWEEP_TC;
+    p->KI = 0;
     p->cs = cs;
-    p->NS = (B + Npad - 1) / Npad;           // drop splits that would be empty
-    p->Npad = Npad;
+    p->groups = (B + Npad - 1) / Npad;       // drop splits that would be empty
+    p->np = Npad;
     const size_t partial_bytes = (size_t)Npad * 512;
     p->stage_bytes = 2 * STC_A_BYTES + 2 * (uint32_t)Npad * 128u;
     // own region for the partial when at least two ring stages still fit beside it
@@ -487,12 +487,15 @@ static bool stc_plan_cs(int H, int B, int ndir, int cs, StcPlan *p) {
     return true;
 }
 
-static bool stc_plan(int H, int B, int ndir, StcPlan *p) {
+static bool stc_plan(int H, int B, int ndir, SweepPlan *p) {
     if (H % 128 != 0 || H < 512 || B < 1) return false;
-    for (int cs = 4; cs >= 1; cs >>= 1)
+    static int cs_env = -1;   // CTCB_SWEEP_TC_CS=n: the largest cluster size tried (co-residency still decides)
+    if (cs_env < 0) { const char *e = getenv("CTCB_SWEEP_TC_CS"); cs_env = e ? atoi(e) : 0; }
+    const int cs_max = (cs_env >= 4 || cs_env <= 0) ? 4 : (cs_env >= 2 ? 2 : 1);
+    for (int cs = cs_max; cs >= 1; cs >>= 1)
         if (stc_plan_cs(H, B, ndir, cs, p)) {
             if (getenv("CTCB_DEBUG"))
-                fprintf(stderr, "[ctcb] tensor-core sweep H=%d B=%d: clusters of %d, %d utterance split(s) of %d\n", H, B, cs, p->NS, p->Npad);
+                fprintf(stderr, "[ctcb] tensor-core sweep H=%d B=%d: clusters of %d, %d utterance split(s) of %d\n", H, B, cs, p->groups, p->np);
             return true;
         }
     return false;
@@ -531,13 +534,13 @@ static cudaError_t stc_launch_np(int np, cudaLaunchConfig_t *cfg, const CUtensor
     }
 }
 
-int run_sweep_tc(int mode, int T, int B, int H, const int32_t *Tlen, const float *pre, const float *Wf, const float *Wb,
-                 float *outF, float *outB, const float *actF, const float *actB, float maxAct, unsigned int *counters,
-                 void *ws, size_t ws_bytes, cudaStream_t st, bool *handled) {
-    *handled = false;
+// the tensor-core plan for (H, B, ndir), when this kernel applies
+bool sweep_tc_plan(int H, int B, int ndir, SweepPlan *p) { return stc_enabled(H) && stc_plan(H, B, ndir, p); }
+
+int run_sweep_tc(const SweepPlan &p, int mode, int T, int B, int H, const int32_t *Tlen, const float *pre, const float *Wf,
+                 const float *Wb, float *outF, float *outB, const float *actF, const float *actB, float maxAct,
+                 unsigned int *counters, void *ws, size_t ws_bytes, cudaStream_t st) {
     const int ndir = Wb ? 2 : 1;
-    StcPlan p;
-    if (!stc_enabled(H) || !stc_plan(H, B, ndir, &p)) return CTCB_OK;
     // the plan applies, so the generic kernel is no substitute: a scratch that cannot hold the operand stacks is an error
     if (!ws || ws_bytes < sweep_tc_workspace_bytes(H, B) || (((uintptr_t)ws) & 255))
         return set_error(CTCB_ENOMEM, "tensor-core sweep (H=%d, B=%d) needs %zu bytes of 256-byte aligned scratch, got %zu%s",
@@ -567,7 +570,7 @@ int run_sweep_tc(int mode, int T, int B, int H, const int32_t *Tlen, const float
         {
             cuuint64_t dims[4] = {(cuuint64_t)H, (cuuint64_t)B, 2, 2};
             cuuint64_t strides[3] = {(cuuint64_t)H * sizeof(float), (cuuint64_t)B * H * sizeof(float), (cuuint64_t)2 * B * H * sizeof(float)};
-            cuuint32_t box[4] = {(cuuint32_t)STC_BK, (cuuint32_t)p.Npad, 2, 1};
+            cuuint32_t box[4] = {(cuuint32_t)STC_BK, (cuuint32_t)p.np, 2, 1};
             cuuint32_t es[4] = {1, 1, 1, 1};
             CUresult r = enc(&tmR[d], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void *)(ring + (size_t)dd * 4 * B * H), dims, strides, box, es,
                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
@@ -580,7 +583,7 @@ int run_sweep_tc(int mode, int T, int B, int H, const int32_t *Tlen, const float
     a.out[0] = outs[0]; a.out[1] = outs[1]; a.act[0] = actF; a.act[1] = Wb ? actB : actF; a.maxAct = maxAct;
     a.ring[0] = ring; a.ring[1] = ring + (size_t)(ndir - 1) * 4 * B * H;
     a.err = counters; a.counters = counters + 16;
-    a.ndir = ndir; a.MT = H / STC_BM; a.NS = p.NS; a.cs = p.cs; a.nkb = H / p.cs / STC_BK;
+    a.ndir = ndir; a.MT = H / STC_BM; a.NS = p.groups; a.cs = p.cs; a.nkb = H / p.cs / STC_BK;
     a.stages = p.stages; a.stage_bytes = p.stage_bytes; a.partial_own = p.partial_own;
     a.trace = nullptr;
     {
@@ -588,9 +591,9 @@ int run_sweep_tc(int mode, int T, int B, int H, const int32_t *Tlen, const float
         if (trace_env < 0) trace_env = getenv("CTCB_SWEEP_TRACE") ? 1 : 0;
         if (trace_env) a.trace = (unsigned long long *)((char *)ws + stc_ws_stack_bytes(H) + stc_ws_ring_bytes(H, B));
     }
-    CTCB_CUDA_CHECK(cudaMemsetAsync(a.counters, 0, sizeof(unsigned int) * (size_t)(ndir * p.NS), st));
+    CTCB_CUDA_CHECK(cudaMemsetAsync(a.counters, 0, sizeof(unsigned int) * (size_t)(ndir * p.groups), st));
     cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(p.cs, a.MT * p.NS, ndir);
+    cfg.gridDim = dim3(p.cs, a.MT * p.groups, ndir);
     cfg.blockDim = dim3(STC_THREADS);
     cfg.dynamicSmemBytes = p.smem;
     cfg.stream = st;
@@ -604,25 +607,17 @@ int run_sweep_tc(int mode, int T, int B, int H, const int32_t *Tlen, const float
     if (coop < 0) { const char *e = getenv("CTCB_SWEEP_TC_COOP"); if (e && atoi(e) == 0) coop = 0; }
     if (coop != 0) {
         cfg.numAttrs = 2;
-        cudaError_t e = stc_launch_np(p.Npad, &cfg, tmW, tmR, a);
-        if (e == cudaSuccess) { coop = 1; count_launch(); *handled = true; return CTCB_OK; }
+        cudaError_t e = stc_launch_np(p.np, &cfg, tmW, tmR, a);
+        if (e == cudaSuccess) { coop = 1; count_launch(); return CTCB_OK; }
         cudaGetLastError();
         if (coop == 1) return set_error(CTCB_ECUDA, "sweep_tc: launch failed: %s", cudaGetErrorString(e));
         coop = 0;
         if (getenv("CTCB_DEBUG")) fprintf(stderr, "[ctcb] tensor-core sweep: cooperative+cluster launch refused (%s), plain cluster launch\n", cudaGetErrorString(e));
     }
     cfg.numAttrs = 1;         // grid <= one wave of clusters by construction (stc_plan)
-    CTCB_CUDA_CHECK(stc_launch_np(p.Npad, &cfg, tmW, tmR, a));
+    CTCB_CUDA_CHECK(stc_launch_np(p.np, &cfg, tmW, tmR, a));
     count_launch();
-    *handled = true;
     return CTCB_OK;
 }
 
-bool sweep_tc_would_run(int H, int B, int ndir) {
-    StcPlan p;
-    return stc_enabled(H) && stc_plan(H, B, ndir, &p);
-}
-
 }  // namespace ctcb
-
-extern "C" int ctcb_sweep_uses_tensor_cores(int H, int B) { return ctcb::sweep_tc_would_run(H, B, 2) ? 1 : 0; }

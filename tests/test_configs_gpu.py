@@ -47,6 +47,10 @@ CASES = {
     # and 41*23 = 943 (TIMIT, timit-utils/runTimit.sh:21) -- the first-layer contractions then run on the tensor cores
     "swbd_input_d615_b4": dict(D=615, K=35, H=512, N=2, tl=1, T=120, L=20, B=4),
     "timit_input_d943_b4": dict(D=943, K=62, H=512, N=2, tl=1, T=120, L=20, B=4),
+    # the uni-directional net (nnets.rnnet) at a C3 width: its recurrence alone on the tensor-core sweep
+    "c3_unidirectional_b8": dict(D=41, K=32, H=1024, N=3, tl=2, T=120, L=20, B=8, uni=True, sweep=dict(kernel=2)),
+    # a C3 micro-batch wider than four-CTA clusters can hold at once: the sweep runs on clusters of two
+    "c3_b260_two_cta_clusters": dict(D=41, K=32, H=1024, N=3, tl=2, T=16, L=5, B=260, sweep=dict(kernel=2, CS=2)),
 }
 
 
@@ -60,9 +64,18 @@ def _record(name, rec):
 
 @pytest.mark.parametrize("name", list(CASES))
 def test_full_net_at_baseline_config(name, cuda):
-    import nnets.brnnet as rnnet
+    import ctypes
+    import nnets.brnnet as brnnet
+    import nnets.rnnet as unirnnet
+    from _ctcb import lib, check
     c = CASES[name]
     D, K, H, N, tl, T, L, B = (c[k] for k in ("D", "K", "H", "N", "tl", "T", "L", "B"))
+    uni = bool(c.get("uni"))
+    if "sweep" in c:       # the recurrent sweep plan this case is meant to run (ctcb_debug_sweep_plan)
+        plan = (ctypes.c_int32 * 8)()
+        check(lib.ctcb_debug_sweep_plan(H, B, 1 if uni else 2, plan))
+        got = dict(kernel=plan[0], CS=plan[2])
+        assert all(got[k] == v for k, v in c["sweep"].items()), (got, c["sweep"])
     rng = np.random.RandomState(5)
     if c.get("ragged"):
         lens = [int(x) for x in rng.randint(int(0.6 * T), T + 1, size=B)]
@@ -72,17 +85,15 @@ def test_full_net_at_baseline_config(name, cuda):
         lens, nlabs = [T] * B, [L] * B
     datas, labelss = recipes.synth_batch(D, K, lens, nlabs, seed=33)
     np.random.seed(33)
-    on = brnn_oracle.NNet(D, K, H, N, T, temporalLayer=tl, dtype=np.float64)
+    on = brnn_oracle.NNet(D, K, H, N, T, temporalLayer=tl, dtype=np.float64, unidirectional=uni)
     on.initParams()
     np.random.seed(33)
-    nn = rnnet.NNet(D, K, H, N, T, temporalLayer=tl, maxUtts=B, maxLabels=L)
+    nn = (unirnnet if uni else brnnet).NNet(D, K, H, N, T, temporalLayer=tl, maxUtts=B, maxLabels=L)
     nn.initParams()
     costs, grad, skips = nn.costAndGradBatch(datas, labelss)
     g_host = [(dw.cpu().numpy().astype(np.float64), db.cpu().numpy().astype(np.float64)) for dw, db in grad]
 
     # the activations the GPU pass left in its workspace, time-major [Tmax][B][n]
-    import ctypes
-    from _ctcb import lib, check
     Tmax = max(lens)
 
     def act(what, layer):
@@ -92,7 +103,9 @@ def test_full_net_at_baseline_config(name, cuda):
         return nn._ws[off.value:off.value + 4 * n].view(cuda.float32).view(Tmax, B, width.value).cpu().numpy()
 
     X = [None] + [act(0, i) for i in range(1, N + 2)]
-    For, Back = act(1, 0), act(2, 0)
+    For, Back = act(1, 0), (None if uni else act(2, 0))
+    if uni:
+        X[tl] = For          # the uni-directional temporal layer's output is the forward sweep itself (rnnet.py:112-116)
     del nn
     cuda.cuda.empty_cache()
 
@@ -114,8 +127,12 @@ def test_full_net_at_baseline_config(name, cuda):
         for i in range(1, N + 2):
             g = X[i][:Tu, u, :].T.astype(np.float64)
             fwd_err = max(fwd_err, float(np.abs(g - h[i]).max() / max(np.abs(h[i]).max(), 1e-30)))
-        gF, gB = For[:Tu, u, :].T.astype(np.float64), Back[:Tu, u, :].T.astype(np.float64)
-        fwd_err = max(fwd_err, float(np.abs(gF - F).max() / np.abs(F).max()), float(np.abs(gB - Bk).max() / np.abs(Bk).max()))
+        gF = For[:Tu, u, :].T.astype(np.float64)
+        fwd_err = max(fwd_err, float(np.abs(gF - F).max() / np.abs(F).max()))
+        gB = None
+        if not uni:
+            gB = Back[:Tu, u, :].T.astype(np.float64)
+            fwd_err = max(fwd_err, float(np.abs(gB - Bk).max() / np.abs(Bk).max()))
         c_, g_, s_ = on.costAndGradGiven(d, l, [X[i][:Tu, u, :].T for i in range(1, N + 2)], gF, gB)
         assert not s_
         for (tw, tb), (gw, gb) in zip(tot, g_):
