@@ -8,9 +8,9 @@
 //   * every CTA holds the complete previous state of its NB utterances in shared memory, laid out
 //     [source CTA][utterance][64 units] so that one CTA's contribution is one contiguous block;
 //   * after a step, each CTA pushes its block into the shared memory of all CS CTAs of the cluster with
-//     cp.async.bulk (shared::cta -> shared::cluster); the copies complete_tx on the DESTINATION's mbarrier,
-//     which is the only inter-CTA synchronisation of the step: a CTA starts step s as soon as the CS blocks of
-//     step s-1 have landed.  Two state buffers / two barriers alternate;
+//     4-byte st.async remote stores; each completes its bytes on the DESTINATION's mbarrier for that source CTA,
+//     which is the only inter-CTA synchronisation of the step: a warp starts step s as soon as the one block of
+//     step s-1 it reads has landed.  Two state buffers, each with CS barriers (one per source CTA), alternate;
 //   * For/Back (dFor/dBack) are still streamed to HBM for the GEMMs that follow, off the chain.
 #include "common.cuh"
 #include <stdlib.h>
@@ -78,6 +78,14 @@ __device__ __forceinline__ void ffma_pair(float2 &d, float2 w, float h) {
 //     sums of an output meet in shared memory (the one CTA barrier of the step), where thread (utterance, unit)
 //     adds them, applies clip/mask, stores the state to HBM and sends it to the CS peers with st.async.
 //   state layout in every CTA: [buffer 2][source CTA][utterance][unit 64]
+// Measured on one H100 80GB HBM3 (power limit 700 W, max SM clock 1980 MHz), tools/sweep_time.py, T = 200, H = 512,
+// forward / BPTT in us per step: B = 4 (NB = 1) 0.69 / 0.62, B = 8 (NB = 2) 0.98 / 0.91, B = 16 (NB = 3) 1.24 / 1.21,
+// B = 32 (NB = 5) 1.77 / 1.78.  Fit: 0.43 / 0.33 us fixed (wait, barrier, reduction, exchange) + 0.27 / 0.29 us per
+// utterance of the cluster, of which 32768 FMA per SM at the FFMA peak (128 per clock) would take 0.13 us.
+// One barrier per source CTA instead of one per buffer: B = 32 went from 1.87 / 1.81 to 1.77 / 1.78 (the fit above);
+// deciding the mask before the barrier and sending before the HBM store then gave 1.74-1.76 / 1.72-1.73.  Sending the
+// state as one 16-byte st.async per lane quad and peer (three shuffles to assemble it) was slower on the same card,
+// 2.00 / 1.96 with the single barrier and 1.85 / 1.81 with per-source barriers, so the stores stay 4-byte.
 // ---------------------------------------------------------------------------------------------------
 template <int KI, int NB>
 __global__ void __launch_bounds__(512, 1) sweep_cluster_kernel(SweepClusterArgs a) {
@@ -90,7 +98,7 @@ __global__ void __launch_bounds__(512, 1) sweep_cluster_kernel(SweepClusterArgs 
     extern __shared__ __align__(128) float sc_smem[];
     float (*hbuf)[CS * BLKF] = reinterpret_cast<float (*)[CS * BLKF]>(sc_smem);                  // [2][source CTA][utterance][unit]
     float (*red)[16][BLKF] = reinterpret_cast<float (*)[16][BLKF]>(sc_smem + 2 * CS * BLKF);     // [2][16 warps][utterance][unit]
-    unsigned long long *mbar = reinterpret_cast<unsigned long long *>(sc_smem + (2 * CS + 32) * BLKF);
+    unsigned long long (*mbar)[CS] = reinterpret_cast<unsigned long long (*)[CS]>(sc_smem + (2 * CS + 32) * BLKF);   // [2][source CTA]
 
     const int B = a.B, T = a.T;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -114,13 +122,13 @@ __global__ void __launch_bounds__(512, 1) sweep_cluster_kernel(SweepClusterArgs 
                      : make_float2(W[(int64_t)j * H + kk], W[(int64_t)(j + 1) * H + kk]);
     }
 
-    const uint32_t bar0 = smem_u32(&mbar[0]), bar1 = smem_u32(&mbar[1]);
+    // one barrier per (state buffer, source CTA), each expecting one block
     if (tid == 0) {
-        mbar_init(bar0, 1);
-        mbar_init(bar1, 1);
+#pragma unroll
+        for (int i = 0; i < 2 * CS; ++i) mbar_init(smem_u32(&mbar[i / CS][i % CS]), 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        mbar_arrive_expect_tx(bar0, CS * BLK_BYTES);
-        mbar_arrive_expect_tx(bar1, CS * BLK_BYTES);
+#pragma unroll
+        for (int i = 0; i < 2 * CS; ++i) mbar_arrive_expect_tx(smem_u32(&mbar[i / CS][i % CS]), BLK_BYTES);
     }
     cluster_sync_all();
 
@@ -130,21 +138,28 @@ __global__ void __launch_bounds__(512, 1) sweep_cluster_kernel(SweepClusterArgs 
     const bool owner = tid < BLKF;
     const bool valid = owner && (b < B);
     const int Tb = valid ? __ldg(a.Tlen + b) : 0;
-    // where this warp's slice of the state sits inside a buffer: source CTA k0/64, offset k0%64
-    const int hoff = (k0 >> 6) * BLKF + (k0 & 63);
+    // where this warp's slice of the state sits inside a buffer: source CTA k0/64, offset k0%64.  The warp reads
+    // nothing else, so it waits only for that source's barrier and starts while later blocks are still landing.
+    const int src = k0 >> 6;
+    const int hoff = src * BLKF + (k0 & 63);
+    // where this thread's state value goes in every CTA (buffer 0; buffer 1 is CS blocks further), and the barrier
+    // of (buffer 0, this CTA) it completes
+    const uint32_t dst0 = smem_u32(&hbuf[0][rank * BLKF + tid]);
+    const uint32_t dbar0 = smem_u32(&mbar[0][rank]);
     bool dead = false;
 
     for (int s = 0; s < T; ++s) {
         const int t = ascending ? s : T - 1 - s;
+        const int64_t o = ((int64_t)t * B + b) * H + oj;       // (t, b, oj) in pre, act and out
         float pre_v = 0.f, act_v = 0.f;
         if (valid) {
-            const int64_t o = ((int64_t)t * B + b) * H + oj;
             pre_v = __ldg(a.pre + o);
             if (bptt) act_v = __ldg(act + o);
         }
+        bool keep = false;                                        // false: v is masked to 0 (padded frame, BPTT outside (0, maxAct))
         float sum = 0.f;
         if (s > 0) {
-            const uint32_t bar = (s & 1) ? bar1 : bar0;
+            const uint32_t bar = smem_u32(&mbar[s & 1][src]);
             const uint32_t parity = (uint32_t)(((s - 1) >> 1) & 1);
             if (!dead && !mbar_try_wait(bar, parity)) {
                 const long long t_start = clock64();
@@ -173,9 +188,17 @@ __global__ void __launch_bounds__(512, 1) sweep_cluster_kernel(SweepClusterArgs 
 #pragma unroll
             for (int u = 0; u < NB; ++u)
                 *reinterpret_cast<float2 *>(&red[s & 1][warp][u * 64 + 2 * lane]) = acc2[u];
+            // the mask needs only this step's inputs: decide it while the other warps finish
+            keep = valid && t < Tb && (!bptt || (act_v > 0.f && act_v < a.maxAct));
             __syncthreads();            // the only CTA barrier of the step (red is double-buffered)
-            // every warp is past its wait on this step's barrier: arm it for step s + 2
-            if (tid == 0 && s + 2 < T) mbar_arrive_expect_tx(bar, CS * BLK_BYTES);
+            // Every warp is past its wait on this step's barriers: arm them for step s + 2.  Reusing buffer s & 1 is
+            // safe because every send of step s comes after the step-s __syncthreads.  A peer writes buffer s & 1
+            // again with its sends of step s + 1, which follow its step-(s + 1) waits, which need this CTA's block of
+            // step s, which this CTA sends only after all its warps have read buffer s & 1 (and so after each
+            // barrier s & 1 has completed this step's phase).  Those writes may still land before the arm below:
+            // their complete_tx only drives the transaction count negative, and the phase cannot complete while
+            // the arm's arrival is pending; the arm then adds BLK_BYTES back and the phase completes at zero.
+            if (tid < CS && s + 2 < T) mbar_arrive_expect_tx(smem_u32(&mbar[s & 1][tid]), BLK_BYTES);
             if (owner) {
                 float s0 = 0.f, s1 = 0.f;
 #pragma unroll
@@ -183,29 +206,29 @@ __global__ void __launch_bounds__(512, 1) sweep_cluster_kernel(SweepClusterArgs 
                 sum = s0 + s1;
             }
         }
-        float v = 0.f;
-        if (valid) {
-            v = pre_v + sum;
-            if (!bptt) v = fminf(fmaxf(v, 0.f), a.maxAct);
-            else v = (act_v > 0.f && act_v < a.maxAct) ? v : 0.f;
-            if (t >= Tb) v = 0.f;
-            out[((int64_t)t * B + b) * H + oj] = v;
-        }
+        if (s == 0) keep = valid && t < Tb && (!bptt || (act_v > 0.f && act_v < a.maxAct));
+        float v = pre_v + sum;
+        if (!bptt) v = fminf(fmaxf(v, 0.f), a.maxAct);
+        v = keep ? v : 0.f;
         if (owner && s + 1 < T) {
             // hand the new state to every CTA of the cluster (this one included): one remote 4-byte store per
-            // peer, each completing 4 bytes on the peer's barrier of step s + 1
-            const int nb = (s + 1) & 1;
-            const uint32_t dst = smem_u32(&hbuf[nb][rank * BLKF + tid]);
-            const uint32_t dbar = nb ? bar1 : bar0;
+            // peer, each completing 4 bytes on the peer's barrier of (step s + 1, this CTA).  Invalid owners send
+            // their zeros too: the barrier expects a whole block.  The sends are the serial chain of the sweep,
+            // so they go out before the HBM store.
+            const uint32_t nbo = (uint32_t)((s + 1) & 1);
+            const uint32_t dst = dst0 + nbo * (uint32_t)(CS * BLK_BYTES);
+            const uint32_t dbar = dbar0 + nbo * (uint32_t)(CS * sizeof(unsigned long long));
 #pragma unroll
             for (int c = 0; c < CS; ++c) st_async_f32(map_to_cta(dst, (uint32_t)c), v, map_to_cta(dbar, (uint32_t)c));
         }
+        if (valid) out[o] = v;
     }
     cluster_sync_all();
 }
 
+// state buffers + partial sums + 2 x CS mbarriers
 static constexpr size_t cluster_smem_bytes(int KI, int NB) {
-    return sizeof(float) * (size_t)(2 * (KI / 2) + 32) * (size_t)(NB * 64) + 16;
+    return sizeof(float) * (size_t)(2 * (KI / 2) + 32) * (size_t)(NB * 64) + 2 * (KI / 2) * sizeof(unsigned long long);
 }
 
 template <int KI, int NB>
