@@ -95,6 +95,24 @@ int ctcb_gemm_f32(int transA, int transB, int M, int N, int K, float alpha,
                   const float *A, int64_t lda, const float *B, int64_t ldb, float beta,
                   float *C, int64_t ldc, const float *bias, int relu, const float *mask_src,
                   void *workspace, size_t ws_bytes, void *stream);
+/* Two contractions of one shape, pitches, alpha and beta (no bias, ReLU or mask): C0 = op(A0) op(B0), C1 = op(A1) op(B1).
+ * On the tensor cores both share one launch and one split-K reduce when every operand can be read in place; each
+ * result is then the same as that of the single call at the same split.  Otherwise two ctcb_gemm_f32 calls. */
+size_t ctcb_gemm_pair_workspace_bytes(int M, int N, int K);
+int ctcb_gemm_pair_f32(int transA, int transB, int M, int N, int K, float alpha,
+                       const float *A0, const float *A1, int64_t lda, const float *B0, const float *B1, int64_t ldb,
+                       float beta, float *C0, float *C1, int64_t ldc, void *workspace, size_t ws_bytes, void *stream);
+/* The plan ctcb_gemm_f32 (problems = 1) or ctcb_gemm_pair_f32 (problems = 2) runs for these arguments under the
+ * environment knobs in effect (INTEGRATION.md section 4), assuming a large enough workspace.  A and B are only
+ * inspected for their alignment.  out (HOST, 8 int32):
+ *   {kernel: 0 FFMA / 1 tensor core, BN (output tile width), ring stages, K splits, CTAs per launch,
+ *    A path, B path: 0 read in place K-major / 1 read in place MN-major, transposed in shared memory / 2 copied into
+ *    the workspace first,  problems per launch (2: the pair shares one launch)}.  The FFMA kernel reports {0, .., 0, 1}. */
+int ctcb_debug_gemm_plan(int transA, int transB, int M, int N, int K, const float *A, int64_t lda,
+                         const float *B, int64_t ldb, int problems, int32_t *out);
+/* Measurement: 1 sends MN-major tensor-core operands through a transposed copy in the workspace, as the environment
+ * variable CTCB_GEMM_TC_COPY=1 does; 0 reads them in place (the default).  Results are the same either way. */
+int ctcb_debug_set_gemm_copy(int on);
 
 /* Diagnostic / measurement: force the CTC kernel organisation used by ctcb_ctc_loss_grad_f32 (and the BRNN step).
  * 0 = automatic (by batch size), 1 = one warp per utterance with the trellis spilled to the workspace, 2 = two warps per

@@ -47,6 +47,12 @@ _PROTOS = {
     "ctcb_gemm_workspace_bytes": (c_sz, [c_int, c_int, c_int]),
     "ctcb_gemm_f32": (c_int, [c_int, c_int, c_int, c_int, c_int, c_f32, c_vp, c_i64, c_vp, c_i64, c_f32, c_vp,
                               c_i64, c_vp, c_int, c_vp, c_vp, c_sz, c_vp]),
+    "ctcb_gemm_pair_workspace_bytes": (c_sz, [c_int, c_int, c_int]),
+    "ctcb_gemm_pair_f32": (c_int, [c_int, c_int, c_int, c_int, c_int, c_f32, c_vp, c_vp, c_i64, c_vp, c_vp, c_i64,
+                                   c_f32, c_vp, c_vp, c_i64, c_vp, c_sz, c_vp]),
+    "ctcb_debug_gemm_plan": (c_int, [c_int, c_int, c_int, c_int, c_int, c_vp, c_i64, c_vp, c_i64, c_int,
+                                     ctypes.POINTER(ctypes.c_int32)]),
+    "ctcb_debug_set_gemm_copy": (c_int, [c_int]),
     "ctcb_debug_gemm_trace": (c_int, [c_vp]),
     "ctcb_debug_set_ctc_kernel": (c_int, [c_int]),
     "ctcb_brnn_param_count": (c_i64, [ctypes.POINTER(BrnnConfig)]),

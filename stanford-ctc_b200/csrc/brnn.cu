@@ -240,7 +240,10 @@ WsLayout ws_layout(const ctcb_brnn_config *c) {
         need(Rint, sizes[i], sizes[i + 1]);      // backward  delta . W
         need(sizes[i + 1], sizes[i], Rint);      // weights   delta^T . X_i
     }
-    need(H, H, Rint);                            // recurrent weight gradients
+    {                                            // recurrent weight gradients (a pair for the bi-directional layer)
+        const size_t b = ctcb_gemm_pair_workspace_bytes(H, H, Rint);
+        if (b > g) g = b;
+    }
     w.gemm = take(g);
     w.gemm2 = take(g);
     w.colsum = take(((R + CS_ROWS_MIN - 1) / CS_ROWS_MIN) * wide * sizeof(float));
@@ -509,11 +512,13 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
                 ProfScope ps("gemm_dw_rec", h->side);
                 if (Tmax > 1) {
                     const int64_t Rm = R - B;
-                    TRY(ctcb_gemm_f32(1, 0, H, H, (int)Rm, 1.f, dFor + (int64_t)B * H, H, For, H, beta_g, G(iWtf), H,
-                                      nullptr, 0, nullptr, gws2, gws2_bytes, h->side));
-                    if (!uni)
-                        TRY(ctcb_gemm_f32(1, 0, H, H, (int)Rm, 1.f, dBack, H, Back + (int64_t)B * H, H, beta_g, G(iWtb),
-                                          H, nullptr, 0, nullptr, gws2, gws2_bytes, h->side));
+                    if (uni)
+                        TRY(ctcb_gemm_f32(1, 0, H, H, (int)Rm, 1.f, dFor + (int64_t)B * H, H, For, H, beta_g, G(iWtf), H,
+                                          nullptr, 0, nullptr, gws2, gws2_bytes, h->side));
+                    else     // both directions in one launch
+                        TRY(ctcb_gemm_pair_f32(1, 0, H, H, (int)Rm, 1.f, dFor + (int64_t)B * H, dBack, H, For,
+                                               Back + (int64_t)B * H, H, beta_g, G(iWtf), G(iWtb), H, gws2, gws2_bytes,
+                                               h->side));
                 } else if (first) {     // one frame: no recurrence, nothing to add to earlier micro-batches
                     CTCB_CUDA_CHECK(cudaMemsetAsync(G(iWtf), 0, sizeof(float) * H * H, h->side));
                     if (!uni) CTCB_CUDA_CHECK(cudaMemsetAsync(G(iWtb), 0, sizeof(float) * H * H, h->side));

@@ -268,6 +268,10 @@ size_t gemm_tc_workspace_bytes(int M, int N, int K);
 int run_gemm_tc(int transA, int transB, int M, int N, int K, float alpha, const float *A, int64_t lda, const float *B,
                 int64_t ldb, float beta, float *C, int64_t ldc, const float *bias, int relu, const float *mask_src,
                 void *ws, size_t ws_bytes, cudaStream_t st);
+size_t gemm_tc_pair_workspace_bytes(int M, int N, int K);
+int run_gemm_tc_pair(int transA, int transB, int M, int N, int K, float alpha, const float *const *A, int64_t lda,
+                     const float *const *B, int64_t ldb, float beta, float *const *C, int64_t ldc, void *ws,
+                     size_t ws_bytes, cudaStream_t st);
 }
 
 using namespace ctcb;
@@ -326,4 +330,29 @@ extern "C" int ctcb_gemm_f32(int transA, int transB, int M, int N, int K, float 
         CTCB_LAUNCH_CHECK();
     }
     return CTCB_OK;
+}
+
+extern "C" size_t ctcb_gemm_pair_workspace_bytes(int M, int N, int K) {
+    const size_t one = ctcb_gemm_workspace_bytes(M, N, K);
+    const size_t tc = gemm_tc_eligible(M, N, K) ? gemm_tc_pair_workspace_bytes(M, N, K) : 0;
+    return one > tc ? one : tc;
+}
+
+extern "C" int ctcb_gemm_pair_f32(int transA, int transB, int M, int N, int K, float alpha, const float *A0,
+                                  const float *A1, int64_t lda, const float *B0, const float *B1, int64_t ldb,
+                                  float beta, float *C0, float *C1, int64_t ldc, void *workspace, size_t ws_bytes,
+                                  void *stream) {
+    if (M <= 0 || N <= 0) return CTCB_OK;
+    if (!A0 || !A1 || !B0 || !B1 || !C0 || !C1 || K < 0) return set_error(CTCB_EINVAL, "ctcb_gemm_pair_f32: bad argument");
+    if (gemm_tc_eligible(M, N, K) && workspace && ws_bytes >= gemm_tc_pair_workspace_bytes(M, N, K)) {
+        const float *A[2] = {A0, A1}, *B[2] = {B0, B1};
+        float *C[2] = {C0, C1};
+        return run_gemm_tc_pair(transA, transB, M, N, K, alpha, A, lda, B, ldb, beta, C, ldc, workspace, ws_bytes,
+                                (cudaStream_t)stream);
+    }
+    const int rc = ctcb_gemm_f32(transA, transB, M, N, K, alpha, A0, lda, B0, ldb, beta, C0, ldc, nullptr, 0, nullptr,
+                                 workspace, ws_bytes, stream);
+    if (rc != CTCB_OK) return rc;
+    return ctcb_gemm_f32(transA, transB, M, N, K, alpha, A1, lda, B1, ldb, beta, C1, ldc, nullptr, 0, nullptr,
+                         workspace, ws_bytes, stream);
 }

@@ -8,15 +8,23 @@
 // and a product is three MMAs accumulated in fp32:  lo.hi + hi.lo + hi.hi
 // (the dropped lo.lo term is ~2^-20 relative) -- "3xTF32", ~1e-6 relative error per product.
 //
-// Kernel shape: C[M x N] = A[M x K] . B[N x K]^T, both operands K-major (wgmma reads .tf32 operands K-major only; an
-// operand stored the other way round is transposed by a prep kernel first).  One CTA (3 warpgroups) per 128 x BN output
-// tile and K split (gridDim.z):
+// Kernel shape: C[M x N] = A[M x K] . B[N x K]^T.  wgmma reads .tf32 operands K-major only, so every tile reaches the
+// consumers K-major and 128-byte swizzled, however the operand is stored:
+//   K-major operand (A as [M][K], B as [N][K]): TMA writes the tile swizzled into the value slot;
+//   MN-major operand (A as [K][M], B as [K][N], e.g. the time-major activations of a weight gradient over T*B rows):
+//     TMA writes the [32 k][rows] box unswizzled into the LOW-HALF slot, and the producer transposes it into the
+//     swizzled value slot while it computes the low halves.  The wgmma then reads the same bytes as if a transposed
+//     copy had been loaded, so both ways give identical results.
+//   An operand TMA cannot describe (row pitch not a multiple of 16 bytes, base not 16-byte aligned) is re-pitched or
+//   transposed into the workspace by a prep kernel first (also forced by CTCB_GEMM_TC_COPY=1).
+// One CTA (3 warpgroups) per 128 x BN output tile, K split and problem (gridDim.z = problems x splits):
 //   warpgroup 0 : producer -- one elected thread TMA-loads the A and B tiles of each k-block of 32 floats into a
 //                 STAGES-deep ring (mbarrier complete_tx); the 128 threads then write the low halves of both tiles
-//                 next to them (element-wise, oblivious to the swizzle) and signal the consumers;
+//                 next to them (and the transposed values of an MN-major tile) and signal the consumers;
 //   warpgroups 1, 2 : consumers -- rows 0..63 / 64..127 of the tile: 4 k-steps x 3 wgmma (m64 x BN x k8) per k-block
 //                 with the accumulator in registers, one k-block in flight while the previous slot is released; then
 //                 the fused alpha/beta/bias/ReLU/mask epilogue (or the split-K partial) straight from registers.
+// Two problems of the same shape (the two recurrent weight gradients) can share one launch and one split-K reduce.
 #include "common.cuh"
 #include "wgmma.cuh"
 #include <cuda.h>
@@ -32,11 +40,12 @@ static unsigned long long *g_gemm_trace = nullptr;     // CTCB_GEMM_TRACE: stamp
 
 struct GemmTcArgs {
     int M, N, K;
-    float *C; int64_t ldc;
+    float *C[2]; int64_t ldc;    // output of problem 0 / 1 (a second problem has no bias, ReLU or mask)
     float alpha, beta;
     const float *bias; int relu; const float *mask;
-    float *partial;      // split-K partials [splits][M][N] or nullptr
-    int kb_per_split;    // k-blocks per gridDim.z slice
+    float *partial;      // split-K partials [problems][splits][M][N] (row blockIdx.z) or nullptr
+    int kb_per_split;    // k-blocks per split
+    int splits;          // K splits per problem: blockIdx.z = problem * splits + split
     unsigned long long *trace;   // optional (CTCB_GEMM_TRACE): [64 k-blocks][8] SM clock stamps of CTA (0,0,0)
 };
 #define TC_STAMP(i, slot)                                                                                       \
@@ -78,9 +87,9 @@ __device__ __forceinline__ void tc_tma_load_2d(uint32_t dst, const CUtensorMap *
                  ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1) : "memory");
 }
 
-__device__ __forceinline__ float tc_epilogue(const GemmTcArgs &g, float acc, int m, int n) {
+__device__ __forceinline__ float tc_epilogue(const GemmTcArgs &g, const float *C, float acc, int m, int n) {
     float v = g.alpha * acc;
-    if (g.beta != 0.f) v += g.beta * g.C[(int64_t)m * g.ldc + n];
+    if (g.beta != 0.f) v += g.beta * C[(int64_t)m * g.ldc + n];
     if (g.bias) v += g.bias[n];
     if (g.relu) v = fmaxf(v, 0.f);
     if (g.mask) v = (g.mask[(int64_t)m * g.ldc + n] > 0.f) ? v : 0.f;
@@ -96,10 +105,53 @@ __device__ __forceinline__ float4 tc_lo4(float4 v) {
     return r;
 }
 
-// A stage holds [A value | A low half | B value | B low half], each tile 1024-byte aligned.
-template <int BN, int STAGES>
+// The producer's share of one ROWS x 32 operand tile: ROWS * 32 / 4 / 128 float4 per thread.
+//   K-major (MN = false): the tile landed swizzled in `hi`; thread t takes float4 t, t + 128, ... in storage order and
+//     writes their low halves to the same places in `lo` (the swizzle does not matter element-wise).
+//   MN-major (MN = true): the tile landed in `lo` as [32 k][ROWS]; thread t takes row r = t % ROWS and the k-quads
+//     c = t / ROWS + (128 / ROWS) q.  Reads: a warp reads 32 consecutive rows of one k, conflict-free.  Writes: element
+//     (r, k) of a K-major 128B-swizzled tile lies at r * 128 + ((k / 4) ^ (r % 8)) * 16 + (k % 4) * 4, so each of the 8
+//     threads of a 16-byte store phase (8 consecutive r, one c) hits a different 16-byte bank group: conflict-free.
+//     Every thread must have loaded before any thread stores, since the stores overwrite `lo`.
+template <int ROWS, bool MN>
+struct TcTile {
+    static constexpr int Q = ROWS * TC_BK / 4 / 128;
+    static __device__ __forceinline__ void load(const uint8_t *hi, const uint8_t *lo, float4 (&v)[Q]) {
+        if (MN) {
+            const float *src = reinterpret_cast<const float *>(lo);
+            const int r = threadIdx.x % ROWS, c0 = threadIdx.x / ROWS;
+#pragma unroll
+            for (int q = 0; q < Q; ++q) {
+                const int k = 4 * (c0 + (128 / ROWS) * q);
+                v[q] = make_float4(src[k * ROWS + r], src[(k + 1) * ROWS + r], src[(k + 2) * ROWS + r], src[(k + 3) * ROWS + r]);
+            }
+        } else {
+#pragma unroll
+            for (int q = 0; q < Q; ++q) v[q] = reinterpret_cast<const float4 *>(hi)[threadIdx.x + 128 * q];
+        }
+    }
+    static __device__ __forceinline__ void store(uint8_t *hi, uint8_t *lo, const float4 (&v)[Q]) {
+        if (MN) {
+            const int r = threadIdx.x % ROWS, c0 = threadIdx.x / ROWS;
+#pragma unroll
+            for (int q = 0; q < Q; ++q) {
+                const int off = r * 128 + (((c0 + (128 / ROWS) * q) ^ (r & 7)) << 4);
+                *reinterpret_cast<float4 *>(hi + off) = v[q];
+                *reinterpret_cast<float4 *>(lo + off) = tc_lo4(v[q]);
+            }
+        } else {
+#pragma unroll
+            for (int q = 0; q < Q; ++q) reinterpret_cast<float4 *>(lo)[threadIdx.x + 128 * q] = tc_lo4(v[q]);
+        }
+    }
+};
+
+// A stage holds [A value | A low half | B value | B low half], each tile 1024-byte aligned.  A_MN / B_MN: the operand is
+// MN-major in global memory (its TMA box lands in the low-half slot, see TcTile).
+template <int BN, int STAGES, bool A_MN, bool B_MN>
 __global__ void __launch_bounds__(TC_THREADS, 1)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmTcArgs g) {
+gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmB0,
+               const __grid_constant__ CUtensorMap tmA1, const __grid_constant__ CUtensorMap tmB1, GemmTcArgs g) {
     constexpr uint32_t A_BYTES = TC_BM * TC_BK * 4, B_BYTES = BN * TC_BK * 4;
     constexpr uint32_t B_OFF = 2 * A_BYTES;
     constexpr uint32_t STAGE_BYTES = B_OFF + 2 * B_BYTES;
@@ -112,8 +164,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 
     const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int m0 = blockIdx.y * TC_BM, n0 = blockIdx.x * BN;
+    const int prob = blockIdx.z / g.splits;
     const int nkb_total = (g.K + TC_BK - 1) / TC_BK;
-    const int kb0 = blockIdx.z * g.kb_per_split;
+    const int kb0 = (blockIdx.z - prob * g.splits) * g.kb_per_split;
     const int kb1 = min(nkb_total, kb0 + g.kb_per_split);
     const int nkb = kb1 - kb0;
 
@@ -131,12 +184,14 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         // ---------------------------------------------------------------- producer: TMA issue runs STAGES - 1 k-blocks
         // ahead of the split.  Split first, then issue: the slot of block i is freed by the consumers once they have
         // started on block i - STAGES + 1, whose low halves this very iteration provides.
+        const CUtensorMap *tmA = prob ? &tmA1 : &tmA0, *tmB = prob ? &tmB1 : &tmB0;
         if (threadIdx.x == 0) {
-            asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
-            asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
+            asm volatile("prefetch.tensormap [%0];" ::"l"(tmA) : "memory");
+            asm volatile("prefetch.tensormap [%0];" ::"l"(tmB) : "memory");
         }
         constexpr int LA = STAGES - 1;
-        constexpr int NQ = (int)((A_BYTES + B_BYTES) / 16) / 128;
+        // an MN-major box lands in the low-half slot, a K-major one in the value slot
+        constexpr uint32_t A_DST = A_MN ? A_BYTES : 0, B_DST = B_OFF + (B_MN ? B_BYTES : 0);
         for (int i = 0; i < nkb + LA; ++i) {
             const int j = i - LA;
             if (j >= 0) {
@@ -144,21 +199,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 tc_mbar_wait(tc_smem_u32(&full[s]), (uint32_t)(use & 1));
                 if (threadIdx.x == 0) TC_STAMP(j, 1);
                 uint8_t *st = base + s * STAGE_BYTES;
-                float4 v[NQ];       // every load first, then every store
-#pragma unroll
-                for (int q = 0; q < NQ; ++q) {
-                    const int idx = threadIdx.x + 128 * q;                  // float4 index over A then B
-                    const int aq = (int)(A_BYTES / 16);
-                    v[q] = idx < aq ? reinterpret_cast<const float4 *>(st)[idx]
-                                    : reinterpret_cast<const float4 *>(st + B_OFF)[idx - aq];
-                }
-#pragma unroll
-                for (int q = 0; q < NQ; ++q) {
-                    const int idx = threadIdx.x + 128 * q;
-                    const int aq = (int)(A_BYTES / 16);
-                    if (idx < aq) reinterpret_cast<float4 *>(st + A_BYTES)[idx] = tc_lo4(v[q]);
-                    else reinterpret_cast<float4 *>(st + B_OFF + B_BYTES)[idx - aq] = tc_lo4(v[q]);
-                }
+                float4 va[TcTile<TC_BM, A_MN>::Q], vb[TcTile<BN, B_MN>::Q];    // every load first, then every store
+                TcTile<TC_BM, A_MN>::load(st, st + A_BYTES, va);
+                TcTile<BN, B_MN>::load(st + B_OFF, st + B_OFF + B_BYTES, vb);
+                if (A_MN || B_MN) asm volatile("bar.sync 1, 128;" ::: "memory");   // the producer warpgroup only
+                TcTile<TC_BM, A_MN>::store(st, st + A_BYTES, va);
+                TcTile<BN, B_MN>::store(st + B_OFF, st + B_OFF + B_BYTES, vb);
                 asm volatile("fence.proxy.async.shared::cta;" ::: "memory");    // generic writes -> tensor-core (async) proxy
                 __syncwarp();
                 if (lane == 0) tc_mbar_arrive(tc_smem_u32(&ready[s]));
@@ -172,8 +218,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 const int k = (kb0 + i) * TC_BK;
                 TC_STAMP(i, 0);
                 tc_mbar_expect_tx(fb, A_BYTES + B_BYTES);
-                tc_tma_load_2d(sa, &tmA, fb, k, m0);
-                tc_tma_load_2d(sa + B_OFF, &tmB, fb, k, n0);
+                // coordinates innermost first: (k, row) for a K-major map, (row, k) for an MN-major one
+                tc_tma_load_2d(sa + A_DST, tmA, fb, A_MN ? m0 : k, A_MN ? k : m0);
+                tc_tma_load_2d(sa + B_DST, tmB, fb, B_MN ? n0 : k, B_MN ? k : n0);
             }
         }
         return;
@@ -213,19 +260,20 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 
     // -------------------------------------------------------------------- epilogue straight from the accumulator
     const int q = warp & 3;
+    float *const Cp = prob ? g.C[1] : g.C[0];     // (a select: indexing the parameter array would copy it to the stack)
     const int rbase = m0 + 64 * cw + 16 * q + (lane >> 2);
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
         const int m = rbase + 8 * h;
         if (m >= g.M) continue;
-        float *drow = g.partial ? g.partial + ((int64_t)blockIdx.z * g.M + m) * g.N : g.C + (int64_t)m * g.ldc;
+        float *drow = g.partial ? g.partial + ((int64_t)blockIdx.z * g.M + m) * g.N : Cp + (int64_t)m * g.ldc;
 #pragma unroll
         for (int j = 0; j < BN / 8; ++j) {
             const int n = n0 + 8 * j + 2 * (lane & 3);
             float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
             if (!g.partial) {
-                if (n < g.N) v0 = tc_epilogue(g, v0, m, n);
-                if (n + 1 < g.N) v1 = tc_epilogue(g, v1, m, n + 1);
+                if (n < g.N) v0 = tc_epilogue(g, Cp, v0, m, n);
+                if (n + 1 < g.N) v1 = tc_epilogue(g, Cp, v1, m, n + 1);
             }
             if (n + 1 < g.N && (((uintptr_t)(drow + n)) & 7) == 0) {
                 *reinterpret_cast<float2 *>(drow + n) = make_float2(v0, v1);
@@ -271,13 +319,18 @@ __global__ void tc_split_transpose_kernel(const float *__restrict__ x, int64_t l
     }
 }
 
-__global__ void tc_splitk_reduce_kernel(GemmTcArgs g, int splits) {
+// sums the splits of every problem in split order, so a problem's result does not depend on the launch it shared
+__global__ void tc_splitk_reduce_kernel(GemmTcArgs g, int problems) {
     const int64_t total = (int64_t)g.M * g.N;
-    for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
+    for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < problems * total; idx += (int64_t)gridDim.x * blockDim.x) {
+        const int p = (int)(idx / total);
+        const int64_t e = idx - p * total;
+        const float *part = g.partial + (int64_t)p * g.splits * total + e;
         float s = 0.f;
-        for (int z = 0; z < splits; ++z) s += g.partial[(int64_t)z * total + idx];
-        const int m = (int)(idx / g.N), n = (int)(idx % g.N);
-        g.C[(int64_t)m * g.ldc + n] = tc_epilogue(g, s, m, n);
+        for (int z = 0; z < g.splits; ++z) s += part[(int64_t)z * total];
+        const int m = (int)(e / g.N), n = (int)(e % g.N);
+        float *const C = p ? g.C[1] : g.C[0];
+        C[(int64_t)m * g.ldc + n] = tc_epilogue(g, C, s, m, n);
     }
 }
 
@@ -302,17 +355,25 @@ static EncodeTiledFn get_encode() {
     return fn;
 }
 
-// rows x K fp32, K-major with pitch ld (elements); box = 32 floats x box_rows, 128B swizzle, OOB -> 0
-static int make_map(CUtensorMap *m, const float *ptr, int rows, int K, int64_t ld, int box_rows) {
+// fp32 2-D tensor map with pitch ld (elements).  K-major (mn = 0): rows x K, box = 32 floats x box_rows, 128B swizzle
+// (the layout the wgmma descriptors read).  MN-major (mn = 1): K x rows, box = box_rows floats x 32, no swizzle (the
+// producer transposes it).  Out-of-bounds elements read as 0 either way.
+static int make_map(CUtensorMap *m, const float *ptr, int rows, int K, int64_t ld, int box_rows, bool mn) {
     EncodeTiledFn enc = get_encode();
     if (!enc) return set_error(CTCB_ECUDA, "cuTensorMapEncodeTiled is not available from this driver");
     cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)rows};
     cuuint64_t strides[1] = {(cuuint64_t)ld * sizeof(float)};
     cuuint32_t box[2] = {(cuuint32_t)TC_BK, (cuuint32_t)box_rows};
     cuuint32_t estr[2] = {1, 1};
+    if (mn) {
+        dims[0] = (cuuint64_t)rows; dims[1] = (cuuint64_t)K;
+        box[0] = (cuuint32_t)box_rows; box[1] = (cuuint32_t)TC_BK;
+    }
     CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void *)ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return set_error(CTCB_ECUDA, "cuTensorMapEncodeTiled failed (%d) rows=%d K=%d ld=%lld", (int)r, rows, K, (long long)ld);
+                     mn ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS)
+        return set_error(CTCB_ECUDA, "cuTensorMapEncodeTiled failed (%d) rows=%d K=%d ld=%lld mn=%d", (int)r, rows, K, (long long)ld, (int)mn);
     return CTCB_OK;
 }
 
@@ -327,9 +388,10 @@ static int tc_pick_bn(int N) { return N <= 64 ? 64 : 128; }
 // round-to-nearest by the reduce kernel (deterministic order).
 constexpr int TC_CHAIN_KB = 64;
 
-static int tc_choose_splits(int M, int N, int K, int BN) {
-    const int tiles = ((M + TC_BM - 1) / TC_BM) * ((N + BN - 1) / BN);
-    const int nkb = (K + TC_BK - 1) / TC_BK;
+// Splits of one problem of `tiles` output tiles over nkb k-blocks: enough CTAs to cover the SMs, at least 8 k-blocks per
+// split, at most 32 splits, and never a chain longer than TC_CHAIN_KB.  A pair of problems keeps the split of one, so
+// that each result is bit-identical to its single call (filling whole waves instead would change the summation order).
+static int tc_choose_splits(int tiles, int nkb) {
     const int sms = num_sms();
     int splits = 1;
     if (tiles < sms && nkb >= 16) {          // fill the device
@@ -353,8 +415,8 @@ bool gemm_tc_enabled() {
     return on == 1;
 }
 
-// Below these sizes the exact FFMA kernel is used: short contractions (K = 41 / 62) would need re-pitched copies and
-// cannot amortise the tensor-core pipeline.  The thresholds have not been re-tuned on H100.
+// Below these sizes the exact FFMA kernel is used: short contractions (K = 41 / 62) cannot amortise the tensor-core
+// pipeline.  The thresholds have not been re-tuned on H100.
 bool gemm_tc_eligible(int M, int N, int K) {
     static int min_k = -1, min_m = -1;      // CTCB_GEMM_MINK / _MINM: smallest contraction length / row count that goes to the tensor cores
     if (min_k < 0) { const char *e = getenv("CTCB_GEMM_MINK"); min_k = e ? atoi(e) : 128; }
@@ -362,70 +424,100 @@ bool gemm_tc_eligible(int M, int N, int K) {
     return gemm_tc_enabled() && M >= min_m && N >= 32 && K >= min_k;
 }
 
-size_t gemm_tc_workspace_bytes(int M, int N, int K) {
-    const int64_t Kp = pad4(K);
-    size_t prep = ((size_t)M * Kp + (size_t)N * Kp) * sizeof(float);     // re-laid-out copies of A and B (when needed)
-    const int BN = tc_pick_bn(N);
-    const int splits = tc_choose_splits(M, N, K, BN);
-    size_t part = splits > 1 ? (size_t)splits * M * N * sizeof(float) : 0;
-    return align_up(prep, 256) + align_up(part, 256) + 1024;
+// How an operand reaches the ring.
+enum { TC_PATH_KMAJOR = 0,     // TMA reads the caller's K-major array
+       TC_PATH_MN = 1,         // TMA reads the caller's MN-major array, the producer transposes in shared memory
+       TC_PATH_COPY = 2 };     // a prep kernel re-pitches or transposes it into the workspace first
+
+// CTCB_GEMM_TC_COPY=1 (or ctcb_debug_set_gemm_copy(1)): MN-major operands go through a transposed copy in the
+// workspace instead of the in-ring transpose; same results at the same split, for comparison and timing
+static int g_copy_forced = -1;
+static bool tc_copy_forced() {
+    if (g_copy_forced < 0) { const char *e = getenv("CTCB_GEMM_TC_COPY"); g_copy_forced = (e && atoi(e) != 0) ? 1 : 0; }
+    return g_copy_forced == 1;
 }
 
-template <int BN, int STAGES>
-static int launch_tc(const CUtensorMap &tA, const CUtensorMap &tB, const GemmTcArgs &g, int splits, cudaStream_t st) {
+// TMA needs a 16-byte aligned base and a row pitch that is a multiple of 16 bytes
+static int tc_operand_path(bool mn_major, const float *p, int64_t ld) {
+    if (ld % 4 != 0 || ((uintptr_t)p) % 16 != 0) return TC_PATH_COPY;
+    if (mn_major) return tc_copy_forced() ? TC_PATH_COPY : TC_PATH_MN;
+    return TC_PATH_KMAJOR;
+}
+
+struct GemmTcPlan {
+    int BN, stages, splits, kb_per_split, ctas, a_path, b_path, problems;
+};
+
+// The one place that decides how a tensor-core contraction runs: the launcher (run_gemm_tc, run_gemm_tc_pair) and
+// ctcb_debug_gemm_plan both call it.  problems = 2 asks for a pair in one launch; a pair with an operand that needs a
+// copy runs as two single launches (problems = 1 in the plan).
+static void gemm_tc_plan(int transA, int transB, int M, int N, int K, const float *A, int64_t lda, const float *B,
+                         int64_t ldb, int problems, GemmTcPlan *p) {
+    p->BN = tc_pick_bn(N);
+    p->stages = p->BN == 64 ? 4 : 3;     // 192 KB of ring either way: 4 stages of 48 KB (64-wide) or 3 of 64 KB
+    p->a_path = tc_operand_path(transA != 0, A, lda);
+    p->b_path = tc_operand_path(transB == 0, B, ldb);
+    p->problems = (problems == 2 && p->a_path != TC_PATH_COPY && p->b_path != TC_PATH_COPY) ? 2 : 1;
+    const int tiles = ((M + TC_BM - 1) / TC_BM) * ((N + p->BN - 1) / p->BN);
+    const int nkb = (K + TC_BK - 1) / TC_BK;
+    const int splits = tc_choose_splits(tiles, nkb);
+    p->kb_per_split = (nkb + splits - 1) / splits;
+    p->splits = (nkb + p->kb_per_split - 1) / p->kb_per_split;
+    p->ctas = p->problems * tiles * p->splits;
+}
+
+static size_t tc_partial_bytes(int M, int N, int splits, int problems) {
+    return splits > 1 ? (size_t)problems * splits * M * N * sizeof(float) : 0;
+}
+
+// Worst case over operand layouts: room for copies of both operands and the partials of a single launch.
+size_t gemm_tc_workspace_bytes(int M, int N, int K) {
+    const int64_t Kp = pad4(K);
+    size_t prep = ((size_t)M * Kp + (size_t)N * Kp) * sizeof(float);
+    GemmTcPlan p;
+    gemm_tc_plan(0, 1, M, N, K, nullptr, 0, nullptr, 0, 1, &p);
+    return align_up(prep, 256) + align_up(tc_partial_bytes(M, N, p.splits, 1), 256) + 1024;
+}
+
+// A pair either shares a launch without copies (partials of both problems) or runs as two single launches.
+size_t gemm_tc_pair_workspace_bytes(int M, int N, int K) {
+    GemmTcPlan p;
+    gemm_tc_plan(0, 1, M, N, K, nullptr, 0, nullptr, 0, 2, &p);
+    const size_t pair = align_up(tc_partial_bytes(M, N, p.splits, 2), 256) + 1024;
+    const size_t single = gemm_tc_workspace_bytes(M, N, K);
+    return pair > single ? pair : single;
+}
+
+template <int BN, int STAGES, bool A_MN, bool B_MN>
+static int launch_tc(const CUtensorMap *tA, const CUtensorMap *tB, const GemmTcArgs &g, int ctas_z, cudaStream_t st) {
     constexpr size_t smem = (size_t)STAGES * (2 * TC_BM * TC_BK * 4 + 2 * BN * TC_BK * 4) + 3 * STAGES * 8 + 1024;
     static_assert(smem <= 227 * 1024, "stage ring exceeds the shared memory of a block");
-    CTCB_CUDA_CHECK(cudaFuncSetAttribute((gemm_tc_kernel<BN, STAGES>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    dim3 grid((g.N + BN - 1) / BN, (g.M + TC_BM - 1) / TC_BM, splits);
-    gemm_tc_kernel<BN, STAGES><<<grid, TC_THREADS, smem, st>>>(tA, tB, g);
+    CTCB_CUDA_CHECK(cudaFuncSetAttribute((gemm_tc_kernel<BN, STAGES, A_MN, B_MN>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    dim3 grid((g.N + BN - 1) / BN, (g.M + TC_BM - 1) / TC_BM, ctas_z);
+    gemm_tc_kernel<BN, STAGES, A_MN, B_MN><<<grid, TC_THREADS, smem, st>>>(tA[0], tB[0], tA[1], tB[1], g);
     CTCB_LAUNCH_CHECK();
     return CTCB_OK;
 }
 
-// Same contract as ctcb_gemm_f32; ws must hold gemm_tc_workspace_bytes(M, N, K).
-int run_gemm_tc(int transA, int transB, int M, int N, int K, float alpha, const float *A, int64_t lda, const float *B,
-                int64_t ldb, float beta, float *C, int64_t ldc, const float *bias, int relu, const float *mask_src,
-                void *ws, size_t ws_bytes, cudaStream_t st) {
-    if (ws_bytes < gemm_tc_workspace_bytes(M, N, K)) return set_error(CTCB_ENOMEM, "run_gemm_tc: workspace too small");
-    const int64_t Kp = pad4(K);
-    float *p = (float *)ws;
-    float *Ahi = p; p += (size_t)M * Kp;
-    float *Bhi = p; p += (size_t)N * Kp;
-    float *part = (float *)((char *)ws + align_up(((size_t)M * Kp + (size_t)N * Kp) * sizeof(float), 256));
+template <int BN, int STAGES>
+static int launch_tc_paths(const GemmTcPlan &p, const CUtensorMap *tA, const CUtensorMap *tB, const GemmTcArgs &g,
+                           cudaStream_t st) {
+    const int z = p.problems * p.splits;
+    const bool am = p.a_path == TC_PATH_MN, bm = p.b_path == TC_PATH_MN;
+    if (am && bm) return launch_tc<BN, STAGES, true, true>(tA, tB, g, z, st);
+    if (am) return launch_tc<BN, STAGES, true, false>(tA, tB, g, z, st);
+    if (bm) return launch_tc<BN, STAGES, false, true>(tA, tB, g, z, st);
+    return launch_tc<BN, STAGES, false, false>(tA, tB, g, z, st);
+}
 
-    // ---- operand A as M x K, K-major: stored M x K (transA=0) or K x M (transA=1, transposed into a copy)
-    const float *Ause; int64_t lda_use;
-    auto ew_grid = [](int64_t n) { int64_t b = (n + 255) / 256; const int cap = 16 * num_sms(); return (int)(b > cap ? cap : (b < 1 ? 1 : b)); };
-    if (transA) {
-        tc_split_transpose_kernel<<<dim3((M + 31) / 32, (K + 31) / 32), dim3(32, 8), 0, st>>>(A, lda, K, M, Ahi, nullptr, Kp);
-        CTCB_LAUNCH_CHECK();
-        Ause = Ahi; lda_use = Kp;
-    } else if ((lda % 4 == 0) && (((uintptr_t)A) % 16 == 0)) {
-        Ause = A; lda_use = lda;                       // TMA reads the caller's array directly
-    } else {
-        tc_split_kernel<<<ew_grid((int64_t)M * Kp), 256, 0, st>>>(A, lda, M, K, Ahi, nullptr, Kp);   // re-pitch to 16-byte rows
-        CTCB_LAUNCH_CHECK();
-        Ause = Ahi; lda_use = Kp;
-    }
-    // ---- operand B as N x K, K-major: stored N x K (transB=1) or K x N (transB=0, transposed into a copy)
-    const float *Buse; int64_t ldb_use;
-    if (!transB) {
-        tc_split_transpose_kernel<<<dim3((N + 31) / 32, (K + 31) / 32), dim3(32, 8), 0, st>>>(B, ldb, K, N, Bhi, nullptr, Kp);
-        CTCB_LAUNCH_CHECK();
-        Buse = Bhi; ldb_use = Kp;
-    } else if ((ldb % 4 == 0) && (((uintptr_t)B) % 16 == 0)) {
-        Buse = B; ldb_use = ldb;
-    } else {
-        tc_split_kernel<<<ew_grid((int64_t)N * Kp), 256, 0, st>>>(B, ldb, N, K, Bhi, nullptr, Kp);
-        CTCB_LAUNCH_CHECK();
-        Buse = Bhi; ldb_use = Kp;
-    }
-
-    const int BN = tc_pick_bn(N);
-    int splits = tc_choose_splits(M, N, K, BN);
-    const int nkb = (K + TC_BK - 1) / TC_BK;
+// One launch (and, with splits, one reduce) of p.problems problems that share shape, pitches, alpha and beta.
+// A/B/C: per problem; operands whose path is TC_PATH_COPY must already have been replaced by their copies.
+static int run_tc_plan(const GemmTcPlan &p, int M, int N, int K, float alpha, const float *const *A, int64_t lda,
+                       const float *const *B, int64_t ldb, float beta, float *const *C, int64_t ldc, const float *bias,
+                       int relu, const float *mask_src, float *part, cudaStream_t st) {
     GemmTcArgs g;
-    g.M = M; g.N = N; g.K = K; g.C = C; g.ldc = ldc; g.alpha = alpha; g.beta = beta; g.bias = bias; g.relu = relu; g.mask = mask_src;
+    g.M = M; g.N = N; g.K = K; g.ldc = ldc; g.alpha = alpha; g.beta = beta; g.bias = bias; g.relu = relu; g.mask = mask_src;
+    g.C[0] = C[0]; g.C[1] = p.problems > 1 ? C[1] : C[0];
     g.trace = nullptr;
     {
         static int tr_env = -1;
@@ -435,28 +527,100 @@ int run_gemm_tc(int transA, int transB, int M, int N, int K, float alpha, const 
             g.trace = g_gemm_trace;
         }
     }
-    g.kb_per_split = (nkb + splits - 1) / splits;
-    splits = (nkb + g.kb_per_split - 1) / g.kb_per_split;
-    g.partial = splits > 1 ? part : nullptr;
+    g.kb_per_split = p.kb_per_split;
+    g.splits = p.splits;
+    g.partial = p.splits > 1 ? part : nullptr;
 
-    CUtensorMap tA, tB;
+    CUtensorMap tA[2], tB[2];
     int rc;
-    if ((rc = make_map(&tA, Ause, M, K, lda_use, TC_BM)) != CTCB_OK) return rc;
-    if ((rc = make_map(&tB, Buse, N, K, ldb_use, BN)) != CTCB_OK) return rc;
-    // 192 KB of ring either way: 4 stages of 48 KB (64-wide) or 3 of 64 KB (128-wide)
-    rc = (BN == 64) ? launch_tc<64, 4>(tA, tB, g, splits, st) : launch_tc<128, 3>(tA, tB, g, splits, st);
+    for (int q = 0; q < p.problems; ++q) {
+        if ((rc = make_map(&tA[q], A[q], M, K, lda, TC_BM, p.a_path == TC_PATH_MN)) != CTCB_OK) return rc;
+        if ((rc = make_map(&tB[q], B[q], N, K, ldb, p.BN, p.b_path == TC_PATH_MN)) != CTCB_OK) return rc;
+    }
+    if (p.problems == 1) { tA[1] = tA[0]; tB[1] = tB[0]; }
+    rc = (p.BN == 64) ? launch_tc_paths<64, 4>(p, tA, tB, g, st) : launch_tc_paths<128, 3>(p, tA, tB, g, st);
     if (rc != CTCB_OK) return rc;
-    if (splits > 1) {
-        const int64_t total = (int64_t)M * N;
+    if (p.splits > 1) {
+        const int64_t total = (int64_t)p.problems * M * N;
         int blocks = (int)((total + 255) / 256);
         if (blocks > 4 * num_sms()) blocks = 4 * num_sms();
-        tc_splitk_reduce_kernel<<<blocks, 256, 0, st>>>(g, splits);
+        tc_splitk_reduce_kernel<<<blocks, 256, 0, st>>>(g, p.problems);
         CTCB_LAUNCH_CHECK();
     }
     return CTCB_OK;
 }
 
+// Same contract as ctcb_gemm_f32; ws must hold gemm_tc_workspace_bytes(M, N, K).
+int run_gemm_tc(int transA, int transB, int M, int N, int K, float alpha, const float *A, int64_t lda, const float *B,
+                int64_t ldb, float beta, float *C, int64_t ldc, const float *bias, int relu, const float *mask_src,
+                void *ws, size_t ws_bytes, cudaStream_t st) {
+    if (ws_bytes < gemm_tc_workspace_bytes(M, N, K)) return set_error(CTCB_ENOMEM, "run_gemm_tc: workspace too small");
+    GemmTcPlan p;
+    gemm_tc_plan(transA, transB, M, N, K, A, lda, B, ldb, 1, &p);
+    const int64_t Kp = pad4(K);
+    float *prep = (float *)ws;
+    size_t prep_bytes = 0;
+    auto ew_grid = [](int64_t n) { int64_t b = (n + 255) / 256; const int cap = 16 * num_sms(); return (int)(b > cap ? cap : (b < 1 ? 1 : b)); };
+    // an operand that TMA cannot read in place becomes rows x Kp, K-major, in the workspace
+    auto copy = [&](const float *X, int64_t ld, int rows, bool mn_major, const float **use, int64_t *ld_use) -> int {
+        float *dst = prep + prep_bytes / sizeof(float);
+        if (mn_major)
+            tc_split_transpose_kernel<<<dim3((rows + 31) / 32, (K + 31) / 32), dim3(32, 8), 0, st>>>(X, ld, K, rows, dst, nullptr, Kp);
+        else
+            tc_split_kernel<<<ew_grid((int64_t)rows * Kp), 256, 0, st>>>(X, ld, rows, K, dst, nullptr, Kp);
+        CTCB_LAUNCH_CHECK();
+        prep_bytes += (size_t)rows * Kp * sizeof(float);
+        *use = dst; *ld_use = Kp;
+        return CTCB_OK;
+    };
+    const float *Ause = A, *Buse = B;
+    int64_t lda_use = lda, ldb_use = ldb;
+    int rc;
+    if (p.a_path == TC_PATH_COPY && (rc = copy(A, lda, M, transA != 0, &Ause, &lda_use)) != CTCB_OK) return rc;
+    if (p.b_path == TC_PATH_COPY && (rc = copy(B, ldb, N, transB == 0, &Buse, &ldb_use)) != CTCB_OK) return rc;
+    float *part = (float *)((char *)ws + align_up(prep_bytes, 256));
+    return run_tc_plan(p, M, N, K, alpha, &Ause, lda_use, &Buse, ldb_use, beta, &C, ldc, bias, relu, mask_src, part, st);
+}
+
+// Two contractions of one shape in one launch: C_q = alpha op(A_q) op(B_q) + beta C_q, q = 0, 1.  Falls back to two
+// run_gemm_tc calls when an operand needs a copy.  ws must hold gemm_tc_pair_workspace_bytes(M, N, K).
+int run_gemm_tc_pair(int transA, int transB, int M, int N, int K, float alpha, const float *const *A, int64_t lda,
+                     const float *const *B, int64_t ldb, float beta, float *const *C, int64_t ldc, void *ws,
+                     size_t ws_bytes, cudaStream_t st) {
+    if (ws_bytes < gemm_tc_pair_workspace_bytes(M, N, K)) return set_error(CTCB_ENOMEM, "run_gemm_tc_pair: workspace too small");
+    GemmTcPlan p, p1;
+    gemm_tc_plan(transA, transB, M, N, K, A[0], lda, B[0], ldb, 2, &p);
+    gemm_tc_plan(transA, transB, M, N, K, A[1], lda, B[1], ldb, 2, &p1);
+    if (p.problems == 2 && p1.problems == 2)
+        return run_tc_plan(p, M, N, K, alpha, A, lda, B, ldb, beta, C, ldc, nullptr, 0, nullptr, (float *)ws, st);
+    for (int q = 0; q < 2; ++q) {
+        const int rc = run_gemm_tc(transA, transB, M, N, K, alpha, A[q], lda, B[q], ldb, beta, C[q], ldc, nullptr, 0,
+                                   nullptr, ws, ws_bytes, st);
+        if (rc != CTCB_OK) return rc;
+    }
+    return CTCB_OK;
+}
+
 }  // namespace ctcb
+
+// The plan a contraction runs on (include/ctcb200.h); A and B are only inspected for their alignment.
+extern "C" int ctcb_debug_gemm_plan(int transA, int transB, int M, int N, int K, const float *A, int64_t lda,
+                                    const float *B, int64_t ldb, int problems, int32_t *out) {
+    if (!out) return ctcb::set_error(CTCB_EINVAL, "ctcb_debug_gemm_plan: null output");
+    if (problems != 1 && problems != 2) return ctcb::set_error(CTCB_EINVAL, "ctcb_debug_gemm_plan: problems must be 1 or 2");
+    for (int i = 0; i < 8; ++i) out[i] = 0;
+    if (M <= 0 || N <= 0 || !ctcb::gemm_tc_eligible(M, N, K)) { out[7] = 1; return CTCB_OK; }     // FFMA kernel
+    ctcb::GemmTcPlan p;
+    ctcb::gemm_tc_plan(transA, transB, M, N, K, A, lda, B, ldb, problems, &p);
+    const int32_t v[8] = {1, p.BN, p.stages, p.splits, p.ctas, p.a_path, p.b_path, p.problems};
+    for (int i = 0; i < 8; ++i) out[i] = v[i];
+    return CTCB_OK;
+}
+
+extern "C" int ctcb_debug_set_gemm_copy(int on) {
+    ctcb::g_copy_forced = on ? 1 : 0;
+    return CTCB_OK;
+}
 
 // Diagnostic: the per-k-block clock stamps of CTA (0,0,0) of the last tensor-core GEMM (CTCB_GEMM_TRACE=1):
 // [64][8] = {TMA issued, tile landed, lo written, consumers saw it, MMAs issued}.  Returns 0 when tracing is off.
