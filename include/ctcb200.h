@@ -155,9 +155,18 @@ size_t ctcb_brnn_workspace_bytes(const ctcb_brnn_config *cfg);
  * inter-CTA wait timed out (results are then invalid; never a hang).  Callers that synchronise anyway
  * (e.g. for the per-step log line) should read it. */
 size_t ctcb_brnn_error_flag_offset(const ctcb_brnn_config *cfg);
+/* Workspace of a forward-only call (grads == NULL): two ping-pong activation slabs, For and Back (For only when
+ * unidirectional, neither without a temporal layer), the split-K area of the forward contractions, the sweep
+ * scratch and counters -- no CTC, delta or weight-gradient buffers.  *error_flag_offset (may be NULL) receives the
+ * byte offset of the sweep error flag inside it (same meaning as ctcb_brnn_error_flag_offset).  0 for an invalid
+ * config.  A forward-only call always uses this layout, in any workspace of at least this size (the training size
+ * included), and launches the same kernels with the same plans as a training call of the same B and Tmax, so its
+ * probs_out is bit-identical to that call's. */
+size_t ctcb_brnn_forward_workspace_bytes(const ctcb_brnn_config *cfg, size_t *error_flag_offset);
 
 /* Diagnostic hook (used by the parity tests): byte offset inside the workspace of the activations the LAST
- * ctcb_brnn_cost_and_grad call left behind, time-major [Tmax][B][*width] with that call's B and Tmax.
+ * ctcb_brnn_cost_and_grad TRAINING call (grads != NULL) left behind, time-major [Tmax][B][*width] with that call's
+ * B and Tmax; a forward-only call lays its buffers out differently (ctcb_brnn_forward_workspace_bytes).
  * what = 0: output of affine map `layer` (1..numLayers+1; For+Back at the temporal layer, logits at the last),
  * what = 1 / 2: For / Back of the temporal layer (brnnet.py:143-153). */
 int ctcb_brnn_activation_offset(const ctcb_brnn_config *cfg, int what, int layer, size_t *offset, int32_t *width);
@@ -170,7 +179,7 @@ void ctcb_brnn_destroy(ctcb_brnn *h);
  * params    : flat parameter vector; grads: same layout, overwritten
  * cost_out  : float32[B] per-utterance nll (L2 term is returned separately in *regcost_out, device float)
  * probs_out : optional [Tmax][B][outputDim] softmax output (forward-only mode when grads==NULL,
- *             brnnet.py:171-173)
+ *             brnnet.py:171-173; that mode needs only ctcb_brnn_forward_workspace_bytes of workspace)
  * stats_out : optional device float[4] = {number of non-skipped utterances, sum of their nll,
  *             number skipped, sweep error flag (see ctcb_brnn_error_flag_offset)}.  Callers place it directly behind the flat gradient so that the
  *             data-parallel all-reduce of the gradient carries it along.

@@ -61,6 +61,7 @@ _PROTOS = {
                                       ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int32)]),
     "ctcb_brnn_workspace_bytes": (c_sz, [ctypes.POINTER(BrnnConfig)]),
     "ctcb_brnn_error_flag_offset": (c_sz, [ctypes.POINTER(BrnnConfig)]),
+    "ctcb_brnn_forward_workspace_bytes": (c_sz, [ctypes.POINTER(BrnnConfig), ctypes.POINTER(c_sz)]),
     "ctcb_brnn_activation_offset": (c_int, [ctypes.POINTER(BrnnConfig), c_int, c_int, ctypes.POINTER(c_sz),
                                             ctypes.POINTER(ctypes.c_int32)]),
     "ctcb_brnn_create": (c_int, [ctypes.POINTER(BrnnConfig), ctypes.POINTER(c_vp)]),

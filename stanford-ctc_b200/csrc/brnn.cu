@@ -125,6 +125,16 @@ __global__ void batch_stats_kernel(const float *__restrict__ cost, const int32_t
 
 using namespace ctcb;
 
+namespace {
+// The buffers of a forward-only call: affine map i writes slab i % 2 and reads the other one (or For, the output of
+// the uni-directional temporal layer), so two slabs of the wider of H and K carry the whole stack.
+struct FwdLayout {
+    size_t slab[2];
+    size_t For, Back, gemm, gemm_bytes, counters, sweep, sweep_bytes;
+    size_t total;
+};
+}  // namespace
+
 struct ctcb_brnn {
     ctcb_brnn_config cfg;
     int nlayers;        // N + 1 affine maps
@@ -142,6 +152,9 @@ struct ctcb_brnn {
     // data-parallel exchange inside the step (ctcb_brnn_set_comm): the gradients of the layers at and above the temporal
     // layer are summed over ranks on the side stream WHILE the BPTT sweep runs, the rest (+ statistics tail) at the end
     ctcb_comm *comm;
+    // the forward layout, computed on the first forward-only call (its GEMM area takes a few hundred size queries)
+    bool fwd_ready;
+    FwdLayout fwd;
 };
 
 static int valid_cfg(const ctcb_brnn_config *c) {
@@ -255,11 +268,64 @@ WsLayout ws_layout(const ctcb_brnn_config *c) {
     w.total = off;
     return w;
 }
+
+// Rows per output tile of both contraction kernels (BM of gemm_simt.cu, TC_BM of gemm_tc.cu): their workspace needs
+// change with the row count only at multiples of it.
+constexpr int GEMM_ROW_TILE = 128;
+
+FwdLayout fwd_layout(const ctcb_brnn_config *c) {
+    FwdLayout f{};
+    int sizes[66];
+    layer_sizes(c, sizes);
+    const size_t R = (size_t)c->maxT * c->maxB;
+    const int N = c->numLayers, H = c->layerSize, K = c->outputDim;
+    const size_t wide = (size_t)(H > K ? H : K);
+    size_t off = 0;
+    auto take = [&](size_t bytes) { size_t o = off; off = align_up(off + bytes, 256); return o; };
+    f.slab[0] = take(R * wide * sizeof(float));
+    f.slab[1] = take(R * wide * sizeof(float));
+    if (eff_tl(c)) {
+        f.For = take(R * H * sizeof(float));
+        if (!c->unidirectional) f.Back = take(R * H * sizeof(float));
+    }
+    // ctcb_gemm_f32 takes a smaller plan when its area is short of ctcb_gemm_workspace_bytes(R, ..), and that need is
+    // not monotone in R = Tmax*B: below one wave of output tiles the tensor-core plan adds split-K partials.  So that a
+    // forward contraction takes, at every R <= maxT*maxB, the plan it takes in the training layout, the area is the
+    // largest forward need over all such R, capped at the training area (a contraction that falls back there must
+    // fall back here too).  The need changes with R only at multiples of the row tile and grows with R once
+    // num_sms() row tiles are exceeded (the split counts are then fixed), so those multiples and R itself bound it.
+    size_t g = 0;
+    const int Rint = (int)((R > 0x7fffffff) ? 0x7fffffff : R);
+    const int Mtop = (Rint < GEMM_ROW_TILE * num_sms()) ? Rint : GEMM_ROW_TILE * num_sms();
+    for (int i = 0; i <= N; ++i) {
+        for (int M = GEMM_ROW_TILE; ; M += GEMM_ROW_TILE) {
+            const size_t b = ctcb_gemm_workspace_bytes(M <= Mtop ? M : Rint, sizes[i + 1], sizes[i]);
+            if (b > g) g = b;
+            if (M > Mtop) break;
+        }
+    }
+    const WsLayout w = ws_layout(c);
+    const size_t train_area = w.gemm2 - w.gemm;
+    f.gemm = take(g < train_area ? g : train_area);
+    f.gemm_bytes = off - f.gemm;
+    f.counters = take(sizeof(unsigned int) * 1024);
+    f.sweep_bytes = eff_tl(c) ? sweep_tc_workspace_bytes(H, c->maxB) : 0;     // as in ws_layout: same sweep plan
+    f.sweep = take(f.sweep_bytes);
+    f.total = off;
+    return f;
+}
 }  // namespace
 
 extern "C" size_t ctcb_brnn_workspace_bytes(const ctcb_brnn_config *cfg) {
     if (!valid_cfg(cfg)) return 0;
     return ws_layout(cfg).total;
+}
+
+extern "C" size_t ctcb_brnn_forward_workspace_bytes(const ctcb_brnn_config *cfg, size_t *error_flag_offset) {
+    if (!valid_cfg(cfg)) return 0;
+    const FwdLayout f = fwd_layout(cfg);
+    if (error_flag_offset) *error_flag_offset = f.counters;
+    return f.total;
 }
 
 extern "C" size_t ctcb_brnn_error_flag_offset(const ctcb_brnn_config *cfg) {
@@ -283,6 +349,7 @@ extern "C" int ctcb_brnn_create(const ctcb_brnn_config *cfg, ctcb_brnn **out) {
     h->side_ready = false;
     h->defer_l2 = false;
     h->comm = nullptr;
+    h->fwd_ready = false;
     *out = h;
     return CTCB_OK;
 }
@@ -347,6 +414,63 @@ static int brnn_reduce_rest(ctcb_brnn *h, float *grads, float *stats, bool early
     return comm_allreduce_ranges(h->comm, ptrs, cnt, k, st);
 }
 
+// Where the forward half reads and writes: X[i] (1..N+1) the output of affine map i (pre-activation, then For+Back,
+// at the temporal layer; the logits at N+1), the two sweep outputs, the split-K area, the sweep counters and scratch.
+struct FwdBufs {
+    float *X[66];
+    float *For, *Back;
+    void *gemm;
+    size_t gemm_bytes;
+    unsigned int *counters;
+    void *sweep;
+    size_t sweep_bytes;
+};
+
+// brnnet.py:136-173: the affine maps with bias(+ReLU) fused, the two-direction sweep and For+Back at the temporal
+// layer, the softmax into probs_out when given.  Clears the sweep error flag first.
+static int brnn_forward(ctcb_brnn *h, const float *feats, const int32_t *T_per_utt, int B, int Tmax,
+                        const float *params, float *probs_out, const FwdBufs &m, cudaStream_t st) {
+    const ctcb_brnn_config &c = h->cfg;
+    const int N = c.numLayers, H = c.layerSize, K = c.outputDim, tl = h->tl;
+    const int *sz = h->sizes;
+    const int64_t R = (int64_t)Tmax * B;
+    auto P = [&](int idx) -> const float * {
+        int64_t off; ctcb_brnn_tensor_info(&c, idx, &off, nullptr, nullptr); return params + off;
+    };
+    const int iWtf = 2 * (N + 1), iWtb = 2 * (N + 1) + 2;
+    const bool uni = (c.unidirectional != 0);
+    // the uni-directional temporal layer's output IS the forward sweep (rnnet.py:112-116)
+    auto Act = [&](int i) -> const float * { return (uni && i == tl && tl > 0) ? m.For : m.X[i]; };
+    // the sweep kernels' error flag (word 0) is cleared once per call, so a forward-sweep timeout survives the BPTT sweep
+    CTCB_CUDA_CHECK(cudaMemsetAsync(m.counters, 0, 16 * sizeof(unsigned int), st));
+    for (int i = 1; i <= N + 1; ++i) {
+        const float *in = (i == 1) ? feats : Act(i - 1);
+        const int relu = (i <= N && i != tl) ? 1 : 0;
+        {
+        ProfScope ps("gemm_fwd", st);
+        TRY(ctcb_gemm_f32(0, 1, (int)R, sz[i], sz[i - 1], 1.f, in, sz[i - 1], P(2 * (i - 1)), sz[i - 1], 0.f,
+                          m.X[i], sz[i], P(2 * (i - 1) + 1), relu, nullptr, m.gemm, m.gemm_bytes, st));
+        }
+        if (i == tl) {
+            {
+            ProfScope ps("sweep_fwd", st);
+            TRY(run_sweep(0, Tmax, B, H, T_per_utt, m.X[i], P(iWtf), uni ? nullptr : P(iWtb), m.For, m.Back, nullptr,
+                          nullptr, c.maxAct, m.counters, m.sweep, m.sweep_bytes, st));
+            }
+            if (!uni) {     // over the pre-activation, which nothing reads after the sweep
+                ProfScope ps("elementwise", st);
+                TRY(run_add2(m.For, m.Back, m.X[i], R * H, st));     // brnnet.py:153
+            }
+        }
+    }
+    if (probs_out) {
+        const int wpb = 8;
+        softmax_rows_kernel<<<(unsigned)((R + wpb - 1) / wpb), wpb * 32, 0, st>>>(m.X[N + 1], probs_out, R, K);
+        CTCB_LAUNCH_CHECK();
+    }
+    return CTCB_OK;
+}
+
 // One micro-batch of a step whose gradient is the sum over several calls (include/ctcb200.h): without
 // CTCB_PART_FIRST every gradient tensor and the statistics tail are added into, with it overwritten; only the
 // CTCB_PART_LAST call exchanges over the ranks and adds the L2 term, so each happens once per step.
@@ -371,15 +495,34 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
         return set_error(CTCB_EINVAL, "ctcb_brnn_cost_and_grad: training mode needs labels and cost/skip outputs");
     if (!train && !probs_out)
         return set_error(CTCB_EINVAL, "ctcb_brnn_cost_and_grad: forward-only mode needs probs_out");
-    const WsLayout w = ws_layout(&c);
-    if (!workspace || ws_bytes < w.total)
-        return set_error(CTCB_ENOMEM, "ctcb_brnn_cost_and_grad: workspace %zu < %zu bytes", ws_bytes, w.total);
     cudaStream_t st = (cudaStream_t)stream;
     char *ws = (char *)workspace;
     const int N = c.numLayers, H = c.layerSize, K = c.outputDim, tl = h->tl;
     const int *sz = h->sizes;
     const int64_t R = (int64_t)Tmax * B;
     if (R > 0x7fffffff) return set_error(CTCB_EINVAL, "ctcb_brnn_cost_and_grad: T*B too large");
+    FwdBufs m{};
+    if (!train) {     // the forward layout whatever the size given: the same kernels and plans as a training call
+        if (!h->fwd_ready) {
+            h->fwd = fwd_layout(&c);
+            h->fwd_ready = true;
+        }
+        const FwdLayout &f = h->fwd;
+        if (!workspace || ws_bytes < f.total)
+            return set_error(CTCB_ENOMEM, "ctcb_brnn_cost_and_grad: workspace %zu < %zu bytes", ws_bytes, f.total);
+        for (int i = 1; i <= N + 1; ++i) m.X[i] = (float *)(ws + f.slab[i % 2]);
+        m.For = f.For ? (float *)(ws + f.For) : nullptr;      // offset 0 is slab 0: For / Back were not laid out
+        m.Back = f.Back ? (float *)(ws + f.Back) : nullptr;
+        m.gemm = ws + f.gemm;
+        m.gemm_bytes = f.gemm_bytes;
+        m.counters = (unsigned int *)(ws + f.counters);
+        m.sweep = ws + f.sweep;
+        m.sweep_bytes = f.sweep_bytes;
+        return brnn_forward(h, feats, T_per_utt, B, Tmax, params, probs_out, m, st);
+    }
+    const WsLayout w = ws_layout(&c);
+    if (!workspace || ws_bytes < w.total)
+        return set_error(CTCB_ENOMEM, "ctcb_brnn_cost_and_grad: workspace %zu < %zu bytes", ws_bytes, w.total);
     auto Xbuf = [&](int i) -> float * { return (float *)(ws + w.X[i]); };
     auto P = [&](int idx) -> const float * {
         int64_t off; ctcb_brnn_tensor_info(&c, idx, &off, nullptr, nullptr); return params + off;
@@ -397,37 +540,18 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
     // activations of layer i as the next layer (and the weight gradients) see them: the uni-directional temporal
     // layer's output IS the forward sweep (rnnet.py:112-116), the bi-directional one's is For + Back
     auto Act = [&](int i) -> float * { return (uni && i == tl && tl > 0) ? For : Xbuf(i); };
-    // the sweep kernels' error flag (word 0) is cleared once per call, so a forward-sweep timeout survives the BPTT sweep
-    CTCB_CUDA_CHECK(cudaMemsetAsync(counters, 0, 16 * sizeof(unsigned int), st));
 
     // ---------------------------------------------------------------- forward (brnnet.py:136-157)
-    for (int i = 1; i <= N + 1; ++i) {
-        const float *in = (i == 1) ? feats : Act(i - 1);
-        const int relu = (i <= N && i != tl) ? 1 : 0;
-        {
-        ProfScope ps("gemm_fwd", st);
-        TRY(ctcb_gemm_f32(0, 1, (int)R, sz[i], sz[i - 1], 1.f, in, sz[i - 1], P(2 * (i - 1)), sz[i - 1], 0.f,
-                          Xbuf(i), sz[i], P(2 * (i - 1) + 1), relu, nullptr, gws, gws_bytes, st));
-        }
-        if (i == tl) {
-            {
-            ProfScope ps("sweep_fwd", st);
-            TRY(run_sweep(0, Tmax, B, H, T_per_utt, Xbuf(i), P(iWtf), uni ? nullptr : P(iWtb), For, Back, nullptr,
-                          nullptr, c.maxAct, counters, ws + w.sweep, w.sweep_bytes, st));
-            }
-            if (!uni) {
-                ProfScope ps("elementwise", st);
-                TRY(run_add2(For, Back, Xbuf(i), R * H, st));     // brnnet.py:153
-            }
-        }
-    }
+    for (int i = 1; i <= N + 1; ++i) m.X[i] = Xbuf(i);
+    m.For = For;
+    m.Back = Back;
+    m.gemm = gws;
+    m.gemm_bytes = gws_bytes;
+    m.counters = counters;
+    m.sweep = ws + w.sweep;
+    m.sweep_bytes = w.sweep_bytes;
+    TRY(brnn_forward(h, feats, T_per_utt, B, Tmax, params, probs_out, m, st));
     float *logits = Xbuf(N + 1);
-    if (probs_out) {
-        const int wpb = 8;
-        softmax_rows_kernel<<<(unsigned)((R + wpb - 1) / wpb), wpb * 32, 0, st>>>(logits, probs_out, R, K);
-        CTCB_LAUNCH_CHECK();
-    }
-    if (!train) return CTCB_OK;
 
     // ---------------------------------------------------------------- CTC (brnnet.py:161-175)
     auto dbuf = [&](int j) -> float * { return (float *)(ws + w.D[j]); };

@@ -17,6 +17,8 @@ single contiguous vector.  New, additive surface for the minibatch/data-parallel
     costAndGradBatch(datas, labelss)         -> (costs[B], grad, skips[B])   host arrays in; more than maxUtts
                                                 utterances are accumulated over micro-batches
     costAndGradDevice(batch, first, last)    -> no host sync; see DeviceBatch
+    forwardBatch(datas)                      -> [K x T float32 probabilities] per utterance, in input order,
+                                                micro-batches of at most maxUtts (the batched costAndGrad(train=False))
 
 torch tensors are buffer handles only; all arithmetic is in the C ABI (include/ctcb200.h).
 """
@@ -210,10 +212,15 @@ class NNet:
         else:
             self.grads = None
             self.stats = None
-        nbytes = lib.ctcb_brnn_workspace_bytes(ctypes.byref(self._cfg))
+        # a forward-only net needs about a quarter of the training workspace (no CTC, delta or gradient buffers)
+        fwd_off = ctypes.c_size_t()
+        fwd_bytes = lib.ctcb_brnn_forward_workspace_bytes(ctypes.byref(self._cfg), ctypes.byref(fwd_off))
+        nbytes = lib.ctcb_brnn_workspace_bytes(ctypes.byref(self._cfg)) if self.train else fwd_bytes
         self._ws = torch.zeros(nbytes, dtype=torch.uint8, device=self.dev)
-        off = lib.ctcb_brnn_error_flag_offset(ctypes.byref(self._cfg))
-        self._errflag = self._ws[off:off + 4].view(torch.int32)      # set by the sweep kernels on a wait timeout
+        # the sweep error flag of a forward-only call, which uses the forward layout in either workspace (a training
+        # call reports its flag in the statistics tail); set by the sweep kernels on a wait timeout
+        self._errflag = self._ws[fwd_off.value:fwd_off.value + 4].view(torch.int32)
+        self._fwd_host = None       # pinned probabilities + error flag of one forward micro-batch (forwardBatch)
         self._batch = DeviceBatch(torch, self.dev, self.maxBatch, self.maxUtts, self.inputDim, self.maxLabels)
         self._batch_alt = None      # second staging buffer, created on first use by SGD.run's prefetch
         # per-utterance outputs: cost (float32) and skip (int32) share one buffer -> one D2H copy reads both
@@ -255,27 +262,34 @@ class NNet:
         the gradient and the statistics tail into what the earlier calls left; only the last=True call exchanges
         over the ranks and adds the L2 term.  `out` optionally names the (cost[B], skip[B]) device tensors to write
         (default: the net's own per-utterance buffers)."""
-        torch = self._torch
+        if not self.train:
+            return self._forward_device(batch)
         B, Tmax = batch.B, batch.Tmax
-        probs = None
-        if want_probs or not self.train:
-            n = Tmax * B * self.outputDim
-            if self._probs is None or self._probs.numel() < n:
-                self._probs = torch.empty(self.maxBatch * self.maxUtts * self.outputDim, dtype=torch.float32,
-                                          device=self.dev)
-            probs = self._probs[:n].view(Tmax, B, self.outputDim)
+        probs = self._probs_view(B, Tmax) if want_probs else None
         cost, skip = out if out is not None else (self._cost[:B], self._skip[:B])
         flags = (_ctcb.PART_FIRST if first else 0) | (_ctcb.PART_LAST if last else 0)
         check(lib.ctcb_brnn_cost_and_grad_part(
             self._h, ptr(batch.d_feats), ptr(batch.d_lens), ptr(batch.d_labels), ptr(batch.d_off), B, Tmax,
-            ptr(self.params), ptr(self.grads) if self.train else None,
-            ptr(cost) if self.train else None, ptr(skip) if self.train else None,
-            ptr(self._regcost) if self.train else None, ptr(probs), ptr(self.stats), flags, ptr(self._ws),
-            self._ws.numel(),
-            _ctcb.current_stream()))
-        if not self.train:
-            return probs
+            ptr(self.params), ptr(self.grads), ptr(cost), ptr(skip), ptr(self._regcost), ptr(probs), ptr(self.stats),
+            flags, ptr(self._ws), self._ws.numel(), _ctcb.current_stream()))
         return cost, skip
+
+    def _probs_view(self, B, Tmax):
+        n = Tmax * B * self.outputDim
+        if self._probs is None or self._probs.numel() < n:
+            self._probs = self._torch.empty(self.maxBatch * self.maxUtts * self.outputDim, dtype=self._torch.float32,
+                                            device=self.dev)
+        return self._probs[:n].view(Tmax, B, self.outputDim)
+
+    def _forward_device(self, batch):
+        """Forward-only call (grads = NULL, the forward workspace layout) on a staged DeviceBatch, whether or not this
+        net trains: enqueues and returns the device probabilities [Tmax][B][K] without synchronising."""
+        probs = self._probs_view(batch.B, batch.Tmax)
+        check(lib.ctcb_brnn_cost_and_grad_part(
+            self._h, ptr(batch.d_feats), ptr(batch.d_lens), None, None, batch.B, batch.Tmax, ptr(self.params), None,
+            None, None, None, ptr(probs), None, _ctcb.PART_FIRST | _ctcb.PART_LAST, ptr(self._ws), self._ws.numel(),
+            _ctcb.current_stream()))
+        return probs
 
     def costAndGradBatch(self, datas, labelss):
         """Minibatch costAndGrad from host arrays: gradients of the utterances are summed.
@@ -350,6 +364,42 @@ class NNet:
         if self.reg > 0:
             cost = cost + self.regcost          # brnnet.py:177-183
         return cost, grad, bool(skips[0])
+
+    def forwardBatch(self, datas):
+        """The K x T float32 probabilities that costAndGrad(data) returns with train=False, for every utterance of
+        `datas` (inputDim x T arrays), in input order.  The utterances are sorted by length and cut into micro-batches
+        of at most maxUtts; micro-batch i+1 is packed into the idle staging buffer while the device computes i, and
+        each micro-batch ends in one synchronisation behind the copy of its probabilities and the sweep error flag
+        into pinned memory.  Works on training nets too (forward-only calls fit in the training workspace)."""
+        torch = self._torch
+        for u, d in enumerate(datas):
+            if d.shape[1] > self.maxBatch:
+                raise ValueError("utterance %d has %d frames; this net was built for at most maxBatch=%d"
+                                 % (u, d.shape[1], self.maxBatch))
+        order = sorted(range(len(datas)), key=lambda u: datas[u].shape[1])
+        pieces = parallel.micro_batches(order, self.maxUtts)
+        if self._fwd_host is None:
+            n = self.maxBatch * self.maxUtts * self.outputDim
+            self._fwd_host = (torch.empty(n, dtype=torch.float32).pin_memory(),
+                              torch.zeros(1, dtype=torch.int32).pin_memory())
+        h_all, h_flag = self._fwd_host
+        out = [None] * len(datas)
+        batch = self.swap_batches().pack([datas[u] for u in pieces[0]], None).upload() if pieces else None
+        for k, idx in enumerate(pieces):
+            probs = self._forward_device(batch)
+            h_probs = h_all[:probs.numel()]
+            h_probs.copy_(probs.view(-1), non_blocking=True)
+            h_flag.copy_(self._errflag, non_blocking=True)
+            if k + 1 < len(pieces):         # host packing of the next micro-batch overlaps this one's compute
+                batch = self.swap_batches().pack([datas[u] for u in pieces[k + 1]], None).upload()
+            torch.cuda.current_stream().synchronize()
+            flag = int(h_flag[0])
+            if flag != 0:
+                raise RuntimeError("recurrent sweep: inter-CTA wait timed out (flag %d); results are invalid" % flag)
+            p = h_probs.numpy().reshape(probs.shape)
+            for j, u in enumerate(idx):
+                out[u] = np.ascontiguousarray(p[:datas[u].shape[1], j, :].T)
+        return out
 
     def updateParams(self, scale, update):
         """w += scale * dw for every [w, b] (brnnet.py:251-256).  When `update` is a list of views of

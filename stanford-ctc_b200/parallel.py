@@ -15,6 +15,13 @@ def shard(items, rank, world):
     return list(items[rank::world])
 
 
+def rank_files(start_file, num_files, rank, world):
+    """The data files rank `rank` of `world` writes likelihoods for (runNNet --test): start_file + rank,
+    start_file + rank + world, ... up to num_files, the last file of the reference's range (runNNet.py:236).
+    Every file is written by exactly one rank, so the ranks neither repeat work nor race on an ark path."""
+    return shard(range(start_file, num_files + 1), rank, world)
+
+
 def select_step_utterances(data_dict, alis, chunk, max_frames, rank, world, log=None, max_labels=None):
     """The utterances of one step that THIS rank computes.  The reference's per-utterance admission rules
     (sgd.py:76-88: skip when longer than the buffers, skip when there are fewer frames than labels) are applied

@@ -45,7 +45,8 @@ FLAGS = [
     # additions
     ("batchSize", int, 1, "utterances per optimisation step (1 = the reference schedule)"),
     ("maxUtts", int, 0, "utterances per micro-batch per GPU: a larger shard accumulates its gradient over several "
-                        "micro-batches (0 = the whole shard, batchSize / number of GPUs rounded up)"),
+                        "micro-batches (0 = the whole shard, batchSize / number of GPUs rounded up); with --test, "
+                        "utterances per forward call per GPU (0 = one, the reference's loop)"),
     ("maxLabels", int, 511, "longest label sequence the buffers are sized for"),
     ("runDir", str, "./runs", "parent of the time-stamped run directory"),
     ("outDir", str, None, "--test: directory for the likelihood arks"),
@@ -156,7 +157,7 @@ def run(args=None):
     cfg["output_dir"] = out_dir
     cfg["in_file"] = cfg["out_file"] = os.path.join(out_dir, "params.pk")
     if cli.test:                                      # these come from the command line, not the stored config
-        for key in ("dataDir", "numFiles", "startFile", "outDir"):
+        for key in ("dataDir", "numFiles", "startFile", "outDir", "maxUtts"):
             cfg[key] = getattr(cli, key)
 
     run_dir = RunDir(out_dir)
@@ -168,7 +169,7 @@ def run(args=None):
     opts = CfgStruct(**cfg)
     opts.cfg_file = cli.cfg_file
     if cli.test:
-        return test(opts)
+        return test(opts, rank, world)
     return _train(opts, cfg, run_dir, log, rank, world)
 
 
@@ -230,13 +231,15 @@ def _train(opts, cfg, run_dir, log, rank, world):
     return optimizer, net
 
 
-def test(opts):
+def test(opts, rank=0, world=1):
     """Forward-only pass of a trained model over data files; writes Kaldi arks + pickles
-    (runNNet.py:208-237, analysis-utils/writeLikelihoods.py)."""
+    (runNNet.py:208-237, analysis-utils/writeLikelihoods.py).  --maxUtts utterances per forward call (0: one, the
+    reference's loop); rank `rank` of `world` processes (run() passes them under torchrun) writes its own share of
+    the files (parallel.rank_files)."""
     trained = CfgStruct(**load_config(opts.cfg_file))
     logging.getLogger().info("Running on %s" % get_hostname())
     net = rnnet.NNet(trained.inputDim, trained.outputDim, trained.layerSize, trained.numLayers, trained.maxUttLen,
-                     temporalLayer=trained.temporalLayer, train=False)
+                     temporalLayer=trained.temporalLayer, train=False, maxUtts=max(1, opts.maxUtts))
     net.initParams()
     with open(trained.in_file, "rb") as fid:
         pickle.load(fid)                              # optimiser state: not needed here
@@ -244,7 +247,7 @@ def test(opts):
     loader = dl.DataLoader(opts.dataDir, trained.rawDim, trained.inputDim, opts.alisDir or opts.dataDir)
     out_dir = getattr(opts, "outDir", None) or os.path.join(opts.output_dir, "ctc_loglikes")
     os.makedirs(out_dir, exist_ok=True)
-    for filenum in range(opts.startFile, opts.numFiles + 1):
+    for filenum in parallel.rank_files(opts.startFile, opts.numFiles, rank, world):
         writeLogLikes(loader, net, filenum, out_dir, writePickle=True)
     return net
 

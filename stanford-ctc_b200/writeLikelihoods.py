@@ -1,6 +1,8 @@
 """writeLikelihoods -- forward-only log-likelihood dump, same function names and on-disk formats as
 ctc_fast/analysis-utils/writeLikelihoods.py:8-55 (Kaldi binary "BFM" float matrix ark
-+ a pickle of {key: log-prob K x T})."""
++ a pickle of {key: log-prob K x T}).  The file's utterances go through the net together
+(NNet.forwardBatch, micro-batches of the net's maxUtts); headers and log-probabilities are written on the host in
+key order, as the reference's per-key loop writes them."""
 import pickle
 import struct
 
@@ -22,10 +24,12 @@ def writeLogLikes(loader, nn, fn, outDir, writePickle=False):
     data_dict, alis, keys, sizes = loader.loadDataFileDict(fn)
     lik_dict = dict()
     with open(outDir + '/loglikelihoods%d.ark' % fn, 'wb') as fid:
-        for i, k in enumerate(keys):
+        for k in keys:
             assert data_dict[k].shape[1] < nn.maxBatch, "Need larger max utt length."
+        probss = nn.forwardBatch([data_dict[k] for k in keys])
+        for i, k in enumerate(keys):
             writeUttHeader(fid, k, int(sizes[i]), nn.outputDim)
-            probs = nn.costAndGrad(data_dict[k])
+            probs = probss[i]
             assert probs.dtype == np.float32, "Probs array malformed."
             assert probs.shape[0] == nn.outputDim, "Probs dimensions mismatch."
             with np.errstate(divide='ignore'):
