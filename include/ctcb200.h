@@ -140,16 +140,25 @@ typedef struct ctcb_brnn_config {
     int32_t unidirectional; /* 0: nnets/brnnet.py (Wtf and Wtb, output For+Back).  1: nnets/rnnet.py:91-191 -- one
                              * recurrent matrix, forward in time only, stack = [...layers, [Wt, dummy]] (rnnet.py:57-65).
                              * temporalLayer <= 0 with either value is the plain DNN of nnets/nnet.py:57-113. */
+    int32_t numTemporal;   /* k: layers temporalLayer .. temporalLayer+k-1 are all temporal, each with its own recurrent
+                            * matrices and sweeps (output For_j + Back_j, uni-directional For_j).  0 and 1 both mean
+                            * one temporal layer, so an initialiser without this member keeps its meaning.  k > 1 needs
+                            * 1 <= temporalLayer and temporalLayer + k - 1 <= numLayers, else the config is invalid. */
 } ctcb_brnn_config;
 
 typedef struct ctcb_brnn ctcb_brnn; /* opaque; owns no device memory */
 
 /* Flat parameter vector layout: the reference's `stack` order (brnnet.py:38-41,66-72):
  * [W1,b1] ... [W_{N+1},b_{N+1}] [Wtf,dummy] [Wtb,dummy]; W row-major (out x in), dummy = 1 float.
- * unidirectional: [W1,b1] ... [W_{N+1},b_{N+1}] [Wt,dummy]. */
+ * unidirectional: [W1,b1] ... [W_{N+1},b_{N+1}] [Wt,dummy].
+ * numTemporal = k > 1: [W1,b1] ... [W_{N+1},b_{N+1}] then, per temporal layer in ascending order,
+ * [Wtf_j,dummy] [Wtb_j,dummy] (unidirectional: [Wt_j,dummy]); for k = 1 this is the layout above. */
 int64_t ctcb_brnn_param_count(const ctcb_brnn_config *cfg);
 int ctcb_brnn_num_tensors(const ctcb_brnn_config *cfg);                    /* 2 * len(stack) */
 int ctcb_brnn_tensor_info(const ctcb_brnn_config *cfg, int idx, int64_t *offset, int32_t *rows, int32_t *cols);
+/* numTemporal = k > 1 adds k * (2 bi-directional / 1 uni-directional) buffers of maxT*maxB*layerSize floats, each
+ * rounded up to 256 bytes, to the one-layer size: For_j (and Back_j) of every temporal layer above the first, and a
+ * second dFor / dBack pair that consecutive layers alternate with. */
 size_t ctcb_brnn_workspace_bytes(const ctcb_brnn_config *cfg);
 /* Byte offset, inside the workspace, of a uint32 that the recurrent-sweep kernels set non-zero when an
  * inter-CTA wait timed out (results are then invalid; never a hang).  Callers that synchronise anyway
@@ -168,7 +177,9 @@ size_t ctcb_brnn_forward_workspace_bytes(const ctcb_brnn_config *cfg, size_t *er
  * ctcb_brnn_cost_and_grad TRAINING call (grads != NULL) left behind, time-major [Tmax][B][*width] with that call's
  * B and Tmax; a forward-only call lays its buffers out differently (ctcb_brnn_forward_workspace_bytes).
  * what = 0: output of affine map `layer` (1..numLayers+1; For+Back at the temporal layer, logits at the last),
- * what = 1 / 2: For / Back of the temporal layer (brnnet.py:143-153). */
+ * what = 1 / 2: For / Back of the temporal layer (brnnet.py:143-153).  With numTemporal > 1, `layer` names which
+ * temporal layer (temporalLayer .. temporalLayer+k-1; Back exists only when bi-directional); with one temporal
+ * layer it is ignored. */
 int ctcb_brnn_activation_offset(const ctcb_brnn_config *cfg, int what, int layer, size_t *offset, int32_t *width);
 
 int ctcb_brnn_create(const ctcb_brnn_config *cfg, ctcb_brnn **out);

@@ -27,7 +27,7 @@ class BrnnConfig(ctypes.Structure):
     _fields_ = [("inputDim", ctypes.c_int32), ("outputDim", ctypes.c_int32), ("layerSize", ctypes.c_int32),
                 ("numLayers", ctypes.c_int32), ("temporalLayer", ctypes.c_int32), ("maxT", ctypes.c_int32),
                 ("maxB", ctypes.c_int32), ("maxLabels", ctypes.c_int32), ("reg", ctypes.c_float),
-                ("maxAct", ctypes.c_float), ("unidirectional", ctypes.c_int32)]
+                ("maxAct", ctypes.c_float), ("unidirectional", ctypes.c_int32), ("numTemporal", ctypes.c_int32)]
 
 
 _PROTOS = {

@@ -8,7 +8,8 @@
 //              contiguous (B x n) slab, so the layer contractions are single GEMMs over R = T*B rows
 //              and the recurrences are (B x H)(H x H) products per step.
 //   forward  : per layer one GEMM with bias(+ReLU) fused in the epilogue (brnnet.py:140-141,155-157);
-//              the temporal layer adds the persistent two-direction sweep (sweep.cu) and For+Back.
+//              each temporal layer (numTemporal of them, stacked) adds the persistent two-direction sweep
+//              (sweep.cu) with its own recurrent matrices and For+Back.
 //   CTC      : softmax + alpha/beta + gradient in one kernel on the device (ctc.cu); nothing leaves HBM.
 //   backward : per layer dW = delta^T X (split-K GEMM over R), db = column sums, delta <- delta W with
 //              the ReLU mask fused (brnnet.py:196-204,235-237); BPTT sweep; the recurrent weight
@@ -138,13 +139,17 @@ struct FwdLayout {
 struct ctcb_brnn {
     ctcb_brnn_config cfg;
     int nlayers;        // N + 1 affine maps
-    int tl;             // temporal layer or 0
+    int tl;             // lowest temporal layer or 0
+    int nt;             // temporal layers tl .. tl+nt-1 (0 without)
     int sizes[66];      // [D, H.., K]
     // weight/bias gradients of the layers at and above the temporal layer depend only on their delta, so they
     // run on a side stream next to the (latency-bound, 112-SM) BPTT sweep; created on first use
     cudaStream_t side;
     cudaEvent_t ev_delta[66];
     cudaEvent_t ev_side;
+    // the two dFor/dBack pairs that stacked temporal layers alternate: ev_pair[p] is recorded on the side stream after
+    // its last read of pair p, and the BPTT sweep that writes pair p next waits for it
+    cudaEvent_t ev_pair[2];
     bool side_ready;
     // data-parallel callers sum the gradient over ranks first and add reg*W ONCE afterwards (ctcb_brnn_apply_l2_f32);
     // the L2 cost is still reported by every call
@@ -163,10 +168,23 @@ static int valid_cfg(const ctcb_brnn_config *c) {
     if (c->numLayers < 1 || c->numLayers > 64) return 0;
     if (c->maxT <= 0 || c->maxB <= 0 || c->maxLabels < 0) return 0;
     if (c->maxLabels > CTCB_CTC_MAX_LABELS) return 0;   // the CTC kernel's register-resident trellis (ctc.cu)
+    if (c->numTemporal < 0) return 0;
+    // a stacked block must lie inside the hidden layers; k <= 1 keeps the silent "no temporal layer" rule below
+    if (c->numTemporal > 1 && (c->temporalLayer <= 0 || c->temporalLayer + c->numTemporal - 1 > c->numLayers)) return 0;
     return 1;
 }
 static int eff_tl(const ctcb_brnn_config *c) {
     return (c->temporalLayer <= 0 || c->temporalLayer > c->numLayers) ? 0 : c->temporalLayer;
+}
+// number of temporal layers of a valid config
+static int eff_nt(const ctcb_brnn_config *c) {
+    if (!eff_tl(c)) return 0;
+    return c->numTemporal > 1 ? c->numTemporal : 1;
+}
+// flat-vector index of the (forward) recurrent matrix of temporal layer j (0-based within the block); the backward
+// one, when bi-directional, is two tensors behind it
+static int rec_index(const ctcb_brnn_config *c, int j) {
+    return 2 * (c->numLayers + 1) + j * (c->unidirectional ? 2 : 4);
 }
 static void layer_sizes(const ctcb_brnn_config *c, int *sizes) {
     sizes[0] = c->inputDim;
@@ -176,7 +194,7 @@ static void layer_sizes(const ctcb_brnn_config *c, int *sizes) {
 
 extern "C" int ctcb_brnn_num_tensors(const ctcb_brnn_config *cfg) {
     if (!valid_cfg(cfg)) return 0;
-    return 2 * (cfg->numLayers + 1) + (eff_tl(cfg) ? (cfg->unidirectional ? 2 : 4) : 0);
+    return 2 * (cfg->numLayers + 1) + eff_nt(cfg) * (cfg->unidirectional ? 2 : 4);
 }
 
 extern "C" int ctcb_brnn_tensor_info(const ctcb_brnn_config *cfg, int idx, int64_t *offset, int32_t *rows, int32_t *cols) {
@@ -221,6 +239,9 @@ namespace {
 struct WsLayout {
     size_t X[66];       // X[1..N] activations, X[N+1] logits
     size_t For, Back, dFor, dBack;
+    // stacked temporal layers: For / Back of temporal layer j (ForJ[0] = For, BackJ[0] = Back) and the second
+    // dFor / dBack pair, which layers of odd j use (0 where not laid out)
+    size_t ForJ[64], BackJ[64], dFor2, dBack2;
     size_t D[67];       // D[j]: gradient w.r.t. the output of affine map j (1..N+1)
     size_t gemm2, colsum2;
     size_t ctc, gemm, colsum, scratch, counters, sweep, sweep_bytes, lens_dummy;
@@ -241,6 +262,20 @@ WsLayout ws_layout(const ctcb_brnn_config *c) {
         w.Back = take(R * H * sizeof(float));
         w.dFor = take(R * H * sizeof(float));
         w.dBack = take(R * H * sizeof(float));
+        w.ForJ[0] = w.For;
+        w.BackJ[0] = w.Back;
+    }
+    // every further temporal layer keeps its own For (and Back): the BPTT masks and the recurrent weight gradients
+    // read them.  The dFor / dBack pairs alternate between consecutive layers, so a stack needs one more pair.
+    const int nt = eff_nt(c);
+    const bool uni = (c->unidirectional != 0);
+    for (int j = 1; j < nt; ++j) {
+        w.ForJ[j] = take(R * H * sizeof(float));
+        if (!uni) w.BackJ[j] = take(R * H * sizeof(float));
+    }
+    if (nt > 1) {
+        w.dFor2 = take(R * H * sizeof(float));
+        if (!uni) w.dBack2 = take(R * H * sizeof(float));
     }
     const size_t wide = (size_t)(H > K ? H : K);
     for (int j = 1; j <= N + 1; ++j) w.D[j] = take(R * wide * sizeof(float));
@@ -337,6 +372,9 @@ extern "C" int ctcb_brnn_create(const ctcb_brnn_config *cfg, ctcb_brnn **out) {
     if (cfg && cfg->maxLabels > CTCB_CTC_MAX_LABELS)
         return set_error(CTCB_EINVAL, "ctcb_brnn_create: maxLabels %d exceeds the CTC kernel's limit of %d labels per utterance",
                          cfg->maxLabels, CTCB_CTC_MAX_LABELS);
+    if (cfg && cfg->numTemporal > 1 && !valid_cfg(cfg))
+        return set_error(CTCB_EINVAL, "ctcb_brnn_create: a block of %d temporal layers from layer %d does not fit in "
+                         "hidden layers 1..%d", cfg->numTemporal, cfg->temporalLayer, cfg->numLayers);
     if (!valid_cfg(cfg) || !out) return set_error(CTCB_EINVAL, "ctcb_brnn_create: bad config");
     ctcb_brnn *h = new (std::nothrow) ctcb_brnn;
     if (!h) return set_error(CTCB_ENOMEM, "ctcb_brnn_create: out of host memory");
@@ -344,6 +382,7 @@ extern "C" int ctcb_brnn_create(const ctcb_brnn_config *cfg, ctcb_brnn **out) {
     if (h->cfg.maxAct <= 0.f) h->cfg.maxAct = 20.0f;   // brnnet.py:32
     h->nlayers = cfg->numLayers + 1;
     h->tl = eff_tl(cfg);
+    h->nt = eff_nt(cfg);
     layer_sizes(cfg, h->sizes);
     h->side = nullptr;
     h->side_ready = false;
@@ -359,6 +398,7 @@ extern "C" void ctcb_brnn_destroy(ctcb_brnn *h) {
         cudaStreamDestroy(h->side);
         for (int i = 0; i < 66; ++i) cudaEventDestroy(h->ev_delta[i]);
         cudaEventDestroy(h->ev_side);
+        for (int p = 0; p < 2; ++p) cudaEventDestroy(h->ev_pair[p]);
     }
     delete h;
 }
@@ -368,6 +408,7 @@ static int ensure_side_stream(ctcb_brnn *h) {
     CTCB_CUDA_CHECK(cudaStreamCreateWithFlags(&h->side, cudaStreamNonBlocking));
     for (int i = 0; i < 66; ++i) CTCB_CUDA_CHECK(cudaEventCreateWithFlags(&h->ev_delta[i], cudaEventDisableTiming));
     CTCB_CUDA_CHECK(cudaEventCreateWithFlags(&h->ev_side, cudaEventDisableTiming));
+    for (int p = 0; p < 2; ++p) CTCB_CUDA_CHECK(cudaEventCreateWithFlags(&h->ev_pair[p], cudaEventDisableTiming));
     h->side_ready = true;
     return CTCB_OK;
 }
@@ -393,7 +434,8 @@ extern "C" int ctcb_brnn_sweep_f32(int mode, int T, int B, int H, const int32_t 
 }
 
 // The part of the flat gradient that was NOT summed early on the side stream, plus the statistics tail, in one grouped
-// NCCL launch: with an early bucket [off(2 tl), end of layer N+1) that is everything before it and everything behind it.
+// NCCL launch: with an early bucket [off(2 tl), end of layer N+1), tl the lowest temporal layer, that is everything
+// before it and everything behind it (the recurrent matrices of every temporal layer among them).
 static int brnn_reduce_rest(ctcb_brnn *h, float *grads, float *stats, bool early_bucket, cudaStream_t st) {
     const ctcb_brnn_config &c = h->cfg;
     const int64_t P = ctcb_brnn_param_count(&c);
@@ -415,10 +457,11 @@ static int brnn_reduce_rest(ctcb_brnn *h, float *grads, float *stats, bool early
 }
 
 // Where the forward half reads and writes: X[i] (1..N+1) the output of affine map i (pre-activation, then For+Back,
-// at the temporal layer; the logits at N+1), the two sweep outputs, the split-K area, the sweep counters and scratch.
+// at a temporal layer; the logits at N+1), the two sweep outputs of each temporal layer j (one pair shared by all
+// layers in the forward-only layout), the split-K area, the sweep counters and scratch.
 struct FwdBufs {
     float *X[66];
-    float *For, *Back;
+    float *For[64], *Back[64];
     void *gemm;
     size_t gemm_bytes;
     unsigned int *counters;
@@ -426,40 +469,41 @@ struct FwdBufs {
     size_t sweep_bytes;
 };
 
-// brnnet.py:136-173: the affine maps with bias(+ReLU) fused, the two-direction sweep and For+Back at the temporal
+// brnnet.py:136-173: the affine maps with bias(+ReLU) fused, the two-direction sweep and For+Back at each temporal
 // layer, the softmax into probs_out when given.  Clears the sweep error flag first.
 static int brnn_forward(ctcb_brnn *h, const float *feats, const int32_t *T_per_utt, int B, int Tmax,
                         const float *params, float *probs_out, const FwdBufs &m, cudaStream_t st) {
     const ctcb_brnn_config &c = h->cfg;
-    const int N = c.numLayers, H = c.layerSize, K = c.outputDim, tl = h->tl;
+    const int N = c.numLayers, H = c.layerSize, K = c.outputDim, tl = h->tl, nt = h->nt;
     const int *sz = h->sizes;
     const int64_t R = (int64_t)Tmax * B;
     auto P = [&](int idx) -> const float * {
         int64_t off; ctcb_brnn_tensor_info(&c, idx, &off, nullptr, nullptr); return params + off;
     };
-    const int iWtf = 2 * (N + 1), iWtb = 2 * (N + 1) + 2;
     const bool uni = (c.unidirectional != 0);
+    auto temporal = [&](int i) { return nt > 0 && i >= tl && i < tl + nt; };
     // the uni-directional temporal layer's output IS the forward sweep (rnnet.py:112-116)
-    auto Act = [&](int i) -> const float * { return (uni && i == tl && tl > 0) ? m.For : m.X[i]; };
+    auto Act = [&](int i) -> const float * { return (uni && temporal(i)) ? m.For[i - tl] : m.X[i]; };
     // the sweep kernels' error flag (word 0) is cleared once per call, so a forward-sweep timeout survives the BPTT sweep
     CTCB_CUDA_CHECK(cudaMemsetAsync(m.counters, 0, 16 * sizeof(unsigned int), st));
     for (int i = 1; i <= N + 1; ++i) {
         const float *in = (i == 1) ? feats : Act(i - 1);
-        const int relu = (i <= N && i != tl) ? 1 : 0;
+        const int relu = (i <= N && !temporal(i)) ? 1 : 0;
         {
         ProfScope ps("gemm_fwd", st);
         TRY(ctcb_gemm_f32(0, 1, (int)R, sz[i], sz[i - 1], 1.f, in, sz[i - 1], P(2 * (i - 1)), sz[i - 1], 0.f,
                           m.X[i], sz[i], P(2 * (i - 1) + 1), relu, nullptr, m.gemm, m.gemm_bytes, st));
         }
-        if (i == tl) {
+        if (temporal(i)) {
+            const int j = i - tl, iWtf = rec_index(&c, j);
             {
             ProfScope ps("sweep_fwd", st);
-            TRY(run_sweep(0, Tmax, B, H, T_per_utt, m.X[i], P(iWtf), uni ? nullptr : P(iWtb), m.For, m.Back, nullptr,
-                          nullptr, c.maxAct, m.counters, m.sweep, m.sweep_bytes, st));
+            TRY(run_sweep(0, Tmax, B, H, T_per_utt, m.X[i], P(iWtf), uni ? nullptr : P(iWtf + 2), m.For[j], m.Back[j],
+                          nullptr, nullptr, c.maxAct, m.counters, m.sweep, m.sweep_bytes, st));
             }
             if (!uni) {     // over the pre-activation, which nothing reads after the sweep
                 ProfScope ps("elementwise", st);
-                TRY(run_add2(m.For, m.Back, m.X[i], R * H, st));     // brnnet.py:153
+                TRY(run_add2(m.For[j], m.Back[j], m.X[i], R * H, st));     // brnnet.py:153
             }
         }
     }
@@ -511,8 +555,10 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
         if (!workspace || ws_bytes < f.total)
             return set_error(CTCB_ENOMEM, "ctcb_brnn_cost_and_grad: workspace %zu < %zu bytes", ws_bytes, f.total);
         for (int i = 1; i <= N + 1; ++i) m.X[i] = (float *)(ws + f.slab[i % 2]);
-        m.For = f.For ? (float *)(ws + f.For) : nullptr;      // offset 0 is slab 0: For / Back were not laid out
-        m.Back = f.Back ? (float *)(ws + f.Back) : nullptr;
+        for (int j = 0; j < h->nt; ++j) {     // one pair for every temporal layer: each sweep runs after the last read
+            m.For[j] = f.For ? (float *)(ws + f.For) : nullptr;   // offset 0 is slab 0: For / Back were not laid out
+            m.Back[j] = f.Back ? (float *)(ws + f.Back) : nullptr;
+        }
         m.gemm = ws + f.gemm;
         m.gemm_bytes = f.gemm_bytes;
         m.counters = (unsigned int *)(ws + f.counters);
@@ -530,21 +576,30 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
     auto G = [&](int idx) -> float * {
         int64_t off; ctcb_brnn_tensor_info(&c, idx, &off, nullptr, nullptr); return grads + off;
     };
-    float *For = (float *)(ws + w.For), *Back = (float *)(ws + w.Back);
-    float *dFor = (float *)(ws + w.dFor), *dBack = (float *)(ws + w.dBack);
+    // For_j / Back_j of temporal layer j; the dFor / dBack pair of layer j is pair j % 2
+    float *ForJ[64], *BackJ[64];
+    for (int j = 0; j < h->nt; ++j) {
+        ForJ[j] = (float *)(ws + w.ForJ[j]);
+        BackJ[j] = (float *)(ws + w.BackJ[j]);      // unused (offset 0) for the uni-directional layers above the first
+    }
+    float *dF[2] = {(float *)(ws + w.dFor), (float *)(ws + w.dFor2)};
+    float *dB[2] = {(float *)(ws + w.dBack), (float *)(ws + w.dBack2)};
     void *gws = ws + w.gemm;
     const size_t gws_bytes = w.gemm2 - w.gemm;
     unsigned int *counters = (unsigned int *)(ws + w.counters);
-    const int iWtf = 2 * (N + 1), iWtb = 2 * (N + 1) + 2;
+    const int nt = h->nt;
     const bool uni = (c.unidirectional != 0);
-    // activations of layer i as the next layer (and the weight gradients) see them: the uni-directional temporal
-    // layer's output IS the forward sweep (rnnet.py:112-116), the bi-directional one's is For + Back
-    auto Act = [&](int i) -> float * { return (uni && i == tl && tl > 0) ? For : Xbuf(i); };
+    auto temporal = [&](int i) { return nt > 0 && i >= tl && i < tl + nt; };
+    // activations of layer i as the next layer (and the weight gradients) see them: a uni-directional temporal
+    // layer's output IS its forward sweep (rnnet.py:112-116), a bi-directional one's is For + Back
+    auto Act = [&](int i) -> float * { return (uni && temporal(i)) ? ForJ[i - tl] : Xbuf(i); };
 
     // ---------------------------------------------------------------- forward (brnnet.py:136-157)
     for (int i = 1; i <= N + 1; ++i) m.X[i] = Xbuf(i);
-    m.For = For;
-    m.Back = Back;
+    for (int j = 0; j < nt; ++j) {
+        m.For[j] = ForJ[j];
+        m.Back[j] = BackJ[j];
+    }
     m.gemm = gws;
     m.gemm_bytes = gws_bytes;
     m.counters = counters;
@@ -562,6 +617,10 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
     }
 
     // ---------------------------------------------------------------- backward (brnnet.py:188-243)
+    // Per temporal layer from the top: the delta GEMM without a mask, the BPTT sweep into pair j % 2, the recurrent
+    // weight-gradient pair on the side stream, add2.  Layer j - 2 writes the pair layer j used: its sweep waits for
+    // ev_pair, recorded on the side stream behind the last read of that pair (the recurrent weight gradients; for a
+    // uni-directional layer the weight gradient of the map above, whose delta the pair is).
     const bool overlap = (tl > 0);     // layers i >= tl: dW/db on the side stream, delta chain + BPTT on the main one
     const bool dp = (h->comm != nullptr) && comm_world(h->comm) > 1;
     if (overlap) TRY(ensure_side_stream(h));
@@ -570,7 +629,8 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
     for (int i = N; i >= 0; --i) {
         const float *Xi = (i == 0) ? feats : Act(i);
         const int n_out = sz[i + 1], n_in = sz[i];
-        float *dcur = (uni && tl > 0 && i + 1 == tl) ? dFor : dbuf(i + 1);   // rnnet.py:162-177: the BPTT result is the delta
+        // rnnet.py:162-177: the BPTT result of a uni-directional layer is the delta
+        float *dcur = (uni && temporal(i + 1)) ? dF[(i + 1 - tl) % 2] : dbuf(i + 1);
         const bool on_side = overlap && i >= tl;
         cudaStream_t sw = on_side ? h->side : st;
         if (on_side) {     // dcur is complete on the main stream here
@@ -606,6 +666,8 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
             else colsum_stage2<true><<<(n_out + 127) / 128, 128, 0, sw>>>(part, nblk, n_out, G(2 * i + 1));
             CTCB_LAUNCH_CHECK();
         }
+        if (uni && temporal(i + 1) && i + 1 - tl >= 2)     // the last read of the pair of uni-directional layer i + 1
+            CTCB_CUDA_CHECK(cudaEventRecord(h->ev_pair[(i + 1 - tl) % 2], h->side));
         if (dp && last && on_side && i == tl) {
             // every gradient tensor of the layers >= tl is now queued on the side stream: sum that contiguous range over
             // the ranks there, next to the BPTT sweep on the main stream
@@ -616,13 +678,17 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
         if (i > 0) {
             float *doth = dbuf(i);
             // delta <- delta . W, with the ReLU mask sign(hActs[i]) fused (brnnet.py:203-204,235-237)
-            const float *mask = (i != tl) ? Xi : nullptr;
+            const float *mask = temporal(i) ? nullptr : Xi;
             {
             ProfScope ps("gemm_delta", st);
             TRY(ctcb_gemm_f32(0, 0, (int)R, n_in, n_out, 1.f, dcur, n_out, P(2 * i), n_in, 0.f, doth, n_in,
                               nullptr, 0, mask, gws, gws_bytes, st));
             }
-            if (i == tl) {   // brnnet.py:207-233
+            if (temporal(i)) {   // brnnet.py:207-233
+                const int j = i - tl, p = j % 2, iWtf = rec_index(&c, j), iWtb = iWtf + 2;
+                float *dFor = dF[p], *dBack = dB[p], *For = ForJ[j], *Back = BackJ[j];
+                if (j + 2 < nt)      // layer j + 2 used this pair
+                    CTCB_CUDA_CHECK(cudaStreamWaitEvent(st, h->ev_pair[p], 0));
                 {
                 ProfScope ps("sweep_bptt", st);
                 TRY(run_sweep(1, Tmax, B, H, T_per_utt, doth, P(iWtf), uni ? nullptr : P(iWtb), dFor, dBack, For, Back,
@@ -648,7 +714,10 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
                     if (!uni) CTCB_CUDA_CHECK(cudaMemsetAsync(G(iWtb), 0, sizeof(float) * H * H, h->side));
                 }
                 }
-                if (!uni) TRY(run_add2(dFor, dBack, doth, R * H, st));
+                if (!uni) {
+                    if (j >= 2) CTCB_CUDA_CHECK(cudaEventRecord(h->ev_pair[p], h->side));
+                    TRY(run_add2(dFor, dBack, doth, R * H, st));
+                }
             }
         }
     }
@@ -656,9 +725,10 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
         CTCB_CUDA_CHECK(cudaEventRecord(h->ev_side, h->side));
         CTCB_CUDA_CHECK(cudaStreamWaitEvent(st, h->ev_side, 0));
     }
-    if (tl) {   // the `dummy` biases never receive gradient
+    for (int j = 0; j < nt; ++j) {   // the `dummy` biases never receive gradient
+        const int iWtf = rec_index(&c, j);
         CTCB_CUDA_CHECK(cudaMemsetAsync(G(iWtf + 1), 0, sizeof(float), st));
-        if (!uni) CTCB_CUDA_CHECK(cudaMemsetAsync(G(iWtb + 1), 0, sizeof(float), st));
+        if (!uni) CTCB_CUDA_CHECK(cudaMemsetAsync(G(iWtf + 3), 0, sizeof(float), st));
     }
 
     if (stats_out) {     // after both sweeps, so that the tail carries the error flag of either
@@ -749,7 +819,8 @@ extern "C" size_t ctcb_brnn_sweep_workspace_bytes(int H, int B) { return 4096 + 
 
 // Test / diagnostic hook: where, inside the workspace, the activations of the LAST ctcb_brnn_cost_and_grad call lie
 // (time-major [Tmax][B][n] with that call's B and Tmax).  what = 0: output of affine map `layer` (1..numLayers+1; the
-// temporal layer's entry holds For + Back, the last one the logits), 1: For, 2: Back (temporal layer only).
+// temporal layer's entry holds For + Back, the last one the logits), 1: For, 2: Back (temporal layer only; with
+// several, `layer` says which).
 extern "C" int ctcb_brnn_activation_offset(const ctcb_brnn_config *cfg, int what, int layer, size_t *offset, int32_t *width) {
     if (!valid_cfg(cfg) || !offset) return set_error(CTCB_EINVAL, "ctcb_brnn_activation_offset: bad arguments");
     const WsLayout w = ws_layout(cfg);
@@ -761,8 +832,18 @@ extern "C" int ctcb_brnn_activation_offset(const ctcb_brnn_config *cfg, int what
         if (width) *width = sizes[layer];
         return CTCB_OK;
     }
-    if ((what == 1 || what == 2) && eff_tl(cfg)) {
+    const int nt = eff_nt(cfg);
+    if ((what == 1 || what == 2) && nt == 1) {     // one temporal layer: `layer` is ignored
         *offset = (what == 1) ? w.For : w.Back;
+        if (width) *width = cfg->layerSize;
+        return CTCB_OK;
+    }
+    if ((what == 1 || (what == 2 && !cfg->unidirectional)) && nt > 1) {
+        const int j = layer - eff_tl(cfg);
+        if (j < 0 || j >= nt)
+            return set_error(CTCB_EINVAL, "ctcb_brnn_activation_offset: layer %d is not one of the temporal layers %d..%d",
+                             layer, eff_tl(cfg), eff_tl(cfg) + nt - 1);
+        *offset = (what == 1) ? w.ForJ[j] : w.BackJ[j];
         if (width) *width = cfg->layerSize;
         return CTCB_OK;
     }

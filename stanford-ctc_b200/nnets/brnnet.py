@@ -14,6 +14,7 @@ flat fp32 device buffer (`params` / `grads`), so the optimiser and the NCCL all-
 single contiguous vector.  New, additive surface for the minibatch/data-parallel path:
 
     NNet(..., maxUtts=B, maxLabels=L)        capacity for B utterances per call (micro-batch)
+    NNet(..., numTemporal=k)                 k stacked temporal layers temporalLayer .. temporalLayer+k-1
     costAndGradBatch(datas, labelss)         -> (costs[B], grad, skips[B])   host arrays in; more than maxUtts
                                                 utterances are accumulated over micro-batches
     costAndGradDevice(batch, first, last)    -> no host sync; see DeviceBatch
@@ -120,7 +121,7 @@ class NNet:
 
     def __init__(self, inputDim, outputDim, layerSize, numLayers, maxBatch,
                  train=True, temporalLayer=-1, reg=0.0, maxUtts=1, maxLabels=None,
-                 allowTopTemporal=False, device=None, unidirectional=False):
+                 allowTopTemporal=False, device=None, unidirectional=False, numTemporal=1):
         torch = _ctcb.require_cuda()
         self._torch = torch
         self.dev = torch.device("cuda", torch.cuda.current_device() if device is None else device)
@@ -150,11 +151,21 @@ class NNet:
         else:
             self.temporalLayer = temporalLayer
         self.maxAct = 20.0
+        # numTemporal = k stacks k temporal layers, temporalLayer .. temporalLayer+k-1, each with its own recurrent
+        # matrices (0 and 1: one layer, the reference's net).  A stack has to fit where one temporal layer may go.
+        if numTemporal < 0:
+            raise ValueError("numTemporal=%d must be >= 0" % numTemporal)
+        if numTemporal > 1 and (temporalLayer <= 0 or temporalLayer + numTemporal - 1 >= hi):
+            raise ValueError("numTemporal=%d from temporalLayer=%d does not fit in hidden layers 1..%d%s"
+                             % (numTemporal, temporalLayer, hi - 1,
+                                "" if allowTopTemporal else " (allowTopTemporal lets it end at numLayers)"))
+        self.numTemporal = max(1, numTemporal) if self.temporalLayer > 0 else 0
 
         # unidirectional: the single forward-in-time recurrence of nnets/rnnet.py (used by nnets.rnnet.NNet)
         self.unidirectional = bool(unidirectional)
         self._cfg = BrnnConfig(inputDim, outputDim, layerSize, numLayers, max(self.temporalLayer, 0), maxBatch,
-                               maxUtts, self.maxLabels, float(reg), float(self.maxAct), int(self.unidirectional))
+                               maxUtts, self.maxLabels, float(reg), float(self.maxAct), int(self.unidirectional),
+                               self.numTemporal)
         self._h = ctypes.c_void_p()
         check(lib.ctcb_brnn_create(ctypes.byref(self._cfg), ctypes.byref(self._h)))
         self.stack = None
@@ -179,13 +190,14 @@ class NNet:
 
     def initParams(self):
         """Initialize parameters using 6/sqrt(fanin+fanout) -- same shapes and the same np.random draw
-        order as brnnet.py:38-41 (layer stack) and :66-70 (Wtf then Wtb)."""
+        order as brnnet.py:38-41 (layer stack) and :66-70 (Wtf then Wtb).  The recurrent matrices of further
+        stacked temporal layers are drawn after those, layer by layer, at the same scale."""
         torch = self._torch
         sizes = [self.inputDim] + self.layerSizes + [self.outputDim]
         scales = [np.sqrt(6) / np.sqrt(n + m) for n, m in zip(sizes[:-1], sizes[1:])]
         host = [[np.random.rand(m, n) * 2 * s - s, np.zeros((m, 1))]
                 for n, m, s in zip(sizes[:-1], sizes[1:], scales)]
-        if self.temporalLayer > 0:
+        for _ in range(self.numTemporal):
             scale = np.sqrt(6) / np.sqrt(self.layerSize * 2)
             wtf = 2 * scale * np.random.rand(self.layerSize, self.layerSize) - scale
             host.append([wtf, np.zeros((1, 1))])

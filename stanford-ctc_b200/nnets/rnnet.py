@@ -8,7 +8,7 @@ recurrent net, computed by libctcb200 on an H100.
 Same kernels as nnets.brnnet with one direction switched off (ctcb_brnn_config.unidirectional = 1):
 stack = [[W1,b1] ... [Wout,bout], [Wt, dummy]] (rnnet.py:38-65), temporal layer
 h[:,t] = clip(pre[:,t] + Wt.h[:,t-1], 0, 20) (rnnet.py:112-116), BPTT rnnet.py:162-177.  There is no L2
-term in this class.  initParams, updateParams, toFile, fromFile, check_grad and the minibatch additions
+term in this class.  numTemporal=k stacks k such layers (stack ends with [Wt_1, dummy] .. [Wt_k, dummy]).  initParams, updateParams, toFile, fromFile, check_grad and the minibatch additions
 (maxUtts, costAndGradBatch, costAndGradDevice) are inherited.
 """
 import numpy as np
@@ -20,10 +20,12 @@ from nnets import brnnet
 class NNet(brnnet.NNet):
 
     def __init__(self, inputDim, outputDim, layerSize, numLayers, maxBatch,
-                 train=True, temporalLayer=-1, maxUtts=1, maxLabels=None, device=None):
+                 train=True, temporalLayer=-1, maxUtts=1, maxLabels=None, device=None, numTemporal=1,
+                 allowTopTemporal=False):
         brnnet.NNet.__init__(self, inputDim, outputDim, layerSize, numLayers, maxBatch, train=train,
                              temporalLayer=temporalLayer, reg=0.0, maxUtts=maxUtts, maxLabels=maxLabels,
-                             device=device, unidirectional=True)
+                             allowTopTemporal=allowTopTemporal, device=device, unidirectional=True,
+                             numTemporal=numTemporal)
 
     def costAndGrad(self, data, labels=None):
         if not self.train:

@@ -7,7 +7,7 @@ last_cost, sentinel, train.log), resume through --cfg_file with the step size re
 (runNNet.py:143-166), the fixed seeds 33 (:113-115) and CUDA_DEVICE device selection (:117-120).
 The implementation is organised differently: a declarative flag table, one RunDir helper that owns the
 side files, and separate train/evaluate phases.  Site paths of run_cfg.py / decoder_config.py became
-flags (--runDir, --outDir); new flags: --batchSize, --maxUtts, --maxLabels, --quiet.  Under torchrun the same
+flags (--runDir, --outDir); new flags: --numTemporal, --batchSize, --maxUtts, --maxLabels, --quiet.  Under torchrun the same
 script trains data-parallel (one process per GPU, one NCCL all-reduce per step).
 """
 import argparse
@@ -43,6 +43,8 @@ FLAGS = [
     ("save_every", int, 10, "checkpoint every this many data files"),
     ("run_desc", str, "", "free-text description stored in cfg.json"),
     # additions
+    ("numTemporal", int, 1, "stacked temporal layers: layers temporalLayer .. temporalLayer+numTemporal-1 are all "
+                            "recurrent (1 = the reference's single temporal layer)"),
     ("batchSize", int, 1, "utterances per optimisation step (1 = the reference schedule)"),
     ("maxUtts", int, 0, "utterances per micro-batch per GPU: a larger shard accumulates its gradient over several "
                         "micro-batches (0 = the whole shard, batchSize / number of GPUs rounded up); with --test, "
@@ -72,6 +74,15 @@ def run_config(cli):
     for name, _, default, _ in FLAGS:                 # configs written by older runs lack the new keys
         cfg.setdefault(name, default)
     return cfg
+
+
+def trained_config(cfg_file):
+    """The stored configuration of a trained model, with the defaults of keys an older run did not record (a model
+    from before --numTemporal has one temporal layer)."""
+    cfg = load_config(cfg_file)
+    for name, _, default, _ in FLAGS:
+        cfg.setdefault(name, default)
+    return CfgStruct(**cfg)
 
 
 def utterance_capacity(opts, world):
@@ -176,7 +187,7 @@ def run(args=None):
 def _train(opts, cfg, run_dir, log, rank, world):
     loader = dl.DataLoader(opts.dataDir, opts.rawDim, opts.inputDim, opts.alisDir or opts.dataDir)
     net = rnnet.NNet(opts.inputDim, opts.outputDim, opts.layerSize, opts.numLayers, opts.maxUttLen,
-                     temporalLayer=opts.temporalLayer, reg=opts.reg,
+                     temporalLayer=opts.temporalLayer, reg=opts.reg, numTemporal=opts.numTemporal,
                      maxUtts=utterance_capacity(opts, world),
                      maxLabels=min(opts.maxLabels, opts.maxUttLen))
     net.initParams()
@@ -236,10 +247,11 @@ def test(opts, rank=0, world=1):
     (runNNet.py:208-237, analysis-utils/writeLikelihoods.py).  --maxUtts utterances per forward call (0: one, the
     reference's loop); rank `rank` of `world` processes (run() passes them under torchrun) writes its own share of
     the files (parallel.rank_files)."""
-    trained = CfgStruct(**load_config(opts.cfg_file))
+    trained = trained_config(opts.cfg_file)
     logging.getLogger().info("Running on %s" % get_hostname())
     net = rnnet.NNet(trained.inputDim, trained.outputDim, trained.layerSize, trained.numLayers, trained.maxUttLen,
-                     temporalLayer=trained.temporalLayer, train=False, maxUtts=max(1, opts.maxUtts))
+                     temporalLayer=trained.temporalLayer, train=False, maxUtts=max(1, opts.maxUtts),
+                     numTemporal=trained.numTemporal)
     net.initParams()
     with open(trained.in_file, "rb") as fid:
         pickle.load(fid)                              # optimiser state: not needed here
