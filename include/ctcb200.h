@@ -53,7 +53,10 @@ int ctcb_profile_report(char *buf, size_t cap);
  *             (ctc_fast.pyx:139-145).  Zero for skipped utterances.
  * nll_out   : float32[B]  -log p(labels | acts)     (ctc_fast.pyx:152)
  * skip_out  : int32[B]    1 where a frame normaliser was 0 (ctc_fast.pyx:147-149)
- * workspace : ctcb_ctc_workspace_bytes(B, Tmax, max_labels) bytes of device scratch
+ * workspace : ctcb_ctc_workspace_bytes(B, Tmax, max_labels) bytes of device scratch.  That size never decreases with B,
+ *             Tmax or max_labels, so a buffer sized for the largest call serves every smaller one: one fp64 trellis
+ *             plane of Tmax x 64P doubles (P = pairs per lane, 1..16 by max_labels) per utterance, two per utterance
+ *             for the first 256 (the frame-parallel kernel spills alpha and beta), i.e. max(B, 2 min(B, 256)) planes.
  */
 size_t ctcb_ctc_workspace_bytes(int B, int Tmax, int max_labels);
 int ctcb_ctc_loss_grad_f32(const float *acts, int is_prob, int64_t utt_stride, int64_t frame_stride,
@@ -118,8 +121,21 @@ int ctcb_debug_set_gemm_copy(int on);
  * 0 = automatic (by batch size), 1 = one warp per utterance with the trellis spilled to the workspace, 2 = two warps per
  * utterance meeting in the middle, 3 = recurrences on two warps + frame-parallel gradient (at most 256 utterances),
  * 4 = one warp per utterance with on-chip checkpoints (at most 127 labels).  Same as the environment variable
- * CTCB_CTC=warp|pair|par|ckpt, which is read on first use.  Results are identical whichever is chosen. */
+ * CTCB_CTC=warp|pair|par|ckpt, which is read on first use.  A forced organisation that cannot run these arguments
+ * (par beyond 256 utterances, par / pair / ckpt with K too large for their tiles, ckpt beyond 127 labels) makes
+ * ctcb_ctc_loss_grad_f32 return CTCB_EINVAL; it never runs another one.  Probability input (is_prob = 1) gives the same
+ * bits whichever organisation runs.  Logits give the same bits within a tile height -- 16 frames: par, pair, and warp
+ * below 16 x SMs utterances or beyond 63 labels; 8 frames: ckpt, and warp otherwise -- but the fused softmax sums a
+ * row's normaliser in another order in the two, so across them the gradient and the loss differ in the last bits. */
 int ctcb_debug_set_ctc_kernel(int shape);
+/* The plan ctcb_ctc_loss_grad_f32 runs for these arguments under the organisation in effect (CTCB_CTC /
+ * ctcb_debug_set_ctc_kernel) and the device's SM count.  acts and grad_out are inspected only for their alignment.
+ * out (HOST, 8 int32): {kernel: 0 par / 1 pair / 2 ckpt / 3 warp, P (pairs per lane), frames per time tile,
+ * activation tiles per warp, warps per CTA (par: the warps of its gradient phase), vec2 (8-byte tile copies and
+ * stores), shared row pitch in floats, dynamic shared memory per CTA in KiB rounded up}.  Returns the error the call
+ * itself would return for these sizes (e.g. K too large for the tile), assuming valid pointers, blank and workspace. */
+int ctcb_debug_ctc_plan(int B, int Tmax, int K, int max_labels, const float *acts, const float *grad_out,
+                        int64_t utt_stride, int64_t frame_stride, int32_t *out);
 
 /* Diagnostic (CTCB_GEMM_TRACE=1): SM clock stamps of CTA (0,0,0) of the last tensor-core GEMM, HOST buffer of 64 x 8
  * uint64 = per k-block {TMA issued, tile landed, low halves written, MMA thread saw it, MMAs issued, -, -, -}. */

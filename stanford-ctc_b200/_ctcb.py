@@ -55,6 +55,8 @@ _PROTOS = {
     "ctcb_debug_set_gemm_copy": (c_int, [c_int]),
     "ctcb_debug_gemm_trace": (c_int, [c_vp]),
     "ctcb_debug_set_ctc_kernel": (c_int, [c_int]),
+    "ctcb_debug_ctc_plan": (c_int, [c_int, c_int, c_int, c_int, c_vp, c_vp, c_i64, c_i64,
+                                    ctypes.POINTER(ctypes.c_int32)]),
     "ctcb_brnn_param_count": (c_i64, [ctypes.POINTER(BrnnConfig)]),
     "ctcb_brnn_num_tensors": (c_int, [ctypes.POINTER(BrnnConfig)]),
     "ctcb_brnn_tensor_info": (c_int, [ctypes.POINTER(BrnnConfig), c_int, ctypes.POINTER(c_i64),

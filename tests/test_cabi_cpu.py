@@ -80,6 +80,26 @@ def test_error_reporting():
     assert _ctcb.lib.ctcb_ctc_workspace_bytes(1000, 100, 30) == 1000 * (100 * 64 + 8) * 8
 
 
+def test_ctc_workspace_never_shrinks_as_the_batch_grows():
+    """A buffer sized once for the largest call (the BRNN sizes its CTC area for maxB) must serve every smaller call:
+    the size is monotone in B, Tmax and the label count, and covers two trellis planes for each of the first 256
+    utterances (the frame-parallel kernel) and one for every utterance."""
+    import _ctcb
+    ws = _ctcb.lib.ctcb_ctc_workspace_bytes
+    for T, L in ((16, 5), (100, 30), (5000, 300)):
+        sizes = [ws(B, T, L) for B in range(1, 1025)]
+        assert all(a <= b for a, b in zip(sizes, sizes[1:])), (T, L)
+        plane = ws(1, T, L) // 2
+        assert all(s >= plane * max(B, 2 * min(B, 256)) for B, s in enumerate(sizes, 1))
+    for B in (1, 200, 256, 260, 1000):
+        sizes = [ws(B, T, 30) for T in range(1, 400)]
+        assert all(a <= b for a, b in zip(sizes, sizes[1:])), B
+        sizes = [ws(B, 100, L) for L in range(0, 512)]
+        assert all(a <= b for a, b in zip(sizes, sizes[1:])), B
+    # the C3-like net of maxB 260, maxT 16, 5 labels: room for a 200-utterance call's 400 planes of 16 x 64 + 2 doubles
+    assert ws(260, 16, 5) >= ws(200, 16, 5) == 400 * (16 * 64 + 2) * 8
+
+
 def test_product_never_imports_the_oracle():
     """The product path must not route through oracle/ (or any CPU fallback)."""
     pkg = os.path.join(ROOT, "stanford-ctc_b200")

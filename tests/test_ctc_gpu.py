@@ -4,6 +4,8 @@ ctc_fast.pyx and (b) the oracle run live on the same inputs.
 
 Tolerance (BASELINE.json north_star / SURVEY.md 8c): |nll - ref| / |ref| <= 1e-4 and
 ||g - g_ref||_F / ||g_ref||_F <= 1e-4 in fp32, skip flags equal."""
+import os
+
 import numpy as np
 import pytest
 
@@ -26,6 +28,11 @@ def _gpu_single(torch, probs, seq, is_prob=True):
     lab = torch.from_numpy(seq if seq.size else np.zeros(1, np.int32)).cuda()
     off = torch.tensor([0, seq.shape[0]], dtype=torch.int32).cuda()
     tl = torch.tensor([T], dtype=torch.int32).cuda()
+    if os.environ.get("CTCB_CTC", "").startswith("c") and seq.shape[0] > 127:
+        # the checkpoint kernel has no build beyond 127 labels: forced, the call is an error, never another kernel
+        with pytest.raises(ValueError, match="ckpt"):
+            ctc_fast.ctc_loss_batch(acts, tl, lab, off, seq.shape[0], is_prob=is_prob)
+        pytest.skip("CTCB_CTC=ckpt refuses %d labels" % seq.shape[0])
     nll, grad, skip = ctc_fast.ctc_loss_batch(acts, tl, lab, off, seq.shape[0], is_prob=is_prob)
     return float(nll.item()), grad.view(T, K).cpu().numpy().T.astype(np.float64), bool(skip.item())
 
@@ -167,24 +174,37 @@ def test_best_path_matches_reference_semantics(cuda):
     assert ctc_fast.decode_best_path(np.asfortranarray(q)) == ([3, 3, 5], [2, 4, 7])
 
 
-@pytest.mark.parametrize("shape", ["warp", "pair", "ckpt"])
-def test_other_kernel_shapes_when_forced(shape, cuda):
-    """Small batches take the three-phase latency kernel (recurrences on two warps, gradient on all warps); CTCB_CTC=warp
-    forces the one-warp-per-utterance kernel that spills the trellis (large batches, long label sequences), CTCB_CTC=ckpt
-    the one-warp kernel that checkpoints and recomputes it on chip (large batches, up to 127 labels; longer ones fall
-    through to the spilling kernel), CTCB_CTC=pair the two-warp meet-in-the-middle kernel (mid-sized batches), through the
-    same golden / edge cases."""
-    import os
+def _run_forced(shape):
+    """The golden / edge cases of this file in a fresh process with CTCB_CTC=shape (read once per process); returns
+    its pytest output."""
     import subprocess
     import sys
     here = os.path.dirname(os.path.abspath(__file__))
     root = os.path.dirname(here)
     code = ("import os,sys; sys.path[:0]=[%r,%r,%r]; import pytest; "
-            "sys.exit(pytest.main(['-q','-p','no:cacheprovider','-k','golden_cases or ragged_batch or pairs_per_lane or fused_softmax or tile_boundaries or full_size', %r]))"
+            "sys.exit(pytest.main(['-q','-rs','-p','no:cacheprovider','-k','golden_cases or ragged_batch or pairs_per_lane or fused_softmax or tile_boundaries or full_size', %r]))"
             % (root, os.path.join(root, "stanford-ctc_b200"), here, os.path.abspath(__file__)))
     env = dict(os.environ, CTCB_CTC=shape)
     r = subprocess.run([sys.executable, "-c", code], env=env, capture_output=True, text=True, timeout=600)
     assert r.returncode == 0, r.stdout[-1500:] + r.stderr[-500:]
+    return r.stdout
+
+
+@pytest.mark.parametrize("shape", ["warp", "pair"])
+def test_other_kernel_shapes_when_forced(shape, cuda):
+    """Small batches take the three-phase latency kernel (recurrences on two warps, gradient on all warps); CTCB_CTC=warp
+    forces the one-warp-per-utterance kernel that spills the trellis (large batches, long label sequences), CTCB_CTC=pair
+    the two-warp meet-in-the-middle kernel (mid-sized batches), through the same golden / edge cases."""
+    _run_forced(shape)
+
+
+def test_checkpoint_kernel_when_forced(cuda):
+    """CTCB_CTC=ckpt forces the one-warp kernel that checkpoints the trellis and recomputes it on chip (large batches) through
+    the same golden / edge cases.  It has no build beyond 127 labels: those cases must be refused with CTCB_EINVAL, never
+    run on another kernel."""
+    out = _run_forced("ckpt")
+    # 3 golden cases and 5 label counts have more than 127 labels; each is skipped after its refusal was checked
+    assert " 8 skipped" in out and "CTCB_CTC=ckpt refuses" in out, out[-1500:]
 
 
 @pytest.mark.parametrize("T", [1, 3, 7, 8, 9, 16, 17, 31, 32, 33, 47, 200])
