@@ -106,22 +106,27 @@ int ctcb_gemm_pair_f32(int transA, int transB, int M, int N, int K, float alpha,
                        const float *A0, const float *A1, int64_t lda, const float *B0, const float *B1, int64_t ldb,
                        float beta, float *C0, float *C1, int64_t ldc, void *workspace, size_t ws_bytes, void *stream);
 /* The plan ctcb_gemm_f32 (problems = 1) or ctcb_gemm_pair_f32 (problems = 2) runs for these arguments under the
- * environment knobs in effect (INTEGRATION.md section 4), assuming a large enough workspace.  A and B are only
+ * knobs in effect (INTEGRATION.md section 4), assuming a large enough workspace.  A and B are only
  * inspected for their alignment.  out (HOST, 8 int32):
  *   {kernel: 0 FFMA / 1 tensor core, BN (output tile width), ring stages, K splits, CTAs per launch,
  *    A path, B path: 0 read in place K-major / 1 read in place MN-major, transposed in shared memory / 2 copied into
  *    the workspace first,  problems per launch (2: the pair shares one launch)}.  The FFMA kernel reports {0, .., 0, 1}. */
 int ctcb_debug_gemm_plan(int transA, int transB, int M, int N, int K, const float *A, int64_t lda,
                          const float *B, int64_t ldb, int problems, int32_t *out);
-/* Measurement: 1 sends MN-major tensor-core operands through a transposed copy in the workspace, as the environment
- * variable CTCB_GEMM_TC_COPY=1 does; 0 reads them in place (the default).  Results are the same either way. */
-int ctcb_debug_set_gemm_copy(int on);
+
+/* Debug hook: set one planner knob of INTEGRATION.md section 4 in this process, e.g. ("CTCB_CTC", "ckpt") or
+ * ("CTCB_SWEEP_TC_CS", "2").  value uses the environment's syntax; value == NULL restores what the environment said at
+ * the library's first use, or the default.  An unknown name or a value outside the documented set returns CTCB_EINVAL
+ * and changes nothing.  Do not call it while other threads make library calls.  A change takes effect at the next
+ * planning call.  Workspace sizes, and the forward layout a net handle caches, reflect the knobs in effect when they
+ * were computed (ctcb_gemm_workspace_bytes depends on CTCB_GEMM): set knobs before sizing workspaces or creating nets. */
+int ctcb_debug_set_knob(const char *name, const char *value);
 
 /* Diagnostic / measurement: force the CTC kernel organisation used by ctcb_ctc_loss_grad_f32 (and the BRNN step).
  * 0 = automatic (by batch size), 1 = one warp per utterance with the trellis spilled to the workspace, 2 = two warps per
  * utterance meeting in the middle, 3 = recurrences on two warps + frame-parallel gradient (at most 256 utterances),
- * 4 = one warp per utterance with on-chip checkpoints (at most 127 labels).  Same as the environment variable
- * CTCB_CTC=warp|pair|par|ckpt, which is read on first use.  A forced organisation that cannot run these arguments
+ * 4 = one warp per utterance with on-chip checkpoints (at most 127 labels).  Same as ctcb_debug_set_knob("CTCB_CTC",
+ * "auto" | "warp" | "pair" | "par" | "ckpt").  A forced organisation that cannot run these arguments
  * (par beyond 256 utterances, par / pair / ckpt with K too large for their tiles, ckpt beyond 127 labels) makes
  * ctcb_ctc_loss_grad_f32 return CTCB_EINVAL; it never runs another one.  Probability input (is_prob = 1) gives the same
  * bits whichever organisation runs.  Logits give the same bits within a tile height -- 16 frames: par, pair, and warp
@@ -263,7 +268,7 @@ int ctcb_brnn_sweep_f32(int mode, int T, int B, int H, const int32_t *T_per_utt,
 /* 1 when the recurrences of a (layerSize H, B utterances, bi-directional) step run on the tensor-core kernel. */
 int ctcb_sweep_uses_tensor_cores(int H, int B);
 /* The plan ctcb_brnn_sweep_f32 launches for (H, B, ndir = 2 bi-directional / 1 forward in time only) on the current
- * device, under the environment knobs in effect (INTEGRATION.md section 4).  out (HOST, 8 int32):
+ * device, under the knobs in effect (INTEGRATION.md section 4).  out (HOST, 8 int32):
  *   {kernel: 0 generic / 1 cluster / 2 tensor-core, KI (H / 32 with register-resident weights, else 0),
  *    CS (tensor-core: K-slices per cluster; cluster: CTAs per cluster; generic: 0),
  *    NB (cluster: utterances per cluster) or NS (tensor-core: utterance splits) or the generic kernel's partitions,

@@ -52,7 +52,7 @@ _PROTOS = {
                                    c_f32, c_vp, c_vp, c_i64, c_vp, c_sz, c_vp]),
     "ctcb_debug_gemm_plan": (c_int, [c_int, c_int, c_int, c_int, c_int, c_vp, c_i64, c_vp, c_i64, c_int,
                                      ctypes.POINTER(ctypes.c_int32)]),
-    "ctcb_debug_set_gemm_copy": (c_int, [c_int]),
+    "ctcb_debug_set_knob": (c_int, [ctypes.c_char_p, ctypes.c_char_p]),
     "ctcb_debug_gemm_trace": (c_int, [c_vp]),
     "ctcb_debug_set_ctc_kernel": (c_int, [c_int]),
     "ctcb_debug_ctc_plan": (c_int, [c_int, c_int, c_int, c_int, c_vp, c_vp, c_i64, c_i64,

@@ -1,8 +1,10 @@
-// common.cu -- error string, launch counter, device queries.
+// common.cu -- error string, launch counter, device queries, planner knobs.
 #include "common.cuh"
 #include <stdarg.h>
+#include <stdlib.h>
 #include <string.h>
 #include <map>
+#include <mutex>
 #include <new>
 #include <string>
 #include <vector>
@@ -28,6 +30,43 @@ int num_sms() {
     }
     return n;
 }
+
+// The documented values of each knob, in the order of enum Knob: the string values[v] sets the value v.  A value the
+// environment gives that is not listed here leaves the default in effect.
+struct KnobDef { const char *name; int dflt; const char *values[9]; };
+static const KnobDef KNOBS[KNOB_COUNT] = {
+    {"CTCB_GEMM", 0, {nullptr, "simt"}},
+    {"CTCB_GEMM_TC_COPY", 0, {"0", "1"}},
+    {"CTCB_GEMM_TRACE", 0, {nullptr, "1"}},
+    {"CTCB_SWEEP", 0, {nullptr, "barrier"}},
+    {"CTCB_SWEEP_NB", 0, {nullptr, "1", "2", "3", "4", "5", "6", "7", "8"}},
+    {"CTCB_SWEEP_TC", 1, {"0", "1", "2"}},
+    {"CTCB_SWEEP_TC_CS", 4, {nullptr, "1", "2", nullptr, "4"}},
+    {"CTCB_SWEEP_TC_COOP", 1, {"0"}},
+    {"CTCB_SWEEP_TRACE", 0, {nullptr, "1"}},
+    {"CTCB_CTC", 0, {"auto", "warp", "pair", "par", "ckpt"}},
+};
+static int g_knob_initial[KNOB_COUNT], g_knob[KNOB_COUNT];     // what the environment said, what is in effect
+static std::once_flag g_knob_once;
+
+static int parse_knob(const KnobDef &d, const char *s) {
+    for (int v = 0; v < 9; ++v)
+        if (d.values[v] && strcmp(d.values[v], s) == 0) return v;
+    return -1;
+}
+
+static int *knob_table() {
+    std::call_once(g_knob_once, [] {
+        for (int k = 0; k < KNOB_COUNT; ++k) {
+            const char *e = getenv(KNOBS[k].name);
+            const int v = e ? parse_knob(KNOBS[k], e) : -1;
+            g_knob_initial[k] = g_knob[k] = v < 0 ? KNOBS[k].dflt : v;
+        }
+    });
+    return g_knob;
+}
+
+int knob(Knob k) { return knob_table()[k]; }
 
 static bool g_prof_on = false;
 struct ProfRec { std::string name; cudaEvent_t a, b; };
@@ -83,6 +122,26 @@ extern "C" int ctcb_profile_report(char *buf, size_t cap) {
 extern "C" int ctcb_version(void) { return 100; }
 extern "C" const char *ctcb_last_error(void) { return ctcb::g_last_error; }
 extern "C" uint64_t ctcb_launch_count(void) { return ctcb::g_launch_count.load(); }
+
+extern "C" int ctcb_debug_set_knob(const char *name, const char *value) {
+    using namespace ctcb;
+    int *table = knob_table();
+    for (int k = 0; name && k < KNOB_COUNT; ++k) {
+        if (strcmp(name, KNOBS[k].name) != 0) continue;
+        const int v = value ? parse_knob(KNOBS[k], value) : g_knob_initial[k];
+        if (v < 0) return set_error(CTCB_EINVAL, "ctcb_debug_set_knob: \"%s\" is not a value of %s", value, name);
+        table[k] = v;
+        return CTCB_OK;
+    }
+    return set_error(CTCB_EINVAL, "ctcb_debug_set_knob: unknown knob %s", name ? name : "(null)");
+}
+
+extern "C" int ctcb_debug_set_ctc_kernel(int shape) {
+    using namespace ctcb;
+    if (shape < 0 || shape > 4) return set_error(CTCB_EINVAL, "ctcb_debug_set_ctc_kernel: shape %d not in 0..4", shape);
+    knob_table()[KNOB_CTC] = shape;
+    return CTCB_OK;
+}
 
 // ---- CUDA graphs: one optimisation step (dozens of small launches on two streams) replayed as ONE graph launch ----
 struct ctcb_graph {

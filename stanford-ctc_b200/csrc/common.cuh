@@ -34,6 +34,12 @@ inline void count_launch(int n = 1) { g_launch_count.fetch_add((uint64_t)n, std:
 
 int num_sms();
 
+// Debug / measurement overrides of the planners (INTEGRATION.md section 4): one table (common.cu), filled from the
+// environment at first use and changed by ctcb_debug_set_knob.  Planners read it through knob() on every planning call.
+enum Knob { KNOB_GEMM, KNOB_GEMM_TC_COPY, KNOB_GEMM_TRACE, KNOB_SWEEP, KNOB_SWEEP_NB, KNOB_SWEEP_TC, KNOB_SWEEP_TC_CS,
+            KNOB_SWEEP_TC_COOP, KNOB_SWEEP_TRACE, KNOB_CTC, KNOB_COUNT };
+int knob(Knob k);
+
 // Optional per-phase device timing (ctcb_profile_*): CUDA events recorded on the launching stream
 // around each phase of the step; off by default so the timed benchmark region carries no events.
 struct ProfScope {

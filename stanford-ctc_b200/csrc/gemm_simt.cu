@@ -304,11 +304,8 @@ extern "C" int ctcb_gemm_f32(int transA, int transB, int M, int N, int K, float 
     splits = K > 0 ? (K + g.k_per_split - 1) / g.k_per_split : 1;
     if (splits <= 1) { g.partial = nullptr; splits = 1; }
     const bool vec = (lda % 4 == 0) && (ldb % 4 == 0) && (((uintptr_t)A | (uintptr_t)B) % 16 == 0);
-    static int vecc_env = -1;       // CTCB_GEMM_SIMT_VECC=0: scalar epilogue stores (measurement)
-    if (vecc_env < 0) { const char *e = getenv("CTCB_GEMM_SIMT_VECC"); vecc_env = e ? atoi(e) : 1; }
-    g.vecc = vecc_env && (g.partial ? (N % 4 == 0 && ((uintptr_t)g.partial) % 16 == 0)
-                                    : (ldc % 4 == 0 && ((uintptr_t)C) % 16 == 0 &&
-                                       (!mask_src || ((uintptr_t)mask_src) % 16 == 0)));
+    g.vecc = g.partial ? (N % 4 == 0 && ((uintptr_t)g.partial) % 16 == 0)
+                       : (ldc % 4 == 0 && ((uintptr_t)C) % 16 == 0 && (!mask_src || ((uintptr_t)mask_src) % 16 == 0));
     dim3 grid((N + BN - 1) / BN, (M + BM - 1) / BM, splits);
     cudaStream_t st = (cudaStream_t)stream;
 #define GO(TA, TB)                                                                  \

@@ -405,23 +405,13 @@ static int tc_choose_splits(int tiles, int nkb) {
     return splits;
 }
 
-bool gemm_tc_enabled() {
-    static int on = -1;
-    if (on < 0) {
-        const char *e = getenv("CTCB_GEMM");
-        on = (e && e[0] == 's') ? 0 : 1;     // CTCB_GEMM=simt forces the FFMA kernel everywhere
-        if (on && !get_encode()) on = 0;
-    }
-    return on == 1;
-}
-
 // Below these sizes the exact FFMA kernel is used: short contractions (K = 41 / 62) cannot amortise the tensor-core
 // pipeline.  The thresholds have not been re-tuned on H100.
+constexpr int TC_MIN_K = 128, TC_MIN_M = 32;
+
+// CTCB_GEMM=simt forces the FFMA kernel everywhere
 bool gemm_tc_eligible(int M, int N, int K) {
-    static int min_k = -1, min_m = -1;      // CTCB_GEMM_MINK / _MINM: smallest contraction length / row count that goes to the tensor cores
-    if (min_k < 0) { const char *e = getenv("CTCB_GEMM_MINK"); min_k = e ? atoi(e) : 128; }
-    if (min_m < 0) { const char *e = getenv("CTCB_GEMM_MINM"); min_m = e ? atoi(e) : 32; }
-    return gemm_tc_enabled() && M >= min_m && N >= 32 && K >= min_k;
+    return !knob(KNOB_GEMM) && get_encode() && M >= TC_MIN_M && N >= 32 && K >= TC_MIN_K;
 }
 
 // How an operand reaches the ring.
@@ -429,18 +419,12 @@ enum { TC_PATH_KMAJOR = 0,     // TMA reads the caller's K-major array
        TC_PATH_MN = 1,         // TMA reads the caller's MN-major array, the producer transposes in shared memory
        TC_PATH_COPY = 2 };     // a prep kernel re-pitches or transposes it into the workspace first
 
-// CTCB_GEMM_TC_COPY=1 (or ctcb_debug_set_gemm_copy(1)): MN-major operands go through a transposed copy in the
-// workspace instead of the in-ring transpose; same results at the same split, for comparison and timing
-static int g_copy_forced = -1;
-static bool tc_copy_forced() {
-    if (g_copy_forced < 0) { const char *e = getenv("CTCB_GEMM_TC_COPY"); g_copy_forced = (e && atoi(e) != 0) ? 1 : 0; }
-    return g_copy_forced == 1;
-}
-
-// TMA needs a 16-byte aligned base and a row pitch that is a multiple of 16 bytes
+// TMA needs a 16-byte aligned base and a row pitch that is a multiple of 16 bytes.  CTCB_GEMM_TC_COPY=1: MN-major
+// operands go through a transposed copy in the workspace instead of the in-ring transpose; same results at the same
+// split, for comparison and timing.
 static int tc_operand_path(bool mn_major, const float *p, int64_t ld) {
     if (ld % 4 != 0 || ((uintptr_t)p) % 16 != 0) return TC_PATH_COPY;
-    if (mn_major) return tc_copy_forced() ? TC_PATH_COPY : TC_PATH_MN;
+    if (mn_major) return knob(KNOB_GEMM_TC_COPY) ? TC_PATH_COPY : TC_PATH_MN;
     return TC_PATH_KMAJOR;
 }
 
@@ -519,13 +503,9 @@ static int run_tc_plan(const GemmTcPlan &p, int M, int N, int K, float alpha, co
     g.M = M; g.N = N; g.K = K; g.ldc = ldc; g.alpha = alpha; g.beta = beta; g.bias = bias; g.relu = relu; g.mask = mask_src;
     g.C[0] = C[0]; g.C[1] = p.problems > 1 ? C[1] : C[0];
     g.trace = nullptr;
-    {
-        static int tr_env = -1;
-        if (tr_env < 0) tr_env = getenv("CTCB_GEMM_TRACE") ? 1 : 0;
-        if (tr_env) {
-            if (!g_gemm_trace) cudaMalloc(&g_gemm_trace, 64 * 8 * sizeof(unsigned long long));
-            g.trace = g_gemm_trace;
-        }
+    if (knob(KNOB_GEMM_TRACE)) {
+        if (!g_gemm_trace) cudaMalloc(&g_gemm_trace, 64 * 8 * sizeof(unsigned long long));
+        g.trace = g_gemm_trace;
     }
     g.kb_per_split = p.kb_per_split;
     g.splits = p.splits;
@@ -614,11 +594,6 @@ extern "C" int ctcb_debug_gemm_plan(int transA, int transB, int M, int N, int K,
     ctcb::gemm_tc_plan(transA, transB, M, N, K, A, lda, B, ldb, problems, &p);
     const int32_t v[8] = {1, p.BN, p.stages, p.splits, p.ctas, p.a_path, p.b_path, p.problems};
     for (int i = 0; i < 8; ++i) out[i] = v[i];
-    return CTCB_OK;
-}
-
-extern "C" int ctcb_debug_set_gemm_copy(int on) {
-    ctcb::g_copy_forced = on ? 1 : 0;
     return CTCB_OK;
 }
 

@@ -237,12 +237,7 @@ int select_sweep(int H, int B, int ndir, SweepPlan *p) {
     if (H <= 0 || B <= 0 || (ndir != 1 && ndir != 2))
         return set_error(CTCB_EINVAL, "recurrent sweep: bad sizes (H=%d, B=%d, ndir=%d)", H, B, ndir);
     if (sweep_tc_plan(H, B, ndir, p)) return CTCB_OK;
-    static int force_barrier = -1;
-    if (force_barrier < 0) {
-        const char *e = getenv("CTCB_SWEEP");
-        force_barrier = (e && e[0] == 'b') ? 1 : 0;
-    }
-    if (!force_barrier && sweep_cluster_plan(H, B, ndir, p)) return CTCB_OK;
+    if (!knob(KNOB_SWEEP) && sweep_cluster_plan(H, B, ndir, p)) return CTCB_OK;
     *p = SweepPlan{};
     p->kernel = SWEEP_GENERIC;
     p->KI = (H == 128 || H == 256 || H == 512 || H == 1024) ? H / 32 : 0;

@@ -276,7 +276,6 @@ static int cluster_max_active() {
         cudaFuncSetAttribute((sweep_cluster_kernel<KI, 8>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cluster_smem_bytes(KI, 8));
         if (cudaOccupancyMaxActiveClusters(&n, (sweep_cluster_kernel<KI, 8>), &cfg) != cudaSuccess) { cudaGetLastError(); n = 0; }
         max_clusters = n;
-        if (getenv("CTCB_DEBUG")) fprintf(stderr, "[ctcb] cluster sweep H=%d: cluster=%d CTAs, max active clusters=%d\n", 32 * KI, CS, n);
     }
     return max_clusters;
 }
@@ -292,13 +291,11 @@ bool sweep_cluster_plan(int H, int B, int ndir, SweepPlan *p) {
         default: return false;
     }
     if (max_clusters < 1) return false;
-    static int nb_env = -1;   // CTCB_SWEEP_NB=1..8 forces the group size
-    if (nb_env < 0) { const char *e = getenv("CTCB_SWEEP_NB"); nb_env = e ? atoi(e) : 0; }
     // fewest utterances per cluster (= least arithmetic per SM and step) that still fits one wave of clusters
     int nb = 0;
     for (int c = 1; c <= 8; ++c)
         if (ndir * ((B + c - 1) / c) <= max_clusters) { nb = c; break; }
-    if (nb_env >= 1 && nb_env <= 8) nb = nb_env;
+    if (knob(KNOB_SWEEP_NB)) nb = knob(KNOB_SWEEP_NB);     // CTCB_SWEEP_NB=1..8 forces the group size
     if (nb == 0) return false;          // would need a second wave of clusters: the general kernel is faster
     *p = SweepPlan{};
     p->kernel = SWEEP_CLUSTER;

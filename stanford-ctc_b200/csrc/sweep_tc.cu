@@ -449,7 +449,6 @@ static int stc_max_clusters(int cs) {
         n = 0;
     }
     cached[cs] = n;
-    if (getenv("CTCB_DEBUG")) fprintf(stderr, "[ctcb] tensor-core sweep: max active clusters of %d CTAs = %d\n", cs, n);
     return n;
 }
 
@@ -460,10 +459,7 @@ static bool stc_plan_cs(int H, int B, int ndir, int cs, SweepPlan *p) {
     if ((H / cs) % STC_BK != 0) return false;
     const int maxc = stc_max_clusters(cs);
     if (maxc < ndir * MT) return false;
-    int ns_cap = maxc / (ndir * MT);
-    static int ns_env = -1;
-    if (ns_env < 0) { const char *e = getenv("CTCB_SWEEP_TC_NS"); ns_env = e ? atoi(e) : 0; }
-    if (ns_env > 0 && ns_env < ns_cap) ns_cap = ns_env;
+    const int ns_cap = maxc / (ndir * MT);
     int NS = (B + 15) / 16;                  // never more splits than 16-utterance groups
     if (NS > ns_cap) NS = ns_cap;
     if (NS < 1) NS = 1;
@@ -489,21 +485,14 @@ static bool stc_plan_cs(int H, int B, int ndir, int cs, SweepPlan *p) {
 
 static bool stc_plan(int H, int B, int ndir, SweepPlan *p) {
     if (H % 128 != 0 || H < 512 || B < 1) return false;
-    static int cs_env = -1;   // CTCB_SWEEP_TC_CS=n: the largest cluster size tried (co-residency still decides)
-    if (cs_env < 0) { const char *e = getenv("CTCB_SWEEP_TC_CS"); cs_env = e ? atoi(e) : 0; }
-    const int cs_max = (cs_env >= 4 || cs_env <= 0) ? 4 : (cs_env >= 2 ? 2 : 1);
-    for (int cs = cs_max; cs >= 1; cs >>= 1)
-        if (stc_plan_cs(H, B, ndir, cs, p)) {
-            if (getenv("CTCB_DEBUG"))
-                fprintf(stderr, "[ctcb] tensor-core sweep H=%d B=%d: clusters of %d, %d utterance split(s) of %d\n", H, B, cs, p->groups, p->np);
-            return true;
-        }
+    // CTCB_SWEEP_TC_CS: the largest cluster size tried (co-residency still decides)
+    for (int cs = knob(KNOB_SWEEP_TC_CS); cs >= 1; cs >>= 1)
+        if (stc_plan_cs(H, B, ndir, cs, p)) return true;
     return false;
 }
 
 static bool stc_enabled(int H) {
-    static int mode = -1;     // CTCB_SWEEP_TC=0 disables, =1 default (H >= 1024), =2 also H = 512
-    if (mode < 0) { const char *e = getenv("CTCB_SWEEP_TC"); mode = e ? atoi(e) : 1; }
+    const int mode = knob(KNOB_SWEEP_TC);     // 0 disables, 1 default (H >= 1024), 2 also H = 512
     if (mode == 0 || !stc_encode()) return false;
     return H >= 1024 || (mode == 2 && H >= 512);
 }
@@ -585,12 +574,8 @@ int run_sweep_tc(const SweepPlan &p, int mode, int T, int B, int H, const int32_
     a.err = counters; a.counters = counters + 16;
     a.ndir = ndir; a.MT = H / STC_BM; a.NS = p.groups; a.cs = p.cs; a.nkb = H / p.cs / STC_BK;
     a.stages = p.stages; a.stage_bytes = p.stage_bytes; a.partial_own = p.partial_own;
-    a.trace = nullptr;
-    {
-        static int trace_env = -1;
-        if (trace_env < 0) trace_env = getenv("CTCB_SWEEP_TRACE") ? 1 : 0;
-        if (trace_env) a.trace = (unsigned long long *)((char *)ws + stc_ws_stack_bytes(H) + stc_ws_ring_bytes(H, B));
-    }
+    a.trace = knob(KNOB_SWEEP_TRACE) ? (unsigned long long *)((char *)ws + stc_ws_stack_bytes(H) + stc_ws_ring_bytes(H, B))
+                                     : nullptr;
     CTCB_CUDA_CHECK(cudaMemsetAsync(a.counters, 0, sizeof(unsigned int) * (size_t)(ndir * p.groups), st));
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3(p.cs, a.MT * p.groups, ndir);
@@ -603,16 +588,14 @@ int run_sweep_tc(const SweepPlan &p, int mode, int T, int B, int H, const int32_
     attr[1].id = cudaLaunchAttributeCooperative;       // co-residency of all CTAs (they meet at the counter barrier)
     attr[1].val.cooperative = 1;
     cfg.attrs = attr;
-    static int coop = -1;     // does this driver accept cluster + cooperative together?  (CTCB_SWEEP_TC_COOP=0: plain cluster launch)
-    if (coop < 0) { const char *e = getenv("CTCB_SWEEP_TC_COOP"); if (e && atoi(e) == 0) coop = 0; }
-    if (coop != 0) {
+    static int coop = -1;     // does this driver accept cluster + cooperative together?  Learned at the first such launch
+    if (knob(KNOB_SWEEP_TC_COOP) && coop != 0) {     // CTCB_SWEEP_TC_COOP=0: plain cluster launch
         cfg.numAttrs = 2;
         cudaError_t e = stc_launch_np(p.np, &cfg, tmW, tmR, a);
         if (e == cudaSuccess) { coop = 1; count_launch(); return CTCB_OK; }
         cudaGetLastError();
         if (coop == 1) return set_error(CTCB_ECUDA, "sweep_tc: launch failed: %s", cudaGetErrorString(e));
         coop = 0;
-        if (getenv("CTCB_DEBUG")) fprintf(stderr, "[ctcb] tensor-core sweep: cooperative+cluster launch refused (%s), plain cluster launch\n", cudaGetErrorString(e));
     }
     cfg.numAttrs = 1;         // grid <= one wave of clusters by construction (stc_plan)
     CTCB_CUDA_CHECK(stc_launch_np(p.np, &cfg, tmW, tmR, a));

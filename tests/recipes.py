@@ -7,6 +7,23 @@ All follow the reference's own eyeball tests (seed 33, legacy np.random streams)
   rnnetcpu    : ctc_fast/debug-utils/rnnetcpu.py:181-193 (D=20,T=10,K=6,H=30,N=3,tl=2)
 """
 import numpy as np
+import pytest
+
+
+@pytest.fixture
+def knobs():
+    """knobs(name, value) sets a planner knob in this process (ctcb_debug_set_knob, environment syntax); every knob it
+    set is restored to what the environment said when the test ends, pass or fail.  A test module that uses it imports
+    it: `from recipes import knobs`."""
+    from _ctcb import lib, check
+    touched = set()
+
+    def set_(name, value):
+        touched.add(name)
+        check(lib.ctcb_debug_set_knob(name.encode(), value.encode()))
+    yield set_
+    for name in touched:
+        check(lib.ctcb_debug_set_knob(name.encode(), None))
 
 
 def softmax_cols(x):

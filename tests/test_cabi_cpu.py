@@ -80,6 +80,61 @@ def test_error_reporting():
     assert _ctcb.lib.ctcb_ctc_workspace_bytes(1000, 100, 30) == 1000 * (100 * 64 + 8) * 8
 
 
+# The knobs of INTEGRATION.md section 4 that ctcb_debug_set_knob takes: every documented value, and a value outside them
+KNOBS = {"CTCB_GEMM": (["simt"], "s"), "CTCB_GEMM_TC_COPY": (["0", "1"], "2"), "CTCB_GEMM_TRACE": (["1"], "0"),
+         "CTCB_SWEEP": (["barrier"], "b"), "CTCB_SWEEP_NB": ([str(n) for n in range(1, 9)], "9"),
+         "CTCB_SWEEP_TC": (["0", "1", "2"], "3"), "CTCB_SWEEP_TC_CS": (["1", "2", "4"], "3"),
+         "CTCB_SWEEP_TC_COOP": (["0"], "1"), "CTCB_SWEEP_TRACE": (["1"], "0"),
+         "CTCB_CTC": (["auto", "warp", "pair", "par", "ckpt"], "pa")}
+
+
+def _ckpt_refuses():
+    """Whether the CTC plan of one 300-frame utterance with 200 labels is refused, as it is under CTCB_CTC=ckpt only
+    (the plan query needs no device)."""
+    import _ctcb
+    out = (ctypes.c_int32 * 8)()
+    return _ctcb.lib.ctcb_debug_ctc_plan(1, 300, 20, 200, 256, 256, 6000, 20, out) == -1
+
+
+def test_set_knob_takes_the_documented_values_only():
+    import _ctcb
+    lib = _ctcb.lib
+    assert lib.ctcb_debug_set_knob(b"CTCB_NO_SUCH_KNOB", b"1") == -1 and b"unknown knob" in lib.ctcb_last_error()
+    assert lib.ctcb_debug_set_knob(None, b"1") == -1
+    for name, (good, bad) in KNOBS.items():
+        for v in good:
+            assert lib.ctcb_debug_set_knob(name.encode(), v.encode()) == 0, (name, v, lib.ctcb_last_error())
+        for v in (bad, ""):
+            assert lib.ctcb_debug_set_knob(name.encode(), v.encode()) == -1, (name, v)
+            assert name.encode() in lib.ctcb_last_error()
+        assert lib.ctcb_debug_set_knob(name.encode(), None) == 0
+    # a refused value leaves the table as it was
+    assert lib.ctcb_debug_set_knob(b"CTCB_CTC", b"ckpt") == 0 and _ckpt_refuses()
+    assert lib.ctcb_debug_set_knob(b"CTCB_CTC", b"pa") == -1 and _ckpt_refuses()
+    assert lib.ctcb_debug_set_knob(b"CTCB_CTC", b"auto") == 0 and not _ckpt_refuses()
+    assert lib.ctcb_debug_set_ctc_kernel(4) == 0 and _ckpt_refuses()
+    assert lib.ctcb_debug_set_knob(b"CTCB_CTC", None) == 0
+
+
+def test_set_knob_null_restores_the_environment():
+    """The library reads the environment at its first use, so this runs in a fresh process started with CTCB_CTC=ckpt
+    (ctypes only, no device): a change overrides it, and NULL brings it back."""
+    import subprocess
+    import sys
+    code = "\n".join([
+        "import ctypes, sys",
+        "sys.path.insert(0, %r)" % os.path.join(ROOT, "stanford-ctc_b200"),
+        "from _ctcb import lib",
+        "out = (ctypes.c_int32 * 8)()",
+        "refused = lambda: lib.ctcb_debug_ctc_plan(1, 300, 20, 200, 256, 256, 6000, 20, out) == -1",
+        "assert refused()",
+        "assert lib.ctcb_debug_set_knob(b'CTCB_CTC', b'auto') == 0 and not refused()",
+        "assert lib.ctcb_debug_set_knob(b'CTCB_CTC', None) == 0 and refused()"])
+    r = subprocess.run([sys.executable, "-c", code], env=dict(os.environ, CTCB_CTC="ckpt"), capture_output=True,
+                       text=True, timeout=120)
+    assert r.returncode == 0, r.stderr[-2000:]
+
+
 def test_ctc_workspace_never_shrinks_as_the_batch_grows():
     """A buffer sized once for the largest call (the BRNN sizes its CTC area for maxB) must serve every smaller call:
     the size is monotone in B, Tmax and the label count, and covers two trellis planes for each of the first 256

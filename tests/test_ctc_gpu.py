@@ -4,16 +4,18 @@ ctc_fast.pyx and (b) the oracle run live on the same inputs.
 
 Tolerance (BASELINE.json north_star / SURVEY.md 8c): |nll - ref| / |ref| <= 1e-4 and
 ||g - g_ref||_F / ||g_ref||_F <= 1e-4 in fp32, skip flags equal."""
-import os
+import functools
 
 import numpy as np
 import pytest
 
 import recipes
 from oracle import ctc_oracle
+from recipes import knobs  # noqa: F401  (fixture)
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-4
+_forced = None             # the organisation _run_forced has set with CTCB_CTC, None: automatic
 
 
 def _rel(a, b):
@@ -28,7 +30,7 @@ def _gpu_single(torch, probs, seq, is_prob=True):
     lab = torch.from_numpy(seq if seq.size else np.zeros(1, np.int32)).cuda()
     off = torch.tensor([0, seq.shape[0]], dtype=torch.int32).cuda()
     tl = torch.tensor([T], dtype=torch.int32).cuda()
-    if os.environ.get("CTCB_CTC", "").startswith("c") and seq.shape[0] > 127:
+    if _forced == "ckpt" and seq.shape[0] > 127:
         # the checkpoint kernel has no build beyond 127 labels: forced, the call is an error, never another kernel
         with pytest.raises(ValueError, match="ckpt"):
             ctc_fast.ctc_loss_batch(acts, tl, lab, off, seq.shape[0], is_prob=is_prob)
@@ -117,7 +119,10 @@ def test_ragged_batch_time_major_layout(cuda):
             assert _rel(grad[:T, u, :].T.astype(np.float64), o_grad) <= TOL, u
 
 
-@pytest.mark.parametrize("nlab", [31, 32, 63, 64, 127, 128, 255, 256, 400, 511])
+PAIRS_PER_LANE_NLAB = [31, 32, 63, 64, 127, 128, 255, 256, 400, 511]
+
+
+@pytest.mark.parametrize("nlab", PAIRS_PER_LANE_NLAB)
 def test_pairs_per_lane_boundaries(nlab, cuda):
     """Label counts around every register-tiling boundary (1,2,4,8,16 pairs per lane)."""
     T = nlab + 40
@@ -174,40 +179,52 @@ def test_best_path_matches_reference_semantics(cuda):
     assert ctc_fast.decode_best_path(np.asfortranarray(q)) == ([3, 3, 5], [2, 4, 7])
 
 
-def _run_forced(shape):
-    """The golden / edge cases of this file in a fresh process with CTCB_CTC=shape (read once per process); returns
-    its pytest output."""
-    import subprocess
-    import sys
-    here = os.path.dirname(os.path.abspath(__file__))
-    root = os.path.dirname(here)
-    code = ("import os,sys; sys.path[:0]=[%r,%r,%r]; import pytest; "
-            "sys.exit(pytest.main(['-q','-rs','-p','no:cacheprovider','-k','golden_cases or ragged_batch or pairs_per_lane or fused_softmax or tile_boundaries or full_size', %r]))"
-            % (root, os.path.join(root, "stanford-ctc_b200"), here, os.path.abspath(__file__)))
-    env = dict(os.environ, CTCB_CTC=shape)
-    r = subprocess.run([sys.executable, "-c", code], env=env, capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stdout[-1500:] + r.stderr[-500:]
-    return r.stdout
+def _run_forced(shape, knobs, golden_ctc, torch):
+    """The golden / edge cases of this file in this process with CTCB_CTC=shape; returns the reasons of those that
+    skipped."""
+    global _forced
+    cases = ([functools.partial(test_golden_cases_through_c_abi, n, golden_ctc) for n in recipes.ALL_CTC]
+             + [test_ragged_batch_time_major_layout]
+             + [functools.partial(test_pairs_per_lane_boundaries, n) for n in PAIRS_PER_LANE_NLAB]
+             + [test_fused_softmax_logits_path]
+             + [functools.partial(test_meet_in_the_middle_tile_boundaries, T) for T in TILE_BOUNDARY_T]
+             + [test_full_size_properties])
+    knobs("CTCB_CTC", shape)
+    _forced = shape
+    skipped = []
+    try:
+        for case in cases:
+            try:
+                case(torch)
+            except pytest.skip.Exception as e:
+                skipped.append(str(e))
+    finally:
+        _forced = None
+    return skipped
 
 
 @pytest.mark.parametrize("shape", ["warp", "pair"])
-def test_other_kernel_shapes_when_forced(shape, cuda):
+def test_other_kernel_shapes_when_forced(shape, knobs, golden_ctc, cuda):
     """Small batches take the three-phase latency kernel (recurrences on two warps, gradient on all warps); CTCB_CTC=warp
     forces the one-warp-per-utterance kernel that spills the trellis (large batches, long label sequences), CTCB_CTC=pair
     the two-warp meet-in-the-middle kernel (mid-sized batches), through the same golden / edge cases."""
-    _run_forced(shape)
+    skipped = _run_forced(shape, knobs, golden_ctc, cuda)
+    assert not skipped, skipped
 
 
-def test_checkpoint_kernel_when_forced(cuda):
+def test_checkpoint_kernel_when_forced(knobs, golden_ctc, cuda):
     """CTCB_CTC=ckpt forces the one-warp kernel that checkpoints the trellis and recomputes it on chip (large batches) through
     the same golden / edge cases.  It has no build beyond 127 labels: those cases must be refused with CTCB_EINVAL, never
     run on another kernel."""
-    out = _run_forced("ckpt")
+    skipped = _run_forced("ckpt", knobs, golden_ctc, cuda)
     # 3 golden cases and 5 label counts have more than 127 labels; each is skipped after its refusal was checked
-    assert " 8 skipped" in out and "CTCB_CTC=ckpt refuses" in out, out[-1500:]
+    assert len(skipped) == 8 and all("CTCB_CTC=ckpt refuses" in s for s in skipped), skipped
 
 
-@pytest.mark.parametrize("T", [1, 3, 7, 8, 9, 16, 17, 31, 32, 33, 47, 200])
+TILE_BOUNDARY_T = [1, 3, 7, 8, 9, 16, 17, 31, 32, 33, 47, 200]
+
+
+@pytest.mark.parametrize("T", TILE_BOUNDARY_T)
 def test_meet_in_the_middle_tile_boundaries(T, cuda):
     """Utterance lengths around the tile sizes (16 frames; 8 in the checkpoint kernel): 1 tile (no first half), odd/even
     tile counts."""

@@ -6,7 +6,7 @@ warps meeting in the middle (pair), one warp per utterance with on-chip checkpoi
 (warp) -- at 1, 2, 4, 8 or 16 (blank, label) pairs per lane, with 8- or 16-frame tiles, one or two tile buffers, and
 4- or 8-byte tile copies and stores (vec2).  Every case names the plan it targets and checks it with ctcb_debug_ctc_plan
 before launching, so no case passes on a plan it did not mean to test; forced organisations are set in process with
-ctcb_debug_set_ctc_kernel and reset by a fixture.
+the CTCB_CTC knob (ctcb_debug_set_knob) and reset by a fixture.
 
 The reference sees the kernel's inputs: the float32 probabilities as they are, or the float64 softmax of the float32
 logits.  The bounds are element-wise: max |g - g_ref| over every valid (t, k) of every compared utterance, and
@@ -21,11 +21,11 @@ import numpy as np
 import pytest
 
 from oracle import ctc_oracle
+from recipes import knobs  # noqa: F401  (fixture)
 
 pytestmark = pytest.mark.gpu
 H100_SMS = 132             # the plans below are laid out for the 132-SM H100 SXM; other parts skip a plan they cannot reach
 KERNELS = ("par", "pair", "ckpt", "warp")
-FORCE = {"auto": 0, "warp": 1, "pair": 2, "par": 3, "ckpt": 4}       # ctcb_debug_set_ctc_kernel
 FIELDS = ("kernel", "P", "th", "nbuf", "warps", "vec2", "Kp", "smem_kb")
 # Bounds per organisation (max |g - g_ref|, |nll - nll_ref| / |nll_ref|), at most 4x the largest error measured on an H100
 # 80GB HBM3 (power limit 700 W) over the cases of this file: par 4.7e-7 / 7.3e-8, pair 1.17e-6 / 9.9e-8, ckpt 5.3e-7 /
@@ -59,15 +59,13 @@ def _check_plan(plan, expect, torch, what):
 
 
 @pytest.fixture
-def force(cuda):
-    """force(name) sets the organisation in this process (overriding CTCB_CTC); automatic again afterwards."""
-    from _ctcb import lib, check
-
+def force(knobs, cuda):
+    """force(name) sets the organisation (auto, warp, pair, par, ckpt) in this process, overriding the environment's
+    CTCB_CTC, which is in effect again afterwards."""
     def set_(name):
-        check(lib.ctcb_debug_set_ctc_kernel(FORCE[name]))
+        knobs("CTCB_CTC", name)
     set_("auto")
-    yield set_
-    lib.ctcb_debug_set_ctc_kernel(0)
+    return set_
 
 
 # ------------------------------------------------------------------------------------------------ one batch

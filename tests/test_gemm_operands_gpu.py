@@ -4,21 +4,18 @@ wgmma reads .tf32 operands K-major only.  An operand stored MN-major (A as [K][M
 over the time-major activations) is read in place and transposed in shared memory; an operand TMA cannot describe
 (pitch not a multiple of 16 bytes, base not 16-byte aligned) is copied into the workspace first.  Every case checks its
 plan with ctcb_debug_gemm_plan (operand paths, splits, accumulator chains of at most 64 k-blocks), its
-result against a float64 product, and, in a subprocess with CTCB_GEMM_TC_COPY=1, that the copy path gives the same
+result against a float64 product, and, with CTCB_GEMM_TC_COPY=1 set in process, that the copy path gives the same
 bytes at the same split.  The recurrent weight-gradient pair (one launch for both directions) must equal two single
 calls byte for byte.  Each case prints its plan and error as one JSON line (shown with pytest -s)."""
 import json
-import os
-import subprocess
-import sys
-import tempfile
 import zlib
 
 import numpy as np
 import pytest
 
+from recipes import knobs  # noqa: F401  (fixture)
+
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 H100_SMS = 132             # the split counts below are those of the 132-SM H100 SXM
 CHAIN_KB = 64              # TC_CHAIN_KB: k-blocks of 32 per accumulator chain
 # Frobenius-relative error against float64.  The tensor-core accumulator truncates, so the error of 3xTF32 grows with
@@ -76,7 +73,7 @@ def _plan(ta, tb, M, N, K, A, lda, Bp, ldb, problems=1):
 
 
 def _run_case(name):
-    """Result (numpy float32), plan and float64 reference of one case, computed on the current process's plan."""
+    """Result (numpy float32), plan and float64 reference of one case, computed on the plan of the knobs in effect."""
     import _ctcb
     from _ctcb import lib, check, ptr
     torch = _dev()
@@ -95,16 +92,6 @@ def _run_case(name):
     b64 = b.astype(np.float64) if not tb else b.astype(np.float64).T
     want = a64 @ b64 + beta * c0.astype(np.float64)
     return C.cpu().numpy(), plan, want
-
-
-def _dump(path):
-    """Every case's result and plan, for the comparison across processes."""
-    out = {}
-    for name in CASES:
-        got, plan, _ = _run_case(name)
-        out[name] = got
-        out[name + "/plan"] = np.array([plan[k] for k in ("splits", "a_path", "b_path")], dtype=np.int32)
-    np.savez(path, **out)
 
 
 def _rel(a, b):
@@ -145,24 +132,19 @@ def test_gemm_operand_paths(name, cuda):
     assert err < bound, (err, bound)
 
 
-def test_gemm_copy_path_same_bytes(cuda):
-    """CTCB_GEMM_TC_COPY=1 (read once per process): the same cases through the workspace copies, byte for byte."""
-    with tempfile.TemporaryDirectory() as td:
-        path = os.path.join(td, "copy.npz")
-        code = ("import sys; sys.path[:0]=[%r,%r,%r]; import test_gemm_operands_gpu as t; t._dump(%r)"
-                % (ROOT, os.path.join(ROOT, "stanford-ctc_b200"), os.path.join(ROOT, "tests"), path))
-        r = subprocess.run([sys.executable, "-c", code], env=dict(os.environ, CTCB_GEMM_TC_COPY="1"),
-                           capture_output=True, text=True, timeout=600)
-        assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
-        ref = dict(np.load(path))
+def test_gemm_copy_path_same_bytes(knobs, cuda):
+    """CTCB_GEMM_TC_COPY=1: the same cases through the workspace copies, byte for byte."""
+    in_place = {name: _run_case(name)[:2] for name in CASES}
+    knobs("CTCB_GEMM_TC_COPY", "1")
     for name in CASES:
-        got, plan, _ = _run_case(name)
-        splits, a_path, b_path = ref[name + "/plan"].tolist()
+        ref, ref_plan, _ = _run_case(name)
+        got, plan = in_place[name]
+        splits, a_path, b_path = ref_plan["splits"], ref_plan["a_path"], ref_plan["b_path"]
         assert splits == plan["splits"], (name, splits, plan)
         # the copy path reads nothing MN-major in place
         assert a_path != MN and b_path != MN, name
         assert (a_path, b_path) == tuple(COPY if p == MN else p for p in (plan["a_path"], plan["b_path"])), name
-        same = np.array_equal(got.view(np.uint32), ref[name].view(np.uint32))
+        same = np.array_equal(got.view(np.uint32), ref.view(np.uint32))
         print(json.dumps({"gemm_copy_" + name: dict(splits=splits, same_bytes=same)}))
         assert same, name
 

@@ -4,7 +4,7 @@ brnnet.py:144-152 (forward) and :208-224 (BPTT), vectorised over utterances.
 The sweep is a planner over three kernels (the tensor-core kernel for H >= 1024, the cluster kernel for H = 128/256/512,
 the generic cooperative kernel for everything else and for batches the others cannot hold).  Every case names the plan it
 targets and checks it with ctcb_debug_sweep_plan before launching, so no case passes on a plan it did not mean to test.
-Cases that need an environment knob run in a subprocess with that knob set.
+Cases that need a planner knob set it in this process (recipes.knobs) and restore it afterwards.
 
 The bound is per kernel family, on  max|gpu - ref| / max(1, max|ref|)  per direction, and it is tight enough to tell the
 fp32-faithful 3xTF32 tensor-core arithmetic from plain TF32: each case also runs a TF32 emulation of the same sweep on the
@@ -12,16 +12,14 @@ CPU (both operands truncated to 10 mantissa bits as the kernel truncates them, o
 float64) and requires it to be at least TF32_MARGIN times the bound away from the float64 result.  Each case prints its
 plan, errors, bound and the emulation's error as one JSON line (shown with pytest -s)."""
 import json
-import os
-import subprocess
-import sys
 import time
 
 import numpy as np
 import pytest
 
+from recipes import knobs  # noqa: F401  (fixture)
+
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 MAXACT = 20.0
 KERNELS = ("generic", "cluster", "tensor-core")
 H100_SMS = 132             # the plans below are laid out for the 132-SM H100 SXM; other parts skip a plan they cannot reach
@@ -113,11 +111,7 @@ def _check_plan(H, B, ndir, expect, torch):
 
 def _natural_family(H):
     """The kernel family the planner picks for a layer size at a small batch, under the knobs in effect."""
-    if H >= 1024 and os.environ.get("CTCB_SWEEP_TC", "1") != "0":
-        return "tensor-core"
-    if H in (128, 256, 512) and not os.environ.get("CTCB_SWEEP", "").startswith("b"):
-        return "cluster"
-    return "generic"
+    return _plan(H, 1, 2)["kernel"]
 
 
 # ------------------------------------------------------------------------------------------------ one case
@@ -175,7 +169,6 @@ def _sweep_case(name, H, B, T, ndir, expect, torch):
     tf32_fwd = min(_err(e, r) for e, r in zip(efwd, rfwd))
     tf32_bptt = min(_err(e, r) for e, r in zip(ebptt, rbptt))
     print(json.dumps({"sweep": name, "H": H, "B": B, "T": T, "ndir": ndir, "plan": plan,
-                      "env": {k: v for k, v in os.environ.items() if k.startswith("CTCB_")},
                       "err_fwd": err_fwd, "err_bptt": err_bptt, "bound": bound,
                       "tf32_err_fwd": tf32_fwd, "tf32_err_bptt": tf32_bptt, "seconds": round(time.time() - t0, 2)}))
 
@@ -198,23 +191,6 @@ def _sweep_case(name, H, B, T, ndir, expect, torch):
         assert tf32_bptt >= TF32_MARGIN * bound, (tf32_bptt, bound)
 
 
-# ------------------------------------------------------------------------------------------------ subprocess helper
-def _run_forced(env, kexpr):
-    """Run the tests of this file selected by `kexpr` in a fresh process with `env` added (the knobs are read once per
-    process), and fail with its output if they fail."""
-    code = ("import sys; sys.path[:0]=[%r,%r,%r]; import pytest; "
-            "sys.exit(pytest.main(['-q','-s','-p','no:cacheprovider','-m','gpu','-k',%r,%r]))"
-            % (ROOT, os.path.join(ROOT, "stanford-ctc_b200"), os.path.join(ROOT, "tests"), kexpr, os.path.abspath(__file__)))
-    r = subprocess.run([sys.executable, "-c", code], env=dict(os.environ, **env), capture_output=True, text=True,
-                       timeout=600)
-    for line in r.stdout.splitlines():
-        if line.startswith("{"):
-            print(line)
-    assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-1000:]
-    if " passed" not in r.stdout:
-        pytest.skip("skipped in the subprocess: " + r.stdout[-500:])
-
-
 # ------------------------------------------------------------------------------------------------ the shapes of the
 # original suite: each on the plan the device chooses by default
 @pytest.mark.parametrize("H,B,T", [(128, 8, 40), (128, 3, 33), (256, 9, 25), (512, 4, 30), (512, 32, 50),
@@ -231,17 +207,20 @@ def test_sweep_forward_and_bptt(H, B, T, cuda):
     _sweep_case("%d-%d-%d" % (H, B, T), H, B, T, 2, {"kernel": _natural_family(H)}, cuda)
 
 
-def test_general_barrier_kernel_when_forced(cuda):
+def test_general_barrier_kernel_when_forced(knobs, cuda):
     """CTCB_SWEEP=barrier forces the L2/counter-barrier kernel for sizes the cluster kernel would take."""
-    _run_forced({"CTCB_SWEEP": "barrier"}, "test_sweep_forward_and_bptt and (512-32-50 or 128-3-33 or 256-9-25)")
+    knobs("CTCB_SWEEP", "barrier")
+    for H, B, T in ((512, 32, 50), (128, 3, 33), (256, 9, 25)):
+        assert _natural_family(H) == GEN, H
+        test_sweep_forward_and_bptt(H, B, T, cuda)
 
 
 # ------------------------------------------------------------------------------------------------ the plan matrix
 TC, CL, GEN = "tensor-core", "cluster", "generic"
 
 
-def _c(name, H, B, T, ndir, env=None, **expect):
-    return pytest.param(H, B, T, ndir, env or {}, expect, id=name)
+def _c(name, H, B, T, ndir, forced=None, **expect):
+    return pytest.param(H, B, T, ndir, forced or {}, expect, id=name)
 
 
 PLAN_CASES = [
@@ -302,12 +281,11 @@ PLAN_CASES = [
 ]
 
 
-@pytest.mark.parametrize("H,B,T,ndir,env,expect", PLAN_CASES)
-def test_sweep_plan(H, B, T, ndir, env, expect, request, cuda):
+@pytest.mark.parametrize("H,B,T,ndir,forced,expect", PLAN_CASES)
+def test_sweep_plan(H, B, T, ndir, forced, expect, request, knobs, cuda):
     name = request.node.callspec.id
-    if any(os.environ.get(k) != v for k, v in env.items()):
-        _run_forced(env, "test_sweep_plan and [%s]" % name)
-        return
+    for k, v in forced.items():
+        knobs(k, v)
     if expect["kernel"] == GEN and H >= 1024:
         from _ctcb import lib
         assert ndir == 1 or lib.ctcb_sweep_uses_tensor_cores(H, B) == 0

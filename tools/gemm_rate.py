@@ -18,4 +18,4 @@ for (M, N, K) in [(6400, 512, 512), (16384, 2048, 2048), (16384, 2048, 256)]:
     for _ in range(10): run()
     e1.record(); torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / 10
-    print("M=%d N=%d K=%d mmas=%s: %.3f ms  %.1f TFLOP/s fp32-equivalent" % (M, N, K, os.environ.get("CTCB_GEMM_MMAS", "3"), ms, 2.0 * M * N * K / ms / 1e9), flush=True)
+    print("M=%d N=%d K=%d: %.3f ms  %.1f TFLOP/s fp32-equivalent" % (M, N, K, ms, 2.0 * M * N * K / ms / 1e9), flush=True)

@@ -1,6 +1,6 @@
 """Time the weight-gradient contractions of the C2 step (H = 512, B = 32, T = 200) and the 48000 x 2048 x 2048 layer
 contraction that bench.py reports, with MN-major operands read in place and through the transposed workspace copies
-(ctcb_debug_set_gemm_copy), alternated in one process.  CUDA events around REPS calls; prints one JSON line per
+(ctcb_debug_set_knob CTCB_GEMM_TC_COPY), alternated in one process.  CUDA events around REPS calls; prints one JSON line per
 contraction with the plan of each path and the median over ROUNDS alternations.
 
     python tools/wgrad_time.py [--reps 20] [--rounds 5]
@@ -81,14 +81,14 @@ def main():
         plans = {}
         reps = max(2, args.reps // 10) if "48000" in name else args.reps
         for rnd_ in range(args.rounds + 1):
-            for mode, flag in (("copy", 1), ("in_place", 0)):
-                check(lib.ctcb_debug_set_gemm_copy(flag))
+            for mode, flag in (("copy", b"1"), ("in_place", b"0")):
+                check(lib.ctcb_debug_set_knob(b"CTCB_GEMM_TC_COPY", flag))
                 run, plan, flops = make()
                 plans[mode] = plan
                 us = time_one(run, reps)
                 if rnd_ > 0:                      # round 0 warms both paths up
                     res[mode].append(us)
-        check(lib.ctcb_debug_set_gemm_copy(0))
+        check(lib.ctcb_debug_set_knob(b"CTCB_GEMM_TC_COPY", None))
         med = {k: sorted(v)[len(v) // 2] for k, v in res.items()}
         print(json.dumps({"contraction": name, "device": dev, "us_median": med, "us_all": res,
                           "speedup": med["copy"] / med["in_place"],
