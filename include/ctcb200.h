@@ -92,7 +92,8 @@ int ctcb_ctc_blankforce_loss_grad_f32(const float *acts, int is_prob, int64_t ut
  * A is M x K (or K x M if transA), leading dimensions in elements.
  * bias (may be NULL): added per output column n.  relu!=0: C = max(C, 0) after bias.
  * mask_src (may be NULL, ldc-strided like C): C *= (mask_src > 0).
- * workspace is used for split-K partial sums (ctcb_gemm_workspace_bytes). */
+ * workspace is used for split-K partial sums (ctcb_gemm_workspace_bytes).  M is at most 8,388,480 (65,535 tiles of
+ * 128 rows); a larger M returns CTCB_EINVAL.  K is not limited. */
 size_t ctcb_gemm_workspace_bytes(int M, int N, int K);
 int ctcb_gemm_f32(int transA, int transB, int M, int N, int K, float alpha,
                   const float *A, int64_t lda, const float *B, int64_t ldb, float beta,
@@ -110,7 +111,10 @@ int ctcb_gemm_pair_f32(int transA, int transB, int M, int N, int K, float alpha,
  * inspected for their alignment.  out (HOST, 8 int32):
  *   {kernel: 0 FFMA / 1 tensor core, BN (output tile width), ring stages, K splits, CTAs per launch,
  *    A path, B path: 0 read in place K-major / 1 read in place MN-major, transposed in shared memory / 2 copied into
- *    the workspace first,  problems per launch (2: the pair shares one launch)}.  The FFMA kernel reports {0, .., 0, 1}. */
+ *    the workspace first,  problems per launch (2: the pair shares one launch)}.  The FFMA kernel reports
+ *   {0, 128, 0, K splits, CTAs per launch, vec, 0, 1}: vec (in the A path slot) = 1 when both operands are read with
+ *   16-byte loads (both pitches multiples of 4 floats, both bases 16-byte aligned); each split accumulates
+ *   ceil(K / splits) rounded up to a multiple of 16.  M <= 0 or N <= 0 reports {0, .., 0, 1}. */
 int ctcb_debug_gemm_plan(int transA, int transB, int M, int N, int K, const float *A, int64_t lda,
                          const float *B, int64_t ldb, int problems, int32_t *out);
 
@@ -154,7 +158,8 @@ typedef struct ctcb_brnn_config {
     int32_t numLayers;
     int32_t temporalLayer; /* <=0: none.  1..numLayers (numLayers itself is an extension, see DESIGN.md) */
     int32_t maxT;          /* frames per utterance the buffers are sized for (reference: maxBatch) */
-    int32_t maxB;          /* utterances per step */
+    int32_t maxB;          /* utterances per step; maxT * maxB is at most 8,388,480 (the rows of a ctcb_gemm_f32), else
+                            * the config is invalid */
     int32_t maxLabels;     /* longest label sequence */
     float reg;             /* L2 coefficient (brnnet.py:11,177-183,197-198,244-247) */
     float maxAct;          /* clip of the temporal layer, 20.0 (brnnet.py:32) */

@@ -168,6 +168,7 @@ static int valid_cfg(const ctcb_brnn_config *c) {
     if (c->numLayers < 1 || c->numLayers > 64) return 0;
     if (c->maxT <= 0 || c->maxB <= 0 || c->maxLabels < 0) return 0;
     if (c->maxLabels > CTCB_CTC_MAX_LABELS) return 0;   // the CTC kernel's register-resident trellis (ctc.cu)
+    if ((int64_t)c->maxT * c->maxB > GEMM_MAX_M) return 0;     // the forward and delta contractions have maxT*maxB rows
     if (c->numTemporal < 0) return 0;
     // a stacked block must lie inside the hidden layers; k <= 1 keeps the silent "no temporal layer" rule below
     if (c->numTemporal > 1 && (c->temporalLayer <= 0 || c->temporalLayer + c->numTemporal - 1 > c->numLayers)) return 0;
@@ -372,6 +373,9 @@ extern "C" int ctcb_brnn_create(const ctcb_brnn_config *cfg, ctcb_brnn **out) {
     if (cfg && cfg->maxLabels > CTCB_CTC_MAX_LABELS)
         return set_error(CTCB_EINVAL, "ctcb_brnn_create: maxLabels %d exceeds the CTC kernel's limit of %d labels per utterance",
                          cfg->maxLabels, CTCB_CTC_MAX_LABELS);
+    if (cfg && (int64_t)cfg->maxT * cfg->maxB > GEMM_MAX_M)
+        return set_error(CTCB_EINVAL, "ctcb_brnn_create: maxT * maxB = %lld rows exceed the contractions' limit of %d",
+                         (long long)cfg->maxT * cfg->maxB, GEMM_MAX_M);
     if (cfg && cfg->numTemporal > 1 && !valid_cfg(cfg))
         return set_error(CTCB_EINVAL, "ctcb_brnn_create: a block of %d temporal layers from layer %d does not fit in "
                          "hidden layers 1..%d", cfg->numTemporal, cfg->temporalLayer, cfg->numLayers);

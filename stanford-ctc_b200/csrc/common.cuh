@@ -78,4 +78,17 @@ struct SweepPlan {
 };
 int select_sweep(int H, int B, int ndir, SweepPlan *p);
 
+// How ctcb_gemm_f32 runs a contraction on the FFMA kernel (gemm_simt.cu); gemm_simt_plan decides it for the launch and
+// ctcb_debug_gemm_plan alike.
+struct GemmSimtPlan {
+    int splits;             // K splits (gridDim.z); > 1 writes partials to the workspace and adds a reduce
+    int k_per_split;        // k per split, a multiple of the 16-deep k-tile: the length of each accumulator chain
+    int vec;                // 16-byte operand loads (both pitches multiples of 4 floats, both bases 16-byte aligned)
+    int ctas;               // CTAs of the launch
+};
+void gemm_simt_plan(int M, int N, int K, const float *A, int64_t lda, const float *B, int64_t ldb, size_t ws_bytes,
+                    GemmSimtPlan *p);
+// Both contraction kernels put 128-row output tiles on gridDim.y (at most 65,535): the largest M they take.
+constexpr int GEMM_MAX_M = 128 * 65535;
+
 }  // namespace ctcb

@@ -260,6 +260,21 @@ static int choose_splits(int M, int N, int K) {
     return splits < 1 ? 1 : splits;
 }
 
+// The one place that decides how an FFMA contraction runs: ctcb_gemm_f32 and ctcb_debug_gemm_plan both call it.
+// Splits need room for their partials in the ws_bytes of workspace; without it the contraction runs unsplit.
+void gemm_simt_plan(int M, int N, int K, const float *A, int64_t lda, const float *B, int64_t ldb, size_t ws_bytes,
+                    GemmSimtPlan *p) {
+    int splits = choose_splits(M, N, K);
+    if (splits > 1 && ws_bytes < (size_t)splits * M * N * sizeof(float)) splits = 1;
+    int kps = (K + splits - 1) / splits;
+    kps = (kps + BK - 1) / BK * BK;
+    p->k_per_split = kps > 0 ? kps : BK;
+    splits = K > 0 ? (K + p->k_per_split - 1) / p->k_per_split : 1;
+    p->splits = splits > 1 ? splits : 1;
+    p->vec = (lda % 4 == 0) && (ldb % 4 == 0) && (((uintptr_t)A | (uintptr_t)B) % 16 == 0);
+    p->ctas = ((N + BN - 1) / BN) * ((M + BM - 1) / BM) * p->splits;
+}
+
 }  // namespace ctcb
 
 namespace ctcb {
@@ -288,6 +303,7 @@ extern "C" int ctcb_gemm_f32(int transA, int transB, int M, int N, int K, float 
                              int relu, const float *mask_src, void *workspace, size_t ws_bytes, void *stream) {
     if (M <= 0 || N <= 0) return CTCB_OK;
     if (!A || !B || !C || K < 0) return set_error(CTCB_EINVAL, "ctcb_gemm_f32: bad argument");
+    if (M > GEMM_MAX_M) return set_error(CTCB_EINVAL, "ctcb_gemm_f32: M = %d exceeds %d rows", M, GEMM_MAX_M);
     // large contractions: 3xTF32 on the wgmma tensor cores (gemm_tc.cu); small or odd ones: exact FFMA below
     if (gemm_tc_eligible(M, N, K) && workspace && ws_bytes >= gemm_tc_workspace_bytes(M, N, K))
         return run_gemm_tc(transA, transB, M, N, K, alpha, A, lda, B, ldb, beta, C, ldc, bias, relu, mask_src, workspace,
@@ -295,15 +311,12 @@ extern "C" int ctcb_gemm_f32(int transA, int transB, int M, int N, int K, float 
     GemmArgs g;
     g.M = M; g.N = N; g.K = K; g.A = A; g.lda = lda; g.B = B; g.ldb = ldb; g.C = C; g.ldc = ldc;
     g.alpha = alpha; g.beta = beta; g.bias = bias; g.relu = relu; g.mask = mask_src;
-    int splits = choose_splits(M, N, K);
-    if (splits > 1 && (!workspace || ws_bytes < (size_t)splits * M * N * sizeof(float))) splits = 1;
+    GemmSimtPlan p;
+    gemm_simt_plan(M, N, K, A, lda, B, ldb, workspace ? ws_bytes : 0, &p);
+    const int splits = p.splits;
+    const bool vec = p.vec;
+    g.k_per_split = p.k_per_split;
     g.partial = splits > 1 ? (float *)workspace : nullptr;
-    int kps = (K + splits - 1) / splits;
-    kps = (kps + BK - 1) / BK * BK;
-    g.k_per_split = kps > 0 ? kps : BK;
-    splits = K > 0 ? (K + g.k_per_split - 1) / g.k_per_split : 1;
-    if (splits <= 1) { g.partial = nullptr; splits = 1; }
-    const bool vec = (lda % 4 == 0) && (ldb % 4 == 0) && (((uintptr_t)A | (uintptr_t)B) % 16 == 0);
     g.vecc = g.partial ? (N % 4 == 0 && ((uintptr_t)g.partial) % 16 == 0)
                        : (ldc % 4 == 0 && ((uintptr_t)C) % 16 == 0 && (!mask_src || ((uintptr_t)mask_src) % 16 == 0));
     dim3 grid((N + BN - 1) / BN, (M + BM - 1) / BM, splits);
@@ -341,6 +354,7 @@ extern "C" int ctcb_gemm_pair_f32(int transA, int transB, int M, int N, int K, f
                                   void *stream) {
     if (M <= 0 || N <= 0) return CTCB_OK;
     if (!A0 || !A1 || !B0 || !B1 || !C0 || !C1 || K < 0) return set_error(CTCB_EINVAL, "ctcb_gemm_pair_f32: bad argument");
+    if (M > GEMM_MAX_M) return set_error(CTCB_EINVAL, "ctcb_gemm_pair_f32: M = %d exceeds %d rows", M, GEMM_MAX_M);
     if (gemm_tc_eligible(M, N, K) && workspace && ws_bytes >= gemm_tc_pair_workspace_bytes(M, N, K)) {
         const float *A[2] = {A0, A1}, *B[2] = {B0, B1};
         float *C[2] = {C0, C1};

@@ -298,24 +298,30 @@ __global__ void tc_split_kernel(const float *__restrict__ x, int64_t ld, int row
         if (lo) lo[idx] = v - h;
     }
 }
-// transposing variant: x is rows x cols (ld); outputs are cols x rows (ldo >= rows), tiled through shared memory
+// transposing variant: x is rows x cols (ld); outputs are cols x rows (ldo >= rows), tiled through shared memory.
+// gridDim.y (at most 65,535) strides over the 32-row tiles, so any row count (K of a weight gradient: T*B) is covered.
 __global__ void tc_split_transpose_kernel(const float *__restrict__ x, int64_t ld, int rows, int cols,
                                           float *__restrict__ hi, float *__restrict__ lo, int64_t ldo) {
     __shared__ float tile[32][33];
-    const int c0 = blockIdx.x * 32, r0 = blockIdx.y * 32;
-    for (int i = threadIdx.y; i < 32; i += 8) {
-        const int r = r0 + i, c = c0 + threadIdx.x;
-        tile[i][threadIdx.x] = (r < rows && c < cols) ? x[(int64_t)r * ld + c] : 0.f;
-    }
-    __syncthreads();
-    for (int i = threadIdx.y; i < 32; i += 8) {
-        const int c = c0 + i, r = r0 + threadIdx.x;     // output row = c, output col = r
-        if (c < cols && r < ldo) {
-            const float v = (r < rows) ? tile[threadIdx.x][i] : 0.f;
-            const float h = __uint_as_float(__float_as_uint(v) & 0xffffe000u);
-            hi[(int64_t)c * ldo + r] = v;
-            if (lo) lo[(int64_t)c * ldo + r] = v - h;
+    const int c0 = blockIdx.x * 32;
+    for (int64_t r0 = (int64_t)blockIdx.y * 32; r0 < ldo; r0 += (int64_t)gridDim.y * 32) {
+        for (int i = threadIdx.y; i < 32; i += 8) {
+            const int64_t r = r0 + i;
+            const int c = c0 + threadIdx.x;
+            tile[i][threadIdx.x] = (r < rows && c < cols) ? x[r * ld + c] : 0.f;
         }
+        __syncthreads();
+        for (int i = threadIdx.y; i < 32; i += 8) {
+            const int c = c0 + i;
+            const int64_t r = r0 + threadIdx.x;     // output row = c, output col = r
+            if (c < cols && r < ldo) {
+                const float v = (r < rows) ? tile[threadIdx.x][i] : 0.f;
+                const float h = __uint_as_float(__float_as_uint(v) & 0xffffe000u);
+                hi[(int64_t)c * ldo + r] = v;
+                if (lo) lo[(int64_t)c * ldo + r] = v - h;
+            }
+        }
+        __syncthreads();
     }
 }
 
@@ -545,7 +551,8 @@ int run_gemm_tc(int transA, int transB, int M, int N, int K, float alpha, const 
     auto copy = [&](const float *X, int64_t ld, int rows, bool mn_major, const float **use, int64_t *ld_use) -> int {
         float *dst = prep + prep_bytes / sizeof(float);
         if (mn_major)
-            tc_split_transpose_kernel<<<dim3((rows + 31) / 32, (K + 31) / 32), dim3(32, 8), 0, st>>>(X, ld, K, rows, dst, nullptr, Kp);
+            tc_split_transpose_kernel<<<dim3((rows + 31) / 32, (K + 31) / 32 < 65535 ? (K + 31) / 32 : 65535), dim3(32, 8), 0,
+                                        st>>>(X, ld, K, rows, dst, nullptr, Kp);
         else
             tc_split_kernel<<<ew_grid((int64_t)rows * Kp), 256, 0, st>>>(X, ld, rows, K, dst, nullptr, Kp);
         CTCB_LAUNCH_CHECK();
@@ -589,7 +596,14 @@ extern "C" int ctcb_debug_gemm_plan(int transA, int transB, int M, int N, int K,
     if (!out) return ctcb::set_error(CTCB_EINVAL, "ctcb_debug_gemm_plan: null output");
     if (problems != 1 && problems != 2) return ctcb::set_error(CTCB_EINVAL, "ctcb_debug_gemm_plan: problems must be 1 or 2");
     for (int i = 0; i < 8; ++i) out[i] = 0;
-    if (M <= 0 || N <= 0 || !ctcb::gemm_tc_eligible(M, N, K)) { out[7] = 1; return CTCB_OK; }     // FFMA kernel
+    if (M <= 0 || N <= 0) { out[7] = 1; return CTCB_OK; }      // nothing runs
+    if (!ctcb::gemm_tc_eligible(M, N, K)) {                     // FFMA kernel, with room for its partials
+        ctcb::GemmSimtPlan s;
+        ctcb::gemm_simt_plan(M, N, K, A, lda, B, ldb, SIZE_MAX, &s);
+        const int32_t v[8] = {0, 128, 0, s.splits, s.ctas, s.vec, 0, 1};
+        for (int i = 0; i < 8; ++i) out[i] = v[i];
+        return CTCB_OK;
+    }
     ctcb::GemmTcPlan p;
     ctcb::gemm_tc_plan(transA, transB, M, N, K, A, lda, B, ldb, problems, &p);
     const int32_t v[8] = {1, p.BN, p.stages, p.splits, p.ctas, p.a_path, p.b_path, p.problems};

@@ -80,6 +80,28 @@ def test_error_reporting():
     assert _ctcb.lib.ctcb_ctc_workspace_bytes(1000, 100, 30) == 1000 * (100 * 64 + 8) * 8
 
 
+def test_gemm_row_limit():
+    """Both contraction kernels put 128-row output tiles on gridDim.y: M beyond 65,535 tiles is refused before anything
+    is read or launched, and so is a net whose maxT * maxB rows would need such a contraction."""
+    import _ctcb
+    lib = _ctcb.lib
+    limit = 128 * 65535
+    buf = (ctypes.c_float * 4)()
+    p = ctypes.addressof(buf)
+    assert lib.ctcb_gemm_f32(0, 1, limit + 1, 1, 1, 1.0, p, 1, p, 1, 0.0, p, 1, None, 0, None, None, 0, None) == -1
+    assert b"exceeds" in lib.ctcb_last_error()
+    assert lib.ctcb_gemm_pair_f32(1, 0, limit + 1, 1, 1, 1.0, p, p, limit + 1, p, p, 1, 0.0, p, p, 1, None, 0,
+                                  None) == -1
+    assert b"exceeds" in lib.ctcb_last_error()
+    ok = _ctcb.BrnnConfig(41, 62, 16, 2, 1, 1000, limit // 1000, 30, 0.0, 20.0)
+    over = _ctcb.BrnnConfig(41, 62, 16, 2, 1, 1000, limit // 1000 + 1, 30, 0.0, 20.0)
+    assert lib.ctcb_brnn_param_count(ctypes.byref(ok)) > 0
+    assert lib.ctcb_brnn_param_count(ctypes.byref(over)) <= 0
+    h = ctypes.c_void_p()
+    assert lib.ctcb_brnn_create(ctypes.byref(over), ctypes.byref(h)) == -1
+    assert b"rows exceed" in lib.ctcb_last_error()
+
+
 # The knobs of INTEGRATION.md section 4 that ctcb_debug_set_knob takes: every documented value, and a value outside them
 KNOBS = {"CTCB_GEMM": (["simt"], "s"), "CTCB_GEMM_TC_COPY": (["0", "1"], "2"), "CTCB_GEMM_TRACE": (["1"], "0"),
          "CTCB_SWEEP": (["barrier"], "b"), "CTCB_SWEEP_NB": ([str(n) for n in range(1, 9)], "9"),
