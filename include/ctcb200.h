@@ -52,7 +52,9 @@ int ctcb_profile_report(char *buf, size_t cap);
  * grad_out  : same indexing as acts; d(nll)/d(logit) = softmax - posterior occupancy
  *             (ctc_fast.pyx:139-145).  Zero for skipped utterances.
  * nll_out   : float32[B]  -log p(labels | acts)     (ctc_fast.pyx:152)
- * skip_out  : int32[B]    1 where a frame normaliser was 0 (ctc_fast.pyx:147-149)
+ * skip_out  : int32[B]    1 where a frame normaliser was 0 (ctc_fast.pyx:147-149), and 1 where the scaled trellis
+ *             lost mass to float64 underflow (forward and backward log-likelihoods more than 1e-4 nats apart: long
+ *             utterances with unaligned outputs, where the reference returns a wrong loss and gradient)
  * workspace : ctcb_ctc_workspace_bytes(B, Tmax, max_labels) bytes of device scratch.  That size never decreases with B,
  *             Tmax or max_labels, so a buffer sized for the largest call serves every smaller one: one fp64 trellis
  *             plane of Tmax x 64P doubles (P = pairs per lane, 1..16 by max_labels) per utterance, two per utterance

@@ -21,8 +21,11 @@
 #define AB(s, t) ab[(size_t)(s) + (size_t)L * (size_t)(t)]
 #define G(k, t) grad[(size_t)(k) + (size_t)K * (size_t)(t)]
 
-int ctc_oracle_loss(const double *params, int K, int T, const int *seq, int seqLen,
-                    int blank, double *grad, double *nll)
+/* *llb, when not NULL, receives the llBackward the reference computes and discards (:84-114).  With exact
+ * arithmetic it equals llForward; where the per-frame normalised trellis loses mass to float64 underflow the two
+ * disagree. */
+int ctc_oracle_loss_fb(const double *params, int K, int T, const int *seq, int seqLen,
+                       int blank, double *grad, double *nll, double *llb)
 {
     /* ctc_fast.pyx:23-34 -- sizes and zero-initialised trellises */
     int L = 2 * seqLen + 1;
@@ -95,7 +98,6 @@ int ctc_oracle_loss(const double *params, int K, int T, const int *seq, int seqL
         for (s = start; s < end; s++) B(s, t) /= c;
         llBackward += log(c);
     }
-    (void)llBackward;
 
     /* :117-131 -- posterior occupancy numerators and the ab/p trellis */
     for (t = 0; t < T; t++)
@@ -121,8 +123,115 @@ int ctc_oracle_loss(const double *params, int K, int T, const int *seq, int seqL
 done:
     /* on skip the reference returns grad as accumulated so far: still all zeros */
     *nll = -llForward;
+    if (llb) *llb = llBackward;
     free(alphas); free(betas); free(ab); free(absum);
     return skip;
+}
+
+int ctc_oracle_loss(const double *params, int K, int T, const int *seq, int seqLen,
+                    int blank, double *grad, double *nll)
+{
+    return ctc_oracle_loss_fb(params, K, T, seq, seqLen, blank, grad, nll, NULL);
+}
+
+/*
+ * The same loss and gradient in the log domain: float64 log-sum-exp recursions with no per-frame scaling, so no
+ * state and no product of alpha and beta leaves float64's range however long the utterance.  Where the scaled
+ * restatement above is in range the two agree to rounding; where it is not (thousands of frames, unaligned
+ * outputs) this one is the truth the tests hold the kernel to.  The reference's contract is kept:
+ *   T < |l|            -> (inf, grad = p, no skip); a one-frame utterance returns -log(p[blank,0] + p[l_0,0]),
+ *                         as the reference's un-windowed initialisation does (:42-47), and skips when that is 0;
+ *   no alignment (P=0) -> skip with a zero gradient (the reference's ZeroDivisionError, :147-149).
+ * g = p - gamma, gamma[k,t] = sum over states s of label k of exp(la[s,t] + lb[s,t] - log p[k,t] - log P).
+ */
+static double lse2(double a, double b)
+{
+    double m = a > b ? a : b;
+    if (m == -INFINITY) return -INFINITY;
+    return m + log(exp(a - m) + exp(b - m));
+}
+
+static double lse3(double a, double b, double c)
+{
+    double m = a > b ? a : b;
+    m = m > c ? m : c;
+    if (m == -INFINITY) return -INFINITY;
+    return m + log(exp(a - m) + exp(b - m) + exp(c - m));
+}
+
+int ctc_oracle_loss_log(const double *params, int K, int T, const int *seq, int seqLen,
+                        int blank, double *grad, double *nll)
+{
+    int L = 2 * seqLen + 1, t, s, k;
+    int *lab = (int *)malloc((size_t)L * sizeof(int));
+    double *la, *lb, *lp, logP;
+    memset(grad, 0, (size_t)K * T * sizeof(double));
+    for (s = 0; s < L; s++) lab[s] = (s % 2 == 0) ? blank : seq[(s - 1) / 2];
+
+    if (T == 1) {                                      /* the reference's normaliser of frame 0 */
+        double c = P(blank, 0) + P(seq[0], 0);
+        if (c == 0.0) { *nll = -log(c); free(lab); return 1; }
+        *nll = -log(c);
+    } else if (T < seqLen) {
+        *nll = INFINITY;
+    }
+    if (T < seqLen) {
+        for (t = 0; t < T; t++)
+            for (k = 0; k < K; k++) G(k, t) = P(k, t);
+        free(lab);
+        return 0;
+    }
+
+    la = (double *)malloc((size_t)L * T * sizeof(double));
+    lb = (double *)malloc((size_t)L * T * sizeof(double));
+    lp = (double *)malloc((size_t)K * T * sizeof(double));
+    for (t = 0; t < T; t++)
+        for (k = 0; k < K; k++) lp[(size_t)k + (size_t)K * t] = log(P(k, t));
+#define LP(k, t) lp[(size_t)(k) + (size_t)K * (size_t)(t)]
+#define LA(s, t) la[(size_t)(s) + (size_t)L * (size_t)(t)]
+#define LB(s, t) lb[(size_t)(s) + (size_t)L * (size_t)(t)]
+    for (s = 0; s < L; s++) LA(s, 0) = (s < 2) ? LP(lab[s], 0) : -INFINITY;
+    for (t = 1; t < T; t++)
+        for (s = 0; s < L; s++) {
+            double x;
+            if (s == 0) x = LA(0, t - 1);
+            else if (s % 2 == 0 || s == 1 || lab[s] == lab[s - 2]) x = lse2(LA(s, t - 1), LA(s - 1, t - 1));
+            else x = lse3(LA(s, t - 1), LA(s - 1, t - 1), LA(s - 2, t - 1));
+            LA(s, t) = x + LP(lab[s], t);
+        }
+    for (s = 0; s < L; s++) LB(s, T - 1) = (s >= L - 2) ? LP(lab[s], T - 1) : -INFINITY;
+    for (t = T - 2; t >= 0; t--)
+        for (s = L - 1; s >= 0; s--) {
+            double x;
+            if (s == L - 1) x = LB(s, t + 1);
+            else if (s % 2 == 0 || s == L - 2 || lab[s] == lab[s + 2]) x = lse2(LB(s, t + 1), LB(s + 1, t + 1));
+            else x = lse3(LB(s, t + 1), LB(s + 1, t + 1), LB(s + 2, t + 1));
+            LB(s, t) = x + LP(lab[s], t);
+        }
+    logP = (L > 1) ? lse2(LA(L - 1, T - 1), LA(L - 2, T - 1)) : LA(0, T - 1);
+    if (logP == -INFINITY) {
+        free(la); free(lb); free(lp);
+        free(lab);
+        if (T == 1) {                                  /* the reference: absum == 0 leaves grad = p */
+            for (k = 0; k < K; k++) G(k, 0) = P(k, 0);
+            return 0;
+        }
+        *nll = INFINITY;                               /* no alignment: skip, gradient all zeros */
+        return 1;
+    }
+    if (T > 1) *nll = -logP;
+    for (t = 0; t < T; t++)
+        for (s = 0; s < L; s++) {
+            double e = LA(s, t) + LB(s, t);
+            if (e != -INFINITY) G(lab[s], t) += exp(e - LP(lab[s], t) - logP);
+        }
+    for (t = 0; t < T; t++)
+        for (k = 0; k < K; k++) G(k, t) = P(k, t) - G(k, t);
+#undef LP
+#undef LA
+#undef LB
+    free(lab); free(la); free(lb); free(lp);
+    return 0;
 }
 
 /* ctc_fast.pyx:154-187 -- per-frame argmax, collapse repeats, drop blank and labels 1,2,8.

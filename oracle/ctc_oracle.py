@@ -39,6 +39,10 @@ def _lib():
         _LIB.ctc_oracle_loss.restype = ctypes.c_int
         _LIB.ctc_oracle_loss.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                          ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]
+        _LIB.ctc_oracle_loss_fb.restype = ctypes.c_int
+        _LIB.ctc_oracle_loss_fb.argtypes = _LIB.ctc_oracle_loss.argtypes + [ctypes.c_void_p]
+        _LIB.ctc_oracle_loss_log.restype = ctypes.c_int
+        _LIB.ctc_oracle_loss_log.argtypes = _LIB.ctc_oracle_loss.argtypes
         _LIB.ctc_oracle_best_path.restype = ctypes.c_int
         _LIB.ctc_oracle_best_path.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                               ctypes.c_void_p, ctypes.c_void_p]
@@ -51,9 +55,7 @@ def _lib():
     return _LIB
 
 
-def ctc_loss(params, seq, blank=0):
-    """Same contract as the reference ctc_loss (ctc_fast.pyx:13-14,152): params K x T float64
-    Fortran-contiguous, seq int32; returns (nll, grad K x T float64 F-order, skip)."""
+def _call(fn, params, seq, blank, *extra):
     if not (isinstance(params, np.ndarray) and params.dtype == np.float64 and params.ndim == 2
             and params.flags.f_contiguous):
         raise ValueError("ndarray is not Fortran contiguous")
@@ -61,9 +63,29 @@ def ctc_loss(params, seq, blank=0):
     K, T = params.shape
     grad = np.zeros((K, T), dtype=np.float64, order="F")
     nll = ctypes.c_double(0.0)
-    skip = _lib().ctc_oracle_loss(params.ctypes.data, K, T, seq.ctypes.data, seq.shape[0], int(blank),
-                                  grad.ctypes.data, ctypes.addressof(nll))
+    skip = fn(params.ctypes.data, K, T, seq.ctypes.data, seq.shape[0], int(blank), grad.ctypes.data,
+              ctypes.addressof(nll), *extra)
     return nll.value, grad, bool(skip)
+
+
+def ctc_loss(params, seq, blank=0):
+    """Same contract as the reference ctc_loss (ctc_fast.pyx:13-14,152): params K x T float64
+    Fortran-contiguous, seq int32; returns (nll, grad K x T float64 F-order, skip)."""
+    return _call(_lib().ctc_oracle_loss, params, seq, blank)
+
+
+def ctc_loss_fb(params, seq, blank=0):
+    """ctc_loss, plus the llBackward the reference computes and discards: (nll, grad, skip, llBackward).
+    -nll == llBackward up to rounding unless the per-frame normalised trellis lost mass to underflow."""
+    llb = ctypes.c_double(0.0)
+    nll, grad, skip = _call(_lib().ctc_oracle_loss_fb, params, seq, blank, ctypes.addressof(llb))
+    return nll, grad, skip, llb.value
+
+
+def ctc_loss_log(params, seq, blank=0):
+    """The same contract computed in the log domain (float64 log-sum-exp, no per-frame scaling): correct where the
+    reference's products of normalised alpha and beta leave float64's range (long, unaligned utterances)."""
+    return _call(_lib().ctc_oracle_loss_log, params, seq, blank)
 
 
 def decode_best_path(probs, blank=0):

@@ -7,6 +7,10 @@
 Both keep the reference's argument contract (params: K x T float64 Fortran-contiguous ndarray of
 per-frame probability distributions, seq: int32 labels) and error behaviour (ValueError for a
 non-Fortran array; numerical infeasibility is reported through skip=True, never raised).
+Where the reference's own float64 arithmetic runs out of range (long utterances with unaligned outputs) the
+results differ from it on purpose: occupancies the reference loses to underflow (its gradient rows left at p)
+are computed, and an utterance whose scaled trellis lost mass (where the reference returns a wrong loss) is
+reported as skip=True with a zero gradient.  DESIGN.md section 4 has the measurements.
 The batched, zero-copy entry `ctc_loss_batch` is what nnets.brnnet uses internally through the
 C ABI; it is exported for callers that already hold activations on the device.
 """

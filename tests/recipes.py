@@ -204,6 +204,85 @@ def random_bf_cases():
         yield np.asfortranarray(probs), seq
 
 
+# ---- batches for the GPU CTC kernel (tests/test_ctc_plans_gpu.py, tests/test_ctc_range_gpu.py) -------------------
+class Batch:
+    """B utterances with element (u, t, k) at off + u*us + t*fs + k of one float32 buffer; gaps hold NaN."""
+
+    def __init__(self, x, lens, seqs, is_prob=False, blank=0, layout="bt", fs_pad=0, off=0):
+        B, Tmax, K = x.shape
+        self.x, self.lens, self.seqs, self.is_prob, self.blank = x, list(lens), list(seqs), is_prob, blank
+        self.B, self.Tmax, self.K = B, Tmax, K
+        if layout == "bt":
+            self.fs = K + fs_pad
+            self.us = Tmax * self.fs
+        else:                       # time-major, as the BRNN lays its logits out: [Tmax][B][K]
+            self.us = K + fs_pad
+            self.fs = B * self.us
+        self.off = off
+        self.n = off + (B - 1) * self.us + (Tmax - 1) * self.fs + K
+        self.idx = (off + np.arange(B)[:, None, None] * self.us + np.arange(Tmax)[None, :, None] * self.fs
+                    + np.arange(K)[None, None, :])
+
+    def flat(self, fill):
+        buf = np.full(self.n + 2, fill, dtype=np.float32)
+        buf[self.idx] = self.x
+        return buf
+
+
+def softmax64(x):
+    """Row softmax in float64 of an (n, K) array."""
+    x = x.astype(np.float64)
+    e = np.exp(x - x.max(axis=1, keepdims=True))
+    return e / e.sum(axis=1, keepdims=True)
+
+
+def ctc_labels(rng, n, K, blank, repeats=0.0):
+    """n labels over the non-blank classes; `repeats`: probability that a label repeats its predecessor."""
+    cls = np.array([k for k in range(K) if k != blank])
+    s = cls[rng.randint(0, len(cls), size=n)]
+    for i in range(1, n):
+        if rng.rand() < repeats:
+            s[i] = s[i - 1]
+    return s.astype(np.int32)
+
+
+def ctc_batch(B, T, K, L, seed, is_prob=False, blank=0, ragged=True, scale=2.0, repeats=0.1, **layout):
+    """Logits ~ N(0, scale^2) (or their float32 softmax, is_prob), labels from ctc_labels; ragged: the first utterance
+    is the longest (T frames, L labels), the others mostly feasible."""
+    rng = np.random.RandomState(seed)
+    x = (rng.randn(B, T, K) * scale).astype(np.float32)
+    lens = [T] * B
+    nl = [L] * B
+    if ragged and B > 1:
+        lens = [T] + [int(v) for v in rng.randint(max(1, 3 * T // 4), T + 1, size=B - 1)]
+        nl = [L] + [int(rng.randint(max(1, L // 2), max(max(1, L // 2), min(L, 4 * t // 5)) + 1)) for t in lens[1:]]
+    seqs = [ctc_labels(rng, nl[u], K, blank, repeats=repeats) for u in range(B)]
+    if is_prob:
+        x = softmax64(x.reshape(B * T, K)).reshape(B, T, K).astype(np.float32)
+    return Batch(x, lens, seqs, is_prob=is_prob, blank=blank, **layout)
+
+
+def ctc_trellis_edges(K=12, seed=5):
+    """(T, labels) of one utterance per edge of the trellis, to be run as one batch."""
+    rng = np.random.RandomState(seed)
+    rows = []
+    distinct = lambda n: (1 + rng.permutation(K - 1)[:n]).astype(np.int32)
+
+    def add(T, s):
+        rows.append((T, np.asarray(s, np.int32)))
+    add(1, [3]); add(2, [3]); add(3, [3, 4])                         # T = 1, 2, 3
+    add(1, [2, 5])                                                   # one frame, two labels: finite, see short_utt_nll
+    add(5, distinct(5))                                              # T = |l|, distinct: one path
+    add(5, [1, 2, 2, 3, 4])                                          # T = |l| with a repeat: infeasible -> skip
+    add(6, [1, 2, 2, 3, 4])                                          # T = |l| + repeats: one path again
+    add(10, [1, 1, 1, 2, 2, 2])                                      # T = |l| + repeats, runs
+    add(4, [5, 6, 7, 8, 9, 10])                                      # T < |l|: inf
+    add(90, [7] * 31)                                                # a run of repeats across lane boundaries
+    add(80, np.repeat(distinct(4), 8)[:30])                          # runs crossing pair i = lane * P + j
+    add(70, distinct(11))
+    return rows
+
+
 def digest(a):
     """SHA-256 of a float64 array's values (row-major, every NaN canonical) as 32 uint8: a stored stand-in for a
     bit-exact comparison with an array that is too large to keep."""

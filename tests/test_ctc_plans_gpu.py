@@ -20,8 +20,10 @@ import time
 import numpy as np
 import pytest
 
+import recipes
 from oracle import ctc_oracle
-from recipes import knobs  # noqa: F401  (fixture)
+from recipes import Batch, knobs  # noqa: F401  (knobs: fixture)
+from recipes import ctc_batch as _make, softmax64 as _softmax64
 
 pytestmark = pytest.mark.gpu
 H100_SMS = 132             # the plans below are laid out for the 132-SM H100 SXM; other parts skip a plan they cannot reach
@@ -69,30 +71,6 @@ def force(knobs, cuda):
 
 
 # ------------------------------------------------------------------------------------------------ one batch
-class Batch:
-    """B utterances with element (u, t, k) at off + u*us + t*fs + k of one float32 buffer; gaps hold NaN."""
-
-    def __init__(self, x, lens, seqs, is_prob=False, blank=0, layout="bt", fs_pad=0, off=0):
-        B, Tmax, K = x.shape
-        self.x, self.lens, self.seqs, self.is_prob, self.blank = x, list(lens), list(seqs), is_prob, blank
-        self.B, self.Tmax, self.K = B, Tmax, K
-        if layout == "bt":
-            self.fs = K + fs_pad
-            self.us = Tmax * self.fs
-        else:                       # time-major, as the BRNN lays its logits out: [Tmax][B][K]
-            self.us = K + fs_pad
-            self.fs = B * self.us
-        self.off = off
-        self.n = off + (B - 1) * self.us + (Tmax - 1) * self.fs + K
-        self.idx = (off + np.arange(B)[:, None, None] * self.us + np.arange(Tmax)[None, :, None] * self.fs
-                    + np.arange(K)[None, None, :])
-
-    def flat(self, fill):
-        buf = np.full(self.n + 2, fill, dtype=np.float32)
-        buf[self.idx] = self.x
-        return buf
-
-
 def _run(torch, b, max_labels=None, plan_expect=None, what="", check_rc=True):
     """Launch ctcb_ctc_loss_grad_f32 on batch b; returns (plan, nll, grad[B][Tmax][K], skip, gaps of the gradient)."""
     import _ctcb
@@ -124,12 +102,6 @@ def _run(torch, b, max_labels=None, plan_expect=None, what="", check_rc=True):
     mask = np.ones(g.shape, bool)
     mask[b.idx] = False
     return plan, nll.cpu().numpy().astype(np.float64), g[b.idx].astype(np.float64), skip.cpu().numpy(), g[mask]
-
-
-def _softmax64(x):
-    x = x.astype(np.float64)
-    e = np.exp(x - x.max(axis=1, keepdims=True))
-    return e / e.sum(axis=1, keepdims=True)
 
 
 def _compare(b, res, utts=None):
@@ -173,31 +145,7 @@ def _report(name, plan, gerr, nerr, n, t0, **extra):
     assert nerr <= nb, (name, nerr, nb)
 
 
-# ------------------------------------------------------------------------------------------------ batch builders
-def _labels(rng, n, K, blank, T=None, repeats=0.0):
-    """n labels over the non-blank classes; `repeats`: probability that a label repeats its predecessor."""
-    cls = np.array([k for k in range(K) if k != blank])
-    s = cls[rng.randint(0, len(cls), size=n)]
-    for i in range(1, n):
-        if rng.rand() < repeats:
-            s[i] = s[i - 1]
-    return s.astype(np.int32)
-
-
-def _make(B, T, K, L, seed, is_prob=False, blank=0, ragged=True, scale=2.0, repeats=0.1, **layout):
-    rng = np.random.RandomState(seed)
-    x = (rng.randn(B, T, K) * scale).astype(np.float32)
-    lens = [T] * B
-    nl = [L] * B
-    if ragged and B > 1:                # the first utterance is the longest; the others mostly feasible
-        lens = [T] + [int(v) for v in rng.randint(max(1, 3 * T // 4), T + 1, size=B - 1)]
-        nl = [L] + [int(rng.randint(max(1, L // 2), max(max(1, L // 2), min(L, 4 * t // 5)) + 1)) for t in lens[1:]]
-    seqs = [_labels(rng, nl[u], K, blank, repeats=repeats) for u in range(B)]
-    if is_prob:
-        x = _softmax64(x.reshape(B * T, K)).reshape(B, T, K).astype(np.float32)
-    return Batch(x, lens, seqs, is_prob=is_prob, blank=blank, **layout)
-
-
+# ------------------------------------------------------------------------------------------------ cases
 def _case(torch, force, name, b, expect, forced="auto", utts=None, max_labels=None):
     t0 = time.time()
     force(forced)
@@ -344,32 +292,11 @@ def test_blank_position(kern, forced, B, blank, cuda, force):
 
 
 # ------------------------------------------------------------------------------------------------ trellis edges
-def _trellis_batch(K=12, seed=5):
-    """One utterance per edge, all in one batch."""
-    rng = np.random.RandomState(seed)
-    rows = []
-    distinct = lambda n: (1 + rng.permutation(K - 1)[:n]).astype(np.int32)
-
-    def add(T, s):
-        rows.append((T, np.asarray(s, np.int32)))
-    add(1, [3]); add(2, [3]); add(3, [3, 4])                         # T = 1, 2, 3
-    add(1, [2, 5])                                                   # one frame, two labels: finite, see short_utt_nll
-    add(5, distinct(5))                                              # T = |l|, distinct: one path
-    add(5, [1, 2, 2, 3, 4])                                          # T = |l| with a repeat: infeasible -> skip
-    add(6, [1, 2, 2, 3, 4])                                          # T = |l| + repeats: one path again
-    add(10, [1, 1, 1, 2, 2, 2])                                      # T = |l| + repeats, runs
-    add(4, [5, 6, 7, 8, 9, 10])                                      # T < |l|: inf
-    add(90, [7] * 31)                                                # a run of repeats across lane boundaries
-    add(80, np.repeat(distinct(4), 8)[:30])                          # runs crossing pair i = lane * P + j
-    add(70, distinct(11))
-    return rows
-
-
 @pytest.mark.parametrize("P", [1, 2, 4])
 @pytest.mark.parametrize("kern,forced", [("par", "auto"), ("pair", "pair"), ("ckpt", "ckpt"), ("warp", "warp")])
 def test_trellis_edges(kern, forced, P, cuda, force):
     K = 12
-    rows = _trellis_batch(K)
+    rows = recipes.ctc_trellis_edges(K)
     Tmax = max(T for T, _ in rows)
     rng = np.random.RandomState(P)
     x = (rng.randn(len(rows), Tmax, K) * 1.5).astype(np.float32)
@@ -422,8 +349,9 @@ def test_zero_mass(kern, forced, cuda, force):
 def test_long_utterance_5000_frames(cuda, force):
     """A C4-length utterance: the float32 sum of log Z over 5000 frames and 300 labels (P = 16), logits and
     probabilities, on the default plan for one utterance.  The logits favour each label on a few frames of its own
-    segment, as a trained net's do.  (With logits that carry no alignment at all, the gradient of one frame differed from
-    the reference's; see DESIGN.md section 4.)"""
+    segment, as a trained net's do, which keeps the reference's scaled trellis in range.  Logits with no alignment at
+    all take the reference out of float64's range; test_ctc_range_gpu.py holds the kernel to the log-domain oracle there
+    (DESIGN.md section 4)."""
     T, K, L = 5000, 35, 300
     for is_prob in (False, True):
         b = _make(1, T, K, L, seed=11, ragged=False)
