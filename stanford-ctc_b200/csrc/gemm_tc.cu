@@ -8,22 +8,26 @@
 // and a product is three MMAs accumulated in fp32:  lo.hi + hi.lo + hi.hi
 // (the dropped lo.lo term is ~2^-20 relative) -- "3xTF32", ~1e-6 relative error per product.
 //
-// Kernel shape: C[M x N] = A[M x K] . B[N x K]^T.  wgmma reads .tf32 operands K-major only, so every tile reaches the
-// consumers K-major and 128-byte swizzled, however the operand is stored:
-//   K-major operand (A as [M][K], B as [N][K]): TMA writes the tile swizzled into the value slot;
-//   MN-major operand (A as [K][M], B as [K][N], e.g. the time-major activations of a weight gradient over T*B rows):
-//     TMA writes the [32 k][rows] box unswizzled into the LOW-HALF slot, and the producer transposes it into the
-//     swizzled value slot while it computes the low halves.  The wgmma then reads the same bytes as if a transposed
-//     copy had been loaded, so both ways give identical results.
+// Kernel shape: C[M x N] = A[M x K] . B[N x K]^T.  wgmma reads .tf32 operands K-major only.  A reaches the MMAs from
+// registers, B from shared memory by descriptor, 128-byte swizzled:
+//   A: TMA writes the tile 128B-swizzled into the A slot, as one [rows][32 k] box (K-major, [M][K]) or as four
+//     [32 k][32 rows] boxes (MN-major, [K][M], e.g. the time-major deltas of a weight gradient over T*B rows); each
+//     consumer loads its fragments from it and splits them into hi and lo in registers (tc_load_split_a), conflict-free.
+//   B: a K-major tile ([N][K]) lands swizzled in the value slot; an MN-major one ([K][N]) lands unswizzled in the
+//     LOW-HALF slot and the producer transposes it into the swizzled value slot while it computes the low halves.  The
+//     wgmma then reads the same bytes as if a transposed copy had been loaded, so both ways give identical results.
 //   An operand TMA cannot describe (row pitch not a multiple of 16 bytes, base not 16-byte aligned) is re-pitched or
 //   transposed into the workspace by a prep kernel first (also forced by CTCB_GEMM_TC_COPY=1).
 // One CTA (3 warpgroups) per 128 x BN output tile, K split and problem (gridDim.z = problems x splits):
 //   warpgroup 0 : producer -- one elected thread TMA-loads the A and B tiles of each k-block of 32 floats into a
-//                 STAGES-deep ring (mbarrier complete_tx); the 128 threads then write the low halves of both tiles
-//                 next to them (and the transposed values of an MN-major tile) and signal the consumers;
-//   warpgroups 1, 2 : consumers -- rows 0..63 / 64..127 of the tile: 4 k-steps x 3 wgmma (m64 x BN x k8) per k-block
-//                 with the accumulator in registers, one k-block in flight while the previous slot is released; then
-//                 the fused alpha/beta/bias/ReLU/mask epilogue (or the split-K partial) straight from registers.
+//                 STAGES-deep ring (mbarrier complete_tx); the 128 threads then write the low half of the B tile next
+//                 to it (and its transposed values when it is MN-major) and signal the consumers;
+//   warpgroups 1, 2 : consumers -- rows 0..63 / 64..127 of the tile: per k-block, load and split the A fragments, then
+//                 4 k-steps x 3 wgmma (m64 x BN x k8, A from registers) with the accumulator in registers, wait for them
+//                 and release the slot; then the fused alpha/beta/bias/ReLU/mask epilogue (or the split-K partial)
+//                 straight from registers.
+// Each product sees the same hi and lo values and the MMAs run in the same order whichever way an operand arrives, so
+// the results do not depend on the operand path.
 // Two problems of the same shape (the two recurrent weight gradients) can share one launch and one split-K reduce.
 #include "common.cuh"
 #include "wgmma.cuh"
@@ -146,19 +150,56 @@ struct TcTile {
     }
 };
 
-// A stage holds [A value | A low half | B value | B low half], each tile 1024-byte aligned.  A_MN / B_MN: the operand is
-// MN-major in global memory (its TMA box lands in the low-half slot, see TcTile).
+// The consumers' A fragments (WgmmaTf32Rs) of one k-block, read from the A slot and split in registers: hi[4 kk + i] is
+// register i of k-step kk as stored (the MMA reads its TF32 part), lo the same minus its TF32 part, tc_lo4's arithmetic.
+// Thread (warp q of consumer cw, lane = 4 g + t) holds the tile rows of fragment rows g and g + 8 at k = 8 kk + t (+ 4).
+//   K-major A (one 128 x 32 box, 128B-swizzled): row r at r * 128, k-quad c at ((c ^ (r % 8)) << 4), with fragment row
+//     r = 64 cw + 16 q + g (+ 8), so r % 8 = g.  A warp's load reads k-quad 2 kk (+ 1) ^ g for its 8 g and word t of
+//     it: 32 different banks.
+//   MN-major A (four 32 k x 32 m boxes, 128B-swizzled, box j holds rows 32 j .. 32 j + 31): element (m, k) of a box lies
+//     at k * 128 + (((m / 4) ^ (k % 8)) << 4) + (m % 4) * 4, so the bank is 4 ((m / 4) ^ (k % 8)) + m % 4.  Reading the
+//     fragment rows as consecutive m (the warp reads 8 m x 4 k) would put two lanes on each bank.  So fragment row
+//     (q, g, h) of consumer cw (h: the + 8 row) reads tile row  64 cw + 32 (q / 2) + 8 (q % 2) + 4 h + 16 (g / 4) + g % 4
+//     (a bijection of the 128 rows; tc_tile_row gives it to the epilogue): the 8 g of a load take the m-quads
+//     c and c + 4 (c = 2 (q % 2) + h) and m % 4 = g % 4, so with k % 8 = t (+ 4) the banks 4 ((c + 4 (g / 4)) ^ k % 8) + g % 4
+//     are 32 different ones.
+template <bool A_MN>
+__device__ __forceinline__ int tc_tile_row(int cw, int q, int g, int h) {
+    return A_MN ? 64 * cw + 32 * (q >> 1) + 8 * (q & 1) + 4 * h + 16 * (g >> 2) + (g & 3) : 64 * cw + 16 * q + g + 8 * h;
+}
+template <bool A_MN>
+__device__ __forceinline__ void tc_load_split_a(uint32_t sA, int cw, int q, int g, int t, uint32_t (&hi)[16],
+                                                uint32_t (&lo)[16]) {
+    // offsets of k-step kk, register i: the swizzle bits (4..6) are XORed in, the rest added
+    const uint32_t p = A_MN ? sA + (2 * cw + (q >> 1)) * 4096 + t * 128 + (((2 * (q & 1) + 4 * (g >> 2)) ^ t) << 4) + (g & 3) * 4
+                            : sA + (64 * cw + 16 * q + g) * 128 + (g << 4) + t * 4;
+#pragma unroll
+    for (int kk = 0; kk < TC_BK / 8; ++kk) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const uint32_t a = A_MN ? ((p + kk * 1024 + (i >> 1) * 512) ^ (((i & 1) << 4) | ((i >> 1) << 6)))
+                                    : ((p ^ ((2 * kk + (i >> 1)) << 4)) + (i & 1) * 1024);
+            uint32_t x;
+            asm volatile("ld.shared.b32 %0, [%1];" : "=r"(x) : "r"(a));
+            hi[4 * kk + i] = x;
+            lo[4 * kk + i] = __float_as_uint(__fsub_rn(__uint_as_float(x), __uint_as_float(x & 0xffffe000u)));
+        }
+    }
+}
+
+// A stage holds [A value | B value | B low half], each tile 1024-byte aligned.  A_MN / B_MN: the operand is MN-major in
+// global memory (A: four swizzled 32-row boxes, see tc_load_split_a; B: its TMA box lands in the low-half slot, see TcTile).
 template <int BN, int STAGES, bool A_MN, bool B_MN>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmB0,
                const __grid_constant__ CUtensorMap tmA1, const __grid_constant__ CUtensorMap tmB1, GemmTcArgs g) {
     constexpr uint32_t A_BYTES = TC_BM * TC_BK * 4, B_BYTES = BN * TC_BK * 4;
-    constexpr uint32_t B_OFF = 2 * A_BYTES;
+    constexpr uint32_t B_OFF = A_BYTES;
     constexpr uint32_t STAGE_BYTES = B_OFF + 2 * B_BYTES;
     extern __shared__ __align__(1024) uint8_t tc_smem[];
     // 1024-byte alignment is required by SWIZZLE_128B: align manually (dynamic smem base is only 16B-aligned by contract)
     uint8_t *base = (uint8_t *)(((uintptr_t)tc_smem + 1023) & ~(uintptr_t)1023);
-    // full[STAGES] (TMA landed), empty[STAGES] (consumers done with the slot), ready[STAGES] (low halves written)
+    // full[STAGES] (TMA landed), empty[STAGES] (consumers done with the slot), ready[STAGES] (B's low half written)
     uint64_t *full = reinterpret_cast<uint64_t *>(base + STAGES * STAGE_BYTES);
     uint64_t *empty = full + STAGES, *ready = full + 2 * STAGES;
 
@@ -183,15 +224,15 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__
     if (wg == 0) {
         // ---------------------------------------------------------------- producer: TMA issue runs STAGES - 1 k-blocks
         // ahead of the split.  Split first, then issue: the slot of block i is freed by the consumers once they have
-        // started on block i - STAGES + 1, whose low halves this very iteration provides.
+        // finished block i - STAGES, and they can only start the block after it once this very iteration provides it.
         const CUtensorMap *tmA = prob ? &tmA1 : &tmA0, *tmB = prob ? &tmB1 : &tmB0;
         if (threadIdx.x == 0) {
             asm volatile("prefetch.tensormap [%0];" ::"l"(tmA) : "memory");
             asm volatile("prefetch.tensormap [%0];" ::"l"(tmB) : "memory");
         }
         constexpr int LA = STAGES - 1;
-        // an MN-major box lands in the low-half slot, a K-major one in the value slot
-        constexpr uint32_t A_DST = A_MN ? A_BYTES : 0, B_DST = B_OFF + (B_MN ? B_BYTES : 0);
+        // an MN-major B box lands in the low-half slot, a K-major one in the value slot
+        constexpr uint32_t B_DST = B_OFF + (B_MN ? B_BYTES : 0);
         for (int i = 0; i < nkb + LA; ++i) {
             const int j = i - LA;
             if (j >= 0) {
@@ -199,11 +240,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__
                 tc_mbar_wait(tc_smem_u32(&full[s]), (uint32_t)(use & 1));
                 if (threadIdx.x == 0) TC_STAMP(j, 1);
                 uint8_t *st = base + s * STAGE_BYTES;
-                float4 va[TcTile<TC_BM, A_MN>::Q], vb[TcTile<BN, B_MN>::Q];    // every load first, then every store
-                TcTile<TC_BM, A_MN>::load(st, st + A_BYTES, va);
+                float4 vb[TcTile<BN, B_MN>::Q];    // every load first, then every store
                 TcTile<BN, B_MN>::load(st + B_OFF, st + B_OFF + B_BYTES, vb);
-                if (A_MN || B_MN) asm volatile("bar.sync 1, 128;" ::: "memory");   // the producer warpgroup only
-                TcTile<TC_BM, A_MN>::store(st, st + A_BYTES, va);
+                if (B_MN) asm volatile("bar.sync 1, 128;" ::: "memory");   // the producer warpgroup only
                 TcTile<BN, B_MN>::store(st + B_OFF, st + B_OFF + B_BYTES, vb);
                 asm volatile("fence.proxy.async.shared::cta;" ::: "memory");    // generic writes -> tensor-core (async) proxy
                 __syncwarp();
@@ -219,7 +258,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__
                 TC_STAMP(i, 0);
                 tc_mbar_expect_tx(fb, A_BYTES + B_BYTES);
                 // coordinates innermost first: (k, row) for a K-major map, (row, k) for an MN-major one
-                tc_tma_load_2d(sa + A_DST, tmA, fb, A_MN ? m0 : k, A_MN ? k : m0);
+                if (A_MN) {
+#pragma unroll
+                    for (int b = 0; b < TC_BM / 32; ++b) tc_tma_load_2d(sa + b * 4096, tmA, fb, m0 + 32 * b, k);
+                } else {
+                    tc_tma_load_2d(sa, tmA, fb, k, m0);
+                }
                 tc_tma_load_2d(sa + B_DST, tmB, fb, B_MN ? n0 : k, B_MN ? k : n0);
             }
         }
@@ -228,43 +272,43 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__
 
     // -------------------------------------------------------------------- consumers
     const int cw = wg - 1;                                        // rows 64 cw .. 64 cw + 63 of the tile
+    const int q = warp & 3;
     float acc[BN / 2];
 #pragma unroll
     for (int r = 0; r < BN / 2; ++r) acc[r] = 0.f;
+    // The A fragments of a k-block are read by its MMAs until they retire, so they cannot be rewritten for the next
+    // k-block while those are in flight (ptxas serializes the wgmma pipeline if they are).  Each consumer therefore waits
+    // for its k-block's MMAs before the next: the other consumer's MMAs keep the tensor pipe busy meanwhile, and the
+    // slot goes back to the producer one k-block earlier than with one k-block in flight.
+    uint32_t ah[16], al[16];
     for (int i = 0; i < nkb; ++i) {
         const int s = i % STAGES, use = i / STAGES;
-        tc_mbar_wait(tc_smem_u32(&ready[s]), (uint32_t)(use & 1));      // hi landed and lo written
+        tc_mbar_wait(tc_smem_u32(&ready[s]), (uint32_t)(use & 1));      // A and B landed, B's low half written
+        tc_mbar_wait(tc_smem_u32(&full[s]), (uint32_t)(use & 1));       // (complete by now) the TMA writes these loads read
         if (threadIdx.x == 128) TC_STAMP(i, 3);
-        const uint32_t sa = tc_smem_u32(base + s * STAGE_BYTES) + (uint32_t)cw * (64 * 128);
-        const uint32_t sb = tc_smem_u32(base + s * STAGE_BYTES) + B_OFF;
-        const uint64_t dA = wg_desc(sa), dAl = wg_desc(sa + A_BYTES), dB = wg_desc(sb), dBl = wg_desc(sb + B_BYTES);
+        const uint32_t sa = tc_smem_u32(base + s * STAGE_BYTES);
+        tc_load_split_a<A_MN>(sa, cw, q, lane >> 2, lane & 3, ah, al);
+        const uint64_t dB = wg_desc(sa + B_OFF), dBl = wg_desc(sa + B_OFF + B_BYTES);
         wg_fence();
 #pragma unroll
         for (int k8 = 0; k8 < TC_BK / 8; ++k8) {
             const uint64_t adv = (uint64_t)((k8 * 32) >> 4);
-            WgmmaTf32<BN>::mma(acc, dAl + adv, dB + adv, (i > 0 || k8 > 0) ? 1u : 0u);   // lo . hi
-            WgmmaTf32<BN>::mma(acc, dA + adv, dBl + adv, 1u);                            // hi . lo
-            WgmmaTf32<BN>::mma(acc, dA + adv, dB + adv, 1u);                             // hi . hi
+            WgmmaTf32Rs<BN>::mma(acc, al + 4 * k8, dB + adv, (i > 0 || k8 > 0) ? 1u : 0u);   // lo . hi
+            WgmmaTf32Rs<BN>::mma(acc, ah + 4 * k8, dBl + adv, 1u);                            // hi . lo
+            WgmmaTf32Rs<BN>::mma(acc, ah + 4 * k8, dB + adv, 1u);                             // hi . hi
         }
         wg_commit();
         if (threadIdx.x == 128) TC_STAMP(i, 4);
-        // the previous k-block's MMAs are complete once at most this one is outstanding: release its slot
-        wg_wait<1>();
-        if (i > 0) {
-            __syncwarp();
-            if (lane == 0) tc_mbar_arrive(tc_smem_u32(&empty[(i - 1) % STAGES]));
-        }
+        wg_wait<0>();
+        __syncwarp();
+        if (lane == 0) tc_mbar_arrive(tc_smem_u32(&empty[s]));
     }
-    wg_wait<0>();
-    // (the last slot is never waited for again: nothing is loaded after it)
 
     // -------------------------------------------------------------------- epilogue straight from the accumulator
-    const int q = warp & 3;
     float *const Cp = prob ? g.C[1] : g.C[0];     // (a select: indexing the parameter array would copy it to the stack)
-    const int rbase = m0 + 64 * cw + 16 * q + (lane >> 2);
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-        const int m = rbase + 8 * h;
+        const int m = m0 + tc_tile_row<A_MN>(cw, q, lane >> 2, h);
         if (m >= g.M) continue;
         float *drow = g.partial ? g.partial + ((int64_t)blockIdx.z * g.M + m) * g.N : Cp + (int64_t)m * g.ldc;
 #pragma unroll
@@ -362,8 +406,9 @@ static EncodeTiledFn get_encode() {
 }
 
 // fp32 2-D tensor map with pitch ld (elements).  K-major (mn = 0): rows x K, box = 32 floats x box_rows, 128B swizzle
-// (the layout the wgmma descriptors read).  MN-major (mn = 1): K x rows, box = box_rows floats x 32, no swizzle (the
-// producer transposes it).  Out-of-bounds elements read as 0 either way.
+// (the layout the wgmma descriptors read).  MN-major (mn = 1): K x rows, box = box_rows floats x 32, 128B-swizzled when
+// box_rows is 32 (A: the consumers read their fragments from it) and unswizzled otherwise (B: the producer transposes it).
+// Out-of-bounds elements read as 0 either way.
 static int make_map(CUtensorMap *m, const float *ptr, int rows, int K, int64_t ld, int box_rows, bool mn) {
     EncodeTiledFn enc = get_encode();
     if (!enc) return set_error(CTCB_ECUDA, "cuTensorMapEncodeTiled is not available from this driver");
@@ -376,7 +421,7 @@ static int make_map(CUtensorMap *m, const float *ptr, int rows, int K, int64_t l
         box[0] = (cuuint32_t)box_rows; box[1] = (cuuint32_t)TC_BK;
     }
     CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void *)ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     mn ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                     (mn && box_rows != TC_BK) ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS)
         return set_error(CTCB_ECUDA, "cuTensorMapEncodeTiled failed (%d) rows=%d K=%d ld=%lld mn=%d", (int)r, rows, K, (long long)ld, (int)mn);
@@ -480,7 +525,7 @@ size_t gemm_tc_pair_workspace_bytes(int M, int N, int K) {
 
 template <int BN, int STAGES, bool A_MN, bool B_MN>
 static int launch_tc(const CUtensorMap *tA, const CUtensorMap *tB, const GemmTcArgs &g, int ctas_z, cudaStream_t st) {
-    constexpr size_t smem = (size_t)STAGES * (2 * TC_BM * TC_BK * 4 + 2 * BN * TC_BK * 4) + 3 * STAGES * 8 + 1024;
+    constexpr size_t smem = (size_t)STAGES * (TC_BM * TC_BK * 4 + 2 * BN * TC_BK * 4) + 3 * STAGES * 8 + 1024;
     static_assert(smem <= 227 * 1024, "stage ring exceeds the shared memory of a block");
     CTCB_CUDA_CHECK(cudaFuncSetAttribute((gemm_tc_kernel<BN, STAGES, A_MN, B_MN>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     dim3 grid((g.N + BN - 1) / BN, (g.M + TC_BM - 1) / TC_BM, ctas_z);
@@ -520,7 +565,8 @@ static int run_tc_plan(const GemmTcPlan &p, int M, int N, int K, float alpha, co
     CUtensorMap tA[2], tB[2];
     int rc;
     for (int q = 0; q < p.problems; ++q) {
-        if ((rc = make_map(&tA[q], A[q], M, K, lda, TC_BM, p.a_path == TC_PATH_MN)) != CTCB_OK) return rc;
+        const bool a_mn = p.a_path == TC_PATH_MN;
+        if ((rc = make_map(&tA[q], A[q], M, K, lda, a_mn ? 32 : TC_BM, a_mn)) != CTCB_OK) return rc;
         if ((rc = make_map(&tB[q], B[q], N, K, ldb, p.BN, p.b_path == TC_PATH_MN)) != CTCB_OK) return rc;
     }
     if (p.problems == 1) { tA[1] = tA[0]; tB[1] = tB[0]; }
@@ -612,7 +658,7 @@ extern "C" int ctcb_debug_gemm_plan(int transA, int transB, int M, int N, int K,
 }
 
 // Diagnostic: the per-k-block clock stamps of CTA (0,0,0) of the last tensor-core GEMM (CTCB_GEMM_TRACE=1):
-// [64][8] = {TMA issued, tile landed, lo written, consumers saw it, MMAs issued}.  Returns 0 when tracing is off.
+// [64][8] = {TMA issued, tiles landed, B's lo written, consumers saw it, MMAs issued}.  Returns 0 when tracing is off.
 extern "C" int ctcb_debug_gemm_trace(unsigned long long *host_out) {
     if (!ctcb::g_gemm_trace || !host_out) return 0;
     if (cudaMemcpy(host_out, ctcb::g_gemm_trace, 64 * 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost) != cudaSuccess) return 0;
