@@ -69,6 +69,7 @@ int ctcb_ctc_loss_grad_f32(const float *acts, int is_prob, int64_t utt_stride, i
 
 /* ---- best-path decode (replaces ctc_fast.decode_best_path, ctc_fast.pyx:154-187) -----------
  * hyp_out/align_out: int32[B*Tmax] (row u holds hyp_len_out[u] valid entries).
+ * The label of a frame is np.argmax's: the first NaN if there is one, else the first maximum (0 for a row of -inf).
  * drop_swbd_noise!=0 reproduces the reference's removal of labels 1, 2 and 8 (ctc_fast.pyx:176-179). */
 int ctcb_ctc_best_path_f32(const float *acts, int64_t utt_stride, int64_t frame_stride,
                            const int32_t *T_per_utt, int B, int Tmax, int K, int blank,
@@ -79,7 +80,13 @@ int ctcb_ctc_best_path_f32(const float *acts, int64_t utt_stride, int64_t frame_
  * Same buffers as ctcb_ctc_loss_grad_f32, but `seq` already contains the blanks (:24-26): utterance u has
  * seq_off[u+1]-seq_off[u] trellis states (at most 1024), moves s->s and s->s+1 only, one start and one end
  * state, no window; state 0 is propagated with row 0 of the probabilities (:49).  grad_out must not alias
- * acts.  workspace: ctcb_ctc_blankforce_workspace_bytes(B, Tmax, max_states) bytes (the alpha trellis).
+ * acts.  workspace: ctcb_ctc_blankforce_workspace_bytes(B, Tmax, max_states) bytes (the log-alpha trellis).
+ * The recursions run in the log domain, so unlike the reference the result stays right on long utterances whose
+ * normalised trellis products underflow float64.  skip_out[u] = 1 with a zero gradient where the reference skips (a
+ * zero frame normaliser, or alpha*beta != 0 where the state's probability is 0), and, checked on the device before
+ * any state is read, where utterance u has T_per_utt <= 0, no state, more states than max_states, or a label outside
+ * [0, K).  The launch refuses (CTCB_EINVAL) max_states outside 1..1024 and 20*max_states + 256 + 8*K > 200 KiB of
+ * shared memory: K <= 25565 at max_states = 1, K <= 23008 at 1024.
  * The best path of that module (:115-142) is ctcb_ctc_best_path_f32 with drop_swbd_noise=0; its align
  * output is simply not used. */
 size_t ctcb_ctc_blankforce_workspace_bytes(int B, int Tmax, int max_states);

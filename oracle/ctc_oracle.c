@@ -234,16 +234,24 @@ int ctc_oracle_loss_log(const double *params, int K, int T, const int *seq, int 
     return 0;
 }
 
+/* The label np.argmax picks in frame t (ctc_fast.pyx:167, ctc_fast_blankforce.pyx:132): the first NaN if the frame has
+ * one, else the first maximum; a frame of -inf gives 0. */
+static int argmax_frame(const double *probs, int K, int t)
+{
+    const double *row = probs + (size_t)K * t;
+    int b = 0, k;
+    for (k = 1; k < K && !isnan(row[b]); k++)
+        if (isnan(row[k]) || row[k] > row[b]) b = k;
+    return b;
+}
+
 /* ctc_fast.pyx:154-187 -- per-frame argmax, collapse repeats, drop blank and labels 1,2,8.
  * hyp/align must hold T ints; returns the hypothesis length. */
 int ctc_oracle_best_path(const double *probs, int K, int T, int blank, int *hyp, int *align)
 {
-    int n = 0, prev = -1, t, k;
+    int n = 0, prev = -1, t;
     for (t = 0; t < T; t++) {
-        int b = 0;
-        double m = probs[(size_t)K * t];
-        for (k = 1; k < K; k++)
-            if (probs[(size_t)k + (size_t)K * t] > m) { m = probs[(size_t)k + (size_t)K * t]; b = k; }
+        int b = argmax_frame(probs, K, t);
         if (b == blank) { prev = b; continue; }                 /* :172-173 */
         if (b == 1 || b == 2 || b == 8) { prev = b; continue; } /* :176-177 */
         if (t != 0 && b == prev) { if (n > 0) align[n - 1] = t; prev = b; continue; } /* :179-181 */
@@ -331,15 +339,88 @@ int ctc_oracle_loss_blankforce(const double *params, int K, int T, const int *se
     return skip;
 }
 
+/*
+ * The blank-forced loss and gradient in the log domain: float64 log-sum-exp recursions with no per-frame scaling, so
+ * neither a state nor a product of alpha and beta leaves float64's range.  The reference's contract is kept, with "0"
+ * meaning -inf, not underflow:
+ *   alpha(0,0) = 1 with no emission, and the loss starts from log p[seq[0],0] (:43-44);
+ *   state 0 takes row 0 in the alpha pass only (:49); beta(L-1,T-1) = 1 with no emission (:64);
+ *   -nll = log p[seq[0],0] + log of the mass of ALL states at T-1 (the product of the frame normalisers);
+ *   grad[k,t] = p - sum_{s: seq[s]=k} ab(s,t) / (p[k,t] * sum_s ab(s,t)/p[seq[s],t]) where p[k,t] * that sum > 0,
+ *               else p (:100-106);
+ *   skip, gradient all zeros: a normaliser of either pass is 0 (:108-110: all states -inf at some frame), or
+ *               ab(s,t) != 0 where p[seq[s],t] == 0 (:88-92).  An utterance with no frame or no state also skips.
+ * On skip *nll is the forward pass's (+inf when the forward mass is 0); the reference's partial llForward is not kept.
+ */
+int ctc_oracle_loss_blankforce_log(const double *params, int K, int T, const int *seq, int seqLen,
+                                   double *grad, double *nll)
+{
+    int L = seqLen, t, s, k, skip = 0;
+    double *la, *lb, *lp, *w, logZ;
+    memset(grad, 0, (size_t)K * (T > 0 ? T : 0) * sizeof(double));
+    if (T <= 0 || L <= 0) { *nll = 0.0; return 1; }
+    la = (double *)malloc((size_t)L * T * sizeof(double));
+    lb = (double *)malloc((size_t)L * T * sizeof(double));
+    lp = (double *)malloc((size_t)K * T * sizeof(double));
+    w = (double *)malloc((size_t)L * sizeof(double));
+    for (t = 0; t < T; t++)
+        for (k = 0; k < K; k++) lp[(size_t)k + (size_t)K * t] = log(P(k, t));
+#define LP(k, t) lp[(size_t)(k) + (size_t)K * (size_t)(t)]
+#define LA(s, t) la[(size_t)(s) + (size_t)L * (size_t)(t)]
+#define LB(s, t) lb[(size_t)(s) + (size_t)L * (size_t)(t)]
+    for (s = 0; s < L; s++) LA(s, 0) = (s == 0) ? 0.0 : -INFINITY;
+    for (t = 1; t < T; t++)
+        for (s = 0; s < L; s++)
+            LA(s, t) = (s == 0) ? LA(0, t - 1) + LP(0, t) : lse2(LA(s, t - 1), LA(s - 1, t - 1)) + LP(seq[s], t);
+    logZ = -INFINITY;
+    for (s = 0; s < L; s++) logZ = lse2(logZ, LA(s, T - 1));
+    *nll = -(LP(seq[0], 0) + logZ);
+    if (logZ == -INFINITY) { skip = 1; goto done; }  /* the forward mass is 0 from some frame on */
+
+    for (s = 0; s < L; s++) LB(s, T - 1) = (s == L - 1) ? 0.0 : -INFINITY;
+    for (t = T - 2; t >= 0; t--) {
+        double any = -INFINITY;
+        for (s = L - 1; s >= 0; s--) {
+            LB(s, t) = ((s == L - 1) ? LB(s, t + 1) : lse2(LB(s, t + 1), LB(s + 1, t + 1))) + LP(seq[s], t);
+            any = any > LB(s, t) ? any : LB(s, t);
+        }
+        if (any == -INFINITY) { skip = 1; goto done; }
+    }
+
+    for (t = 0; t < T; t++) {
+        double m = -INFINITY, q = 0.0;
+        for (s = 0; s < L; s++) {
+            double e = LA(s, t) + LB(s, t);
+            w[s] = -INFINITY;
+            if (e == -INFINITY) continue;
+            if (P(seq[s], t) == 0.0) { skip = 1; goto done; }
+            w[s] = e - LP(seq[s], t);
+            m = w[s] > m ? w[s] : m;
+        }
+        if (m == -INFINITY) {                            /* absum == 0: the row stays p */
+            for (k = 0; k < K; k++) G(k, t) = P(k, t);
+            continue;
+        }
+        for (s = 0; s < L; s++) q += exp(w[s] - m);
+        for (s = 0; s < L; s++) G(seq[s], t) += exp(w[s] - m) / q;
+        for (k = 0; k < K; k++) G(k, t) = (P(k, t) > 0.0) ? P(k, t) - G(k, t) : P(k, t);
+    }
+done:
+    if (skip) memset(grad, 0, (size_t)K * T * sizeof(double));
+#undef LP
+#undef LA
+#undef LB
+    free(la); free(lb); free(lp); free(w);
+    return skip;
+}
+
 /* ctc_fast_blankforce.pyx:115-142: argmax per frame, drop blanks and repeats (no label filter, no
  * alignment output).  Returns the hypothesis length. */
 int ctc_oracle_best_path_blankforce(const double *probs, int K, int T, int blank, int *hyp)
 {
-    int n = 0, prev = -1, t, k;
+    int n = 0, prev = -1, t;
     for (t = 0; t < T; ++t) {
-        int b = 0;
-        for (k = 1; k < K; ++k)
-            if (probs[(size_t)k + (size_t)K * t] > probs[(size_t)b + (size_t)K * t]) b = k;
+        int b = argmax_frame(probs, K, t);
         if (b != blank && !(t != 0 && b == prev)) hyp[n++] = b;
         prev = b;
     }

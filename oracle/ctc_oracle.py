@@ -49,6 +49,8 @@ def _lib():
         _LIB.ctc_oracle_loss_blankforce.restype = ctypes.c_int
         _LIB.ctc_oracle_loss_blankforce.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                                     ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]
+        _LIB.ctc_oracle_loss_blankforce_log.restype = ctypes.c_int
+        _LIB.ctc_oracle_loss_blankforce_log.argtypes = _LIB.ctc_oracle_loss_blankforce.argtypes
         _LIB.ctc_oracle_best_path_blankforce.restype = ctypes.c_int
         _LIB.ctc_oracle_best_path_blankforce.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                                          ctypes.c_void_p]
@@ -97,8 +99,7 @@ def decode_best_path(probs, blank=0):
     return hyp[:n].tolist(), align[:n].tolist()
 
 
-def ctc_loss_blankforce(params, seq):
-    """ctc_fast_blankforce.pyx:13-113 restated (oracle/ctc_oracle.c): seq already holds the blanks."""
+def _call_bf(fn, params, seq):
     if not (isinstance(params, np.ndarray) and params.dtype == np.float64 and params.ndim == 2
             and params.flags.f_contiguous):
         raise ValueError("ndarray is not Fortran contiguous")
@@ -106,9 +107,19 @@ def ctc_loss_blankforce(params, seq):
     K, T = params.shape
     grad = np.zeros((K, T), dtype=np.float64, order="F")
     nll = ctypes.c_double(0.0)
-    skip = _lib().ctc_oracle_loss_blankforce(params.ctypes.data, K, T, seq.ctypes.data, seq.shape[0],
-                                             grad.ctypes.data, ctypes.addressof(nll))
+    skip = fn(params.ctypes.data, K, T, seq.ctypes.data, seq.shape[0], grad.ctypes.data, ctypes.addressof(nll))
     return nll.value, grad, bool(skip)
+
+
+def ctc_loss_blankforce(params, seq):
+    """ctc_fast_blankforce.pyx:13-113 restated (oracle/ctc_oracle.c): seq already holds the blanks."""
+    return _call_bf(_lib().ctc_oracle_loss_blankforce, params, seq)
+
+
+def ctc_loss_blankforce_log(params, seq):
+    """The blank-forced contract in the log domain (float64 log-sum-exp, no per-frame scaling): correct where the
+    reference's normalised trellises underflow (long, unaligned utterances).  An empty seq or T = 0 is skip."""
+    return _call_bf(_lib().ctc_oracle_loss_blankforce_log, params, seq)
 
 
 def decode_best_path_blankforce(probs, blank=0):

@@ -5,15 +5,22 @@
 // L = len(seq) states, transitions s -> s and s -> s+1 only (:51-52, :73-74), one start state (:43) and one
 // end state (:64), no [start,end) window -- every state enters the frame normaliser (:55-59), so the
 // returned cost is the log of the total mass of all states at the last frame.  State 0 is propagated with
-// the probability of ROW 0 (`params[s,t]`, :49), not of seq[0]; kept as is.
+// the probability of ROW 0 (`params[s,t]`, :49), not of seq[s]; kept as is.
 //
-// One CTA per utterance, float64 state as in the reference.  Per frame one block-wide reduction gives the
-// normaliser c; the un-normalised states are exchanged through shared memory and every reader divides by c
-// itself, so the alpha pass costs one barrier per frame and the beta/gradient pass two.  The normalised
-// alpha trellis (T x L doubles) is spilled to the workspace; the probabilities are written into grad_out
-// first (softmax of the logits, float32 as brnnet.py:170 hands them over) and each row is replaced by its
-// gradient when the beta pass reaches it.  Occupancies are summed as 2^40 fixed point (integer shared
+// One CTA per utterance, float64 state.  Unlike the reference, both passes run in the log domain with no per-frame
+// normalisation: the reference's normalised alpha and beta and their product underflow float64 on long utterances
+// with unaligned outputs (gradient rows left at p from ~3000 frames x 600 states, a loss off by hundreds of nats
+// further out).  Here log alpha and log beta have the range of float64's exponent, and an occupancy is
+// exp(la + lb - log p - frame max) / sum, which cannot underflow where it matters.  "A normaliser is 0" becomes "every
+// state is -inf", so the reference's skips stay exact.  The alpha pass exchanges neighbouring states through shared
+// memory (one barrier per frame); the beta/gradient pass needs a block reduction of (max, sum) pairs and the
+// occupancy atomics (two barriers).  log alpha (T x L doubles) is spilled to the workspace; the probabilities are
+// written into grad_out first (softmax of the logits, float32 as brnnet.py:170 hands them over) and each row is
+// replaced by its gradient when the beta pass reaches it.  Occupancies are summed as 2^40 fixed point (integer shared
 // atomics: order-independent, run-to-run identical).
+//
+// An utterance with no frame, no state, more states than max_states or a label outside [0, K) is skipped with a zero
+// gradient; the check comes before anything reads its states.
 #include <math_constants.h>
 
 #include "common.cuh"
@@ -24,6 +31,7 @@ constexpr int BF_THREADS = 256;
 constexpr int BF_WARPS = BF_THREADS / 32;
 constexpr int BF_SPT = 4;                      // states per thread -> at most 1024 states
 constexpr double BF_FIX = 1099511627776.0;     // 2^40
+constexpr double NEG_INF = -__builtin_huge_val();
 
 struct BfArgs {
     const float *acts;
@@ -36,22 +44,31 @@ struct BfArgs {
     double *ws;
 };
 
-__device__ __forceinline__ double warp_sum_d(double v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
+__device__ __forceinline__ double lse2(double a, double b) {
+    const double m = fmax(a, b);
+    if (m == NEG_INF) return m;
+    return m + log1p(exp(-fabs(a - b)));
 }
 
-// Sum over the CTA; `slot` is a [BF_WARPS] shared array that the caller alternates between consecutive calls,
-// so one barrier per reduction is enough.  Fixed summation order: the result is identical in every thread.
-__device__ __forceinline__ double block_sum(double v, double *slot) {
-    v = warp_sum_d(v);
-    if ((threadIdx.x & 31) == 0) slot[threadIdx.x >> 5] = v;
-    __syncthreads();
-    double s = 0.0;
+// (m, s) stands for s * e^m.  Symmetric in its two operands bit for bit, so both lanes of a shuffle get the same pair.
+__device__ __forceinline__ void ms_add(double &m, double &s, double om, double os) {
+    const double n = fmax(m, om);
+    if (n == NEG_INF) return;
+    s = s * exp(m - n) + os * exp(om - n);
+    m = n;
+}
+
+__device__ __forceinline__ void warp_ms(double &m, double &s) {
 #pragma unroll
-    for (int w = 0; w < BF_WARPS; ++w) s += slot[w];
-    return s;
+    for (int o = 16; o > 0; o >>= 1) ms_add(m, s, __shfl_xor_sync(0xffffffffu, m, o), __shfl_xor_sync(0xffffffffu, s, o));
+}
+
+// Combine the warps' pairs of `slot` ([2][BF_WARPS]) in a fixed order: the result is identical in every thread.
+__device__ __forceinline__ void block_ms(const double *slot, double &m, double &s) {
+    m = NEG_INF;
+    s = 0.0;
+#pragma unroll
+    for (int w = 0; w < BF_WARPS; ++w) ms_add(m, s, slot[w], slot[BF_WARPS + w]);
 }
 
 __global__ void __launch_bounds__(BF_THREADS) ctc_blankforce_kernel(BfArgs a) {
@@ -62,19 +79,29 @@ __global__ void __launch_bounds__(BF_THREADS) ctc_blankforce_kernel(BfArgs a) {
     const int so = a.soff[u];
     const int L = a.soff[u + 1] - so;
     const int Lp = a.Lmax;
-    double *xbuf = sm_d;                                  // [2][Lp] un-normalised states of two frames
-    double *red = xbuf + 2 * Lp;                          // [2][2][BF_WARPS]
+    double *xbuf = sm_d;                                  // [2][Lp] log states of two frames
+    double *red = xbuf + 2 * Lp;                          // [2][2][BF_WARPS] (max, sum) pairs
     unsigned long long *occ = (unsigned long long *)(red + 4 * BF_WARPS);   // [K]
     int *lab = (int *)(occ + K);                          // [Lp]
     const float *acts = a.acts + (int64_t)u * a.us;
     float *g = a.grad + (int64_t)u * a.us;
     double *trellis = a.ws + (int64_t)u * a.Tmax * Lp;
 
-    // ---- probabilities into grad_out (rows >= T: zero gradient)
+    // ---- what the reference could not evaluate, or would read out of bounds for: skip with a zero gradient
+    bool bad = T <= 0 || L <= 0 || L > Lp;
+    if (!bad)
+        for (int s = tid; s < L; s += BF_THREADS) {
+            const int l = a.seq[so + s];
+            if (l < 0 || l >= K) bad = true;
+            else lab[s] = l;
+        }
+    bad = __syncthreads_or(bad);
+
+    // ---- probabilities into grad_out (rows >= T, and every row of a skipped utterance: zero gradient)
     for (int t = warp; t < a.Tmax; t += BF_WARPS) {
         const float *xr = acts + (int64_t)t * a.fs;
         float *pr = g + (int64_t)t * a.fs;
-        if (t >= T) {
+        if (t >= T || bad) {
             for (int k = lane; k < K; k += 32) pr[k] = 0.f;
         } else if (a.is_prob) {
             for (int k = lane; k < K; k += 32) pr[k] = xr[k];
@@ -89,12 +116,11 @@ __global__ void __launch_bounds__(BF_THREADS) ctc_blankforce_kernel(BfArgs a) {
             for (int k = lane; k < K; k += 32) pr[k] = expf(xr[k] - m) * inv;
         }
     }
-    for (int s = tid; s < L; s += BF_THREADS) lab[s] = a.seq[so + s];
-    for (int k = tid; k < K; k += BF_THREADS) occ[k] = 0ull;
-    if (T <= 0 || L <= 0 || L > BF_SPT * BF_THREADS) {     // nothing the reference could evaluate
+    if (bad) {
         if (tid == 0) { a.nll[u] = 0.f; a.skip[u] = 1; }
         return;
     }
+    for (int k = tid; k < K; k += BF_THREADS) occ[k] = 0ull;
     __syncthreads();
 
     int myl[BF_SPT];
@@ -106,14 +132,13 @@ __global__ void __launch_bounds__(BF_THREADS) ctc_blankforce_kernel(BfArgs a) {
     // row of the probability each state multiplies with in the ALPHA pass: state 0 uses row 0 (:49)
     auto alpha_row = [&](int j) { return (tid + j * BF_THREADS == 0) ? 0 : myl[j]; };
 
-    bool fail = false;
-    // ------------------------------------------------------------------ alpha (:43-59)
-    double llF = log((double)g[lab[0]]);                   // :44, frame 0
-    double c_prev = 1.0;
+    // ------------------------------------------------------------------ log alpha (:43-59)
+    double la[BF_SPT];
 #pragma unroll
     for (int j = 0; j < BF_SPT; ++j) {
         const int s = tid + j * BF_THREADS;
-        if (s < L) xbuf[s] = (s == 0) ? 1.0 : 0.0;          // :43
+        la[j] = (s == 0) ? 0.0 : NEG_INF;                  // alpha(0,0) = 1, no emission (:43)
+        if (s < L) xbuf[s] = la[j];
     }
     __syncthreads();
     float pn[BF_SPT];
@@ -128,41 +153,53 @@ __global__ void __launch_bounds__(BF_THREADS) ctc_blankforce_kernel(BfArgs a) {
             pc[j] = pn[j];
             pn[j] = (t + 1 < T && tid + j * BF_THREADS < L) ? g[(int64_t)(t + 1) * a.fs + alpha_row(j)] : 0.f;
         }
-        double part = 0.0;
 #pragma unroll
         for (int j = 0; j < BF_SPT; ++j) {
             const int s = tid + j * BF_THREADS;
             if (s < L) {
-                const double ap = xp[s] / c_prev;                         // normalised alpha[s, t-1] (:57-58)
-                trellis[(int64_t)(t - 1) * Lp + s] = ap;
-                const double am = (s > 0) ? xp[s - 1] / c_prev : 0.0;
-                const double v = (s == 0) ? ap * (double)pc[j] : (ap + am) * (double)pc[j];   // :48-52
-                xc[s] = v;
-                part += v;
+                trellis[(int64_t)(t - 1) * Lp + s] = la[j];
+                const double v = (s == 0) ? la[j] : lse2(la[j], xp[s - 1]);            // :48-52
+                la[j] = v + log((double)pc[j]);
+                xc[s] = la[j];
             }
         }
-        const double c = block_sum(part, red + (t & 1) * BF_WARPS);
-        if (c == 0.0) { fail = true; break; }               // ZeroDivisionError in the reference (:108)
-        llF += log(c);
-        c_prev = c;
+        __syncthreads();
     }
-    if (!fail) {
-        const double *xp = xbuf + ((T - 1) & 1) * Lp;
-        for (int s = tid; s < L; s += BF_THREADS) trellis[(int64_t)(T - 1) * Lp + s] = xp[s] / c_prev;
+    // -llForward = -(log p[seq[0],0] + log of the mass of all states at T-1) (:44, :55-59)
+    double *red2 = red + 2 * BF_WARPS;
+    double llF, logZ;
+    {
+        double m = NEG_INF, sm = 0.0;
+#pragma unroll
+        for (int j = 0; j < BF_SPT; ++j) {
+            const int s = tid + j * BF_THREADS;
+            if (s < L) {
+                trellis[(int64_t)(T - 1) * Lp + s] = la[j];
+                ms_add(m, sm, la[j], 1.0);
+            }
+        }
+        warp_ms(m, sm);
+        if (lane == 0) { red2[warp] = m; red2[BF_WARPS + warp] = sm; }
+        __syncthreads();
+        block_ms(red2, m, sm);
+        logZ = (m == NEG_INF) ? NEG_INF : m + log(sm);
+        llF = log((double)g[lab[0]]) + logZ;
     }
-    __syncthreads();
+    // the mass of the last frame is 0 exactly when a frame normaliser of the reference is (:108)
+    bool fail = logZ == NEG_INF;
+    bool zero_p = false;
 
-    // ------------------------------------------------------------------ beta + gradient (:62-106)
+    // ------------------------------------------------------------------ log beta + gradient (:62-106)
     if (!fail) {
-        double *red2 = red + 2 * BF_WARPS;
-        c_prev = 1.0;
+        double lb[BF_SPT];
         float bn[BF_SPT];
         double an[BF_SPT];
 #pragma unroll
         for (int j = 0; j < BF_SPT; ++j) {
             const int s = tid + j * BF_THREADS;
+            lb[j] = NEG_INF;
             bn[j] = (s < L) ? g[(int64_t)(T - 1) * a.fs + myl[j]] : 0.f;
-            an[j] = (s < L) ? trellis[(int64_t)(T - 1) * Lp + s] : 0.0;
+            an[j] = (s < L) ? trellis[(int64_t)(T - 1) * Lp + s] : NEG_INF;
         }
         for (int t = T - 1; t >= 0; --t) {
             const int step = T - 1 - t;
@@ -176,61 +213,58 @@ __global__ void __launch_bounds__(BF_THREADS) ctc_blankforce_kernel(BfArgs a) {
                 pc[j] = bn[j];
                 al[j] = an[j];
                 bn[j] = (t > 0 && s < L) ? g[(int64_t)(t - 1) * a.fs + myl[j]] : 0.f;
-                an[j] = (t > 0 && s < L) ? trellis[(int64_t)(t - 1) * Lp + s] : 0.0;
+                an[j] = (t > 0 && s < L) ? trellis[(int64_t)(t - 1) * Lp + s] : NEG_INF;
             }
-            double w[BF_SPT];
-            double part_c = 0.0, part_q = 0.0;
+            double e[BF_SPT];
+            double m = NEG_INF, sm = 0.0;
+            bool alive = false;
 #pragma unroll
             for (int j = 0; j < BF_SPT; ++j) {
                 const int s = tid + j * BF_THREADS;
-                w[j] = 0.0;
+                e[j] = NEG_INF;
                 if (s < L) {
+                    const double lpk = log((double)pc[j]);
                     double v;
-                    if (t == T - 1) {
-                        v = (s == L - 1) ? 1.0 : 0.0;                                   // :64
-                    } else {
-                        const double bp = xp[s] / c_prev;
-                        const double bq = (s < L - 1) ? xp[s + 1] / c_prev : 0.0;
-                        v = (s == L - 1) ? bp * (double)pc[j] : (bp + bq) * (double)pc[j];   // :71-74
-                    }
+                    if (t == T - 1) v = (s == L - 1) ? 0.0 : NEG_INF;                           // :64
+                    else v = ((s == L - 1) ? lb[j] : lse2(lb[j], xp[s + 1])) + lpk;              // :71-74
+                    lb[j] = v;
                     xc[s] = v;
-                    part_c += v;
-                    // alpha*beta/p of :85-92, still carrying the factor c of this frame
-                    const double ab = al[j] * v;
-                    if (ab != 0.0 && pc[j] != 0.f) w[j] = ab / (double)pc[j];
-                    part_q += w[j];
+                    alive |= v != NEG_INF;
+                    // alpha*beta/p of :85-92; alpha*beta != 0 where p == 0 is the reference's skip (:88-92)
+                    const double ab = al[j] + v;
+                    if (ab != NEG_INF) {
+                        if (pc[j] == 0.f) {
+                            zero_p = true;
+                        } else {
+                            e[j] = ab - lpk;
+                            ms_add(m, sm, e[j], 1.0);
+                        }
+                    }
                 }
             }
-            // both sums with one barrier
-            part_c = warp_sum_d(part_c);
-            part_q = warp_sum_d(part_q);
+            warp_ms(m, sm);
             double *slot = ((step & 1) ? red2 : red);
-            if (lane == 0) { slot[warp] = part_c; slot[BF_WARPS + warp] = part_q; }
-            __syncthreads();
-            double c = 0.0, q = 0.0;
-#pragma unroll
-            for (int x = 0; x < BF_WARPS; ++x) { c += slot[x]; q += slot[BF_WARPS + x]; }
-            if (c == 0.0) { fail = true; break; }
-            c_prev = c;
-            if (q > 0.0) {
+            if (lane == 0) { slot[warp] = m; slot[BF_WARPS + warp] = sm; }
+            if (!__syncthreads_or(alive)) { fail = true; break; }                  // beta normaliser 0 (:108)
+            block_ms(slot, m, sm);
+            const bool any = m != NEG_INF;                                         // absum > 0 (:94-97)
+            if (any) {
 #pragma unroll
                 for (int j = 0; j < BF_SPT; ++j)
-                    if (w[j] != 0.0)
-                        atomicAdd(&occ[myl[j]], (unsigned long long)(w[j] / q * BF_FIX + 0.5));
+                    if (e[j] != NEG_INF)
+                        atomicAdd(&occ[myl[j]], (unsigned long long)(exp(e[j] - m) / sm * BF_FIX + 0.5));
             }
             __syncthreads();
-            const double absum = q / c;                                                   // :94-97
             float *pr = g + (int64_t)t * a.fs;
             for (int k = tid; k < K; k += BF_THREADS) {
                 const double p = (double)pr[k];
-                const double tmp = p * absum;                                             // :102
                 const double gam = (double)occ[k] * (1.0 / BF_FIX);
                 occ[k] = 0ull;
-                pr[k] = (float)((tmp > 0.0) ? p - gam : p);                               // :103-106
+                pr[k] = (float)((any && p > 0.0) ? p - gam : p);                   // tmp > 0 rule (:102-106)
             }
         }
     }
-    __syncthreads();
+    fail = __syncthreads_or(fail || zero_p);
     if (fail) {                                            // skipped utterances carry no gradient
         for (int t = warp; t < T; t += BF_WARPS)
             for (int k = lane; k < K; k += 32) g[(int64_t)t * a.fs + k] = 0.f;

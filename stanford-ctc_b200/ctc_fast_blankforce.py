@@ -16,7 +16,9 @@ from ctc_fast import _check_params
 
 def ctc_loss_batch(acts, T_per_utt, seq, seq_off, max_states, is_prob=False, utt_stride=None, frame_stride=None,
                    grad=None, workspace=None):
-    """Batched form on device tensors (layout and return values as ctc_fast.ctc_loss_batch)."""
+    """Batched form on device tensors (layout and return values as ctc_fast.ctc_loss_batch).  Utterance u's states are
+    seq[seq_off[u]:seq_off[u+1]].  The device checks each utterance before it reads its states: no frame, no state, more
+    than max_states states, or a label outside [0, K) gives skip = 1 with a zero gradient."""
     torch = _ctcb.require_cuda()
     assert acts.is_cuda and acts.dtype == torch.float32 and acts.is_contiguous()
     B = T_per_utt.numel()

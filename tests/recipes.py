@@ -148,6 +148,16 @@ def bf_case(name):
 ALL_BF = list(BF_CASES)
 
 
+def bf_utt(T, K, nlab, scale, seed):
+    """One blank-forced utterance: float32 logits (T x K) ~ N(0, scale^2) and 0 l1 0 l2 ... 0 with nlab labels drawn
+    uniformly from 1..K-1 (2 nlab + 1 states)."""
+    rng = np.random.RandomState(seed)
+    x = (rng.randn(T, K) * scale).astype(np.float32)
+    seq = np.zeros(2 * nlab + 1, dtype=np.int32)
+    seq[1::2] = 1 + rng.randint(K - 1, size=nlab)
+    return x, seq
+
+
 RNN_VARIANTS = (("uni", dict(temporalLayer=2, unidirectional=True)), ("dnn", dict(temporalLayer=-1)))
 
 
