@@ -214,7 +214,8 @@ size_t ctcb_brnn_forward_workspace_bytes(const ctcb_brnn_config *cfg, size_t *er
  * what = 0: output of affine map `layer` (1..numLayers+1; For+Back at the temporal layer, logits at the last),
  * what = 1 / 2: For / Back of the temporal layer (brnnet.py:143-153).  With numTemporal > 1, `layer` names which
  * temporal layer (temporalLayer .. temporalLayer+k-1; Back exists only when bi-directional); with one temporal
- * layer it is ignored. */
+ * layer it is ignored.  With dropout on (ctcb_brnn_set_dropout), the ReLU hidden layers' entries hold the dropped and
+ * rescaled activations. */
 int ctcb_brnn_activation_offset(const ctcb_brnn_config *cfg, int what, int layer, size_t *offset, int32_t *width);
 
 int ctcb_brnn_create(const ctcb_brnn_config *cfg, ctcb_brnn **out);
@@ -263,6 +264,30 @@ int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, const int32_t
  * calls ctcb_brnn_apply_l2_f32 on the reduced gradient. */
 int ctcb_brnn_set_deferred_l2(ctcb_brnn *h, int deferred);
 int ctcb_brnn_apply_l2_f32(ctcb_brnn *h, const float *params, float *grads, void *stream);
+
+/* ---- inverted dropout on the ReLU hidden layers (not in the reference) ----------------------------------------
+ * When p > 0, every TRAINING call (grads != NULL) masks the output X_i of each hidden layer i (1..numLayers) that is
+ * not temporal, in place, right after its forward contraction: the input, the temporal layers' outputs and the logits
+ * are never dropped, and forward-only calls (grads == NULL) never drop.  The mask is a pure function of
+ * (seed, step, i, g, t, j) -- g the utterance's index in the step's whole minibatch, t the frame, j the unit:
+ *     r = Philox4x32-10(counter = (step mod 2^32, g mod 2^32, t, (i << 24) | (j / 4)),
+ *                       key = (seed mod 2^32, seed >> 32))[j % 4]       (curand_Philox4x32_10, one call per 4 units)
+ *     keep iff r >= thr,  thr = floor(p * 2^32)  (float64);  kept: x * s,  s = float32(1 / (1 - p))  (float64, rounded
+ *     once);  dropped: 0.
+ * step is the int64 at `step` (DEVICE memory), read by every training call when it runs, so a captured CUDA graph
+ * draws the mask of the counter's current value; the handle owns no memory, the caller owns the counter.  The delta
+ * contraction of layer i runs with alpha = s and the ReLU mask X_i > 0 (which removes the dropped units), so the
+ * gradient is that of the dropped net.  The activation hook (ctcb_brnn_activation_offset) returns the dropped X_i.
+ * p == 0 (the default) disables it: a training call then issues exactly the launches and bits it does without.
+ * CTCB_EINVAL for p < 0, p >= 1, NaN, or p > 0 with a null step.  Host-only: no device work. */
+int ctcb_brnn_set_dropout(ctcb_brnn *h, float p, uint64_t seed, const int64_t *step);
+/* Utterance u of the following calls is minibatch utterance g = first + stride * u: rank + world * (u0 + u) for rank
+ * `rank` of `world` (round-robin shards) and a micro-batch starting at position u0 of the rank's shard, so one call, a
+ * micro-batched step and a data-parallel step draw the same mask for the same utterance.  Default (0, 1).  CTCB_EINVAL
+ * for first < 0 or stride < 1.  Host-only. */
+int ctcb_brnn_set_dropout_utts(ctcb_brnn *h, int64_t first, int64_t stride);
+/* *step += 1 on `stream` (one thread); inside a capture it becomes part of the graph like any other launch. */
+int ctcb_dropout_advance(int64_t *step, void *stream);
 
 /* ---- the time recurrences of the temporal layer on their own (replaces the per-frame loops
  *      brnnet.py:144-152 [mode 0] and brnnet.py:208-224 [mode 1]) -------------------------------

@@ -79,6 +79,9 @@ _PROTOS = {
     "ctcb_debug_sweep_plan": (c_int, [c_int, c_int, c_int, ctypes.POINTER(ctypes.c_int32)]),
     "ctcb_brnn_set_deferred_l2": (c_int, [c_vp, c_int]),
     "ctcb_brnn_apply_l2_f32": (c_int, [c_vp, c_vp, c_vp, c_vp]),
+    "ctcb_brnn_set_dropout": (c_int, [c_vp, c_f32, ctypes.c_uint64, c_vp]),
+    "ctcb_brnn_set_dropout_utts": (c_int, [c_vp, c_i64, c_i64]),
+    "ctcb_dropout_advance": (c_int, [c_vp, c_vp]),
     "ctcb_comm_get_unique_id": (c_int, [c_vp]),
     "ctcb_comm_create": (c_int, [c_vp, c_int, c_int, ctypes.POINTER(c_vp)]),
     "ctcb_comm_destroy": (None, [c_vp]),

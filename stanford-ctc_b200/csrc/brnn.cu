@@ -17,6 +17,7 @@
 // Gradients of the utterances of the batch are summed (the reference never normalises, cf.
 // ctc/nnet.py:193-195); a skipped utterance contributes nothing.
 #include "common.cuh"
+#include <cmath>
 #include <new>
 
 namespace ctcb {
@@ -28,6 +29,8 @@ int run_add2(const float *x, const float *y, float *z, int64_t n, cudaStream_t s
 int run_sumsq(const float *g, int64_t n, float *out, float scale, int accumulate, void *scratch, cudaStream_t st);
 int comm_allreduce_ranges(ctcb_comm *c, float *const *ptrs, const int64_t *counts, int k, cudaStream_t st);
 int comm_world(const ctcb_comm *c);
+int run_dropout(float *X, int64_t R, int B, int H, int layer, uint64_t seed, const int64_t *step, int64_t first,
+                int64_t stride, uint32_t thr, float scale, cudaStream_t st);
 
 // ---- small kernels ---------------------------------------------------------------------------
 // column sums of a row-major R x N matrix: stage 1 partials over row blocks, stage 2 final
@@ -160,6 +163,13 @@ struct ctcb_brnn {
     // the forward layout, computed on the first forward-only call (its GEMM area takes a few hundred size queries)
     bool fwd_ready;
     FwdLayout fwd;
+    // inverted dropout of the ReLU hidden layers in training calls (ctcb_brnn_set_dropout); drop_p == 0: off
+    float drop_p;
+    uint64_t drop_seed;
+    const int64_t *drop_step;       // the caller's device counter
+    uint32_t drop_thr;              // keep iff Philox output >= drop_thr
+    float drop_scale;               // 1 / (1 - p), rounded once; also the delta contraction's alpha
+    int64_t drop_first, drop_stride;
 };
 
 static int valid_cfg(const ctcb_brnn_config *c) {
@@ -393,6 +403,13 @@ extern "C" int ctcb_brnn_create(const ctcb_brnn_config *cfg, ctcb_brnn **out) {
     h->defer_l2 = false;
     h->comm = nullptr;
     h->fwd_ready = false;
+    h->drop_p = 0.f;
+    h->drop_seed = 0;
+    h->drop_step = nullptr;
+    h->drop_thr = 0;
+    h->drop_scale = 1.f;
+    h->drop_first = 0;
+    h->drop_stride = 1;
     *out = h;
     return CTCB_OK;
 }
@@ -474,9 +491,11 @@ struct FwdBufs {
 };
 
 // brnnet.py:136-173: the affine maps with bias(+ReLU) fused, the two-direction sweep and For+Back at each temporal
-// layer, the softmax into probs_out when given.  Clears the sweep error flag first.
+// layer, the softmax into probs_out when given.  Clears the sweep error flag first.  drop: a training call with dropout
+// on masks the output of every ReLU hidden layer in place right behind its contraction, so the next layer, the weight
+// gradients and the ReLU mask of the delta contraction all read the dropped activations.
 static int brnn_forward(ctcb_brnn *h, const float *feats, const int32_t *T_per_utt, int B, int Tmax,
-                        const float *params, float *probs_out, const FwdBufs &m, cudaStream_t st) {
+                        const float *params, float *probs_out, const FwdBufs &m, bool drop, cudaStream_t st) {
     const ctcb_brnn_config &c = h->cfg;
     const int N = c.numLayers, H = c.layerSize, K = c.outputDim, tl = h->tl, nt = h->nt;
     const int *sz = h->sizes;
@@ -497,6 +516,11 @@ static int brnn_forward(ctcb_brnn *h, const float *feats, const int32_t *T_per_u
         ProfScope ps("gemm_fwd", st);
         TRY(ctcb_gemm_f32(0, 1, (int)R, sz[i], sz[i - 1], 1.f, in, sz[i - 1], P(2 * (i - 1)), sz[i - 1], 0.f,
                           m.X[i], sz[i], P(2 * (i - 1) + 1), relu, nullptr, m.gemm, m.gemm_bytes, st));
+        }
+        if (drop && relu) {
+            ProfScope ps("dropout", st);
+            TRY(run_dropout(m.X[i], R, B, sz[i], i, h->drop_seed, h->drop_step, h->drop_first, h->drop_stride,
+                            h->drop_thr, h->drop_scale, st));
         }
         if (temporal(i)) {
             const int j = i - tl, iWtf = rec_index(&c, j);
@@ -568,7 +592,7 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
         m.counters = (unsigned int *)(ws + f.counters);
         m.sweep = ws + f.sweep;
         m.sweep_bytes = f.sweep_bytes;
-        return brnn_forward(h, feats, T_per_utt, B, Tmax, params, probs_out, m, st);
+        return brnn_forward(h, feats, T_per_utt, B, Tmax, params, probs_out, m, false, st);
     }
     const WsLayout w = ws_layout(&c);
     if (!workspace || ws_bytes < w.total)
@@ -609,7 +633,8 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
     m.counters = counters;
     m.sweep = ws + w.sweep;
     m.sweep_bytes = w.sweep_bytes;
-    TRY(brnn_forward(h, feats, T_per_utt, B, Tmax, params, probs_out, m, st));
+    const bool drop = h->drop_p > 0.f;
+    TRY(brnn_forward(h, feats, T_per_utt, B, Tmax, params, probs_out, m, drop, st));
     float *logits = Xbuf(N + 1);
 
     // ---------------------------------------------------------------- CTC (brnnet.py:161-175)
@@ -681,11 +706,14 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
         }
         if (i > 0) {
             float *doth = dbuf(i);
-            // delta <- delta . W, with the ReLU mask sign(hActs[i]) fused (brnnet.py:203-204,235-237)
+            // delta <- delta . W, with the ReLU mask sign(hActs[i]) fused (brnnet.py:203-204,235-237).  A dropped
+            // layer's X_i is 0 at every dropped unit, so the same mask removes those; the kept ones were scaled by
+            // drop_scale in the forward pass, and so is their delta, through alpha.
             const float *mask = temporal(i) ? nullptr : Xi;
+            const float alpha = (drop && !temporal(i)) ? h->drop_scale : 1.f;
             {
             ProfScope ps("gemm_delta", st);
-            TRY(ctcb_gemm_f32(0, 0, (int)R, n_in, n_out, 1.f, dcur, n_out, P(2 * i), n_in, 0.f, doth, n_in,
+            TRY(ctcb_gemm_f32(0, 0, (int)R, n_in, n_out, alpha, dcur, n_out, P(2 * i), n_in, 0.f, doth, n_in,
                               nullptr, 0, mask, gws, gws_bytes, st));
             }
             if (temporal(i)) {   // brnnet.py:207-233
@@ -816,6 +844,29 @@ extern "C" int ctcb_brnn_exchange_only(ctcb_brnn *h, const float *params, float 
     }
     TRY(brnn_reduce_rest(h, grads, stats_out, early, st));
     if (c.reg > 0.f && !h->defer_l2) return ctcb_brnn_apply_l2_f32(h, params, grads, stream);
+    return CTCB_OK;
+}
+
+extern "C" int ctcb_brnn_set_dropout(ctcb_brnn *h, float p, uint64_t seed, const int64_t *step) {
+    if (!h) return set_error(CTCB_EINVAL, "ctcb_brnn_set_dropout: null handle");
+    if (!(p >= 0.f && p < 1.f)) return set_error(CTCB_EINVAL, "ctcb_brnn_set_dropout: p = %g is not in [0, 1)", (double)p);
+    if (p > 0.f && !step) return set_error(CTCB_EINVAL, "ctcb_brnn_set_dropout: p = %g needs a step counter", (double)p);
+    const double pd = (double)p;
+    h->drop_p = p;
+    h->drop_seed = seed;
+    h->drop_step = step;
+    h->drop_thr = (uint32_t)std::floor(pd * 4294967296.0);     // < 2^32: p <= 1 - 2^-24
+    h->drop_scale = (float)(1.0 / (1.0 - pd));
+    return CTCB_OK;
+}
+
+extern "C" int ctcb_brnn_set_dropout_utts(ctcb_brnn *h, int64_t first, int64_t stride) {
+    if (!h) return set_error(CTCB_EINVAL, "ctcb_brnn_set_dropout_utts: null handle");
+    if (first < 0 || stride < 1)
+        return set_error(CTCB_EINVAL, "ctcb_brnn_set_dropout_utts: first = %lld, stride = %lld (need first >= 0, "
+                         "stride >= 1)", (long long)first, (long long)stride);
+    h->drop_first = first;
+    h->drop_stride = stride;
     return CTCB_OK;
 }
 

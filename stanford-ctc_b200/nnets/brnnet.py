@@ -15,6 +15,9 @@ single contiguous vector.  New, additive surface for the minibatch/data-parallel
 
     NNet(..., maxUtts=B, maxLabels=L)        capacity for B utterances per call (micro-batch)
     NNet(..., numTemporal=k)                 k stacked temporal layers temporalLayer .. temporalLayer+k-1
+    NNet(..., dropout=p, dropoutSeed=33)     inverted dropout on the ReLU hidden layers of training calls; the mask
+                                                of an utterance is drawn from (seed, the device counter dropoutStep,
+                                                layer, its index in the step's minibatch, frame, unit)
     costAndGradBatch(datas, labelss)         -> (costs[B], grad, skips[B])   host arrays in; more than maxUtts
                                                 utterances are accumulated over micro-batches
     costAndGradDevice(batch, first, last)    -> no host sync; see DeviceBatch
@@ -121,7 +124,8 @@ class NNet:
 
     def __init__(self, inputDim, outputDim, layerSize, numLayers, maxBatch,
                  train=True, temporalLayer=-1, reg=0.0, maxUtts=1, maxLabels=None,
-                 allowTopTemporal=False, device=None, unidirectional=False, numTemporal=1):
+                 allowTopTemporal=False, device=None, unidirectional=False, numTemporal=1, dropout=0.0,
+                 dropoutSeed=33):
         torch = _ctcb.require_cuda()
         self._torch = torch
         self.dev = torch.device("cuda", torch.cuda.current_device() if device is None else device)
@@ -170,6 +174,20 @@ class NNet:
         check(lib.ctcb_brnn_create(ctypes.byref(self._cfg), ctypes.byref(self._h)))
         self.stack = None
         self.grad = None
+        # Inverted dropout (include/ctcb200.h: ctcb_brnn_set_dropout).  The step counter lives on the device, so a CUDA
+        # graph of an SGD step reads its current value at every replay; sgd.SGD advances it once per step.
+        # dropoutShard = (rank, world) places this process's utterances in the step's minibatch (None: from
+        # torch.distributed).
+        self.dropout = float(dropout)
+        self.dropoutSeed = int(dropoutSeed)
+        self.dropoutStep = None
+        self.dropoutShard = None
+        if self.dropout != 0.0:
+            if not 0.0 < self.dropout < 1.0:
+                raise ValueError("dropout=%r must be in [0, 1)" % (dropout,))
+            self.dropoutStep = torch.zeros(1, dtype=torch.int64, device=self.dev)
+            check(lib.ctcb_brnn_set_dropout(self._h, self.dropout, self.dropoutSeed & 0xFFFFFFFFFFFFFFFF,
+                                            ptr(self.dropoutStep)))
 
     def __del__(self):
         h = getattr(self, "_h", None)
@@ -266,16 +284,20 @@ class NNet:
         assert batchSize <= self.maxBatch, "Batch size exceeds max batch"
 
     # ------------------------------------------------------------------ compute
-    def costAndGradDevice(self, batch, want_probs=False, first=True, last=True, out=None):
+    def costAndGradDevice(self, batch, want_probs=False, first=True, last=True, out=None, u0=0):
         """Enqueue forward/CTC/backward for a staged DeviceBatch on the current stream.  Returns device
         tensors (cost[B], skip[B]) -- or probs [Tmax][B][K] when train=False -- without synchronising.
 
         Gradient accumulation over the micro-batches of one step (ctcb_brnn_cost_and_grad_part): first=False adds
         the gradient and the statistics tail into what the earlier calls left; only the last=True call exchanges
         over the ranks and adds the L2 term.  `out` optionally names the (cost[B], skip[B]) device tensors to write
-        (default: the net's own per-utterance buffers)."""
+        (default: the net's own per-utterance buffers).  u0: position of the batch's first utterance in this rank's
+        shard of the step, which with the rank places each utterance in the minibatch for its dropout mask."""
         if not self.train:
             return self._forward_device(batch)
+        if self.dropout > 0.0:
+            rank, world = self.dropoutShard or parallel.world_info()[1:]
+            check(lib.ctcb_brnn_set_dropout_utts(self._h, rank + world * u0, world))
         B, Tmax = batch.B, batch.Tmax
         probs = self._probs_view(B, Tmax) if want_probs else None
         cost, skip = out if out is not None else (self._cost[:B], self._skip[:B])
@@ -346,7 +368,7 @@ class NNet:
                                              None if labelss is None else [labelss[i] for i in idx]).upload()
             n = len(idx)
             self.costAndGradDevice(batch, first=(k == 0), last=(k == len(pieces) - 1),
-                                   out=(cost_all[u0:u0 + n], skip_all[u0:u0 + n]))
+                                   out=(cost_all[u0:u0 + n], skip_all[u0:u0 + n]), u0=u0)
             u0 += n
         host = self._out_all_host[:2 * B]
         host.copy_(self._out_all[:2 * B], non_blocking=True)
@@ -446,7 +468,8 @@ class NNet:
 
     def check_grad(self, data, labels, epsilon=1e-3, maxChecks=10, verbose=True):
         """Finite-difference check on a small section of every weight matrix (brnnet.py:279-297).
-        Returns the list of (analytic, numeric) pairs it printed."""
+        Returns the list of (analytic, numeric) pairs it printed.  costAndGrad never advances the dropout counter,
+        so every evaluation sees the same mask."""
         cost, grad, _ = self.costAndGrad(data, labels)
         out = []
         ana = [dw.clone() for dw, _ in grad]

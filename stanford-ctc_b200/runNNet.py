@@ -7,7 +7,7 @@ last_cost, sentinel, train.log), resume through --cfg_file with the step size re
 (runNNet.py:143-166), the fixed seeds 33 (:113-115) and CUDA_DEVICE device selection (:117-120).
 The implementation is organised differently: a declarative flag table, one RunDir helper that owns the
 side files, and separate train/evaluate phases.  Site paths of run_cfg.py / decoder_config.py became
-flags (--runDir, --outDir); new flags: --numTemporal, --batchSize, --maxUtts, --maxLabels, --quiet.  Under torchrun the same
+flags (--runDir, --outDir); new flags: --numTemporal, --batchSize, --maxUtts, --maxLabels, --dropout, --quiet.  Under torchrun the same
 script trains data-parallel (one process per GPU, one NCCL all-reduce per step).
 """
 import argparse
@@ -50,6 +50,8 @@ FLAGS = [
                         "micro-batches (0 = the whole shard, batchSize / number of GPUs rounded up); with --test, "
                         "utterances per forward call per GPU (0 = one, the reference's loop)"),
     ("maxLabels", int, 511, "longest label sequence the buffers are sized for"),
+    ("dropout", float, 0.0, "inverted dropout probability on the ReLU hidden layers while training (0 = off; "
+                            "--test never drops)"),
     ("runDir", str, "./runs", "parent of the time-stamped run directory"),
     ("outDir", str, None, "--test: directory for the likelihood arks"),
     ("quiet", None, False, "no console logging / per-iteration prints"),
@@ -189,7 +191,7 @@ def _train(opts, cfg, run_dir, log, rank, world):
     net = rnnet.NNet(opts.inputDim, opts.outputDim, opts.layerSize, opts.numLayers, opts.maxUttLen,
                      temporalLayer=opts.temporalLayer, reg=opts.reg, numTemporal=opts.numTemporal,
                      maxUtts=utterance_capacity(opts, world),
-                     maxLabels=min(opts.maxLabels, opts.maxUttLen))
+                     maxLabels=min(opts.maxLabels, opts.maxUttLen), dropout=opts.dropout)
     net.initParams()
     optimizer = sgd.SGD(net, opts.maxUttLen, alpha=opts.step, momentum=opts.momentum, batchSize=opts.batchSize,
                         verbose=(rank == 0 and not opts.quiet))

@@ -13,6 +13,8 @@ all-reduce (NCCL over NVLink) before the identical, redundant update on every ra
 threshold `maxGradNorm` applies to the norm of the summed (reduced) gradient.  A rank whose shard of a step
 holds more utterances than the net's buffers (`model.maxUtts`) accumulates the gradient over micro-batches of at
 most that many and then updates once (step_device_parts), so the batch size is not limited by device memory.
+A net built with dropout > 0 has its device step counter advanced once per optimisation step, as the step's first
+launch (inside the CUDA graph of step_device), so step `it` draws the masks of step `it` and the counter equals `it`.
 """
 import logging
 import pickle
@@ -90,6 +92,8 @@ class SGD:
         self.it = it
         self.costt = costt
         self.expcost = expcost
+        if self.model.dropoutStep is not None:      # a resumed run draws the masks an uninterrupted one would
+            self.model.dropoutStep.fill_(int(it))
         for (w, b), (wi, bi) in zip(self.velocity, stack):
             w.copy_(torch.from_numpy(np.ascontiguousarray(wi, dtype=np.float32).reshape(tuple(w.shape))))
             b.copy_(torch.from_numpy(np.ascontiguousarray(bi, dtype=np.float32).reshape(tuple(b.shape))))
@@ -127,9 +131,15 @@ class SGD:
             self._graphs[key] = g
         check(lib.ctcb_graph_launch(g, stream))
 
+    def _advance_dropout(self, stream):
+        m = self.model
+        if m.dropoutStep is not None:
+            check(lib.ctcb_dropout_advance(ptr(m.dropoutStep), stream))
+
     def _step_eager(self, batch, mom):
         m = self.model
         stream = _ctcb.current_stream()
+        self._advance_dropout(stream)
         # w = w + mom*velocity (evaluate gradient at future point)      sgd.py:91-93
         check(lib.ctcb_axpy_f32(ptr(m.params), ptr(self._vflat), float(mom), m.nparams, stream))
         # forward, CTC, backward -- and, with a communicator attached (ensure_comm), the exchange: the flat gradient and
@@ -151,10 +161,13 @@ class SGD:
         collectives whatever its number of micro-batches."""
         m = self.model
         stream = _ctcb.current_stream()
+        self._advance_dropout(stream)
         check(lib.ctcb_axpy_f32(ptr(m.params), ptr(self._vflat), float(mom), m.nparams, stream))
+        u0 = 0
         for k, piece in enumerate(pieces):
             batch = m.swap_batches().pack([d for d, _ in piece], [l for _, l in piece]).upload()
-            m.costAndGradDevice(batch, first=(k == 0), last=(k == len(pieces) - 1))
+            m.costAndGradDevice(batch, first=(k == 0), last=(k == len(pieces) - 1), u0=u0)
+            u0 += len(piece)
         check(lib.ctcb_sumsq_f32(ptr(m.grads), m.nparams, ptr(self._gnorm2), ptr(self._scratch), stream))
         check(lib.ctcb_sgd_nesterov_step_f32(ptr(m.params), ptr(self._vflat), ptr(m.grads), m.nparams, float(mom),
                                              float(self.alpha), float(self.maxGNorm), ptr(self._gnorm2),
@@ -211,6 +224,7 @@ class SGD:
             self.step_device_parts(prep["pieces"], mom)
         else:                  # this rank has no utterance this step: contribute zeros to the exchange
             st = _ctcb.current_stream()
+            self._advance_dropout(st)
             m.grads_ext.zero_()
             check(lib.ctcb_brnn_exchange_only(m._h, ptr(m.params), ptr(m.grads), ptr(m.stats), st))
             check(lib.ctcb_sumsq_f32(ptr(m.grads), m.nparams, ptr(self._gnorm2), ptr(self._scratch), st))
@@ -301,6 +315,7 @@ class SGD:
                 self._launch(prep, dist)
             else:
                 self.it += 1               # the reference counts skipped utterances too (sgd.py:71)
+                self._advance_dropout(_ctcb.current_stream())
             if pending is not None:
                 self._finish(pending, rank)
             pending = prep if active else None
