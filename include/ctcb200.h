@@ -286,7 +286,9 @@ int ctcb_brnn_set_dropout(ctcb_brnn *h, float p, uint64_t seed, const int64_t *s
  * micro-batched step and a data-parallel step draw the same mask for the same utterance.  Default (0, 1).  CTCB_EINVAL
  * for first < 0 or stride < 1.  Host-only. */
 int ctcb_brnn_set_dropout_utts(ctcb_brnn *h, int64_t first, int64_t stride);
-/* *step += 1 on `stream` (one thread); inside a capture it becomes part of the graph like any other launch. */
+/* *step += 1 on `stream` (one thread); inside a capture it becomes part of the graph like any other launch.  The
+ * counter is the optimisation step: the dropout mask and the adaptive optimisers (ctcb_adagrad_step_f32,
+ * ctcb_adam_step_f32) read the same one, and sgd.SGD advances it once per step, so it equals SGD.it. */
 int ctcb_dropout_advance(int64_t *step, void *stream);
 
 /* ---- the time recurrences of the temporal layer on their own (replaces the per-frame loops
@@ -329,6 +331,23 @@ int ctcb_sumsq_f32(const float *g, int64_t n, float *gnorm2_out, void *scratch, 
  * reference's `if skip: continue` does (sgd.py:109-111). */
 int ctcb_sgd_nesterov_step_f32(float *w, float *v, const float *g, int64_t n, float mom, float alpha,
                                float max_gnorm, const float *gnorm2, const float *n_valid, void *stream);
+/* The adaptive rules (not in the reference's working code: its AdaGrad branch, sgd.py:143-158, is never reached).
+ * Both run on the step's reduced gradient g (the L2 term already in it), with no look-ahead, clipped as a gradient:
+ *   g_c = c*g,  c = min(1, maxGNorm / sqrt(*gnorm2))           (gnorm2 read on the device, as for Nesterov)
+ * t is the int64 at `step` (DEVICE memory: the counter of ctcb_dropout_advance), read when the kernel runs; a value
+ * below 1 is taken as 1.  When n_valid (optional device float) reads 0, w and every state are left bit for bit
+ * unchanged.  Per-step scalars are computed in float64 and rounded to float32 once; the element arithmetic is float32.
+ * AdaGrad, state r (the reference's gradt):
+ *   gamma_t = 1 - 1/(0.01 t + 1);  r = gamma_t*r + g_c^2;  w -= alpha * g_c / sqrt(r + 1e-10)
+ * Adam (Kingma & Ba, Algorithm 1), states m and v:
+ *   m = b1*m + (1-b1)*g_c;  v = b2*v + (1-b2)*g_c^2;  w -= alpha * (m/(1-b1^t)) / (sqrt(v/(1-b2^t)) + eps)
+ * Checked on the host before any launch: n <= 0 is a no-op; CTCB_EINVAL for a null w, state, g, gnorm2 or step, a
+ * non-finite or negative alpha, a beta outside [0, 1), and a non-finite eps or eps <= 0. */
+int ctcb_adagrad_step_f32(float *w, float *r, const float *g, int64_t n, float alpha, float max_gnorm,
+                          const float *gnorm2, const float *n_valid, const int64_t *step, void *stream);
+int ctcb_adam_step_f32(float *w, float *m, float *v, const float *g, int64_t n, float alpha, float beta1,
+                       float beta2, float eps, float max_gnorm, const float *gnorm2, const float *n_valid,
+                       const int64_t *step, void *stream);
 
 /* ---- CUDA graphs: replay one optimisation step (the reference issues ~16(N+3)+8(T-1) launches per utterance,
  *      sgd.py:91-161 + brnnet.py:117-249; this library ~40 per minibatch) as ONE graph launch -----------------------

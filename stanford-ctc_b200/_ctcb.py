@@ -97,6 +97,9 @@ _PROTOS = {
     "ctcb_axpy_f32": (c_int, [c_vp, c_vp, c_f32, c_i64, c_vp]),
     "ctcb_sumsq_f32": (c_int, [c_vp, c_i64, c_vp, c_vp, c_vp]),
     "ctcb_sgd_nesterov_step_f32": (c_int, [c_vp, c_vp, c_vp, c_i64, c_f32, c_f32, c_f32, c_vp, c_vp, c_vp]),
+    "ctcb_adagrad_step_f32": (c_int, [c_vp, c_vp, c_vp, c_i64, c_f32, c_f32, c_vp, c_vp, c_vp, c_vp]),
+    "ctcb_adam_step_f32": (c_int, [c_vp, c_vp, c_vp, c_vp, c_i64, c_f32, c_f32, c_f32, c_f32, c_f32, c_vp, c_vp, c_vp,
+                                   c_vp]),
 }
 
 EXPORTS = sorted(_PROTOS)

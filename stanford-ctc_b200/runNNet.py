@@ -7,7 +7,8 @@ last_cost, sentinel, train.log), resume through --cfg_file with the step size re
 (runNNet.py:143-166), the fixed seeds 33 (:113-115) and CUDA_DEVICE device selection (:117-120).
 The implementation is organised differently: a declarative flag table, one RunDir helper that owns the
 side files, and separate train/evaluate phases.  Site paths of run_cfg.py / decoder_config.py became
-flags (--runDir, --outDir); new flags: --numTemporal, --batchSize, --maxUtts, --maxLabels, --dropout, --quiet.  Under torchrun the same
+flags (--runDir, --outDir); new flags: --numTemporal, --batchSize, --maxUtts, --maxLabels, --dropout, --optimizer,
+--beta1, --beta2, --epsilon, --quiet.  Under torchrun the same
 script trains data-parallel (one process per GPU, one NCCL all-reduce per step).
 """
 import argparse
@@ -52,6 +53,11 @@ FLAGS = [
     ("maxLabels", int, 511, "longest label sequence the buffers are sized for"),
     ("dropout", float, 0.0, "inverted dropout probability on the ReLU hidden layers while training (0 = off; "
                             "--test never drops)"),
+    ("optimizer", str, "nesterov", "update rule: nesterov (the reference's, with --momentum), adagrad or adam; --step "
+                                   "is the step size of each and --anneal applies to it"),
+    ("beta1", float, 0.9, "adam: decay of the first-moment estimate"),
+    ("beta2", float, 0.999, "adam: decay of the second-moment estimate"),
+    ("epsilon", float, 1e-8, "adam: added to the square root of the second moment"),
     ("runDir", str, "./runs", "parent of the time-stamped run directory"),
     ("outDir", str, None, "--test: directory for the likelihood arks"),
     ("quiet", None, False, "no console logging / per-iteration prints"),
@@ -193,8 +199,9 @@ def _train(opts, cfg, run_dir, log, rank, world):
                      maxUtts=utterance_capacity(opts, world),
                      maxLabels=min(opts.maxLabels, opts.maxUttLen), dropout=opts.dropout)
     net.initParams()
-    optimizer = sgd.SGD(net, opts.maxUttLen, alpha=opts.step, momentum=opts.momentum, batchSize=opts.batchSize,
-                        verbose=(rank == 0 and not opts.quiet))
+    optimizer = sgd.SGD(net, opts.maxUttLen, alpha=opts.step, optimizer=opts.optimizer, momentum=opts.momentum,
+                        batchSize=opts.batchSize, verbose=(rank == 0 and not opts.quiet), beta1=opts.beta1,
+                        beta2=opts.beta2, epsilon=opts.epsilon)
     cfg["param_count"] = net.paramCount()
     if rank == 0:
         dump_config(cfg, opts.cfg_file)

@@ -15,6 +15,10 @@ holds more utterances than the net's buffers (`model.maxUtts`) accumulates the g
 most that many and then updates once (step_device_parts), so the batch size is not limited by device memory.
 A net built with dropout > 0 has its device step counter advanced once per optimisation step, as the step's first
 launch (inside the CUDA graph of step_device), so step `it` draws the masks of step `it` and the counter equals `it`.
+`optimizer` is 'nesterov' (the reference's rule and the default), 'adagrad' (the reference's unfinished branch,
+sgd.py:24-26,143-158, state `gradt`) or 'adam' (state `moment1`, `moment2`; beta1, beta2, epsilon); the rules are stated
+in include/ctcb200.h.  The adaptive rules read the step number t from the same device counter (allocated here when
+the net has no dropout), so graph replays see the current step.
 """
 import logging
 import pickle
@@ -27,11 +31,42 @@ from _ctcb import lib, check, ptr
 from nnets.brnnet import FlatList
 import parallel
 
+# the state vectors of each rule, by the attribute names that hold them as [W, b] FlatLists (velocity: sgd.py:30-33,
+# gradt: sgd.py:28)
+OPTIMIZERS = {"nesterov": ("velocity",), "adagrad": ("gradt",), "adam": ("moment1", "moment2")}
+
+
+def pack_state(optimizer, pairs):
+    """The optimiser state entry of the first pickle of params.pk.  pairs: {state name: [[W, b], ...]}.  Nesterov's is
+    the reference's list of velocity pairs; the adaptive rules' is a dict that names its rule."""
+    if optimizer == "nesterov":
+        return pairs["velocity"]
+    return dict(optimizer=optimizer, **{name: pairs[name] for name in OPTIMIZERS[optimizer]})
+
+
+def unpack_state(optimizer, state):
+    """{state name: [[W, b], ...]} of a pack_state entry; ValueError when it belongs to another rule."""
+    saved = state.get("optimizer") if isinstance(state, dict) else "nesterov"
+    if saved != optimizer:
+        raise ValueError("the checkpoint holds the state of the %r optimizer; this SGD runs %r" % (saved, optimizer))
+    if optimizer == "nesterov":
+        return {"velocity": state}
+    return {name: state[name] for name in OPTIMIZERS[optimizer]}
+
 
 class SGD:
 
     def __init__(self, model, maxBatch, alpha=1e-2, optimizer='nesterov',
-                 momentum=0.9, maxGradNorm=1500, batchSize=1, verbose=True, bucketPool=16):
+                 momentum=0.9, maxGradNorm=1500, batchSize=1, verbose=True, bucketPool=16,
+                 beta1=0.9, beta2=0.999, epsilon=1e-8):
+        if optimizer not in OPTIMIZERS:          # ctc/sgd.py:27
+            raise ValueError("optimizer=%r: one of %s" % (optimizer, ", ".join(sorted(OPTIMIZERS))))
+        if optimizer == "adam":
+            for name, beta in (("beta1", beta1), ("beta2", beta2)):
+                if not 0.0 <= beta < 1.0:
+                    raise ValueError("%s=%r must be in [0, 1)" % (name, beta))
+            if not (0.0 < epsilon < float("inf")):
+                raise ValueError("epsilon=%r must be finite and > 0" % (epsilon,))
         torch = _ctcb.require_cuda()
         self._torch = torch
         self.model = model
@@ -40,6 +75,7 @@ class SGD:
         self.momentum = momentum  # momentum
         self.alpha = alpha  # learning rate
         self.optimizer = optimizer
+        self.beta1, self.beta2, self.epsilon = beta1, beta2, epsilon      # adam only
         self.maxGNorm = maxGradNorm  # gradient clip norm value
         self.batchSize = batchSize
         self.verbose = verbose
@@ -54,11 +90,18 @@ class SGD:
         self._stream = None
         self.padded_frames = 0
         self.real_frames = 0
-        # the reference's adagrad branch is dead code (`assert False`, sgd.py:24-26)
-        assert self.optimizer == 'nesterov', "only the nesterov optimizer exists (sgd.py:24-26)"
 
-        self._vflat = torch.zeros(model.nparams, dtype=torch.float32, device=model.dev)
-        self.velocity = FlatList(model._views(self._vflat), self._vflat)
+        # each state is one flat fp32 vector, exposed as the FlatList attribute OPTIMIZERS names (self.velocity, ...)
+        self._flat = {}
+        for name in OPTIMIZERS[optimizer]:
+            self._flat[name] = torch.zeros(model.nparams, dtype=torch.float32, device=model.dev)
+            setattr(self, name, FlatList(model._views(self._flat[name]), self._flat[name]))
+        self._vflat = self._flat.get("velocity")
+        # the optimisation step on the device: the dropout counter when the net has one, else one of our own where the
+        # rule reads t (a Nesterov step on a net without dropout needs none and launches nothing for it)
+        self._step = model.dropoutStep
+        if self._step is None and optimizer != "nesterov":
+            self._step = torch.zeros(1, dtype=torch.int64, device=model.dev)
         self._gnorm2 = model._gnorm2          # lives in the 8-float record behind the flat gradient
         self._scratch = torch.zeros(8192, dtype=torch.uint8, device=model.dev)
         # per-step log record {n_valid, sum nll, n_skipped, sweep error flag, gnorm^2, regcost, -, -}: the 8 floats behind
@@ -78,8 +121,9 @@ class SGD:
 
     # ------------------------------------------------------------------ persistence (sgd.py:36-55)
     def toFile(self, fid):
-        stack = [[w.cpu().numpy(), b.cpu().numpy()] for w, b in self.velocity]
-        pickle.dump([self.it, self.costt, self.expcost, stack], fid)
+        pairs = {name: [[w.cpu().numpy(), b.cpu().numpy()] for w, b in getattr(self, name)]
+                 for name in OPTIMIZERS[self.optimizer]}
+        pickle.dump([self.it, self.costt, self.expcost, pack_state(self.optimizer, pairs)], fid)
 
     def fromFile(self, fid):
         torch = self._torch
@@ -88,28 +132,31 @@ class SGD:
         except UnicodeDecodeError:
             fid.seek(0)
             params = pickle.load(fid, encoding="latin1")
-        it, costt, expcost, stack = params
+        it, costt, expcost, state = params
+        states = unpack_state(self.optimizer, state)
         self.it = it
         self.costt = costt
         self.expcost = expcost
-        if self.model.dropoutStep is not None:      # a resumed run draws the masks an uninterrupted one would
-            self.model.dropoutStep.fill_(int(it))
-        for (w, b), (wi, bi) in zip(self.velocity, stack):
-            w.copy_(torch.from_numpy(np.ascontiguousarray(wi, dtype=np.float32).reshape(tuple(w.shape))))
-            b.copy_(torch.from_numpy(np.ascontiguousarray(bi, dtype=np.float32).reshape(tuple(b.shape))))
+        if self._step is not None:      # a resumed run draws the masks and takes the steps an uninterrupted one would
+            self._step.fill_(int(it))
+        for name, stack in states.items():
+            for (w, b), (wi, bi) in zip(getattr(self, name), stack):
+                w.copy_(torch.from_numpy(np.ascontiguousarray(wi, dtype=np.float32).reshape(tuple(w.shape))))
+                b.copy_(torch.from_numpy(np.ascontiguousarray(bi, dtype=np.float32).reshape(tuple(b.shape))))
 
     # ------------------------------------------------------------------ one optimisation step
     def step_device(self, batch, mom):
-        """Enqueue one full Nesterov step for a staged DeviceBatch; never synchronises with the host.
-        sgd.py:91-161: look-ahead, costAndGrad, (all-reduce), global norm, clip, velocity, update.
+        """Enqueue one full optimisation step for a staged DeviceBatch; never synchronises with the host.
+        sgd.py:91-161: (Nesterov: look-ahead,) costAndGrad, (all-reduce), global norm, clip, update.
         On a non-default stream the step is captured into a CUDA graph the third time the same (buffers, B, Tmax,
-        momentum, step size) combination is seen and replayed as one launch from then on (the first two occurrences
-        run eagerly: first-use initialisation is not capturable)."""
+        rule and its scalars, step size) combination is seen and replayed as one launch from then on (the first two
+        occurrences run eagerly: first-use initialisation is not capturable)."""
         stream = _ctcb.current_stream()
         if not self.useGraphs or not stream:          # the legacy default stream cannot be captured
             return self._step_eager(batch, mom)
         import ctypes
-        key = (id(batch), batch.B, batch.Tmax, float(mom), float(self.alpha), float(self.maxGNorm), stream)
+        key = (id(batch), batch.B, batch.Tmax, float(mom), float(self.alpha), float(self.maxGNorm), stream,
+               self.optimizer, float(self.beta1), float(self.beta2), float(self.epsilon))
         g = self._graphs.get(key)
         if g is None:
             seen = self._graph_seen.get(key, 0)
@@ -131,47 +178,65 @@ class SGD:
             self._graphs[key] = g
         check(lib.ctcb_graph_launch(g, stream))
 
-    def _advance_dropout(self, stream):
+    def _advance_step(self, stream):
+        """The step's first launch: the device step counter (dropout's and the adaptive rules' t), where one exists."""
+        if self._step is not None:
+            check(lib.ctcb_dropout_advance(ptr(self._step), stream))
+
+    def _look_ahead(self, mom, stream):
+        """Nesterov evaluates the gradient at w + mom*velocity (sgd.py:91-93); the adaptive rules at w."""
         m = self.model
-        if m.dropoutStep is not None:
-            check(lib.ctcb_dropout_advance(ptr(m.dropoutStep), stream))
+        if self.optimizer == "nesterov":
+            check(lib.ctcb_axpy_f32(ptr(m.params), ptr(self._vflat), float(mom), m.nparams, stream))
+
+    def _update(self, mom, stream):
+        """Global norm of the (reduced) gradient, then the rule's fused clip and update; a step whose utterances were
+        all skipped (n_valid = 0, the first float of m.stats) changes nothing but Nesterov's undo of the look-ahead."""
+        m = self.model
+        # gnorm over all parameters as one vector                       sgd.py:103-107
+        check(lib.ctcb_sumsq_f32(ptr(m.grads), m.nparams, ptr(self._gnorm2), ptr(self._scratch), stream))
+        if self.optimizer == "nesterov":
+            # undo look-ahead, clip, velocity, update                   sgd.py:97-100,130-140,161
+            check(lib.ctcb_sgd_nesterov_step_f32(ptr(m.params), ptr(self._vflat), ptr(m.grads), m.nparams, float(mom),
+                                                 float(self.alpha), float(self.maxGNorm), ptr(self._gnorm2),
+                                                 ptr(m.stats), stream))
+        elif self.optimizer == "adagrad":
+            check(lib.ctcb_adagrad_step_f32(ptr(m.params), ptr(self._flat["gradt"]), ptr(m.grads), m.nparams,
+                                            float(self.alpha), float(self.maxGNorm), ptr(self._gnorm2), ptr(m.stats),
+                                            ptr(self._step), stream))
+        else:
+            check(lib.ctcb_adam_step_f32(ptr(m.params), ptr(self._flat["moment1"]), ptr(self._flat["moment2"]),
+                                         ptr(m.grads), m.nparams, float(self.alpha), float(self.beta1),
+                                         float(self.beta2), float(self.epsilon), float(self.maxGNorm),
+                                         ptr(self._gnorm2), ptr(m.stats), ptr(self._step), stream))
 
     def _step_eager(self, batch, mom):
         m = self.model
         stream = _ctcb.current_stream()
-        self._advance_dropout(stream)
-        # w = w + mom*velocity (evaluate gradient at future point)      sgd.py:91-93
-        check(lib.ctcb_axpy_f32(ptr(m.params), ptr(self._vflat), float(mom), m.nparams, stream))
+        self._advance_step(stream)
+        self._look_ahead(mom, stream)
         # forward, CTC, backward -- and, with a communicator attached (ensure_comm), the exchange: the flat gradient and
         # its statistics tail summed over ranks by libctcb200 itself (NCCL), part of it under the BPTT sweep
         m.costAndGradDevice(batch)
-        # gnorm over all parameters as one vector                       sgd.py:103-107
-        check(lib.ctcb_sumsq_f32(ptr(m.grads), m.nparams, ptr(self._gnorm2), ptr(self._scratch), stream))
-        # undo look-ahead, clip, velocity, update                       sgd.py:97-100,130-140,161
-        check(lib.ctcb_sgd_nesterov_step_f32(ptr(m.params), ptr(self._vflat), ptr(m.grads), m.nparams, float(mom),
-                                             float(self.alpha), float(self.maxGNorm), ptr(self._gnorm2),
-                                             ptr(m.stats), stream))
+        self._update(mom, stream)
 
     def step_device_parts(self, pieces, mom):
-        """One Nesterov step whose shard holds more utterances than the net's buffers (model.maxUtts): the gradient is
-        accumulated over consecutive micro-batches (`pieces`: lists of (data, labels) pairs, each at most maxUtts
+        """One optimisation step whose shard holds more utterances than the net's buffers (model.maxUtts): the gradient
+        is accumulated over consecutive micro-batches (`pieces`: lists of (data, labels) pairs, each at most maxUtts
         long), then the norm and the update run once.  Each micro-batch is packed into the staging buffer the
         device is not reading while the previous one computes; the step runs eagerly (not as a CUDA graph).  With a
         communicator attached, only the last micro-batch's call exchanges, so every rank issues the same
         collectives whatever its number of micro-batches."""
         m = self.model
         stream = _ctcb.current_stream()
-        self._advance_dropout(stream)
-        check(lib.ctcb_axpy_f32(ptr(m.params), ptr(self._vflat), float(mom), m.nparams, stream))
+        self._advance_step(stream)
+        self._look_ahead(mom, stream)
         u0 = 0
         for k, piece in enumerate(pieces):
             batch = m.swap_batches().pack([d for d, _ in piece], [l for _, l in piece]).upload()
             m.costAndGradDevice(batch, first=(k == 0), last=(k == len(pieces) - 1), u0=u0)
             u0 += len(piece)
-        check(lib.ctcb_sumsq_f32(ptr(m.grads), m.nparams, ptr(self._gnorm2), ptr(self._scratch), stream))
-        check(lib.ctcb_sgd_nesterov_step_f32(ptr(m.params), ptr(self._vflat), ptr(m.grads), m.nparams, float(mom),
-                                             float(self.alpha), float(self.maxGNorm), ptr(self._gnorm2),
-                                             ptr(m.stats), stream))
+        self._update(mom, stream)
 
     def ensure_comm(self):
         """Data parallelism: create this process's ctcb communicator (once per model) and attach it to the net.  The
@@ -224,14 +289,13 @@ class SGD:
             self.step_device_parts(prep["pieces"], mom)
         else:                  # this rank has no utterance this step: contribute zeros to the exchange
             st = _ctcb.current_stream()
-            self._advance_dropout(st)
+            self._advance_step(st)
             m.grads_ext.zero_()
             check(lib.ctcb_brnn_exchange_only(m._h, ptr(m.params), ptr(m.grads), ptr(m.stats), st))
-            check(lib.ctcb_sumsq_f32(ptr(m.grads), m.nparams, ptr(self._gnorm2), ptr(self._scratch), st))
-            check(lib.ctcb_axpy_f32(ptr(m.params), ptr(self._vflat), float(mom), m.nparams, st))
-            check(lib.ctcb_sgd_nesterov_step_f32(ptr(m.params), ptr(self._vflat), ptr(m.grads), m.nparams, float(mom),
-                                                 float(self.alpha), float(self.maxGNorm), ptr(self._gnorm2),
-                                                 ptr(m.stats), st))
+            # the look-ahead after the exchange (which reads w for the L2 term), as this branch has always done it;
+            # it writes only w and the norm reads only g, so _update's norm after it gives the same bits
+            self._look_ahead(mom, st)
+            self._update(mom, st)
         slot = self._log_slot
         self._log_slot ^= 1
         self._log_host[slot].copy_(m.record, non_blocking=True)
@@ -271,7 +335,8 @@ class SGD:
                      prep["nlab"], prep["nframes"]))
 
     def run(self, data_dict, alis, keys, sizes):
-        """Runs stochastic gradient descent with nesterov acceleration.  Model is objective.
+        """Runs stochastic gradient descent with the optimizer's rule (nesterov acceleration by default).  Model is
+        objective.
         Steps are software-pipelined: while the device works on minibatch i the host checks, packs, uploads and
         enqueues minibatch i+1 (second staging buffer); step i's log record is read after that."""
         dist, rank, world = self._world()
@@ -315,7 +380,7 @@ class SGD:
                 self._launch(prep, dist)
             else:
                 self.it += 1               # the reference counts skipped utterances too (sgd.py:71)
-                self._advance_dropout(_ctcb.current_stream())
+                self._advance_step(_ctcb.current_stream())
             if pending is not None:
                 self._finish(pending, rank)
             pending = prep if active else None
