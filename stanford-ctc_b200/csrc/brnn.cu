@@ -148,8 +148,12 @@ struct ctcb_brnn {
     // weight/bias gradients of the layers at and above the temporal layer depend only on their delta, so they
     // run on a side stream next to the (latency-bound, 112-SM) BPTT sweep; created on first use
     cudaStream_t side;
+    // the main chain of a training call (forward, CTC, delta contractions, sweeps, the tail below the temporal layer)
+    // runs on `hi`, forked from the caller's stream and joined back into it: the greatest priority, so its kernels take
+    // SMs ahead of the side stream's pending CTAs (the recurrent weight-gradient pair in particular)
+    cudaStream_t hi;
     cudaEvent_t ev_delta[66];
-    cudaEvent_t ev_side;
+    cudaEvent_t ev_side, ev_fork, ev_hi;
     // the two dFor/dBack pairs that stacked temporal layers alternate: ev_pair[p] is recorded on the side stream after
     // its last read of pair p, and the BPTT sweep that writes pair p next waits for it
     cudaEvent_t ev_pair[2];
@@ -417,6 +421,9 @@ extern "C" int ctcb_brnn_create(const ctcb_brnn_config *cfg, ctcb_brnn **out) {
 extern "C" void ctcb_brnn_destroy(ctcb_brnn *h) {
     if (h && h->side_ready) {
         cudaStreamDestroy(h->side);
+        cudaStreamDestroy(h->hi);
+        cudaEventDestroy(h->ev_fork);
+        cudaEventDestroy(h->ev_hi);
         for (int i = 0; i < 66; ++i) cudaEventDestroy(h->ev_delta[i]);
         cudaEventDestroy(h->ev_side);
         for (int p = 0; p < 2; ++p) cudaEventDestroy(h->ev_pair[p]);
@@ -426,9 +433,13 @@ extern "C" void ctcb_brnn_destroy(ctcb_brnn *h) {
 
 static int ensure_side_stream(ctcb_brnn *h) {
     if (h->side_ready) return CTCB_OK;
-    CTCB_CUDA_CHECK(cudaStreamCreateWithFlags(&h->side, cudaStreamNonBlocking));
+    // the lowest priority: the side stream's CTAs never take an SM that a pending sweep cluster could use
+    CTCB_CUDA_CHECK(cudaStreamCreateWithPriority(&h->side, cudaStreamNonBlocking, stream_priority_least()));
     for (int i = 0; i < 66; ++i) CTCB_CUDA_CHECK(cudaEventCreateWithFlags(&h->ev_delta[i], cudaEventDisableTiming));
+    CTCB_CUDA_CHECK(cudaStreamCreateWithPriority(&h->hi, cudaStreamNonBlocking, stream_priority_greatest()));
     CTCB_CUDA_CHECK(cudaEventCreateWithFlags(&h->ev_side, cudaEventDisableTiming));
+    CTCB_CUDA_CHECK(cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming));
+    CTCB_CUDA_CHECK(cudaEventCreateWithFlags(&h->ev_hi, cudaEventDisableTiming));
     for (int p = 0; p < 2; ++p) CTCB_CUDA_CHECK(cudaEventCreateWithFlags(&h->ev_pair[p], cudaEventDisableTiming));
     h->side_ready = true;
     return CTCB_OK;
@@ -634,6 +645,14 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
     m.sweep = ws + w.sweep;
     m.sweep_bytes = w.sweep_bytes;
     const bool drop = h->drop_p > 0.f;
+    const bool overlap = (tl > 0);     // layers i >= tl: dW/db on the side stream, delta chain + BPTT on the main one
+    const cudaStream_t caller = st;
+    if (overlap) {     // fork: the main chain runs on h->hi until the join below
+        TRY(ensure_side_stream(h));
+        CTCB_CUDA_CHECK(cudaEventRecord(h->ev_fork, caller));
+        CTCB_CUDA_CHECK(cudaStreamWaitEvent(h->hi, h->ev_fork, 0));
+        st = h->hi;
+    }
     TRY(brnn_forward(h, feats, T_per_utt, B, Tmax, params, probs_out, m, drop, st));
     float *logits = Xbuf(N + 1);
 
@@ -646,26 +665,24 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
     }
 
     // ---------------------------------------------------------------- backward (brnnet.py:188-243)
-    // Per temporal layer from the top: the delta GEMM without a mask, the BPTT sweep into pair j % 2, the recurrent
-    // weight-gradient pair on the side stream, add2.  Layer j - 2 writes the pair layer j used: its sweep waits for
-    // ev_pair, recorded on the side stream behind the last read of that pair (the recurrent weight gradients; for a
-    // uni-directional layer the weight gradient of the map above, whose delta the pair is).
-    const bool overlap = (tl > 0);     // layers i >= tl: dW/db on the side stream, delta chain + BPTT on the main one
+    // Per temporal layer from the top: the delta GEMM without a mask, the BPTT sweep into pair j % 2, then on the side
+    // stream the weight gradients of the maps from the last sweep's down to this layer and the recurrent
+    // weight-gradient pair, add2.  The side stream's weight gradients become ready together with the sweep, not before
+    // it: the sweep's clusters (the higher priority) take their SMs first and the GEMMs run on the rest for the length
+    // of the sweep, instead of holding SMs the sweep then waits for.  Layer j - 2 writes the pair layer j used: its
+    // sweep waits for ev_pair, recorded on the side stream behind the last read of that pair (the recurrent weight
+    // gradients; for a uni-directional layer the weight gradient of the map above, whose delta the pair is).
     const bool dp = (h->comm != nullptr) && comm_world(h->comm) > 1;
-    if (overlap) TRY(ensure_side_stream(h));
     void *gws2 = ws + w.gemm2;
     const size_t gws2_bytes = w.colsum - w.gemm2;
-    for (int i = N; i >= 0; --i) {
+    // rnnet.py:162-177: the BPTT result of a uni-directional layer is the delta
+    auto delta_of = [&](int i) -> float * { return (uni && temporal(i + 1)) ? dF[(i + 1 - tl) % 2] : dbuf(i + 1); };
+    // the weight and bias gradients of map i on stream sw, where its delta is complete
+    auto weight_grads = [&](int i, cudaStream_t sw) -> int {
         const float *Xi = (i == 0) ? feats : Act(i);
         const int n_out = sz[i + 1], n_in = sz[i];
-        // rnnet.py:162-177: the BPTT result of a uni-directional layer is the delta
-        float *dcur = (uni && temporal(i + 1)) ? dF[(i + 1 - tl) % 2] : dbuf(i + 1);
-        const bool on_side = overlap && i >= tl;
-        cudaStream_t sw = on_side ? h->side : st;
-        if (on_side) {     // dcur is complete on the main stream here
-            CTCB_CUDA_CHECK(cudaEventRecord(h->ev_delta[i], st));
-            CTCB_CUDA_CHECK(cudaStreamWaitEvent(h->side, h->ev_delta[i], 0));
-        }
+        float *dcur = delta_of(i);
+        const bool on_side = (sw != st);
         // dW = delta^T . X_i   (brnnet.py:196)
         {
         ProfScope ps("gemm_dw", sw);
@@ -704,6 +721,14 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
             const int64_t na = (G(2 * N + 1) + sz[N + 1]) - pa;
             TRY(comm_allreduce_ranges(h->comm, &pa, &na, 1, h->side));
         }
+        return CTCB_OK;
+    };
+    int side_top = N;      // the highest map >= tl whose weight gradients are not queued yet
+    for (int i = N; i >= 0; --i) {
+        const float *Xi = (i == 0) ? feats : Act(i);
+        const int n_out = sz[i + 1], n_in = sz[i];
+        float *dcur = delta_of(i);
+        if (!(overlap && i >= tl)) TRY(weight_grads(i, st));
         if (i > 0) {
             float *doth = dbuf(i);
             // delta <- delta . W, with the ReLU mask sign(hActs[i]) fused (brnnet.py:203-204,235-237).  A dropped
@@ -721,11 +746,15 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
                 float *dFor = dF[p], *dBack = dB[p], *For = ForJ[j], *Back = BackJ[j];
                 if (j + 2 < nt)      // layer j + 2 used this pair
                     CTCB_CUDA_CHECK(cudaStreamWaitEvent(st, h->ev_pair[p], 0));
+                // the deltas of maps side_top..i are complete here
+                CTCB_CUDA_CHECK(cudaEventRecord(h->ev_delta[i], st));
                 {
                 ProfScope ps("sweep_bptt", st);
                 TRY(run_sweep(1, Tmax, B, H, T_per_utt, doth, P(iWtf), uni ? nullptr : P(iWtb), dFor, dBack, For, Back,
                               c.maxAct, counters, ws + w.sweep, w.sweep_bytes, st));
                 }
+                CTCB_CUDA_CHECK(cudaStreamWaitEvent(h->side, h->ev_delta[i], 0));
+                for (; side_top >= i; --side_top) TRY(weight_grads(side_top, h->side));
                 // recurrent weight gradients (brnnet.py:227-230): independent of the rest of the backward pass,
                 // so they go to the side stream as well
                 CTCB_CUDA_CHECK(cudaEventRecord(h->ev_delta[65], st));
@@ -753,10 +782,7 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
             }
         }
     }
-    if (overlap) {     // join: every gradient tensor is complete on the caller's stream from here on
-        CTCB_CUDA_CHECK(cudaEventRecord(h->ev_side, h->side));
-        CTCB_CUDA_CHECK(cudaStreamWaitEvent(st, h->ev_side, 0));
-    }
+    // the main stream's tail writes nothing the side stream touches, so it runs next to the recurrent weight gradients
     for (int j = 0; j < nt; ++j) {   // the `dummy` biases never receive gradient
         const int iWtf = rec_index(&c, j);
         CTCB_CUDA_CHECK(cudaMemsetAsync(G(iWtf + 1), 0, sizeof(float), st));
@@ -767,6 +793,13 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
         if (first) batch_stats_kernel<false><<<1, 32, 0, st>>>(cost_out, skip_out, B, stats_out, counters);
         else batch_stats_kernel<true><<<1, 32, 0, st>>>(cost_out, skip_out, B, stats_out, counters);
         CTCB_LAUNCH_CHECK();
+    }
+    if (overlap) {     // join: every gradient tensor is complete on the caller's stream from here on
+        CTCB_CUDA_CHECK(cudaEventRecord(h->ev_side, h->side));
+        CTCB_CUDA_CHECK(cudaEventRecord(h->ev_hi, h->hi));
+        CTCB_CUDA_CHECK(cudaStreamWaitEvent(caller, h->ev_side, 0));
+        CTCB_CUDA_CHECK(cudaStreamWaitEvent(caller, h->ev_hi, 0));
+        st = caller;
     }
     // an earlier micro-batch of the step: the exchange and the L2 term wait for the sum of all of them
     if (!last) return CTCB_OK;

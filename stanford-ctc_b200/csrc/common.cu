@@ -31,6 +31,19 @@ int num_sms() {
     return n;
 }
 
+static void stream_priority_range(int *least, int *greatest) {
+    static int lo = 0, hi = 0;
+    static bool read = false;
+    if (!read) {
+        if (cudaDeviceGetStreamPriorityRange(&lo, &hi) != cudaSuccess) { cudaGetLastError(); lo = hi = 0; }
+        read = true;
+    }
+    *least = lo;
+    *greatest = hi;
+}
+int stream_priority_least() { int lo, hi; stream_priority_range(&lo, &hi); return lo; }
+int stream_priority_greatest() { int lo, hi; stream_priority_range(&lo, &hi); return hi; }
+
 // The documented values of each knob, in the order of enum Knob: the string values[v] sets the value v.  A value the
 // environment gives that is not listed here leaves the default in effect.
 struct KnobDef { const char *name; int dflt; const char *values[9]; };
@@ -171,7 +184,9 @@ extern "C" int ctcb_graph_capture_end(void *stream, ctcb_graph **out) {
     if (!h) { cudaGraphDestroy(g); return set_error(CTCB_ENOMEM, "ctcb_graph_capture_end: out of host memory"); }
     h->launches = g_launch_count.load() - g_capture_launch0;
     g_launch_count.fetch_sub(h->launches);      // nothing ran during capture
-    e = cudaGraphInstantiate(&h->exec, g, 0);
+    // per-node priorities: without the flag every node runs at the launching stream's priority, and the BPTT sweep
+    // would no longer take its SMs ahead of the side stream's weight gradients (brnn.cu)
+    e = cudaGraphInstantiateWithFlags(&h->exec, g, cudaGraphInstantiateFlagUseNodePriority);
     cudaGraphDestroy(g);
     if (e != cudaSuccess) {
         delete h;

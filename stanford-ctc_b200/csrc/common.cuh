@@ -33,6 +33,9 @@ inline void count_launch(int n = 1) { g_launch_count.fetch_add((uint64_t)n, std:
     } while (0)
 
 int num_sms();
+// The device's stream priority range (cudaDeviceGetStreamPriorityRange): least is the default, greatest runs first.
+int stream_priority_least();
+int stream_priority_greatest();
 
 // Debug / measurement overrides of the planners (INTEGRATION.md section 4): one table (common.cu), filled from the
 // environment at first use and changed by ctcb_debug_set_knob.  Planners read it through knob() on every planning call.

@@ -246,13 +246,17 @@ static int launch_cluster_nb(const SweepClusterArgs &a, int ntiles, cudaStream_t
     cfg.blockDim = dim3(512);
     cfg.dynamicSmemBytes = SMEM;
     cfg.stream = st;
-    cudaLaunchAttribute attr[1];
+    cudaLaunchAttribute attr[2];
     attr[0].id = cudaLaunchAttributeClusterDimension;
     attr[0].val.clusterDim.x = CS;
     attr[0].val.clusterDim.y = 1;
     attr[0].val.clusterDim.z = 1;
+    // the serial chain of the step: its clusters are placed before any pending CTA of a lower-priority stream (the
+    // weight gradients that run next to the BPTT sweep, brnn.cu).  A launch attribute, so a captured graph keeps it.
+    attr[1].id = cudaLaunchAttributePriority;
+    attr[1].val.priority = stream_priority_greatest();
     cfg.attrs = attr;
-    cfg.numAttrs = 1;
+    cfg.numAttrs = 2;
     CTCB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, a));
     count_launch();
     return CTCB_OK;
