@@ -125,68 +125,75 @@ __global__ void batch_stats_kernel(const float *__restrict__ cost, const int32_t
     }
 }
 
+
+// both stages of the column sums of the row-major R x n matrix `delta` into out[n]; `partial` holds one row of n floats
+// per CS_ROWS_MIN rows of R
+int run_colsum(const float *delta, int64_t R, int n, float *partial, float *out, bool accumulate, cudaStream_t st) {
+    int nblk;
+    if (n % 4 == 0 && (((uintptr_t)delta) & 15) == 0) {
+        const int n4 = n / 4;
+        const int bx = n4 >= 256 ? 256 : (n4 + 31) / 32 * 32;
+        const int ncb = (n4 + bx - 1) / bx;
+        int64_t rpb = R / (2 * num_sms() / ncb > 0 ? 2 * num_sms() / ncb : 1);     // ~2 blocks per SM
+        if (rpb < CS_ROWS_MIN) rpb = CS_ROWS_MIN;
+        if (rpb > CS_ROWS) rpb = CS_ROWS;
+        nblk = (int)((R + rpb - 1) / rpb);
+        colsum_stage1_wide<<<dim3(ncb, nblk), bx, 0, st>>>((const float4 *)delta, R, n4, (int)rpb, (float4 *)partial);
+    } else {
+        nblk = (int)((R + CS_ROWS - 1) / CS_ROWS);
+        colsum_stage1<<<dim3((n + 31) / 32, nblk), dim3(32, 8), 0, st>>>(delta, R, n, partial);
+    }
+    CTCB_LAUNCH_CHECK();
+    if (!accumulate) colsum_stage2<false><<<(n + 127) / 128, 128, 0, st>>>(partial, nblk, n, out);
+    else colsum_stage2<true><<<(n + 127) / 128, 128, 0, st>>>(partial, nblk, n, out);
+    CTCB_LAUNCH_CHECK();
+    return CTCB_OK;
+}
+
+int run_batch_stats(const float *cost, const int32_t *skip, int B, float *stats, const unsigned int *errflag,
+                    bool accumulate, cudaStream_t st) {
+    if (!accumulate) batch_stats_kernel<false><<<1, 32, 0, st>>>(cost, skip, B, stats, errflag);
+    else batch_stats_kernel<true><<<1, 32, 0, st>>>(cost, skip, B, stats, errflag);
+    CTCB_LAUNCH_CHECK();
+    return CTCB_OK;
+}
+
 }  // namespace ctcb
 
 using namespace ctcb;
 
-namespace {
-// The buffers of a forward-only call: affine map i writes slab i % 2 and reads the other one (or For, the output of
-// the uni-directional temporal layer), so two slabs of the wider of H and K carry the whole stack.
-struct FwdLayout {
-    size_t slab[2];
-    size_t For, Back, gemm, gemm_bytes, counters, sweep, sweep_bytes;
-    size_t total;
-};
-}  // namespace
+#define TRY(expr)                    \
+    do {                             \
+        int _rc = (expr);            \
+        if (_rc != CTCB_OK) return _rc; \
+    } while (0)
 
-struct ctcb_brnn {
-    ctcb_brnn_config cfg;
-    int nlayers;        // N + 1 affine maps
-    int tl;             // lowest temporal layer or 0
-    int nt;             // temporal layers tl .. tl+nt-1 (0 without)
-    int sizes[66];      // [D, H.., K]
-    // weight/bias gradients of the layers at and above the temporal layer depend only on their delta, so they
-    // run on a side stream next to the (latency-bound, 112-SM) BPTT sweep; created on first use
-    cudaStream_t side;
-    // the main chain of a training call (forward, CTC, delta contractions, sweeps, the tail below the temporal layer)
-    // runs on `hi`, forked from the caller's stream and joined back into it: the greatest priority, so its kernels take
-    // SMs ahead of the side stream's pending CTAs (the recurrent weight-gradient pair in particular)
-    cudaStream_t hi;
-    cudaEvent_t ev_delta[66];
-    cudaEvent_t ev_side, ev_fork, ev_hi;
-    // the two dFor/dBack pairs that stacked temporal layers alternate: ev_pair[p] is recorded on the side stream after
-    // its last read of pair p, and the BPTT sweep that writes pair p next waits for it
-    cudaEvent_t ev_pair[2];
-    bool side_ready;
-    // data-parallel callers sum the gradient over ranks first and add reg*W ONCE afterwards (ctcb_brnn_apply_l2_f32);
-    // the L2 cost is still reported by every call
-    bool defer_l2;
-    // data-parallel exchange inside the step (ctcb_brnn_set_comm): the gradients of the layers at and above the temporal
-    // layer are summed over ranks on the side stream WHILE the BPTT sweep runs, the rest (+ statistics tail) at the end
-    ctcb_comm *comm;
-    // the forward layout, computed on the first forward-only call (its GEMM area takes a few hundred size queries)
-    bool fwd_ready;
-    FwdLayout fwd;
-    // inverted dropout of the ReLU hidden layers in training calls (ctcb_brnn_set_dropout); drop_p == 0: off
-    float drop_p;
-    uint64_t drop_seed;
-    const int64_t *drop_step;       // the caller's device counter
-    uint32_t drop_thr;              // keep iff Philox output >= drop_thr
-    float drop_scale;               // 1 / (1 - p), rounded once; also the delta contraction's alpha
-    int64_t drop_first, drop_stride;
-};
-
+// ---- the config: validity, layer sizes, the flat parameter vector ------------------------------
+// Why a config cannot be used, worded for the caller of ctcb_brnn_create (into `buf` where it has numbers), or null.
+static const char *cfg_error(const ctcb_brnn_config *c, char (&buf)[192]) {
+    auto say = [&buf](const char *fmt, auto... args) -> const char * {
+        snprintf(buf, sizeof(buf), fmt, args...);
+        return buf;
+    };
+    if (!c) return "bad config";
+    if (c->maxLabels > CTCB_CTC_MAX_LABELS)     // the CTC kernel's register-resident trellis (ctc.cu)
+        return say("maxLabels %d exceeds the CTC kernel's limit of %d labels per utterance", c->maxLabels,
+                   CTCB_CTC_MAX_LABELS);
+    if ((int64_t)c->maxT * c->maxB > GEMM_MAX_M)     // the forward and delta contractions have maxT*maxB rows
+        return say("maxT * maxB = %lld rows exceed the contractions' limit of %d", (long long)c->maxT * c->maxB,
+                   GEMM_MAX_M);
+    const bool ok = c->inputDim > 0 && c->outputDim > 1 && c->layerSize > 0 && c->numLayers >= 1 && c->numLayers <= 64 &&
+                    c->maxT > 0 && c->maxB > 0 && c->maxLabels >= 0 && c->numTemporal >= 0 &&
+                    // a stacked block must lie inside the hidden layers; k <= 1 keeps the silent "no temporal layer" rule below
+                    !(c->numTemporal > 1 && (c->temporalLayer <= 0 || c->temporalLayer + c->numTemporal - 1 > c->numLayers));
+    if (ok) return nullptr;
+    if (c->numTemporal <= 1) return "bad config";
+    return say("a block of %d temporal layers from layer %d does not fit in hidden layers 1..%d", c->numTemporal,
+               c->temporalLayer, c->numLayers);
+}
 static int valid_cfg(const ctcb_brnn_config *c) {
-    if (!c) return 0;
-    if (c->inputDim <= 0 || c->outputDim <= 1 || c->layerSize <= 0) return 0;
-    if (c->numLayers < 1 || c->numLayers > 64) return 0;
-    if (c->maxT <= 0 || c->maxB <= 0 || c->maxLabels < 0) return 0;
-    if (c->maxLabels > CTCB_CTC_MAX_LABELS) return 0;   // the CTC kernel's register-resident trellis (ctc.cu)
-    if ((int64_t)c->maxT * c->maxB > GEMM_MAX_M) return 0;     // the forward and delta contractions have maxT*maxB rows
-    if (c->numTemporal < 0) return 0;
-    // a stacked block must lie inside the hidden layers; k <= 1 keeps the silent "no temporal layer" rule below
-    if (c->numTemporal > 1 && (c->temporalLayer <= 0 || c->temporalLayer + c->numTemporal - 1 > c->numLayers)) return 0;
-    return 1;
+    char buf[192];
+    return cfg_error(c, buf) == nullptr;
 }
 static int eff_tl(const ctcb_brnn_config *c) {
     return (c->temporalLayer <= 0 || c->temporalLayer > c->numLayers) ? 0 : c->temporalLayer;
@@ -201,10 +208,12 @@ static int eff_nt(const ctcb_brnn_config *c) {
 static int rec_index(const ctcb_brnn_config *c, int j) {
     return 2 * (c->numLayers + 1) + j * (c->unidirectional ? 2 : 4);
 }
-static void layer_sizes(const ctcb_brnn_config *c, int *sizes) {
-    sizes[0] = c->inputDim;
-    for (int i = 1; i <= c->numLayers; ++i) sizes[i] = c->layerSize;
-    sizes[c->numLayers + 1] = c->outputDim;
+// width of layer i of [D, H.., K]
+static int layer_size(const ctcb_brnn_config *c, int i) {
+    return i == 0 ? c->inputDim : (i <= c->numLayers ? c->layerSize : c->outputDim);
+}
+static size_t wider_of_H_K(const ctcb_brnn_config *c) {
+    return (size_t)(c->layerSize > c->outputDim ? c->layerSize : c->outputDim);
 }
 
 extern "C" int ctcb_brnn_num_tensors(const ctcb_brnn_config *cfg) {
@@ -212,109 +221,145 @@ extern "C" int ctcb_brnn_num_tensors(const ctcb_brnn_config *cfg) {
     return 2 * (cfg->numLayers + 1) + eff_nt(cfg) * (cfg->unidirectional ? 2 : 4);
 }
 
-extern "C" int ctcb_brnn_tensor_info(const ctcb_brnn_config *cfg, int idx, int64_t *offset, int32_t *rows, int32_t *cols) {
-    if (!valid_cfg(cfg)) return set_error(CTCB_EINVAL, "ctcb_brnn_tensor_info: bad config");
-    const int nt = ctcb_brnn_num_tensors(cfg);
-    if (idx < 0 || idx >= nt) return set_error(CTCB_EINVAL, "ctcb_brnn_tensor_info: index %d out of range", idx);
-    int sizes[66];
-    layer_sizes(cfg, sizes);
+namespace {
+// The flat parameter (and gradient) vector of a valid config: W and b of every affine map, then per temporal layer its
+// recurrent matrices, each followed by the reference's `dummy` bias (brnnet.py:60-72); every tensor 16-byte aligned.
+struct NetTable {
+    struct Tensor { int64_t off; int32_t rows, cols; };
+    int n;
+    Tensor t[2 * 65 + 4 * 64];
+    int64_t params;
+    // The gradients that a data-parallel step sums over the ranks early, on the side stream next to the BPTT sweep: the
+    // contiguous range from W of the lowest temporal layer to the end of b of layer N+1; empty (at `params`) without a
+    // temporal layer.  Everything before and behind it goes with the statistics tail at the end of the step.
+    int64_t early_lo, early_hi;
+};
+
+void net_table(const ctcb_brnn_config *c, NetTable *nt) {
+    const int nl = c->numLayers + 1;
+    nt->n = ctcb_brnn_num_tensors(c);
     int64_t off = 0;
-    for (int t = 0; t < nt; ++t) {
-        int r, c;
-        const int nl = cfg->numLayers + 1;
+    for (int t = 0; t < nt->n; ++t) {
+        int r, cc;
         if (t < 2 * nl) {
-            const int i = t / 2;
-            if (t % 2 == 0) { r = sizes[i + 1]; c = sizes[i]; }
-            else { r = sizes[i + 1]; c = 1; }
+            r = layer_size(c, t / 2 + 1);
+            cc = (t % 2 == 0) ? layer_size(c, t / 2) : 1;
+        } else if ((t - 2 * nl) % 2 == 0) {
+            r = cc = c->layerSize;
         } else {
-            if ((t - 2 * nl) % 2 == 0) { r = cfg->layerSize; c = cfg->layerSize; }
-            else { r = 1; c = 1; }   // the reference's `dummy` bias (brnnet.py:60-72)
+            r = cc = 1;
         }
-        if (t == idx) {
-            if (offset) *offset = off;
-            if (rows) *rows = r;
-            if (cols) *cols = c;
-            return CTCB_OK;
-        }
-        off += (int64_t)r * c;
+        nt->t[t] = {off, r, cc};
+        off += (int64_t)r * cc;
         off = (off + 3) / 4 * 4;   // keep every tensor 16-byte aligned
     }
-    return CTCB_EINVAL;
+    nt->params = off;
+    nt->early_lo = nt->early_hi = off;
+    if (eff_tl(c)) {
+        nt->early_lo = nt->t[2 * eff_tl(c)].off;
+        nt->early_hi = nt->t[2 * nl - 1].off + c->outputDim;
+    }
+}
+}  // namespace
+
+extern "C" int ctcb_brnn_tensor_info(const ctcb_brnn_config *cfg, int idx, int64_t *offset, int32_t *rows, int32_t *cols) {
+    if (!valid_cfg(cfg)) return set_error(CTCB_EINVAL, "ctcb_brnn_tensor_info: bad config");
+    NetTable nt;
+    net_table(cfg, &nt);
+    if (idx < 0 || idx >= nt.n) return set_error(CTCB_EINVAL, "ctcb_brnn_tensor_info: index %d out of range", idx);
+    if (offset) *offset = nt.t[idx].off;
+    if (rows) *rows = nt.t[idx].rows;
+    if (cols) *cols = nt.t[idx].cols;
+    return CTCB_OK;
 }
 
 extern "C" int64_t ctcb_brnn_param_count(const ctcb_brnn_config *cfg) {
-    const int nt = ctcb_brnn_num_tensors(cfg);
-    if (nt == 0) return 0;
-    int64_t off; int32_t r, c;
-    ctcb_brnn_tensor_info(cfg, nt - 1, &off, &r, &c);
-    return (off + (int64_t)r * c + 3) / 4 * 4;
+    if (!valid_cfg(cfg)) return 0;
+    NetTable nt;
+    net_table(cfg, &nt);
+    return nt.params;
 }
 
+// ---- the two workspace layouts ------------------------------------------------------------------
 namespace {
+// The next 256-byte-aligned area behind `off`.  `extent` receives its aligned size: what a callee that is given the
+// area with a size gets (the contraction planners choose their splits from it).
+size_t take(size_t &off, size_t bytes, size_t *extent = nullptr) {
+    const size_t o = off;
+    off = align_up(off + bytes, 256);
+    if (extent) *extent = off - o;
+    return o;
+}
+// the tail both layouts end with: the sweeps' counters (word 0 the error flag) and their scratch, sized for one plan
+struct SweepWs {
+    size_t counters, scratch, scratch_bytes;
+};
+SweepWs take_sweep_ws(size_t &off, const ctcb_brnn_config *c) {
+    SweepWs s{};
+    s.counters = take(off, sizeof(unsigned int) * 1024);
+    s.scratch_bytes = eff_tl(c) ? sweep_tc_workspace_bytes(c->layerSize, c->maxB) : 0;
+    s.scratch = take(off, s.scratch_bytes);
+    return s;
+}
+
 struct WsLayout {
     size_t X[66];       // X[1..N] activations, X[N+1] logits
-    size_t For, Back, dFor, dBack;
-    // stacked temporal layers: For / Back of temporal layer j (ForJ[0] = For, BackJ[0] = Back) and the second
-    // dFor / dBack pair, which layers of odd j use (0 where not laid out)
-    size_t ForJ[64], BackJ[64], dFor2, dBack2;
+    // For / Back of temporal layer j, and the two dFor / dBack pairs, which consecutive layers alternate (layer j uses
+    // pair j % 2); 0 where not laid out
+    size_t For[64], Back[64], dFor[2], dBack[2];
     size_t D[67];       // D[j]: gradient w.r.t. the output of affine map j (1..N+1)
-    size_t gemm2, colsum2;
-    size_t ctc, gemm, colsum, scratch, counters, sweep, sweep_bytes, lens_dummy;
+    size_t ctc, ctc_bytes;
+    size_t gemm, gemm_bytes, gemm2, gemm2_bytes;     // split-K areas of the main chain and of the side stream
+    size_t colsum, colsum2, l2_scratch;
+    SweepWs sweep;
     size_t total;
 };
 
 WsLayout ws_layout(const ctcb_brnn_config *c) {
     WsLayout w{};
-    int sizes[66];
-    layer_sizes(c, sizes);
     const size_t R = (size_t)c->maxT * c->maxB;
-    const int N = c->numLayers, H = c->layerSize, K = c->outputDim;
+    const int N = c->numLayers, H = c->layerSize, nt = eff_nt(c);
+    const bool uni = (c->unidirectional != 0);
+    const size_t RH = R * H * sizeof(float);
     size_t off = 0;
-    auto take = [&](size_t bytes) { size_t o = off; off = align_up(off + bytes, 256); return o; };
-    for (int i = 1; i <= N + 1; ++i) w.X[i] = take(R * sizes[i] * sizeof(float));
-    if (eff_tl(c)) {
-        w.For = take(R * H * sizeof(float));
-        w.Back = take(R * H * sizeof(float));
-        w.dFor = take(R * H * sizeof(float));
-        w.dBack = take(R * H * sizeof(float));
-        w.ForJ[0] = w.For;
-        w.BackJ[0] = w.Back;
+    for (int i = 1; i <= N + 1; ++i) w.X[i] = take(off, R * layer_size(c, i) * sizeof(float));
+    if (nt) {       // all four for every net with a temporal layer, a uni-directional one too
+        w.For[0] = take(off, RH);
+        w.Back[0] = take(off, RH);
+        w.dFor[0] = take(off, RH);
+        w.dBack[0] = take(off, RH);
     }
     // every further temporal layer keeps its own For (and Back): the BPTT masks and the recurrent weight gradients
     // read them.  The dFor / dBack pairs alternate between consecutive layers, so a stack needs one more pair.
-    const int nt = eff_nt(c);
-    const bool uni = (c->unidirectional != 0);
     for (int j = 1; j < nt; ++j) {
-        w.ForJ[j] = take(R * H * sizeof(float));
-        if (!uni) w.BackJ[j] = take(R * H * sizeof(float));
+        w.For[j] = take(off, RH);
+        if (!uni) w.Back[j] = take(off, RH);
     }
     if (nt > 1) {
-        w.dFor2 = take(R * H * sizeof(float));
-        if (!uni) w.dBack2 = take(R * H * sizeof(float));
+        w.dFor[1] = take(off, RH);
+        if (!uni) w.dBack[1] = take(off, RH);
     }
-    const size_t wide = (size_t)(H > K ? H : K);
-    for (int j = 1; j <= N + 1; ++j) w.D[j] = take(R * wide * sizeof(float));
-    w.ctc = take(ctcb_ctc_workspace_bytes(c->maxB, c->maxT, c->maxLabels));
+    const size_t wide = wider_of_H_K(c);
+    for (int j = 1; j <= N + 1; ++j) w.D[j] = take(off, R * wide * sizeof(float));
+    w.ctc = take(off, ctcb_ctc_workspace_bytes(c->maxB, c->maxT, c->maxLabels), &w.ctc_bytes);
     size_t g = 0;
-    const int Rint = (int)((R > 0x7fffffff) ? 0x7fffffff : R);
+    const int Rint = (int)R;      // a valid config: R <= GEMM_MAX_M
     auto need = [&](int M_, int N_, int K_) { size_t b = ctcb_gemm_workspace_bytes(M_, N_, K_); if (b > g) g = b; };
     for (int i = 0; i <= N; ++i) {
-        need(Rint, sizes[i + 1], sizes[i]);      // forward   X_i . W^T
-        need(Rint, sizes[i], sizes[i + 1]);      // backward  delta . W
-        need(sizes[i + 1], sizes[i], Rint);      // weights   delta^T . X_i
+        need(Rint, layer_size(c, i + 1), layer_size(c, i));      // forward   X_i . W^T
+        need(Rint, layer_size(c, i), layer_size(c, i + 1));      // backward  delta . W
+        need(layer_size(c, i + 1), layer_size(c, i), Rint);      // weights   delta^T . X_i
     }
     {                                            // recurrent weight gradients (a pair for the bi-directional layer)
         const size_t b = ctcb_gemm_pair_workspace_bytes(H, H, Rint);
         if (b > g) g = b;
     }
-    w.gemm = take(g);
-    w.gemm2 = take(g);
-    w.colsum = take(((R + CS_ROWS_MIN - 1) / CS_ROWS_MIN) * wide * sizeof(float));
-    w.colsum2 = take(((R + CS_ROWS_MIN - 1) / CS_ROWS_MIN) * wide * sizeof(float));
-    w.scratch = take(8192);
-    w.counters = take(sizeof(unsigned int) * 1024);
-    w.sweep_bytes = eff_tl(c) ? sweep_tc_workspace_bytes(H, c->maxB) : 0;
-    w.sweep = take(w.sweep_bytes);
+    w.gemm = take(off, g, &w.gemm_bytes);
+    w.gemm2 = take(off, g, &w.gemm2_bytes);
+    w.colsum = take(off, ((R + CS_ROWS_MIN - 1) / CS_ROWS_MIN) * wide * sizeof(float));
+    w.colsum2 = take(off, ((R + CS_ROWS_MIN - 1) / CS_ROWS_MIN) * wide * sizeof(float));
+    w.l2_scratch = take(off, 8192);
+    w.sweep = take_sweep_ws(off, c);
     w.total = off;
     return w;
 }
@@ -323,20 +368,26 @@ WsLayout ws_layout(const ctcb_brnn_config *c) {
 // change with the row count only at multiples of it.
 constexpr int GEMM_ROW_TILE = 128;
 
+// The buffers of a forward-only call: affine map i writes slab i % 2 and reads the other one (or For, the output of
+// the uni-directional temporal layer), so two slabs of the wider of H and K carry the whole stack.  One For (and Back,
+// when bi-directional) serves every temporal layer; 0 where not laid out.
+struct FwdLayout {
+    size_t slab[2];
+    size_t For, Back, gemm, gemm_bytes;
+    SweepWs sweep;      // as in ws_layout: the same sweep plan
+    size_t total;
+};
+
 FwdLayout fwd_layout(const ctcb_brnn_config *c) {
     FwdLayout f{};
-    int sizes[66];
-    layer_sizes(c, sizes);
     const size_t R = (size_t)c->maxT * c->maxB;
-    const int N = c->numLayers, H = c->layerSize, K = c->outputDim;
-    const size_t wide = (size_t)(H > K ? H : K);
+    const int N = c->numLayers, H = c->layerSize;
     size_t off = 0;
-    auto take = [&](size_t bytes) { size_t o = off; off = align_up(off + bytes, 256); return o; };
-    f.slab[0] = take(R * wide * sizeof(float));
-    f.slab[1] = take(R * wide * sizeof(float));
+    f.slab[0] = take(off, R * wider_of_H_K(c) * sizeof(float));
+    f.slab[1] = take(off, R * wider_of_H_K(c) * sizeof(float));
     if (eff_tl(c)) {
-        f.For = take(R * H * sizeof(float));
-        if (!c->unidirectional) f.Back = take(R * H * sizeof(float));
+        f.For = take(off, R * H * sizeof(float));
+        if (!c->unidirectional) f.Back = take(off, R * H * sizeof(float));
     }
     // ctcb_gemm_f32 takes a smaller plan when its area is short of ctcb_gemm_workspace_bytes(R, ..), and that need is
     // not monotone in R = Tmax*B: below one wave of output tiles the tensor-core plan adds split-K partials.  So that a
@@ -345,147 +396,20 @@ FwdLayout fwd_layout(const ctcb_brnn_config *c) {
     // fall back here too).  The need changes with R only at multiples of the row tile and grows with R once
     // num_sms() row tiles are exceeded (the split counts are then fixed), so those multiples and R itself bound it.
     size_t g = 0;
-    const int Rint = (int)((R > 0x7fffffff) ? 0x7fffffff : R);
+    const int Rint = (int)R;
     const int Mtop = (Rint < GEMM_ROW_TILE * num_sms()) ? Rint : GEMM_ROW_TILE * num_sms();
     for (int i = 0; i <= N; ++i) {
         for (int M = GEMM_ROW_TILE; ; M += GEMM_ROW_TILE) {
-            const size_t b = ctcb_gemm_workspace_bytes(M <= Mtop ? M : Rint, sizes[i + 1], sizes[i]);
+            const size_t b = ctcb_gemm_workspace_bytes(M <= Mtop ? M : Rint, layer_size(c, i + 1), layer_size(c, i));
             if (b > g) g = b;
             if (M > Mtop) break;
         }
     }
-    const WsLayout w = ws_layout(c);
-    const size_t train_area = w.gemm2 - w.gemm;
-    f.gemm = take(g < train_area ? g : train_area);
-    f.gemm_bytes = off - f.gemm;
-    f.counters = take(sizeof(unsigned int) * 1024);
-    f.sweep_bytes = eff_tl(c) ? sweep_tc_workspace_bytes(H, c->maxB) : 0;     // as in ws_layout: same sweep plan
-    f.sweep = take(f.sweep_bytes);
+    const size_t train_area = ws_layout(c).gemm_bytes;
+    f.gemm = take(off, g < train_area ? g : train_area, &f.gemm_bytes);
+    f.sweep = take_sweep_ws(off, c);
     f.total = off;
     return f;
-}
-}  // namespace
-
-extern "C" size_t ctcb_brnn_workspace_bytes(const ctcb_brnn_config *cfg) {
-    if (!valid_cfg(cfg)) return 0;
-    return ws_layout(cfg).total;
-}
-
-extern "C" size_t ctcb_brnn_forward_workspace_bytes(const ctcb_brnn_config *cfg, size_t *error_flag_offset) {
-    if (!valid_cfg(cfg)) return 0;
-    const FwdLayout f = fwd_layout(cfg);
-    if (error_flag_offset) *error_flag_offset = f.counters;
-    return f.total;
-}
-
-extern "C" size_t ctcb_brnn_error_flag_offset(const ctcb_brnn_config *cfg) {
-    if (!valid_cfg(cfg)) return 0;
-    return ws_layout(cfg).counters;
-}
-
-extern "C" int ctcb_brnn_create(const ctcb_brnn_config *cfg, ctcb_brnn **out) {
-    if (cfg && cfg->maxLabels > CTCB_CTC_MAX_LABELS)
-        return set_error(CTCB_EINVAL, "ctcb_brnn_create: maxLabels %d exceeds the CTC kernel's limit of %d labels per utterance",
-                         cfg->maxLabels, CTCB_CTC_MAX_LABELS);
-    if (cfg && (int64_t)cfg->maxT * cfg->maxB > GEMM_MAX_M)
-        return set_error(CTCB_EINVAL, "ctcb_brnn_create: maxT * maxB = %lld rows exceed the contractions' limit of %d",
-                         (long long)cfg->maxT * cfg->maxB, GEMM_MAX_M);
-    if (cfg && cfg->numTemporal > 1 && !valid_cfg(cfg))
-        return set_error(CTCB_EINVAL, "ctcb_brnn_create: a block of %d temporal layers from layer %d does not fit in "
-                         "hidden layers 1..%d", cfg->numTemporal, cfg->temporalLayer, cfg->numLayers);
-    if (!valid_cfg(cfg) || !out) return set_error(CTCB_EINVAL, "ctcb_brnn_create: bad config");
-    ctcb_brnn *h = new (std::nothrow) ctcb_brnn;
-    if (!h) return set_error(CTCB_ENOMEM, "ctcb_brnn_create: out of host memory");
-    h->cfg = *cfg;
-    if (h->cfg.maxAct <= 0.f) h->cfg.maxAct = 20.0f;   // brnnet.py:32
-    h->nlayers = cfg->numLayers + 1;
-    h->tl = eff_tl(cfg);
-    h->nt = eff_nt(cfg);
-    layer_sizes(cfg, h->sizes);
-    h->side = nullptr;
-    h->side_ready = false;
-    h->defer_l2 = false;
-    h->comm = nullptr;
-    h->fwd_ready = false;
-    h->drop_p = 0.f;
-    h->drop_seed = 0;
-    h->drop_step = nullptr;
-    h->drop_thr = 0;
-    h->drop_scale = 1.f;
-    h->drop_first = 0;
-    h->drop_stride = 1;
-    *out = h;
-    return CTCB_OK;
-}
-
-extern "C" void ctcb_brnn_destroy(ctcb_brnn *h) {
-    if (h && h->side_ready) {
-        cudaStreamDestroy(h->side);
-        cudaStreamDestroy(h->hi);
-        cudaEventDestroy(h->ev_fork);
-        cudaEventDestroy(h->ev_hi);
-        for (int i = 0; i < 66; ++i) cudaEventDestroy(h->ev_delta[i]);
-        cudaEventDestroy(h->ev_side);
-        for (int p = 0; p < 2; ++p) cudaEventDestroy(h->ev_pair[p]);
-    }
-    delete h;
-}
-
-static int ensure_side_stream(ctcb_brnn *h) {
-    if (h->side_ready) return CTCB_OK;
-    // the lowest priority: the side stream's CTAs never take an SM that a pending sweep cluster could use
-    CTCB_CUDA_CHECK(cudaStreamCreateWithPriority(&h->side, cudaStreamNonBlocking, stream_priority_least()));
-    for (int i = 0; i < 66; ++i) CTCB_CUDA_CHECK(cudaEventCreateWithFlags(&h->ev_delta[i], cudaEventDisableTiming));
-    CTCB_CUDA_CHECK(cudaStreamCreateWithPriority(&h->hi, cudaStreamNonBlocking, stream_priority_greatest()));
-    CTCB_CUDA_CHECK(cudaEventCreateWithFlags(&h->ev_side, cudaEventDisableTiming));
-    CTCB_CUDA_CHECK(cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming));
-    CTCB_CUDA_CHECK(cudaEventCreateWithFlags(&h->ev_hi, cudaEventDisableTiming));
-    for (int p = 0; p < 2; ++p) CTCB_CUDA_CHECK(cudaEventCreateWithFlags(&h->ev_pair[p], cudaEventDisableTiming));
-    h->side_ready = true;
-    return CTCB_OK;
-}
-
-#define TRY(expr)                    \
-    do {                             \
-        int _rc = (expr);            \
-        if (_rc != CTCB_OK) return _rc; \
-    } while (0)
-
-extern "C" int ctcb_brnn_sweep_f32(int mode, int T, int B, int H, const int32_t *T_per_utt, const float *pre,
-                                   const float *Wf, const float *Wb, float *outF, float *outB, const float *actF,
-                                   const float *actB, float maxAct, void *scratch, size_t scratch_bytes, void *stream) {
-    if (!T_per_utt || !pre || !Wf || !outF || !scratch || (mode == 1 && !actF) ||
-        (Wb && (!outB || (mode == 1 && !actB))))
-        return set_error(CTCB_EINVAL, "ctcb_brnn_sweep_f32: null pointer argument");
-    if (T <= 0 || B <= 0 || H <= 0 || (mode != 0 && mode != 1))
-        return set_error(CTCB_EINVAL, "ctcb_brnn_sweep_f32: bad sizes");
-    CTCB_CUDA_CHECK(cudaMemsetAsync(scratch, 0, 16 * sizeof(unsigned int), (cudaStream_t)stream));   // error flag
-    if (scratch_bytes < 4096) return set_error(CTCB_ENOMEM, "ctcb_brnn_sweep_f32: scratch %zu < 4096 bytes", scratch_bytes);
-    return run_sweep(mode, T, B, H, T_per_utt, pre, Wf, Wb, outF, outB, actF, actB, maxAct,
-                     (unsigned int *)scratch, (char *)scratch + 4096, scratch_bytes - 4096, (cudaStream_t)stream);
-}
-
-// The part of the flat gradient that was NOT summed early on the side stream, plus the statistics tail, in one grouped
-// NCCL launch: with an early bucket [off(2 tl), end of layer N+1), tl the lowest temporal layer, that is everything
-// before it and everything behind it (the recurrent matrices of every temporal layer among them).
-static int brnn_reduce_rest(ctcb_brnn *h, float *grads, float *stats, bool early_bucket, cudaStream_t st) {
-    const ctcb_brnn_config &c = h->cfg;
-    const int64_t P = ctcb_brnn_param_count(&c);
-    float *ptrs[3];
-    int64_t cnt[3];
-    int k = 0;
-    int64_t lo = P, hi = P;      // [lo, hi) was reduced early
-    if (early_bucket) {
-        int64_t o; int32_t r, cc;
-        ctcb_brnn_tensor_info(&c, 2 * h->tl, &lo, nullptr, nullptr);
-        ctcb_brnn_tensor_info(&c, 2 * c.numLayers + 1, &o, &r, &cc);
-        hi = o + (int64_t)r * cc;
-    }
-    ptrs[k] = grads; cnt[k] = lo; ++k;
-    const bool tail_adjacent = (stats == grads + P);
-    ptrs[k] = grads + hi; cnt[k] = P - hi + (stats && tail_adjacent ? 4 : 0); ++k;
-    if (stats && !tail_adjacent) { ptrs[k] = stats; cnt[k] = 4; ++k; }
-    return comm_allreduce_ranges(h->comm, ptrs, cnt, k, st);
 }
 
 // Where the forward half reads and writes: X[i] (1..N+1) the output of affine map i (pre-activation, then For+Back,
@@ -501,6 +425,176 @@ struct FwdBufs {
     size_t sweep_bytes;
 };
 
+void fwd_bufs(const FwdLayout &f, int N, int nt, char *ws, FwdBufs *m) {
+    for (int i = 1; i <= N + 1; ++i) m->X[i] = (float *)(ws + f.slab[i % 2]);
+    for (int j = 0; j < nt; ++j) {     // one pair for every temporal layer: each sweep runs after the last read
+        m->For[j] = f.For ? (float *)(ws + f.For) : nullptr;   // offset 0 is slab 0: For / Back were not laid out
+        m->Back[j] = f.Back ? (float *)(ws + f.Back) : nullptr;
+    }
+    m->gemm = ws + f.gemm;
+    m->gemm_bytes = f.gemm_bytes;
+    m->counters = (unsigned int *)(ws + f.sweep.counters);
+    m->sweep = ws + f.sweep.scratch;
+    m->sweep_bytes = f.sweep.scratch_bytes;
+}
+void train_bufs(const WsLayout &w, int N, int nt, char *ws, FwdBufs *m) {
+    for (int i = 1; i <= N + 1; ++i) m->X[i] = (float *)(ws + w.X[i]);
+    for (int j = 0; j < nt; ++j) {
+        m->For[j] = (float *)(ws + w.For[j]);
+        m->Back[j] = (float *)(ws + w.Back[j]);      // unused (offset 0) for the uni-directional layers above the first
+    }
+    m->gemm = ws + w.gemm;
+    m->gemm_bytes = w.gemm_bytes;
+    m->counters = (unsigned int *)(ws + w.sweep.counters);
+    m->sweep = ws + w.sweep.scratch;
+    m->sweep_bytes = w.sweep.scratch_bytes;
+}
+}  // namespace
+
+struct ctcb_brnn {
+    ctcb_brnn_config cfg;
+    int tl = 0;         // lowest temporal layer or 0
+    int nt = 0;         // temporal layers tl .. tl+nt-1 (0 without)
+    NetTable net;
+    // weight/bias gradients of the layers at and above the temporal layer depend only on their delta, so they
+    // run on a side stream next to the (latency-bound, 112-SM) BPTT sweep; created on first use
+    cudaStream_t side = nullptr;
+    // the main chain of a training call (forward, CTC, delta contractions, sweeps, the tail below the temporal layer)
+    // runs on `hi`, forked from the caller's stream and joined back into it: the greatest priority, so its kernels take
+    // SMs ahead of the side stream's pending CTAs (the recurrent weight-gradient pair in particular)
+    cudaStream_t hi = nullptr;
+    // ev_delta[i], temporal layers i only: the deltas of the maps from the last sweep's down to i are complete.
+    // ev_sweep: the BPTT sweep of the current temporal layer is queued.
+    cudaEvent_t ev_delta[66] = {}, ev_sweep = nullptr;
+    cudaEvent_t ev_side = nullptr, ev_fork = nullptr, ev_hi = nullptr;
+    // the two dFor/dBack pairs that stacked temporal layers alternate: ev_pair[p] is recorded on the side stream after
+    // its last read of pair p, and the BPTT sweep that writes pair p next waits for it
+    cudaEvent_t ev_pair[2] = {};
+    bool side_ready = false;
+    // data-parallel callers sum the gradient over ranks first and add reg*W ONCE afterwards (ctcb_brnn_apply_l2_f32);
+    // the L2 cost is still reported by every call
+    bool defer_l2 = false;
+    // data-parallel exchange inside the step (ctcb_brnn_set_comm): the gradients of the layers at and above the temporal
+    // layer are summed over ranks on the side stream WHILE the BPTT sweep runs, the rest (+ statistics tail) at the end
+    ctcb_comm *comm = nullptr;
+    // the forward layout, computed on the first forward-only call (its GEMM area takes a few hundred size queries)
+    bool fwd_ready = false;
+    FwdLayout fwd;
+    // inverted dropout of the ReLU hidden layers in training calls (ctcb_brnn_set_dropout); drop_p == 0: off
+    float drop_p = 0.f;
+    uint64_t drop_seed = 0;
+    const int64_t *drop_step = nullptr;     // the caller's device counter
+    uint32_t drop_thr = 0;                  // keep iff Philox output >= drop_thr
+    float drop_scale = 1.f;                 // 1 / (1 - p), rounded once; also the delta contraction's alpha
+    int64_t drop_first = 0, drop_stride = 1;
+
+    bool uni() const { return cfg.unidirectional != 0; }
+    bool temporal(int i) const { return nt > 0 && i >= tl && i < tl + nt; }
+    int size(int i) const { return layer_size(&cfg, i); }
+    int rec(int j) const { return rec_index(&cfg, j); }
+    template <typename T> T *tensor(T *flat, int idx) const { return flat + net.t[idx].off; }
+    // activations of layer i as the next layer (and the weight gradients) see them: a uni-directional temporal
+    // layer's output IS its forward sweep (rnnet.py:112-116), a bi-directional one's is For + Back
+    float *act(const FwdBufs &m, int i) const { return (uni() && temporal(i)) ? m.For[i - tl] : m.X[i]; }
+};
+
+extern "C" size_t ctcb_brnn_workspace_bytes(const ctcb_brnn_config *cfg) {
+    if (!valid_cfg(cfg)) return 0;
+    return ws_layout(cfg).total;
+}
+
+extern "C" size_t ctcb_brnn_forward_workspace_bytes(const ctcb_brnn_config *cfg, size_t *error_flag_offset) {
+    if (!valid_cfg(cfg)) return 0;
+    const FwdLayout f = fwd_layout(cfg);
+    if (error_flag_offset) *error_flag_offset = f.sweep.counters;
+    return f.total;
+}
+
+extern "C" size_t ctcb_brnn_error_flag_offset(const ctcb_brnn_config *cfg) {
+    if (!valid_cfg(cfg)) return 0;
+    return ws_layout(cfg).sweep.counters;
+}
+
+extern "C" int ctcb_brnn_create(const ctcb_brnn_config *cfg, ctcb_brnn **out) {
+    char buf[192];
+    if (const char *why = cfg_error(cfg, buf)) return set_error(CTCB_EINVAL, "ctcb_brnn_create: %s", why);
+    if (!out) return set_error(CTCB_EINVAL, "ctcb_brnn_create: bad config");
+    ctcb_brnn *h = new (std::nothrow) ctcb_brnn;
+    if (!h) return set_error(CTCB_ENOMEM, "ctcb_brnn_create: out of host memory");
+    h->cfg = *cfg;
+    if (h->cfg.maxAct <= 0.f) h->cfg.maxAct = 20.0f;   // brnnet.py:32
+    h->tl = eff_tl(cfg);
+    h->nt = eff_nt(cfg);
+    net_table(cfg, &h->net);
+    *out = h;
+    return CTCB_OK;
+}
+
+extern "C" void ctcb_brnn_destroy(ctcb_brnn *h) {
+    if (h && h->side_ready) {
+        cudaStreamDestroy(h->side);
+        cudaStreamDestroy(h->hi);
+        cudaEventDestroy(h->ev_fork);
+        cudaEventDestroy(h->ev_hi);
+        for (int i = h->tl; i < h->tl + h->nt; ++i) cudaEventDestroy(h->ev_delta[i]);
+        cudaEventDestroy(h->ev_sweep);
+        cudaEventDestroy(h->ev_side);
+        for (int p = 0; p < 2; ++p) cudaEventDestroy(h->ev_pair[p]);
+    }
+    delete h;
+}
+
+static int ensure_side_stream(ctcb_brnn *h) {
+    if (h->side_ready) return CTCB_OK;
+    // the lowest priority: the side stream's CTAs never take an SM that a pending sweep cluster could use
+    CTCB_CUDA_CHECK(cudaStreamCreateWithPriority(&h->side, cudaStreamNonBlocking, stream_priority_least()));
+    for (int i = h->tl; i < h->tl + h->nt; ++i)
+        CTCB_CUDA_CHECK(cudaEventCreateWithFlags(&h->ev_delta[i], cudaEventDisableTiming));
+    CTCB_CUDA_CHECK(cudaEventCreateWithFlags(&h->ev_sweep, cudaEventDisableTiming));
+    CTCB_CUDA_CHECK(cudaStreamCreateWithPriority(&h->hi, cudaStreamNonBlocking, stream_priority_greatest()));
+    CTCB_CUDA_CHECK(cudaEventCreateWithFlags(&h->ev_side, cudaEventDisableTiming));
+    CTCB_CUDA_CHECK(cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming));
+    CTCB_CUDA_CHECK(cudaEventCreateWithFlags(&h->ev_hi, cudaEventDisableTiming));
+    for (int p = 0; p < 2; ++p) CTCB_CUDA_CHECK(cudaEventCreateWithFlags(&h->ev_pair[p], cudaEventDisableTiming));
+    h->side_ready = true;
+    return CTCB_OK;
+}
+
+extern "C" int ctcb_brnn_sweep_f32(int mode, int T, int B, int H, const int32_t *T_per_utt, const float *pre,
+                                   const float *Wf, const float *Wb, float *outF, float *outB, const float *actF,
+                                   const float *actB, float maxAct, void *scratch, size_t scratch_bytes, void *stream) {
+    if (!T_per_utt || !pre || !Wf || !outF || !scratch || (mode == 1 && !actF) ||
+        (Wb && (!outB || (mode == 1 && !actB))))
+        return set_error(CTCB_EINVAL, "ctcb_brnn_sweep_f32: null pointer argument");
+    if (T <= 0 || B <= 0 || H <= 0 || (mode != 0 && mode != 1))
+        return set_error(CTCB_EINVAL, "ctcb_brnn_sweep_f32: bad sizes");
+    CTCB_CUDA_CHECK(cudaMemsetAsync(scratch, 0, 16 * sizeof(unsigned int), (cudaStream_t)stream));   // error flag
+    if (scratch_bytes < 4096) return set_error(CTCB_ENOMEM, "ctcb_brnn_sweep_f32: scratch %zu < 4096 bytes", scratch_bytes);
+    return run_sweep(mode, T, B, H, T_per_utt, pre, Wf, Wb, outF, outB, actF, actB, maxAct,
+                     (unsigned int *)scratch, (char *)scratch + 4096, scratch_bytes - 4096, (cudaStream_t)stream);
+}
+
+// ---- the data-parallel exchange: the early range of the net table, then everything else --------------------
+static int brnn_reduce_early(ctcb_brnn *h, float *grads, cudaStream_t st) {
+    float *pa = grads + h->net.early_lo;
+    const int64_t na = h->net.early_hi - h->net.early_lo;
+    return comm_allreduce_ranges(h->comm, &pa, &na, 1, st);
+}
+
+// The part of the flat gradient that was NOT summed early, plus the statistics tail, in one grouped NCCL launch.
+static int brnn_reduce_rest(ctcb_brnn *h, float *grads, float *stats, cudaStream_t st) {
+    const int64_t P = h->net.params, lo = h->net.early_lo, hi = h->net.early_hi;
+    float *ptrs[3];
+    int64_t cnt[3];
+    int k = 0;
+    ptrs[k] = grads; cnt[k] = lo; ++k;
+    const bool tail_adjacent = (stats == grads + P);
+    ptrs[k] = grads + hi; cnt[k] = P - hi + (stats && tail_adjacent ? 4 : 0); ++k;
+    if (stats && !tail_adjacent) { ptrs[k] = stats; cnt[k] = 4; ++k; }
+    return comm_allreduce_ranges(h->comm, ptrs, cnt, k, st);
+}
+
+// ---- the step -----------------------------------------------------------------------------------
 // brnnet.py:136-173: the affine maps with bias(+ReLU) fused, the two-direction sweep and For+Back at each temporal
 // layer, the softmax into probs_out when given.  Clears the sweep error flag first.  drop: a training call with dropout
 // on masks the output of every ReLU hidden layer in place right behind its contraction, so the next layer, the weight
@@ -508,37 +602,32 @@ struct FwdBufs {
 static int brnn_forward(ctcb_brnn *h, const float *feats, const int32_t *T_per_utt, int B, int Tmax,
                         const float *params, float *probs_out, const FwdBufs &m, bool drop, cudaStream_t st) {
     const ctcb_brnn_config &c = h->cfg;
-    const int N = c.numLayers, H = c.layerSize, K = c.outputDim, tl = h->tl, nt = h->nt;
-    const int *sz = h->sizes;
+    const int N = c.numLayers, H = c.layerSize, K = c.outputDim;
     const int64_t R = (int64_t)Tmax * B;
-    auto P = [&](int idx) -> const float * {
-        int64_t off; ctcb_brnn_tensor_info(&c, idx, &off, nullptr, nullptr); return params + off;
-    };
-    const bool uni = (c.unidirectional != 0);
-    auto temporal = [&](int i) { return nt > 0 && i >= tl && i < tl + nt; };
-    // the uni-directional temporal layer's output IS the forward sweep (rnnet.py:112-116)
-    auto Act = [&](int i) -> const float * { return (uni && temporal(i)) ? m.For[i - tl] : m.X[i]; };
+    const bool uni = h->uni();
     // the sweep kernels' error flag (word 0) is cleared once per call, so a forward-sweep timeout survives the BPTT sweep
     CTCB_CUDA_CHECK(cudaMemsetAsync(m.counters, 0, 16 * sizeof(unsigned int), st));
     for (int i = 1; i <= N + 1; ++i) {
-        const float *in = (i == 1) ? feats : Act(i - 1);
-        const int relu = (i <= N && !temporal(i)) ? 1 : 0;
+        const float *in = (i == 1) ? feats : h->act(m, i - 1);
+        const int relu = (i <= N && !h->temporal(i)) ? 1 : 0;
+        const int n_out = h->size(i), n_in = h->size(i - 1);
         {
         ProfScope ps("gemm_fwd", st);
-        TRY(ctcb_gemm_f32(0, 1, (int)R, sz[i], sz[i - 1], 1.f, in, sz[i - 1], P(2 * (i - 1)), sz[i - 1], 0.f,
-                          m.X[i], sz[i], P(2 * (i - 1) + 1), relu, nullptr, m.gemm, m.gemm_bytes, st));
+        TRY(ctcb_gemm_f32(0, 1, (int)R, n_out, n_in, 1.f, in, n_in, h->tensor(params, 2 * (i - 1)), n_in, 0.f, m.X[i],
+                          n_out, h->tensor(params, 2 * (i - 1) + 1), relu, nullptr, m.gemm, m.gemm_bytes, st));
         }
         if (drop && relu) {
             ProfScope ps("dropout", st);
-            TRY(run_dropout(m.X[i], R, B, sz[i], i, h->drop_seed, h->drop_step, h->drop_first, h->drop_stride,
+            TRY(run_dropout(m.X[i], R, B, n_out, i, h->drop_seed, h->drop_step, h->drop_first, h->drop_stride,
                             h->drop_thr, h->drop_scale, st));
         }
-        if (temporal(i)) {
-            const int j = i - tl, iWtf = rec_index(&c, j);
+        if (h->temporal(i)) {
+            const int j = i - h->tl, iWtf = h->rec(j);
             {
             ProfScope ps("sweep_fwd", st);
-            TRY(run_sweep(0, Tmax, B, H, T_per_utt, m.X[i], P(iWtf), uni ? nullptr : P(iWtf + 2), m.For[j], m.Back[j],
-                          nullptr, nullptr, c.maxAct, m.counters, m.sweep, m.sweep_bytes, st));
+            TRY(run_sweep(0, Tmax, B, H, T_per_utt, m.X[i], h->tensor(params, iWtf),
+                          uni ? nullptr : h->tensor(params, iWtf + 2), m.For[j], m.Back[j], nullptr, nullptr, c.maxAct,
+                          m.counters, m.sweep, m.sweep_bytes, st));
             }
             if (!uni) {     // over the pre-activation, which nothing reads after the sweep
                 ProfScope ps("elementwise", st);
@@ -551,6 +640,162 @@ static int brnn_forward(ctcb_brnn *h, const float *feats, const int32_t *T_per_u
         softmax_rows_kernel<<<(unsigned)((R + wpb - 1) / wpb), wpb * 32, 0, st>>>(m.X[N + 1], probs_out, R, K);
         CTCB_LAUNCH_CHECK();
     }
+    return CTCB_OK;
+}
+
+namespace {
+// What the stages of one training call share: the handle, the forward half's buffers `m`, the layout `w` of the
+// workspace `ws` for what only the backward half uses, the call's arguments.  `main` carries the forward pass, the
+// CTC, the delta chain and the sweeps, `side` the weight gradients of the layers at and above the lowest temporal
+// layer; `caller` is the stream the call was given, which `main` is forked from and both are joined into.  Without a
+// temporal layer main == caller and there is no side stream.
+struct Step {
+    ctcb_brnn *h;
+    const FwdBufs &m;
+    const WsLayout &w;
+    char *ws;
+    const float *feats, *params;
+    const int32_t *T_per_utt;
+    float *grads;
+    int B, Tmax;
+    int64_t R;
+    bool first, last;       // CTCB_PART_FIRST: overwrite the gradients, else add to them; CTCB_PART_LAST: exchange and L2
+    bool drop, dp;
+    cudaStream_t main, side, caller;
+
+    float *buf(size_t off) const { return (float *)(ws + off); }
+    const float *P(int idx) const { return h->tensor(params, idx); }
+    float *G(int idx) const { return h->tensor(grads, idx); }
+    float beta_g() const { return first ? 0.f : 1.f; }      // weight-gradient contractions: C = dW (+ C)
+    // the delta of map i; rnnet.py:162-177: the BPTT result of a uni-directional layer is the delta
+    float *delta(int i) const {
+        return buf((h->uni() && h->temporal(i + 1)) ? w.dFor[(i + 1 - h->tl) % 2] : w.D[i + 1]);
+    }
+    int weight_grads(int i, bool on_side) const;
+    int rec_weight_grads(int j) const;
+    int backward() const;
+    int finish(float *stats, float *regcost_out) const;
+};
+}  // namespace
+
+// the weight and bias gradients of map i, on the side stream or in the main chain, where its delta is complete
+int Step::weight_grads(int i, bool on_side) const {
+    const cudaStream_t st = on_side ? side : main;
+    const float *Xi = (i == 0) ? feats : h->act(m, i);
+    const int n_out = h->size(i + 1), n_in = h->size(i);
+    // dW = delta^T . X_i   (brnnet.py:196)
+    {
+    ProfScope ps("gemm_dw", st);
+    TRY(ctcb_gemm_f32(1, 0, n_out, n_in, (int)R, 1.f, delta(i), n_out, Xi, n_in, beta_g(), G(2 * i), n_in, nullptr, 0,
+                      nullptr, on_side ? ws + w.gemm2 : m.gemm, on_side ? w.gemm2_bytes : m.gemm_bytes, st));
+    }
+    // db = row sums of delta   (brnnet.py:200)
+    {
+    ProfScope ps("colsum", st);
+    TRY(run_colsum(delta(i), R, n_out, buf(on_side ? w.colsum2 : w.colsum), G(2 * i + 1), !first, st));
+    }
+    if (h->uni() && h->temporal(i + 1) && i + 1 - h->tl >= 2)     // the last read of the pair of uni-directional layer i + 1
+        CTCB_CUDA_CHECK(cudaEventRecord(h->ev_pair[(i + 1 - h->tl) % 2], side));
+    // every gradient tensor of the layers >= tl is now queued on the side stream: sum that contiguous range over
+    // the ranks there, next to the BPTT sweep on the main stream
+    if (dp && last && on_side && i == h->tl) TRY(brnn_reduce_early(h, grads, side));
+    return CTCB_OK;
+}
+
+// The recurrent weight gradients of temporal layer j (brnnet.py:227-230), behind its BPTT sweep: independent of the
+// rest of the backward pass, so they go to the side stream as well.
+int Step::rec_weight_grads(int j) const {
+    const int H = h->cfg.layerSize, iWtf = h->rec(j), iWtb = iWtf + 2;
+    float *dFor = buf(w.dFor[j % 2]), *dBack = buf(w.dBack[j % 2]);
+    CTCB_CUDA_CHECK(cudaEventRecord(h->ev_sweep, main));
+    CTCB_CUDA_CHECK(cudaStreamWaitEvent(side, h->ev_sweep, 0));
+    ProfScope ps("gemm_dw_rec", side);
+    if (Tmax > 1) {
+        const int64_t Rm = R - B;
+        if (h->uni())
+            TRY(ctcb_gemm_f32(1, 0, H, H, (int)Rm, 1.f, dFor + (int64_t)B * H, H, m.For[j], H, beta_g(), G(iWtf), H,
+                              nullptr, 0, nullptr, ws + w.gemm2, w.gemm2_bytes, side));
+        else     // both directions in one launch
+            TRY(ctcb_gemm_pair_f32(1, 0, H, H, (int)Rm, 1.f, dFor + (int64_t)B * H, dBack, H, m.For[j],
+                                   m.Back[j] + (int64_t)B * H, H, beta_g(), G(iWtf), G(iWtb), H, ws + w.gemm2,
+                                   w.gemm2_bytes, side));
+    } else if (first) {     // one frame: no recurrence, nothing to add to earlier micro-batches
+        CTCB_CUDA_CHECK(cudaMemsetAsync(G(iWtf), 0, sizeof(float) * H * H, side));
+        if (!h->uni()) CTCB_CUDA_CHECK(cudaMemsetAsync(G(iWtb), 0, sizeof(float) * H * H, side));
+    }
+    return CTCB_OK;
+}
+
+// brnnet.py:188-243.  Per temporal layer from the top: the delta GEMM without a mask, the BPTT sweep into pair j % 2,
+// then on the side stream the weight gradients of the maps from the last sweep's down to this layer and the recurrent
+// weight-gradient pair, add2.  The side stream's weight gradients become ready together with the sweep, not before
+// it: the sweep's clusters (the higher priority) take their SMs first and the GEMMs run on the rest for the length
+// of the sweep, instead of holding SMs the sweep then waits for.  Layer j - 2 writes the pair layer j used: its
+// sweep waits for ev_pair, recorded on the side stream behind the last read of that pair (the recurrent weight
+// gradients; for a uni-directional layer the weight gradient of the map above, whose delta the pair is).
+int Step::backward() const {
+    const int N = h->cfg.numLayers, H = h->cfg.layerSize, tl = h->tl, nt = h->nt;
+    const bool uni = h->uni();
+    int side_top = N;      // the highest map >= tl whose weight gradients are not queued yet
+    for (int i = N; i >= 0; --i) {
+        // layers i >= tl > 0: dW/db on the side stream, delta chain + BPTT on the main one
+        if (!(tl > 0 && i >= tl)) TRY(weight_grads(i, false));
+        if (i == 0) break;
+        const int n_out = h->size(i + 1), n_in = h->size(i);
+        float *doth = buf(w.D[i]);
+        // delta <- delta . W, with the ReLU mask sign(hActs[i]) fused (brnnet.py:203-204,235-237).  A dropped
+        // layer's X_i is 0 at every dropped unit, so the same mask removes those; the kept ones were scaled by
+        // drop_scale in the forward pass, and so is their delta, through alpha.
+        const float *mask = h->temporal(i) ? nullptr : h->act(m, i);
+        const float alpha = (drop && !h->temporal(i)) ? h->drop_scale : 1.f;
+        {
+        ProfScope ps("gemm_delta", main);
+        TRY(ctcb_gemm_f32(0, 0, (int)R, n_in, n_out, alpha, delta(i), n_out, P(2 * i), n_in, 0.f, doth, n_in, nullptr, 0,
+                          mask, m.gemm, m.gemm_bytes, main));
+        }
+        if (!h->temporal(i)) continue;
+        // brnnet.py:207-233
+        const int j = i - tl, p = j % 2, iWtf = h->rec(j);
+        if (j + 2 < nt)      // layer j + 2 used this pair
+            CTCB_CUDA_CHECK(cudaStreamWaitEvent(main, h->ev_pair[p], 0));
+        // the deltas of maps side_top..i are complete here
+        CTCB_CUDA_CHECK(cudaEventRecord(h->ev_delta[i], main));
+        {
+        ProfScope ps("sweep_bptt", main);
+        TRY(run_sweep(1, Tmax, B, H, T_per_utt, doth, P(iWtf), uni ? nullptr : P(iWtf + 2), buf(w.dFor[p]),
+                      buf(w.dBack[p]), m.For[j], m.Back[j], h->cfg.maxAct, m.counters, m.sweep, m.sweep_bytes, main));
+        }
+        CTCB_CUDA_CHECK(cudaStreamWaitEvent(side, h->ev_delta[i], 0));
+        for (; side_top >= i; --side_top) TRY(weight_grads(side_top, true));
+        TRY(rec_weight_grads(j));
+        if (!uni) {
+            if (j >= 2) CTCB_CUDA_CHECK(cudaEventRecord(h->ev_pair[p], side));
+            TRY(run_add2(buf(w.dFor[p]), buf(w.dBack[p]), doth, R * H, main));
+        }
+    }
+    // the main stream's tail writes nothing the side stream touches, so it runs next to the recurrent weight gradients
+    for (int j = 0; j < nt; ++j) {   // the `dummy` biases never receive gradient
+        CTCB_CUDA_CHECK(cudaMemsetAsync(G(h->rec(j) + 1), 0, sizeof(float), main));
+        if (!uni) CTCB_CUDA_CHECK(cudaMemsetAsync(G(h->rec(j) + 3), 0, sizeof(float), main));
+    }
+    return CTCB_OK;
+}
+
+// What only the last micro-batch of a step does, on the caller's stream behind the join: the rest of the exchange and
+// the L2 term (brnnet.py:177-183,197-198,244-247).
+int Step::finish(float *stats, float *regcost_out) const {
+    const float reg = h->cfg.reg;
+    if (dp) TRY(brnn_reduce_rest(h, grads, stats, caller));
+    if (regcost_out) {
+        set_scalar_kernel<<<1, 1, 0, caller>>>(regcost_out, 0.f);
+        CTCB_LAUNCH_CHECK();
+    }
+    if (!h->defer_l2) TRY(ctcb_brnn_apply_l2_f32(h, params, grads, caller));
+    if (regcost_out && reg > 0.f)
+        for (int idx = 0; idx < h->net.n; idx += 2) {     // the same weight matrices
+            const NetTable::Tensor &t = h->net.t[idx];
+            TRY(run_sumsq(params + t.off, (int64_t)t.rows * t.cols, regcost_out, 0.5f * reg, 1, ws + w.l2_scratch, caller));
+        }
     return CTCB_OK;
 }
 
@@ -568,7 +813,6 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
     if (flags & ~(CTCB_PART_FIRST | CTCB_PART_LAST))
         return set_error(CTCB_EINVAL, "ctcb_brnn_cost_and_grad_part: unknown flags 0x%x", flags);
     const bool first = (flags & CTCB_PART_FIRST) != 0, last = (flags & CTCB_PART_LAST) != 0;
-    const float beta_g = first ? 0.f : 1.f;      // weight-gradient contractions: C = dW (+ C)
     const ctcb_brnn_config &c = h->cfg;
     if (B <= 0 || B > c.maxB || Tmax <= 0 || Tmax > c.maxT)
         return set_error(CTCB_EINVAL, "ctcb_brnn_cost_and_grad: batch %d x %d frames exceeds the configured %d x %d",
@@ -578,250 +822,56 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
         return set_error(CTCB_EINVAL, "ctcb_brnn_cost_and_grad: training mode needs labels and cost/skip outputs");
     if (!train && !probs_out)
         return set_error(CTCB_EINVAL, "ctcb_brnn_cost_and_grad: forward-only mode needs probs_out");
-    cudaStream_t st = (cudaStream_t)stream;
+    const cudaStream_t caller = (cudaStream_t)stream;
     char *ws = (char *)workspace;
-    const int N = c.numLayers, H = c.layerSize, K = c.outputDim, tl = h->tl;
-    const int *sz = h->sizes;
+    const int N = c.numLayers, K = c.outputDim;
     const int64_t R = (int64_t)Tmax * B;
     if (R > 0x7fffffff) return set_error(CTCB_EINVAL, "ctcb_brnn_cost_and_grad: T*B too large");
-    FwdBufs m{};
     if (!train) {     // the forward layout whatever the size given: the same kernels and plans as a training call
         if (!h->fwd_ready) {
             h->fwd = fwd_layout(&c);
             h->fwd_ready = true;
         }
-        const FwdLayout &f = h->fwd;
-        if (!workspace || ws_bytes < f.total)
-            return set_error(CTCB_ENOMEM, "ctcb_brnn_cost_and_grad: workspace %zu < %zu bytes", ws_bytes, f.total);
-        for (int i = 1; i <= N + 1; ++i) m.X[i] = (float *)(ws + f.slab[i % 2]);
-        for (int j = 0; j < h->nt; ++j) {     // one pair for every temporal layer: each sweep runs after the last read
-            m.For[j] = f.For ? (float *)(ws + f.For) : nullptr;   // offset 0 is slab 0: For / Back were not laid out
-            m.Back[j] = f.Back ? (float *)(ws + f.Back) : nullptr;
-        }
-        m.gemm = ws + f.gemm;
-        m.gemm_bytes = f.gemm_bytes;
-        m.counters = (unsigned int *)(ws + f.counters);
-        m.sweep = ws + f.sweep;
-        m.sweep_bytes = f.sweep_bytes;
-        return brnn_forward(h, feats, T_per_utt, B, Tmax, params, probs_out, m, false, st);
+        if (!workspace || ws_bytes < h->fwd.total)
+            return set_error(CTCB_ENOMEM, "ctcb_brnn_cost_and_grad: workspace %zu < %zu bytes", ws_bytes, h->fwd.total);
+        FwdBufs m{};
+        fwd_bufs(h->fwd, N, h->nt, ws, &m);
+        return brnn_forward(h, feats, T_per_utt, B, Tmax, params, probs_out, m, false, caller);
     }
+    // planned on every call: the contraction planners' overrides may change under a live handle (common.cuh)
     const WsLayout w = ws_layout(&c);
     if (!workspace || ws_bytes < w.total)
         return set_error(CTCB_ENOMEM, "ctcb_brnn_cost_and_grad: workspace %zu < %zu bytes", ws_bytes, w.total);
-    auto Xbuf = [&](int i) -> float * { return (float *)(ws + w.X[i]); };
-    auto P = [&](int idx) -> const float * {
-        int64_t off; ctcb_brnn_tensor_info(&c, idx, &off, nullptr, nullptr); return params + off;
-    };
-    auto G = [&](int idx) -> float * {
-        int64_t off; ctcb_brnn_tensor_info(&c, idx, &off, nullptr, nullptr); return grads + off;
-    };
-    // For_j / Back_j of temporal layer j; the dFor / dBack pair of layer j is pair j % 2
-    float *ForJ[64], *BackJ[64];
-    for (int j = 0; j < h->nt; ++j) {
-        ForJ[j] = (float *)(ws + w.ForJ[j]);
-        BackJ[j] = (float *)(ws + w.BackJ[j]);      // unused (offset 0) for the uni-directional layers above the first
-    }
-    float *dF[2] = {(float *)(ws + w.dFor), (float *)(ws + w.dFor2)};
-    float *dB[2] = {(float *)(ws + w.dBack), (float *)(ws + w.dBack2)};
-    void *gws = ws + w.gemm;
-    const size_t gws_bytes = w.gemm2 - w.gemm;
-    unsigned int *counters = (unsigned int *)(ws + w.counters);
-    const int nt = h->nt;
-    const bool uni = (c.unidirectional != 0);
-    auto temporal = [&](int i) { return nt > 0 && i >= tl && i < tl + nt; };
-    // activations of layer i as the next layer (and the weight gradients) see them: a uni-directional temporal
-    // layer's output IS its forward sweep (rnnet.py:112-116), a bi-directional one's is For + Back
-    auto Act = [&](int i) -> float * { return (uni && temporal(i)) ? ForJ[i - tl] : Xbuf(i); };
-
-    // ---------------------------------------------------------------- forward (brnnet.py:136-157)
-    for (int i = 1; i <= N + 1; ++i) m.X[i] = Xbuf(i);
-    for (int j = 0; j < nt; ++j) {
-        m.For[j] = ForJ[j];
-        m.Back[j] = BackJ[j];
-    }
-    m.gemm = gws;
-    m.gemm_bytes = gws_bytes;
-    m.counters = counters;
-    m.sweep = ws + w.sweep;
-    m.sweep_bytes = w.sweep_bytes;
-    const bool drop = h->drop_p > 0.f;
-    const bool overlap = (tl > 0);     // layers i >= tl: dW/db on the side stream, delta chain + BPTT on the main one
-    const cudaStream_t caller = st;
+    FwdBufs m{};
+    train_bufs(w, N, h->nt, ws, &m);
+    const bool dp = (h->comm != nullptr) && comm_world(h->comm) > 1;
+    Step s{h, m, w, ws, feats, params, T_per_utt, grads, B, Tmax, R, first, last, h->drop_p > 0.f, dp,
+           caller, nullptr, caller};
+    const bool overlap = (h->tl > 0);
     if (overlap) {     // fork: the main chain runs on h->hi until the join below
         TRY(ensure_side_stream(h));
         CTCB_CUDA_CHECK(cudaEventRecord(h->ev_fork, caller));
         CTCB_CUDA_CHECK(cudaStreamWaitEvent(h->hi, h->ev_fork, 0));
-        st = h->hi;
+        s.main = h->hi;
+        s.side = h->side;
     }
-    TRY(brnn_forward(h, feats, T_per_utt, B, Tmax, params, probs_out, m, drop, st));
-    float *logits = Xbuf(N + 1);
-
-    // ---------------------------------------------------------------- CTC (brnnet.py:161-175)
-    auto dbuf = [&](int j) -> float * { return (float *)(ws + w.D[j]); };
-    {
-    ProfScope ps("ctc", st);
-    TRY(ctcb_ctc_loss_grad_f32(logits, 0, (int64_t)K, (int64_t)B * K, labels, label_off, T_per_utt, B, Tmax, K,
-                               c.maxLabels, 0, dbuf(N + 1), cost_out, skip_out, ws + w.ctc, w.gemm - w.ctc, st));
+    TRY(brnn_forward(h, feats, T_per_utt, B, Tmax, params, probs_out, m, s.drop, s.main));
+    {     // brnnet.py:161-175
+    ProfScope ps("ctc", s.main);
+    TRY(ctcb_ctc_loss_grad_f32(m.X[N + 1], 0, (int64_t)K, (int64_t)B * K, labels, label_off, T_per_utt, B, Tmax, K,
+                               c.maxLabels, 0, s.buf(w.D[N + 1]), cost_out, skip_out, ws + w.ctc, w.ctc_bytes, s.main));
     }
-
-    // ---------------------------------------------------------------- backward (brnnet.py:188-243)
-    // Per temporal layer from the top: the delta GEMM without a mask, the BPTT sweep into pair j % 2, then on the side
-    // stream the weight gradients of the maps from the last sweep's down to this layer and the recurrent
-    // weight-gradient pair, add2.  The side stream's weight gradients become ready together with the sweep, not before
-    // it: the sweep's clusters (the higher priority) take their SMs first and the GEMMs run on the rest for the length
-    // of the sweep, instead of holding SMs the sweep then waits for.  Layer j - 2 writes the pair layer j used: its
-    // sweep waits for ev_pair, recorded on the side stream behind the last read of that pair (the recurrent weight
-    // gradients; for a uni-directional layer the weight gradient of the map above, whose delta the pair is).
-    const bool dp = (h->comm != nullptr) && comm_world(h->comm) > 1;
-    void *gws2 = ws + w.gemm2;
-    const size_t gws2_bytes = w.colsum - w.gemm2;
-    // rnnet.py:162-177: the BPTT result of a uni-directional layer is the delta
-    auto delta_of = [&](int i) -> float * { return (uni && temporal(i + 1)) ? dF[(i + 1 - tl) % 2] : dbuf(i + 1); };
-    // the weight and bias gradients of map i on stream sw, where its delta is complete
-    auto weight_grads = [&](int i, cudaStream_t sw) -> int {
-        const float *Xi = (i == 0) ? feats : Act(i);
-        const int n_out = sz[i + 1], n_in = sz[i];
-        float *dcur = delta_of(i);
-        const bool on_side = (sw != st);
-        // dW = delta^T . X_i   (brnnet.py:196)
-        {
-        ProfScope ps("gemm_dw", sw);
-        TRY(ctcb_gemm_f32(1, 0, n_out, n_in, (int)R, 1.f, dcur, n_out, Xi, n_in, beta_g, G(2 * i), n_in, nullptr, 0,
-                          nullptr, on_side ? gws2 : gws, on_side ? gws2_bytes : gws_bytes, sw));
-        }
-        // db = row sums of delta   (brnnet.py:200)
-        {
-            ProfScope ps("colsum", sw);
-            float *part = (float *)(ws + (on_side ? w.colsum2 : w.colsum));
-            int nblk;
-            if (n_out % 4 == 0 && (((uintptr_t)dcur) & 15) == 0) {
-                const int n4 = n_out / 4;
-                const int bx = n4 >= 256 ? 256 : (n4 + 31) / 32 * 32;
-                const int ncb = (n4 + bx - 1) / bx;
-                int64_t rpb = R / (2 * num_sms() / ncb > 0 ? 2 * num_sms() / ncb : 1);     // ~2 blocks per SM
-                if (rpb < CS_ROWS_MIN) rpb = CS_ROWS_MIN;
-                if (rpb > CS_ROWS) rpb = CS_ROWS;
-                nblk = (int)((R + rpb - 1) / rpb);
-                colsum_stage1_wide<<<dim3(ncb, nblk), bx, 0, sw>>>((const float4 *)dcur, R, n4, (int)rpb, (float4 *)part);
-            } else {
-                nblk = (int)((R + CS_ROWS - 1) / CS_ROWS);
-                colsum_stage1<<<dim3((n_out + 31) / 32, nblk), dim3(32, 8), 0, sw>>>(dcur, R, n_out, part);
-            }
-            CTCB_LAUNCH_CHECK();
-            if (first) colsum_stage2<false><<<(n_out + 127) / 128, 128, 0, sw>>>(part, nblk, n_out, G(2 * i + 1));
-            else colsum_stage2<true><<<(n_out + 127) / 128, 128, 0, sw>>>(part, nblk, n_out, G(2 * i + 1));
-            CTCB_LAUNCH_CHECK();
-        }
-        if (uni && temporal(i + 1) && i + 1 - tl >= 2)     // the last read of the pair of uni-directional layer i + 1
-            CTCB_CUDA_CHECK(cudaEventRecord(h->ev_pair[(i + 1 - tl) % 2], h->side));
-        if (dp && last && on_side && i == tl) {
-            // every gradient tensor of the layers >= tl is now queued on the side stream: sum that contiguous range over
-            // the ranks there, next to the BPTT sweep on the main stream
-            float *pa = G(2 * tl);
-            const int64_t na = (G(2 * N + 1) + sz[N + 1]) - pa;
-            TRY(comm_allreduce_ranges(h->comm, &pa, &na, 1, h->side));
-        }
-        return CTCB_OK;
-    };
-    int side_top = N;      // the highest map >= tl whose weight gradients are not queued yet
-    for (int i = N; i >= 0; --i) {
-        const float *Xi = (i == 0) ? feats : Act(i);
-        const int n_out = sz[i + 1], n_in = sz[i];
-        float *dcur = delta_of(i);
-        if (!(overlap && i >= tl)) TRY(weight_grads(i, st));
-        if (i > 0) {
-            float *doth = dbuf(i);
-            // delta <- delta . W, with the ReLU mask sign(hActs[i]) fused (brnnet.py:203-204,235-237).  A dropped
-            // layer's X_i is 0 at every dropped unit, so the same mask removes those; the kept ones were scaled by
-            // drop_scale in the forward pass, and so is their delta, through alpha.
-            const float *mask = temporal(i) ? nullptr : Xi;
-            const float alpha = (drop && !temporal(i)) ? h->drop_scale : 1.f;
-            {
-            ProfScope ps("gemm_delta", st);
-            TRY(ctcb_gemm_f32(0, 0, (int)R, n_in, n_out, alpha, dcur, n_out, P(2 * i), n_in, 0.f, doth, n_in,
-                              nullptr, 0, mask, gws, gws_bytes, st));
-            }
-            if (temporal(i)) {   // brnnet.py:207-233
-                const int j = i - tl, p = j % 2, iWtf = rec_index(&c, j), iWtb = iWtf + 2;
-                float *dFor = dF[p], *dBack = dB[p], *For = ForJ[j], *Back = BackJ[j];
-                if (j + 2 < nt)      // layer j + 2 used this pair
-                    CTCB_CUDA_CHECK(cudaStreamWaitEvent(st, h->ev_pair[p], 0));
-                // the deltas of maps side_top..i are complete here
-                CTCB_CUDA_CHECK(cudaEventRecord(h->ev_delta[i], st));
-                {
-                ProfScope ps("sweep_bptt", st);
-                TRY(run_sweep(1, Tmax, B, H, T_per_utt, doth, P(iWtf), uni ? nullptr : P(iWtb), dFor, dBack, For, Back,
-                              c.maxAct, counters, ws + w.sweep, w.sweep_bytes, st));
-                }
-                CTCB_CUDA_CHECK(cudaStreamWaitEvent(h->side, h->ev_delta[i], 0));
-                for (; side_top >= i; --side_top) TRY(weight_grads(side_top, h->side));
-                // recurrent weight gradients (brnnet.py:227-230): independent of the rest of the backward pass,
-                // so they go to the side stream as well
-                CTCB_CUDA_CHECK(cudaEventRecord(h->ev_delta[65], st));
-                CTCB_CUDA_CHECK(cudaStreamWaitEvent(h->side, h->ev_delta[65], 0));
-                {
-                ProfScope ps("gemm_dw_rec", h->side);
-                if (Tmax > 1) {
-                    const int64_t Rm = R - B;
-                    if (uni)
-                        TRY(ctcb_gemm_f32(1, 0, H, H, (int)Rm, 1.f, dFor + (int64_t)B * H, H, For, H, beta_g, G(iWtf), H,
-                                          nullptr, 0, nullptr, gws2, gws2_bytes, h->side));
-                    else     // both directions in one launch
-                        TRY(ctcb_gemm_pair_f32(1, 0, H, H, (int)Rm, 1.f, dFor + (int64_t)B * H, dBack, H, For,
-                                               Back + (int64_t)B * H, H, beta_g, G(iWtf), G(iWtb), H, gws2, gws2_bytes,
-                                               h->side));
-                } else if (first) {     // one frame: no recurrence, nothing to add to earlier micro-batches
-                    CTCB_CUDA_CHECK(cudaMemsetAsync(G(iWtf), 0, sizeof(float) * H * H, h->side));
-                    if (!uni) CTCB_CUDA_CHECK(cudaMemsetAsync(G(iWtb), 0, sizeof(float) * H * H, h->side));
-                }
-                }
-                if (!uni) {
-                    if (j >= 2) CTCB_CUDA_CHECK(cudaEventRecord(h->ev_pair[p], h->side));
-                    TRY(run_add2(dFor, dBack, doth, R * H, st));
-                }
-            }
-        }
-    }
-    // the main stream's tail writes nothing the side stream touches, so it runs next to the recurrent weight gradients
-    for (int j = 0; j < nt; ++j) {   // the `dummy` biases never receive gradient
-        const int iWtf = rec_index(&c, j);
-        CTCB_CUDA_CHECK(cudaMemsetAsync(G(iWtf + 1), 0, sizeof(float), st));
-        if (!uni) CTCB_CUDA_CHECK(cudaMemsetAsync(G(iWtf + 3), 0, sizeof(float), st));
-    }
-
-    if (stats_out) {     // after both sweeps, so that the tail carries the error flag of either
-        if (first) batch_stats_kernel<false><<<1, 32, 0, st>>>(cost_out, skip_out, B, stats_out, counters);
-        else batch_stats_kernel<true><<<1, 32, 0, st>>>(cost_out, skip_out, B, stats_out, counters);
-        CTCB_LAUNCH_CHECK();
-    }
+    TRY(s.backward());
+    if (stats_out)     // after both sweeps, so that the tail carries the error flag of either
+        TRY(run_batch_stats(cost_out, skip_out, B, stats_out, m.counters, !first, s.main));
     if (overlap) {     // join: every gradient tensor is complete on the caller's stream from here on
         CTCB_CUDA_CHECK(cudaEventRecord(h->ev_side, h->side));
         CTCB_CUDA_CHECK(cudaEventRecord(h->ev_hi, h->hi));
         CTCB_CUDA_CHECK(cudaStreamWaitEvent(caller, h->ev_side, 0));
         CTCB_CUDA_CHECK(cudaStreamWaitEvent(caller, h->ev_hi, 0));
-        st = caller;
     }
     // an earlier micro-batch of the step: the exchange and the L2 term wait for the sum of all of them
-    if (!last) return CTCB_OK;
-
-    if (dp) TRY(brnn_reduce_rest(h, grads, stats_out, overlap, st));
-
-    // ---------------------------------------------------------------- L2 (brnnet.py:177-183,197-198,244-247)
-    if (regcost_out) {
-        set_scalar_kernel<<<1, 1, 0, st>>>(regcost_out, 0.f);
-        CTCB_LAUNCH_CHECK();
-    }
-    if (c.reg > 0.f) {
-        const int nt = ctcb_brnn_num_tensors(&c);
-        for (int idx = 0; idx < nt; idx += 2) {
-            int64_t off; int32_t r, cc;
-            ctcb_brnn_tensor_info(&c, idx, &off, &r, &cc);
-            const int64_t n = (int64_t)r * cc;
-            if (!h->defer_l2) TRY(ctcb_axpy_f32(grads + off, params + off, c.reg, n, st));
-            if (regcost_out) TRY(run_sumsq(params + off, n, regcost_out, 0.5f * c.reg, 1, ws + w.scratch, st));
-        }
-    }
-    return CTCB_OK;
+    return last ? s.finish(stats_out, regcost_out) : CTCB_OK;
 }
 
 extern "C" int ctcb_brnn_cost_and_grad(ctcb_brnn *h, const float *feats, const int32_t *T_per_utt,
@@ -842,13 +892,10 @@ extern "C" int ctcb_brnn_set_deferred_l2(ctcb_brnn *h, int deferred) {
 
 extern "C" int ctcb_brnn_apply_l2_f32(ctcb_brnn *h, const float *params, float *grads, void *stream) {
     if (!h || !params || !grads) return set_error(CTCB_EINVAL, "ctcb_brnn_apply_l2_f32: null pointer argument");
-    const ctcb_brnn_config &c = h->cfg;
-    if (c.reg <= 0.f) return CTCB_OK;
-    const int nt = ctcb_brnn_num_tensors(&c);
-    for (int idx = 0; idx < nt; idx += 2) {     // weight matrices only, as brnnet.py:197-198,244-247
-        int64_t off; int32_t r, cc;
-        ctcb_brnn_tensor_info(&c, idx, &off, &r, &cc);
-        TRY(ctcb_axpy_f32(grads + off, params + off, c.reg, (int64_t)r * cc, stream));
+    if (h->cfg.reg <= 0.f) return CTCB_OK;
+    for (int idx = 0; idx < h->net.n; idx += 2) {     // weight matrices only, as brnnet.py:197-198,244-247
+        const NetTable::Tensor &t = h->net.t[idx];
+        TRY(ctcb_axpy_f32(grads + t.off, params + t.off, h->cfg.reg, (int64_t)t.rows * t.cols, stream));
     }
     return CTCB_OK;
 }
@@ -864,20 +911,9 @@ extern "C" int ctcb_brnn_set_comm(ctcb_brnn *h, ctcb_comm *comm) {
 extern "C" int ctcb_brnn_exchange_only(ctcb_brnn *h, const float *params, float *grads, float *stats_out, void *stream) {
     if (!h || !params || !grads) return set_error(CTCB_EINVAL, "ctcb_brnn_exchange_only: null pointer argument");
     if (!h->comm || comm_world(h->comm) <= 1) return CTCB_OK;
-    const ctcb_brnn_config &c = h->cfg;
-    cudaStream_t st = (cudaStream_t)stream;
-    const bool early = (h->tl > 0);
-    if (early) {
-        int64_t lo, o; int32_t r, cc;
-        ctcb_brnn_tensor_info(&c, 2 * h->tl, &lo, nullptr, nullptr);
-        ctcb_brnn_tensor_info(&c, 2 * c.numLayers + 1, &o, &r, &cc);
-        float *pa = grads + lo;
-        const int64_t na = o + (int64_t)r * cc - lo;
-        TRY(comm_allreduce_ranges(h->comm, &pa, &na, 1, st));
-    }
-    TRY(brnn_reduce_rest(h, grads, stats_out, early, st));
-    if (c.reg > 0.f && !h->defer_l2) return ctcb_brnn_apply_l2_f32(h, params, grads, stream);
-    return CTCB_OK;
+    if (h->tl > 0) TRY(brnn_reduce_early(h, grads, (cudaStream_t)stream));
+    TRY(brnn_reduce_rest(h, grads, stats_out, (cudaStream_t)stream));
+    return h->defer_l2 ? CTCB_OK : ctcb_brnn_apply_l2_f32(h, params, grads, stream);
 }
 
 extern "C" int ctcb_brnn_set_dropout(ctcb_brnn *h, float p, uint64_t seed, const int64_t *step) {
@@ -908,32 +944,24 @@ extern "C" size_t ctcb_brnn_sweep_workspace_bytes(int H, int B) { return 4096 + 
 // Test / diagnostic hook: where, inside the workspace, the activations of the LAST ctcb_brnn_cost_and_grad call lie
 // (time-major [Tmax][B][n] with that call's B and Tmax).  what = 0: output of affine map `layer` (1..numLayers+1; the
 // temporal layer's entry holds For + Back, the last one the logits), 1: For, 2: Back (temporal layer only; with
-// several, `layer` says which).
+// several, `layer` says which, and only a bi-directional stack has a Back of every layer).
 extern "C" int ctcb_brnn_activation_offset(const ctcb_brnn_config *cfg, int what, int layer, size_t *offset, int32_t *width) {
     if (!valid_cfg(cfg) || !offset) return set_error(CTCB_EINVAL, "ctcb_brnn_activation_offset: bad arguments");
     const WsLayout w = ws_layout(cfg);
-    int sizes[66];
-    layer_sizes(cfg, sizes);
     if (what == 0) {
         if (layer < 1 || layer > cfg->numLayers + 1) return set_error(CTCB_EINVAL, "ctcb_brnn_activation_offset: layer %d", layer);
         *offset = w.X[layer];
-        if (width) *width = sizes[layer];
+        if (width) *width = layer_size(cfg, layer);
         return CTCB_OK;
     }
-    const int nt = eff_nt(cfg);
-    if ((what == 1 || what == 2) && nt == 1) {     // one temporal layer: `layer` is ignored
-        *offset = (what == 1) ? w.For : w.Back;
-        if (width) *width = cfg->layerSize;
-        return CTCB_OK;
-    }
-    if ((what == 1 || (what == 2 && !cfg->unidirectional)) && nt > 1) {
-        const int j = layer - eff_tl(cfg);
-        if (j < 0 || j >= nt)
-            return set_error(CTCB_EINVAL, "ctcb_brnn_activation_offset: layer %d is not one of the temporal layers %d..%d",
-                             layer, eff_tl(cfg), eff_tl(cfg) + nt - 1);
-        *offset = (what == 1) ? w.ForJ[j] : w.BackJ[j];
-        if (width) *width = cfg->layerSize;
-        return CTCB_OK;
-    }
-    return set_error(CTCB_EINVAL, "ctcb_brnn_activation_offset: nothing of kind %d in this net", what);
+    const int nt = eff_nt(cfg), tl = eff_tl(cfg);
+    if ((what != 1 && what != 2) || nt == 0 || (what == 2 && nt > 1 && cfg->unidirectional))
+        return set_error(CTCB_EINVAL, "ctcb_brnn_activation_offset: nothing of kind %d in this net", what);
+    const int j = (nt == 1) ? 0 : layer - tl;     // one temporal layer: `layer` is ignored
+    if (j < 0 || j >= nt)
+        return set_error(CTCB_EINVAL, "ctcb_brnn_activation_offset: layer %d is not one of the temporal layers %d..%d",
+                         layer, tl, tl + nt - 1);
+    *offset = (what == 1) ? w.For[j] : w.Back[j];
+    if (width) *width = cfg->layerSize;
+    return CTCB_OK;
 }
