@@ -179,7 +179,25 @@ typedef struct ctcb_brnn_config {
                             * matrices and sweeps (output For_j + Back_j, uni-directional For_j).  0 and 1 both mean
                             * one temporal layer, so an initialiser without this member keeps its meaning.  k > 1 needs
                             * 1 <= temporalLayer and temporalLayer + k - 1 <= numLayers, else the config is invalid. */
+    int32_t cell;          /* recurrence of every temporal layer: 0 the reference's clipped ReLU (so an initialiser without
+                            * this member keeps its meaning), 1 LSTM (below); any other value makes the config invalid. */
 } ctcb_brnn_config;
+
+/* The LSTM cell (cell = 1; not in the reference).  Temporal layer i with input width n, H = layerSize, ndir = 2
+ * (bi-directional) or 1, G = ndir * 4H:
+ *   affine map [W_i, b_i] is G x n and G x 1; rows 0..4H-1 belong to the forward-in-time direction, 4H..8H-1 to the
+ *   backward one, each block in gate order i, f, g, o (torch.nn.LSTM's).  pre = W_i x + b_i.
+ *   each recurrent matrix is U (4H x H), still followed by its 1-float dummy; tensor count and order are unchanged.
+ *   per direction (the backward one mirrored in time), float32 with accurate expf / tanhf:
+ *     z_t = pre_t + U h_{t-1};  i, f, o = sigmoid(z_i, z_f, z_o);  g = tanh(z_g);  c_t = f c_{t-1} + i g;  h_t = o tanh(c_t)
+ *     h and c are 0 before the first frame and at every frame t >= T_u (the backward direction starts at T_u - 1);
+ *     there is no clip and maxAct is ignored.
+ *   layer output h_f + h_b (uni-directional: h_f), H wide.
+ *   BPTT: dh_t = delta_t + U^T dz_{t+1};  dc_t = dh_t o (1 - tanh^2 c_t) + dc_{t+1} f_{t+1};
+ *     dz = [dc g i(1-i), dc c_{t-1} f(1-f), dc i (1-g^2), dh tanh(c_t) o(1-o)];  dU = sum_t dz_t h_{t-1}^T,
+ *     dW_i = sum_t dz_t x_t^T, db_i = sum_t dz_t, delta_{i-1} = W_i^T dz; L2 adds reg W to W_i and U as to every matrix.
+ * ctcb_brnn_create refuses (CTCB_EINVAL, the message names the width) a layerSize whose sweep the device cannot hold
+ * co-resident: ndir * ceil(H / 8) CTAs of 256 threads, at most two per SM (bi-directional H = 2048 on an H100). */
 
 typedef struct ctcb_brnn ctcb_brnn; /* opaque; owns no device memory */
 
@@ -193,7 +211,11 @@ int ctcb_brnn_num_tensors(const ctcb_brnn_config *cfg);                    /* 2 
 int ctcb_brnn_tensor_info(const ctcb_brnn_config *cfg, int idx, int64_t *offset, int32_t *rows, int32_t *cols);
 /* numTemporal = k > 1 adds k * (2 bi-directional / 1 uni-directional) buffers of maxT*maxB*layerSize floats, each
  * rounded up to 256 bytes, to the one-layer size: For_j (and Back_j) of every temporal layer above the first, and a
- * second dFor / dBack pair that consecutive layers alternate with. */
+ * second dFor / dBack pair that consecutive layers alternate with.
+ * cell = 1 (R = maxT*maxB, every buffer rounded up to 256 bytes): an LSTM layer's X_i is G wide instead of H, its D_i
+ * max(H, outputDim, G) wide; per LSTM layer c of each direction and, bi-directional, the output For + Back (R*H
+ * each); the two column-sum areas grow to G wide, the sweep scratch holds 2*maxB*H floats, and the split-K areas
+ * are sized for the G-row contractions and the 4H x H recurrent weight gradients. */
 size_t ctcb_brnn_workspace_bytes(const ctcb_brnn_config *cfg);
 /* Byte offset, inside the workspace, of a uint32 that the recurrent-sweep kernels set non-zero when an
  * inter-CTA wait timed out (results are then invalid; never a hang).  Callers that synchronise anyway
@@ -215,7 +237,8 @@ size_t ctcb_brnn_forward_workspace_bytes(const ctcb_brnn_config *cfg, size_t *er
  * what = 1 / 2: For / Back of the temporal layer (brnnet.py:143-153).  With numTemporal > 1, `layer` names which
  * temporal layer (temporalLayer .. temporalLayer+k-1; Back exists only when bi-directional); with one temporal
  * layer it is ignored.  With dropout on (ctcb_brnn_set_dropout), the ReLU hidden layers' entries hold the dropped and
- * rescaled activations. */
+ * rescaled activations.  cell = 1 only: what = 3 the activated gates (G wide, the same buffer as what = 0 of that layer),
+ * 4 / 5 c of the forward / backward direction (H wide). */
 int ctcb_brnn_activation_offset(const ctcb_brnn_config *cfg, int what, int layer, size_t *offset, int32_t *width);
 
 int ctcb_brnn_create(const ctcb_brnn_config *cfg, ctcb_brnn **out);
@@ -306,6 +329,20 @@ size_t ctcb_brnn_sweep_workspace_bytes(int H, int B);
 int ctcb_brnn_sweep_f32(int mode, int T, int B, int H, const int32_t *T_per_utt, const float *pre,
                         const float *Wf, const float *Wb, float *outF, float *outB, const float *actF,
                         const float *actB, float maxAct, void *scratch, size_t scratch_bytes, void *stream);
+/* The LSTM recurrences of one temporal layer on their own (cell = 1).  Time-major arrays; G = 8H with Ub, 4H without.
+ * mode 0: gates [T][B][G] holds pre = W x + b on entry and the activated gates i, f, g, o (0 at padded frames) on
+ *   return; hF / hB [T][B][H] receive h, cF / cB [T][B][H] receive c.
+ * mode 1: gates, cF / cB as mode 0 left them, dh [T][B][H] the gradient w.r.t. the layer's output (the same for both
+ *   directions); dz [T][B][G] receives the gate gradients of both directions (hF / hB are not read).
+ * Ub == NULL runs the forward-in-time direction alone.  scratch: 256-byte aligned, ctcb_lstm_sweep_workspace_bytes(H,
+ * B) bytes (word 0 = error flag, cleared by the call and set when a wait between CTAs timed out; the dc carry). */
+size_t ctcb_lstm_sweep_workspace_bytes(int H, int B);
+int ctcb_lstm_sweep_f32(int mode, int T, int B, int H, const int32_t *T_per_utt, float *gates, const float *Uf,
+                        const float *Ub, float *hF, float *hB, float *cF, float *cB, const float *dh, float *dz,
+                        void *scratch, size_t scratch_bytes, void *stream);
+/* The LSTM sweep's plan for (H, B, ndir): out (HOST, 2 int32) = {KI (H / 32 with U in registers, else 0), utterance
+ * partitions}; the error ctcb_brnn_create returns for a width the device cannot hold. */
+int ctcb_debug_lstm_plan(int H, int B, int ndir, int32_t *out);
 /* 1 when the recurrences of a (layerSize H, B utterances, bi-directional) step run on the tensor-core kernel. */
 int ctcb_sweep_uses_tensor_cores(int H, int B);
 /* The plan ctcb_brnn_sweep_f32 launches for (H, B, ndir = 2 bi-directional / 1 forward in time only) on the current

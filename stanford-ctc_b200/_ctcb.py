@@ -21,13 +21,15 @@ c_int, c_i64, c_f32, c_vp, c_sz = ctypes.c_int, ctypes.c_int64, ctypes.c_float, 
 
 
 PART_FIRST, PART_LAST = 1, 2      # CTCB_PART_FIRST / CTCB_PART_LAST (ctcb_brnn_cost_and_grad_part)
+CELLS = {"relu": 0, "lstm": 1}   # ctcb_brnn_config.cell
 
 
 class BrnnConfig(ctypes.Structure):
     _fields_ = [("inputDim", ctypes.c_int32), ("outputDim", ctypes.c_int32), ("layerSize", ctypes.c_int32),
                 ("numLayers", ctypes.c_int32), ("temporalLayer", ctypes.c_int32), ("maxT", ctypes.c_int32),
                 ("maxB", ctypes.c_int32), ("maxLabels", ctypes.c_int32), ("reg", ctypes.c_float),
-                ("maxAct", ctypes.c_float), ("unidirectional", ctypes.c_int32), ("numTemporal", ctypes.c_int32)]
+                ("maxAct", ctypes.c_float), ("unidirectional", ctypes.c_int32), ("numTemporal", ctypes.c_int32),
+                ("cell", ctypes.c_int32)]
 
 
 _PROTOS = {
@@ -76,6 +78,10 @@ _PROTOS = {
                                     c_vp, c_sz, c_vp]),
     "ctcb_brnn_sweep_workspace_bytes": (c_sz, [c_int, c_int]),
     "ctcb_sweep_uses_tensor_cores": (c_int, [c_int, c_int]),
+    "ctcb_lstm_sweep_workspace_bytes": (c_sz, [c_int, c_int]),
+    "ctcb_lstm_sweep_f32": (c_int, [c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                    c_vp, c_vp, c_sz, c_vp]),
+    "ctcb_debug_lstm_plan": (c_int, [c_int, c_int, c_int, ctypes.POINTER(ctypes.c_int32)]),
     "ctcb_debug_sweep_plan": (c_int, [c_int, c_int, c_int, ctypes.POINTER(ctypes.c_int32)]),
     "ctcb_brnn_set_deferred_l2": (c_int, [c_vp, c_int]),
     "ctcb_brnn_apply_l2_f32": (c_int, [c_vp, c_vp, c_vp, c_vp]),

@@ -31,6 +31,11 @@ int comm_allreduce_ranges(ctcb_comm *c, float *const *ptrs, const int64_t *count
 int comm_world(const ctcb_comm *c);
 int run_dropout(float *X, int64_t R, int B, int H, int layer, uint64_t seed, const int64_t *step, int64_t first,
                 int64_t stride, uint32_t thr, float scale, cudaStream_t st);
+size_t lstm_carry_bytes(int H, int B);
+int run_lstm_sweep(int mode, int T, int B, int H, const int32_t *Tlen, float *gates, const float *Uf, const float *Ub,
+                   float *hF, float *hB, float *cF, float *cB, const float *dh, float *dz, unsigned int *counters,
+                   float *dc, cudaStream_t st);
+int lstm_check(int H, int B, int ndir);
 
 // ---- small kernels ---------------------------------------------------------------------------
 // column sums of a row-major R x N matrix: stage 1 partials over row blocks, stage 2 final
@@ -182,6 +187,7 @@ static const char *cfg_error(const ctcb_brnn_config *c, char (&buf)[192]) {
     if ((int64_t)c->maxT * c->maxB > GEMM_MAX_M)     // the forward and delta contractions have maxT*maxB rows
         return say("maxT * maxB = %lld rows exceed the contractions' limit of %d", (long long)c->maxT * c->maxB,
                    GEMM_MAX_M);
+    if (c->cell != 0 && c->cell != 1) return say("cell %d is neither 0 (clipped ReLU) nor 1 (LSTM)", c->cell);
     const bool ok = c->inputDim > 0 && c->outputDim > 1 && c->layerSize > 0 && c->numLayers >= 1 && c->numLayers <= 64 &&
                     c->maxT > 0 && c->maxB > 0 && c->maxLabels >= 0 && c->numTemporal >= 0 &&
                     // a stacked block must lie inside the hidden layers; k <= 1 keeps the silent "no temporal layer" rule below
@@ -215,6 +221,16 @@ static int layer_size(const ctcb_brnn_config *c, int i) {
 static size_t wider_of_H_K(const ctcb_brnn_config *c) {
     return (size_t)(c->layerSize > c->outputDim ? c->layerSize : c->outputDim);
 }
+static bool is_temporal(const ctcb_brnn_config *c, int i) {
+    const int tl = eff_tl(c);
+    return tl > 0 && i >= tl && i < tl + eff_nt(c);
+}
+// G = ndir * 4H: the rows of an LSTM layer's affine map, the pre-activations of the four gates of both directions
+static int lstm_rows(const ctcb_brnn_config *c) { return (c->unidirectional ? 1 : 2) * 4 * c->layerSize; }
+// rows of affine map i (1..N+1), the width of its output X_i: G at an LSTM layer, else the width of layer i
+static int map_rows(const ctcb_brnn_config *c, int i) {
+    return (c->cell == 1 && is_temporal(c, i)) ? lstm_rows(c) : layer_size(c, i);
+}
 
 extern "C" int ctcb_brnn_num_tensors(const ctcb_brnn_config *cfg) {
     if (!valid_cfg(cfg)) return 0;
@@ -242,10 +258,11 @@ void net_table(const ctcb_brnn_config *c, NetTable *nt) {
     for (int t = 0; t < nt->n; ++t) {
         int r, cc;
         if (t < 2 * nl) {
-            r = layer_size(c, t / 2 + 1);
+            r = map_rows(c, t / 2 + 1);
             cc = (t % 2 == 0) ? layer_size(c, t / 2) : 1;
         } else if ((t - 2 * nl) % 2 == 0) {
-            r = cc = c->layerSize;
+            r = c->cell == 1 ? 4 * c->layerSize : c->layerSize;     // U of an LSTM layer: the four gate blocks
+            cc = c->layerSize;
         } else {
             r = cc = 1;
         }
@@ -297,7 +314,9 @@ struct SweepWs {
 SweepWs take_sweep_ws(size_t &off, const ctcb_brnn_config *c) {
     SweepWs s{};
     s.counters = take(off, sizeof(unsigned int) * 1024);
-    s.scratch_bytes = eff_tl(c) ? sweep_tc_workspace_bytes(c->layerSize, c->maxB) : 0;
+    // the LSTM sweep's scratch is its dc carry
+    s.scratch_bytes = !eff_tl(c) ? 0 : c->cell == 1 ? lstm_carry_bytes(c->layerSize, c->maxB)
+                                                    : sweep_tc_workspace_bytes(c->layerSize, c->maxB);
     s.scratch = take(off, s.scratch_bytes);
     return s;
 }
@@ -307,6 +326,8 @@ struct WsLayout {
     // For / Back of temporal layer j, and the two dFor / dBack pairs, which consecutive layers alternate (layer j uses
     // pair j % 2); 0 where not laid out
     size_t For[64], Back[64], dFor[2], dBack[2];
+    // LSTM layers only: c of each direction, and the output For + Back of a bi-directional layer (X holds its gates)
+    size_t Cf[64], Cb[64], Out[64];
     size_t D[67];       // D[j]: gradient w.r.t. the output of affine map j (1..N+1)
     size_t ctc, ctc_bytes;
     size_t gemm, gemm_bytes, gemm2, gemm2_bytes;     // split-K areas of the main chain and of the side stream
@@ -322,7 +343,7 @@ WsLayout ws_layout(const ctcb_brnn_config *c) {
     const bool uni = (c->unidirectional != 0);
     const size_t RH = R * H * sizeof(float);
     size_t off = 0;
-    for (int i = 1; i <= N + 1; ++i) w.X[i] = take(off, R * layer_size(c, i) * sizeof(float));
+    for (int i = 1; i <= N + 1; ++i) w.X[i] = take(off, R * map_rows(c, i) * sizeof(float));
     if (nt) {       // all four for every net with a temporal layer, a uni-directional one too
         w.For[0] = take(off, RH);
         w.Back[0] = take(off, RH);
@@ -339,25 +360,35 @@ WsLayout ws_layout(const ctcb_brnn_config *c) {
         w.dFor[1] = take(off, RH);
         if (!uni) w.dBack[1] = take(off, RH);
     }
+    const bool lstm = (c->cell == 1);
+    for (int j = 0; lstm && j < nt; ++j) {
+        w.Cf[j] = take(off, RH);
+        if (!uni) {
+            w.Cb[j] = take(off, RH);
+            w.Out[j] = take(off, RH);
+        }
+    }
     const size_t wide = wider_of_H_K(c);
-    for (int j = 1; j <= N + 1; ++j) w.D[j] = take(off, R * wide * sizeof(float));
+    // an LSTM layer's D holds dz, G wide
+    const size_t wide_g = lstm && (size_t)lstm_rows(c) > wide ? (size_t)lstm_rows(c) : wide;
+    for (int j = 1; j <= N + 1; ++j) w.D[j] = take(off, R * (map_rows(c, j) == layer_size(c, j) ? wide : wide_g) * sizeof(float));
     w.ctc = take(off, ctcb_ctc_workspace_bytes(c->maxB, c->maxT, c->maxLabels), &w.ctc_bytes);
     size_t g = 0;
     const int Rint = (int)R;      // a valid config: R <= GEMM_MAX_M
     auto need = [&](int M_, int N_, int K_) { size_t b = ctcb_gemm_workspace_bytes(M_, N_, K_); if (b > g) g = b; };
     for (int i = 0; i <= N; ++i) {
-        need(Rint, layer_size(c, i + 1), layer_size(c, i));      // forward   X_i . W^T
-        need(Rint, layer_size(c, i), layer_size(c, i + 1));      // backward  delta . W
-        need(layer_size(c, i + 1), layer_size(c, i), Rint);      // weights   delta^T . X_i
+        need(Rint, map_rows(c, i + 1), layer_size(c, i));        // forward   X_i . W^T
+        need(Rint, layer_size(c, i), map_rows(c, i + 1));        // backward  delta . W
+        need(map_rows(c, i + 1), layer_size(c, i), Rint);        // weights   delta^T . X_i
     }
     {                                            // recurrent weight gradients (a pair for the bi-directional layer)
-        const size_t b = ctcb_gemm_pair_workspace_bytes(H, H, Rint);
+        const size_t b = ctcb_gemm_pair_workspace_bytes(lstm ? 4 * H : H, H, Rint);
         if (b > g) g = b;
     }
     w.gemm = take(off, g, &w.gemm_bytes);
     w.gemm2 = take(off, g, &w.gemm2_bytes);
-    w.colsum = take(off, ((R + CS_ROWS_MIN - 1) / CS_ROWS_MIN) * wide * sizeof(float));
-    w.colsum2 = take(off, ((R + CS_ROWS_MIN - 1) / CS_ROWS_MIN) * wide * sizeof(float));
+    w.colsum = take(off, ((R + CS_ROWS_MIN - 1) / CS_ROWS_MIN) * wide_g * sizeof(float));
+    w.colsum2 = take(off, ((R + CS_ROWS_MIN - 1) / CS_ROWS_MIN) * wide_g * sizeof(float));
     w.l2_scratch = take(off, 8192);
     w.sweep = take_sweep_ws(off, c);
     w.total = off;
@@ -374,6 +405,7 @@ constexpr int GEMM_ROW_TILE = 128;
 struct FwdLayout {
     size_t slab[2];
     size_t For, Back, gemm, gemm_bytes;
+    size_t Cf, Cb, Out;     // LSTM layers: c of each direction and the bi-directional output, shared as For / Back are
     SweepWs sweep;      // as in ws_layout: the same sweep plan
     size_t total;
 };
@@ -383,11 +415,20 @@ FwdLayout fwd_layout(const ctcb_brnn_config *c) {
     const size_t R = (size_t)c->maxT * c->maxB;
     const int N = c->numLayers, H = c->layerSize;
     size_t off = 0;
-    f.slab[0] = take(off, R * wider_of_H_K(c) * sizeof(float));
-    f.slab[1] = take(off, R * wider_of_H_K(c) * sizeof(float));
+    const bool lstm = (c->cell == 1) && eff_tl(c);
+    const size_t slab = (lstm && (size_t)lstm_rows(c) > wider_of_H_K(c)) ? (size_t)lstm_rows(c) : wider_of_H_K(c);
+    f.slab[0] = take(off, R * slab * sizeof(float));
+    f.slab[1] = take(off, R * slab * sizeof(float));
     if (eff_tl(c)) {
         f.For = take(off, R * H * sizeof(float));
         if (!c->unidirectional) f.Back = take(off, R * H * sizeof(float));
+    }
+    if (lstm) {
+        f.Cf = take(off, R * H * sizeof(float));
+        if (!c->unidirectional) {
+            f.Cb = take(off, R * H * sizeof(float));
+            f.Out = take(off, R * H * sizeof(float));
+        }
     }
     // ctcb_gemm_f32 takes a smaller plan when its area is short of ctcb_gemm_workspace_bytes(R, ..), and that need is
     // not monotone in R = Tmax*B: below one wave of output tiles the tensor-core plan adds split-K partials.  So that a
@@ -400,7 +441,7 @@ FwdLayout fwd_layout(const ctcb_brnn_config *c) {
     const int Mtop = (Rint < GEMM_ROW_TILE * num_sms()) ? Rint : GEMM_ROW_TILE * num_sms();
     for (int i = 0; i <= N; ++i) {
         for (int M = GEMM_ROW_TILE; ; M += GEMM_ROW_TILE) {
-            const size_t b = ctcb_gemm_workspace_bytes(M <= Mtop ? M : Rint, layer_size(c, i + 1), layer_size(c, i));
+            const size_t b = ctcb_gemm_workspace_bytes(M <= Mtop ? M : Rint, map_rows(c, i + 1), layer_size(c, i));
             if (b > g) g = b;
             if (M > Mtop) break;
         }
@@ -418,6 +459,7 @@ FwdLayout fwd_layout(const ctcb_brnn_config *c) {
 struct FwdBufs {
     float *X[66];
     float *For[64], *Back[64];
+    float *Cf[64], *Cb[64], *Out[64];     // LSTM layers
     void *gemm;
     size_t gemm_bytes;
     unsigned int *counters;
@@ -430,6 +472,9 @@ void fwd_bufs(const FwdLayout &f, int N, int nt, char *ws, FwdBufs *m) {
     for (int j = 0; j < nt; ++j) {     // one pair for every temporal layer: each sweep runs after the last read
         m->For[j] = f.For ? (float *)(ws + f.For) : nullptr;   // offset 0 is slab 0: For / Back were not laid out
         m->Back[j] = f.Back ? (float *)(ws + f.Back) : nullptr;
+        m->Cf[j] = f.Cf ? (float *)(ws + f.Cf) : nullptr;
+        m->Cb[j] = f.Cb ? (float *)(ws + f.Cb) : nullptr;
+        m->Out[j] = f.Out ? (float *)(ws + f.Out) : nullptr;
     }
     m->gemm = ws + f.gemm;
     m->gemm_bytes = f.gemm_bytes;
@@ -442,6 +487,9 @@ void train_bufs(const WsLayout &w, int N, int nt, char *ws, FwdBufs *m) {
     for (int j = 0; j < nt; ++j) {
         m->For[j] = (float *)(ws + w.For[j]);
         m->Back[j] = (float *)(ws + w.Back[j]);      // unused (offset 0) for the uni-directional layers above the first
+        m->Cf[j] = (float *)(ws + w.Cf[j]);          // these three: unused (offset 0) unless LSTM
+        m->Cb[j] = (float *)(ws + w.Cb[j]);
+        m->Out[j] = (float *)(ws + w.Out[j]);
     }
     m->gemm = ws + w.gemm;
     m->gemm_bytes = w.gemm_bytes;
@@ -489,13 +537,19 @@ struct ctcb_brnn {
     int64_t drop_first = 0, drop_stride = 1;
 
     bool uni() const { return cfg.unidirectional != 0; }
+    bool lstm() const { return cfg.cell == 1; }
     bool temporal(int i) const { return nt > 0 && i >= tl && i < tl + nt; }
     int size(int i) const { return layer_size(&cfg, i); }
+    int rows(int i) const { return map_rows(&cfg, i); }     // width of X_i
     int rec(int j) const { return rec_index(&cfg, j); }
     template <typename T> T *tensor(T *flat, int idx) const { return flat + net.t[idx].off; }
     // activations of layer i as the next layer (and the weight gradients) see them: a uni-directional temporal
-    // layer's output IS its forward sweep (rnnet.py:112-116), a bi-directional one's is For + Back
-    float *act(const FwdBufs &m, int i) const { return (uni() && temporal(i)) ? m.For[i - tl] : m.X[i]; }
+    // layer's output IS its forward sweep (rnnet.py:112-116), a bi-directional one's is For + Back (in X_i, or in Out
+    // at an LSTM layer, whose X_i holds the gates)
+    float *act(const FwdBufs &m, int i) const {
+        if (!temporal(i)) return m.X[i];
+        return uni() ? m.For[i - tl] : lstm() ? m.Out[i - tl] : m.X[i];
+    }
 };
 
 extern "C" size_t ctcb_brnn_workspace_bytes(const ctcb_brnn_config *cfg) {
@@ -525,6 +579,15 @@ extern "C" int ctcb_brnn_create(const ctcb_brnn_config *cfg, ctcb_brnn **out) {
     if (h->cfg.maxAct <= 0.f) h->cfg.maxAct = 20.0f;   // brnnet.py:32
     h->tl = eff_tl(cfg);
     h->nt = eff_nt(cfg);
+    if (cfg->cell == 1 && h->nt) {      // a width whose LSTM sweep the device cannot hold co-resident
+        const int rc = lstm_check(cfg->layerSize, cfg->maxB, cfg->unidirectional ? 1 : 2);
+        if (rc != CTCB_OK) {
+            char why[512];
+            snprintf(why, sizeof(why), "%s", ctcb_last_error());
+            delete h;
+            return set_error(rc, "ctcb_brnn_create: %s", why);
+        }
+    }
     net_table(cfg, &h->net);
     *out = h;
     return CTCB_OK;
@@ -610,7 +673,7 @@ static int brnn_forward(ctcb_brnn *h, const float *feats, const int32_t *T_per_u
     for (int i = 1; i <= N + 1; ++i) {
         const float *in = (i == 1) ? feats : h->act(m, i - 1);
         const int relu = (i <= N && !h->temporal(i)) ? 1 : 0;
-        const int n_out = h->size(i), n_in = h->size(i - 1);
+        const int n_out = h->rows(i), n_in = h->size(i - 1);
         {
         ProfScope ps("gemm_fwd", st);
         TRY(ctcb_gemm_f32(0, 1, (int)R, n_out, n_in, 1.f, in, n_in, h->tensor(params, 2 * (i - 1)), n_in, 0.f, m.X[i],
@@ -621,7 +684,19 @@ static int brnn_forward(ctcb_brnn *h, const float *feats, const int32_t *T_per_u
             TRY(run_dropout(m.X[i], R, B, n_out, i, h->drop_seed, h->drop_step, h->drop_first, h->drop_stride,
                             h->drop_thr, h->drop_scale, st));
         }
-        if (h->temporal(i)) {
+        if (h->temporal(i) && h->lstm()) {     // the gates over X_i in place, h into For / Back
+            const int j = i - h->tl, iU = h->rec(j);
+            {
+            ProfScope ps("sweep_fwd", st);
+            TRY(run_lstm_sweep(0, Tmax, B, H, T_per_utt, m.X[i], h->tensor(params, iU),
+                               uni ? nullptr : h->tensor(params, iU + 2), m.For[j], m.Back[j], m.Cf[j], m.Cb[j], nullptr,
+                               nullptr, m.counters, (float *)m.sweep, st));
+            }
+            if (!uni) {
+                ProfScope ps("elementwise", st);
+                TRY(run_add2(m.For[j], m.Back[j], m.Out[j], R * H, st));
+            }
+        } else if (h->temporal(i)) {
             const int j = i - h->tl, iWtf = h->rec(j);
             {
             ProfScope ps("sweep_fwd", st);
@@ -668,8 +743,9 @@ struct Step {
     float *G(int idx) const { return h->tensor(grads, idx); }
     float beta_g() const { return first ? 0.f : 1.f; }      // weight-gradient contractions: C = dW (+ C)
     // the delta of map i; rnnet.py:162-177: the BPTT result of a uni-directional layer is the delta
+    // (an LSTM layer's BPTT writes its dz, the delta of its map, into D)
     float *delta(int i) const {
-        return buf((h->uni() && h->temporal(i + 1)) ? w.dFor[(i + 1 - h->tl) % 2] : w.D[i + 1]);
+        return buf((h->uni() && h->temporal(i + 1) && !h->lstm()) ? w.dFor[(i + 1 - h->tl) % 2] : w.D[i + 1]);
     }
     int weight_grads(int i, bool on_side) const;
     int rec_weight_grads(int j) const;
@@ -682,7 +758,7 @@ struct Step {
 int Step::weight_grads(int i, bool on_side) const {
     const cudaStream_t st = on_side ? side : main;
     const float *Xi = (i == 0) ? feats : h->act(m, i);
-    const int n_out = h->size(i + 1), n_in = h->size(i);
+    const int n_out = h->rows(i + 1), n_in = h->size(i);
     // dW = delta^T . X_i   (brnnet.py:196)
     {
     ProfScope ps("gemm_dw", st);
@@ -694,7 +770,7 @@ int Step::weight_grads(int i, bool on_side) const {
     ProfScope ps("colsum", st);
     TRY(run_colsum(delta(i), R, n_out, buf(on_side ? w.colsum2 : w.colsum), G(2 * i + 1), !first, st));
     }
-    if (h->uni() && h->temporal(i + 1) && i + 1 - h->tl >= 2)     // the last read of the pair of uni-directional layer i + 1
+    if (h->uni() && h->temporal(i + 1) && !h->lstm() && i + 1 - h->tl >= 2)  // the last read of the pair of uni-directional layer i + 1
         CTCB_CUDA_CHECK(cudaEventRecord(h->ev_pair[(i + 1 - h->tl) % 2], side));
     // every gradient tensor of the layers >= tl is now queued on the side stream: sum that contiguous range over
     // the ranks there, next to the BPTT sweep on the main stream
@@ -710,7 +786,23 @@ int Step::rec_weight_grads(int j) const {
     CTCB_CUDA_CHECK(cudaEventRecord(h->ev_sweep, main));
     CTCB_CUDA_CHECK(cudaStreamWaitEvent(side, h->ev_sweep, 0));
     ProfScope ps("gemm_dw_rec", side);
-    if (Tmax > 1) {
+    if (h->lstm()) {     // dU = sum_t dz_t h_prev^T: the dz of both directions lie side by side in the layer's D, G wide
+        const int ldz = h->rows(h->tl + j), M = 4 * H;
+        const float *dz = buf(w.D[h->tl + j]);
+        if (Tmax > 1) {
+            const int64_t Rm = R - B;
+            if (h->uni())
+                TRY(ctcb_gemm_f32(1, 0, M, H, (int)Rm, 1.f, dz + (int64_t)B * ldz, ldz, m.For[j], H, beta_g(), G(iWtf), H,
+                                  nullptr, 0, nullptr, ws + w.gemm2, w.gemm2_bytes, side));
+            else
+                TRY(ctcb_gemm_pair_f32(1, 0, M, H, (int)Rm, 1.f, dz + (int64_t)B * ldz, dz + M, ldz, m.For[j],
+                                       m.Back[j] + (int64_t)B * H, H, beta_g(), G(iWtf), G(iWtb), H, ws + w.gemm2,
+                                       w.gemm2_bytes, side));
+        } else if (first) {
+            CTCB_CUDA_CHECK(cudaMemsetAsync(G(iWtf), 0, sizeof(float) * M * H, side));
+            if (!h->uni()) CTCB_CUDA_CHECK(cudaMemsetAsync(G(iWtb), 0, sizeof(float) * M * H, side));
+        }
+    } else if (Tmax > 1) {
         const int64_t Rm = R - B;
         if (h->uni())
             TRY(ctcb_gemm_f32(1, 0, H, H, (int)Rm, 1.f, dFor + (int64_t)B * H, H, m.For[j], H, beta_g(), G(iWtf), H,
@@ -741,8 +833,10 @@ int Step::backward() const {
         // layers i >= tl > 0: dW/db on the side stream, delta chain + BPTT on the main one
         if (!(tl > 0 && i >= tl)) TRY(weight_grads(i, false));
         if (i == 0) break;
-        const int n_out = h->size(i + 1), n_in = h->size(i);
-        float *doth = buf(w.D[i]);
+        const int n_out = h->rows(i + 1), n_in = h->size(i);
+        // an LSTM layer's dh goes to the pair; its BPTT writes dz into D[i]
+        const bool lstm = h->temporal(i) && h->lstm();
+        float *doth = buf(lstm ? w.dFor[(i - tl) % 2] : w.D[i]);
         // delta <- delta . W, with the ReLU mask sign(hActs[i]) fused (brnnet.py:203-204,235-237).  A dropped
         // layer's X_i is 0 at every dropped unit, so the same mask removes those; the kept ones were scaled by
         // drop_scale in the forward pass, and so is their delta, through alpha.
@@ -756,19 +850,23 @@ int Step::backward() const {
         if (!h->temporal(i)) continue;
         // brnnet.py:207-233
         const int j = i - tl, p = j % 2, iWtf = h->rec(j);
-        if (j + 2 < nt)      // layer j + 2 used this pair
+        if (j + 2 < nt && !lstm)      // layer j + 2 used this pair (an LSTM layer's pair is read on this stream only)
             CTCB_CUDA_CHECK(cudaStreamWaitEvent(main, h->ev_pair[p], 0));
         // the deltas of maps side_top..i are complete here
         CTCB_CUDA_CHECK(cudaEventRecord(h->ev_delta[i], main));
         {
         ProfScope ps("sweep_bptt", main);
-        TRY(run_sweep(1, Tmax, B, H, T_per_utt, doth, P(iWtf), uni ? nullptr : P(iWtf + 2), buf(w.dFor[p]),
-                      buf(w.dBack[p]), m.For[j], m.Back[j], h->cfg.maxAct, m.counters, m.sweep, m.sweep_bytes, main));
+        if (lstm)
+            TRY(run_lstm_sweep(1, Tmax, B, H, T_per_utt, m.X[i], P(iWtf), uni ? nullptr : P(iWtf + 2), nullptr, nullptr,
+                               m.Cf[j], m.Cb[j], doth, buf(w.D[i]), m.counters, (float *)m.sweep, main));
+        else
+            TRY(run_sweep(1, Tmax, B, H, T_per_utt, doth, P(iWtf), uni ? nullptr : P(iWtf + 2), buf(w.dFor[p]),
+                          buf(w.dBack[p]), m.For[j], m.Back[j], h->cfg.maxAct, m.counters, m.sweep, m.sweep_bytes, main));
         }
         CTCB_CUDA_CHECK(cudaStreamWaitEvent(side, h->ev_delta[i], 0));
         for (; side_top >= i; --side_top) TRY(weight_grads(side_top, true));
         TRY(rec_weight_grads(j));
-        if (!uni) {
+        if (!uni && !lstm) {
             if (j >= 2) CTCB_CUDA_CHECK(cudaEventRecord(h->ev_pair[p], side));
             TRY(run_add2(buf(w.dFor[p]), buf(w.dBack[p]), doth, R * H, main));
         }
@@ -951,17 +1049,19 @@ extern "C" int ctcb_brnn_activation_offset(const ctcb_brnn_config *cfg, int what
     if (what == 0) {
         if (layer < 1 || layer > cfg->numLayers + 1) return set_error(CTCB_EINVAL, "ctcb_brnn_activation_offset: layer %d", layer);
         *offset = w.X[layer];
-        if (width) *width = layer_size(cfg, layer);
+        if (width) *width = map_rows(cfg, layer);     // an LSTM layer's X holds its gates
         return CTCB_OK;
     }
     const int nt = eff_nt(cfg), tl = eff_tl(cfg);
-    if ((what != 1 && what != 2) || nt == 0 || (what == 2 && nt > 1 && cfg->unidirectional))
+    const bool lstm_kind = (what >= 3 && what <= 5);
+    if ((what != 1 && what != 2 && !lstm_kind) || nt == 0 || (what == 2 && nt > 1 && cfg->unidirectional) ||
+        (lstm_kind && cfg->cell != 1) || (what == 5 && cfg->unidirectional))
         return set_error(CTCB_EINVAL, "ctcb_brnn_activation_offset: nothing of kind %d in this net", what);
     const int j = (nt == 1) ? 0 : layer - tl;     // one temporal layer: `layer` is ignored
     if (j < 0 || j >= nt)
         return set_error(CTCB_EINVAL, "ctcb_brnn_activation_offset: layer %d is not one of the temporal layers %d..%d",
                          layer, tl, tl + nt - 1);
-    *offset = (what == 1) ? w.For[j] : w.Back[j];
-    if (width) *width = cfg->layerSize;
+    *offset = (what == 1) ? w.For[j] : (what == 2) ? w.Back[j] : (what == 3) ? w.X[tl + j] : (what == 4) ? w.Cf[j] : w.Cb[j];
+    if (width) *width = (what == 3) ? map_rows(cfg, tl + j) : cfg->layerSize;
     return CTCB_OK;
 }

@@ -1,0 +1,391 @@
+// sweep_lstm.cu -- the LSTM recurrences of a temporal layer (cell = 1, include/ctcb200.h) as ONE persistent kernel.
+//
+// Per direction, with z = pre + U h_prev in gate order i, f, g, o (torch.nn.LSTM's):
+//   forward : i, f, o = sigmoid(z_i, z_f, z_o), g = tanh(z_g);  c = f c_prev + i g;  h = o tanh(c)
+//   BPTT    : dh = delta + U^T dz_next;  dc = dh o (1 - tanh^2 c) + dc_next f_next;
+//             dz = [dc g i(1-i), dc c_prev f(1-f), dc i (1-g^2), dh tanh(c) o(1-o)]
+// h, c, dz and dc are 0 at every frame t >= T_u, so the backward-in-time direction starts at T_u - 1.
+//
+// Design: the generic sweep's (sweep.cu) with the rows regrouped.  A CTA of 8 warps owns 8 hidden units; warp w keeps
+// the FOUR gate rows of unit j0 + w (forward: rows U[r H + j][:], BPTT: the columns U[r H + :][j] of the four gate
+// blocks), so after the transposing butterfly lane (r, b) holds gate r -- or, in BPTT, the part of dh that gate block r
+// contributes -- of utterance b, and the cell update is four shuffles inside the warp: no second exchange per step.
+// The state of the previous step (h, or the dz of all 4H rows in BPTT) is exchanged through L2, as the generic sweep
+// does, behind one counter barrier per step whose wait is bounded: a timeout sets the error flag and the sweep runs on
+// (results invalid, never a hang).  U lives in registers where the CTAs that hold it are co-resident (H = 64..1024 in
+// steps of powers of two, while ndir * H / 8 CTAs fit one per SM), else it is re-read through L1/L2.
+//
+// The forward mode writes the activated gates over the pre-activations in place, c of every frame, and h into the
+// layer's For / Back; the BPTT mode reads those back and carries dc from step to step in a [B][H] scratch per direction.
+#include "common.cuh"
+
+namespace ctcb {
+
+constexpr int LS_THREADS = 256;
+constexpr int LS_UNITS = 8;    // hidden units per CTA (one per warp, four gate rows each)
+constexpr int LS_NB = 8;       // utterances per inner tile
+
+struct LstmArgs {
+    int mode;                  // 0: forward recurrences, 1: BPTT
+    int T, B, H;
+    const int32_t *Tlen;       // [B]
+    float *gates;              // [T][B][G], G = ndir 4H: mode 0 pre-activations in, activated gates out; mode 1 in
+    const float *U[2];         // 4H x H per direction, row-major (gate row x unit)
+    float *h[2];               // mode 0: [T][B][H] out
+    float *c[2];               // [T][B][H]: mode 0 out, mode 1 in
+    const float *dh;           // mode 1: [T][B][H], the gradient w.r.t. the layer's output
+    float *dz;                 // mode 1: [T][B][G] out
+    float *dc;                 // mode 1: [ndir][B][H] carry
+    int parts;                 // utterance partitions (gridDim.y)
+    int ndir;
+    unsigned int *err;         // word 0 of the scratch: the error flag, cleared by the caller
+    unsigned int *counters;    // [ndir * parts], zeroed before the launch
+};
+
+// The per-step barrier of the CTAs of one (direction, partition).  A wait longer than ~0.5 s sets the error flag and
+// gives up waiting for the rest of the sweep.
+__device__ __forceinline__ void lstm_barrier(unsigned int *ctr, unsigned int target, unsigned int *err, bool &dead) {
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        __threadfence();
+        atomicAdd(ctr, 1u);
+        if (!dead) {
+            const long long t0 = clock64();
+            while (true) {
+                unsigned int v;
+                asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(ctr) : "memory");
+                if (v >= target) break;
+                if (clock64() - t0 > 1000000000LL) {
+                    dead = true;
+                    atomicExch(err, 4u);
+                    break;
+                }
+            }
+        }
+    }
+    __syncthreads();
+}
+
+// [LS_NB][Hp] <- nb rows of H floats at src, src + pitch, ...; the rows beyond nb are zeroed
+__device__ __forceinline__ void lstm_load_state(float *hs, int Hp, const float *src, int64_t pitch, int nb, int H) {
+    if ((H & 3) == 0 && (pitch & 3) == 0 && (((uintptr_t)src) & 15) == 0) {
+        const int h4 = H >> 2;
+        for (int idx = threadIdx.x; idx < nb * h4; idx += LS_THREADS) {
+            const int bb = idx / h4, k4 = idx - bb * h4;
+            const float4 v = __ldcg(reinterpret_cast<const float4 *>(src + bb * pitch) + k4);
+            *reinterpret_cast<float4 *>(hs + bb * Hp + 4 * k4) = v;
+        }
+    } else {
+        for (int idx = threadIdx.x; idx < nb * H; idx += LS_THREADS) {
+            const int bb = idx / H, k = idx - bb * H;
+            hs[bb * Hp + k] = __ldcg(src + bb * pitch + k);
+        }
+    }
+    for (int idx = threadIdx.x + nb * Hp; idx < LS_NB * Hp; idx += LS_THREADS) hs[idx] = 0.f;
+}
+
+__device__ __forceinline__ float lstm_sigmoid(float z) { return 1.f / (1.f + expf(-z)); }
+
+// KI > 0: H == 32 KI and U lives in registers (one CTA per SM).  KI == 0: any H, U re-read (two CTAs per SM).
+template <int KI>
+__global__ void __launch_bounds__(LS_THREADS, KI > 0 ? 1 : 2) lstm_sweep_kernel(LstmArgs a) {
+    extern __shared__ __align__(16) float hs[];   // [LS_NB][Hp]
+    const int H = a.H, B = a.B, T = a.T;
+    const int64_t G = (int64_t)a.ndir * 4 * H;
+    const int Hp = (H + 3) / 4 * 4 + 4;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int dir = blockIdx.z;
+    const int j = blockIdx.x * LS_UNITS + warp;     // this warp's hidden unit
+    const bool bptt = (a.mode == 1);
+    const bool ascending = (dir == 0) != bptt;      // time runs forward for (forward, dir 0) and (BPTT, dir 1)
+    const float *U = a.U[dir];
+    const int64_t gbase = (int64_t)dir * 4 * H;     // this direction's gate block inside a row of G
+    float wreg[4][KI > 0 ? KI : 1];
+    if (KI > 0) {
+#pragma unroll
+        for (int r = 0; r < 4; ++r)
+#pragma unroll
+            for (int i = 0; i < KI; ++i) {
+                const int k = lane + 32 * i;
+                wreg[r][i] = (j < H) ? (bptt ? U[(int64_t)(r * H + k) * H + j] : U[(int64_t)(r * H + j) * H + k]) : 0.f;
+            }
+    }
+    const int ntiles = (B + LS_NB - 1) / LS_NB;
+    const int tiles_per_part = (ntiles + a.parts - 1) / a.parts;
+    const int tile_beg = blockIdx.y * tiles_per_part;
+    const int tile_end = min(ntiles, tile_beg + tiles_per_part);
+    unsigned int *ctr = a.counters + (dir * a.parts + blockIdx.y);
+    const unsigned int nslices = gridDim.x;
+    bool dead = false;
+
+    // lane -> (gate r, utterance b) of the value it owns after the butterfly
+    const int orow = lane >> 3, ob = lane & 7;
+
+    for (int s = 0; s < T; ++s) {
+        const int t = ascending ? s : T - 1 - s;
+        const int tp = (dir == 0) ? t - 1 : t + 1;     // predecessor of t in the forward recurrence
+        const int tn = (dir == 0) ? t + 1 : t - 1;     // its successor: the step BPTT came from
+        for (int tile = tile_beg; tile < tile_end; ++tile) {
+            const int b0 = tile * LS_NB;
+            const int b = b0 + ob;
+            const bool valid = (j < H) && (b < B);
+            const int64_t go = ((int64_t)t * B + b) * G + gbase + (int64_t)orow * H + j;    // this lane's gate
+            float gv = 0.f;
+            int Tb = 0;
+            if (valid) {
+                gv = __ldg(a.gates + go);      // mode 0: pre-activation; mode 1: activated gate
+                Tb = __ldg(a.Tlen + b);
+            }
+            float acc[32];
+#pragma unroll
+            for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+            if (s > 0) {
+                const int nb = min(LS_NB, B - b0);
+                if (!bptt) {       // U h_prev: the four gate rows of unit j
+                    lstm_load_state(hs, Hp, a.h[dir] + ((int64_t)tp * B + b0) * H, H, nb, H);
+                    __syncthreads();
+                    if (KI > 0) {
+#pragma unroll
+                        for (int i = 0; i < KI; ++i) {
+                            float hv[LS_NB];
+#pragma unroll
+                            for (int bb = 0; bb < LS_NB; ++bb) hv[bb] = hs[bb * Hp + lane + 32 * i];
+#pragma unroll
+                            for (int r = 0; r < 4; ++r)
+#pragma unroll
+                                for (int bb = 0; bb < LS_NB; ++bb) acc[r * 8 + bb] = fmaf(wreg[r][i], hv[bb], acc[r * 8 + bb]);
+                        }
+                    } else if (j < H) {
+                        for (int k = lane; k < H; k += 32) {
+                            float hv[LS_NB], wv[4];
+#pragma unroll
+                            for (int bb = 0; bb < LS_NB; ++bb) hv[bb] = hs[bb * Hp + k];
+#pragma unroll
+                            for (int r = 0; r < 4; ++r) wv[r] = __ldg(U + (int64_t)(r * H + j) * H + k);
+#pragma unroll
+                            for (int r = 0; r < 4; ++r)
+#pragma unroll
+                                for (int bb = 0; bb < LS_NB; ++bb) acc[r * 8 + bb] = fmaf(wv[r], hv[bb], acc[r * 8 + bb]);
+                        }
+                    }
+                    __syncthreads();   // hs is reused by the next tile
+                } else {           // U^T dz_next, one gate block r at a time: row r of the warp sums block r
+#pragma unroll
+                    for (int r = 0; r < 4; ++r) {
+                        lstm_load_state(hs, Hp, a.dz + ((int64_t)tn * B + b0) * G + gbase + (int64_t)r * H, G, nb, H);
+                        __syncthreads();
+                        if (KI > 0) {
+#pragma unroll
+                            for (int i = 0; i < KI; ++i)
+#pragma unroll
+                                for (int bb = 0; bb < LS_NB; ++bb)
+                                    acc[r * 8 + bb] = fmaf(wreg[r][i], hs[bb * Hp + lane + 32 * i], acc[r * 8 + bb]);
+                        } else if (j < H) {
+                            for (int k = lane; k < H; k += 32) {
+                                const float wv = __ldg(U + (int64_t)(r * H + k) * H + j);
+#pragma unroll
+                                for (int bb = 0; bb < LS_NB; ++bb) acc[r * 8 + bb] = fmaf(wv, hs[bb * Hp + k], acc[r * 8 + bb]);
+                            }
+                        }
+                        __syncthreads();
+                    }
+                }
+                // transposing butterfly: lane l ends with the sum over lanes of acc[l]
+#pragma unroll
+                for (int off = 16, n = 32; off >= 1; off >>= 1, n >>= 1) {
+                    const bool up = (lane & off) != 0;
+#pragma unroll
+                    for (int i = 0; i < n / 2; ++i) {
+                        const float send = up ? acc[i] : acc[i + n / 2];
+                        const float keep = up ? acc[i + n / 2] : acc[i];
+                        acc[i] = keep + __shfl_xor_sync(0xffffffffu, send, off);
+                    }
+                }
+            }
+            const bool live = valid && t < Tb;
+            const int64_t hc = ((int64_t)t * B + b) * H + j;      // (t, b, j) in the [T][B][H] arrays
+            if (!bptt) {
+                const float z = gv + acc[0];
+                const float act = (orow == 2) ? tanhf(z) : lstm_sigmoid(z);
+                const float gi = __shfl_sync(0xffffffffu, act, ob), gf = __shfl_sync(0xffffffffu, act, 8 + ob);
+                const float gg = __shfl_sync(0xffffffffu, act, 16 + ob), gO = __shfl_sync(0xffffffffu, act, 24 + ob);
+                if (valid) {
+                    a.gates[go] = live ? act : 0.f;
+                    if (orow == 0) {
+                        const float cp = (live && s > 0) ? a.c[dir][((int64_t)tp * B + b) * H + j] : 0.f;
+                        const float cn = fmaf(gf, cp, gi * gg);
+                        const float hn = gO * tanhf(cn);
+                        a.c[dir][hc] = live ? cn : 0.f;
+                        a.h[dir][hc] = live ? hn : 0.f;
+                    }
+                }
+            } else {
+                const float p0 = __shfl_sync(0xffffffffu, acc[0], ob), p1 = __shfl_sync(0xffffffffu, acc[0], 8 + ob);
+                const float p2 = __shfl_sync(0xffffffffu, acc[0], 16 + ob), p3 = __shfl_sync(0xffffffffu, acc[0], 24 + ob);
+                const float gi = __shfl_sync(0xffffffffu, gv, ob), gf = __shfl_sync(0xffffffffu, gv, 8 + ob);
+                const float gg = __shfl_sync(0xffffffffu, gv, 16 + ob), gO = __shfl_sync(0xffffffffu, gv, 24 + ob);
+                if (valid && orow == 0) {
+                    float *dcp = a.dc + ((int64_t)dir * B + b) * H + j;
+                    float dzi = 0.f, dzf = 0.f, dzg = 0.f, dzo = 0.f, dct = 0.f;
+                    if (live) {
+                        const float dh = __ldg(a.dh + hc) + ((p0 + p1) + (p2 + p3));
+                        const float ct = a.c[dir][hc], tc = tanhf(ct);
+                        const bool has_prev = (tp >= 0 && tp < T), has_next = (s > 0);
+                        const float cp = has_prev ? a.c[dir][((int64_t)tp * B + b) * H + j] : 0.f;
+                        const float carry = has_next ? *dcp * a.gates[((int64_t)tn * B + b) * G + gbase + H + j] : 0.f;
+                        dct = dh * gO * (1.f - tc * tc) + carry;
+                        dzi = dct * gg * (gi * (1.f - gi));
+                        dzf = dct * cp * (gf * (1.f - gf));
+                        dzg = dct * gi * (1.f - gg * gg);
+                        dzo = dh * tc * (gO * (1.f - gO));
+                    }
+                    *dcp = dct;
+                    float *dzp = a.dz + ((int64_t)t * B + b) * G + gbase + j;
+                    dzp[0] = dzi;
+                    dzp[H] = dzf;
+                    dzp[2 * H] = dzg;
+                    dzp[3 * H] = dzo;
+                }
+            }
+        }
+        if (s + 1 < T) lstm_barrier(ctr, nslices * (unsigned int)(s + 1), a.err, dead);
+    }
+}
+
+// The launch of (H, B, ndir): register-resident U where its CTAs fit one per SM, else U re-read at two CTAs per SM.
+struct LstmPlan {
+    int KI, parts;
+    size_t smem;
+};
+
+template <int KI>
+static int lstm_capacity(size_t smem, int *capacity) {
+    int per_sm = 0;
+    CTCB_CUDA_CHECK(cudaFuncSetAttribute(lstm_sweep_kernel<KI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CTCB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, lstm_sweep_kernel<KI>, LS_THREADS, smem));
+    *capacity = per_sm * num_sms();
+    return CTCB_OK;
+}
+
+static int lstm_capacity_of(int KI, size_t smem, int *capacity) {
+    switch (KI) {
+        case 2: return lstm_capacity<2>(smem, capacity);
+        case 4: return lstm_capacity<4>(smem, capacity);
+        case 8: return lstm_capacity<8>(smem, capacity);
+        case 16: return lstm_capacity<16>(smem, capacity);
+        case 32: return lstm_capacity<32>(smem, capacity);
+        default: return lstm_capacity<0>(smem, capacity);
+    }
+}
+
+int lstm_plan(int H, int B, int ndir, LstmPlan *p) {
+    if (H <= 0 || B <= 0 || (ndir != 1 && ndir != 2))
+        return set_error(CTCB_EINVAL, "LSTM sweep: bad sizes (H=%d, B=%d, ndir=%d)", H, B, ndir);
+    const int slices = (H + LS_UNITS - 1) / LS_UNITS;
+    const int Hp = (H + 3) / 4 * 4 + 4;
+    p->smem = (size_t)LS_NB * Hp * sizeof(float);
+    const int ki_reg = (H == 64 || H == 128 || H == 256 || H == 512 || H == 1024) ? H / 32 : 0;
+    int capacity = 0;
+    for (p->KI = ki_reg;; p->KI = 0) {     // U does not fit the register files of the CTAs the device holds: re-read it
+        const int rc = lstm_capacity_of(p->KI, p->smem, &capacity);
+        if (rc != CTCB_OK) return rc;
+        if (ndir * slices <= capacity) break;
+        if (p->KI == 0)
+            return set_error(CTCB_EINVAL, "LSTM sweep: layerSize %d needs %d co-resident CTAs, device holds %d", H,
+                             ndir * slices, capacity);
+    }
+    const int ntiles = (B + LS_NB - 1) / LS_NB;
+    int parts = capacity / (ndir * slices);
+    if (parts > ntiles) parts = ntiles;
+    if (parts > 500) parts = 500;   // the counters region holds 1024 words
+    if (parts < 1) parts = 1;
+    p->parts = parts;
+    return CTCB_OK;
+}
+
+template <int KI>
+static int lstm_launch(LstmArgs &a, int slices, const LstmPlan &p, cudaStream_t st) {
+    dim3 grid(slices, a.parts, a.ndir);
+    void *params[] = {&a};
+    CTCB_CUDA_CHECK(cudaLaunchCooperativeKernel((void *)lstm_sweep_kernel<KI>, grid, dim3(LS_THREADS), params, p.smem, st));
+    count_launch();
+    return CTCB_OK;
+}
+
+// ctcb_brnn_create's check that the device holds the sweep of a config; without a device there is nothing to check
+// against, and the launch checks again
+int lstm_check(int H, int B, int ndir) {
+    int n = 0;
+    if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) {
+        (void)cudaGetLastError();
+        return CTCB_OK;
+    }
+    LstmPlan p;
+    return lstm_plan(H, B, ndir, &p);
+}
+
+size_t lstm_carry_bytes(int H, int B) { return align_up((size_t)2 * B * H * sizeof(float), 256); }
+
+// counters: 4096 bytes of device scratch (word 0 = error flag, cleared by the caller); dc: lstm_carry_bytes(H, B)
+int run_lstm_sweep(int mode, int T, int B, int H, const int32_t *Tlen, float *gates, const float *Uf, const float *Ub,
+                   float *hF, float *hB, float *cF, float *cB, const float *dh, float *dz, unsigned int *counters,
+                   float *dc, cudaStream_t st) {
+    LstmPlan p;
+    const int ndir = Ub ? 2 : 1;
+    const int rc = lstm_plan(H, B, ndir, &p);
+    if (rc != CTCB_OK) return rc;
+    LstmArgs a;
+    a.mode = mode; a.T = T; a.B = B; a.H = H; a.Tlen = Tlen; a.gates = gates;
+    a.U[0] = Uf; a.U[1] = Ub ? Ub : Uf;
+    a.h[0] = hF; a.h[1] = Ub ? hB : hF;
+    a.c[0] = cF; a.c[1] = Ub ? cB : cF;
+    a.dh = dh; a.dz = dz; a.dc = dc;
+    a.parts = p.parts; a.ndir = ndir;
+    a.err = counters;
+    a.counters = counters + 16;     // words [0..15] are reserved for error flags
+    CTCB_CUDA_CHECK(cudaMemsetAsync(a.counters, 0, sizeof(unsigned int) * (ndir * p.parts), st));
+    const int slices = (H + LS_UNITS - 1) / LS_UNITS;
+    switch (p.KI) {
+        case 2: return lstm_launch<2>(a, slices, p, st);
+        case 4: return lstm_launch<4>(a, slices, p, st);
+        case 8: return lstm_launch<8>(a, slices, p, st);
+        case 16: return lstm_launch<16>(a, slices, p, st);
+        case 32: return lstm_launch<32>(a, slices, p, st);
+        default: return lstm_launch<0>(a, slices, p, st);
+    }
+}
+
+}  // namespace ctcb
+
+extern "C" size_t ctcb_lstm_sweep_workspace_bytes(int H, int B) {
+    if (H <= 0 || B <= 0) return 0;
+    return 4096 + ctcb::lstm_carry_bytes(H, B);
+}
+
+extern "C" int ctcb_lstm_sweep_f32(int mode, int T, int B, int H, const int32_t *T_per_utt, float *gates,
+                                   const float *Uf, const float *Ub, float *hF, float *hB, float *cF, float *cB,
+                                   const float *dh, float *dz, void *scratch, size_t scratch_bytes, void *stream) {
+    using namespace ctcb;
+    if (!T_per_utt || !gates || !Uf || !cF || !scratch || (mode == 0 && !hF) || (mode == 1 && (!dh || !dz)) ||
+        (Ub && (!cB || (mode == 0 && !hB))))
+        return set_error(CTCB_EINVAL, "ctcb_lstm_sweep_f32: null pointer argument");
+    if (T <= 0 || B <= 0 || H <= 0 || (mode != 0 && mode != 1))
+        return set_error(CTCB_EINVAL, "ctcb_lstm_sweep_f32: bad sizes");
+    const size_t need = ctcb_lstm_sweep_workspace_bytes(H, B);
+    if (scratch_bytes < need || (((uintptr_t)scratch) & 255))
+        return set_error(CTCB_ENOMEM, "ctcb_lstm_sweep_f32: scratch of %zu bytes (256-byte aligned) needed, got %zu",
+                         need, scratch_bytes);
+    CTCB_CUDA_CHECK(cudaMemsetAsync(scratch, 0, 16 * sizeof(unsigned int), (cudaStream_t)stream));   // error flag
+    return run_lstm_sweep(mode, T, B, H, T_per_utt, gates, Uf, Ub, hF, hB, cF, cB, dh, dz, (unsigned int *)scratch,
+                          (float *)((char *)scratch + 4096), (cudaStream_t)stream);
+}
+
+extern "C" int ctcb_debug_lstm_plan(int H, int B, int ndir, int32_t *out) {
+    if (!out) return ctcb::set_error(CTCB_EINVAL, "ctcb_debug_lstm_plan: null output");
+    ctcb::LstmPlan p;
+    const int rc = ctcb::lstm_plan(H, B, ndir, &p);
+    if (rc != CTCB_OK) return rc;
+    out[0] = p.KI;
+    out[1] = p.parts;
+    return CTCB_OK;
+}

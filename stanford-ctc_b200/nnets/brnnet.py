@@ -15,6 +15,9 @@ single contiguous vector.  New, additive surface for the minibatch/data-parallel
 
     NNet(..., maxUtts=B, maxLabels=L)        capacity for B utterances per call (micro-batch)
     NNet(..., numTemporal=k)                 k stacked temporal layers temporalLayer .. temporalLayer+k-1
+    NNet(..., cell='lstm')                   LSTM temporal layers instead of the clipped-ReLU recurrence (include/ctcb200.h:
+                                                the cell): each layer's affine map has ndir*4H rows, each recurrent
+                                                matrix is 4H x H; 'relu' (the default) is the reference's net
     NNet(..., dropout=p, dropoutSeed=33)     inverted dropout on the ReLU hidden layers of training calls; the mask
                                                 of an utterance is drawn from (seed, the device counter dropoutStep,
                                                 layer, its index in the step's minibatch, frame, unit)
@@ -125,7 +128,7 @@ class NNet:
     def __init__(self, inputDim, outputDim, layerSize, numLayers, maxBatch,
                  train=True, temporalLayer=-1, reg=0.0, maxUtts=1, maxLabels=None,
                  allowTopTemporal=False, device=None, unidirectional=False, numTemporal=1, dropout=0.0,
-                 dropoutSeed=33):
+                 dropoutSeed=33, cell="relu"):
         torch = _ctcb.require_cuda()
         self._torch = torch
         self.dev = torch.device("cuda", torch.cuda.current_device() if device is None else device)
@@ -167,9 +170,12 @@ class NNet:
 
         # unidirectional: the single forward-in-time recurrence of nnets/rnnet.py (used by nnets.rnnet.NNet)
         self.unidirectional = bool(unidirectional)
+        if cell not in _ctcb.CELLS:
+            raise ValueError("cell=%r must be one of %s" % (cell, ", ".join(sorted(_ctcb.CELLS))))
+        self.cell = cell
         self._cfg = BrnnConfig(inputDim, outputDim, layerSize, numLayers, max(self.temporalLayer, 0), maxBatch,
                                maxUtts, self.maxLabels, float(reg), float(self.maxAct), int(self.unidirectional),
-                               self.numTemporal)
+                               self.numTemporal, _ctcb.CELLS[cell])
         self._h = ctypes.c_void_p()
         check(lib.ctcb_brnn_create(ctypes.byref(self._cfg), ctypes.byref(self._h)))
         self.stack = None
@@ -209,18 +215,23 @@ class NNet:
     def initParams(self):
         """Initialize parameters using 6/sqrt(fanin+fanout) -- same shapes and the same np.random draw
         order as brnnet.py:38-41 (layer stack) and :66-70 (Wtf then Wtb).  The recurrent matrices of further
-        stacked temporal layers are drawn after those, layer by layer, at the same scale."""
+        stacked temporal layers are drawn after those, layer by layer, at the same scale.  With cell='lstm' the same
+        rule and order apply to the LSTM shapes (a temporal layer's map has G = ndir*4H rows, each U is 4H x H), each
+        matrix at the scale of its own shape."""
         torch = self._torch
         sizes = [self.inputDim] + self.layerSizes + [self.outputDim]
-        scales = [np.sqrt(6) / np.sqrt(n + m) for n, m in zip(sizes[:-1], sizes[1:])]
+        rows = [self._map_rows(i) for i in range(1, self.numLayers + 2)]
+        scales = [np.sqrt(6) / np.sqrt(n + m) for n, m in zip(sizes[:-1], rows)]
         host = [[np.random.rand(m, n) * 2 * s - s, np.zeros((m, 1))]
-                for n, m, s in zip(sizes[:-1], sizes[1:], scales)]
+                for n, m, s in zip(sizes[:-1], rows, scales)]
+        H = self.layerSize
+        rec_rows = 4 * H if self.cell == "lstm" else H
         for _ in range(self.numTemporal):
-            scale = np.sqrt(6) / np.sqrt(self.layerSize * 2)
-            wtf = 2 * scale * np.random.rand(self.layerSize, self.layerSize) - scale
+            scale = np.sqrt(6) / np.sqrt(rec_rows + H)
+            wtf = 2 * scale * np.random.rand(rec_rows, H) - scale
             host.append([wtf, np.zeros((1, 1))])
             if not self.unidirectional:            # rnnet.py:57-61 draws a single recurrent matrix
-                wtb = 2 * scale * np.random.rand(self.layerSize, self.layerSize) - scale
+                wtb = 2 * scale * np.random.rand(rec_rows, H) - scale
                 host.append([wtb, np.zeros((1, 1))])
 
         self.nparams = int(lib.ctcb_brnn_param_count(ctypes.byref(self._cfg)))
@@ -275,6 +286,12 @@ class NNet:
                                           self.maxLabels)
         self._batch, self._batch_alt = self._batch_alt, self._batch
         return self._batch
+
+    def _map_rows(self, i):
+        """Rows of affine map i (1..numLayers+1): ndir*4H at an LSTM layer, else the width of layer i."""
+        if self.cell == "lstm" and self.numTemporal and self.temporalLayer <= i < self.temporalLayer + self.numTemporal:
+            return (1 if self.unidirectional else 2) * 4 * self.layerSize
+        return self.layerSize if i <= self.numLayers else self.outputDim
 
     def paramCount(self):
         return int(sum(w.numel() + b.numel() for w, b in self.stack))
@@ -462,6 +479,11 @@ class NNet:
         except UnicodeDecodeError:          # checkpoints written by the Python-2 reference
             fid.seek(0)
             stack = pickle.load(fid, encoding="latin1")
+        for k, ((w, b), (wi, bi)) in enumerate(zip(self.stack, stack)):
+            for x, xi in ((w, wi), (b, bi)):
+                if np.size(xi) != x.numel():
+                    raise ValueError("checkpoint tensor %d has shape %s where this net (cell=%r) has %s: a checkpoint "
+                                     "of another cell or shape" % (k, tuple(np.shape(xi)), self.cell, tuple(x.shape)))
         for (w, b), (wi, bi) in zip(self.stack, stack):
             w.copy_(torch.from_numpy(np.ascontiguousarray(wi, dtype=np.float32).reshape(tuple(w.shape))))
             b.copy_(torch.from_numpy(np.ascontiguousarray(bi, dtype=np.float32).reshape(tuple(b.shape))))
