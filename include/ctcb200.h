@@ -181,7 +181,22 @@ typedef struct ctcb_brnn_config {
                             * 1 <= temporalLayer and temporalLayer + k - 1 <= numLayers, else the config is invalid. */
     int32_t cell;          /* recurrence of every temporal layer: 0 the reference's clipped ReLU (so an initialiser without
                             * this member keeps its meaning), 1 LSTM (below); any other value makes the config invalid. */
+    int32_t layerNorm;     /* 0: off (so an initialiser without this member keeps its meaning); 1: layer normalisation of
+                            * the ReLU hidden layers (below); any other value makes the config invalid. */
 } ctcb_brnn_config;
+
+/* Layer normalisation (layerNorm = 1; not in the reference; Ba, Kiros & Hinton 2016).  Hidden layer i is normalised
+ * when 1 <= i <= numLayers and i is not temporal -- exactly the layers dropout drops.  Per frame row, H = layerSize:
+ *   z = W_i x + b_i;  mu = mean_j z_j;  var = mean_j (z_j - mu)^2 (biased);  rstd = 1 / sqrt(var + 1e-5)
+ *   xh = (z - mu) rstd;  X_i = relu(gamma_i xh + beta_i)      (then inverted dropout, unchanged, when p > 0)
+ * i.e. torch.nn.functional.layer_norm with eps = 1e-5, then ReLU.  The input, the temporal layers and the logits are
+ * never normalised; padded frames are normalised like any row (their delta is 0, so they add nothing to a gradient).
+ * Backward, g = dL/d(gamma xh + beta) (the masked delta contraction, with dropout's alpha), gh = g gamma:
+ *   dz = rstd (gh - mean_j gh - xh mean_j(gh xh));  dgamma = sum over rows of g xh;  dbeta = sum over rows of g.
+ * Each normalised layer adds [gamma_i, beta_i], each H x 1, behind every other tensor of the flat vector, in layer
+ * order; gamma and beta are not L2-regularised.  Statistics are fp32, the mean first and then the squared deviations
+ * from it, in an order that depends only on H.  layerSize above CTCB_LAYERNORM_MAX_H makes such a config invalid. */
+#define CTCB_LAYERNORM_MAX_H 8192
 
 /* The LSTM cell (cell = 1; not in the reference).  Temporal layer i with input width n, H = layerSize, ndir = 2
  * (bi-directional) or 1, G = ndir * 4H:
@@ -205,7 +220,8 @@ typedef struct ctcb_brnn ctcb_brnn; /* opaque; owns no device memory */
  * [W1,b1] ... [W_{N+1},b_{N+1}] [Wtf,dummy] [Wtb,dummy]; W row-major (out x in), dummy = 1 float.
  * unidirectional: [W1,b1] ... [W_{N+1},b_{N+1}] [Wt,dummy].
  * numTemporal = k > 1: [W1,b1] ... [W_{N+1},b_{N+1}] then, per temporal layer in ascending order,
- * [Wtf_j,dummy] [Wtb_j,dummy] (unidirectional: [Wt_j,dummy]); for k = 1 this is the layout above. */
+ * [Wtf_j,dummy] [Wtb_j,dummy] (unidirectional: [Wt_j,dummy]); for k = 1 this is the layout above.
+ * layerNorm = 1 appends [gamma_i, beta_i] of every normalised hidden layer i, in ascending i. */
 int64_t ctcb_brnn_param_count(const ctcb_brnn_config *cfg);
 int ctcb_brnn_num_tensors(const ctcb_brnn_config *cfg);                    /* 2 * len(stack) */
 int ctcb_brnn_tensor_info(const ctcb_brnn_config *cfg, int idx, int64_t *offset, int32_t *rows, int32_t *cols);
@@ -215,7 +231,10 @@ int ctcb_brnn_tensor_info(const ctcb_brnn_config *cfg, int idx, int64_t *offset,
  * cell = 1 (R = maxT*maxB, every buffer rounded up to 256 bytes): an LSTM layer's X_i is G wide instead of H, its D_i
  * max(H, outputDim, G) wide; per LSTM layer c of each direction and, bi-directional, the output For + Back (R*H
  * each); the two column-sum areas grow to G wide, the sweep scratch holds 2*maxB*H floats, and the split-K areas
- * are sized for the G-row contractions and the 4H x H recurrent weight gradients. */
+ * are sized for the G-row contractions and the 4H x H recurrent weight gradients.
+ * layerNorm = 1 appends, behind everything else: per normalised layer z (R*H floats) and the row statistics mu and
+ * rstd (R floats each), then ctcb_layernorm_workspace_bytes(R, H) for the parameter-gradient partials.  The forward
+ * workspace (ctcb_brnn_forward_workspace_bytes) does not grow: a forward-only call normalises in place. */
 size_t ctcb_brnn_workspace_bytes(const ctcb_brnn_config *cfg);
 /* Byte offset, inside the workspace, of a uint32 that the recurrent-sweep kernels set non-zero when an
  * inter-CTA wait timed out (results are then invalid; never a hang).  Callers that synchronise anyway
@@ -313,6 +332,21 @@ int ctcb_brnn_set_dropout_utts(ctcb_brnn *h, int64_t first, int64_t stride);
  * counter is the optimisation step: the dropout mask and the adaptive optimisers (ctcb_adagrad_step_f32,
  * ctcb_adam_step_f32) read the same one, and sgd.SGD advances it once per step, so it equals SGD.it. */
 int ctcb_dropout_advance(int64_t *step, void *stream);
+
+/* ---- layer normalisation on its own (layerNorm = 1, above) -----------------------------------------------------
+ * Rows are [R][H] fp32, 1 <= H <= CTCB_LAYERNORM_MAX_H; with H % 4 == 0 every pointer must be 16-byte aligned.
+ * forward : y = relu(gamma (z - mu) rstd + beta) per row; y may alias z; mu / rstd (R floats each) receive the row
+ *           statistics, or are both NULL.  The same device code writes y either way, so the bits of y do not depend on it.
+ * backward: delta holds g on entry and dz on return (in place); z, mu, rstd as the forward left them; dgamma / dbeta
+ *           (H floats each) receive the sums over the rows, or, with accumulate != 0, have them added.  workspace:
+ *           ctcb_layernorm_workspace_bytes(R, H) bytes (per-CTA partial sums, added in a fixed order: the bits depend
+ *           only on R, H and the inputs).  0 for H out of range. */
+size_t ctcb_layernorm_workspace_bytes(int64_t R, int H);
+int ctcb_layernorm_forward_f32(const float *z, float *y, float *mu, float *rstd, const float *gamma, const float *beta,
+                               int64_t R, int H, void *stream);
+int ctcb_layernorm_backward_f32(float *delta, const float *z, const float *mu, const float *rstd, const float *gamma,
+                                float *dgamma, float *dbeta, int64_t R, int H, int accumulate, void *workspace,
+                                size_t ws_bytes, void *stream);
 
 /* ---- the time recurrences of the temporal layer on their own (replaces the per-frame loops
  *      brnnet.py:144-152 [mode 0] and brnnet.py:208-224 [mode 1]) -------------------------------

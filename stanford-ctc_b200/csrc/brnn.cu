@@ -36,6 +36,12 @@ int run_lstm_sweep(int mode, int T, int B, int H, const int32_t *Tlen, float *ga
                    float *hF, float *hB, float *cF, float *cB, const float *dh, float *dz, unsigned int *counters,
                    float *dc, cudaStream_t st);
 int lstm_check(int H, int B, int ndir);
+size_t layernorm_workspace_bytes(int64_t R, int H);
+int run_layernorm_forward(const float *z, float *y, float *mu, float *rstd, const float *gamma, const float *beta,
+                          int64_t R, int H, cudaStream_t st);
+int run_layernorm_backward(float *d, const float *z, const float *mu, const float *rstd, const float *gamma,
+                           float *dgamma, float *dbeta, int64_t R, int H, bool accumulate, float *partial,
+                           cudaStream_t st);
 
 // ---- small kernels ---------------------------------------------------------------------------
 // column sums of a row-major R x N matrix: stage 1 partials over row blocks, stage 2 final
@@ -188,6 +194,11 @@ static const char *cfg_error(const ctcb_brnn_config *c, char (&buf)[192]) {
         return say("maxT * maxB = %lld rows exceed the contractions' limit of %d", (long long)c->maxT * c->maxB,
                    GEMM_MAX_M);
     if (c->cell != 0 && c->cell != 1) return say("cell %d is neither 0 (clipped ReLU) nor 1 (LSTM)", c->cell);
+    if (c->layerNorm != 0 && c->layerNorm != 1)
+        return say("layerNorm %d is neither 0 (off) nor 1 (layer normalisation of the ReLU hidden layers)", c->layerNorm);
+    if (c->layerNorm == 1 && c->layerSize > CTCB_LAYERNORM_MAX_H)
+        return say("layerNorm needs layerSize <= %d (the normalisation kernels hold a row on chip); layerSize is %d",
+                   CTCB_LAYERNORM_MAX_H, c->layerSize);
     const bool ok = c->inputDim > 0 && c->outputDim > 1 && c->layerSize > 0 && c->numLayers >= 1 && c->numLayers <= 64 &&
                     c->maxT > 0 && c->maxB > 0 && c->maxLabels >= 0 && c->numTemporal >= 0 &&
                     // a stacked block must lie inside the hidden layers; k <= 1 keeps the silent "no temporal layer" rule below
@@ -231,19 +242,37 @@ static int lstm_rows(const ctcb_brnn_config *c) { return (c->unidirectional ? 1 
 static int map_rows(const ctcb_brnn_config *c, int i) {
     return (c->cell == 1 && is_temporal(c, i)) ? lstm_rows(c) : layer_size(c, i);
 }
+// hidden layer i is layer-normalised: a ReLU hidden layer of a layerNorm config (the layers dropout drops)
+static bool is_normed(const ctcb_brnn_config *c, int i) {
+    return c->layerNorm == 1 && i >= 1 && i <= c->numLayers && !is_temporal(c, i);
+}
+// the tensors of the flat vector before the [gamma, beta] pairs: the maps, the recurrent matrices and their dummies
+static int base_tensors(const ctcb_brnn_config *c) {
+    return 2 * (c->numLayers + 1) + eff_nt(c) * (c->unidirectional ? 2 : 4);
+}
+// flat-vector index of gamma of normalised layer i; beta is the next tensor
+static int ln_index(const ctcb_brnn_config *c, int i) {
+    int k = 0;
+    for (int l = 1; l < i; ++l) k += is_normed(c, l);
+    return base_tensors(c) + 2 * k;
+}
 
 extern "C" int ctcb_brnn_num_tensors(const ctcb_brnn_config *cfg) {
     if (!valid_cfg(cfg)) return 0;
-    return 2 * (cfg->numLayers + 1) + eff_nt(cfg) * (cfg->unidirectional ? 2 : 4);
+    int n = base_tensors(cfg);
+    for (int i = 1; i <= cfg->numLayers; ++i) n += 2 * is_normed(cfg, i);
+    return n;
 }
 
 namespace {
 // The flat parameter (and gradient) vector of a valid config: W and b of every affine map, then per temporal layer its
-// recurrent matrices, each followed by the reference's `dummy` bias (brnnet.py:60-72); every tensor 16-byte aligned.
+// recurrent matrices, each followed by the reference's `dummy` bias (brnnet.py:60-72), then [gamma, beta] of every
+// layer-normalised hidden layer; every tensor 16-byte aligned.
 struct NetTable {
     struct Tensor { int64_t off; int32_t rows, cols; };
     int n;
-    Tensor t[2 * 65 + 4 * 64];
+    int nreg;       // tensors 0 .. nreg-1 are the ones L2 regularisation sees (its even ones): all but the LN pairs
+    Tensor t[2 * 65 + 4 * 64 + 2 * 64];
     int64_t params;
     // The gradients that a data-parallel step sums over the ranks early, on the side stream next to the BPTT sweep: the
     // contiguous range from W of the lowest temporal layer to the end of b of layer N+1; empty (at `params`) without a
@@ -254,10 +283,14 @@ struct NetTable {
 void net_table(const ctcb_brnn_config *c, NetTable *nt) {
     const int nl = c->numLayers + 1;
     nt->n = ctcb_brnn_num_tensors(c);
+    nt->nreg = base_tensors(c);
     int64_t off = 0;
     for (int t = 0; t < nt->n; ++t) {
         int r, cc;
-        if (t < 2 * nl) {
+        if (t >= nt->nreg) {        // gamma or beta of a normalised layer
+            r = c->layerSize;
+            cc = 1;
+        } else if (t < 2 * nl) {
             r = map_rows(c, t / 2 + 1);
             cc = (t % 2 == 0) ? layer_size(c, t / 2) : 1;
         } else if ((t - 2 * nl) % 2 == 0) {
@@ -333,6 +366,9 @@ struct WsLayout {
     size_t gemm, gemm_bytes, gemm2, gemm2_bytes;     // split-K areas of the main chain and of the side stream
     size_t colsum, colsum2, l2_scratch;
     SweepWs sweep;
+    // layer-normalised hidden layers only (0 elsewhere): z, and the row statistics of the forward pass; the
+    // parameter-gradient partials of the backward pass
+    size_t Z[65], Mu[65], Rstd[65], ln_part;
     size_t total;
 };
 
@@ -391,6 +427,15 @@ WsLayout ws_layout(const ctcb_brnn_config *c) {
     w.colsum2 = take(off, ((R + CS_ROWS_MIN - 1) / CS_ROWS_MIN) * wide_g * sizeof(float));
     w.l2_scratch = take(off, 8192);
     w.sweep = take_sweep_ws(off, c);
+    if (c->layerNorm == 1) {
+        for (int i = 1; i <= N; ++i) {
+            if (!is_normed(c, i)) continue;
+            w.Z[i] = take(off, RH);
+            w.Mu[i] = take(off, R * sizeof(float));
+            w.Rstd[i] = take(off, R * sizeof(float));
+        }
+        w.ln_part = take(off, layernorm_workspace_bytes((int64_t)R, H));
+    }
     w.total = off;
     return w;
 }
@@ -458,6 +503,7 @@ FwdLayout fwd_layout(const ctcb_brnn_config *c) {
 // layers in the forward-only layout), the split-K area, the sweep counters and scratch.
 struct FwdBufs {
     float *X[66];
+    float *Z[65], *Mu[65], *Rstd[65];     // normalised layers of a training call: z and the row statistics; else null
     float *For[64], *Back[64];
     float *Cf[64], *Cb[64], *Out[64];     // LSTM layers
     void *gemm;
@@ -484,6 +530,11 @@ void fwd_bufs(const FwdLayout &f, int N, int nt, char *ws, FwdBufs *m) {
 }
 void train_bufs(const WsLayout &w, int N, int nt, char *ws, FwdBufs *m) {
     for (int i = 1; i <= N + 1; ++i) m->X[i] = (float *)(ws + w.X[i]);
+    for (int i = 1; i <= N; ++i) {
+        m->Z[i] = w.Z[i] ? (float *)(ws + w.Z[i]) : nullptr;
+        m->Mu[i] = w.Z[i] ? (float *)(ws + w.Mu[i]) : nullptr;
+        m->Rstd[i] = w.Z[i] ? (float *)(ws + w.Rstd[i]) : nullptr;
+    }
     for (int j = 0; j < nt; ++j) {
         m->For[j] = (float *)(ws + w.For[j]);
         m->Back[j] = (float *)(ws + w.Back[j]);      // unused (offset 0) for the uni-directional layers above the first
@@ -539,6 +590,7 @@ struct ctcb_brnn {
     bool uni() const { return cfg.unidirectional != 0; }
     bool lstm() const { return cfg.cell == 1; }
     bool temporal(int i) const { return nt > 0 && i >= tl && i < tl + nt; }
+    bool normed(int i) const { return is_normed(&cfg, i); }
     int size(int i) const { return layer_size(&cfg, i); }
     int rows(int i) const { return map_rows(&cfg, i); }     // width of X_i
     int rec(int j) const { return rec_index(&cfg, j); }
@@ -674,10 +726,20 @@ static int brnn_forward(ctcb_brnn *h, const float *feats, const int32_t *T_per_u
         const float *in = (i == 1) ? feats : h->act(m, i - 1);
         const int relu = (i <= N && !h->temporal(i)) ? 1 : 0;
         const int n_out = h->rows(i), n_in = h->size(i - 1);
+        // a normalised layer: the contraction writes z (into Z in a training call, in place in the slab otherwise),
+        // the normalisation kernel the ReLU output X_i
+        const bool ln = h->normed(i);
+        float *zi = (ln && m.Z[i]) ? m.Z[i] : m.X[i];
         {
         ProfScope ps("gemm_fwd", st);
-        TRY(ctcb_gemm_f32(0, 1, (int)R, n_out, n_in, 1.f, in, n_in, h->tensor(params, 2 * (i - 1)), n_in, 0.f, m.X[i],
-                          n_out, h->tensor(params, 2 * (i - 1) + 1), relu, nullptr, m.gemm, m.gemm_bytes, st));
+        TRY(ctcb_gemm_f32(0, 1, (int)R, n_out, n_in, 1.f, in, n_in, h->tensor(params, 2 * (i - 1)), n_in, 0.f, zi,
+                          n_out, h->tensor(params, 2 * (i - 1) + 1), ln ? 0 : relu, nullptr, m.gemm, m.gemm_bytes, st));
+        }
+        if (ln) {
+            const int ig = ln_index(&c, i);
+            ProfScope ps("layernorm", st);
+            TRY(run_layernorm_forward(zi, m.X[i], m.Mu[i], m.Rstd[i], h->tensor(params, ig), h->tensor(params, ig + 1),
+                                      R, n_out, st));
         }
         if (drop && relu) {
             ProfScope ps("dropout", st);
@@ -847,6 +909,12 @@ int Step::backward() const {
         TRY(ctcb_gemm_f32(0, 0, (int)R, n_in, n_out, alpha, delta(i), n_out, P(2 * i), n_in, 0.f, doth, n_in, nullptr, 0,
                           mask, m.gemm, m.gemm_bytes, main));
         }
+        if (h->normed(i)) {     // g -> dz in place, before anything reads D[i]; dgamma / dbeta of the layer
+            const int ig = ln_index(&h->cfg, i);
+            ProfScope ps("layernorm", main);
+            TRY(run_layernorm_backward(doth, m.Z[i], m.Mu[i], m.Rstd[i], P(ig), G(ig), G(ig + 1), R, n_in, !first,
+                                       buf(w.ln_part), main));
+        }
         if (!h->temporal(i)) continue;
         // brnnet.py:207-233
         const int j = i - tl, p = j % 2, iWtf = h->rec(j);
@@ -890,7 +958,7 @@ int Step::finish(float *stats, float *regcost_out) const {
     }
     if (!h->defer_l2) TRY(ctcb_brnn_apply_l2_f32(h, params, grads, caller));
     if (regcost_out && reg > 0.f)
-        for (int idx = 0; idx < h->net.n; idx += 2) {     // the same weight matrices
+        for (int idx = 0; idx < h->net.nreg; idx += 2) {     // the same weight matrices
             const NetTable::Tensor &t = h->net.t[idx];
             TRY(run_sumsq(params + t.off, (int64_t)t.rows * t.cols, regcost_out, 0.5f * reg, 1, ws + w.l2_scratch, caller));
         }
@@ -991,7 +1059,7 @@ extern "C" int ctcb_brnn_set_deferred_l2(ctcb_brnn *h, int deferred) {
 extern "C" int ctcb_brnn_apply_l2_f32(ctcb_brnn *h, const float *params, float *grads, void *stream) {
     if (!h || !params || !grads) return set_error(CTCB_EINVAL, "ctcb_brnn_apply_l2_f32: null pointer argument");
     if (h->cfg.reg <= 0.f) return CTCB_OK;
-    for (int idx = 0; idx < h->net.n; idx += 2) {     // weight matrices only, as brnnet.py:197-198,244-247
+    for (int idx = 0; idx < h->net.nreg; idx += 2) {     // weight matrices only, as brnnet.py:197-198,244-247
         const NetTable::Tensor &t = h->net.t[idx];
         TRY(ctcb_axpy_f32(grads + t.off, params + t.off, h->cfg.reg, (int64_t)t.rows * t.cols, stream));
     }

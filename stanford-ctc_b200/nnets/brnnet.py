@@ -18,6 +18,9 @@ single contiguous vector.  New, additive surface for the minibatch/data-parallel
     NNet(..., cell='lstm')                   LSTM temporal layers instead of the clipped-ReLU recurrence (include/ctcb200.h:
                                                 the cell): each layer's affine map has ndir*4H rows, each recurrent
                                                 matrix is 4H x H; 'relu' (the default) is the reference's net
+    NNet(..., layerNorm=True)                layer normalisation of the ReLU hidden layers (include/ctcb200.h:
+                                                layerNorm): relu(gamma * layer_norm(z) + beta), one [gamma, beta] pair
+                                                per normalised layer appended to `stack`, gamma = 1 and beta = 0 at start
     NNet(..., dropout=p, dropoutSeed=33)     inverted dropout on the ReLU hidden layers of training calls; the mask
                                                 of an utterance is drawn from (seed, the device counter dropoutStep,
                                                 layer, its index in the step's minibatch, frame, unit)
@@ -115,6 +118,15 @@ class DeviceBatch(object):
         return self
 
 
+def check_ln_pairs(got, want, n_ln, what):
+    """A net with layer normalisation loads only a checkpoint with its own number of [W, b] pairs (n_ln of them the
+    [gamma, beta] pairs behind the rest): zip() would otherwise leave the normalisation parameters unset."""
+    if got != want:
+        raise ValueError("the checkpoint's %s has %d pairs where this net (layerNorm, %d normalised layers) has %d: a "
+                         "checkpoint of a net %s layer normalisation or of another shape"
+                         % (what, got, n_ln, want, "without" if got < want else "with more"))
+
+
 class FlatList(list):
     """A stack-shaped list of [w, b] views that remembers the flat buffer it views."""
 
@@ -128,7 +140,7 @@ class NNet:
     def __init__(self, inputDim, outputDim, layerSize, numLayers, maxBatch,
                  train=True, temporalLayer=-1, reg=0.0, maxUtts=1, maxLabels=None,
                  allowTopTemporal=False, device=None, unidirectional=False, numTemporal=1, dropout=0.0,
-                 dropoutSeed=33, cell="relu"):
+                 dropoutSeed=33, cell="relu", layerNorm=False):
         torch = _ctcb.require_cuda()
         self._torch = torch
         self.dev = torch.device("cuda", torch.cuda.current_device() if device is None else device)
@@ -173,9 +185,10 @@ class NNet:
         if cell not in _ctcb.CELLS:
             raise ValueError("cell=%r must be one of %s" % (cell, ", ".join(sorted(_ctcb.CELLS))))
         self.cell = cell
+        self.layerNorm = bool(layerNorm)
         self._cfg = BrnnConfig(inputDim, outputDim, layerSize, numLayers, max(self.temporalLayer, 0), maxBatch,
                                maxUtts, self.maxLabels, float(reg), float(self.maxAct), int(self.unidirectional),
-                               self.numTemporal, _ctcb.CELLS[cell])
+                               self.numTemporal, _ctcb.CELLS[cell], int(self.layerNorm))
         self._h = ctypes.c_void_p()
         check(lib.ctcb_brnn_create(ctypes.byref(self._cfg), ctypes.byref(self._h)))
         self.stack = None
@@ -233,6 +246,8 @@ class NNet:
             if not self.unidirectional:            # rnnet.py:57-61 draws a single recurrent matrix
                 wtb = 2 * scale * np.random.rand(rec_rows, H) - scale
                 host.append([wtb, np.zeros((1, 1))])
+        # [gamma, beta] of every normalised layer, behind everything else: no draw, so the other tensors are unchanged
+        host += [[np.ones((H, 1)), np.zeros((H, 1))] for _ in self.normedLayers()]
 
         self.nparams = int(lib.ctcb_brnn_param_count(ctypes.byref(self._cfg)))
         self.params = torch.zeros(self.nparams, dtype=torch.float32, device=self.dev)
@@ -292,6 +307,14 @@ class NNet:
         if self.cell == "lstm" and self.numTemporal and self.temporalLayer <= i < self.temporalLayer + self.numTemporal:
             return (1 if self.unidirectional else 2) * 4 * self.layerSize
         return self.layerSize if i <= self.numLayers else self.outputDim
+
+    def normedLayers(self):
+        """The layer-normalised hidden layers (layerNorm=True): every ReLU hidden layer 1..numLayers that is not
+        temporal, in the order of their [gamma, beta] pairs at the end of `stack`."""
+        if not self.layerNorm:
+            return []
+        tl, k = self.temporalLayer, self.numTemporal
+        return [i for i in range(1, self.numLayers + 1) if not (k and tl <= i < tl + k)]
 
     def paramCount(self):
         return int(sum(w.numel() + b.numel() for w, b in self.stack))
@@ -479,6 +502,8 @@ class NNet:
         except UnicodeDecodeError:          # checkpoints written by the Python-2 reference
             fid.seek(0)
             stack = pickle.load(fid, encoding="latin1")
+        if self.layerNorm:
+            check_ln_pairs(len(stack), len(self.stack), len(self.normedLayers()), "stack")
         for k, ((w, b), (wi, bi)) in enumerate(zip(self.stack, stack)):
             for x, xi in ((w, wi), (b, bi)):
                 if np.size(xi) != x.numel():

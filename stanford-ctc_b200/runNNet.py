@@ -7,8 +7,8 @@ last_cost, sentinel, train.log), resume through --cfg_file with the step size re
 (runNNet.py:143-166), the fixed seeds 33 (:113-115) and CUDA_DEVICE device selection (:117-120).
 The implementation is organised differently: a declarative flag table, one RunDir helper that owns the
 side files, and separate train/evaluate phases.  Site paths of run_cfg.py / decoder_config.py became
-flags (--runDir, --outDir); new flags: --numTemporal, --cell, --batchSize, --maxUtts, --maxLabels, --dropout, --optimizer,
---beta1, --beta2, --epsilon, --quiet.  Under torchrun the same
+flags (--runDir, --outDir); new flags: --numTemporal, --cell, --layerNorm, --batchSize, --maxUtts, --maxLabels,
+--dropout, --optimizer, --beta1, --beta2, --epsilon, --quiet.  Under torchrun the same
 script trains data-parallel (one process per GPU, one NCCL all-reduce per step).
 """
 import argparse
@@ -48,6 +48,8 @@ FLAGS = [
                             "recurrent (1 = the reference's single temporal layer)"),
     ("cell", str, "relu", "recurrence of the temporal layers: relu (the reference's clipped ReLU) or lstm; a cfg.json "
                           "written without it is relu"),
+    ("layerNorm", None, False, "layer normalisation of the ReLU hidden layers (gamma * layer_norm(z) + beta, then "
+                               "ReLU); a cfg.json written without it has none"),
     ("batchSize", int, 1, "utterances per optimisation step (1 = the reference schedule)"),
     ("maxUtts", int, 0, "utterances per micro-batch per GPU: a larger shard accumulates its gradient over several "
                         "micro-batches (0 = the whole shard, batchSize / number of GPUs rounded up); with --test, "
@@ -199,7 +201,8 @@ def _train(opts, cfg, run_dir, log, rank, world):
     net = rnnet.NNet(opts.inputDim, opts.outputDim, opts.layerSize, opts.numLayers, opts.maxUttLen,
                      temporalLayer=opts.temporalLayer, reg=opts.reg, numTemporal=opts.numTemporal,
                      maxUtts=utterance_capacity(opts, world),
-                     maxLabels=min(opts.maxLabels, opts.maxUttLen), dropout=opts.dropout, cell=opts.cell)
+                     maxLabels=min(opts.maxLabels, opts.maxUttLen), dropout=opts.dropout, cell=opts.cell,
+                     layerNorm=opts.layerNorm)
     net.initParams()
     optimizer = sgd.SGD(net, opts.maxUttLen, alpha=opts.step, optimizer=opts.optimizer, momentum=opts.momentum,
                         batchSize=opts.batchSize, verbose=(rank == 0 and not opts.quiet), beta1=opts.beta1,
@@ -262,7 +265,7 @@ def test(opts, rank=0, world=1):
     logging.getLogger().info("Running on %s" % get_hostname())
     net = rnnet.NNet(trained.inputDim, trained.outputDim, trained.layerSize, trained.numLayers, trained.maxUttLen,
                      temporalLayer=trained.temporalLayer, train=False, maxUtts=max(1, opts.maxUtts),
-                     numTemporal=trained.numTemporal, cell=trained.cell)
+                     numTemporal=trained.numTemporal, cell=trained.cell, layerNorm=trained.layerNorm)
     net.initParams()
     with open(trained.in_file, "rb") as fid:
         pickle.load(fid)                              # optimiser state: not needed here

@@ -18,7 +18,8 @@ launch (inside the CUDA graph of step_device), so step `it` draws the masks of s
 `optimizer` is 'nesterov' (the reference's rule and the default), 'adagrad' (the reference's unfinished branch,
 sgd.py:24-26,143-158, state `gradt`) or 'adam' (state `moment1`, `moment2`; beta1, beta2, epsilon); the rules are stated
 in include/ctcb200.h.  The adaptive rules read the step number t from the same device counter (allocated here when
-the net has no dropout), so graph replays see the current step.
+the net has no dropout), so graph replays see the current step.  The states follow the flat vector, so a net with
+layer normalisation simply has its [gamma, beta] pairs in them too.
 """
 import logging
 import pickle
@@ -134,6 +135,11 @@ class SGD:
             params = pickle.load(fid, encoding="latin1")
         it, costt, expcost, state = params
         states = unpack_state(self.optimizer, state)
+        if getattr(self.model, "layerNorm", False):
+            from nnets.brnnet import check_ln_pairs
+            for name, stack in states.items():
+                check_ln_pairs(len(stack), len(getattr(self, name)), len(self.model.normedLayers()),
+                               "optimiser state %r" % name)
         self.it = it
         self.costt = costt
         self.expcost = expcost
