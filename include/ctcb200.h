@@ -183,7 +183,28 @@ typedef struct ctcb_brnn_config {
                             * this member keeps its meaning), 1 LSTM (below); any other value makes the config invalid. */
     int32_t layerNorm;     /* 0: off (so an initialiser without this member keeps its meaning); 1: layer normalisation of
                             * the ReLU hidden layers (below); any other value makes the config invalid. */
+    int32_t subsample;     /* k: 0 and 1 off (so an initialiser without this member keeps its meaning); k >= 2 runs affine
+                            * map subsampleLayer and everything above it at 1/k of the input frame rate (below); a
+                            * negative value makes the config invalid. */
+    int32_t subsampleLayer; /* L: ignored for k <= 1; with k >= 2 it needs 1 <= L <= numLayers + 1, else the config is
+                             * invalid. */
 } ctcb_brnn_config;
+
+/* Frame subsampling (subsample = k >= 2; not in the reference; cf. Deep Speech 2's striding and the frame stacking of
+ * pyramidal and low-frame-rate CTC models).  Affine map L = subsampleLayer reads k consecutive frames of layer L - 1
+ * concatenated: the input features when L = 1, else that layer's activations as the next map sees them without
+ * subsampling (dropped, normalised, For + Back, ...).  Utterance u has T'_u = ceil(T_u / k) frames from map L upward,
+ * and a call with Tmax has Tmax' = ceil(Tmax / k):
+ *   S[t'] = [x_{k t'}, x_{k t' + 1}, ..., x_{k t' + k - 1}]   (frame-major: unit j of sub-frame m is column m n + j)
+ *   with x_t = 0 for t >= T_u (not the padded row's content), so W_L is rows(L) x k n.
+ * Maps L .. numLayers + 1, their temporal layers (both cells, both directions: the sweeps start and end at T'_u, the
+ * recurrent weight gradients use the rows shifted by B of the reduced-rate buffers), the softmax and the CTC run on
+ * T'_u frames.  probs_out of a forward-only call is [Tmax'][B][outputDim].  The CTC skips an utterance it cannot align
+ * in T'_u frames as it does in T_u.  Dropout keeps its definition with t the frame at the layer's own rate (t' for
+ * layers >= L); layer normalisation is per row and unchanged.  The flat vector keeps its tensor count and order; only
+ * W_L widens.  Backward: dS = (W_L^T delta_L) * (S > 0) where layer L - 1 is a ReLU hidden layer (with dropout's
+ * alpha), unmasked at a temporal layer; then D[t][u][j] = dS[t / k][u][(t % k) n + j] for t < T_u, 0 beyond;
+ * dW_L = delta_L^T S. */
 
 /* Layer normalisation (layerNorm = 1; not in the reference; Ba, Kiros & Hinton 2016).  Hidden layer i is normalised
  * when 1 <= i <= numLayers and i is not temporal -- exactly the layers dropout drops.  Per frame row, H = layerSize:
@@ -234,7 +255,13 @@ int ctcb_brnn_tensor_info(const ctcb_brnn_config *cfg, int idx, int64_t *offset,
  * are sized for the G-row contractions and the 4H x H recurrent weight gradients.
  * layerNorm = 1 appends, behind everything else: per normalised layer z (R*H floats) and the row statistics mu and
  * rstd (R floats each), then ctcb_layernorm_workspace_bytes(R, H) for the parameter-gradient partials.  The forward
- * workspace (ctcb_brnn_forward_workspace_bytes) does not grow: a forward-only call normalises in place. */
+ * workspace (ctcb_brnn_forward_workspace_bytes) does not grow: a forward-only call normalises in place.
+ * subsample = k >= 2 sizes every buffer that only maps >= L use (X_i, D_i, For / Back, c, the LSTM output, z / mu /
+ * rstd, the CTC area at Tmax') for R' = ceil(maxT / k) * maxB rows; the dFor / dBack pairs, the split-K, column-sum and
+ * layer-norm partial areas for their largest user; and appends, behind everything else, S and dS (R' * k * n floats
+ * each, n the width of layer L - 1) and T' (maxB int32).  The forward workspace sizes its slabs, For / Back and c
+ * from the rows of the maps that use them in the same way and appends S and T', so it stays within the training
+ * workspace.  With k <= 1 no offset moves and nothing is appended. */
 size_t ctcb_brnn_workspace_bytes(const ctcb_brnn_config *cfg);
 /* Byte offset, inside the workspace, of a uint32 that the recurrent-sweep kernels set non-zero when an
  * inter-CTA wait timed out (results are then invalid; never a hang).  Callers that synchronise anyway
@@ -257,7 +284,9 @@ size_t ctcb_brnn_forward_workspace_bytes(const ctcb_brnn_config *cfg, size_t *er
  * temporal layer (temporalLayer .. temporalLayer+k-1; Back exists only when bi-directional); with one temporal
  * layer it is ignored.  With dropout on (ctcb_brnn_set_dropout), the ReLU hidden layers' entries hold the dropped and
  * rescaled activations.  cell = 1 only: what = 3 the activated gates (G wide, the same buffer as what = 0 of that layer),
- * 4 / 5 c of the forward / backward direction (H wide). */
+ * 4 / 5 c of the forward / backward direction (H wide).  subsample = k >= 2: the entries of maps >= L (and of their
+ * temporal layers) are [Tmax'][B][width] with that call's Tmax' = ceil(Tmax / k); what = 6 is S, the stacked input of
+ * map L, [Tmax'][B][k n] (`layer` is ignored). */
 int ctcb_brnn_activation_offset(const ctcb_brnn_config *cfg, int what, int layer, size_t *offset, int32_t *width);
 
 int ctcb_brnn_create(const ctcb_brnn_config *cfg, ctcb_brnn **out);
@@ -347,6 +376,17 @@ int ctcb_layernorm_forward_f32(const float *z, float *y, float *mu, float *rstd,
 int ctcb_layernorm_backward_f32(float *delta, const float *z, const float *mu, const float *rstd, const float *gamma,
                                 float *dgamma, float *dbeta, int64_t R, int H, int accumulate, void *workspace,
                                 size_t ws_bytes, void *stream);
+
+/* ---- frame stacking on its own (subsample = k, above) ----------------------------------------------------------
+ * x / d_out are time-major [Tmax][B][n], s_out / ds [ceil(Tmax / k)][B][k n], T_per_utt int32[B] (<= Tmax).
+ * stack  : s_out[t'][u][m n + j] = x[k t' + m][u][j], 0 where k t' + m >= T_u; lens_out (int32[B], may be NULL)
+ *          receives ceil(T_u / k).
+ * unstack: d_out[t][u][j] = ds[t / k][u][(t % k) n + j] for t < T_u, 0 beyond.
+ * Exact copies: 16-byte accesses where n % 4 == 0 and both arrays are 16-byte aligned, else 4-byte ones. */
+int ctcb_frame_stack_f32(const float *x, const int32_t *T_per_utt, int Tmax, int B, int n, int k, float *s_out,
+                         int32_t *lens_out, void *stream);
+int ctcb_frame_unstack_f32(const float *ds, const int32_t *T_per_utt, int Tmax, int B, int n, int k, float *d_out,
+                           void *stream);
 
 /* ---- the time recurrences of the temporal layer on their own (replaces the per-frame loops
  *      brnnet.py:144-152 [mode 0] and brnnet.py:208-224 [mode 1]) -------------------------------

@@ -29,7 +29,8 @@ class BrnnConfig(ctypes.Structure):
                 ("numLayers", ctypes.c_int32), ("temporalLayer", ctypes.c_int32), ("maxT", ctypes.c_int32),
                 ("maxB", ctypes.c_int32), ("maxLabels", ctypes.c_int32), ("reg", ctypes.c_float),
                 ("maxAct", ctypes.c_float), ("unidirectional", ctypes.c_int32), ("numTemporal", ctypes.c_int32),
-                ("cell", ctypes.c_int32), ("layerNorm", ctypes.c_int32)]
+                ("cell", ctypes.c_int32), ("layerNorm", ctypes.c_int32), ("subsample", ctypes.c_int32),
+                ("subsampleLayer", ctypes.c_int32)]
 
 
 _PROTOS = {
@@ -86,6 +87,8 @@ _PROTOS = {
     "ctcb_layernorm_forward_f32": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_int, c_vp]),
     "ctcb_layernorm_backward_f32": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_int, c_int, c_vp, c_sz,
                                             c_vp]),
+    "ctcb_frame_stack_f32": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp]),
+    "ctcb_frame_unstack_f32": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp]),
     "ctcb_debug_sweep_plan": (c_int, [c_int, c_int, c_int, ctypes.POINTER(ctypes.c_int32)]),
     "ctcb_brnn_set_deferred_l2": (c_int, [c_vp, c_int]),
     "ctcb_brnn_apply_l2_f32": (c_int, [c_vp, c_vp, c_vp, c_vp]),

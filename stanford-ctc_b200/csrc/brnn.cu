@@ -42,6 +42,10 @@ int run_layernorm_forward(const float *z, float *y, float *mu, float *rstd, cons
 int run_layernorm_backward(float *d, const float *z, const float *mu, const float *rstd, const float *gamma,
                            float *dgamma, float *dbeta, int64_t R, int H, bool accumulate, float *partial,
                            cudaStream_t st);
+int64_t subsampled_frames(int T, int k);
+int run_frame_stack(const float *x, const int32_t *Tlen, int Tmax, int B, int n, int k, float *s_out, int32_t *lens_out,
+                    cudaStream_t st);
+int run_frame_unstack(const float *ds, const int32_t *Tlen, int Tmax, int B, int n, int k, float *d_out, cudaStream_t st);
 
 // ---- small kernels ---------------------------------------------------------------------------
 // column sums of a row-major R x N matrix: stage 1 partials over row blocks, stage 2 final
@@ -199,6 +203,17 @@ static const char *cfg_error(const ctcb_brnn_config *c, char (&buf)[192]) {
     if (c->layerNorm == 1 && c->layerSize > CTCB_LAYERNORM_MAX_H)
         return say("layerNorm needs layerSize <= %d (the normalisation kernels hold a row on chip); layerSize is %d",
                    CTCB_LAYERNORM_MAX_H, c->layerSize);
+    if (c->subsample < 0)
+        return say("subsample %d is negative (0 and 1: every layer at the input frame rate; k >= 2: maps subsampleLayer "
+                   "and above at 1/k of it)", c->subsample);
+    if (c->subsample >= 2) {
+        if (c->subsampleLayer < 1 || c->subsampleLayer > c->numLayers + 1)
+            return say("subsampleLayer %d is not one of the affine maps 1..%d (numLayers + 1) that subsample %d can "
+                       "start at", c->subsampleLayer, c->numLayers + 1, c->subsample);
+        const int k = c->subsample, n = c->subsampleLayer == 1 ? c->inputDim : c->layerSize;
+        if ((int64_t)k * n > 0x7fffffff || ((int64_t)c->maxT + k - 1) / k * k * c->maxB > 0x7fffffff)
+            return say("subsample %d: %d x %d stacked columns or ceil(maxT / k) * k * maxB rows exceed 2^31 - 1", k, k, n);
+    }
     const bool ok = c->inputDim > 0 && c->outputDim > 1 && c->layerSize > 0 && c->numLayers >= 1 && c->numLayers <= 64 &&
                     c->maxT > 0 && c->maxB > 0 && c->maxLabels >= 0 && c->numTemporal >= 0 &&
                     // a stacked block must lie inside the hidden layers; k <= 1 keeps the silent "no temporal layer" rule below
@@ -229,6 +244,14 @@ static int rec_index(const ctcb_brnn_config *c, int j) {
 static int layer_size(const ctcb_brnn_config *c, int i) {
     return i == 0 ? c->inputDim : (i <= c->numLayers ? c->layerSize : c->outputDim);
 }
+// the subsampling factor of a valid config: 1 when off
+static int eff_k(const ctcb_brnn_config *c) { return c->subsample >= 2 ? c->subsample : 1; }
+// affine map i (1..N+1) and the layer it writes run at the reduced frame rate
+static bool is_reduced(const ctcb_brnn_config *c, int i) { return eff_k(c) > 1 && i >= c->subsampleLayer; }
+// affine map i reads the stacked frames S of layer i - 1
+static bool is_stacked(const ctcb_brnn_config *c, int i) { return eff_k(c) > 1 && i == c->subsampleLayer; }
+// columns of affine map i: the width of layer i - 1, k times that where the map reads S
+static int map_cols(const ctcb_brnn_config *c, int i) { return (is_stacked(c, i) ? eff_k(c) : 1) * layer_size(c, i - 1); }
 static size_t wider_of_H_K(const ctcb_brnn_config *c) {
     return (size_t)(c->layerSize > c->outputDim ? c->layerSize : c->outputDim);
 }
@@ -292,7 +315,7 @@ void net_table(const ctcb_brnn_config *c, NetTable *nt) {
             cc = 1;
         } else if (t < 2 * nl) {
             r = map_rows(c, t / 2 + 1);
-            cc = (t % 2 == 0) ? layer_size(c, t / 2) : 1;
+            cc = (t % 2 == 0) ? map_cols(c, t / 2 + 1) : 1;
         } else if ((t - 2 * nl) % 2 == 0) {
             r = c->cell == 1 ? 4 * c->layerSize : c->layerSize;     // U of an LSTM layer: the four gate blocks
             cc = c->layerSize;
@@ -369,72 +392,93 @@ struct WsLayout {
     // layer-normalised hidden layers only (0 elsewhere): z, and the row statistics of the forward pass; the
     // parameter-gradient partials of the backward pass
     size_t Z[65], Mu[65], Rstd[65], ln_part;
+    // subsampling only (0 elsewhere): the stacked input S of map L, its delta dS (L >= 2), T'_u of the call
+    size_t S, dS, lens;
     size_t total;
 };
 
+// rows of the buffers of map / layer i for maxT x maxB: R, or R' = ceil(maxT / k) * maxB from map L up
+size_t max_rows(const ctcb_brnn_config *c, int i) {
+    return (size_t)(is_reduced(c, i) ? subsampled_frames(c->maxT, eff_k(c)) : c->maxT) * c->maxB;
+}
+// S: R' x k n floats, n the width of layer L - 1
+size_t stacked_bytes(const ctcb_brnn_config *c) {
+    return max_rows(c, c->subsampleLayer) * map_cols(c, c->subsampleLayer) * sizeof(float);
+}
+
 WsLayout ws_layout(const ctcb_brnn_config *c) {
     WsLayout w{};
-    const size_t R = (size_t)c->maxT * c->maxB;
-    const int N = c->numLayers, H = c->layerSize, nt = eff_nt(c);
+    const int N = c->numLayers, H = c->layerSize, nt = eff_nt(c), tl = eff_tl(c);
     const bool uni = (c->unidirectional != 0);
-    const size_t RH = R * H * sizeof(float);
+    // H-wide buffers of layer i; the rows only fall from one map to the next, so the lowest user is the largest one
+    auto RH = [&](int i) { return max_rows(c, i) * H * sizeof(float); };
     size_t off = 0;
-    for (int i = 1; i <= N + 1; ++i) w.X[i] = take(off, R * map_rows(c, i) * sizeof(float));
+    for (int i = 1; i <= N + 1; ++i) w.X[i] = take(off, max_rows(c, i) * map_rows(c, i) * sizeof(float));
     if (nt) {       // all four for every net with a temporal layer, a uni-directional one too
-        w.For[0] = take(off, RH);
-        w.Back[0] = take(off, RH);
-        w.dFor[0] = take(off, RH);
-        w.dBack[0] = take(off, RH);
+        w.For[0] = take(off, RH(tl));
+        w.Back[0] = take(off, RH(tl));
+        w.dFor[0] = take(off, RH(tl));
+        w.dBack[0] = take(off, RH(tl));
     }
     // every further temporal layer keeps its own For (and Back): the BPTT masks and the recurrent weight gradients
     // read them.  The dFor / dBack pairs alternate between consecutive layers, so a stack needs one more pair.
     for (int j = 1; j < nt; ++j) {
-        w.For[j] = take(off, RH);
-        if (!uni) w.Back[j] = take(off, RH);
+        w.For[j] = take(off, RH(tl + j));
+        if (!uni) w.Back[j] = take(off, RH(tl + j));
     }
     if (nt > 1) {
-        w.dFor[1] = take(off, RH);
-        if (!uni) w.dBack[1] = take(off, RH);
+        w.dFor[1] = take(off, RH(tl + 1));
+        if (!uni) w.dBack[1] = take(off, RH(tl + 1));
     }
     const bool lstm = (c->cell == 1);
     for (int j = 0; lstm && j < nt; ++j) {
-        w.Cf[j] = take(off, RH);
+        w.Cf[j] = take(off, RH(tl + j));
         if (!uni) {
-            w.Cb[j] = take(off, RH);
-            w.Out[j] = take(off, RH);
+            w.Cb[j] = take(off, RH(tl + j));
+            w.Out[j] = take(off, RH(tl + j));
         }
     }
     const size_t wide = wider_of_H_K(c);
     // an LSTM layer's D holds dz, G wide
     const size_t wide_g = lstm && (size_t)lstm_rows(c) > wide ? (size_t)lstm_rows(c) : wide;
-    for (int j = 1; j <= N + 1; ++j) w.D[j] = take(off, R * (map_rows(c, j) == layer_size(c, j) ? wide : wide_g) * sizeof(float));
-    w.ctc = take(off, ctcb_ctc_workspace_bytes(c->maxB, c->maxT, c->maxLabels), &w.ctc_bytes);
+    for (int j = 1; j <= N + 1; ++j)
+        w.D[j] = take(off, max_rows(c, j) * (map_rows(c, j) == layer_size(c, j) ? wide : wide_g) * sizeof(float));
+    w.ctc = take(off, ctcb_ctc_workspace_bytes(c->maxB, (int)(max_rows(c, N + 1) / c->maxB), c->maxLabels), &w.ctc_bytes);
     size_t g = 0;
-    const int Rint = (int)R;      // a valid config: R <= GEMM_MAX_M
     auto need = [&](int M_, int N_, int K_) { size_t b = ctcb_gemm_workspace_bytes(M_, N_, K_); if (b > g) g = b; };
     for (int i = 0; i <= N; ++i) {
-        need(Rint, map_rows(c, i + 1), layer_size(c, i));        // forward   X_i . W^T
-        need(Rint, layer_size(c, i), map_rows(c, i + 1));        // backward  delta . W
-        need(map_rows(c, i + 1), layer_size(c, i), Rint);        // weights   delta^T . X_i
+        const int Ri = (int)max_rows(c, i + 1);     // a valid config: R <= GEMM_MAX_M
+        need(Ri, map_rows(c, i + 1), map_cols(c, i + 1));        // forward   X_i . W^T
+        need(Ri, map_cols(c, i + 1), map_rows(c, i + 1));        // backward  delta . W
+        need(map_rows(c, i + 1), map_cols(c, i + 1), Ri);        // weights   delta^T . X_i
     }
     {                                            // recurrent weight gradients (a pair for the bi-directional layer)
-        const size_t b = ctcb_gemm_pair_workspace_bytes(lstm ? 4 * H : H, H, Rint);
+        const size_t b = ctcb_gemm_pair_workspace_bytes(lstm ? 4 * H : H, H, (int)max_rows(c, tl > 0 ? tl : 1));
         if (b > g) g = b;
     }
     w.gemm = take(off, g, &w.gemm_bytes);
     w.gemm2 = take(off, g, &w.gemm2_bytes);
-    w.colsum = take(off, ((R + CS_ROWS_MIN - 1) / CS_ROWS_MIN) * wide_g * sizeof(float));
-    w.colsum2 = take(off, ((R + CS_ROWS_MIN - 1) / CS_ROWS_MIN) * wide_g * sizeof(float));
+    const size_t R1 = max_rows(c, 1);       // the deltas of map 1, the most rows of any
+    w.colsum = take(off, ((R1 + CS_ROWS_MIN - 1) / CS_ROWS_MIN) * wide_g * sizeof(float));
+    w.colsum2 = take(off, ((R1 + CS_ROWS_MIN - 1) / CS_ROWS_MIN) * wide_g * sizeof(float));
     w.l2_scratch = take(off, 8192);
     w.sweep = take_sweep_ws(off, c);
     if (c->layerNorm == 1) {
+        size_t ln_bytes = layernorm_workspace_bytes((int64_t)max_rows(c, N), H);   // laid out with no normalised layer too
         for (int i = 1; i <= N; ++i) {
             if (!is_normed(c, i)) continue;
-            w.Z[i] = take(off, RH);
-            w.Mu[i] = take(off, R * sizeof(float));
-            w.Rstd[i] = take(off, R * sizeof(float));
+            w.Z[i] = take(off, RH(i));
+            w.Mu[i] = take(off, max_rows(c, i) * sizeof(float));
+            w.Rstd[i] = take(off, max_rows(c, i) * sizeof(float));
+            const size_t b = layernorm_workspace_bytes((int64_t)max_rows(c, i), H);
+            if (b > ln_bytes) ln_bytes = b;
         }
-        w.ln_part = take(off, layernorm_workspace_bytes((int64_t)R, H));
+        w.ln_part = take(off, ln_bytes);
+    }
+    if (eff_k(c) > 1) {
+        w.S = take(off, stacked_bytes(c));
+        if (c->subsampleLayer >= 2) w.dS = take(off, stacked_bytes(c));
+        w.lens = take(off, (size_t)c->maxB * sizeof(int32_t));
     }
     w.total = off;
     return w;
@@ -445,25 +489,31 @@ WsLayout ws_layout(const ctcb_brnn_config *c) {
 constexpr int GEMM_ROW_TILE = 128;
 
 // The buffers of a forward-only call: affine map i writes slab i % 2 and reads the other one (or For, the output of
-// the uni-directional temporal layer), so two slabs of the wider of H and K carry the whole stack.  One For (and Back,
-// when bi-directional) serves every temporal layer; 0 where not laid out.
+// the uni-directional temporal layer), so two slabs of the largest map output carry the whole stack.  One For (and
+// Back, when bi-directional) serves every temporal layer; 0 where not laid out.  Each buffer is sized for the rows of
+// the maps that use it (R' from map L up), so a forward-only call fits in the training workspace with subsampling too.
 struct FwdLayout {
     size_t slab[2];
     size_t For, Back, gemm, gemm_bytes;
     size_t Cf, Cb, Out;     // LSTM layers: c of each direction and the bi-directional output, shared as For / Back are
     SweepWs sweep;      // as in ws_layout: the same sweep plan
+    size_t S, lens;     // subsampling only: the stacked input of map L and T'_u
     size_t total;
 };
 
 FwdLayout fwd_layout(const ctcb_brnn_config *c) {
     FwdLayout f{};
-    const size_t R = (size_t)c->maxT * c->maxB;
     const int N = c->numLayers, H = c->layerSize;
     size_t off = 0;
     const bool lstm = (c->cell == 1) && eff_tl(c);
-    const size_t slab = (lstm && (size_t)lstm_rows(c) > wider_of_H_K(c)) ? (size_t)lstm_rows(c) : wider_of_H_K(c);
-    f.slab[0] = take(off, R * slab * sizeof(float));
-    f.slab[1] = take(off, R * slab * sizeof(float));
+    size_t slab = 0;        // floats: X_i of every map i (its rows x its width; G at an LSTM layer)
+    for (int i = 1; i <= N + 1; ++i) {
+        const size_t x = max_rows(c, i) * map_rows(c, i);
+        if (x > slab) slab = x;
+    }
+    f.slab[0] = take(off, slab * sizeof(float));
+    f.slab[1] = take(off, slab * sizeof(float));
+    const size_t R = eff_tl(c) ? max_rows(c, eff_tl(c)) : 0;     // the lowest temporal layer has the most rows
     if (eff_tl(c)) {
         f.For = take(off, R * H * sizeof(float));
         if (!c->unidirectional) f.Back = take(off, R * H * sizeof(float));
@@ -481,12 +531,13 @@ FwdLayout fwd_layout(const ctcb_brnn_config *c) {
     // largest forward need over all such R, capped at the training area (a contraction that falls back there must
     // fall back here too).  The need changes with R only at multiples of the row tile and grows with R once
     // num_sms() row tiles are exceeded (the split counts are then fixed), so those multiples and R itself bound it.
+    // Each map's own rows bound its R (R' from map L up).
     size_t g = 0;
-    const int Rint = (int)R;
-    const int Mtop = (Rint < GEMM_ROW_TILE * num_sms()) ? Rint : GEMM_ROW_TILE * num_sms();
     for (int i = 0; i <= N; ++i) {
+        const int Rint = (int)max_rows(c, i + 1);
+        const int Mtop = (Rint < GEMM_ROW_TILE * num_sms()) ? Rint : GEMM_ROW_TILE * num_sms();
         for (int M = GEMM_ROW_TILE; ; M += GEMM_ROW_TILE) {
-            const size_t b = ctcb_gemm_workspace_bytes(M <= Mtop ? M : Rint, map_rows(c, i + 1), layer_size(c, i));
+            const size_t b = ctcb_gemm_workspace_bytes(M <= Mtop ? M : Rint, map_rows(c, i + 1), map_cols(c, i + 1));
             if (b > g) g = b;
             if (M > Mtop) break;
         }
@@ -494,6 +545,10 @@ FwdLayout fwd_layout(const ctcb_brnn_config *c) {
     const size_t train_area = ws_layout(c).gemm_bytes;
     f.gemm = take(off, g < train_area ? g : train_area, &f.gemm_bytes);
     f.sweep = take_sweep_ws(off, c);
+    if (eff_k(c) > 1) {     // the slabs ping-pong, and map L - 1 wrote the one map L does not
+        f.S = take(off, stacked_bytes(c));
+        f.lens = take(off, (size_t)c->maxB * sizeof(int32_t));
+    }
     f.total = off;
     return f;
 }
@@ -511,6 +566,8 @@ struct FwdBufs {
     unsigned int *counters;
     void *sweep;
     size_t sweep_bytes;
+    float *S;           // subsampling: the stacked input of map L, and T'_u of the call; else null
+    int32_t *lens;
 };
 
 void fwd_bufs(const FwdLayout &f, int N, int nt, char *ws, FwdBufs *m) {
@@ -527,6 +584,8 @@ void fwd_bufs(const FwdLayout &f, int N, int nt, char *ws, FwdBufs *m) {
     m->counters = (unsigned int *)(ws + f.sweep.counters);
     m->sweep = ws + f.sweep.scratch;
     m->sweep_bytes = f.sweep.scratch_bytes;
+    m->S = f.S ? (float *)(ws + f.S) : nullptr;
+    m->lens = f.S ? (int32_t *)(ws + f.lens) : nullptr;
 }
 void train_bufs(const WsLayout &w, int N, int nt, char *ws, FwdBufs *m) {
     for (int i = 1; i <= N + 1; ++i) m->X[i] = (float *)(ws + w.X[i]);
@@ -547,6 +606,8 @@ void train_bufs(const WsLayout &w, int N, int nt, char *ws, FwdBufs *m) {
     m->counters = (unsigned int *)(ws + w.sweep.counters);
     m->sweep = ws + w.sweep.scratch;
     m->sweep_bytes = w.sweep.scratch_bytes;
+    m->S = w.S ? (float *)(ws + w.S) : nullptr;
+    m->lens = w.S ? (int32_t *)(ws + w.lens) : nullptr;
 }
 }  // namespace
 
@@ -591,6 +652,11 @@ struct ctcb_brnn {
     bool lstm() const { return cfg.cell == 1; }
     bool temporal(int i) const { return nt > 0 && i >= tl && i < tl + nt; }
     bool normed(int i) const { return is_normed(&cfg, i); }
+    bool reduced(int i) const { return is_reduced(&cfg, i); }     // map i runs at 1/k of the input frame rate
+    bool stacked(int i) const { return is_stacked(&cfg, i); }     // map i reads S
+    int k() const { return eff_k(&cfg); }
+    int cols(int i) const { return map_cols(&cfg, i); }           // columns of W_i
+    int frames(int i, int Tmax) const { return reduced(i) ? (int)subsampled_frames(Tmax, k()) : Tmax; }
     int size(int i) const { return layer_size(&cfg, i); }
     int rows(int i) const { return map_rows(&cfg, i); }     // width of X_i
     int rec(int j) const { return rec_index(&cfg, j); }
@@ -714,18 +780,26 @@ static int brnn_reduce_rest(ctcb_brnn *h, float *grads, float *stats, cudaStream
 // layer, the softmax into probs_out when given.  Clears the sweep error flag first.  drop: a training call with dropout
 // on masks the output of every ReLU hidden layer in place right behind its contraction, so the next layer, the weight
 // gradients and the ReLU mask of the delta contraction all read the dropped activations.
-static int brnn_forward(ctcb_brnn *h, const float *feats, const int32_t *T_per_utt, int B, int Tmax,
+// With subsampling, map L first stacks its input into S (and T'_u into m.lens); maps L and above run on Tmax' frames.
+static int brnn_forward(ctcb_brnn *h, const float *feats, const int32_t *T_per_utt, int B, int Tmax0,
                         const float *params, float *probs_out, const FwdBufs &m, bool drop, cudaStream_t st) {
     const ctcb_brnn_config &c = h->cfg;
     const int N = c.numLayers, H = c.layerSize, K = c.outputDim;
-    const int64_t R = (int64_t)Tmax * B;
     const bool uni = h->uni();
     // the sweep kernels' error flag (word 0) is cleared once per call, so a forward-sweep timeout survives the BPTT sweep
     CTCB_CUDA_CHECK(cudaMemsetAsync(m.counters, 0, 16 * sizeof(unsigned int), st));
     for (int i = 1; i <= N + 1; ++i) {
         const float *in = (i == 1) ? feats : h->act(m, i - 1);
         const int relu = (i <= N && !h->temporal(i)) ? 1 : 0;
-        const int n_out = h->rows(i), n_in = h->size(i - 1);
+        const int n_out = h->rows(i), n_in = h->cols(i);
+        const int Tmax = h->frames(i, Tmax0);
+        const int64_t R = (int64_t)Tmax * B;
+        const int32_t *Tlen = h->reduced(i) ? m.lens : T_per_utt;
+        if (h->stacked(i)) {
+            ProfScope ps("subsample", st);
+            TRY(run_frame_stack(in, T_per_utt, Tmax0, B, h->size(i - 1), h->k(), m.S, m.lens, st));
+            in = m.S;
+        }
         // a normalised layer: the contraction writes z (into Z in a training call, in place in the slab otherwise),
         // the normalisation kernel the ReLU output X_i
         const bool ln = h->normed(i);
@@ -750,7 +824,7 @@ static int brnn_forward(ctcb_brnn *h, const float *feats, const int32_t *T_per_u
             const int j = i - h->tl, iU = h->rec(j);
             {
             ProfScope ps("sweep_fwd", st);
-            TRY(run_lstm_sweep(0, Tmax, B, H, T_per_utt, m.X[i], h->tensor(params, iU),
+            TRY(run_lstm_sweep(0, Tmax, B, H, Tlen, m.X[i], h->tensor(params, iU),
                                uni ? nullptr : h->tensor(params, iU + 2), m.For[j], m.Back[j], m.Cf[j], m.Cb[j], nullptr,
                                nullptr, m.counters, (float *)m.sweep, st));
             }
@@ -762,7 +836,7 @@ static int brnn_forward(ctcb_brnn *h, const float *feats, const int32_t *T_per_u
             const int j = i - h->tl, iWtf = h->rec(j);
             {
             ProfScope ps("sweep_fwd", st);
-            TRY(run_sweep(0, Tmax, B, H, T_per_utt, m.X[i], h->tensor(params, iWtf),
+            TRY(run_sweep(0, Tmax, B, H, Tlen, m.X[i], h->tensor(params, iWtf),
                           uni ? nullptr : h->tensor(params, iWtf + 2), m.For[j], m.Back[j], nullptr, nullptr, c.maxAct,
                           m.counters, m.sweep, m.sweep_bytes, st));
             }
@@ -773,6 +847,7 @@ static int brnn_forward(ctcb_brnn *h, const float *feats, const int32_t *T_per_u
         }
     }
     if (probs_out) {
+        const int64_t R = (int64_t)h->frames(N + 1, Tmax0) * B;
         const int wpb = 8;
         softmax_rows_kernel<<<(unsigned)((R + wpb - 1) / wpb), wpb * 32, 0, st>>>(m.X[N + 1], probs_out, R, K);
         CTCB_LAUNCH_CHECK();
@@ -794,8 +869,7 @@ struct Step {
     const float *feats, *params;
     const int32_t *T_per_utt;
     float *grads;
-    int B, Tmax;
-    int64_t R;
+    int B, Tmax;            // Tmax of the input; map i runs on T(i) frames
     bool first, last;       // CTCB_PART_FIRST: overwrite the gradients, else add to them; CTCB_PART_LAST: exchange and L2
     bool drop, dp;
     cudaStream_t main, side, caller;
@@ -804,6 +878,10 @@ struct Step {
     const float *P(int idx) const { return h->tensor(params, idx); }
     float *G(int idx) const { return h->tensor(grads, idx); }
     float beta_g() const { return first ? 0.f : 1.f; }      // weight-gradient contractions: C = dW (+ C)
+    // frames, rows and frame counts of map / layer i: Tmax' and T'_u from map L up when subsampled
+    int T(int i) const { return h->frames(i, Tmax); }
+    int64_t R(int i) const { return (int64_t)T(i) * B; }
+    const int32_t *lens(int i) const { return h->reduced(i) ? m.lens : T_per_utt; }
     // the delta of map i; rnnet.py:162-177: the BPTT result of a uni-directional layer is the delta
     // (an LSTM layer's BPTT writes its dz, the delta of its map, into D)
     float *delta(int i) const {
@@ -819,18 +897,18 @@ struct Step {
 // the weight and bias gradients of map i, on the side stream or in the main chain, where its delta is complete
 int Step::weight_grads(int i, bool on_side) const {
     const cudaStream_t st = on_side ? side : main;
-    const float *Xi = (i == 0) ? feats : h->act(m, i);
-    const int n_out = h->rows(i + 1), n_in = h->size(i);
-    // dW = delta^T . X_i   (brnnet.py:196)
+    const float *Xi = h->stacked(i + 1) ? m.S : (i == 0) ? feats : h->act(m, i);
+    const int n_out = h->rows(i + 1), n_in = h->cols(i + 1);
+    // dW = delta^T . X_i   (brnnet.py:196); dW_L = delta^T . S
     {
     ProfScope ps("gemm_dw", st);
-    TRY(ctcb_gemm_f32(1, 0, n_out, n_in, (int)R, 1.f, delta(i), n_out, Xi, n_in, beta_g(), G(2 * i), n_in, nullptr, 0,
-                      nullptr, on_side ? ws + w.gemm2 : m.gemm, on_side ? w.gemm2_bytes : m.gemm_bytes, st));
+    TRY(ctcb_gemm_f32(1, 0, n_out, n_in, (int)R(i + 1), 1.f, delta(i), n_out, Xi, n_in, beta_g(), G(2 * i), n_in, nullptr,
+                      0, nullptr, on_side ? ws + w.gemm2 : m.gemm, on_side ? w.gemm2_bytes : m.gemm_bytes, st));
     }
     // db = row sums of delta   (brnnet.py:200)
     {
     ProfScope ps("colsum", st);
-    TRY(run_colsum(delta(i), R, n_out, buf(on_side ? w.colsum2 : w.colsum), G(2 * i + 1), !first, st));
+    TRY(run_colsum(delta(i), R(i + 1), n_out, buf(on_side ? w.colsum2 : w.colsum), G(2 * i + 1), !first, st));
     }
     if (h->uni() && h->temporal(i + 1) && !h->lstm() && i + 1 - h->tl >= 2)  // the last read of the pair of uni-directional layer i + 1
         CTCB_CUDA_CHECK(cudaEventRecord(h->ev_pair[(i + 1 - h->tl) % 2], side));
@@ -848,6 +926,8 @@ int Step::rec_weight_grads(int j) const {
     CTCB_CUDA_CHECK(cudaEventRecord(h->ev_sweep, main));
     CTCB_CUDA_CHECK(cudaStreamWaitEvent(side, h->ev_sweep, 0));
     ProfScope ps("gemm_dw_rec", side);
+    const int Tmax = T(h->tl + j);
+    const int64_t R = this->R(h->tl + j);
     if (h->lstm()) {     // dU = sum_t dz_t h_prev^T: the dz of both directions lie side by side in the layer's D, G wide
         const int ldz = h->rows(h->tl + j), M = 4 * H;
         const float *dz = buf(w.D[h->tl + j]);
@@ -895,24 +975,32 @@ int Step::backward() const {
         // layers i >= tl > 0: dW/db on the side stream, delta chain + BPTT on the main one
         if (!(tl > 0 && i >= tl)) TRY(weight_grads(i, false));
         if (i == 0) break;
-        const int n_out = h->rows(i + 1), n_in = h->size(i);
+        const int n_out = h->rows(i + 1), n_in = h->cols(i + 1), n = h->size(i);
+        const int64_t R = this->R(i);
         // an LSTM layer's dh goes to the pair; its BPTT writes dz into D[i]
         const bool lstm = h->temporal(i) && h->lstm();
         float *doth = buf(lstm ? w.dFor[(i - tl) % 2] : w.D[i]);
+        // below map L the contraction writes dS, in the layout of S, and dS is unstacked into doth
+        const bool stacked = h->stacked(i + 1);
         // delta <- delta . W, with the ReLU mask sign(hActs[i]) fused (brnnet.py:203-204,235-237).  A dropped
         // layer's X_i is 0 at every dropped unit, so the same mask removes those; the kept ones were scaled by
-        // drop_scale in the forward pass, and so is their delta, through alpha.
-        const float *mask = h->temporal(i) ? nullptr : h->act(m, i);
+        // drop_scale in the forward pass, and so is their delta, through alpha.  S holds X_i stacked, and 0 at the
+        // padding frames, whose delta is 0 either way.
+        const float *mask = h->temporal(i) ? nullptr : stacked ? m.S : h->act(m, i);
         const float alpha = (drop && !h->temporal(i)) ? h->drop_scale : 1.f;
         {
         ProfScope ps("gemm_delta", main);
-        TRY(ctcb_gemm_f32(0, 0, (int)R, n_in, n_out, alpha, delta(i), n_out, P(2 * i), n_in, 0.f, doth, n_in, nullptr, 0,
-                          mask, m.gemm, m.gemm_bytes, main));
+        TRY(ctcb_gemm_f32(0, 0, (int)this->R(i + 1), n_in, n_out, alpha, delta(i), n_out, P(2 * i), n_in, 0.f,
+                          stacked ? buf(w.dS) : doth, n_in, nullptr, 0, mask, m.gemm, m.gemm_bytes, main));
+        }
+        if (stacked) {
+            ProfScope ps("subsample", main);
+            TRY(run_frame_unstack(buf(w.dS), T_per_utt, T(i), B, n, h->k(), doth, main));
         }
         if (h->normed(i)) {     // g -> dz in place, before anything reads D[i]; dgamma / dbeta of the layer
             const int ig = ln_index(&h->cfg, i);
             ProfScope ps("layernorm", main);
-            TRY(run_layernorm_backward(doth, m.Z[i], m.Mu[i], m.Rstd[i], P(ig), G(ig), G(ig + 1), R, n_in, !first,
+            TRY(run_layernorm_backward(doth, m.Z[i], m.Mu[i], m.Rstd[i], P(ig), G(ig), G(ig + 1), R, n, !first,
                                        buf(w.ln_part), main));
         }
         if (!h->temporal(i)) continue;
@@ -925,10 +1013,10 @@ int Step::backward() const {
         {
         ProfScope ps("sweep_bptt", main);
         if (lstm)
-            TRY(run_lstm_sweep(1, Tmax, B, H, T_per_utt, m.X[i], P(iWtf), uni ? nullptr : P(iWtf + 2), nullptr, nullptr,
+            TRY(run_lstm_sweep(1, T(i), B, H, lens(i), m.X[i], P(iWtf), uni ? nullptr : P(iWtf + 2), nullptr, nullptr,
                                m.Cf[j], m.Cb[j], doth, buf(w.D[i]), m.counters, (float *)m.sweep, main));
         else
-            TRY(run_sweep(1, Tmax, B, H, T_per_utt, doth, P(iWtf), uni ? nullptr : P(iWtf + 2), buf(w.dFor[p]),
+            TRY(run_sweep(1, T(i), B, H, lens(i), doth, P(iWtf), uni ? nullptr : P(iWtf + 2), buf(w.dFor[p]),
                           buf(w.dBack[p]), m.For[j], m.Back[j], h->cfg.maxAct, m.counters, m.sweep, m.sweep_bytes, main));
         }
         CTCB_CUDA_CHECK(cudaStreamWaitEvent(side, h->ev_delta[i], 0));
@@ -1011,7 +1099,7 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
     FwdBufs m{};
     train_bufs(w, N, h->nt, ws, &m);
     const bool dp = (h->comm != nullptr) && comm_world(h->comm) > 1;
-    Step s{h, m, w, ws, feats, params, T_per_utt, grads, B, Tmax, R, first, last, h->drop_p > 0.f, dp,
+    Step s{h, m, w, ws, feats, params, T_per_utt, grads, B, Tmax, first, last, h->drop_p > 0.f, dp,
            caller, nullptr, caller};
     const bool overlap = (h->tl > 0);
     if (overlap) {     // fork: the main chain runs on h->hi until the join below
@@ -1024,7 +1112,7 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
     TRY(brnn_forward(h, feats, T_per_utt, B, Tmax, params, probs_out, m, s.drop, s.main));
     {     // brnnet.py:161-175
     ProfScope ps("ctc", s.main);
-    TRY(ctcb_ctc_loss_grad_f32(m.X[N + 1], 0, (int64_t)K, (int64_t)B * K, labels, label_off, T_per_utt, B, Tmax, K,
+    TRY(ctcb_ctc_loss_grad_f32(m.X[N + 1], 0, (int64_t)K, (int64_t)B * K, labels, label_off, s.lens(N + 1), B, s.T(N + 1), K,
                                c.maxLabels, 0, s.buf(w.D[N + 1]), cost_out, skip_out, ws + w.ctc, w.ctc_bytes, s.main));
     }
     TRY(s.backward());
@@ -1110,10 +1198,16 @@ extern "C" size_t ctcb_brnn_sweep_workspace_bytes(int H, int B) { return 4096 + 
 // Test / diagnostic hook: where, inside the workspace, the activations of the LAST ctcb_brnn_cost_and_grad call lie
 // (time-major [Tmax][B][n] with that call's B and Tmax).  what = 0: output of affine map `layer` (1..numLayers+1; the
 // temporal layer's entry holds For + Back, the last one the logits), 1: For, 2: Back (temporal layer only; with
-// several, `layer` says which, and only a bi-directional stack has a Back of every layer).
+// several, `layer` says which, and only a bi-directional stack has a Back of every layer).  Subsampled nets: entries of
+// maps >= L are [Tmax'][B][n]; what = 6: S, the stacked input of map L, k n wide.
 extern "C" int ctcb_brnn_activation_offset(const ctcb_brnn_config *cfg, int what, int layer, size_t *offset, int32_t *width) {
     if (!valid_cfg(cfg) || !offset) return set_error(CTCB_EINVAL, "ctcb_brnn_activation_offset: bad arguments");
     const WsLayout w = ws_layout(cfg);
+    if (what == 6 && eff_k(cfg) > 1) {
+        *offset = w.S;
+        if (width) *width = map_cols(cfg, cfg->subsampleLayer);
+        return CTCB_OK;
+    }
     if (what == 0) {
         if (layer < 1 || layer > cfg->numLayers + 1) return set_error(CTCB_EINVAL, "ctcb_brnn_activation_offset: layer %d", layer);
         *offset = w.X[layer];

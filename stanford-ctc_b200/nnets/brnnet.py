@@ -21,6 +21,10 @@ single contiguous vector.  New, additive surface for the minibatch/data-parallel
     NNet(..., layerNorm=True)                layer normalisation of the ReLU hidden layers (include/ctcb200.h:
                                                 layerNorm): relu(gamma * layer_norm(z) + beta), one [gamma, beta] pair
                                                 per normalised layer appended to `stack`, gamma = 1 and beta = 0 at start
+    NNet(..., subsample=k, subsampleLayer=L) affine map L reads k consecutive frames of the layer below it (W_L is
+                                                rows x k*n) and maps L and above run on ceil(T / k) frames
+                                                (include/ctcb200.h: subsample); the probabilities, the CTC and the
+                                                likelihood arks are at that rate
     NNet(..., dropout=p, dropoutSeed=33)     inverted dropout on the ReLU hidden layers of training calls; the mask
                                                 of an utterance is drawn from (seed, the device counter dropoutStep,
                                                 layer, its index in the step's minibatch, frame, unit)
@@ -140,7 +144,7 @@ class NNet:
     def __init__(self, inputDim, outputDim, layerSize, numLayers, maxBatch,
                  train=True, temporalLayer=-1, reg=0.0, maxUtts=1, maxLabels=None,
                  allowTopTemporal=False, device=None, unidirectional=False, numTemporal=1, dropout=0.0,
-                 dropoutSeed=33, cell="relu", layerNorm=False):
+                 dropoutSeed=33, cell="relu", layerNorm=False, subsample=1, subsampleLayer=1):
         torch = _ctcb.require_cuda()
         self._torch = torch
         self.dev = torch.device("cuda", torch.cuda.current_device() if device is None else device)
@@ -186,9 +190,12 @@ class NNet:
             raise ValueError("cell=%r must be one of %s" % (cell, ", ".join(sorted(_ctcb.CELLS))))
         self.cell = cell
         self.layerNorm = bool(layerNorm)
+        # 0 and 1: off; the config refuses k < 0 and an L outside 1..numLayers+1 with a message (ValueError)
+        self.subsample, self.subsampleLayer = int(subsample), int(subsampleLayer)
         self._cfg = BrnnConfig(inputDim, outputDim, layerSize, numLayers, max(self.temporalLayer, 0), maxBatch,
                                maxUtts, self.maxLabels, float(reg), float(self.maxAct), int(self.unidirectional),
-                               self.numTemporal, _ctcb.CELLS[cell], int(self.layerNorm))
+                               self.numTemporal, _ctcb.CELLS[cell], int(self.layerNorm), self.subsample,
+                               self.subsampleLayer)
         self._h = ctypes.c_void_p()
         check(lib.ctcb_brnn_create(ctypes.byref(self._cfg), ctypes.byref(self._h)))
         self.stack = None
@@ -230,13 +237,15 @@ class NNet:
         order as brnnet.py:38-41 (layer stack) and :66-70 (Wtf then Wtb).  The recurrent matrices of further
         stacked temporal layers are drawn after those, layer by layer, at the same scale.  With cell='lstm' the same
         rule and order apply to the LSTM shapes (a temporal layer's map has G = ndir*4H rows, each U is 4H x H), each
-        matrix at the scale of its own shape."""
+        matrix at the scale of its own shape.  With subsample=k, W_L has k*n columns and fan-in k*n."""
         torch = self._torch
         sizes = [self.inputDim] + self.layerSizes + [self.outputDim]
+        cols = [n * (self.subsample if self.subsample > 1 and i + 1 == self.subsampleLayer else 1)
+                for i, n in enumerate(sizes[:-1])]
         rows = [self._map_rows(i) for i in range(1, self.numLayers + 2)]
-        scales = [np.sqrt(6) / np.sqrt(n + m) for n, m in zip(sizes[:-1], rows)]
+        scales = [np.sqrt(6) / np.sqrt(n + m) for n, m in zip(cols, rows)]
         host = [[np.random.rand(m, n) * 2 * s - s, np.zeros((m, 1))]
-                for n, m, s in zip(sizes[:-1], rows, scales)]
+                for n, m, s in zip(cols, rows, scales)]
         H = self.layerSize
         rec_rows = 4 * H if self.cell == "lstm" else H
         for _ in range(self.numTemporal):
@@ -316,6 +325,10 @@ class NNet:
         tl, k = self.temporalLayer, self.numTemporal
         return [i for i in range(1, self.numLayers + 1) if not (k and tl <= i < tl + k)]
 
+    def frames(self, T):
+        """Frames of the probabilities (and of the CTC) for an utterance of T input frames: ceil(T / k)."""
+        return -(-T // self.subsample) if self.subsample > 1 else T
+
     def paramCount(self):
         return int(sum(w.numel() + b.numel() for w, b in self.stack))
 
@@ -339,7 +352,7 @@ class NNet:
             rank, world = self.dropoutShard or parallel.world_info()[1:]
             check(lib.ctcb_brnn_set_dropout_utts(self._h, rank + world * u0, world))
         B, Tmax = batch.B, batch.Tmax
-        probs = self._probs_view(B, Tmax) if want_probs else None
+        probs = self._probs_view(B, self.frames(Tmax)) if want_probs else None
         cost, skip = out if out is not None else (self._cost[:B], self._skip[:B])
         flags = (_ctcb.PART_FIRST if first else 0) | (_ctcb.PART_LAST if last else 0)
         check(lib.ctcb_brnn_cost_and_grad_part(
@@ -357,8 +370,9 @@ class NNet:
 
     def _forward_device(self, batch):
         """Forward-only call (grads = NULL, the forward workspace layout) on a staged DeviceBatch, whether or not this
-        net trains: enqueues and returns the device probabilities [Tmax][B][K] without synchronising."""
-        probs = self._probs_view(batch.B, batch.Tmax)
+        net trains: enqueues and returns the device probabilities [Tmax'][B][K] (Tmax' = frames(Tmax)) without
+        synchronising."""
+        probs = self._probs_view(batch.B, self.frames(batch.Tmax))
         check(lib.ctcb_brnn_cost_and_grad_part(
             self._h, ptr(batch.d_feats), ptr(batch.d_lens), None, None, batch.B, batch.Tmax, ptr(self.params), None,
             None, None, None, ptr(probs), None, _ctcb.PART_FIRST | _ctcb.PART_LAST, ptr(self._ws), self._ws.numel(),
@@ -422,13 +436,13 @@ class NNet:
 
     def costAndGrad(self, data, labels=None, sentence=None):
         """Reference signature (brnnet.py:117): data is inputDim x T float32; returns (cost, grad, skip)
-        when training, else the K x T float32 softmax outputs."""
+        when training, else the K x T float32 softmax outputs (K x ceil(T / k) with subsample=k)."""
         T = data.shape[1]
         self.setViews(T)
         if not self.train:
             self._batch.pack([data], None).upload()
             probs = self.costAndGradDevice(self._batch)
-            out = np.ascontiguousarray(probs.view(T, self.outputDim).cpu().numpy().T)
+            out = np.ascontiguousarray(probs.view(self.frames(T), self.outputDim).cpu().numpy().T)
             flag = int(self._errflag.item())
             if flag != 0:
                 raise RuntimeError("recurrent sweep: inter-CTA wait timed out (flag %d); results are invalid" % flag)
@@ -441,7 +455,7 @@ class NNet:
 
     def forwardBatch(self, datas):
         """The K x T float32 probabilities that costAndGrad(data) returns with train=False, for every utterance of
-        `datas` (inputDim x T arrays), in input order.  The utterances are sorted by length and cut into micro-batches
+        `datas` (inputDim x T arrays; K x ceil(T / k) with subsample=k), in input order.  The utterances are sorted by length and cut into micro-batches
         of at most maxUtts; micro-batch i+1 is packed into the idle staging buffer while the device computes i, and
         each micro-batch ends in one synchronisation behind the copy of its probabilities and the sweep error flag
         into pinned memory.  Works on training nets too (forward-only calls fit in the training workspace)."""
@@ -472,7 +486,7 @@ class NNet:
                 raise RuntimeError("recurrent sweep: inter-CTA wait timed out (flag %d); results are invalid" % flag)
             p = h_probs.numpy().reshape(probs.shape)
             for j, u in enumerate(idx):
-                out[u] = np.ascontiguousarray(p[:datas[u].shape[1], j, :].T)
+                out[u] = np.ascontiguousarray(p[:self.frames(datas[u].shape[1]), j, :].T)
         return out
 
     def updateParams(self, scale, update):
@@ -504,14 +518,21 @@ class NNet:
             stack = pickle.load(fid, encoding="latin1")
         if self.layerNorm:
             check_ln_pairs(len(stack), len(self.stack), len(self.normedLayers()), "stack")
-        for k, ((w, b), (wi, bi)) in enumerate(zip(self.stack, stack)):
-            for x, xi in ((w, wi), (b, bi)):
-                if np.size(xi) != x.numel():
-                    raise ValueError("checkpoint tensor %d has shape %s where this net (cell=%r) has %s: a checkpoint "
-                                     "of another cell or shape" % (k, tuple(np.shape(xi)), self.cell, tuple(x.shape)))
+        self.check_shapes(stack, self.stack, "stack")
         for (w, b), (wi, bi) in zip(self.stack, stack):
             w.copy_(torch.from_numpy(np.ascontiguousarray(wi, dtype=np.float32).reshape(tuple(w.shape))))
             b.copy_(torch.from_numpy(np.ascontiguousarray(bi, dtype=np.float32).reshape(tuple(b.shape))))
+
+    def check_shapes(self, got, views, what):
+        """Every tensor of a checkpoint's `what` (a list of [w, b]) has the size of this net's: a checkpoint of another
+        cell, subsampling (W_L is rows x k*n) or shape is refused, naming both shapes."""
+        for k, ((w, b), (wi, bi)) in enumerate(zip(views, got)):
+            for x, xi in ((w, wi), (b, bi)):
+                if np.size(xi) != x.numel():
+                    raise ValueError("checkpoint %s tensor %d has shape %s where this net (cell=%r, subsample=%d at map "
+                                     "%d) has %s: a checkpoint of another cell, subsampling or shape"
+                                     % (what, k, tuple(np.shape(xi)), self.cell, max(1, self.subsample),
+                                        self.subsampleLayer, tuple(x.shape)))
 
     def check_grad(self, data, labels, epsilon=1e-3, maxChecks=10, verbose=True):
         """Finite-difference check on a small section of every weight matrix (brnnet.py:279-297).

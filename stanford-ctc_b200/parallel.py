@@ -22,11 +22,12 @@ def rank_files(start_file, num_files, rank, world):
     return shard(range(start_file, num_files + 1), rank, world)
 
 
-def select_step_utterances(data_dict, alis, chunk, max_frames, rank, world, log=None, max_labels=None):
+def select_step_utterances(data_dict, alis, chunk, max_frames, rank, world, log=None, max_labels=None, subsample=1):
     """The utterances of one step that THIS rank computes.  The reference's per-utterance admission rules
     (sgd.py:76-88: skip when longer than the buffers, skip when there are fewer frames than labels) are applied
     to the whole step in the same order on every rank -- two cheap length look-ups per key -- and only then is
-    the list sharded, so all ranks agree on the shards without looking at each other's data."""
+    the list sharded, so all ranks agree on the shards without looking at each other's data.  A net that subsamples
+    by k aligns its labels to ceil(T / k) frames, so that is what the label count is compared with."""
     used = []
     for k in chunk:
         nframes = data_dict[k].shape[1]
@@ -35,9 +36,10 @@ def select_step_utterances(data_dict, alis, chunk, max_frames, rank, world, log=
                 log("SKIPPING utt exceeds batch length (Utterance length %d)." % nframes)
             continue
         nlab = len(alis[k])
-        if nframes < nlab:
+        nout = -(-nframes // subsample) if subsample > 1 else nframes
+        if nout < nlab:
             if log:
-                log("SKIPPING utt frames less than label length (Utterance length %d, Num Labels %d)." % (nframes, nlab))
+                log("SKIPPING utt frames less than label length (Utterance length %d, Num Labels %d)." % (nout, nlab))
             continue
         if max_labels is not None and nlab > max_labels:
             # not a reference rule: the device buffers (and the CTC kernel) hold at most max_labels labels per utterance

@@ -7,7 +7,7 @@ last_cost, sentinel, train.log), resume through --cfg_file with the step size re
 (runNNet.py:143-166), the fixed seeds 33 (:113-115) and CUDA_DEVICE device selection (:117-120).
 The implementation is organised differently: a declarative flag table, one RunDir helper that owns the
 side files, and separate train/evaluate phases.  Site paths of run_cfg.py / decoder_config.py became
-flags (--runDir, --outDir); new flags: --numTemporal, --cell, --layerNorm, --batchSize, --maxUtts, --maxLabels,
+flags (--runDir, --outDir); new flags: --numTemporal, --cell, --layerNorm, --subsample, --subsampleLayer, --batchSize, --maxUtts, --maxLabels,
 --dropout, --optimizer, --beta1, --beta2, --epsilon, --quiet.  Under torchrun the same
 script trains data-parallel (one process per GPU, one NCCL all-reduce per step).
 """
@@ -50,6 +50,10 @@ FLAGS = [
                           "written without it is relu"),
     ("layerNorm", None, False, "layer normalisation of the ReLU hidden layers (gamma * layer_norm(z) + beta, then "
                                "ReLU); a cfg.json written without it has none"),
+    ("subsample", int, 1, "k >= 2: map --subsampleLayer reads k consecutive frames of the layer below it, and it and "
+                          "every layer above run at 1/k of the frame rate (the arks of --test too); 1 = off, and a "
+                          "cfg.json written without it"),
+    ("subsampleLayer", int, 1, "the affine map (1..numLayers+1) that reads the stacked frames when --subsample >= 2"),
     ("batchSize", int, 1, "utterances per optimisation step (1 = the reference schedule)"),
     ("maxUtts", int, 0, "utterances per micro-batch per GPU: a larger shard accumulates its gradient over several "
                         "micro-batches (0 = the whole shard, batchSize / number of GPUs rounded up); with --test, "
@@ -202,7 +206,7 @@ def _train(opts, cfg, run_dir, log, rank, world):
                      temporalLayer=opts.temporalLayer, reg=opts.reg, numTemporal=opts.numTemporal,
                      maxUtts=utterance_capacity(opts, world),
                      maxLabels=min(opts.maxLabels, opts.maxUttLen), dropout=opts.dropout, cell=opts.cell,
-                     layerNorm=opts.layerNorm)
+                     layerNorm=opts.layerNorm, subsample=opts.subsample, subsampleLayer=opts.subsampleLayer)
     net.initParams()
     optimizer = sgd.SGD(net, opts.maxUttLen, alpha=opts.step, optimizer=opts.optimizer, momentum=opts.momentum,
                         batchSize=opts.batchSize, verbose=(rank == 0 and not opts.quiet), beta1=opts.beta1,
@@ -265,7 +269,8 @@ def test(opts, rank=0, world=1):
     logging.getLogger().info("Running on %s" % get_hostname())
     net = rnnet.NNet(trained.inputDim, trained.outputDim, trained.layerSize, trained.numLayers, trained.maxUttLen,
                      temporalLayer=trained.temporalLayer, train=False, maxUtts=max(1, opts.maxUtts),
-                     numTemporal=trained.numTemporal, cell=trained.cell, layerNorm=trained.layerNorm)
+                     numTemporal=trained.numTemporal, cell=trained.cell, layerNorm=trained.layerNorm,
+                     subsample=trained.subsample, subsampleLayer=trained.subsampleLayer)
     net.initParams()
     with open(trained.in_file, "rb") as fid:
         pickle.load(fid)                              # optimiser state: not needed here

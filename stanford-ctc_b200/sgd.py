@@ -140,6 +140,9 @@ class SGD:
             for name, stack in states.items():
                 check_ln_pairs(len(stack), len(getattr(self, name)), len(self.model.normedLayers()),
                                "optimiser state %r" % name)
+        if hasattr(self.model, "check_shapes"):
+            for name, stack in states.items():
+                self.model.check_shapes(stack, getattr(self, name), "optimiser state %r" % name)
         self.it = it
         self.costt = costt
         self.expcost = expcost
@@ -270,7 +273,7 @@ class SGD:
         the idle staging buffer and the asynchronous H2D copy."""
         m = self.model
         used = parallel.select_step_utterances(data_dict, alis, chunk, self.maxBatch, rank, world, log=logging.info,
-                                               max_labels=m.maxLabels)
+                                               max_labels=m.maxLabels, subsample=getattr(m, "subsample", 1))
         datas = [data_dict[k] for k in used]
         labels = [np.array(alis[k], dtype=np.int32) for k in used]     # only this rank's utterances are converted
         batch, pieces = None, None

@@ -28,8 +28,11 @@ def writeLogLikes(loader, nn, fn, outDir, writePickle=False):
             assert data_dict[k].shape[1] < nn.maxBatch, "Need larger max utt length."
         probss = nn.forwardBatch([data_dict[k] for k in keys])
         for i, k in enumerate(keys):
-            writeUttHeader(fid, k, int(sizes[i]), nn.outputDim)
             probs = probss[i]
+            # a net that subsamples by k writes ceil(T / k) rows; otherwise exactly the utterance's frames
+            if getattr(nn, "subsample", 1) <= 1:
+                assert probs.shape[1] == int(sizes[i]), "Probs frames mismatch."
+            writeUttHeader(fid, k, probs.shape[1], nn.outputDim)
             assert probs.dtype == np.float32, "Probs array malformed."
             assert probs.shape[0] == nn.outputDim, "Probs dimensions mismatch."
             with np.errstate(divide='ignore'):
