@@ -1,16 +1,16 @@
 """CPU tests of inverted dropout on the ReLU hidden layers (ctcb_brnn_set_dropout): the NumPy mask of
-tests/dropout_oracle.py against the published Philox4x32-10 answers and for its statistics, the float64 net with dropout
-against central finite differences, the minibatch index g of every utterance however a step is sharded and cut, the
-setters' argument contract through the C ABI (host-only calls, no device), and the runNNet flag.  No compute call is
-made on a device here."""
+tests/net_oracle.py against the published Philox4x32-10 answers and for its statistics, the float64 net with dropout
+back-propagating through given activations as through its own, the minibatch index g of every utterance however a step
+is sharded and cut, the setters' argument contract through the C ABI (host-only calls, no device), and the runNNet flag.
+No compute call is made on a device here."""
 import ctypes
 import math
 
 import numpy as np
 import pytest
 
-import dropout_oracle as do
 import parallel
+from net_oracle import Net, draws, keep_mask, philox4x32_10, threshold_scale
 
 
 # ---------------------------------------------------------------------------------------------------------- Philox
@@ -21,22 +21,22 @@ def test_philox_known_answers():
              ((0x243f6a88, 0x85a308d3, 0x13198a2e, 0x03707344), (0xa4093822, 0x299f31d0),
               (0xd16cfe09, 0x94fdcceb, 0x5001e420, 0x24126ea1))]
     for ctr, key, want in cases:
-        got = do.philox4x32_10(np.array([ctr], dtype=np.uint64), key)[0]
+        got = philox4x32_10(np.array([ctr], dtype=np.uint64), key)[0]
         assert tuple(int(x) for x in got) == want
 
 
 def test_threshold_and_scale():
-    assert do.threshold_scale(0.5) == (2 ** 31, np.float32(2.0))
-    thr, s = do.threshold_scale(0.1)
+    assert threshold_scale(0.5) == (2 ** 31, np.float32(2.0))
+    thr, s = threshold_scale(0.1)
     assert thr == math.floor(float(np.float32(0.1)) * 2 ** 32) and s == np.float32(1.0 / (1.0 - float(np.float32(0.1))))
-    assert do.threshold_scale(0.0) == (0, np.float32(1.0))
-    assert do.threshold_scale(np.nextafter(np.float32(1), np.float32(0)))[0] < 2 ** 32
+    assert threshold_scale(0.0) == (0, np.float32(1.0))
+    assert threshold_scale(np.nextafter(np.float32(1), np.float32(0)))[0] < 2 ** 32
 
 
 @pytest.mark.parametrize("p", [0.05, 0.1, 0.5])
 def test_keep_fraction_is_one_minus_p(p):
     """Over 2500 frames x 4096 units (1.02e7 draws) the kept fraction is within 6 sigma of 1 - p."""
-    keep = do.keep_mask(p, 33, 7, 2, 5, 2500, 4096)
+    keep = keep_mask(p, 33, 7, 2, 5, 2500, 4096)
     n = keep.size
     assert n >= 10 ** 7
     frac = keep.mean()
@@ -54,10 +54,10 @@ def test_masks_of_different_steps_layers_utterances_and_seeds_are_uncorrelated()
     differ and their correlation is within 6 / sqrt(n) of 0."""
     p, T, H = 0.3, 400, 1000
     base = dict(seed=33, step=4, layer=2, g=9)
-    ref = do.keep_mask(p, T=T, H=H, **base)
+    ref = keep_mask(p, T=T, H=H, **base)
     bound = 6.0 / math.sqrt(T * H)
     for key, val in [("step", 5), ("layer", 3), ("g", 10), ("g", 9 + 2 ** 20), ("seed", 34), ("seed", 33 + 2 ** 32)]:
-        other = do.keep_mask(p, T=T, H=H, **dict(base, **{key: val}))
+        other = keep_mask(p, T=T, H=H, **dict(base, **{key: val}))
         assert not np.array_equal(ref, other), key
         assert abs(_corr(ref, other)) < bound, (key, val, _corr(ref, other))
     # frames and units of one mask are not copies of each other either
@@ -66,8 +66,8 @@ def test_masks_of_different_steps_layers_utterances_and_seeds_are_uncorrelated()
 
 def test_units_beyond_the_last_float4_are_drawn_like_the_rest():
     """H not a multiple of 4: the tail units are the first outputs of the last group's draw."""
-    full = do.draws(1, 2, 3, 4, 6, 12)
-    tail = do.draws(1, 2, 3, 4, 6, 10)
+    full = draws(1, 2, 3, 4, 6, 12)
+    tail = draws(1, 2, 3, 4, 6, 10)
     assert np.array_equal(full[:, :10], tail)
 
 
@@ -92,82 +92,20 @@ def test_each_minibatch_utterance_gets_one_index_however_the_step_is_split(n, wo
 
 
 # ---------------------------------------------------------------------------------------- the float64 restatement
-NETS = {     # kwargs of DropoutNet: bi- and uni-directional, the DNN, ReLU layers above and below a (stacked) block
-    "bi": dict(numLayers=3, temporalLayer=2),
-    "uni": dict(numLayers=3, temporalLayer=2, unidirectional=True),
-    "dnn": dict(numLayers=3, temporalLayer=0),
-    "relu_around_one_temporal": dict(numLayers=4, temporalLayer=2),
-    "relu_around_two_temporal": dict(numLayers=5, temporalLayer=2, numTemporal=2),
-}
-
-
-@pytest.mark.parametrize("name", list(NETS))
-def test_dropout_restatement_gradcheck(name):
-    """float64, no float32 hand-offs, p = 0.3, a fixed mask (seed, step, utterance): central differences with eps = 1e-6
-    agree with the analytic gradient to 1e-4 on every weight matrix and bias.  The mask drops units of every ReLU
-    hidden layer and changes the cost."""
-    kw = NETS[name]
-    rng = np.random.RandomState(11)
-    np.random.seed(11)
-    nn = do.DropoutNet(7, 5, 12, maxBatch=9, dtype=np.float64, round_f32=False, reg=1e-3,
-                       dropout=do.Dropout(0.3, seed=5, step=3, g=2), **kw)
-    nn.initParams()
-    data = rng.randn(7, 9)
-    labels = np.array([1, 2, 2, 4], dtype=np.int32)
-    cost, grad, skip = nn.costAndGrad(data, labels)
-    assert not skip
-    grad = [[dw.copy(), db.copy()] for dw, db in grad]
-    hActs = nn.forward(data)[0]
-    dropped = [i for i in range(1, nn.numLayers + 1) if nn.dropped(i)]
-    assert dropped and all((hActs[i] == 0).mean() > 0.3 for i in dropped)
-    drop, nn.dropout = nn.dropout, None
-    assert abs(nn.costAndGrad(data, labels)[0] - cost) > 1e-3
-    nn.dropout = drop
-    eps = 1e-6
-    for pi, (w, b) in enumerate(nn.stack):
-        for _ in range(5):
-            i, j = rng.randint(w.shape[0]), rng.randint(w.shape[1])
-            w[i, j] += eps; cp = nn.costAndGrad(data, labels)[0]
-            w[i, j] -= 2 * eps; cm = nn.costAndGrad(data, labels)[0]
-            w[i, j] += eps
-            assert abs(grad[pi][0][i, j] - (cp - cm) / (2 * eps)) < 1e-4, (pi, i, j)
-        if pi <= nn.numLayers:
-            i = rng.randint(b.shape[0])
-            b[i, 0] += eps; cp = nn.costAndGrad(data, labels)[0]
-            b[i, 0] -= 2 * eps; cm = nn.costAndGrad(data, labels)[0]
-            b[i, 0] += eps
-            assert abs(grad[pi][1][i, 0] - (cp - cm) / (2 * eps)) < 1e-4, (pi, i)
-
-
 def test_back_propagation_through_given_activations_is_the_same():
     """costAndGradGiven on the net's own dropped activations = costAndGrad (the GPU tests feed it the device's)."""
     np.random.seed(2)
-    nn = do.DropoutNet(7, 5, 12, 4, 9, temporalLayer=2, dtype=np.float64, round_f32=False,
-                       dropout=do.Dropout(0.5, seed=1, step=2, g=3))
+    nn = Net(7, 5, 12, 4, 9, temporalLayer=2, round_f32=False, dropout=0.5, dropoutSeed=1)
     nn.initParams()
+    nn.dropoutStep, nn.utt = 2, 3
     data = np.random.RandomState(1).randn(7, 9)
     labels = np.array([1, 3, 2], dtype=np.int32)
     c1, g1, _ = nn.costAndGrad(data, labels)
     g1 = [[a.copy(), b.copy()] for a, b in g1]
-    h, F, Bk, _ = nn.forward(data)
-    c2, g2, _ = nn.costAndGradGiven(data, labels, h[1:], F, Bk)
+    h, temporal, _ = nn.forward(data)
+    c2, g2, _ = nn.costAndGradGiven(data, labels, h[1:], temporal)
     assert c1 == c2
     for (a, b), (x, y) in zip(g1, g2):
-        assert np.array_equal(a, x) and np.array_equal(b, y)
-
-
-def test_without_dropout_it_is_the_stacked_restatement():
-    from stack_oracle import StackNet
-    import recipes
-    datas, labelss = recipes.synth_batch(13, 11, [20, 17], [5, 4], seed=1)
-    out = []
-    for cls in (StackNet, do.DropoutNet):
-        np.random.seed(5)
-        nn = cls(13, 11, 32, 3, 20, temporalLayer=2, reg=1e-3)
-        nn.initParams()
-        out.append(nn.costAndGradBatch(datas, labelss))
-    assert np.array_equal(out[0][0], out[1][0])
-    for (a, b), (x, y) in zip(out[0][1], out[1][1]):
         assert np.array_equal(a, x) and np.array_equal(b, y)
 
 

@@ -3,7 +3,7 @@
   * p = 0 is today's behaviour: a handle given p = 0 (and any utterance map) issues the launches and writes the bits of
     one that never heard of dropout.
   * The mask is bit-exact: every dropped X_i, read back through ctcb_brnn_activation_offset, is exactly 0 where the
-    NumPy mask (tests/dropout_oracle.py) drops; the first hidden layer is bit-identical to the undropped net's times s
+    NumPy mask (tests/net_oracle.py) drops; the first hidden layer is bit-identical to the undropped net's times s
     where it keeps; every activation is within the forward bound of test_configs_gpu.py (1e-4 of the array's largest
     magnitude) of the float64 net with the same mask; the gradient is within 1e-4 per tensor of that net's
     back-propagation through the GPU's own activations, the cost within 1e-4.
@@ -23,8 +23,9 @@ import sys
 import numpy as np
 import pytest
 
-import dropout_oracle as do
 import recipes
+from net_check import bits as _bits, compare, rel as _rel, workspace_activations
+from net_oracle import Net, keep_mask, threshold_scale
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -32,46 +33,21 @@ COST_TOL, FWD_TOL, GRAD_TOL = 1e-4, 1e-4, 1e-4
 D, K = 41, 32
 
 
-def _rel(a, b):
-    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
-    nb = np.linalg.norm(b)
-    if nb == 0.0:
-        return 0.0 if np.linalg.norm(a) == 0.0 else float("inf")
-    return float(np.linalg.norm(a - b) / nb)
-
-
-def _bits(t):
-    return t.detach().cpu().numpy().view(np.uint32)
+def _kwargs(c):
+    """The keyword arguments of nnets.brnnet.NNet and net_oracle.Net that make case c (kind bi / uni / dnn)."""
+    kind = c.get("kind", "bi")
+    return dict(temporalLayer=-1 if kind == "dnn" else c["tl"], numTemporal=c.get("k", 1),
+                unidirectional=kind == "uni", reg=c.get("reg", 0.0))
 
 
 def _net(c, B, p=0.0, seed=33, train=True, maxUtts=None):
-    """The GPU net of case c: kind bi / uni / dnn, with the parameters of np.random.seed(33)."""
+    """The GPU net of case c with the parameters of np.random.seed(33)."""
     import nnets.brnnet
-    import nnets.nnet
-    import nnets.rnnet
     np.random.seed(33)
-    kw = dict(maxUtts=maxUtts or B, maxLabels=c["L"], train=train, dropout=p, dropoutSeed=seed)
-    kind = c.get("kind", "bi")
-    if kind == "dnn":
-        nn = nnets.nnet.NNet(c.get("D", D), c.get("K", K), c["H"], c["N"], c["T"], **kw)
-    elif kind == "uni":
-        nn = nnets.rnnet.NNet(c.get("D", D), c.get("K", K), c["H"], c["N"], c["T"], temporalLayer=c["tl"],
-                              numTemporal=c.get("k", 1), **kw)
-    else:
-        nn = nnets.brnnet.NNet(c.get("D", D), c.get("K", K), c["H"], c["N"], c["T"], temporalLayer=c["tl"],
-                               numTemporal=c.get("k", 1), reg=c.get("reg", 0.0), **kw)
+    nn = nnets.brnnet.NNet(c.get("D", D), c.get("K", K), c["H"], c["N"], c["T"], maxUtts=maxUtts or B,
+                           maxLabels=c["L"], train=train, dropout=p, dropoutSeed=seed, **_kwargs(c))
     nn.initParams()
     return nn
-
-
-def _oracle(c, p, seed, step):
-    np.random.seed(33)
-    on = do.DropoutNet(c.get("D", D), c.get("K", K), c["H"], c["N"], c["T"],
-                       temporalLayer=0 if c.get("kind") == "dnn" else c["tl"], numTemporal=c.get("k", 1),
-                       unidirectional=c.get("kind") == "uni", reg=c.get("reg", 0.0),
-                       dropout=do.Dropout(p, seed=seed, step=step))
-    on.initParams()
-    return on
 
 
 def _batch(c, seed=5):
@@ -86,15 +62,6 @@ def _batch(c, seed=5):
     return lens, recipes.synth_batch(c.get("D", D), c.get("K", K), lens, nlabs, seed=33)
 
 
-def _act(nn, what, layer, B, Tmax):
-    import torch
-    from _ctcb import lib, check
-    off, width = ctypes.c_size_t(), ctypes.c_int32()
-    check(lib.ctcb_brnn_activation_offset(ctypes.byref(nn._cfg), what, layer, ctypes.byref(off), ctypes.byref(width)))
-    n = Tmax * B * width.value
-    return nn._ws[off.value:off.value + 4 * n].view(torch.float32).view(Tmax, B, width.value).cpu().numpy()
-
-
 def _dropped_layers(nn):
     tl, k = nn.temporalLayer, nn.numTemporal
     return [i for i in range(1, nn.numLayers + 1) if not (tl > 0 and tl <= i < tl + k)]
@@ -102,7 +69,7 @@ def _dropped_layers(nn):
 
 def _keep(p, seed, step, layer, gs, Tmax, H):
     """[Tmax][B][H] keep mask of a call whose utterances have minibatch indices gs."""
-    return np.stack([do.keep_mask(p, seed, step, layer, g, Tmax, H) for g in gs], axis=1)
+    return np.stack([keep_mask(p, seed, step, layer, g, Tmax, H) for g in gs], axis=1)
 
 
 # ------------------------------------------------------------------------------------------------ 4. p = 0
@@ -179,26 +146,23 @@ def test_mask_is_bit_exact_and_gradient_matches_float64(name, p, cuda):
     ref = _net(c, B)                                   # the same net without dropout: layer 1 before the mask
     batch = ref._batch.pack(datas, labelss).upload()
     ref.costAndGradDevice(batch)
-    X1_plain = _act(ref, 0, 1, B, Tmax)
+    X1_plain = workspace_activations(ref, B, Tmax)[0, 1]
     del ref
 
     nn = _net(c, B, p=p, seed=seed)
     nn.dropoutStep.fill_(step)
     batch = nn._batch.pack(datas, labelss).upload()
     nn.costAndGradDevice(batch, u0=u0)
-    costs = nn._cost[:B].cpu().numpy().astype(np.float64)
-    skips = nn._skip[:B].cpu().numpy()
-    g_host = [(dw.cpu().numpy().astype(np.float64), db.cpu().numpy().astype(np.float64)) for dw, db in nn.grad]
     assert nn.stats.cpu().numpy()[3] == 0
-    uni, tl, k = c.get("kind") == "uni", nn.temporalLayer, nn.numTemporal
-    X = [None] + [_act(nn, 0, i, B, Tmax) for i in range(1, N + 2)]
-    Fors = [_act(nn, 1, tl + j, B, Tmax) for j in range(k)]
-    Backs = None if uni else [_act(nn, 2, tl + j, B, Tmax) for j in range(k)]
-    if uni:
-        for j in range(k):
-            X[tl + j] = Fors[j]
     assert int(nn.dropoutStep.item()) == step           # a training call reads the counter, never moves it
-    s = do.threshold_scale(p)[1]
+    np.random.seed(33)
+    on = Net(c.get("D", D), c.get("K", K), H, N, c["T"], dropout=p, dropoutSeed=seed, **_kwargs(c))
+    on.initParams()
+    on.dropoutStep = step
+    # 6. forward activations and the gradient through the GPU's own activations, against float64
+    r = compare(nn, on, datas, labelss, lens, utts=gs)
+    X = r["acts"]
+    s = threshold_scale(p)[1]
 
     # 5. the mask, on every row (padded frames included)
     dropped = _dropped_layers(nn)
@@ -206,48 +170,20 @@ def test_mask_is_bit_exact_and_gradient_matches_float64(name, p, cuda):
     zero_frac = {}
     for i in dropped:
         keep = _keep(p, seed, step, i, gs, Tmax, H)
-        assert (X[i][~keep] == 0).all(), i
-        zero_frac[i] = float((X[i] == 0).mean())
+        assert (X[0, i][~keep] == 0).all(), i
+        zero_frac[i] = float((X[0, i] == 0).mean())
         if i == 1:      # layer 1 reads the features: bit for bit the undropped layer times s, or 0
             want = np.where(keep, X1_plain * s, np.float32(0))
-            assert np.array_equal(want.view(np.uint32), X[1].view(np.uint32))
+            assert np.array_equal(want.view(np.uint32), X[0, 1].view(np.uint32))
     del nn
     cuda.cuda.empty_cache()
 
-    # 6. forward activations and the gradient through the GPU's own activations, against float64
-    on = _oracle(c, p, seed, step)
-    on.reg = 0.0          # per utterance without L2 (the GPU's costs exclude it); reg * W is added once below
-    fwd_err, cost_err = 0.0, 0.0
-    tot = [[np.zeros_like(w), np.zeros_like(b)] for w, b in on.stack]
-    for u, (d, l) in enumerate(zip(datas, labelss)):
-        Tu = lens[u]
-        on.dropout.g = gs[u]
-        h, _, _, _ = on.forward(d)
-        for i in range(1, N + 2):
-            o = h[i]
-            fwd_err = max(fwd_err, float(np.abs(X[i][:Tu, u, :].T - o).max() / max(np.abs(o).max(), 1e-30)))
-        c_, g_, s_ = on.costAndGradGiven(d, l, [X[i][:Tu, u, :].T for i in range(1, N + 2)],
-                                         [f[:Tu, u, :].T for f in Fors],
-                                         None if uni else [b_[:Tu, u, :].T for b_ in Backs])
-        assert bool(s_) == bool(skips[u])
-        if s_:
-            continue
-        cost_err = max(cost_err, abs(costs[u] - c_) / abs(c_))
-        for (tw, tb), (gw, gb) in zip(tot, g_):
-            tw += gw
-            tb += gb
-    if c.get("reg", 0.0) > 0:
-        for (w, _), (tw, _) in zip(on.stack, tot):
-            tw += c["reg"] * w
-    given = []
-    for i, ((dw, db), (tw, tb)) in enumerate(zip(g_host, tot)):
-        given.append(_rel(dw, tw))
-        if i <= N:
-            given.append(_rel(db.reshape(-1), tb.reshape(-1)))
+    assert np.array_equal(r["skips"], r["skips_given"])
+    cost_err, fwd_err, given = r["cost_given"], max(r["fwd"]["X"]), r["grad_given"]
     print(json.dumps({"dropout_%s_p%g" % (name, p): dict(config=c, zero_fraction=zero_frac, cost_rel_err_max=cost_err,
                                                          forward_activation_rel_err_max=fwd_err,
                                                          grad_rel_err_given_gpu_activations_max=max(given))}))
-    assert not skips.all()
+    assert not r["skips"].all()
     assert cost_err <= COST_TOL, cost_err
     assert fwd_err <= FWD_TOL, fwd_err
     assert max(given) <= GRAD_TOL, given
@@ -262,17 +198,18 @@ def test_frames_beyond_16_bits(cuda):
     ref = _net(c, 1)
     batch = ref._batch.pack(datas, labelss).upload()
     ref.costAndGradDevice(batch)
-    X1_plain = _act(ref, 0, 1, 1, c["T"])
+    X1_plain = workspace_activations(ref, 1, c["T"])[0, 1]
     del ref
     nn = _net(c, 1, p=p, seed=seed)
     nn.dropoutStep.fill_(step)
     batch = nn._batch.pack(datas, labelss).upload()
     nn.costAndGradDevice(batch)
     keep = _keep(p, seed, step, 1, [0], c["T"], c["H"])
-    want = np.where(keep, X1_plain * do.threshold_scale(p)[1], np.float32(0))
-    assert np.array_equal(want.view(np.uint32), _act(nn, 0, 1, 1, c["T"]).view(np.uint32))
+    want = np.where(keep, X1_plain * threshold_scale(p)[1], np.float32(0))
+    acts = workspace_activations(nn, 1, c["T"])
+    assert np.array_equal(want.view(np.uint32), acts[0, 1].view(np.uint32))
     assert not np.array_equal(keep[:1000], keep[65536:66536])
-    X2 = _act(nn, 0, 2, 1, c["T"])
+    X2 = acts[0, 2]
     assert (X2[~_keep(p, seed, step, 2, [0], c["T"], c["H"])] == 0).all()
 
 
@@ -298,8 +235,9 @@ def _corpus():
 def _step_masks_hold(nn, it, B):
     """X_1 and X_3 of the last step hold the masks of step `it` (dropped units 0), not those of step it - 1."""
     ok, other = True, True
+    acts = workspace_activations(nn, B, nn._batch.Tmax)
     for i in (1, 3):
-        X = _act(nn, 0, i, B, nn._batch.Tmax)
+        X = acts[0, i]
         Tmax = X.shape[0]
         ok &= bool((X[~_keep(nn.dropout, nn.dropoutSeed, it, i, range(B), Tmax, X.shape[2])] == 0).all())
         other &= bool((X[~_keep(nn.dropout, nn.dropoutSeed, it - 1, i, range(B), Tmax, X.shape[2])] == 0).all())
@@ -319,7 +257,7 @@ def test_graph_replays_draw_new_masks_and_equal_eager_steps(cuda):
         cuda.cuda.synchronize()
         assert int(nn.dropoutStep.item()) == opt.it
         assert _step_masks_hold(nn, opt.it, 8), opt.it
-        masks.append(_act(nn, 0, 1, 8, nn._batch.Tmax) == 0)
+        masks.append(workspace_activations(nn, 8, nn._batch.Tmax)[0, 1] == 0)
     assert len(opt._graphs) >= 1
     assert not np.array_equal(masks[-1], masks[-2])
     p_g, v_g = nn.params.cpu().numpy(), opt._vflat.cpu().numpy()
@@ -537,7 +475,7 @@ def test_check_grad_with_dropout(cuda):
     """NNet.check_grad (forward differences in fp32, as test_brnn_gpu.py) with dropout 0.3 on layer 2: costAndGrad
     never advances the counter, so every evaluation sees one mask.  The step is 1e-3, not test_brnn_gpu.py's 1e-2: with
     this mask the cost is curved enough over a 1e-2 step of W1[0, 0] that its forward difference is 0.456 against a
-    derivative of 0.836, and the float64 net of tests/dropout_oracle.py with the same parameters and mask gives the same
+    derivative of 0.836, and the float64 net of tests/net_oracle.py with the same parameters and mask gives the same
     two numbers (0.0122 apart at 1e-3, 0.0012 at 1e-4)."""
     import nnets.brnnet as rnnet
     datas, labelss = recipes.synth_batch(6, 5, [12], [3], seed=4)

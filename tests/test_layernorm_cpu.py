@@ -1,14 +1,10 @@
 """CPU tests of layer normalisation (ctcb_brnn_config.layerNorm = 1): the config contract of the library (tensor table,
-both workspaces, refusal of bad values), the float64 oracle of tests/layernorm_oracle.py against
-torch.nn.functional.layer_norm and against central finite differences, and runNNet's --layerNorm flag."""
+both workspaces, refusal of bad values) and runNNet's --layerNorm flag (the float64 restatement of the net is tested
+in tests/test_net_oracle_cpu.py)."""
 import ctypes
 
-import numpy as np
 import pytest
 
-import recipes
-from dropout_oracle import Dropout
-from layernorm_oracle import LayerNormNet, layer_norm, layer_norm_backward
 from test_lstm_cpu import _training_ws
 
 
@@ -93,15 +89,6 @@ def test_pairs_go_behind_every_old_tensor(net):
     for (o0, r0, c0), (o1, _, _) in zip(on, on[1:]):
         assert o1 == (o0 + r0 * c0 + 3) // 4 * 4
     assert lib.ctcb_brnn_param_count(ctypes.byref(_cfg(*net))) == (on[-1][0] + H + 3) // 4 * 4
-    shapes = [tuple(w.shape) for w, _ in _oracle(net).stack]
-    assert [(r, c) for _, r, c in on[0::2]] == shapes
-
-
-def _oracle(net, **kw):
-    D, K, H, N, tl, T, B, L, uni, nt, cell = net
-    o = LayerNormNet(D, K, H, N, T, tl, nt, cell=("lstm" if cell else "relu"), unidirectional=bool(uni), **kw)
-    o.initParams()
-    return o
 
 
 @pytest.mark.parametrize("net", NETS)
@@ -143,93 +130,6 @@ def test_entry_points_check_their_arguments():
     assert lib.ctcb_layernorm_forward_f32(None, None, None, None, None, None, 4, 9000, None) == -1
     assert "H = 9000" in lib.ctcb_last_error().decode()
     assert lib.ctcb_layernorm_backward_f32(None, None, None, None, None, None, None, 4, 64, 0, None, 0, None) == -1
-
-
-# ------------------------------------------------------------------------------------------- the oracle
-def test_oracle_normalisation_is_torch_layer_norm():
-    torch = pytest.importorskip("torch")
-    rng = np.random.RandomState(1)
-    for H, T, shift in ((13, 9, 0.0), (64, 5, 300.0), (7, 3, -2.0)):
-        z = rng.randn(H, T) * rng.rand(1, T) * 3 + shift
-        z[:, 0] = 0.25                               # a constant frame: var = 0
-        gamma, beta = rng.randn(H, 1), rng.randn(H, 1)
-        xh, rstd = layer_norm(z)
-        ref = torch.nn.functional.layer_norm(torch.from_numpy(z.T.copy()), (H,), torch.from_numpy(gamma[:, 0].copy()),
-                                             torch.from_numpy(beta[:, 0].copy()), eps=1e-5).numpy().T
-        assert np.allclose(gamma * xh + beta, ref, rtol=1e-9, atol=1e-9)
-        # and its backward against torch's autograd
-        zt = torch.from_numpy(z.T.copy()).requires_grad_()
-        gt = torch.from_numpy(gamma[:, 0].copy()).requires_grad_()
-        bt = torch.from_numpy(beta[:, 0].copy()).requires_grad_()
-        g = rng.randn(H, T)
-        torch.nn.functional.layer_norm(zt, (H,), gt, bt, eps=1e-5).backward(torch.from_numpy(g.T.copy()))
-        dz, dgamma, dbeta = layer_norm_backward(g, gamma, xh, rstd)
-        assert np.allclose(dz, zt.grad.numpy().T, rtol=1e-10, atol=1e-10)
-        assert np.allclose(dgamma[:, 0], gt.grad.numpy(), rtol=1e-10, atol=1e-12)
-        assert np.allclose(dbeta[:, 0], bt.grad.numpy(), rtol=1e-10, atol=1e-12)
-
-
-FD_NETS = {
-    "bi": dict(tl=2, k=1), "uni": dict(tl=2, k=1, uni=True), "dnn": dict(tl=0, k=0), "stack2": dict(tl=2, k=2, N=4),
-    "lstm": dict(tl=2, k=1, cell="lstm"), "bi_dropout": dict(tl=2, k=1, p=0.3),
-}
-
-
-@pytest.mark.parametrize("name", list(FD_NETS))
-def test_oracle_gradient_matches_central_differences(name):
-    """float64 throughout, reg > 0, gamma and beta moved off their initial values: every tensor's analytic gradient at
-    a few entries (gamma and beta at every entry) against (f(w + e) - f(w - e)) / 2e."""
-    c = FD_NETS[name]
-    D, K, H, N = 5, 6, 6, c.get("N", 3)
-    np.random.seed(11)
-    drop = Dropout(c["p"], seed=5) if "p" in c else None
-    net = LayerNormNet(D, K, H, N, 8, c["tl"], c["k"], dropout=drop, cell=c.get("cell", "relu"), reg=1e-3,
-                       unidirectional=bool(c.get("uni")), round_f32=False)
-    net.initParams()
-    rng = np.random.RandomState(2)
-    for i in net.normedLayers():
-        gamma, beta = net.stack[net.ln_index(i)]
-        gamma += 0.3 * rng.randn(*gamma.shape)
-        beta += 0.3 * rng.randn(*beta.shape)
-    datas, labels = recipes.synth_batch(D, K, [7, 4], [3, 2], seed=3)
-    _, grad, skips = net.costAndGradBatch(datas, labels)
-    assert not skips.any()
-    eps = 1e-6
-    base = N + 1 + net.numTemporal * net.nrec
-    ln_pairs = range(base, len(net.stack))
-    assert len(ln_pairs) == len(net.normedLayers()) > 0
-    for ti, (w, b) in enumerate(net.stack):
-        for x, gx in ((w, grad[ti][0]), (b, grad[ti][1])):
-            if N < ti < base and x is b:        # the recurrent matrices' dummies take no part
-                continue
-            idxs = list(np.ndindex(x.shape)) if ti in ln_pairs else \
-                [tuple(rng.randint(0, s) for s in x.shape) for _ in range(3)]
-            for idx in idxs:
-                old = x[idx]
-                x[idx] = old + eps
-                cp = net.costAndGradBatch(datas, labels)[0].sum() + net.regcost
-                x[idx] = old - eps
-                cm = net.costAndGradBatch(datas, labels)[0].sum() + net.regcost
-                x[idx] = old
-                num = (cp - cm) / (2 * eps)
-                assert abs(num - gx[idx]) <= 1e-6 * max(1.0, abs(num)), (name, ti, idx, num, gx[idx])
-
-
-def test_oracle_without_layer_norm_is_the_dropout_oracle():
-    from dropout_oracle import DropoutNet
-    D, K, H, N = 5, 6, 6, 3
-    np.random.seed(4)
-    a = LayerNormNet(D, K, H, N, 8, 2, 1, layerNorm=False, reg=1e-3)
-    a.initParams()
-    np.random.seed(4)
-    b = DropoutNet(D, K, H, N, 8, 2, 1, reg=1e-3)
-    b.initParams()
-    datas, labels = recipes.synth_batch(D, K, [7, 4], [3, 2], seed=3)
-    ca, ga, _ = a.costAndGradBatch(datas, labels)
-    cb, gb, _ = b.costAndGradBatch(datas, labels)
-    assert np.allclose(ca, cb, rtol=1e-12)
-    for (x, y), (u, v) in zip(ga, gb):
-        assert np.allclose(x, u, rtol=1e-10, atol=1e-14) and np.allclose(y, v, rtol=1e-10, atol=1e-14)
 
 
 # ------------------------------------------------------------------------------------------- runNNet

@@ -11,13 +11,12 @@
                C u rstd (|gh| + mean|gh| + |xh| (mean|gh xh| + |b|)), b = mean(gh xh), C_FWD again; dgamma / dbeta
                sum over rows in chunks of rpp rows, then parts / 8 strided terms and 8: depth D = rpp + parts/8 + 8,
                |err| <= 2 (D + 4) u sum_r |g xh| (|g| for dbeta).
-2. The whole net against tests/layernorm_oracle.py: cost, every activation, and every gradient tensor against the
-   oracle's back-propagation through the GPU's own activations (relative Frobenius <= 1e-4), for bi-, uni-directional,
-   DNN, stacked, LSTM and dropout nets with mixed utterance lengths.
+2. The whole net against tests/net_oracle.py (compared by tests/net_check.py): cost, every activation, and every
+   gradient tensor against the oracle's back-propagation through the GPU's own activations (relative Frobenius <= 1e-4),
+   for bi-, uni-directional, DNN, stacked, LSTM and dropout nets with mixed utterance lengths.
 3. Consistency: micro-batches and shards, graph replay, forward-only probabilities, reruns; Adam and Nesterov; toFile /
    fromFile and the pair-count check; runNNet --layerNorm end to end; check_grad and a finite difference of beta.
 Each comparison prints its measured errors as one JSON line (pytest -s)."""
-import ctypes
 import io
 import json
 import os
@@ -27,30 +26,13 @@ import numpy as np
 import pytest
 
 import recipes
-from dropout_oracle import Dropout
-from layernorm_oracle import LayerNormNet
+from net_check import bits as _bits, compare, rel as _rel
+from net_oracle import Net
 
 pytestmark = pytest.mark.gpu
 U32 = 2.0 ** -24
 C_FWD = 64.0
 FWD_TOL, GRAD_TOL = 1e-4, 1e-4
-
-
-def _rel(a, b):
-    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
-    nb = np.linalg.norm(b)
-    if nb == 0.0:
-        return 0.0 if np.linalg.norm(a) == 0.0 else float("inf")
-    return float(np.linalg.norm(a - b) / nb)
-
-
-def _relmax(a, b):
-    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
-    return float(np.max(np.abs(a - b)) / max(np.max(np.abs(b)), 1e-30))
-
-
-def _bits(t):
-    return t.detach().cpu().numpy().view(np.uint32)
 
 
 def _ratio(err, bound):
@@ -196,17 +178,15 @@ NETS = {
 }
 
 
+def _kwargs(c, reg=0.0):
+    """The keyword arguments of nnets.brnnet.NNet and net_oracle.Net that make net c."""
+    return dict(temporalLayer=c["tl"] or -1, numTemporal=max(1, c["k"]), reg=reg, unidirectional=bool(c.get("uni")),
+                cell=c.get("cell", "relu"), dropout=c.get("p", 0.0), layerNorm=True)
+
+
 def _gpu_net(c, B, reg=0.0, train=True):
     import nnets.brnnet as brnnet
-    return brnnet.NNet(D_IN, K, c["H"], c["N"], c["T"], temporalLayer=c["tl"] or -1, maxUtts=B, maxLabels=c["L"],
-                       numTemporal=max(1, c["k"]), train=train, reg=reg, unidirectional=bool(c.get("uni")),
-                       cell=c.get("cell", "relu"), dropout=c.get("p", 0.0), layerNorm=True)
-
-
-def _oracle(c, reg=0.0):
-    drop = Dropout(c["p"], seed=33, step=0) if "p" in c else None
-    return LayerNormNet(D_IN, K, c["H"], c["N"], c["T"], c["tl"], c["k"], dropout=drop, cell=c.get("cell", "relu"),
-                        reg=reg, unidirectional=bool(c.get("uni")))
+    return brnnet.NNet(D_IN, K, c["H"], c["N"], c["T"], maxUtts=B, maxLabels=c["L"], train=train, **_kwargs(c, reg))
 
 
 def _ragged(c, seed=5):
@@ -218,26 +198,17 @@ def _ragged(c, seed=5):
     return lens, recipes.synth_batch(D_IN, K, lens, nlabs, seed=33)
 
 
-def _ws_array(nn, what, layer, Tmax, B):
-    from _ctcb import lib, check
-    off, w = ctypes.c_size_t(), ctypes.c_int32()
-    check(lib.ctcb_brnn_activation_offset(ctypes.byref(nn._cfg), what, layer, ctypes.byref(off), ctypes.byref(w)))
-    n = Tmax * B * w.value
-    return nn._ws[off.value:off.value + 4 * n].view(nn._torch.float32).cpu().numpy().reshape(Tmax, B, w.value)
-
-
 @pytest.mark.parametrize("name", list(NETS))
 def test_layer_norm_net_matches_float64_oracle(name, cuda):
     c = NETS[name]
     lens, (datas, labelss) = _ragged(c)
-    B, Tmax, N, tl, k = c["B"], max(lens), c["N"], c["tl"], c["k"]
-    uni, lstm = bool(c.get("uni")), c.get("cell") == "lstm"
+    B, N = c["B"], c["N"]
     reg = 1e-3
     np.random.seed(21)
     nn = _gpu_net(c, B, reg=reg)
     nn.initParams()
     np.random.seed(21)
-    on = _oracle(c, reg)
+    on = Net(D_IN, K, c["H"], N, c["T"], **_kwargs(c, reg))
     on.initParams()
     assert nn.normedLayers() == on.normedLayers() and len(nn.normedLayers()) > 0
     for (w, b), (ow, ob) in zip(nn.stack, on.stack):        # the same draws, shapes and order; gamma 1, beta 0
@@ -250,55 +221,11 @@ def test_layer_norm_net_matches_float64_oracle(name, cuda):
             v = (on.stack[kk][t] + 0.2 * rng.randn(*on.stack[kk][t].shape)).astype(np.float32)
             on.stack[kk][t] = v.astype(np.float64)
             nn.stack[kk][t].copy_(cuda.from_numpy(v))
-    costs, grad, skips = nn.costAndGradBatch(datas, labelss)
-    o_costs, o_grad, o_skips = on.costAndGradBatch(datas, labelss)
-    assert np.array_equal(skips, o_skips) and not skips.any()
-    cost_err = float(np.max(np.abs(costs - o_costs) / np.abs(o_costs)))
-    temporal = list(range(tl, tl + k)) if tl else []
-    X = {i: _ws_array(nn, 0, i, Tmax, B) for i in range(1, N + 2)}
-    hF = {i: _ws_array(nn, 1, i, Tmax, B) for i in temporal}
-    hB = {i: _ws_array(nn, 2, i, Tmax, B) for i in temporal} if not uni else {}
-    cF = {i: _ws_array(nn, 4, i, Tmax, B) for i in temporal} if lstm else {}
-    cB = {i: _ws_array(nn, 5, i, Tmax, B) for i in temporal} if lstm and not uni else {}
-    fwd = 0.0
-    given = [[np.zeros_like(w), np.zeros_like(b)] for w, b in on.stack]
-    for u in range(B):
-        Tu = lens[u]
-        if on.dropout is not None:
-            on.dropout.g = u
-        hActs, _, _ = on.forward(datas[u])
-        g_acts, g_temp = [], []
-        for i in range(1, N + 2):
-            act = X[i][:Tu, u].T
-            if i in temporal and lstm:          # X holds the gates; the output is h_f + h_b
-                gh = [hF[i][:Tu, u].T] + ([] if uni else [hB[i][:Tu, u].T])
-                gc = [cF[i][:Tu, u].T] + ([] if uni else [cB[i][:Tu, u].T])
-                g_temp.append((X[i][:Tu, u].T, gc, gh))
-                act = sum(x.astype(np.float64) for x in gh)
-            elif i in temporal:                 # a uni-directional layer's output is For
-                g_temp.append((hF[i][:Tu, u].T, None if uni else hB[i][:Tu, u].T))
-                if uni:
-                    act = hF[i][:Tu, u].T
-            g_acts.append(act)
-            fwd = max(fwd, _relmax(act, hActs[i]))
-        on.reg = 0.0
-        _, gg, _ = on.costAndGradGiven(datas[u], labelss[u], g_acts, g_temp)
-        on.reg = reg
-        for (a, b), (x, y) in zip(given, gg):
-            a += x
-            b += y
-    for kk in on.weight_indices():
-        given[kk][0] += reg * on.stack[kk][0]
-    grad_err, grad_elem, plain = [], [], []
-    for (dw, db), (gw, gb), (ow, ob) in zip(grad, given, o_grad):
-        for x, y, z in ((dw, gw, ow), (db, gb, ob)):
-            x = x.cpu().numpy().astype(np.float64).reshape(y.shape)
-            if not np.any(y):
-                assert not np.any(x)
-                continue
-            grad_err.append(_rel(x, y))
-            grad_elem.append(_relmax(x, y))
-            plain.append(_rel(x, z))
+    nn.costAndGradBatch(datas, labelss)
+    r = compare(nn, on, datas, labelss, lens)
+    assert np.array_equal(r["skips"], r["skips_own"]) and not r["skips"].any()
+    cost_err, fwd = r["cost_own"], max(r["fwd"]["X"])
+    grad_err, grad_elem, plain = r["grad_given"], r["grad_given_elem"], r["grad_plain"]
     print(json.dumps({"layernorm_net_" + name: dict(cost=cost_err, fwd=fwd, grad_given_frob_max=max(grad_err),
                                                     grad_given_elem_max=max(grad_elem), grad_plain_frob_max=max(plain))}))
     assert cost_err <= FWD_TOL and fwd <= FWD_TOL

@@ -1,14 +1,9 @@
-"""CPU tests of the LSTM cell (ctcb_brnn_config.cell = 1): the float64 restatement of the net (tests/lstm_oracle.py)
-against torch.nn.LSTM and against central finite differences, and the config contract the library reports -- an
-invalid cell, the tensor shapes, the training workspace against its formula, the runNNet flag and an old cfg.json.
-No compute call is made on a device here."""
+"""CPU tests of the LSTM cell (ctcb_brnn_config.cell = 1): the config contract the library reports -- an invalid
+cell, the tensor layout, the training workspace against its formula, the runNNet flag and an old cfg.json (the float64
+restatement of the net is tested in tests/test_net_oracle_cpu.py).  No compute call is made on a device here."""
 import ctypes
 
-import numpy as np
 import pytest
-
-import recipes
-from lstm_oracle import LstmNet, lstm_direction, lstm_direction_bptt
 
 
 def _cfg(D, K, H, N, tl, T, B, L, uni=0, nt=1, cell=1):
@@ -27,84 +22,6 @@ def _layout(cfg):
     return out
 
 
-# ------------------------------------------------------------------------------------------- oracle vs torch
-@pytest.mark.parametrize("uni", [True, False])
-def test_oracle_matches_torch_lstm(uni):
-    """One LSTM layer of the oracle against torch.nn.LSTM in float64 (bias_hh = 0), per utterance of a ragged batch:
-    the forward h of each direction, and the gradients of sum(out * R) w.r.t. the input, W_ih, b_ih and W_hh."""
-    torch = pytest.importorskip("torch")
-    rng = np.random.RandomState(5)
-    n, H = 7, 6
-    ndir = 1 if uni else 2
-    lstm = torch.nn.LSTM(n, H, bidirectional=not uni).double()
-    with torch.no_grad():
-        for name, p in lstm.named_parameters():
-            p.copy_(torch.from_numpy(rng.uniform(-0.6, 0.6, tuple(p.shape))))
-            if name.startswith("bias_hh"):
-                p.zero_()
-    sfx = ["", "_reverse"][:ndir]
-    W = np.concatenate([getattr(lstm, "weight_ih_l0" + s).detach().numpy() for s in sfx])
-    b = np.concatenate([getattr(lstm, "bias_ih_l0" + s).detach().numpy() for s in sfx])
-    Us = [getattr(lstm, "weight_hh_l0" + s).detach().numpy() for s in sfx]
-    for T in (1, 2, 9, 5):      # the utterances of a ragged batch, each run at its own length
-        x = rng.randn(n, T)
-        Rw = rng.randn(H, T)
-        xt = torch.from_numpy(x.T[:, None, :].copy()).requires_grad_(True)
-        out, _ = lstm(xt)
-        out = out[:, 0, :].T     # [ndir*H][T]
-        loss = sum((out[d * H:(d + 1) * H] * torch.from_numpy(Rw)).sum() for d in range(ndir))
-        loss.backward()
-        pre = W.dot(x) + b[:, None]
-        dz_all = []
-        for d in range(ndir):
-            gates, c, h = lstm_direction(pre[d * 4 * H:(d + 1) * 4 * H], Us[d], reverse=(d == 1))
-            np.testing.assert_allclose(h, out[d * H:(d + 1) * H].detach().numpy(), rtol=1e-12, atol=1e-13)
-            dz, dU = lstm_direction_bptt(Rw, gates, c, h, Us[d], reverse=(d == 1))
-            np.testing.assert_allclose(dU, getattr(lstm, "weight_hh_l0" + sfx[d]).grad.numpy(), rtol=1e-10, atol=1e-12)
-            dz_all.append(dz)
-        dz = np.concatenate(dz_all)
-        np.testing.assert_allclose(dz.dot(x.T), np.concatenate([getattr(lstm, "weight_ih_l0" + s).grad.numpy()
-                                                                for s in sfx]), rtol=1e-10, atol=1e-12)
-        np.testing.assert_allclose(dz.sum(axis=1), np.concatenate([getattr(lstm, "bias_ih_l0" + s).grad.numpy()
-                                                                   for s in sfx]), rtol=1e-10, atol=1e-12)
-        np.testing.assert_allclose(W.T.dot(dz), xt.grad.numpy()[:, 0, :].T, rtol=1e-10, atol=1e-12)
-        lstm.zero_grad()
-
-
-# ------------------------------------------------------------------------------------------- finite differences
-@pytest.mark.parametrize("k", [1, 2, 3])
-@pytest.mark.parametrize("uni", [False, True])
-def test_oracle_gradient_matches_central_differences(k, uni):
-    """k stacked LSTM layers between ReLU layers (one below, one above), float64 throughout, reg > 0: every tensor's
-    analytic gradient at a few entries against (f(w + e) - f(w - e)) / 2e."""
-    D, K, H = 5, 6, 4
-    N = k + 2
-    np.random.seed(11)
-    net = LstmNet(D, K, H, N, temporalLayer=2, numTemporal=k, reg=1e-3, unidirectional=uni, round_f32=False)
-    net.initParams()
-    for w, _ in net.stack:          # larger weights than the init, so the cells saturate somewhat
-        w *= 2.0
-    datas, labels = recipes.synth_batch(D, K, [7, 4], [3, 2], seed=3)
-    _, grad, skips = net.costAndGradBatch(datas, labels)
-    assert not skips.any()
-    rng = np.random.RandomState(0)
-    eps = 1e-6
-    for ti, (w, b) in enumerate(net.stack):
-        for x, gx in ((w, grad[ti][0]), (b, grad[ti][1])):
-            if ti > N and x is b:       # the recurrent matrices' dummies take no part
-                continue
-            for _ in range(3):
-                idx = tuple(rng.randint(0, s) for s in x.shape)
-                old = x[idx]
-                x[idx] = old + eps
-                cp = net.costAndGradBatch(datas, labels)[0].sum() + net.regcost
-                x[idx] = old - eps
-                cm = net.costAndGradBatch(datas, labels)[0].sum() + net.regcost
-                x[idx] = old
-                num = (cp - cm) / (2 * eps)
-                assert abs(num - gx[idx]) <= 1e-6 * max(1.0, abs(num)), (ti, idx, num, gx[idx])
-
-
 # ------------------------------------------------------------------------------------------- the config contract
 def test_invalid_cell_is_refused_with_a_message():
     import _ctcb
@@ -120,12 +37,12 @@ def test_invalid_cell_is_refused_with_a_message():
 
 @pytest.mark.parametrize("uni", [0, 1])
 @pytest.mark.parametrize("nt", [1, 2, 3])
-def test_tensor_shapes_follow_the_oracle(uni, nt):
+def test_lstm_tensor_layout(uni, nt):
+    """The tensors are packed at 16-byte alignment, and only the temporal maps and the recurrent matrices differ from
+    the relu config's (test_net_oracle_cpu.py checks every shape against the float64 restatement)."""
     D, K, H, N, tl = 13, 11, 70, 4, 2
     cfg = _cfg(D, K, H, N, tl, 60, 8, 20, uni, nt)
     lay = _layout(cfg)
-    shapes = LstmNet(D, K, H, N, tl, nt, unidirectional=bool(uni)).shapes()
-    assert [(r, c) for _, r, c in lay] == shapes
     for (o0, r0, c0), (o1, _, _) in zip(lay, lay[1:]):
         assert o1 == (o0 + r0 * c0 + 3) // 4 * 4
     from _ctcb import lib

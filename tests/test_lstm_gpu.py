@@ -1,16 +1,16 @@
 """GPU tests of the LSTM cell (ctcb_brnn_config.cell = 1) on one H100.
 
-The sweep alone (ctcb_lstm_sweep_f32) against the float64 recurrence of tests/lstm_oracle.py computed from the
-kernel's own float32 inputs, element-wise: every forward output x (gates, c, h) satisfies |x - x64| <= C u S with
-u = 2^-24 and S the sum of the magnitudes of the terms that make it, the float64 of the step computed from the GPU's
-own state of the step before (S = 1 + |pre| + |U| |h_prev| for a gate, |f c_prev| + |i g| for c, |o| for h); the BPTT
-output dz, which carries dc from step to step inside the kernel, against the float64 BPTT of the GPU's own forward
-activations with S = max(1, max |dz64|) over the case.  Then the whole net against lstm_oracle.LstmNet: per-utterance
-cost, logits, gates, c and h of every LSTM layer relative to their largest magnitude (<= 1e-4), every gradient tensor
-against the oracle's back-propagation through the GPU's own activations (relative Frobenius <= 1e-4, and the largest
-element-wise error relative to the tensor's largest magnitude printed).  Then micro-batches, two emulated shards,
-graph replay, forward-only probabilities, dropout on the ReLU layers, Adam, runNNet end to end and a width the device
-cannot hold.  Each comparison prints its measured errors as one JSON line (pytest -s)."""
+The sweep alone (ctcb_lstm_sweep_f32) against the float64 recurrence of tests/net_oracle.py computed from the kernel's
+own float32 inputs, element-wise: every forward output x (gates, c, h) satisfies |x - x64| <= C u S with u = 2^-24 and S
+the sum of the magnitudes of the terms that make it, the float64 of the step computed from the GPU's own state of the
+step before (S = 1 + |pre| + |U| |h_prev| for a gate, |f c_prev| + |i g| for c, |o| for h); the BPTT output dz, which
+carries dc from step to step inside the kernel, against the float64 BPTT of the GPU's own forward activations with S =
+max(1, max |dz64|) over the case. Then the whole net against net_oracle.Net (tests/net_check.py): per-utterance cost,
+logits, gates, c and h of every LSTM layer relative to their largest magnitude (<= 1e-4), every gradient tensor against
+the oracle's back-propagation through the GPU's own activations (relative Frobenius <= 1e-4, and the largest
+element-wise error relative to the tensor's largest magnitude printed). Then micro-batches, two emulated shards, graph
+replay, forward-only probabilities, dropout on the ReLU layers, Adam, runNNet end to end and a width the device cannot
+hold. Each comparison prints its measured errors as one JSON line (pytest -s)."""
 import ctypes
 import json
 import os
@@ -19,29 +19,13 @@ import numpy as np
 import pytest
 
 import recipes
-from lstm_oracle import LstmNet, lstm_direction, lstm_direction_bptt
+from net_check import bits as _bits, compare, rel as _rel, workspace_activations
+from net_oracle import Net, lstm_direction_bptt
 
 pytestmark = pytest.mark.gpu
 U32 = 2.0 ** -24
 C_FWD, C_BPTT = 8.0, 32.0     # measured on an H100 80GB HBM3 at 700 W: at most 2.2 and 3.8
 COST_TOL, FWD_TOL, GRAD_TOL = 1e-4, 1e-4, 1e-4
-
-
-def _rel(a, b):
-    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
-    nb = np.linalg.norm(b)
-    if nb == 0.0:
-        return 0.0 if np.linalg.norm(a) == 0.0 else float("inf")
-    return float(np.linalg.norm(a - b) / nb)
-
-
-def _relmax(a, b):
-    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
-    return float(np.max(np.abs(a - b)) / max(np.max(np.abs(b)), 1e-30))
-
-
-def _bits(t):
-    return t.detach().cpu().numpy().view(np.uint32)
 
 
 def _sig(z):
@@ -137,11 +121,14 @@ NETS = {
 }
 
 
-def _gpu_net(c, B, reg=0.0, train=True, dropout=0.0):
+def _kwargs(c, reg=0.0):
+    """The keyword arguments of nnets.brnnet.NNet and net_oracle.Net that make net c."""
+    return dict(temporalLayer=c["tl"], numTemporal=c["k"], reg=reg, unidirectional=bool(c.get("uni")), cell="lstm")
+
+
+def _gpu_net(c, B, reg=0.0, train=True):
     import nnets.brnnet as brnnet
-    return brnnet.NNet(D, K, c["H"], c["N"], c["T"], temporalLayer=c["tl"], maxUtts=B, maxLabels=c["L"],
-                       numTemporal=c["k"], train=train, reg=reg, unidirectional=bool(c.get("uni")), cell="lstm",
-                       dropout=dropout)
+    return brnnet.NNet(D, K, c["H"], c["N"], c["T"], maxUtts=B, maxLabels=c["L"], train=train, **_kwargs(c, reg))
 
 
 def _batch(c, seed=5):
@@ -156,80 +143,32 @@ def _batch(c, seed=5):
     return lens, recipes.synth_batch(D, K, lens, nlabs, seed=33)
 
 
-def _ws_array(nn, what, layer, Tmax, B):
-    from _ctcb import lib, check
-    off, w = ctypes.c_size_t(), ctypes.c_int32()
-    check(lib.ctcb_brnn_activation_offset(ctypes.byref(nn._cfg), what, layer, ctypes.byref(off), ctypes.byref(w)))
-    n = Tmax * B * w.value
-    return nn._ws[off.value:off.value + 4 * n].view(nn._torch.float32).cpu().numpy().reshape(Tmax, B, w.value)
-
-
 @pytest.mark.parametrize("name", list(NETS))
 def test_lstm_net_matches_float64_oracle(name, cuda):
     c = NETS[name]
     lens, (datas, labelss) = _batch(c)
-    B, Tmax, H, N, tl, k = c["B"], max(lens), c["H"], c["N"], c["tl"], c["k"]
+    B, H, N, tl, k = c["B"], c["H"], c["N"], c["tl"], c["k"]
     uni = bool(c.get("uni"))
     reg = 1e-3
     np.random.seed(21)
     nn = _gpu_net(c, B, reg=reg)
     nn.initParams()
     np.random.seed(21)
-    on = LstmNet(D, K, H, N, tl, k, reg=reg, unidirectional=uni)
+    on = Net(D, K, H, N, c["T"], **_kwargs(c, reg))
     on.initParams()
     for (w, b), (ow, ob) in zip(nn.stack, on.stack):        # the same draws, shapes and order
         assert np.array_equal(w.cpu().numpy(), ow.astype(np.float32)) and tuple(b.shape) == ob.shape
-    costs, grad, skips = nn.costAndGradBatch(datas, labelss)
-    o_costs, o_grad, o_skips = on.costAndGradBatch(datas, labelss)
-    assert np.array_equal(skips, o_skips) and not skips.any()
-    cost_err = float(np.max(np.abs(costs - o_costs) / np.abs(o_costs)))
-    # what the GPU left in its workspace
-    X = {i: _ws_array(nn, 0, i, Tmax, B) for i in range(1, N + 2)}
-    hF = {i: _ws_array(nn, 1, i, Tmax, B) for i in range(tl, tl + k)}
-    cF = {i: _ws_array(nn, 4, i, Tmax, B) for i in range(tl, tl + k)}
-    hB = {i: _ws_array(nn, 2, i, Tmax, B) for i in range(tl, tl + k)} if not uni else {}
-    cB = {i: _ws_array(nn, 5, i, Tmax, B) for i in range(tl, tl + k)} if not uni else {}
-    fwd = dict(logits=0.0, gates=0.0, c=0.0, h=0.0)
-    given = [[np.zeros_like(w), np.zeros_like(b)] for w, b in on.stack]
-    for u in range(B):
-        Tu = lens[u]
-        for i in range(tl, tl + k):         # padded frames of every LSTM buffer are exactly 0
-            for arr in [X[i], hF[i], cF[i]] + ([hB[i], cB[i]] if not uni else []):
-                assert not np.any(arr[Tu:, u]), "padded frame not 0"
-        hActs, cells, _ = on.forward(datas[u])
-        fwd["logits"] = max(fwd["logits"], _relmax(X[N + 1][:Tu, u].T, hActs[N + 1]))
-        g_acts, g_cells = [], []
-        for i in range(1, N + 2):
-            if tl <= i < tl + k:
-                j = i - tl
-                gates, cs, hs = cells[j]
-                gh = [hF[i][:Tu, u].T] + ([] if uni else [hB[i][:Tu, u].T])
-                gc = [cF[i][:Tu, u].T] + ([] if uni else [cB[i][:Tu, u].T])
-                fwd["gates"] = max(fwd["gates"], _relmax(X[i][:Tu, u].T, gates))
-                fwd["c"] = max(fwd["c"], max(_relmax(a, b) for a, b in zip(gc, cs)))
-                fwd["h"] = max(fwd["h"], max(_relmax(a, b) for a, b in zip(gh, hs)))
-                g_cells.append((X[i][:Tu, u].T, gc, gh))
-                g_acts.append(sum(x.astype(np.float64) for x in gh))
-            else:
-                g_acts.append(X[i][:Tu, u].T)
-        on.reg = 0.0
-        _, gg, _ = on.costAndGradGiven(datas[u], labelss[u], g_acts, g_cells)
-        on.reg = reg
-        for (a, b), (x, y) in zip(given, gg):
-            a += x
-            b += y
-    for (a, _), (w, _) in zip(given, on.stack):
-        a += reg * w
-    grad_err, grad_elem, plain = [], [], []
-    for (dw, db), (gw, gb), (ow, ob) in zip(grad, given, o_grad):
-        for x, y, z in ((dw, gw, ow), (db, gb, ob)):
-            x = x.cpu().numpy().astype(np.float64).reshape(y.shape)
-            if not np.any(y):
-                assert not np.any(x)
-                continue
-            grad_err.append(_rel(x, y))
-            grad_elem.append(_relmax(x, y))
-            plain.append(_rel(x, z))
+    nn.costAndGradBatch(datas, labelss)
+    r = compare(nn, on, datas, labelss, lens)
+    assert np.array_equal(r["skips"], r["skips_own"]) and not r["skips"].any()
+    cost_err = r["cost_own"]
+    acts = r["acts"]
+    for u in range(B):                      # padded frames of every LSTM buffer are exactly 0
+        for i in range(tl, tl + k):
+            for what in (0, 1, 4) + (() if uni else (2, 5)):
+                assert not np.any(acts[what, i][lens[u]:, u]), "padded frame not 0"
+    fwd = dict(logits=r["fwd"]["X"][N], gates=r["fwd"]["gates"], c=r["fwd"]["c"], h=r["fwd"]["h"])
+    grad_err, grad_elem, plain = r["grad_given"], r["grad_given_elem"], r["grad_plain"]
     print(json.dumps({"lstm_net_" + name: dict(cost=cost_err, fwd=fwd, grad_given_frob_max=max(grad_err),
                                                grad_given_elem_max=max(grad_elem), grad_plain_frob_max=max(plain))}))
     assert cost_err <= COST_TOL
@@ -359,29 +298,27 @@ def test_dropout_masks_only_the_relu_layers_of_an_lstm_net(cuda):
     ref.costAndGradBatch(datas, labelss)
     B, Tmax = 8, 60
     lens = [d.shape[1] for d in datas]
-    X = {i: _ws_array(nn, 0, i, Tmax, B) for i in range(1, 6)}
-    Xr = {i: _ws_array(ref, 0, i, Tmax, B) for i in (1, 3, 4)}
+    acts = workspace_activations(nn, B, Tmax)
+    ref_acts = workspace_activations(ref, B, Tmax)
+    X = {i: acts[0, i] for i in range(1, 6)}
+    Xr = {i: ref_acts[0, i] for i in (1, 3, 4)}
     kept = X[1] != 0        # layer 1 sees the same input in both nets: its kept units are the undropped ones times 2
     assert np.array_equal(X[1][kept], Xr[1][kept] * np.float32(2.0))
     for i in (1, 3, 4):     # about half of each ReLU layer's non-zero units are dropped
         frac = (X[i] != 0).sum() / (Xr[i] != 0).sum()
         assert 0.35 < frac < 0.65, (i, frac)
     # the oracle through the GPU's activations, the dropped layers' deltas scaled by 1/(1-p)
-    on = LstmNet(13, 11, 64, 4, 2, 1)
+    on = Net(13, 11, 64, 4, 60, temporalLayer=2, cell="lstm", dropout=p)
     on.stack = [[w.cpu().numpy().astype(np.float64), b.cpu().numpy().astype(np.float64)] for w, b in nn.stack]
-    hF, hB = _ws_array(nn, 1, 2, Tmax, B), _ws_array(nn, 2, 2, Tmax, B)
-    cF, cB = _ws_array(nn, 4, 2, Tmax, B), _ws_array(nn, 5, 2, Tmax, B)
     tot = [[np.zeros_like(w), np.zeros_like(b)] for w, b in on.stack]
     for u in range(B):
-        Tu = lens[u]
-        acts = [X[i][:Tu, u].T for i in range(1, 6)]
-        acts[1] = (hF[:Tu, u].T.astype(np.float64) + hB[:Tu, u].T)
-        hActs = [np.asarray(datas[u], np.float64)] + [np.asarray(a, np.float64) for a in acts]
-        cells = [(X[2][:Tu, u].T.astype(np.float64), [cF[:Tu, u].T.astype(np.float64), cB[:Tu, u].T.astype(np.float64)],
-                  [hF[:Tu, u].T.astype(np.float64), hB[:Tu, u].T.astype(np.float64)])]
-        _, g, _ = _given_with_scale(on, labelss[u], hActs, cells, 1.0 / (1.0 - p))
-        for (a, b), (x, y) in zip(tot, g):
-            a += x
+        a = lambda what, i: acts[what, i][:lens[u], u].T        # noqa: E731
+        hs = [a(1, 2), a(2, 2)]
+        g_acts = [a(0, i) for i in range(1, 6)]
+        g_acts[1] = hs[0].astype(np.float64) + hs[1]
+        _, g, _ = on.costAndGradGiven(datas[u], labelss[u], g_acts, [(a(0, 2), [a(4, 2), a(5, 2)], hs)])
+        for (a_, b), (x, y) in zip(tot, g):
+            a_ += x
             b += y
     errs = [_rel(dw.cpu().numpy().reshape(a.shape), a) for (dw, _), (a, _) in zip(nn.grad, tot) if np.any(a)]
     inf_nn = _small(8, 0.0, False, k=1, dropout=p)
@@ -391,38 +328,6 @@ def test_dropout_masks_only_the_relu_layers_of_an_lstm_net(cuda):
     assert max(errs) <= GRAD_TOL, errs
     assert all(np.array_equal(a, b) for a, b in zip(pr, pr0))
     torch.cuda.synchronize()
-
-
-def _given_with_scale(net, labels, hActs, cells, scale):
-    """LstmNet's back-propagation through given activations with the delta of every ReLU hidden layer masked and
-    multiplied by `scale`: the gradient of the net with inverted dropout, whose dropped units are 0 in hActs."""
-    from oracle import brnn_oracle
-    H = net.layerSize
-    probs = net._softmax(hActs[-1])
-    cost, deltas, skip = brnn_oracle._ctc_loss(np.asfortranarray(probs.astype(np.float64)),
-                                               np.asarray(labels, dtype=np.int32))
-    grad = [[np.zeros_like(w), np.zeros_like(b)] for w, b in net.stack]
-    deltasIn = deltas.astype(np.float32).astype(np.float64)
-    for i in range(net.numLayers, -1, -1):
-        w = net.stack[i][0]
-        grad[i][0] = deltasIn.dot(hActs[i].T)
-        grad[i][1] = deltasIn.sum(axis=1)[:, None]
-        if i == 0:
-            break
-        deltasOut = w.T.dot(deltasIn)
-        if net.temporal(i):
-            gates, cs, hs = cells[i - net.temporalLayer]
-            dzs = []
-            for d, idx in enumerate(net.rec(i - net.temporalLayer)[:net.ndir]):
-                dz, dU = lstm_direction_bptt(deltasOut, gates[d * 4 * H:(d + 1) * 4 * H], cs[d], hs[d],
-                                             net.stack[idx][0], reverse=(d == 1))
-                grad[idx][0] = dU
-                dzs.append(dz)
-            deltasOut = np.concatenate(dzs)
-        else:
-            deltasOut = deltasOut * (hActs[i] > 0.0) * scale
-        deltasIn = deltasOut
-    return cost, grad, skip
 
 
 # ------------------------------------------------------------------------------------------------ end to end

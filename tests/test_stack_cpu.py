@@ -1,15 +1,9 @@
 """CPU tests of stacked temporal layers (ctcb_brnn_config.numTemporal): the flat layout and both workspace sizes the
-library reports, the rejection of blocks that do not fit, the float64 restatement of the stacked net (tests/
-stack_oracle.py) against central finite differences and, at one layer, against the pinned oracle, and the runNNet
-flag.  No compute call is made on a device here."""
+library reports, the rejection of blocks that do not fit, and the runNNet flag (the float64 restatement of the
+stacked net is tested in tests/test_net_oracle_cpu.py).  No compute call is made on a device here."""
 import ctypes
 
-import numpy as np
 import pytest
-
-import recipes
-from oracle import brnn_oracle
-from stack_oracle import StackNet
 
 # (D, K, H, N, tl, T, B, L, uni)
 NETS = [(41, 62, 512, 2, 1, 200, 32, 30, 0), (13, 11, 64, 3, 2, 60, 8, 20, 1), (41, 32, 1024, 3, 2, 800, 8, 100, 0),
@@ -134,77 +128,6 @@ def test_blocks_that_do_not_fit_are_rejected(tl, k, N):
     assert lib.ctcb_brnn_num_tensors(ctypes.byref(_cfg(13, 11, 64, 3, 1, 60, 8, 20, 0, -1))) == 0
     # the block may end at the top hidden layer
     assert lib.ctcb_brnn_num_tensors(ctypes.byref(_cfg(13, 11, 64, 3, 2, 60, 8, 20, 0, 2))) == 2 * 4 + 8
-
-
-# ---------------------------------------------------------------------------------------- the float64 restatement
-@pytest.mark.parametrize("uni", [False, True])
-@pytest.mark.parametrize("k", [2, 3])
-def test_stacked_restatement_gradcheck(k, uni):
-    """The recipe of rnnetcpu.py:181-190 / tests/test_oracle.py: float64, no float32 hand-offs, central differences
-    with eps = 1e-6, |analytic - numeric| < 1e-4, here with numLayers = 4, temporalLayer = 1 and k stacked layers.
-    Every matrix is probed, the recurrent ones of each layer included, with L2 on."""
-    rng = np.random.RandomState(3 + k)
-    np.random.seed(3 + k)
-    nn = StackNet(7, 5, 12, 4, 9, temporalLayer=1, numTemporal=k, reg=1e-3, dtype=np.float64, round_f32=False,
-                  unidirectional=uni)
-    nn.initParams()
-    assert len(nn.stack) == 5 + k * (1 if uni else 2)
-    data = rng.randn(7, 9)
-    labels = np.array([1, 2, 2, 4], dtype=np.int32)
-    cost, grad, skip = nn.costAndGrad(data, labels)
-    assert not skip
-    grad = [[dw.copy(), db.copy()] for dw, db in grad]
-    eps = 1e-6
-    worst = 0.0
-    for pi, (w, b) in enumerate(nn.stack):
-        for _ in range(6):
-            i, j = rng.randint(w.shape[0]), rng.randint(w.shape[1])
-            w[i, j] += eps; cp = nn.costAndGrad(data, labels)[0]
-            w[i, j] -= 2 * eps; cm = nn.costAndGrad(data, labels)[0]
-            w[i, j] += eps
-            d = abs(grad[pi][0][i, j] - (cp - cm) / (2 * eps))
-            worst = max(worst, d)
-            assert d < 1e-4, (pi, i, j, d)
-        if pi < 5:     # the biases of the affine maps as well
-            i = rng.randint(b.shape[0])
-            b[i, 0] += eps; cp = nn.costAndGrad(data, labels)[0]
-            b[i, 0] -= 2 * eps; cm = nn.costAndGrad(data, labels)[0]
-            b[i, 0] += eps
-            assert abs(grad[pi][1][i, 0] - (cp - cm) / (2 * eps)) < 1e-4
-    # the recurrent gradients are not trivially zero (the probes above would then prove nothing)
-    assert all(np.abs(grad[5 + r][0]).max() > 1e-6 for r in range(k * (1 if uni else 2)))
-
-
-@pytest.mark.parametrize("uni", [False, True])
-def test_stacked_restatement_at_one_layer_is_the_pinned_oracle(uni):
-    datas, labelss = recipes.synth_batch(13, 11, [20, 17, 9], [5, 4, 3], seed=1)
-    outs = []
-    for cls in ("stack", "oracle"):
-        np.random.seed(5)
-        if cls == "stack":
-            nn = StackNet(13, 11, 32, 3, 20, temporalLayer=2, numTemporal=1, reg=1e-3 * (not uni), unidirectional=uni)
-        else:
-            nn = brnn_oracle.NNet(13, 11, 32, 3, 20, temporalLayer=2, reg=1e-3 * (not uni), unidirectional=uni)
-        nn.initParams()
-        costs, grad, skips = nn.costAndGradBatch(datas, labelss)
-        outs.append((costs, [np.array(x) for g in grad for x in g], nn.stack))
-    (c1, g1, s1), (c2, g2, s2) = outs
-    assert all(np.array_equal(a[0], b[0]) for a, b in zip(s1, s2))      # same draws, same order
-    assert np.allclose(c1, c2, rtol=1e-12, atol=0)
-    for a, b in zip(g1, g2):
-        assert np.abs(a - b).max() <= 1e-12 * max(1.0, np.abs(b).max())
-
-
-def test_stacked_restatement_draws_the_extra_matrices_after_todays():
-    np.random.seed(33)
-    one = StackNet(13, 11, 16, 4, 20, temporalLayer=1, numTemporal=1)
-    one.initParams()
-    np.random.seed(33)
-    three = StackNet(13, 11, 16, 4, 20, temporalLayer=1, numTemporal=3)
-    three.initParams()
-    assert len(three.stack) == len(one.stack) + 4
-    for (a, _), (b, _) in zip(one.stack, three.stack):
-        assert np.array_equal(a, b)
 
 
 # ---------------------------------------------------------------------------------------------------- runNNet

@@ -1,17 +1,17 @@
 """GPU tests of stacked temporal layers (numTemporal = k > 1) on one H100.
 
-Parity against the float64 restatement (tests/stack_oracle.py) with the criteria of test_configs_gpu.py: per-utterance
-cost <= 1e-4; every activation array, For_j / Back_j of each temporal layer included (read back through
-ctcb_brnn_activation_offset), within 1e-4 of the oracle's relative to its largest magnitude; every gradient tensor
-within 1e-4 (Frobenius) of the oracle's back-propagation through the GPU's own activations; the plain comparison
-(oracle with its own float64 masks) printed and bounded: 1e-4 where the sweeps run on FFMA, 1e-2 at H = 1024, where
-float32 noise flips the ReLU / clip mask of units near a kink (test_configs_gpu.py) and each flip reaches the layers
-below through every stacked recurrence (measured 3.2e-3 and 5.4e-3, while the gradients given the GPU's activations
-agree to 1.4e-5).  The cases cover each sweep family, checked with
-ctcb_debug_sweep_plan, bi- and uni-directional layers, k = 2 and 3, a ragged batch, T = 1 and a block that ends at the
-top hidden layer.  Then: the bits of k = 1 against a config without the field, forward-only against training
-probabilities, micro-batches, shards with L2, CUDA-graph replay, two ranks over NCCL, and runNNet end to end.
-Each comparison prints its measured errors as one JSON line (pytest -s)."""
+Parity against the float64 restatement (tests/net_oracle.py, compared by tests/net_check.py) with the criteria of
+test_configs_gpu.py: per-utterance cost <= 1e-4; every activation array, For_j / Back_j of each temporal layer included
+(read back through ctcb_brnn_activation_offset), within 1e-4 of the oracle's relative to its largest magnitude; every
+gradient tensor within 1e-4 (Frobenius) of the oracle's back-propagation through the GPU's own activations; the plain
+comparison (oracle with its own float64 masks) printed and bounded: 1e-4 where the sweeps run on FFMA, 1e-2 at H = 1024,
+where float32 noise flips the ReLU / clip mask of units near a kink (test_configs_gpu.py) and each flip reaches the
+layers below through every stacked recurrence (measured 3.2e-3 and 5.4e-3, while the gradients given the GPU's
+activations agree to 1.4e-5). The cases cover each sweep family, checked with ctcb_debug_sweep_plan, bi- and
+uni-directional layers, k = 2 and 3, a ragged batch, T = 1 and a block that ends at the top hidden layer. Then: the bits
+of k = 1 against a config without the field, forward-only against training probabilities, micro-batches, shards with L2,
+CUDA-graph replay, two ranks over NCCL, and runNNet end to end. Each comparison prints its measured errors as one JSON
+line (pytest -s)."""
 import ctypes
 import json
 import os
@@ -22,7 +22,8 @@ import numpy as np
 import pytest
 
 import recipes
-from stack_oracle import StackNet
+from net_check import bits as _bits, compare, rel as _rel
+from net_oracle import Net
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -42,26 +43,10 @@ CASES = {
 D, K = 41, 32
 
 
-def _rel(a, b):
-    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
-    nb = np.linalg.norm(b)
-    if nb == 0.0:
-        return 0.0 if np.linalg.norm(a) == 0.0 else float("inf")
-    return float(np.linalg.norm(a - b) / nb)
-
-
-def _bits(t):
-    return t.detach().cpu().numpy().view(np.uint32)
-
-
-def _gpu_net(c, B, reg=0.0, train=True):
-    import nnets.brnnet as brnnet
-    import nnets.rnnet as unirnnet
-    kw = dict(temporalLayer=c["tl"], maxUtts=B, maxLabels=c["L"], numTemporal=c["k"], train=train,
-              allowTopTemporal=bool(c.get("top")))
-    if c.get("uni"):
-        return unirnnet.NNet(D, K, c["H"], c["N"], c["T"], **kw)
-    return brnnet.NNet(D, K, c["H"], c["N"], c["T"], reg=reg, **kw)
+def _kwargs(c):
+    """The keyword arguments of nnets.brnnet.NNet and net_oracle.Net that make case c."""
+    return dict(temporalLayer=c["tl"], numTemporal=c["k"], unidirectional=bool(c.get("uni")),
+                allowTopTemporal=bool(c.get("top")))
 
 
 def _batch(c, seed=5):
@@ -78,6 +63,7 @@ def _batch(c, seed=5):
 
 @pytest.mark.parametrize("name", list(CASES))
 def test_stacked_net_matches_float64_oracle(name, cuda):
+    import nnets.brnnet as brnnet
     from _ctcb import lib, check
     c = CASES[name]
     H, N, tl, k, B = c["H"], c["N"], c["tl"], c["k"], c["B"]
@@ -88,11 +74,10 @@ def test_stacked_net_matches_float64_oracle(name, cuda):
     lens, (datas, labelss) = _batch(c)
     Tmax = max(lens)
     np.random.seed(33)
-    on = StackNet(D, K, H, N, c["T"], temporalLayer=tl, numTemporal=k, unidirectional=uni,
-                  allow_top_temporal=bool(c.get("top")))
+    on = Net(D, K, H, N, c["T"], **_kwargs(c))
     on.initParams()
     np.random.seed(33)
-    nn = _gpu_net(c, B)
+    nn = brnnet.NNet(D, K, H, N, c["T"], maxUtts=B, maxLabels=c["L"], **_kwargs(c))
     nn.initParams()
     assert nn.numTemporal == k and len(nn.stack) == len(on.stack)
     for (w, _), (ow, _) in zip(nn.stack, on.stack):         # same draws, same order
@@ -100,60 +85,20 @@ def test_stacked_net_matches_float64_oracle(name, cuda):
     batch = nn._batch.pack(datas, labelss).upload()
     nn.costAndGradDevice(batch, want_probs=True)
     probs_train = nn._probs_view(B, Tmax).clone()
-    costs = nn._cost[:B].cpu().numpy().astype(np.float64)
-    g_host = [(dw.cpu().numpy().astype(np.float64), db.cpu().numpy().astype(np.float64)) for dw, db in nn.grad]
     assert nn.stats.cpu().numpy()[3] == 0
-
-    def act(what, layer):
-        off, width = ctypes.c_size_t(), ctypes.c_int32()
-        check(lib.ctcb_brnn_activation_offset(ctypes.byref(nn._cfg), what, layer, ctypes.byref(off),
-                                              ctypes.byref(width)))
-        n = Tmax * B * width.value
-        return nn._ws[off.value:off.value + 4 * n].view(cuda.float32).view(Tmax, B, width.value).cpu().numpy()
-
-    X = [None] + [act(0, i) for i in range(1, N + 2)]
-    Fors = [act(1, tl + j) for j in range(k)]
-    Backs = None if uni else [act(2, tl + j) for j in range(k)]
-    if uni:
-        for j in range(k):
-            X[tl + j] = Fors[j]       # a uni-directional temporal layer's output is its forward sweep
-
+    r = compare(nn, on, datas, labelss, lens)
+    if c["T"] == 1:     # one frame: no recurrence, the recurrent gradients are exactly zero on both sides
+        assert all(np.abs(dw.cpu().numpy()).max() == 0 for dw, _ in nn.grad[N + 1:])
     # forward-only probabilities of the same net are the training call's, bit for bit
     probs_fwd = nn._forward_device(batch)
     same_probs = bool(np.array_equal(_bits(probs_fwd), _bits(probs_train)))
-    del nn
-    cuda.cuda.empty_cache()
 
-    o_costs, o_grad, o_skips = on.costAndGradBatch(datas, labelss)
-    assert not o_skips.any()
-    cost_err = float(np.max(np.abs(costs - o_costs) / np.abs(o_costs)))
-    fwd_err = 0.0
-    tot = [[np.zeros_like(w), np.zeros_like(b)] for w, b in on.stack]
-    for u, (d, l) in enumerate(zip(datas, labelss)):
-        Tu = lens[u]
-        h, F, Bk, _ = on.forward(d)
-        pairs = [(X[i][:Tu, u, :].T, h[i]) for i in range(1, N + 2)]
-        pairs += [(Fors[j][:Tu, u, :].T, F[j]) for j in range(k)]
-        if not uni:
-            pairs += [(Backs[j][:Tu, u, :].T, Bk[j]) for j in range(k)]
-        for g, o in pairs:
-            fwd_err = max(fwd_err, float(np.abs(g.astype(np.float64) - o).max() / max(np.abs(o).max(), 1e-30)))
-        _, g_, s_ = on.costAndGradGiven(d, l, [X[i][:Tu, u, :].T for i in range(1, N + 2)],
-                                        [f[:Tu, u, :].T for f in Fors],
-                                        None if uni else [b[:Tu, u, :].T for b in Backs])
-        assert not s_
-        for (tw, tb), (gw, gb) in zip(tot, g_):
-            tw += gw
-            tb += gb
-    given, plain = [], []
-    for i, ((dw, db), (tw, tb), (odw, odb)) in enumerate(zip(g_host, tot, o_grad)):
-        given.append(_rel(dw, tw))
-        plain.append(_rel(dw, odw))
-        if i <= N:
-            given.append(_rel(db.reshape(-1), tb.reshape(-1)))
-            plain.append(_rel(db.reshape(-1), odb.reshape(-1)))
-    if c["T"] == 1:     # one frame: no recurrence, the recurrent gradients are exactly zero on both sides
-        assert all(np.abs(dw).max() == 0 for dw, _ in g_host[N + 1:])
+    assert not r["skips_own"].any()
+    cost_err = r["cost_own"]
+    fwd_err = max(r["fwd"]["X"] + [r["fwd"]["For"], r["fwd"].get("Back", 0.0)])
+    tensors = [t for t in range(len(r["grad_given"])) if t % 2 == 0 or t // 2 <= N]    # matrices, the maps' biases
+    given = [r["grad_given"][t] for t in tensors]
+    plain = [r["grad_plain"][t] for t in tensors]
     print(json.dumps({name: dict(config=c, cost_rel_err_max=cost_err, forward_activation_rel_err_max=fwd_err,
                                  grad_rel_err_given_gpu_activations_max=max(given),
                                  grad_rel_err_vs_float64_masks_max=max(plain), grad_rel_err_vs_float64_masks=plain,
@@ -169,11 +114,12 @@ def test_one_temporal_layer_gives_the_bits_of_a_config_without_the_field(cuda):
     """numTemporal = 1 (what NNet passes) against a handle made from the 11-member initialiser (numTemporal = 0):
     probabilities, costs, gradient and statistics tail, bit for bit, on a ragged batch with L2."""
     import _ctcb
+    import nnets.brnnet as brnnet
     from _ctcb import lib, check
     c = dict(H=256, N=3, tl=2, k=1, T=50, B=6, L=10, ragged=True)
     lens, (datas, labelss) = _batch(c)
     np.random.seed(4)
-    nn = _gpu_net(c, c["B"], reg=1e-2)
+    nn = brnnet.NNet(D, K, c["H"], c["N"], c["T"], maxUtts=c["B"], maxLabels=c["L"], reg=1e-2, **_kwargs(c))
     nn.initParams()
     batch = nn._batch.pack(datas, labelss).upload()
     snaps = []
@@ -407,7 +353,7 @@ def test_run_nnet_trains_resumes_and_tests_a_stacked_net(cuda, tmp_path):
     assert cfg["numTemporal"] == 2
     p_epoch0 = net.params.cpu().numpy().copy()
     np.random.seed(33)
-    fresh = StackNet(16, 9, 64, 4, 40, temporalLayer=1, numTemporal=2)
+    fresh = Net(16, 9, 64, 4, 40, temporalLayer=1, numTemporal=2)
     fresh.initParams()
     assert not np.array_equal(net.stack[5][0].cpu().numpy(), fresh.stack[5][0].astype(np.float32))    # it trained
     cfg["epochs"] = 2                                   # resume: one more epoch

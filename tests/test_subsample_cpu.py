@@ -1,7 +1,7 @@
 """CPU tests of frame subsampling (ctcb_brnn_config.subsample = k at map subsampleLayer = L): subsampling off is the net
 without the members (every config answer over 25,600 configs against the build before them), the config contract
-(refusals, W_L's shape, the workspace), the float64 oracle of tests/subsample_oracle.py against torch autograd and
-central differences, the host admission rule at ceil(T / k), and runNNet's flags."""
+(refusals, W_L's shape, the workspace), the host admission rule at ceil(T / k), and runNNet's flags (the float64
+restatement of the net is tested in tests/test_net_oracle_cpu.py)."""
 import ctypes
 import os
 
@@ -9,9 +9,6 @@ import numpy as np
 import pytest
 
 import config_matrix
-import recipes
-from dropout_oracle import Dropout
-from subsample_oracle import SubsampleNet, frames, stack_frames, unstack_frames
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
@@ -99,10 +96,6 @@ def test_only_w_l_widens(k, sl):
         assert c1 == (k * c0 if t == 2 * (sl - 1) else c0)
         assert o1 == o0 + (0 if t <= 2 * (sl - 1) else growth)
     assert on[2 * (sl - 1)][2] == k * n
-    # and the oracle draws the same shapes
-    o = SubsampleNet(D, K, H, 3, 60, 2, subsample=k, subsampleLayer=sl)
-    o.initParams()
-    assert [tuple(w.shape) for w, _ in o.stack] == [(r, c) for _, r, c in on[0::2]]
 
 
 def _ws(cfg):
@@ -153,171 +146,6 @@ def test_workspace_above_the_subsampling_point_shrinks():
     one = _cfg(41, 32, 1024, 3, 2, 800, 128, L=100, k=2, sl=1)
     assert lib.ctcb_brnn_activation_offset(ctypes.byref(one), 6, 0, ctypes.byref(o), ctypes.byref(w)) == 0
     assert w.value == 2 * 41 and _ws(one) - o.value == al(51200 * 82 * 4) + al(128 * 4)
-
-
-# ------------------------------------------------------------------------------------------- the oracle
-def test_stack_and_unstack_follow_the_definition():
-    rng = np.random.RandomState(0)
-    for n, T, k in ((3, 7, 2), (5, 9, 3), (4, 2, 3), (1, 1, 4), (6, 12, 3)):
-        x = rng.randn(n, T)
-        S = stack_frames(x, k)
-        assert S.shape == (k * n, frames(T, k))
-        for tp in range(S.shape[1]):
-            for m in range(k):
-                t = k * tp + m
-                assert np.array_equal(S[m * n:(m + 1) * n, tp], x[:, t] if t < T else np.zeros(n))
-        assert np.array_equal(unstack_frames(S, k, T), x)
-
-
-def _torch_net(o, datas, labels):
-    """The same net as SubsampleNet o (clipped-ReLU temporal layers, layer norm, dropout; no LSTM) in torch float64 with
-    autograd and torch's CTC: (summed cost, gradient of every tensor)."""
-    import torch
-    P = [[torch.tensor(w, requires_grad=True), torch.tensor(b, requires_grad=True)] for w, b in o.stack]
-    total = 0.0
-    for u, (d, lab) in enumerate(zip(datas, labels)):
-        if o.dropout is not None:
-            o.dropout.g = u
-        x = torch.tensor(np.asarray(d, dtype=np.float64))
-        for i in range(1, o.numLayers + 2):
-            if o.stacked(i):
-                n, T = x.shape
-                Tp = frames(T, o.k)
-                x = torch.cat([x, torch.zeros(n, Tp * o.k - T, dtype=x.dtype)], 1).T.reshape(Tp, o.k * n).T
-            w, b = P[i - 1]
-            z = w @ x + b
-            T = z.shape[1]
-            if o.temporal(i):
-                idx = o.rec(i - o.temporalLayer)
-
-                def sweep(U, order, prev):
-                    cols = [None] * T
-                    for m, t in enumerate(order):
-                        v = z[:, t] + (U @ cols[t + prev] if m else 0.0)
-                        cols[t] = torch.clamp(v, 0.0, o.maxAct)
-                    return torch.stack(cols, 1)
-                For = sweep(P[idx[0]][0], range(T), -1)
-                z = For if o.unidirectional else For + sweep(P[idx[1]][0], range(T - 1, -1, -1), 1)
-            elif i <= o.numLayers:
-                if o.normed(i):
-                    g, be = P[o.ln_index(i)]
-                    z = torch.nn.functional.layer_norm(z.T, (z.shape[0],), g[:, 0], be[:, 0], eps=1e-5).T
-                z = torch.relu(z)
-                if o.dropped(i):
-                    keep = o.dropout.apply(np.ones(tuple(z.shape)), i)
-                    z = z * torch.tensor(keep)
-            x = z
-        lp = torch.log_softmax(x.T, 1)[:, None, :]
-        total = total + torch.nn.functional.ctc_loss(lp, torch.tensor(lab, dtype=torch.long)[None],
-                                                     torch.tensor([lp.shape[0]]), torch.tensor([len(lab)]),
-                                                     blank=0, reduction="sum")
-    total.backward()
-    g = lambda t: np.zeros(tuple(t.shape)) if t.grad is None else t.grad.numpy()     # noqa: E731 (the dummies)
-    return total.item(), [[g(w), g(b)] for w, b in P]
-
-
-# name: N, tl, nt, k, L, extra
-NETS = {
-    "bi_L1_k2": (3, 2, 1, 2, 1, {}),
-    "bi_Ltl_k3": (3, 2, 1, 3, 2, {}),
-    "uni_stack_inside_k2": (4, 2, 2, 2, 3, dict(uni=True)),
-    "bi_stack_inside_k3": (4, 2, 2, 3, 3, {}),
-    "bi_above_k2_ln_drop": (3, 1, 1, 2, 3, dict(ln=True, p=0.3)),
-    "bi_top_k3": (3, 2, 1, 3, 4, {}),
-    "dnn_k2_ln": (2, 0, 0, 2, 2, dict(ln=True)),
-    "dnn_L1_k3_drop": (2, 0, 0, 3, 1, dict(p=0.25)),
-    "lstm_bi_Ltl_k2": (3, 2, 1, 2, 2, dict(cell="lstm")),
-    "lstm_uni_above_k3": (3, 1, 1, 3, 2, dict(cell="lstm", uni=True, ln=True)),
-}
-
-
-def _oracle(name, D=5, K=6, H=6, **kw):
-    N, tl, nt, k, L, x = NETS[name]
-    drop = Dropout(x["p"], seed=5) if "p" in x else None
-    o = SubsampleNet(D, K, H, N, 40, tl, nt, subsample=k, subsampleLayer=L, dropout=drop, cell=x.get("cell", "relu"),
-                     unidirectional=bool(x.get("uni")), layerNorm=bool(x.get("ln")), **kw)
-    o.initParams()
-    return o
-
-
-# ragged lengths, none a multiple of 2 or 3 but one; every T mod k
-LENS, NLABS = [13, 8, 11, 7], [3, 2, 2, 1]
-
-
-@pytest.mark.parametrize("name", [n for n in NETS if NETS[n][5].get("cell") != "lstm"])
-def test_oracle_matches_torch_autograd(name):
-    pytest.importorskip("torch")
-    np.random.seed(7)
-    o = _oracle(name, reg=0.0, round_f32=False)
-    datas, labels = recipes.synth_batch(5, 6, LENS, NLABS, seed=3)
-    costs, grad, skips = o.costAndGradBatch(datas, labels)
-    assert not skips.any()
-    tc, tg = _torch_net(o, datas, labels)
-    assert abs(costs.sum() - tc) <= 1e-9 * abs(tc)
-    for (a, b), (c, d) in zip(grad, tg):
-        assert np.allclose(a, c, rtol=1e-8, atol=1e-11) and np.allclose(b, d, rtol=1e-8, atol=1e-11)
-
-
-@pytest.mark.parametrize("name", list(NETS))
-def test_oracle_gradient_matches_central_differences(name):
-    """float64, reg > 0: a few entries of every tensor (W_L included, each of its k column blocks) against
-    (f(w + e) - f(w - e)) / 2e."""
-    np.random.seed(11)
-    net = _oracle(name, reg=1e-3, round_f32=False)
-    rng = np.random.RandomState(2)
-    for i in net.normedLayers():
-        gamma, beta = net.stack[net.ln_index(i)]
-        gamma += 0.3 * rng.randn(*gamma.shape)
-        beta += 0.3 * rng.randn(*beta.shape)
-    datas, labels = recipes.synth_batch(5, 6, LENS, NLABS, seed=3)
-    _, grad, skips = net.costAndGradBatch(datas, labels)
-    assert not skips.any()
-    eps = 1e-6
-    N = net.numLayers
-    base = N + 1 + net.numTemporal * net.nrec
-    for ti, (w, b) in enumerate(net.stack):
-        for x, gx in ((w, grad[ti][0]), (b, grad[ti][1])):
-            if N < ti < base and x is b:        # the recurrent matrices' dummies take no part
-                continue
-            idxs = [tuple(rng.randint(0, s) for s in x.shape) for _ in range(3)]
-            if ti == net.L - 1 and x is w:      # one entry in every sub-frame block of W_L
-                n = x.shape[1] // net.k
-                idxs += [(rng.randint(0, x.shape[0]), m * n + rng.randint(0, n)) for m in range(net.k)]
-            for idx in idxs:
-                old = x[idx]
-                x[idx] = old + eps
-                cp = net.costAndGradBatch(datas, labels)[0].sum() + net.regcost
-                x[idx] = old - eps
-                cm = net.costAndGradBatch(datas, labels)[0].sum() + net.regcost
-                x[idx] = old
-                num = (cp - cm) / (2 * eps)
-                assert abs(num - gx[idx]) <= 1e-6 * max(1.0, abs(num)), (name, ti, idx, num, gx[idx])
-
-
-def test_oracle_with_k_1_is_the_layer_norm_oracle():
-    from layernorm_oracle import LayerNormNet
-    np.random.seed(4)
-    a = SubsampleNet(5, 6, 6, 3, 8, 2, 1, subsample=1, subsampleLayer=2, layerNorm=True, reg=1e-3)
-    a.initParams()
-    np.random.seed(4)
-    b = LayerNormNet(5, 6, 6, 3, 8, 2, 1, reg=1e-3)
-    b.initParams()
-    datas, labels = recipes.synth_batch(5, 6, [7, 4], [3, 2], seed=3)
-    ca, ga, _ = a.costAndGradBatch(datas, labels)
-    cb, gb, _ = b.costAndGradBatch(datas, labels)
-    assert np.array_equal(ca, cb)
-    for (x, y), (u, v) in zip(ga, gb):
-        assert np.array_equal(x, u) and np.array_equal(y, v)
-
-
-def test_utterance_too_short_for_its_labels_at_the_reduced_rate_is_skipped():
-    """T = 7 frames, k = 3: 3 output frames, which 3 labels with a repeat cannot be aligned to: the CTC's own skip (the
-    host rule for fewer frames than labels is test_admission_compares_ceil_t_over_k_with_the_labels)."""
-    np.random.seed(1)
-    o = SubsampleNet(5, 6, 6, 3, 40, 2, subsample=3, subsampleLayer=1)
-    o.initParams()
-    cost, _, skip = o.costAndGrad(np.random.RandomState(0).randn(5, 7), np.array([1, 2, 2], dtype=np.int32))
-    assert skip
 
 
 # ------------------------------------------------------------------------------------------- host side

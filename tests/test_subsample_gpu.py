@@ -3,10 +3,10 @@
 1. The kernels alone (ctcb_frame_stack_f32 / ctcb_frame_unstack_f32) are exact copies: bit for bit against NumPy for
    k = 2, 3, 4, n odd and n % 4 == 0 (16-byte and, misaligned, 4-byte accesses), B = 1 and larger, Tmax < k and every
    T_u mod k; padding is zero and every output element is written.
-2. The whole net against tests/subsample_oracle.py for L = 1, L at the lowest temporal layer, L inside a stack, L above
-   the temporal block and L = numLayers + 1, bi- and uni-directional, DNN, LSTM, layer norm and dropout: cost, every
-   activation (S through what = 6) and every gradient tensor against the oracle's back-propagation through the GPU's own
-   activations, with the bounds of tests/test_layernorm_gpu.py (relative, 1e-4).
+2. The whole net against tests/net_oracle.py (compared by tests/net_check.py) for L = 1, L at the lowest temporal layer,
+   L inside a stack, L above the temporal block and L = numLayers + 1, bi- and uni-directional, DNN, LSTM, layer norm
+   and dropout: cost, every activation (S through what = 6) and every gradient tensor against the oracle's
+   back-propagation through the GPU's own activations, with the bounds of tests/test_layernorm_gpu.py (relative, 1e-4).
 3. Consistency: micro-batches and two emulated shards, graph replay, forward-only probabilities, the likelihood arks,
    runNNet end to end, checkpoints of the other width, check_grad on W_L, and the skip of utterances too short for
    their labels at the reduced rate.
@@ -21,28 +21,11 @@ import numpy as np
 import pytest
 
 import recipes
-from dropout_oracle import Dropout
-from subsample_oracle import SubsampleNet, frames, stack_frames
+from net_check import bits as _bits, compare, rel as _rel
+from net_oracle import Net, frames
 
 pytestmark = pytest.mark.gpu
 FWD_TOL, GRAD_TOL = 1e-4, 1e-4
-
-
-def _rel(a, b):
-    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
-    nb = np.linalg.norm(b)
-    if nb == 0.0:
-        return 0.0 if np.linalg.norm(a) == 0.0 else float("inf")
-    return float(np.linalg.norm(a - b) / nb)
-
-
-def _relmax(a, b):
-    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
-    return float(np.max(np.abs(a - b)) / max(np.max(np.abs(b)), 1e-30))
-
-
-def _bits(t):
-    return t.detach().cpu().numpy().view(np.uint32)
 
 
 # ------------------------------------------------------------------------------------------------ 1. the kernels
@@ -117,19 +100,16 @@ NETS = {
 }
 
 
-def _gpu_net(c, B, reg=0.0, train=True, k=None):
+def _kwargs(c, reg=0.0):
+    """The keyword arguments of nnets.brnnet.NNet and net_oracle.Net that make net c."""
+    return dict(temporalLayer=c["tl"] or -1, numTemporal=max(1, c["nt"]), reg=reg, unidirectional=bool(c.get("uni")),
+                cell=c.get("cell", "relu"), dropout=c.get("p", 0.0), layerNorm=bool(c.get("ln")), subsample=c["k"],
+                subsampleLayer=c["sl"])
+
+
+def _gpu_net(c, B, reg=0.0, train=True):
     import nnets.brnnet as brnnet
-    return brnnet.NNet(D_IN, K, c["H"], c["N"], c["T"], temporalLayer=c["tl"] or -1, maxUtts=B, maxLabels=c["L"],
-                       numTemporal=max(1, c["nt"]), train=train, reg=reg, unidirectional=bool(c.get("uni")),
-                       cell=c.get("cell", "relu"), dropout=c.get("p", 0.0), layerNorm=bool(c.get("ln")),
-                       subsample=c["k"] if k is None else k, subsampleLayer=c["sl"])
-
-
-def _oracle(c, reg=0.0):
-    drop = Dropout(c["p"], seed=33, step=0) if "p" in c else None
-    return SubsampleNet(D_IN, K, c["H"], c["N"], c["T"], c["tl"], c["nt"], subsample=c["k"], subsampleLayer=c["sl"],
-                        dropout=drop, cell=c.get("cell", "relu"), reg=reg, unidirectional=bool(c.get("uni")),
-                        layerNorm=bool(c.get("ln")))
+    return brnnet.NNet(D_IN, K, c["H"], c["N"], c["T"], maxUtts=B, maxLabels=c["L"], train=train, **_kwargs(c, reg))
 
 
 def _ragged(c, seed=5):
@@ -142,85 +122,29 @@ def _ragged(c, seed=5):
     return lens, recipes.synth_batch(D_IN, K, lens, nlabs, seed=33)
 
 
-def _ws_array(nn, what, layer, T, B):
-    from _ctcb import lib, check
-    off, w = ctypes.c_size_t(), ctypes.c_int32()
-    check(lib.ctcb_brnn_activation_offset(ctypes.byref(nn._cfg), what, layer, ctypes.byref(off), ctypes.byref(w)))
-    n = T * B * w.value
-    return nn._ws[off.value:off.value + 4 * n].view(nn._torch.float32).cpu().numpy().reshape(T, B, w.value)
-
-
 @pytest.mark.parametrize("name", list(NETS))
 def test_subsampled_net_matches_float64_oracle(name, cuda):
     c = NETS[name]
     lens, (datas, labelss) = _ragged(c)
-    B, Tmax, N, tl, nt, k, sl = c["B"], max(lens), c["N"], c["tl"], c["nt"], c["k"], c["sl"]
-    uni, lstm = bool(c.get("uni")), c.get("cell") == "lstm"
+    B, k, sl = c["B"], c["k"], c["sl"]
     reg = 1e-3
     np.random.seed(21)
     nn = _gpu_net(c, B, reg=reg)
     nn.initParams()
     np.random.seed(21)
-    on = _oracle(c, reg)
+    on = Net(D_IN, K, c["H"], c["N"], c["T"], **_kwargs(c, reg))
     on.initParams()
     for (w, b), (ow, ob) in zip(nn.stack, on.stack):        # the same draws, shapes (W_L k n wide) and order
         assert np.array_equal(w.cpu().numpy(), ow.astype(np.float32))
         assert np.array_equal(b.cpu().numpy(), ob.astype(np.float32))
     assert tuple(nn.stack[sl - 1][0].shape)[1] == k * (D_IN if sl == 1 else c["H"])
-    costs, grad, skips = nn.costAndGradBatch(datas, labelss)
-    o_costs, o_grad, o_skips = on.costAndGradBatch(datas, labelss)
-    assert np.array_equal(skips, o_skips) and not skips.any()
-    cost_err = float(np.max(np.abs(costs - o_costs) / np.abs(o_costs)))
-    Tr = lambda i: frames(Tmax, k) if i >= sl else Tmax      # noqa: E731
-    temporal = list(range(tl, tl + nt)) if tl else []
-    X = {i: _ws_array(nn, 0, i, Tr(i), B) for i in range(1, N + 2)}
-    S = _ws_array(nn, 6, 0, frames(Tmax, k), B)
-    hF = {i: _ws_array(nn, 1, i, Tr(i), B) for i in temporal}
-    hB = {i: _ws_array(nn, 2, i, Tr(i), B) for i in temporal} if not uni else {}
-    cF = {i: _ws_array(nn, 4, i, Tr(i), B) for i in temporal} if lstm else {}
-    cB = {i: _ws_array(nn, 5, i, Tr(i), B) for i in temporal} if lstm and not uni else {}
-    fwd = 0.0
-    given = [[np.zeros_like(w), np.zeros_like(b)] for w, b in on.stack]
-    for u in range(B):
-        if on.dropout is not None:
-            on.dropout.g = u
-        hActs, _, _ = on.forward(datas[u])
-        g_acts, g_temp = [], []
-        for i in range(1, N + 2):
-            Tu = frames(lens[u], k) if i >= sl else lens[u]
-            act = X[i][:Tu, u].T
-            if i in temporal and lstm:          # X holds the gates; the output is h_f + h_b
-                gh = [hF[i][:Tu, u].T] + ([] if uni else [hB[i][:Tu, u].T])
-                gc = [cF[i][:Tu, u].T] + ([] if uni else [cB[i][:Tu, u].T])
-                g_temp.append((X[i][:Tu, u].T, gc, gh))
-                act = sum(x.astype(np.float64) for x in gh)
-            elif i in temporal:
-                g_temp.append((hF[i][:Tu, u].T, None if uni else hB[i][:Tu, u].T))
-                if uni:
-                    act = hF[i][:Tu, u].T
-            g_acts.append(act)
-            fwd = max(fwd, _relmax(act, hActs[i]))
-        s_u = S[:frames(lens[u], k), u].T                   # zero beyond T_u
-        fwd = max(fwd, _relmax(s_u, stack_frames(hActs[sl - 1], k)))
-        assert not np.any(S[frames(lens[u], k):, u])
-        on.reg = 0.0
-        _, gg, _ = on.costAndGradGiven(datas[u], labelss[u], g_acts, g_temp)
-        on.reg = reg
-        for (a, b), (x, y) in zip(given, gg):
-            a += x
-            b += y
-    for kk in on.weight_indices():
-        given[kk][0] += reg * on.stack[kk][0]
-    grad_err, grad_elem, plain = [], [], []
-    for (dw, db), (gw, gb), (ow, ob) in zip(grad, given, o_grad):
-        for x, y, z in ((dw, gw, ow), (db, gb, ob)):
-            x = x.cpu().numpy().astype(np.float64).reshape(y.shape)
-            if not np.any(y):
-                assert not np.any(x)
-                continue
-            grad_err.append(_rel(x, y))
-            grad_elem.append(_relmax(x, y))
-            plain.append(_rel(x, z))
+    nn.costAndGradBatch(datas, labelss)
+    r = compare(nn, on, datas, labelss, lens)
+    assert np.array_equal(r["skips"], r["skips_own"]) and not r["skips"].any()
+    for u in range(B):                                      # S is zero beyond T'_u
+        assert not np.any(r["acts"][6, 0][frames(lens[u], k):, u])
+    cost_err, fwd = r["cost_own"], max(r["fwd"]["X"] + [r["fwd"]["S"]])
+    grad_err, grad_elem, plain = r["grad_given"], r["grad_given_elem"], r["grad_plain"]
     print(json.dumps({"subsample_net_" + name: dict(cost=cost_err, fwd=fwd, grad_given_frob_max=max(grad_err),
                                                     grad_given_elem_max=max(grad_elem), grad_plain_frob_max=max(plain))}))
     assert cost_err <= FWD_TOL and fwd <= FWD_TOL
