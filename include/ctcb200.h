@@ -188,6 +188,9 @@ typedef struct ctcb_brnn_config {
                             * negative value makes the config invalid. */
     int32_t subsampleLayer; /* L: ignored for k <= 1; with k >= 2 it needs 1 <= L <= numLayers + 1, else the config is
                              * invalid. */
+    int32_t peephole;      /* 0: off (so an initialiser without this member keeps its meaning); 1: peephole connections of
+                            * the LSTM cell (below), which needs cell = 1; any other value, or 1 with cell = 0, makes the
+                            * config invalid.  Without a temporal layer it lays out and launches nothing. */
 } ctcb_brnn_config;
 
 /* Frame subsampling (subsample = k >= 2; not in the reference; cf. Deep Speech 2's striding and the frame stacking of
@@ -235,6 +238,21 @@ typedef struct ctcb_brnn_config {
  * ctcb_brnn_create refuses (CTCB_EINVAL, the message names the width) a layerSize whose sweep the device cannot hold
  * co-resident: ndir * ceil(H / 8) CTAs of 256 threads, at most two per SM (bi-directional H = 2048 on an H100). */
 
+/* Peephole connections (peephole = 1 with cell = 1; Graves, Mohamed & Hinton 2013, eqs. 3-7; the cell of EESEN and of
+ * Kaldi's nnet1 LSTM).  Per direction of every LSTM layer three H-vectors p_i, p_f, p_o; only the sigmoid gates change:
+ *     i = sigmoid(z_i + p_i c_{t-1});  f = sigmoid(z_f + p_f c_{t-1});  g = tanh(z_g);  c_t = f c_{t-1} + i g;
+ *     o = sigmoid(z_o + p_o c_t);  h_t = o tanh(c_t)
+ *   (the backward-in-time direction mirrored: c_{t+1} in place of c_{t-1}).  c is 0 before the first frame and at every
+ *   frame t >= T_u, as without peepholes.  The gates buffer holds o after its peephole.
+ *   BPTT ("next" = t + 1 in the direction's order):
+ *     dz_o = dh tanh(c_t) o(1-o);  dc_t = dh o (1 - tanh^2 c_t) + p_o dz_o + f_{t+1} dc_{t+1} + p_i dz_i,{t+1} + p_f dz_f,{t+1}
+ *     dz_i, dz_f, dz_g as without peepholes, from this dc_t;
+ *     dp_i = sum_{t,u} dz_i,t c_{t-1};  dp_f = sum dz_f,t c_{t-1};  dp_o = sum dz_o,t c_t   (padded frames add nothing).
+ * Each LSTM layer adds one entry per direction, [P_d (3 x H, rows i, f, o), dummy (1 x 1)], in the recurrent entries'
+ * order (temporal layers ascending, forward before backward), behind every other tensor of the flat vector (the
+ * [gamma, beta] pairs included), so no other offset and not the early all-reduce range moves; the peephole gradients
+ * travel with the exchange at the end of the step.  P is not L2-regularised; the dummies get a zero gradient. */
+
 typedef struct ctcb_brnn ctcb_brnn; /* opaque; owns no device memory */
 
 /* Flat parameter vector layout: the reference's `stack` order (brnnet.py:38-41,66-72):
@@ -242,7 +260,9 @@ typedef struct ctcb_brnn ctcb_brnn; /* opaque; owns no device memory */
  * unidirectional: [W1,b1] ... [W_{N+1},b_{N+1}] [Wt,dummy].
  * numTemporal = k > 1: [W1,b1] ... [W_{N+1},b_{N+1}] then, per temporal layer in ascending order,
  * [Wtf_j,dummy] [Wtb_j,dummy] (unidirectional: [Wt_j,dummy]); for k = 1 this is the layout above.
- * layerNorm = 1 appends [gamma_i, beta_i] of every normalised hidden layer i, in ascending i. */
+ * layerNorm = 1 appends [gamma_i, beta_i] of every normalised hidden layer i, in ascending i.
+ * peephole = 1 then appends [P_f,j, dummy] [P_b,j, dummy] (unidirectional: [P_j, dummy]) of every temporal layer j in
+ * ascending order, each P 3 x H. */
 int64_t ctcb_brnn_param_count(const ctcb_brnn_config *cfg);
 int ctcb_brnn_num_tensors(const ctcb_brnn_config *cfg);                    /* 2 * len(stack) */
 int ctcb_brnn_tensor_info(const ctcb_brnn_config *cfg, int idx, int64_t *offset, int32_t *rows, int32_t *cols);
@@ -261,7 +281,10 @@ int ctcb_brnn_tensor_info(const ctcb_brnn_config *cfg, int idx, int64_t *offset,
  * layer-norm partial areas for their largest user; and appends, behind everything else, S and dS (R' * k * n floats
  * each, n the width of layer L - 1) and T' (maxB int32).  The forward workspace sizes its slabs, For / Back and c
  * from the rows of the maps that use them in the same way and appends S and T', so it stays within the training
- * workspace.  With k <= 1 no offset moves and nothing is appended. */
+ * workspace.  With k <= 1 no offset moves and nothing is appended.
+ * peephole = 1 (with a temporal layer) appends, behind everything else, the partial sums of the peephole weight
+ * gradients, ctcb_lstm_peephole_grad_workspace_bytes(Tmax_l, maxB, layerSize, ndir) bytes for the frames Tmax_l of the
+ * lowest temporal layer (maxT, or ceil(maxT / k) above the subsampling point).  The forward workspace does not grow. */
 size_t ctcb_brnn_workspace_bytes(const ctcb_brnn_config *cfg);
 /* Byte offset, inside the workspace, of a uint32 that the recurrent-sweep kernels set non-zero when an
  * inter-CTA wait timed out (results are then invalid; never a hang).  Callers that synchronise anyway
@@ -414,6 +437,18 @@ size_t ctcb_lstm_sweep_workspace_bytes(int H, int B);
 int ctcb_lstm_sweep_f32(int mode, int T, int B, int H, const int32_t *T_per_utt, float *gates, const float *Uf,
                         const float *Ub, float *hF, float *hB, float *cF, float *cB, const float *dh, float *dz,
                         void *scratch, size_t scratch_bytes, void *stream);
+/* The same with peephole connections (peephole = 1, above): Pf / Pb the [3][H] peephole vectors (rows i, f, o) of the
+ * two directions; Pb is ignored when Ub == NULL.  Same scratch; mode 1 carries the whole dc_{t+1} term of dc_t in it. */
+int ctcb_lstm_sweep_peephole_f32(int mode, int T, int B, int H, const int32_t *T_per_utt, float *gates, const float *Uf,
+                                 const float *Ub, const float *Pf, const float *Pb, float *hF, float *hB, float *cF,
+                                 float *cB, const float *dh, float *dz, void *scratch, size_t scratch_bytes, void *stream);
+/* The peephole weight gradients of one LSTM layer: dz [T][B][G] as mode 1 of the sweep wrote it, cF / cB [T][B][H] as
+ * mode 0 did (cB == NULL: one direction, G = 4H, dPb ignored); dPf / dPb [3][H] receive dp_i, dp_f, dp_o, or with
+ * accumulate != 0 have them added.  workspace: ctcb_lstm_peephole_grad_workspace_bytes(T, B, H, ndir) bytes of partial
+ * sums over fixed chunks of rows, added in a fixed order: the bits depend only on T, B, H and the inputs. */
+size_t ctcb_lstm_peephole_grad_workspace_bytes(int T, int B, int H, int ndir);
+int ctcb_lstm_peephole_grad_f32(int T, int B, int H, const float *dz, const float *cF, const float *cB, float *dPf,
+                                float *dPb, int accumulate, void *workspace, size_t ws_bytes, void *stream);
 /* The LSTM sweep's plan for (H, B, ndir): out (HOST, 2 int32) = {KI (H / 32 with U in registers, else 0), utterance
  * partitions}; the error ctcb_brnn_create returns for a width the device cannot hold. */
 int ctcb_debug_lstm_plan(int H, int B, int ndir, int32_t *out);

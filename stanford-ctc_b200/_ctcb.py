@@ -30,7 +30,7 @@ class BrnnConfig(ctypes.Structure):
                 ("maxB", ctypes.c_int32), ("maxLabels", ctypes.c_int32), ("reg", ctypes.c_float),
                 ("maxAct", ctypes.c_float), ("unidirectional", ctypes.c_int32), ("numTemporal", ctypes.c_int32),
                 ("cell", ctypes.c_int32), ("layerNorm", ctypes.c_int32), ("subsample", ctypes.c_int32),
-                ("subsampleLayer", ctypes.c_int32)]
+                ("subsampleLayer", ctypes.c_int32), ("peephole", ctypes.c_int32)]
 
 
 _PROTOS = {
@@ -82,6 +82,10 @@ _PROTOS = {
     "ctcb_lstm_sweep_workspace_bytes": (c_sz, [c_int, c_int]),
     "ctcb_lstm_sweep_f32": (c_int, [c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
                                     c_vp, c_vp, c_sz, c_vp]),
+    "ctcb_lstm_sweep_peephole_f32": (c_int, [c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                             c_vp, c_vp, c_vp, c_vp, c_vp, c_sz, c_vp]),
+    "ctcb_lstm_peephole_grad_workspace_bytes": (c_sz, [c_int, c_int, c_int, c_int]),
+    "ctcb_lstm_peephole_grad_f32": (c_int, [c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_sz, c_vp]),
     "ctcb_debug_lstm_plan": (c_int, [c_int, c_int, c_int, ctypes.POINTER(ctypes.c_int32)]),
     "ctcb_layernorm_workspace_bytes": (c_sz, [c_i64, c_int]),
     "ctcb_layernorm_forward_f32": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_int, c_vp]),

@@ -33,9 +33,12 @@ int run_dropout(float *X, int64_t R, int B, int H, int layer, uint64_t seed, con
                 int64_t stride, uint32_t thr, float scale, cudaStream_t st);
 size_t lstm_carry_bytes(int H, int B);
 int run_lstm_sweep(int mode, int T, int B, int H, const int32_t *Tlen, float *gates, const float *Uf, const float *Ub,
-                   float *hF, float *hB, float *cF, float *cB, const float *dh, float *dz, unsigned int *counters,
-                   float *dc, cudaStream_t st);
-int lstm_check(int H, int B, int ndir);
+                   const float *Pf, const float *Pb, float *hF, float *hB, float *cF, float *cB, const float *dh,
+                   float *dz, unsigned int *counters, float *dc, cudaStream_t st);
+int lstm_check(int H, int B, int ndir, bool peep);
+size_t lstm_peephole_grad_bytes(int64_t R, int H, int ndir);
+int run_lstm_peephole_grad(int T, int B, int H, const float *dz, const float *cF, const float *cB, float *dPf,
+                           float *dPb, bool accumulate, float *partial, cudaStream_t st);
 size_t layernorm_workspace_bytes(int64_t R, int H);
 int run_layernorm_forward(const float *z, float *y, float *mu, float *rstd, const float *gamma, const float *beta,
                           int64_t R, int H, cudaStream_t st);
@@ -200,6 +203,10 @@ static const char *cfg_error(const ctcb_brnn_config *c, char (&buf)[192]) {
     if (c->cell != 0 && c->cell != 1) return say("cell %d is neither 0 (clipped ReLU) nor 1 (LSTM)", c->cell);
     if (c->layerNorm != 0 && c->layerNorm != 1)
         return say("layerNorm %d is neither 0 (off) nor 1 (layer normalisation of the ReLU hidden layers)", c->layerNorm);
+    if (c->peephole != 0 && c->peephole != 1)
+        return say("peephole %d is neither 0 (off) nor 1 (peephole connections of the LSTM cell)", c->peephole);
+    if (c->peephole == 1 && c->cell != 1)
+        return say("peephole 1 needs the LSTM cell (cell 1); cell is %d", c->cell);
     if (c->layerNorm == 1 && c->layerSize > CTCB_LAYERNORM_MAX_H)
         return say("layerNorm needs layerSize <= %d (the normalisation kernels hold a row on chip); layerSize is %d",
                    CTCB_LAYERNORM_MAX_H, c->layerSize);
@@ -280,22 +287,34 @@ static int ln_index(const ctcb_brnn_config *c, int i) {
     return base_tensors(c) + 2 * k;
 }
 
+// the [P, dummy] entries of a peephole net: one per direction of every temporal layer; 0 without
+static int peep_tensors(const ctcb_brnn_config *c) {
+    return c->peephole == 1 ? eff_nt(c) * (c->unidirectional ? 2 : 4) : 0;
+}
+// flat-vector index of P of the forward direction of temporal layer j; the backward one, when bi-directional, is two
+// tensors behind it.  The entries follow the [gamma, beta] pairs.
+static int peep_index(const ctcb_brnn_config *c, int j) {
+    return ln_index(c, c->numLayers + 1) + j * (c->unidirectional ? 2 : 4);
+}
+
 extern "C" int ctcb_brnn_num_tensors(const ctcb_brnn_config *cfg) {
     if (!valid_cfg(cfg)) return 0;
     int n = base_tensors(cfg);
     for (int i = 1; i <= cfg->numLayers; ++i) n += 2 * is_normed(cfg, i);
-    return n;
+    return n + peep_tensors(cfg);
 }
 
 namespace {
 // The flat parameter (and gradient) vector of a valid config: W and b of every affine map, then per temporal layer its
 // recurrent matrices, each followed by the reference's `dummy` bias (brnnet.py:60-72), then [gamma, beta] of every
-// layer-normalised hidden layer; every tensor 16-byte aligned.
+// layer-normalised hidden layer, then [P, dummy] of every direction of every peephole LSTM layer; every tensor 16-byte
+// aligned.
 struct NetTable {
     struct Tensor { int64_t off; int32_t rows, cols; };
     int n;
-    int nreg;       // tensors 0 .. nreg-1 are the ones L2 regularisation sees (its even ones): all but the LN pairs
-    Tensor t[2 * 65 + 4 * 64 + 2 * 64];
+    int nreg;       // tensors 0 .. nreg-1 are the ones L2 regularisation sees (its even ones): all but the LN pairs and
+                    // the peephole entries
+    Tensor t[2 * 65 + 4 * 64 + 2 * 64 + 4 * 64];
     int64_t params;
     // The gradients that a data-parallel step sums over the ranks early, on the side stream next to the BPTT sweep: the
     // contiguous range from W of the lowest temporal layer to the end of b of layer N+1; empty (at `params`) without a
@@ -307,10 +326,14 @@ void net_table(const ctcb_brnn_config *c, NetTable *nt) {
     const int nl = c->numLayers + 1;
     nt->n = ctcb_brnn_num_tensors(c);
     nt->nreg = base_tensors(c);
+    const int peep0 = nt->n - peep_tensors(c);
     int64_t off = 0;
     for (int t = 0; t < nt->n; ++t) {
         int r, cc;
-        if (t >= nt->nreg) {        // gamma or beta of a normalised layer
+        if (t >= peep0) {           // P (rows i, f, o) of one direction, or its dummy
+            r = (t - peep0) % 2 == 0 ? 3 : 1;
+            cc = (t - peep0) % 2 == 0 ? c->layerSize : 1;
+        } else if (t >= nt->nreg) {        // gamma or beta of a normalised layer
             r = c->layerSize;
             cc = 1;
         } else if (t < 2 * nl) {
@@ -394,6 +417,7 @@ struct WsLayout {
     size_t Z[65], Mu[65], Rstd[65], ln_part;
     // subsampling only (0 elsewhere): the stacked input S of map L, its delta dS (L >= 2), T'_u of the call
     size_t S, dS, lens;
+    size_t peep_part;   // peephole nets only (0 elsewhere): the partial sums of the peephole weight gradients
     size_t total;
 };
 
@@ -480,6 +504,8 @@ WsLayout ws_layout(const ctcb_brnn_config *c) {
         if (c->subsampleLayer >= 2) w.dS = take(off, stacked_bytes(c));
         w.lens = take(off, (size_t)c->maxB * sizeof(int32_t));
     }
+    if (peep_tensors(c))     // the lowest temporal layer has the most rows
+        w.peep_part = take(off, lstm_peephole_grad_bytes((int64_t)max_rows(c, tl), H, uni ? 1 : 2));
     w.total = off;
     return w;
 }
@@ -650,6 +676,8 @@ struct ctcb_brnn {
 
     bool uni() const { return cfg.unidirectional != 0; }
     bool lstm() const { return cfg.cell == 1; }
+    bool peep() const { return cfg.peephole == 1; }
+    int peep_idx(int j) const { return peep_index(&cfg, j); }
     bool temporal(int i) const { return nt > 0 && i >= tl && i < tl + nt; }
     bool normed(int i) const { return is_normed(&cfg, i); }
     bool reduced(int i) const { return is_reduced(&cfg, i); }     // map i runs at 1/k of the input frame rate
@@ -698,7 +726,7 @@ extern "C" int ctcb_brnn_create(const ctcb_brnn_config *cfg, ctcb_brnn **out) {
     h->tl = eff_tl(cfg);
     h->nt = eff_nt(cfg);
     if (cfg->cell == 1 && h->nt) {      // a width whose LSTM sweep the device cannot hold co-resident
-        const int rc = lstm_check(cfg->layerSize, cfg->maxB, cfg->unidirectional ? 1 : 2);
+        const int rc = lstm_check(cfg->layerSize, cfg->maxB, cfg->unidirectional ? 1 : 2, cfg->peephole == 1);
         if (rc != CTCB_OK) {
             char why[512];
             snprintf(why, sizeof(why), "%s", ctcb_last_error());
@@ -821,12 +849,14 @@ static int brnn_forward(ctcb_brnn *h, const float *feats, const int32_t *T_per_u
                             h->drop_thr, h->drop_scale, st));
         }
         if (h->temporal(i) && h->lstm()) {     // the gates over X_i in place, h into For / Back
-            const int j = i - h->tl, iU = h->rec(j);
+            const int j = i - h->tl, iU = h->rec(j), iP = h->peep_idx(j);
+            const float *Pf = h->peep() ? h->tensor(params, iP) : nullptr;
+            const float *Pb = h->peep() && !uni ? h->tensor(params, iP + 2) : nullptr;
             {
             ProfScope ps("sweep_fwd", st);
             TRY(run_lstm_sweep(0, Tmax, B, H, Tlen, m.X[i], h->tensor(params, iU),
-                               uni ? nullptr : h->tensor(params, iU + 2), m.For[j], m.Back[j], m.Cf[j], m.Cb[j], nullptr,
-                               nullptr, m.counters, (float *)m.sweep, st));
+                               uni ? nullptr : h->tensor(params, iU + 2), Pf, Pb, m.For[j], m.Back[j], m.Cf[j], m.Cb[j],
+                               nullptr, nullptr, m.counters, (float *)m.sweep, st));
             }
             if (!uni) {
                 ProfScope ps("elementwise", st);
@@ -944,6 +974,11 @@ int Step::rec_weight_grads(int j) const {
             CTCB_CUDA_CHECK(cudaMemsetAsync(G(iWtf), 0, sizeof(float) * M * H, side));
             if (!h->uni()) CTCB_CUDA_CHECK(cudaMemsetAsync(G(iWtb), 0, sizeof(float) * M * H, side));
         }
+        if (h->peep()) {     // dP = sums of dz . c over the rows (one frame has dp_o too), in this phase's profile
+            const int iP = h->peep_idx(j);
+            TRY(run_lstm_peephole_grad(Tmax, B, H, dz, m.Cf[j], h->uni() ? nullptr : m.Cb[j], G(iP),
+                                       h->uni() ? nullptr : G(iP + 2), !first, buf(w.peep_part), side));
+        }
     } else if (Tmax > 1) {
         const int64_t Rm = R - B;
         if (h->uni())
@@ -1013,8 +1048,10 @@ int Step::backward() const {
         {
         ProfScope ps("sweep_bptt", main);
         if (lstm)
-            TRY(run_lstm_sweep(1, T(i), B, H, lens(i), m.X[i], P(iWtf), uni ? nullptr : P(iWtf + 2), nullptr, nullptr,
-                               m.Cf[j], m.Cb[j], doth, buf(w.D[i]), m.counters, (float *)m.sweep, main));
+            TRY(run_lstm_sweep(1, T(i), B, H, lens(i), m.X[i], P(iWtf), uni ? nullptr : P(iWtf + 2),
+                               h->peep() ? P(h->peep_idx(j)) : nullptr,
+                               h->peep() && !uni ? P(h->peep_idx(j) + 2) : nullptr, nullptr, nullptr, m.Cf[j], m.Cb[j],
+                               doth, buf(w.D[i]), m.counters, (float *)m.sweep, main));
         else
             TRY(run_sweep(1, T(i), B, H, lens(i), doth, P(iWtf), uni ? nullptr : P(iWtf + 2), buf(w.dFor[p]),
                           buf(w.dBack[p]), m.For[j], m.Back[j], h->cfg.maxAct, m.counters, m.sweep, m.sweep_bytes, main));
@@ -1031,6 +1068,10 @@ int Step::backward() const {
     for (int j = 0; j < nt; ++j) {   // the `dummy` biases never receive gradient
         CTCB_CUDA_CHECK(cudaMemsetAsync(G(h->rec(j) + 1), 0, sizeof(float), main));
         if (!uni) CTCB_CUDA_CHECK(cudaMemsetAsync(G(h->rec(j) + 3), 0, sizeof(float), main));
+        if (h->peep()) {
+            CTCB_CUDA_CHECK(cudaMemsetAsync(G(h->peep_idx(j) + 1), 0, sizeof(float), main));
+            if (!uni) CTCB_CUDA_CHECK(cudaMemsetAsync(G(h->peep_idx(j) + 3), 0, sizeof(float), main));
+        }
     }
     return CTCB_OK;
 }

@@ -17,6 +17,12 @@
 //
 // The forward mode writes the activated gates over the pre-activations in place, c of every frame, and h into the
 // layer's For / Back; the BPTT mode reads those back and carries dc from step to step in a [B][H] scratch per direction.
+//
+// Peephole mode (PEEP, include/ctcb200.h: peephole = 1): z_i and z_f also get p_i c_prev and p_f c_prev, and z_o gets
+// p_o c, so the output gate is activated behind the cell update.  Every term is element-wise in the warp that owns the
+// unit.  BPTT: dc = dh o (1 - tanh^2 c) + p_o dz_o + carry, and the scratch carries f dc + p_i dz_i + p_f dz_f of the
+// step just finished instead of dc.  The peephole weight gradients are a separate reduction over dz and c
+// (lstm_peephole_grad below).
 #include "common.cuh"
 
 namespace ctcb {
@@ -41,6 +47,12 @@ struct LstmArgs {
     unsigned int *err;         // word 0 of the scratch: the error flag, cleared by the caller
     unsigned int *counters;    // [ndir * parts], zeroed before the launch
 };
+// peephole mode: the three peephole vectors of each direction, [3][H] (rows i, f, o)
+struct LstmPeepArgs : LstmArgs {
+    const float *P[2];
+};
+template <bool PEEP> struct LstmArgsOf { using type = LstmArgs; };
+template <> struct LstmArgsOf<true> { using type = LstmPeepArgs; };
 
 // The per-step barrier of the CTAs of one (direction, partition).  A wait longer than ~0.5 s sets the error flag and
 // gives up waiting for the rest of the sweep.
@@ -87,8 +99,8 @@ __device__ __forceinline__ void lstm_load_state(float *hs, int Hp, const float *
 __device__ __forceinline__ float lstm_sigmoid(float z) { return 1.f / (1.f + expf(-z)); }
 
 // KI > 0: H == 32 KI and U lives in registers (one CTA per SM).  KI == 0: any H, U re-read (two CTAs per SM).
-template <int KI>
-__global__ void __launch_bounds__(LS_THREADS, KI > 0 ? 1 : 2) lstm_sweep_kernel(LstmArgs a) {
+template <int KI, bool PEEP>
+__global__ void __launch_bounds__(LS_THREADS, KI > 0 ? 1 : 2) lstm_sweep_kernel(typename LstmArgsOf<PEEP>::type a) {
     extern __shared__ __align__(16) float hs[];   // [LS_NB][Hp]
     const int H = a.H, B = a.B, T = a.T;
     const int64_t G = (int64_t)a.ndir * 4 * H;
@@ -120,6 +132,15 @@ __global__ void __launch_bounds__(LS_THREADS, KI > 0 ? 1 : 2) lstm_sweep_kernel(
 
     // lane -> (gate r, utterance b) of the value it owns after the butterfly
     const int orow = lane >> 3, ob = lane & 7;
+    float pi = 0.f, pf = 0.f, po = 0.f;     // peephole weights of unit j
+    if constexpr (PEEP) {
+        if (j < H) {
+            const float *P = a.P[dir];
+            pi = __ldg(P + j);
+            pf = __ldg(P + H + j);
+            po = __ldg(P + 2 * H + j);
+        }
+    }
 
     for (int s = 0; s < T; ++s) {
         const int t = ascending ? s : T - 1 - s;
@@ -204,7 +225,28 @@ __global__ void __launch_bounds__(LS_THREADS, KI > 0 ? 1 : 2) lstm_sweep_kernel(
             }
             const bool live = valid && t < Tb;
             const int64_t hc = ((int64_t)t * B + b) * H + j;      // (t, b, j) in the [T][B][H] arrays
-            if (!bptt) {
+            if (!bptt && PEEP) {
+                // c_prev of utterance b from the lane that wrote it, to the four gate lanes of b
+                const float cp0 = (valid && orow == 0 && live && s > 0) ? a.c[dir][((int64_t)tp * B + b) * H + j] : 0.f;
+                const float cp = __shfl_sync(0xffffffffu, cp0, ob);
+                float z = gv + acc[0];
+                if (orow == 0) z = fmaf(pi, cp, z);
+                if (orow == 1) z = fmaf(pf, cp, z);
+                float act = (orow == 2) ? tanhf(z) : lstm_sigmoid(z);
+                const float gi = __shfl_sync(0xffffffffu, act, ob), gf = __shfl_sync(0xffffffffu, act, 8 + ob);
+                const float gg = __shfl_sync(0xffffffffu, act, 16 + ob);
+                const float cn = fmaf(gf, cp, gi * gg);
+                if (orow == 3) act = lstm_sigmoid(fmaf(po, cn, z));
+                const float gO = __shfl_sync(0xffffffffu, act, 24 + ob);
+                if (valid) {
+                    a.gates[go] = live ? act : 0.f;
+                    if (orow == 0) {
+                        const float hn = gO * tanhf(cn);
+                        a.c[dir][hc] = live ? cn : 0.f;
+                        a.h[dir][hc] = live ? hn : 0.f;
+                    }
+                }
+            } else if (!bptt) {
                 const float z = gv + acc[0];
                 const float act = (orow == 2) ? tanhf(z) : lstm_sigmoid(z);
                 const float gi = __shfl_sync(0xffffffffu, act, ob), gf = __shfl_sync(0xffffffffu, act, 8 + ob);
@@ -232,14 +274,21 @@ __global__ void __launch_bounds__(LS_THREADS, KI > 0 ? 1 : 2) lstm_sweep_kernel(
                         const float ct = a.c[dir][hc], tc = tanhf(ct);
                         const bool has_prev = (tp >= 0 && tp < T), has_next = (s > 0);
                         const float cp = has_prev ? a.c[dir][((int64_t)tp * B + b) * H + j] : 0.f;
-                        const float carry = has_next ? *dcp * a.gates[((int64_t)tn * B + b) * G + gbase + H + j] : 0.f;
-                        dct = dh * gO * (1.f - tc * tc) + carry;
+                        if constexpr (PEEP) {     // the scratch holds the whole carry of the step after t
+                            dzo = dh * tc * (gO * (1.f - gO));
+                            const float carry = has_next ? *dcp : 0.f;
+                            dct = fmaf(po, dzo, dh * gO * (1.f - tc * tc)) + carry;
+                        } else {
+                            const float carry = has_next ? *dcp * a.gates[((int64_t)tn * B + b) * G + gbase + H + j] : 0.f;
+                            dct = dh * gO * (1.f - tc * tc) + carry;
+                        }
                         dzi = dct * gg * (gi * (1.f - gi));
                         dzf = dct * cp * (gf * (1.f - gf));
                         dzg = dct * gi * (1.f - gg * gg);
-                        dzo = dh * tc * (gO * (1.f - gO));
+                        if constexpr (!PEEP) dzo = dh * tc * (gO * (1.f - gO));
                     }
-                    *dcp = dct;
+                    if constexpr (PEEP) *dcp = fmaf(gf, dct, fmaf(pi, dzi, pf * dzf));
+                    else *dcp = dct;
                     float *dzp = a.dz + ((int64_t)t * B + b) * G + gbase + j;
                     dzp[0] = dzi;
                     dzp[H] = dzf;
@@ -258,27 +307,30 @@ struct LstmPlan {
     size_t smem;
 };
 
-template <int KI>
+template <int KI, bool PEEP>
 static int lstm_capacity(size_t smem, int *capacity) {
     int per_sm = 0;
-    CTCB_CUDA_CHECK(cudaFuncSetAttribute(lstm_sweep_kernel<KI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    CTCB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, lstm_sweep_kernel<KI>, LS_THREADS, smem));
+    CTCB_CUDA_CHECK(cudaFuncSetAttribute(lstm_sweep_kernel<KI, PEEP>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)smem));
+    CTCB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, lstm_sweep_kernel<KI, PEEP>, LS_THREADS, smem));
     *capacity = per_sm * num_sms();
     return CTCB_OK;
 }
 
+template <bool PEEP>
 static int lstm_capacity_of(int KI, size_t smem, int *capacity) {
     switch (KI) {
-        case 2: return lstm_capacity<2>(smem, capacity);
-        case 4: return lstm_capacity<4>(smem, capacity);
-        case 8: return lstm_capacity<8>(smem, capacity);
-        case 16: return lstm_capacity<16>(smem, capacity);
-        case 32: return lstm_capacity<32>(smem, capacity);
-        default: return lstm_capacity<0>(smem, capacity);
+        case 2: return lstm_capacity<2, PEEP>(smem, capacity);
+        case 4: return lstm_capacity<4, PEEP>(smem, capacity);
+        case 8: return lstm_capacity<8, PEEP>(smem, capacity);
+        case 16: return lstm_capacity<16, PEEP>(smem, capacity);
+        case 32: return lstm_capacity<32, PEEP>(smem, capacity);
+        default: return lstm_capacity<0, PEEP>(smem, capacity);
     }
 }
 
-int lstm_plan(int H, int B, int ndir, LstmPlan *p) {
+// the plan of the kernel that runs: the peephole mode's occupancy is its own
+int lstm_plan(int H, int B, int ndir, bool peep, LstmPlan *p) {
     if (H <= 0 || B <= 0 || (ndir != 1 && ndir != 2))
         return set_error(CTCB_EINVAL, "LSTM sweep: bad sizes (H=%d, B=%d, ndir=%d)", H, B, ndir);
     const int slices = (H + LS_UNITS - 1) / LS_UNITS;
@@ -287,7 +339,8 @@ int lstm_plan(int H, int B, int ndir, LstmPlan *p) {
     const int ki_reg = (H == 64 || H == 128 || H == 256 || H == 512 || H == 1024) ? H / 32 : 0;
     int capacity = 0;
     for (p->KI = ki_reg;; p->KI = 0) {     // U does not fit the register files of the CTAs the device holds: re-read it
-        const int rc = lstm_capacity_of(p->KI, p->smem, &capacity);
+        const int rc = peep ? lstm_capacity_of<true>(p->KI, p->smem, &capacity)
+                            : lstm_capacity_of<false>(p->KI, p->smem, &capacity);
         if (rc != CTCB_OK) return rc;
         if (ndir * slices <= capacity) break;
         if (p->KI == 0)
@@ -303,38 +356,53 @@ int lstm_plan(int H, int B, int ndir, LstmPlan *p) {
     return CTCB_OK;
 }
 
-template <int KI>
-static int lstm_launch(LstmArgs &a, int slices, const LstmPlan &p, cudaStream_t st) {
+template <int KI, bool PEEP>
+static int lstm_launch(typename LstmArgsOf<PEEP>::type &a, int slices, const LstmPlan &p, cudaStream_t st) {
     dim3 grid(slices, a.parts, a.ndir);
     void *params[] = {&a};
-    CTCB_CUDA_CHECK(cudaLaunchCooperativeKernel((void *)lstm_sweep_kernel<KI>, grid, dim3(LS_THREADS), params, p.smem, st));
+    CTCB_CUDA_CHECK(cudaLaunchCooperativeKernel((void *)lstm_sweep_kernel<KI, PEEP>, grid, dim3(LS_THREADS), params, p.smem,
+                                                st));
     count_launch();
     return CTCB_OK;
 }
 
+template <bool PEEP>
+static int lstm_launch_of(typename LstmArgsOf<PEEP>::type &a, int slices, const LstmPlan &p, cudaStream_t st) {
+    switch (p.KI) {
+        case 2: return lstm_launch<2, PEEP>(a, slices, p, st);
+        case 4: return lstm_launch<4, PEEP>(a, slices, p, st);
+        case 8: return lstm_launch<8, PEEP>(a, slices, p, st);
+        case 16: return lstm_launch<16, PEEP>(a, slices, p, st);
+        case 32: return lstm_launch<32, PEEP>(a, slices, p, st);
+        default: return lstm_launch<0, PEEP>(a, slices, p, st);
+    }
+}
+
 // ctcb_brnn_create's check that the device holds the sweep of a config; without a device there is nothing to check
 // against, and the launch checks again
-int lstm_check(int H, int B, int ndir) {
+int lstm_check(int H, int B, int ndir, bool peep) {
     int n = 0;
     if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) {
         (void)cudaGetLastError();
         return CTCB_OK;
     }
     LstmPlan p;
-    return lstm_plan(H, B, ndir, &p);
+    return lstm_plan(H, B, ndir, peep, &p);
 }
 
 size_t lstm_carry_bytes(int H, int B) { return align_up((size_t)2 * B * H * sizeof(float), 256); }
 
-// counters: 4096 bytes of device scratch (word 0 = error flag, cleared by the caller); dc: lstm_carry_bytes(H, B)
+// counters: 4096 bytes of device scratch (word 0 = error flag, cleared by the caller); dc: lstm_carry_bytes(H, B).
+// Pf (and Pb with Ub) non-null: the peephole mode.
 int run_lstm_sweep(int mode, int T, int B, int H, const int32_t *Tlen, float *gates, const float *Uf, const float *Ub,
-                   float *hF, float *hB, float *cF, float *cB, const float *dh, float *dz, unsigned int *counters,
-                   float *dc, cudaStream_t st) {
+                   const float *Pf, const float *Pb, float *hF, float *hB, float *cF, float *cB, const float *dh,
+                   float *dz, unsigned int *counters, float *dc, cudaStream_t st) {
     LstmPlan p;
     const int ndir = Ub ? 2 : 1;
-    const int rc = lstm_plan(H, B, ndir, &p);
+    const bool peep = (Pf != nullptr);
+    const int rc = lstm_plan(H, B, ndir, peep, &p);
     if (rc != CTCB_OK) return rc;
-    LstmArgs a;
+    LstmPeepArgs a;
     a.mode = mode; a.T = T; a.B = B; a.H = H; a.Tlen = Tlen; a.gates = gates;
     a.U[0] = Uf; a.U[1] = Ub ? Ub : Uf;
     a.h[0] = hF; a.h[1] = Ub ? hB : hF;
@@ -343,16 +411,86 @@ int run_lstm_sweep(int mode, int T, int B, int H, const int32_t *Tlen, float *ga
     a.parts = p.parts; a.ndir = ndir;
     a.err = counters;
     a.counters = counters + 16;     // words [0..15] are reserved for error flags
+    a.P[0] = Pf; a.P[1] = Ub ? Pb : Pf;
     CTCB_CUDA_CHECK(cudaMemsetAsync(a.counters, 0, sizeof(unsigned int) * (ndir * p.parts), st));
     const int slices = (H + LS_UNITS - 1) / LS_UNITS;
-    switch (p.KI) {
-        case 2: return lstm_launch<2>(a, slices, p, st);
-        case 4: return lstm_launch<4>(a, slices, p, st);
-        case 8: return lstm_launch<8>(a, slices, p, st);
-        case 16: return lstm_launch<16>(a, slices, p, st);
-        case 32: return lstm_launch<32>(a, slices, p, st);
-        default: return lstm_launch<0>(a, slices, p, st);
+    if (peep) return lstm_launch_of<true>(a, slices, p, st);
+    return lstm_launch_of<false>(static_cast<LstmArgs &>(a), slices, p, st);
+}
+
+// ---- the peephole weight gradients -----------------------------------------------------------------------------
+// dP_d[r][j] = sum over the rows (t, b) of dz_r[t][b][j] * c'[t][b][j], r = i, f, o (gate blocks 0, 1, 3 of direction
+// d), c' = c_{t-1} (direction 0) / c_{t+1} (direction 1) for i and f, c_t for o; c' = 0 outside 0..T-1, and dz and c are
+// 0 at the padded frames, so the sum needs no lengths.  Column q = (d, r, j) of ndir * 3H; stage 1 sums fixed chunks of
+// LPG_ROWS rows per column (32 columns x 8 row lanes per CTA), stage 2 adds the chunks in order: the bits depend only
+// on T, B, H and the inputs.
+constexpr int LPG_ROWS = 1024;
+
+__global__ void lstm_peephole_grad_stage1(const float *__restrict__ dz, const float *__restrict__ cF,
+                                          const float *__restrict__ cB, int T, int B, int H, int ndir,
+                                          float *__restrict__ partial) {
+    __shared__ float sh[8][33];
+    const int Q = ndir * 3 * H;
+    const int q = blockIdx.x * 32 + threadIdx.x;
+    const int64_t R = (int64_t)T * B;
+    const int64_t r0 = (int64_t)blockIdx.y * LPG_ROWS;
+    const int64_t r1 = (r0 + LPG_ROWS < R) ? r0 + LPG_ROWS : R;
+    float s = 0.f;
+    if (q < Q) {
+        const int d = q / (3 * H), rr = (q - d * 3 * H) / H, j = q - d * 3 * H - rr * H;
+        const int64_t G = (int64_t)ndir * 4 * H;
+        const float *z = dz + (int64_t)d * 4 * H + (int64_t)(rr == 2 ? 3 : rr) * H + j;
+        const float *c = (d == 0 ? cF : cB) + j;
+        // the row of c' relative to the row of dz: the step before in this direction's order, or the frame itself
+        const int64_t shift = (rr == 2) ? 0 : (d == 0 ? -(int64_t)B : (int64_t)B);
+        for (int64_t r = r0 + threadIdx.y; r < r1; r += 8) {
+            const int64_t rc = r + shift;
+            const float cv = (rc >= 0 && rc < R) ? __ldg(c + rc * H) : 0.f;
+            s = fmaf(__ldg(z + r * G), cv, s);
+        }
     }
+    sh[threadIdx.y][threadIdx.x] = s;
+    __syncthreads();
+    if (threadIdx.y == 0 && q < Q) {
+        float t = 0.f;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) t += sh[i][threadIdx.x];
+        partial[(int64_t)blockIdx.y * Q + q] = t;
+    }
+}
+
+template <bool ACC>
+__global__ void lstm_peephole_grad_stage2(const float *__restrict__ partial, int nblk, int H, int ndir, float *dPf,
+                                          float *dPb) {
+    const int Q = ndir * 3 * H;
+    const int q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= Q) return;
+    float s = 0.f;
+    for (int i = 0; i < nblk; ++i) s += partial[(int64_t)i * Q + q];
+    float *out = (q < 3 * H) ? dPf + q : dPb + (q - 3 * H);
+    if (ACC) s += *out;
+    *out = s;
+}
+
+size_t lstm_peephole_grad_bytes(int64_t R, int H, int ndir) {
+    const int64_t nblk = (R + LPG_ROWS - 1) / LPG_ROWS;
+    return align_up((size_t)(nblk > 0 ? nblk : 1) * ndir * 3 * H * sizeof(float), 256);
+}
+
+// cB == nullptr: one direction (dz [T][B][4H]); partial: lstm_peephole_grad_bytes(T * B, H, ndir)
+int run_lstm_peephole_grad(int T, int B, int H, const float *dz, const float *cF, const float *cB, float *dPf,
+                           float *dPb, bool accumulate, float *partial, cudaStream_t st) {
+    const int ndir = cB ? 2 : 1;
+    const int Q = ndir * 3 * H;
+    const int64_t R = (int64_t)T * B;
+    const int nblk = (int)((R + LPG_ROWS - 1) / LPG_ROWS);
+    lstm_peephole_grad_stage1<<<dim3((Q + 31) / 32, nblk), dim3(32, 8), 0, st>>>(dz, cF, cB ? cB : cF, T, B, H, ndir,
+                                                                               partial);
+    CTCB_LAUNCH_CHECK();
+    if (accumulate) lstm_peephole_grad_stage2<true><<<(Q + 127) / 128, 128, 0, st>>>(partial, nblk, H, ndir, dPf, dPb);
+    else lstm_peephole_grad_stage2<false><<<(Q + 127) / 128, 128, 0, st>>>(partial, nblk, H, ndir, dPf, dPb);
+    CTCB_LAUNCH_CHECK();
+    return CTCB_OK;
 }
 
 }  // namespace ctcb
@@ -362,28 +500,66 @@ extern "C" size_t ctcb_lstm_sweep_workspace_bytes(int H, int B) {
     return 4096 + ctcb::lstm_carry_bytes(H, B);
 }
 
-extern "C" int ctcb_lstm_sweep_f32(int mode, int T, int B, int H, const int32_t *T_per_utt, float *gates,
-                                   const float *Uf, const float *Ub, float *hF, float *hB, float *cF, float *cB,
-                                   const float *dh, float *dz, void *scratch, size_t scratch_bytes, void *stream) {
+static int lstm_sweep_entry(const char *name, int mode, int T, int B, int H, const int32_t *T_per_utt, float *gates,
+                            const float *Uf, const float *Ub, const float *Pf, const float *Pb, float *hF, float *hB,
+                            float *cF, float *cB, const float *dh, float *dz, void *scratch, size_t scratch_bytes,
+                            void *stream) {
     using namespace ctcb;
     if (!T_per_utt || !gates || !Uf || !cF || !scratch || (mode == 0 && !hF) || (mode == 1 && (!dh || !dz)) ||
         (Ub && (!cB || (mode == 0 && !hB))))
-        return set_error(CTCB_EINVAL, "ctcb_lstm_sweep_f32: null pointer argument");
+        return set_error(CTCB_EINVAL, "%s: null pointer argument", name);
     if (T <= 0 || B <= 0 || H <= 0 || (mode != 0 && mode != 1))
-        return set_error(CTCB_EINVAL, "ctcb_lstm_sweep_f32: bad sizes");
+        return set_error(CTCB_EINVAL, "%s: bad sizes", name);
     const size_t need = ctcb_lstm_sweep_workspace_bytes(H, B);
     if (scratch_bytes < need || (((uintptr_t)scratch) & 255))
-        return set_error(CTCB_ENOMEM, "ctcb_lstm_sweep_f32: scratch of %zu bytes (256-byte aligned) needed, got %zu",
-                         need, scratch_bytes);
+        return set_error(CTCB_ENOMEM, "%s: scratch of %zu bytes (256-byte aligned) needed, got %zu", name, need,
+                         scratch_bytes);
     CTCB_CUDA_CHECK(cudaMemsetAsync(scratch, 0, 16 * sizeof(unsigned int), (cudaStream_t)stream));   // error flag
-    return run_lstm_sweep(mode, T, B, H, T_per_utt, gates, Uf, Ub, hF, hB, cF, cB, dh, dz, (unsigned int *)scratch,
-                          (float *)((char *)scratch + 4096), (cudaStream_t)stream);
+    return run_lstm_sweep(mode, T, B, H, T_per_utt, gates, Uf, Ub, Pf, Pb, hF, hB, cF, cB, dh, dz,
+                          (unsigned int *)scratch, (float *)((char *)scratch + 4096), (cudaStream_t)stream);
+}
+
+extern "C" int ctcb_lstm_sweep_f32(int mode, int T, int B, int H, const int32_t *T_per_utt, float *gates,
+                                   const float *Uf, const float *Ub, float *hF, float *hB, float *cF, float *cB,
+                                   const float *dh, float *dz, void *scratch, size_t scratch_bytes, void *stream) {
+    return lstm_sweep_entry("ctcb_lstm_sweep_f32", mode, T, B, H, T_per_utt, gates, Uf, Ub, nullptr, nullptr, hF, hB,
+                            cF, cB, dh, dz, scratch, scratch_bytes, stream);
+}
+
+extern "C" int ctcb_lstm_sweep_peephole_f32(int mode, int T, int B, int H, const int32_t *T_per_utt, float *gates,
+                                            const float *Uf, const float *Ub, const float *Pf, const float *Pb,
+                                            float *hF, float *hB, float *cF, float *cB, const float *dh, float *dz,
+                                            void *scratch, size_t scratch_bytes, void *stream) {
+    if (!Pf || (Ub && !Pb)) return ctcb::set_error(CTCB_EINVAL, "ctcb_lstm_sweep_peephole_f32: null pointer argument");
+    return lstm_sweep_entry("ctcb_lstm_sweep_peephole_f32", mode, T, B, H, T_per_utt, gates, Uf, Ub, Pf, Pb, hF, hB,
+                            cF, cB, dh, dz, scratch, scratch_bytes, stream);
+}
+
+extern "C" size_t ctcb_lstm_peephole_grad_workspace_bytes(int T, int B, int H, int ndir) {
+    if (T <= 0 || B <= 0 || H <= 0 || (ndir != 1 && ndir != 2)) return 0;
+    return ctcb::lstm_peephole_grad_bytes((int64_t)T * B, H, ndir);
+}
+
+extern "C" int ctcb_lstm_peephole_grad_f32(int T, int B, int H, const float *dz, const float *cF, const float *cB,
+                                           float *dPf, float *dPb, int accumulate, void *workspace, size_t ws_bytes,
+                                           void *stream) {
+    using namespace ctcb;
+    if (!dz || !cF || !dPf || (cB && !dPb) || !workspace)
+        return set_error(CTCB_EINVAL, "ctcb_lstm_peephole_grad_f32: null pointer argument");
+    if (T <= 0 || B <= 0 || H <= 0 || (int64_t)T * B > 0x7fffffff)
+        return set_error(CTCB_EINVAL, "ctcb_lstm_peephole_grad_f32: bad sizes (T=%d, B=%d, H=%d)", T, B, H);
+    const size_t need = ctcb_lstm_peephole_grad_workspace_bytes(T, B, H, cB ? 2 : 1);
+    if (ws_bytes < need)
+        return set_error(CTCB_ENOMEM, "ctcb_lstm_peephole_grad_f32: workspace of %zu bytes needed, got %zu", need,
+                         ws_bytes);
+    return run_lstm_peephole_grad(T, B, H, dz, cF, cB, dPf, dPb, accumulate != 0, (float *)workspace,
+                                  (cudaStream_t)stream);
 }
 
 extern "C" int ctcb_debug_lstm_plan(int H, int B, int ndir, int32_t *out) {
     if (!out) return ctcb::set_error(CTCB_EINVAL, "ctcb_debug_lstm_plan: null output");
     ctcb::LstmPlan p;
-    const int rc = ctcb::lstm_plan(H, B, ndir, &p);
+    const int rc = ctcb::lstm_plan(H, B, ndir, false, &p);
     if (rc != CTCB_OK) return rc;
     out[0] = p.KI;
     out[1] = p.parts;

@@ -18,6 +18,10 @@ single contiguous vector.  New, additive surface for the minibatch/data-parallel
     NNet(..., cell='lstm')                   LSTM temporal layers instead of the clipped-ReLU recurrence (include/ctcb200.h:
                                                 the cell): each layer's affine map has ndir*4H rows, each recurrent
                                                 matrix is 4H x H; 'relu' (the default) is the reference's net
+    NNet(..., cell='lstm', peephole=True)    peephole connections of the LSTM cell (include/ctcb200.h: peephole): i and
+                                                f also see c_{t-1}, o sees c_t, through three H-vectors per direction;
+                                                one [P (3 x H), dummy] pair per direction appended to `stack` behind
+                                                everything else, P = 0 at start
     NNet(..., layerNorm=True)                layer normalisation of the ReLU hidden layers (include/ctcb200.h:
                                                 layerNorm): relu(gamma * layer_norm(z) + beta), one [gamma, beta] pair
                                                 per normalised layer appended to `stack`, gamma = 1 and beta = 0 at start
@@ -131,6 +135,15 @@ def check_ln_pairs(got, want, n_ln, what):
                          % (what, got, n_ln, want, "without" if got < want else "with more"))
 
 
+def check_peephole_pairs(got, want, peephole, what):
+    """An LSTM net loads only a checkpoint with its own number of [W, b] pairs: one of the other peephole setting has
+    [P, dummy] pairs more or fewer, which zip() would leave unset or drop."""
+    if got != want:
+        raise ValueError("the checkpoint's %s has %d tensors where this net (cell='lstm', peephole=%s) has %d: a "
+                         "checkpoint of an LSTM net %s peephole connections, or of another shape"
+                         % (what, 2 * got, peephole, 2 * want, "with" if got > want else "without"))
+
+
 class FlatList(list):
     """A stack-shaped list of [w, b] views that remembers the flat buffer it views."""
 
@@ -144,7 +157,7 @@ class NNet:
     def __init__(self, inputDim, outputDim, layerSize, numLayers, maxBatch,
                  train=True, temporalLayer=-1, reg=0.0, maxUtts=1, maxLabels=None,
                  allowTopTemporal=False, device=None, unidirectional=False, numTemporal=1, dropout=0.0,
-                 dropoutSeed=33, cell="relu", layerNorm=False, subsample=1, subsampleLayer=1):
+                 dropoutSeed=33, cell="relu", layerNorm=False, subsample=1, subsampleLayer=1, peephole=False):
         torch = _ctcb.require_cuda()
         self._torch = torch
         self.dev = torch.device("cuda", torch.cuda.current_device() if device is None else device)
@@ -189,13 +202,16 @@ class NNet:
         if cell not in _ctcb.CELLS:
             raise ValueError("cell=%r must be one of %s" % (cell, ", ".join(sorted(_ctcb.CELLS))))
         self.cell = cell
+        if peephole and cell != "lstm":
+            raise ValueError("peephole=True needs cell='lstm'; cell is %r" % (cell,))
+        self.peephole = bool(peephole)
         self.layerNorm = bool(layerNorm)
         # 0 and 1: off; the config refuses k < 0 and an L outside 1..numLayers+1 with a message (ValueError)
         self.subsample, self.subsampleLayer = int(subsample), int(subsampleLayer)
         self._cfg = BrnnConfig(inputDim, outputDim, layerSize, numLayers, max(self.temporalLayer, 0), maxBatch,
                                maxUtts, self.maxLabels, float(reg), float(self.maxAct), int(self.unidirectional),
                                self.numTemporal, _ctcb.CELLS[cell], int(self.layerNorm), self.subsample,
-                               self.subsampleLayer)
+                               self.subsampleLayer, int(self.peephole))
         self._h = ctypes.c_void_p()
         check(lib.ctcb_brnn_create(ctypes.byref(self._cfg), ctypes.byref(self._h)))
         self.stack = None
@@ -257,6 +273,9 @@ class NNet:
                 host.append([wtb, np.zeros((1, 1))])
         # [gamma, beta] of every normalised layer, behind everything else: no draw, so the other tensors are unchanged
         host += [[np.ones((H, 1)), np.zeros((H, 1))] for _ in self.normedLayers()]
+        # [P, dummy] of every direction of every peephole LSTM layer, behind those: P = 0 without a draw, so the net starts
+        # out as the same net without peepholes
+        host += [[np.zeros((3, H)), np.zeros((1, 1))] for _ in range(self.peepholeEntries())]
 
         self.nparams = int(lib.ctcb_brnn_param_count(ctypes.byref(self._cfg)))
         self.params = torch.zeros(self.nparams, dtype=torch.float32, device=self.dev)
@@ -324,6 +343,10 @@ class NNet:
             return []
         tl, k = self.temporalLayer, self.numTemporal
         return [i for i in range(1, self.numLayers + 1) if not (k and tl <= i < tl + k)]
+
+    def peepholeEntries(self):
+        """Number of [P, dummy] pairs at the end of `stack`: one per direction of every LSTM layer with peephole=True."""
+        return self.numTemporal * (1 if self.unidirectional else 2) if self.peephole else 0
 
     def frames(self, T):
         """Frames of the probabilities (and of the CTC) for an utterance of T input frames: ceil(T / k)."""
@@ -516,12 +539,19 @@ class NNet:
         except UnicodeDecodeError:          # checkpoints written by the Python-2 reference
             fid.seek(0)
             stack = pickle.load(fid, encoding="latin1")
-        if self.layerNorm:
-            check_ln_pairs(len(stack), len(self.stack), len(self.normedLayers()), "stack")
+        self.check_pair_count(stack, self.stack, "stack")
         self.check_shapes(stack, self.stack, "stack")
         for (w, b), (wi, bi) in zip(self.stack, stack):
             w.copy_(torch.from_numpy(np.ascontiguousarray(wi, dtype=np.float32).reshape(tuple(w.shape))))
             b.copy_(torch.from_numpy(np.ascontiguousarray(bi, dtype=np.float32).reshape(tuple(b.shape))))
+
+    def check_pair_count(self, got, views, what):
+        """A checkpoint's `what` (a list of [w, b]) has as many pairs as this net's: a layer-norm net refuses one with
+        other [gamma, beta] pairs, an LSTM net one of the other peephole setting."""
+        if self.cell == "lstm" and self.numTemporal:
+            check_peephole_pairs(len(got), len(views), self.peephole, what)
+        if self.layerNorm:
+            check_ln_pairs(len(got), len(views), len(self.normedLayers()), what)
 
     def check_shapes(self, got, views, what):
         """Every tensor of a checkpoint's `what` (a list of [w, b]) has the size of this net's: a checkpoint of another

@@ -7,7 +7,7 @@ last_cost, sentinel, train.log), resume through --cfg_file with the step size re
 (runNNet.py:143-166), the fixed seeds 33 (:113-115) and CUDA_DEVICE device selection (:117-120).
 The implementation is organised differently: a declarative flag table, one RunDir helper that owns the
 side files, and separate train/evaluate phases.  Site paths of run_cfg.py / decoder_config.py became
-flags (--runDir, --outDir); new flags: --numTemporal, --cell, --layerNorm, --subsample, --subsampleLayer, --batchSize, --maxUtts, --maxLabels,
+flags (--runDir, --outDir); new flags: --numTemporal, --cell, --peephole, --layerNorm, --subsample, --subsampleLayer, --batchSize, --maxUtts, --maxLabels,
 --dropout, --optimizer, --beta1, --beta2, --epsilon, --quiet.  Under torchrun the same
 script trains data-parallel (one process per GPU, one NCCL all-reduce per step).
 """
@@ -48,6 +48,8 @@ FLAGS = [
                             "recurrent (1 = the reference's single temporal layer)"),
     ("cell", str, "relu", "recurrence of the temporal layers: relu (the reference's clipped ReLU) or lstm; a cfg.json "
                           "written without it is relu"),
+    ("peephole", None, False, "peephole connections of the LSTM cell (needs --cell lstm; the cell of Graves' TIMIT and "
+                              "EESEN models); a cfg.json written without it has none"),
     ("layerNorm", None, False, "layer normalisation of the ReLU hidden layers (gamma * layer_norm(z) + beta, then "
                                "ReLU); a cfg.json written without it has none"),
     ("subsample", int, 1, "k >= 2: map --subsampleLayer reads k consecutive frames of the layer below it, and it and "
@@ -206,7 +208,8 @@ def _train(opts, cfg, run_dir, log, rank, world):
                      temporalLayer=opts.temporalLayer, reg=opts.reg, numTemporal=opts.numTemporal,
                      maxUtts=utterance_capacity(opts, world),
                      maxLabels=min(opts.maxLabels, opts.maxUttLen), dropout=opts.dropout, cell=opts.cell,
-                     layerNorm=opts.layerNorm, subsample=opts.subsample, subsampleLayer=opts.subsampleLayer)
+                     layerNorm=opts.layerNorm, subsample=opts.subsample, subsampleLayer=opts.subsampleLayer,
+                     peephole=opts.peephole)
     net.initParams()
     optimizer = sgd.SGD(net, opts.maxUttLen, alpha=opts.step, optimizer=opts.optimizer, momentum=opts.momentum,
                         batchSize=opts.batchSize, verbose=(rank == 0 and not opts.quiet), beta1=opts.beta1,
@@ -270,7 +273,7 @@ def test(opts, rank=0, world=1):
     net = rnnet.NNet(trained.inputDim, trained.outputDim, trained.layerSize, trained.numLayers, trained.maxUttLen,
                      temporalLayer=trained.temporalLayer, train=False, maxUtts=max(1, opts.maxUtts),
                      numTemporal=trained.numTemporal, cell=trained.cell, layerNorm=trained.layerNorm,
-                     subsample=trained.subsample, subsampleLayer=trained.subsampleLayer)
+                     subsample=trained.subsample, subsampleLayer=trained.subsampleLayer, peephole=trained.peephole)
     net.initParams()
     with open(trained.in_file, "rb") as fid:
         pickle.load(fid)                              # optimiser state: not needed here

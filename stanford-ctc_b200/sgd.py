@@ -135,11 +135,9 @@ class SGD:
             params = pickle.load(fid, encoding="latin1")
         it, costt, expcost, state = params
         states = unpack_state(self.optimizer, state)
-        if getattr(self.model, "layerNorm", False):
-            from nnets.brnnet import check_ln_pairs
+        if hasattr(self.model, "check_pair_count"):
             for name, stack in states.items():
-                check_ln_pairs(len(stack), len(getattr(self, name)), len(self.model.normedLayers()),
-                               "optimiser state %r" % name)
+                self.model.check_pair_count(stack, getattr(self, name), "optimiser state %r" % name)
         if hasattr(self.model, "check_shapes"):
             for name, stack in states.items():
                 self.model.check_shapes(stack, getattr(self, name), "optimiser state %r" % name)

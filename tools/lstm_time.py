@@ -5,9 +5,10 @@ temporalLayer=2, B=128, T=800, D=41, K=32, |l|=100), each built with cell='relu'
 over whole optimisation steps (sgd.SGD.step_device: CUDA graph replay, host packing and upload included as SGD.run
 does it), the arms alternated over two rounds after a warm-up; then one eager pass per arm with the per-phase events
 of ctcb_profile_* gives the two sweeps alone (sweep_fwd, sweep_bptt) and the rest of the step.  The card's name, power
-limit and clock are read in the same run.  Prints one JSON object (and writes it to --out).
+limit and clock are read in the same run.  Prints one JSON object (and writes it to --out).  With --peephole the two
+arms are the LSTM net without and with peephole connections (peephole=True), and the ratio is theirs.
 
-    python tools/lstm_time.py [--steps 5] [--warmup 4] [--shapes c2,c3] [--out FILE]
+    python tools/lstm_time.py [--steps 5] [--warmup 4] [--shapes c2,c3] [--peephole] [--out FILE]
 """
 import argparse
 import ctypes
@@ -28,12 +29,12 @@ SHAPES = {
 }
 
 
-def make_opt(c, cell):
+def make_opt(c, cell, peephole=False):
     import nnets.brnnet as rnnet
     import sgd
     np.random.seed(33)
     nn = rnnet.NNet(c["D"], c["K"], c["H"], c["N"], c["T"], temporalLayer=c["tl"], maxUtts=c["B"], maxLabels=c["L"],
-                    cell=cell)
+                    cell=cell, peephole=peephole)
     nn.initParams()
     opt = sgd.SGD(nn, c["T"], alpha=1e-5, momentum=0.9, batchSize=c["B"], verbose=False)
     opt.it = 11                      # past the momentum warm-up: one step shape
@@ -45,6 +46,7 @@ def main():
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=4)
     ap.add_argument("--shapes", default="c2,c3")
+    ap.add_argument("--peephole", action="store_true", help="time LSTM with peepholes against LSTM without")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     import torch
@@ -59,7 +61,9 @@ def main():
         datas, labels = make_batch(c, c["B"], seed=33)
         out = {}
         with torch.cuda.stream(stream):
-            arms = {cell: make_opt(c, cell) for cell in ("relu", "lstm")}
+            kinds = {"lstm": ("lstm", False), "lstm_peephole": ("lstm", True)} if args.peephole else \
+                {"relu": ("relu", False), "lstm": ("lstm", False)}
+            arms = {arm: make_opt(c, *kind) for arm, kind in kinds.items()}
             for cell, (nn, opt) in arms.items():
                 for _ in range(args.warmup):
                     one_step(opt, datas, labels)
@@ -69,7 +73,7 @@ def main():
                     rec[cell].append(time_steps(torch, opt, datas, labels, args.steps))
             for cell, (nn, opt) in arms.items():
                 plan = (ctypes.c_int32 * 2)()
-                if cell == "lstm":
+                if cell != "relu":
                     lib.ctcb_debug_lstm_plan(c["H"], c["B"], 2, plan)
                 out[cell] = dict(ms_per_step_device=[round(r[0], 3) for r in rec[cell]],
                                  ms_per_step_wall=[round(r[1], 3) for r in rec[cell]],
@@ -78,8 +82,9 @@ def main():
                                  workspace_bytes=int(lib.ctcb_brnn_workspace_bytes(ctypes.byref(nn._cfg))),
                                  params_finite=bool(torch.isfinite(nn.params).all()),
                                  sweep_error_flag=float(nn.record[3]),
-                                 lstm_plan=dict(KI=plan[0], parts=plan[1]) if cell == "lstm" else None)
-            out["lstm_over_relu_step"] = round(min(r[0] for r in rec["lstm"]) / min(r[0] for r in rec["relu"]), 3)
+                                 lstm_plan=dict(KI=plan[0], parts=plan[1]) if cell != "relu" else None)
+            a, b = list(arms)
+            out["%s_over_%s_step" % (b, a)] = round(min(r[0] for r in rec[b]) / min(r[0] for r in rec[a]), 4)
         res["shapes"][name] = dict(shape=c, arms=out)
         del arms
         torch.cuda.empty_cache()
