@@ -449,9 +449,12 @@ int ctcb_lstm_sweep_peephole_f32(int mode, int T, int B, int H, const int32_t *T
 size_t ctcb_lstm_peephole_grad_workspace_bytes(int T, int B, int H, int ndir);
 int ctcb_lstm_peephole_grad_f32(int T, int B, int H, const float *dz, const float *cF, const float *cB, float *dPf,
                                 float *dPb, int accumulate, void *workspace, size_t ws_bytes, void *stream);
-/* The LSTM sweep's plan for (H, B, ndir): out (HOST, 2 int32) = {KI (H / 32 with U in registers, else 0), utterance
- * partitions}; the error ctcb_brnn_create returns for a width the device cannot hold. */
-int ctcb_debug_lstm_plan(int H, int B, int ndir, int32_t *out);
+/* The LSTM sweep's plan for (H, B, ndir) of the kernel that runs, without (peephole = 0) or with peephole connections,
+ * under the knobs in effect (INTEGRATION.md section 4: CTCB_LSTM, CTCB_LSTM_PARTS): out (HOST, 4 int32) = {KI (H / 32
+ * with U in registers, else 0), utterance partitions, CTAs of that kernel per SM, 8-utterance tiles per partition (the
+ * last partitions may get fewer, or none)}; or the error the sweep call and ctcb_brnn_create return for a width, or a
+ * forced partition count, the device cannot hold. */
+int ctcb_debug_lstm_plan(int H, int B, int ndir, int peephole, int32_t *out);
 /* 1 when the recurrences of a (layerSize H, B utterances, bi-directional) step run on the tensor-core kernel. */
 int ctcb_sweep_uses_tensor_cores(int H, int B);
 /* The plan ctcb_brnn_sweep_f32 launches for (H, B, ndir = 2 bi-directional / 1 forward in time only) on the current

@@ -86,7 +86,7 @@ _PROTOS = {
                                              c_vp, c_vp, c_vp, c_vp, c_vp, c_sz, c_vp]),
     "ctcb_lstm_peephole_grad_workspace_bytes": (c_sz, [c_int, c_int, c_int, c_int]),
     "ctcb_lstm_peephole_grad_f32": (c_int, [c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_sz, c_vp]),
-    "ctcb_debug_lstm_plan": (c_int, [c_int, c_int, c_int, ctypes.POINTER(ctypes.c_int32)]),
+    "ctcb_debug_lstm_plan": (c_int, [c_int, c_int, c_int, c_int, ctypes.POINTER(ctypes.c_int32)]),
     "ctcb_layernorm_workspace_bytes": (c_sz, [c_i64, c_int]),
     "ctcb_layernorm_forward_f32": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_int, c_vp]),
     "ctcb_layernorm_backward_f32": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_int, c_int, c_vp, c_sz,

@@ -44,9 +44,10 @@ static void stream_priority_range(int *least, int *greatest) {
 int stream_priority_least() { int lo, hi; stream_priority_range(&lo, &hi); return lo; }
 int stream_priority_greatest() { int lo, hi; stream_priority_range(&lo, &hi); return hi; }
 
-// The documented values of each knob, in the order of enum Knob: the string values[v] sets the value v.  A value the
-// environment gives that is not listed here leaves the default in effect.
-struct KnobDef { const char *name; int dflt; const char *values[9]; };
+// The documented values of each knob, in the order of enum Knob: the string values[v] sets the value v, and where
+// count > 0 the decimal numbers 1..count set themselves.  A value the environment gives that is not listed here leaves
+// the default in effect.
+struct KnobDef { const char *name; int dflt; const char *values[9]; int count; };
 static const KnobDef KNOBS[KNOB_COUNT] = {
     {"CTCB_GEMM", 0, {nullptr, "simt"}},
     {"CTCB_GEMM_TC_COPY", 0, {"0", "1"}},
@@ -58,6 +59,8 @@ static const KnobDef KNOBS[KNOB_COUNT] = {
     {"CTCB_SWEEP_TC_COOP", 1, {"0"}},
     {"CTCB_SWEEP_TRACE", 0, {nullptr, "1"}},
     {"CTCB_CTC", 0, {"auto", "warp", "pair", "par", "ckpt"}},
+    {"CTCB_LSTM", 0, {"auto", "reread"}},
+    {"CTCB_LSTM_PARTS", 0, {"auto"}, LSTM_MAX_PARTS},
 };
 static int g_knob_initial[KNOB_COUNT], g_knob[KNOB_COUNT];     // what the environment said, what is in effect
 static std::once_flag g_knob_once;
@@ -65,6 +68,14 @@ static std::once_flag g_knob_once;
 static int parse_knob(const KnobDef &d, const char *s) {
     for (int v = 0; v < 9; ++v)
         if (d.values[v] && strcmp(d.values[v], s) == 0) return v;
+    if (d.count > 0 && s[0] >= '1' && s[0] <= '9' && strlen(s) <= 9) {
+        int v = 0;
+        for (const char *c = s; *c; ++c) {
+            if (*c < '0' || *c > '9') return -1;
+            v = 10 * v + (*c - '0');
+        }
+        if (v <= d.count) return v;
+    }
     return -1;
 }
 

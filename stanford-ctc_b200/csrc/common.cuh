@@ -40,8 +40,11 @@ int stream_priority_greatest();
 // Debug / measurement overrides of the planners (INTEGRATION.md section 4): one table (common.cu), filled from the
 // environment at first use and changed by ctcb_debug_set_knob.  Planners read it through knob() on every planning call.
 enum Knob { KNOB_GEMM, KNOB_GEMM_TC_COPY, KNOB_GEMM_TRACE, KNOB_SWEEP, KNOB_SWEEP_NB, KNOB_SWEEP_TC, KNOB_SWEEP_TC_CS,
-            KNOB_SWEEP_TC_COOP, KNOB_SWEEP_TRACE, KNOB_CTC, KNOB_COUNT };
+            KNOB_SWEEP_TC_COOP, KNOB_SWEEP_TRACE, KNOB_CTC, KNOB_LSTM, KNOB_LSTM_PARTS, KNOB_COUNT };
 int knob(Knob k);
+// The most utterance partitions of an LSTM sweep: its barrier counters ([ndir][parts] words) share 4 KB of scratch with
+// the error flags.  CTCB_LSTM_PARTS takes auto or 1..LSTM_MAX_PARTS.
+constexpr int LSTM_MAX_PARTS = 500;
 
 // Optional per-phase device timing (ctcb_profile_*): CUDA events recorded on the launching stream
 // around each phase of the step; off by default so the timed benchmark region carries no events.

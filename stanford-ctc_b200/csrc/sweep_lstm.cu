@@ -304,44 +304,46 @@ __global__ void __launch_bounds__(LS_THREADS, KI > 0 ? 1 : 2) lstm_sweep_kernel(
 // The launch of (H, B, ndir): register-resident U where its CTAs fit one per SM, else U re-read at two CTAs per SM.
 struct LstmPlan {
     int KI, parts;
+    int per_sm;                // CTAs of this kernel one SM holds
     size_t smem;
 };
 
 template <int KI, bool PEEP>
-static int lstm_capacity(size_t smem, int *capacity) {
-    int per_sm = 0;
+static int lstm_occupancy(size_t smem, int *per_sm) {
     CTCB_CUDA_CHECK(cudaFuncSetAttribute(lstm_sweep_kernel<KI, PEEP>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          (int)smem));
-    CTCB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, lstm_sweep_kernel<KI, PEEP>, LS_THREADS, smem));
-    *capacity = per_sm * num_sms();
+    CTCB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(per_sm, lstm_sweep_kernel<KI, PEEP>, LS_THREADS, smem));
     return CTCB_OK;
 }
 
 template <bool PEEP>
-static int lstm_capacity_of(int KI, size_t smem, int *capacity) {
+static int lstm_occupancy_of(int KI, size_t smem, int *per_sm) {
     switch (KI) {
-        case 2: return lstm_capacity<2, PEEP>(smem, capacity);
-        case 4: return lstm_capacity<4, PEEP>(smem, capacity);
-        case 8: return lstm_capacity<8, PEEP>(smem, capacity);
-        case 16: return lstm_capacity<16, PEEP>(smem, capacity);
-        case 32: return lstm_capacity<32, PEEP>(smem, capacity);
-        default: return lstm_capacity<0, PEEP>(smem, capacity);
+        case 2: return lstm_occupancy<2, PEEP>(smem, per_sm);
+        case 4: return lstm_occupancy<4, PEEP>(smem, per_sm);
+        case 8: return lstm_occupancy<8, PEEP>(smem, per_sm);
+        case 16: return lstm_occupancy<16, PEEP>(smem, per_sm);
+        case 32: return lstm_occupancy<32, PEEP>(smem, per_sm);
+        default: return lstm_occupancy<0, PEEP>(smem, per_sm);
     }
 }
 
-// the plan of the kernel that runs: the peephole mode's occupancy is its own
+// the plan of the kernel that runs: the peephole mode's occupancy is its own.  CTCB_LSTM=reread takes KI = 0 at any
+// H; CTCB_LSTM_PARTS forces the partition count, refused here, before any launch, where its CTAs cannot all be
+// co-resident.
 int lstm_plan(int H, int B, int ndir, bool peep, LstmPlan *p) {
     if (H <= 0 || B <= 0 || (ndir != 1 && ndir != 2))
         return set_error(CTCB_EINVAL, "LSTM sweep: bad sizes (H=%d, B=%d, ndir=%d)", H, B, ndir);
     const int slices = (H + LS_UNITS - 1) / LS_UNITS;
     const int Hp = (H + 3) / 4 * 4 + 4;
     p->smem = (size_t)LS_NB * Hp * sizeof(float);
-    const int ki_reg = (H == 64 || H == 128 || H == 256 || H == 512 || H == 1024) ? H / 32 : 0;
+    const bool reg = (H == 64 || H == 128 || H == 256 || H == 512 || H == 1024) && knob(KNOB_LSTM) == 0;
     int capacity = 0;
-    for (p->KI = ki_reg;; p->KI = 0) {     // U does not fit the register files of the CTAs the device holds: re-read it
-        const int rc = peep ? lstm_capacity_of<true>(p->KI, p->smem, &capacity)
-                            : lstm_capacity_of<false>(p->KI, p->smem, &capacity);
+    for (p->KI = reg ? H / 32 : 0;; p->KI = 0) {   // U does not fit the register files the device holds: re-read it
+        const int rc = peep ? lstm_occupancy_of<true>(p->KI, p->smem, &p->per_sm)
+                            : lstm_occupancy_of<false>(p->KI, p->smem, &p->per_sm);
         if (rc != CTCB_OK) return rc;
+        capacity = p->per_sm * num_sms();
         if (ndir * slices <= capacity) break;
         if (p->KI == 0)
             return set_error(CTCB_EINVAL, "LSTM sweep: layerSize %d needs %d co-resident CTAs, device holds %d", H,
@@ -349,8 +351,14 @@ int lstm_plan(int H, int B, int ndir, bool peep, LstmPlan *p) {
     }
     const int ntiles = (B + LS_NB - 1) / LS_NB;
     int parts = capacity / (ndir * slices);
+    if (knob(KNOB_LSTM_PARTS)) {
+        if (knob(KNOB_LSTM_PARTS) > parts)
+            return set_error(CTCB_EINVAL, "LSTM sweep: CTCB_LSTM_PARTS=%d needs %d co-resident CTAs, device holds %d",
+                             knob(KNOB_LSTM_PARTS), knob(KNOB_LSTM_PARTS) * ndir * slices, capacity);
+        parts = knob(KNOB_LSTM_PARTS);
+    }
     if (parts > ntiles) parts = ntiles;
-    if (parts > 500) parts = 500;   // the counters region holds 1024 words
+    if (parts > LSTM_MAX_PARTS) parts = LSTM_MAX_PARTS;
     if (parts < 1) parts = 1;
     p->parts = parts;
     return CTCB_OK;
@@ -556,12 +564,15 @@ extern "C" int ctcb_lstm_peephole_grad_f32(int T, int B, int H, const float *dz,
                                   (cudaStream_t)stream);
 }
 
-extern "C" int ctcb_debug_lstm_plan(int H, int B, int ndir, int32_t *out) {
+extern "C" int ctcb_debug_lstm_plan(int H, int B, int ndir, int peephole, int32_t *out) {
     if (!out) return ctcb::set_error(CTCB_EINVAL, "ctcb_debug_lstm_plan: null output");
     ctcb::LstmPlan p;
-    const int rc = ctcb::lstm_plan(H, B, ndir, false, &p);
+    const int rc = ctcb::lstm_plan(H, B, ndir, peephole != 0, &p);
     if (rc != CTCB_OK) return rc;
+    const int ntiles = (B + ctcb::LS_NB - 1) / ctcb::LS_NB;
     out[0] = p.KI;
     out[1] = p.parts;
+    out[2] = p.per_sm;
+    out[3] = (ntiles + p.parts - 1) / p.parts;
     return CTCB_OK;
 }

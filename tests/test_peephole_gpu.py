@@ -1,16 +1,10 @@
 """GPU tests of the peephole connections of the LSTM cell (ctcb_brnn_config.peephole = 1) on one H100.
 
-The sweep alone (ctcb_lstm_sweep_peephole_f32) against the float64 recurrence of tests/peephole_oracle.py computed
-from the kernel's own float32 inputs, element-wise, with the bound of tests/test_lstm_gpu.py: |x - x64| <= C u S,
-u = 2^-24, S the sum of the magnitudes of the terms that make x, the float64 of the step computed from the GPU's own state of the
-step before (S = 1 + |pre| + |U| |h_prev| + |p| |c_prev| for the i and f gates, + |p_o| |c_t| for o; |f c_prev| + |i g|
-for c; |o| for h), C = 8; dz, which carries the whole dc term from step to step inside the kernel, against the float64
-BPTT of the GPU's own forward activations with S = max(1, max |dz64|), C = 32.  The peephole weight gradients
-(ctcb_lstm_peephole_grad_f32) against float64 of their inputs with a bound derived below.  Then the whole net
-against peephole_oracle.PeepholeNet (tests/net_check.py) with P drawn non-zero, and micro-batches, shards, graph
+The sweep alone in peephole mode (ctcb_lstm_sweep_peephole_f32), on every plan, and the peephole weight gradients
+alone (ctcb_lstm_peephole_grad_f32) are tests/test_lstm_plans_gpu.py.  Here the whole net against
+peephole_oracle.PeepholeNet (tests/net_check.py) with P drawn non-zero, and micro-batches, shards, graph
 replay, forward-only probabilities, runNNet and checkpoints.  Each comparison prints its measured numbers as one JSON
 line (pytest -s)."""
-import ctypes
 import json
 import os
 import pickle
@@ -20,158 +14,10 @@ import pytest
 
 import recipes
 from net_check import bits as _bits, compare, rel as _rel
-from peephole_oracle import PeepholeNet, lstm_direction_bptt
+from peephole_oracle import PeepholeNet
 
 pytestmark = pytest.mark.gpu
-U32 = 2.0 ** -24
-C_FWD, C_BPTT = 8.0, 32.0
 COST_TOL, FWD_TOL, GRAD_TOL = 1e-4, 1e-4, 1e-4
-
-
-def _sig(z):
-    return 1.0 / (1.0 + np.exp(-z))
-
-
-def _p(t):
-    return None if t is None else t.data_ptr()
-
-
-# ------------------------------------------------------------------------------------------------ the sweep alone
-SWEEPS = [(H, uni, B, T) for H in (64, 70, 512, 1024) for uni in (False, True) for B, T in ((1, 1), (13, 9))] + \
-    [(1024, False, 128, 5), (70, True, 128, 4), (512, False, 128, 3)]
-
-
-@pytest.mark.parametrize("H,uni,B,T", SWEEPS)
-def test_peephole_sweep_matches_float64(H, uni, B, T, cuda):
-    torch = cuda
-    from _ctcb import lib, check
-    ndir = 1 if uni else 2
-    G = ndir * 4 * H
-    plan = (ctypes.c_int32 * 2)()
-    check(lib.ctcb_debug_lstm_plan(H, B, ndir, plan))
-    rng = np.random.RandomState(H + B + T + 1)
-    lens = rng.randint(1, T + 1, size=B).astype(np.int32)
-    lens[0] = T
-    pre = rng.uniform(-1.5, 1.5, (T, B, G)).astype(np.float32)
-    s = 1.5 / np.sqrt(H)
-    Us = [rng.uniform(-s, s, (4 * H, H)).astype(np.float32) for _ in range(ndir)]
-    Ps = [rng.uniform(-0.5, 0.5, (3, H)).astype(np.float32) for _ in range(ndir)]
-    dh = rng.randn(T, B, H).astype(np.float32)
-    dev = torch.device("cuda")
-    d_pre = torch.from_numpy(pre).to(dev)
-    d_U = [torch.from_numpy(u).to(dev) for u in Us]
-    d_P = [torch.from_numpy(x).to(dev) for x in Ps]
-    d_h = [torch.full((T, B, H), float("nan"), device=dev) for _ in range(ndir)]
-    d_c = [torch.full((T, B, H), float("nan"), device=dev) for _ in range(ndir)]
-    d_dh = torch.from_numpy(dh).to(dev)
-    d_dz = torch.full((T, B, G), float("nan"), device=dev)
-    d_len = torch.from_numpy(lens).to(dev)
-    ws = lib.ctcb_lstm_sweep_workspace_bytes(H, B)
-    scratch = torch.zeros(ws, dtype=torch.uint8, device=dev)
-    st = torch.cuda.current_stream().cuda_stream
-    Ub, Pb, hB, cB = (None, None, None, None) if uni else (d_U[1], d_P[1], d_h[1], d_c[1])
-    check(lib.ctcb_lstm_sweep_peephole_f32(0, T, B, H, _p(d_len), _p(d_pre), _p(d_U[0]), _p(Ub), _p(d_P[0]), _p(Pb),
-                                           _p(d_h[0]), _p(hB), _p(d_c[0]), _p(cB), None, None, _p(scratch), ws, st))
-    check(lib.ctcb_lstm_sweep_peephole_f32(1, T, B, H, _p(d_len), _p(d_pre), _p(d_U[0]), _p(Ub), _p(d_P[0]), _p(Pb),
-                                           None, None, _p(d_c[0]), _p(cB), _p(d_dh), _p(d_dz), _p(scratch), ws, st))
-    torch.cuda.synchronize()
-    assert int(scratch[:4].view(torch.int32).item()) == 0
-    gates = d_pre.cpu().numpy().astype(np.float64)
-    hs = [x.cpu().numpy().astype(np.float64) for x in d_h]
-    cs = [x.cpu().numpy().astype(np.float64) for x in d_c]
-    dz = d_dz.cpu().numpy().astype(np.float64)
-    ratio = dict(gates=0.0, c=0.0, h=0.0, dz=0.0)
-    for u in range(B):
-        Tu = int(lens[u])
-        for d in range(ndir):
-            blk = slice(d * 4 * H, (d + 1) * 4 * H)
-            for arr in (gates[Tu:, u, blk], hs[d][Tu:, u], cs[d][Tu:, u], dz[Tu:, u, blk]):
-                assert not np.any(arr), "padded frame not 0"
-            U, P = Us[d].astype(np.float64), Ps[d].astype(np.float64)
-            g, c, h = gates[:Tu, u, blk].T, cs[d][:Tu, u].T, hs[d][:Tu, u].T
-            pz = pre[:Tu, u, blk].T.astype(np.float64)
-            for t in range(Tu):
-                tp = t + 1 if d == 1 else t - 1
-                hp = h[:, tp] if 0 <= tp < Tu else np.zeros(H)
-                cp = c[:, tp] if 0 <= tp < Tu else np.zeros(H)
-                z = pz[:, t] + U.dot(hp)
-                Sz = 1.0 + np.abs(pz[:, t]) + np.abs(U).dot(np.abs(hp))
-                i64 = _sig(z[:H] + P[0] * cp)
-                f64 = _sig(z[H:2 * H] + P[1] * cp)
-                g64 = np.tanh(z[2 * H:3 * H])
-                o64 = _sig(z[3 * H:] + P[2] * c[:, t])     # from the GPU's own c_t
-                S = Sz + np.concatenate([np.abs(P[0] * cp), np.abs(P[1] * cp), np.zeros(H), np.abs(P[2] * c[:, t])])
-                a64 = np.concatenate([i64, f64, g64, o64])
-                ratio["gates"] = max(ratio["gates"], float(np.max(np.abs(g[:, t] - a64) / (U32 * S))))
-                i_, f_, g_, o_ = g[:H, t], g[H:2 * H, t], g[2 * H:3 * H, t], g[3 * H:, t]
-                c64 = f_ * cp + i_ * g_
-                Sc = np.abs(f_ * cp) + np.abs(i_ * g_) + 1e-30
-                ratio["c"] = max(ratio["c"], float(np.max(np.abs(c[:, t] - c64) / (U32 * Sc))))
-                h64 = o_ * np.tanh(c[:, t])
-                ratio["h"] = max(ratio["h"], float(np.max(np.abs(h[:, t] - h64) / (U32 * (np.abs(o_) + 1e-30)))))
-            dz64, _, _ = lstm_direction_bptt(dh[:Tu, u].T.astype(np.float64), g, c, h, U, reverse=(d == 1), peephole=P)
-            S = max(1.0, float(np.max(np.abs(dz64))))
-            ratio["dz"] = max(ratio["dz"], float(np.max(np.abs(dz[:Tu, u, blk].T - dz64)) / (U32 * S)))
-    print(json.dumps({"peephole_sweep_H%d_%s_B%d_T%d" % (H, "uni" if uni else "bi", B, T):
-                      dict(plan_KI=plan[0], parts=plan[1], **ratio)}))
-    assert ratio["gates"] <= C_FWD and ratio["c"] <= C_FWD and ratio["h"] <= C_FWD
-    assert ratio["dz"] <= C_BPTT
-
-
-# ------------------------------------------------------------------------------------------------ dP alone
-@pytest.mark.parametrize("T,B,H,ndir", [(1, 3, 64, 2), (9, 13, 70, 1), (37, 5, 512, 2), (300, 8, 1024, 2)])
-def test_peephole_grad_matches_float64(T, B, H, ndir, cuda):
-    """dP against float64 of the same float32 dz and c.  Each output is a sum of n = T B products, each product exact
-    to u in float32 and the sum of fixed chunks of 1024 rows (8 interleaved partial sums of 128 products each, combined
-    in a tree of 8, then the chunks in order): a recursive sum of m terms errs by at most (m - 1) u sum |terms|, so the
-    bound is (128 + 8 + ceil(n / 1024) + 1) u sum |dz c'|.  A rerun is bit-identical, and accumulate adds."""
-    torch = cuda
-    from _ctcb import lib, check
-    rng = np.random.RandomState(T + B + H)
-    G = ndir * 4 * H
-    lens = rng.randint(1, T + 1, size=B)
-    lens[0] = T
-    mask = (np.arange(T)[:, None] < lens[None, :]).astype(np.float32)        # [T][B]
-    dz = (rng.randn(T, B, G) * mask[:, :, None]).astype(np.float32)
-    cs = [(rng.randn(T, B, H) * mask[:, :, None]).astype(np.float32) for _ in range(ndir)]
-    dev = torch.device("cuda")
-    d_dz = torch.from_numpy(dz).to(dev)
-    d_c = [torch.from_numpy(c).to(dev) for c in cs]
-    d_dP = [torch.full((3, H), float("nan"), device=dev) for _ in range(ndir)]
-    nbytes = lib.ctcb_lstm_peephole_grad_workspace_bytes(T, B, H, ndir)
-    ws = torch.zeros(nbytes, dtype=torch.uint8, device=dev)
-    st = torch.cuda.current_stream().cuda_stream
-    cB, dPb = (None, None) if ndir == 1 else (d_c[1], d_dP[1])
-
-    def run(acc):
-        check(lib.ctcb_lstm_peephole_grad_f32(T, B, H, _p(d_dz), _p(d_c[0]), _p(cB), _p(d_dP[0]), _p(dPb), acc, _p(ws),
-                                              nbytes, st))
-        torch.cuda.synchronize()
-        return [x.cpu().numpy().copy() for x in d_dP]
-
-    first = run(0)
-    again = run(0)
-    twice = run(1)
-    n = T * B
-    K = 128 + 8 + (n + 1023) // 1024 + 1
-    worst = 0.0
-    for d in range(ndir):
-        blk = dz[:, :, d * 4 * H:(d + 1) * 4 * H].astype(np.float64)
-        c = cs[d].astype(np.float64)
-        cprev = np.zeros_like(c)
-        if d == 0:
-            cprev[1:] = c[:-1]
-        else:
-            cprev[:-1] = c[1:]
-        terms = [blk[:, :, :H] * cprev, blk[:, :, H:2 * H] * cprev, blk[:, :, 3 * H:] * c]
-        want = np.stack([x.sum(axis=(0, 1)) for x in terms])
-        S = np.stack([np.abs(x).sum(axis=(0, 1)) for x in terms]) + 1e-30
-        worst = max(worst, float(np.max(np.abs(first[d] - want) / (K * U32 * S))))
-        assert np.array_equal(first[d].view(np.uint32), again[d].view(np.uint32))
-        assert np.array_equal(twice[d], first[d] + first[d])       # x + x is exact
-    print(json.dumps({"peephole_grad_T%d_B%d_H%d_%s" % (T, B, H, "bi" if ndir == 2 else "uni"):
-                      dict(ratio_to_bound=worst, bound_C=K)}))
-    assert worst <= 1.0
 
 
 # ------------------------------------------------------------------------------------------------ the whole net

@@ -72,9 +72,9 @@ def main():
                 for cell, (nn, opt) in arms.items():
                     rec[cell].append(time_steps(torch, opt, datas, labels, args.steps))
             for cell, (nn, opt) in arms.items():
-                plan = (ctypes.c_int32 * 2)()
+                plan = (ctypes.c_int32 * 4)()
                 if cell != "relu":
-                    lib.ctcb_debug_lstm_plan(c["H"], c["B"], 2, plan)
+                    lib.ctcb_debug_lstm_plan(c["H"], c["B"], 2, int(kinds[cell][1]), plan)
                 out[cell] = dict(ms_per_step_device=[round(r[0], 3) for r in rec[cell]],
                                  ms_per_step_wall=[round(r[1], 3) for r in rec[cell]],
                                  phases_ms=phase_profile(torch, opt, datas, labels),
@@ -82,7 +82,8 @@ def main():
                                  workspace_bytes=int(lib.ctcb_brnn_workspace_bytes(ctypes.byref(nn._cfg))),
                                  params_finite=bool(torch.isfinite(nn.params).all()),
                                  sweep_error_flag=float(nn.record[3]),
-                                 lstm_plan=dict(KI=plan[0], parts=plan[1]) if cell != "relu" else None)
+                                 lstm_plan=dict(KI=plan[0], parts=plan[1], per_sm=plan[2], tiles_per_part=plan[3])
+                                 if cell != "relu" else None)
             a, b = list(arms)
             out["%s_over_%s_step" % (b, a)] = round(min(r[0] for r in rec[b]) / min(r[0] for r in rec[a]), 4)
         res["shapes"][name] = dict(shape=c, arms=out)
