@@ -312,6 +312,10 @@ size_t ctcb_brnn_forward_workspace_bytes(const ctcb_brnn_config *cfg, size_t *er
  * map L, [Tmax'][B][k n] (`layer` is ignored). */
 int ctcb_brnn_activation_offset(const ctcb_brnn_config *cfg, int what, int layer, size_t *offset, int32_t *width);
 
+/* With temporal layers, refuses (CTCB_EINVAL, with the planner's message) a config whose recurrent sweep the device
+ * cannot hold at maxB: the LSTM sweep (above), or for cell = 0 the plan ctcb_debug_sweep_plan(layerSize, maxB, ndir)
+ * reports, whose tensor-core plan shrinks with the batch and whose generic plan needs ndir * ceil(H / 32) co-resident
+ * CTAs at any batch.  Without a device nothing is checked. */
 int ctcb_brnn_create(const ctcb_brnn_config *cfg, ctcb_brnn **out);
 void ctcb_brnn_destroy(ctcb_brnn *h);
 
@@ -458,13 +462,15 @@ int ctcb_debug_lstm_plan(int H, int B, int ndir, int peephole, int32_t *out);
 /* 1 when the recurrences of a (layerSize H, B utterances, bi-directional) step run on the tensor-core kernel. */
 int ctcb_sweep_uses_tensor_cores(int H, int B);
 /* The plan ctcb_brnn_sweep_f32 launches for (H, B, ndir = 2 bi-directional / 1 forward in time only) on the current
- * device, under the knobs in effect (INTEGRATION.md section 4).  out (HOST, 8 int32):
+ * device, under the knobs in effect (INTEGRATION.md section 4: CTCB_SWEEP*).  out (HOST, 8 int32):
  *   {kernel: 0 generic / 1 cluster / 2 tensor-core, KI (H / 32 with register-resident weights, else 0),
  *    CS (tensor-core: K-slices per cluster; cluster: CTAs per cluster; generic: 0),
  *    NB (cluster: utterances per cluster) or NS (tensor-core: utterance splits) or the generic kernel's partitions,
  *    NP (tensor-core: utterances per split), ring stages, partial_own (tensor-core: 1 when the split-K partial has its
- *    own shared memory), 0}.
- * Returns the error the launch itself would return for a plan the device cannot hold. */
+ *    own shared memory), CTAs of the generic kernel per SM (other kernels: 0)}.
+ * Returns the error the launch itself, and ctcb_brnn_create for a ReLU net of that width at maxB, would return for a
+ * plan the device cannot hold: CTCB_EINVAL for a width whose shared memory or co-resident CTAs exceed the device, or a
+ * forced partition count it cannot hold co-resident. */
 int ctcb_debug_sweep_plan(int H, int B, int ndir, int32_t *out);
 
 /* ---- optimiser (replaces sgd.SGD.run arithmetic, ctc_fast/sgd.py:91-161, and

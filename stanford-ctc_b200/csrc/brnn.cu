@@ -36,6 +36,7 @@ int run_lstm_sweep(int mode, int T, int B, int H, const int32_t *Tlen, float *ga
                    const float *Pf, const float *Pb, float *hF, float *hB, float *cF, float *cB, const float *dh,
                    float *dz, unsigned int *counters, float *dc, cudaStream_t st);
 int lstm_check(int H, int B, int ndir, bool peep);
+int sweep_check(int H, int B, int ndir);
 size_t lstm_peephole_grad_bytes(int64_t R, int H, int ndir);
 int run_lstm_peephole_grad(int T, int B, int H, const float *dz, const float *cF, const float *cB, float *dPf,
                            float *dPb, bool accumulate, float *partial, cudaStream_t st);
@@ -725,8 +726,10 @@ extern "C" int ctcb_brnn_create(const ctcb_brnn_config *cfg, ctcb_brnn **out) {
     if (h->cfg.maxAct <= 0.f) h->cfg.maxAct = 20.0f;   // brnnet.py:32
     h->tl = eff_tl(cfg);
     h->nt = eff_nt(cfg);
-    if (cfg->cell == 1 && h->nt) {      // a width whose LSTM sweep the device cannot hold co-resident
-        const int rc = lstm_check(cfg->layerSize, cfg->maxB, cfg->unidirectional ? 1 : 2, cfg->peephole == 1);
+    if (h->nt) {      // a width or batch whose sweep the device cannot hold co-resident
+        const int ndir = cfg->unidirectional ? 1 : 2;
+        const int rc = cfg->cell == 1 ? lstm_check(cfg->layerSize, cfg->maxB, ndir, cfg->peephole == 1)
+                                      : sweep_check(cfg->layerSize, cfg->maxB, ndir);
         if (rc != CTCB_OK) {
             char why[512];
             snprintf(why, sizeof(why), "%s", ctcb_last_error());

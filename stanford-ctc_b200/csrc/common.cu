@@ -31,6 +31,19 @@ int num_sms() {
     return n;
 }
 
+size_t max_smem_optin() {
+    static int n = 0;
+    if (n == 0) {
+        int dev = 0;
+        if (cudaGetDevice(&dev) != cudaSuccess ||
+            cudaDeviceGetAttribute(&n, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess) {
+            cudaGetLastError();
+            return 232448;
+        }
+    }
+    return (size_t)n;
+}
+
 static void stream_priority_range(int *least, int *greatest) {
     static int lo = 0, hi = 0;
     static bool read = false;
@@ -52,7 +65,7 @@ static const KnobDef KNOBS[KNOB_COUNT] = {
     {"CTCB_GEMM", 0, {nullptr, "simt"}},
     {"CTCB_GEMM_TC_COPY", 0, {"0", "1"}},
     {"CTCB_GEMM_TRACE", 0, {nullptr, "1"}},
-    {"CTCB_SWEEP", 0, {nullptr, "barrier"}},
+    {"CTCB_SWEEP", 0, {"auto", "barrier", "reread"}},
     {"CTCB_SWEEP_NB", 0, {nullptr, "1", "2", "3", "4", "5", "6", "7", "8"}},
     {"CTCB_SWEEP_TC", 1, {"0", "1", "2"}},
     {"CTCB_SWEEP_TC_CS", 4, {nullptr, "1", "2", nullptr, "4"}},
@@ -61,6 +74,7 @@ static const KnobDef KNOBS[KNOB_COUNT] = {
     {"CTCB_CTC", 0, {"auto", "warp", "pair", "par", "ckpt"}},
     {"CTCB_LSTM", 0, {"auto", "reread"}},
     {"CTCB_LSTM_PARTS", 0, {"auto"}, LSTM_MAX_PARTS},
+    {"CTCB_SWEEP_PARTS", 0, {"auto"}, SWEEP_MAX_PARTS},
 };
 static int g_knob_initial[KNOB_COUNT], g_knob[KNOB_COUNT];     // what the environment said, what is in effect
 static std::once_flag g_knob_once;

@@ -33,6 +33,9 @@ inline void count_launch(int n = 1) { g_launch_count.fetch_add((uint64_t)n, std:
     } while (0)
 
 int num_sms();
+// The most dynamic shared memory one CTA can opt in to (cudaDevAttrMaxSharedMemoryPerBlockOptin).  A planner refuses a
+// footprint above it with CTCB_EINVAL before it asks for the kernel attribute, whose failure is a CUDA error.
+size_t max_smem_optin();
 // The device's stream priority range (cudaDeviceGetStreamPriorityRange): least is the default, greatest runs first.
 int stream_priority_least();
 int stream_priority_greatest();
@@ -40,11 +43,13 @@ int stream_priority_greatest();
 // Debug / measurement overrides of the planners (INTEGRATION.md section 4): one table (common.cu), filled from the
 // environment at first use and changed by ctcb_debug_set_knob.  Planners read it through knob() on every planning call.
 enum Knob { KNOB_GEMM, KNOB_GEMM_TC_COPY, KNOB_GEMM_TRACE, KNOB_SWEEP, KNOB_SWEEP_NB, KNOB_SWEEP_TC, KNOB_SWEEP_TC_CS,
-            KNOB_SWEEP_TC_COOP, KNOB_SWEEP_TRACE, KNOB_CTC, KNOB_LSTM, KNOB_LSTM_PARTS, KNOB_COUNT };
+            KNOB_SWEEP_TC_COOP, KNOB_SWEEP_TRACE, KNOB_CTC, KNOB_LSTM, KNOB_LSTM_PARTS, KNOB_SWEEP_PARTS, KNOB_COUNT };
 int knob(Knob k);
 // The most utterance partitions of an LSTM sweep: its barrier counters ([ndir][parts] words) share 4 KB of scratch with
 // the error flags.  CTCB_LSTM_PARTS takes auto or 1..LSTM_MAX_PARTS.
 constexpr int LSTM_MAX_PARTS = 500;
+// The same for the generic recurrent sweep (sweep.cu), whose counters take the same scratch: CTCB_SWEEP_PARTS.
+constexpr int SWEEP_MAX_PARTS = 500;
 
 // Optional per-phase device timing (ctcb_profile_*): CUDA events recorded on the launching stream
 // around each phase of the step; off by default so the timed benchmark region carries no events.
@@ -81,6 +86,7 @@ struct SweepPlan {
     int partial_own;        // tensor-core: 1 when the partial product has a shared-memory region of its own
     uint32_t stage_bytes;   // tensor-core: bytes per ring stage
     size_t smem;            // dynamic shared memory per CTA
+    int per_sm;             // generic: CTAs of the kernel one SM holds
 };
 int select_sweep(int H, int B, int ndir, SweepPlan *p);
 

@@ -199,13 +199,11 @@ __global__ void add2_kernel(const float *__restrict__ x, const float *__restrict
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) z[i] = x[i] + y[i];
 }
 
-// co-resident CTAs of the generic kernel with this much dynamic shared memory
+// CTAs of the generic kernel one SM holds with this much dynamic shared memory (at most max_smem_optin())
 template <int KI>
-static int sweep_capacity(size_t smem, int *capacity) {
-    int per_sm = 0;
+static int sweep_occupancy(size_t smem, int *per_sm) {
     CTCB_CUDA_CHECK(cudaFuncSetAttribute(sweep_kernel<KI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    CTCB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sweep_kernel<KI>, SW_THREADS, smem));
-    *capacity = per_sm * num_sms();
+    CTCB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(per_sm, sweep_kernel<KI>, SW_THREADS, smem));
     return CTCB_OK;
 }
 
@@ -231,8 +229,10 @@ int run_sweep_tc(const SweepPlan &p, int mode, int T, int B, int H, const int32_
                  unsigned int *counters, void *ws, size_t ws_bytes, cudaStream_t st);
 
 // The one place that decides which kernel runs a sweep of (H, B, ndir): the tensor-core kernel where it applies
-// (H >= 1024, CTCB_SWEEP_TC), else the cluster kernel (H = 128/256/512; CTCB_SWEEP=barrier skips it), else the generic
-// kernel, whose CTAs must all be co-resident.
+// (H >= 1024, CTCB_SWEEP_TC), else the cluster kernel (H = 128/256/512; CTCB_SWEEP=barrier or reread skips it), else the
+// generic kernel, whose CTAs must all be co-resident.  CTCB_SWEEP=reread takes the generic kernel's KI = 0 at any H;
+// CTCB_SWEEP_PARTS forces its partition count.  A width whose shared memory or CTAs the device cannot hold, or a forced
+// count it cannot hold co-resident, is refused here, before any launch.
 int select_sweep(int H, int B, int ndir, SweepPlan *p) {
     if (H <= 0 || B <= 0 || (ndir != 1 && ndir != 2))
         return set_error(CTCB_EINVAL, "recurrent sweep: bad sizes (H=%d, B=%d, ndir=%d)", H, B, ndir);
@@ -240,29 +240,52 @@ int select_sweep(int H, int B, int ndir, SweepPlan *p) {
     if (!knob(KNOB_SWEEP) && sweep_cluster_plan(H, B, ndir, p)) return CTCB_OK;
     *p = SweepPlan{};
     p->kernel = SWEEP_GENERIC;
-    p->KI = (H == 128 || H == 256 || H == 512 || H == 1024) ? H / 32 : 0;
+    const bool reg = (H == 128 || H == 256 || H == 512 || H == 1024) && knob(KNOB_SWEEP) != 2;
+    p->KI = reg ? H / 32 : 0;
     const int Hp = (H + 3) / 4 * 4 + 4;
     p->smem = (size_t)SW_NB * Hp * sizeof(float);
-    int capacity = 0, rc;
+    if (p->smem > max_smem_optin())
+        return set_error(CTCB_EINVAL, "recurrent sweep: layerSize %d needs %zu bytes of shared memory per CTA, device "
+                         "allows %zu", H, p->smem, max_smem_optin());
+    int rc;
     switch (p->KI) {
-        case 4: rc = sweep_capacity<4>(p->smem, &capacity); break;
-        case 8: rc = sweep_capacity<8>(p->smem, &capacity); break;
-        case 16: rc = sweep_capacity<16>(p->smem, &capacity); break;
-        case 32: rc = sweep_capacity<32>(p->smem, &capacity); break;
-        default: rc = sweep_capacity<0>(p->smem, &capacity); break;
+        case 4: rc = sweep_occupancy<4>(p->smem, &p->per_sm); break;
+        case 8: rc = sweep_occupancy<8>(p->smem, &p->per_sm); break;
+        case 16: rc = sweep_occupancy<16>(p->smem, &p->per_sm); break;
+        case 32: rc = sweep_occupancy<32>(p->smem, &p->per_sm); break;
+        default: rc = sweep_occupancy<0>(p->smem, &p->per_sm); break;
     }
     if (rc != CTCB_OK) return rc;
+    const int capacity = p->per_sm * num_sms();
     const int slices = (H + SW_ROWS - 1) / SW_ROWS;
     if (ndir * slices > capacity)
         return set_error(CTCB_EINVAL, "recurrent sweep: layerSize %d needs %d co-resident CTAs, device holds %d",
                          H, ndir * slices, capacity);
     const int ntiles = (B + SW_NB - 1) / SW_NB;
     int parts = capacity / (ndir * slices);
+    if (knob(KNOB_SWEEP_PARTS)) {
+        if (knob(KNOB_SWEEP_PARTS) > parts)
+            return set_error(CTCB_EINVAL, "recurrent sweep: CTCB_SWEEP_PARTS=%d needs %d co-resident CTAs, device holds %d",
+                             knob(KNOB_SWEEP_PARTS), knob(KNOB_SWEEP_PARTS) * ndir * slices, capacity);
+        parts = knob(KNOB_SWEEP_PARTS);
+    }
     if (parts > ntiles) parts = ntiles;
-    if (parts > 500) parts = 500;   // counters region holds 1024 words
+    if (parts > SWEEP_MAX_PARTS) parts = SWEEP_MAX_PARTS;   // the counters region holds 1008 words
     if (parts < 1) parts = 1;
     p->groups = parts;
     return CTCB_OK;
+}
+
+// ctcb_brnn_create's check that the device holds the ReLU sweep of a config at its largest batch (every plan that holds
+// maxB holds a smaller batch); without a device there is nothing to check against, and the launch checks again
+int sweep_check(int H, int B, int ndir) {
+    int n = 0;
+    if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) {
+        (void)cudaGetLastError();
+        return CTCB_OK;
+    }
+    SweepPlan p;
+    return select_sweep(H, B, ndir, &p);
 }
 
 // counters: 4096 bytes of device scratch (word 0 = error flag, cleared by the caller); ws: optional further scratch
@@ -309,7 +332,8 @@ extern "C" int ctcb_debug_sweep_plan(int H, int B, int ndir, int32_t *out) {
     ctcb::SweepPlan p;
     const int rc = ctcb::select_sweep(H, B, ndir, &p);
     if (rc != CTCB_OK) return rc;
-    const int32_t v[8] = {p.kernel, p.KI, p.cs, p.groups, p.np, p.stages, p.partial_own, 0};
+    const int32_t v[8] = {p.kernel, p.KI, p.cs, p.groups, p.np, p.stages, p.partial_own,
+                          p.kernel == ctcb::SWEEP_GENERIC ? p.per_sm : 0};
     for (int i = 0; i < 8; ++i) out[i] = v[i];
     return CTCB_OK;
 }

@@ -330,13 +330,16 @@ static int lstm_occupancy_of(int KI, size_t smem, int *per_sm) {
 
 // the plan of the kernel that runs: the peephole mode's occupancy is its own.  CTCB_LSTM=reread takes KI = 0 at any
 // H; CTCB_LSTM_PARTS forces the partition count, refused here, before any launch, where its CTAs cannot all be
-// co-resident.
+// co-resident.  A width whose shared memory exceeds the opt-in maximum is refused before the attribute call.
 int lstm_plan(int H, int B, int ndir, bool peep, LstmPlan *p) {
     if (H <= 0 || B <= 0 || (ndir != 1 && ndir != 2))
         return set_error(CTCB_EINVAL, "LSTM sweep: bad sizes (H=%d, B=%d, ndir=%d)", H, B, ndir);
     const int slices = (H + LS_UNITS - 1) / LS_UNITS;
     const int Hp = (H + 3) / 4 * 4 + 4;
     p->smem = (size_t)LS_NB * Hp * sizeof(float);
+    if (p->smem > max_smem_optin())
+        return set_error(CTCB_EINVAL, "LSTM sweep: layerSize %d needs %zu bytes of shared memory per CTA, device allows "
+                         "%zu", H, p->smem, max_smem_optin());
     const bool reg = (H == 64 || H == 128 || H == 256 || H == 512 || H == 1024) && knob(KNOB_LSTM) == 0;
     int capacity = 0;
     for (p->KI = reg ? H / 32 : 0;; p->KI = 0) {   // U does not fit the register files the device holds: re-read it

@@ -104,11 +104,12 @@ def test_gemm_row_limit():
 
 # The knobs of INTEGRATION.md section 4 that ctcb_debug_set_knob takes: every documented value, and a value outside them
 KNOBS = {"CTCB_GEMM": (["simt"], "s"), "CTCB_GEMM_TC_COPY": (["0", "1"], "2"), "CTCB_GEMM_TRACE": (["1"], "0"),
-         "CTCB_SWEEP": (["barrier"], "b"), "CTCB_SWEEP_NB": ([str(n) for n in range(1, 9)], "9"),
+         "CTCB_SWEEP": (["auto", "barrier", "reread"], "b"), "CTCB_SWEEP_NB": ([str(n) for n in range(1, 9)], "9"),
          "CTCB_SWEEP_TC": (["0", "1", "2"], "3"), "CTCB_SWEEP_TC_CS": (["1", "2", "4"], "3"),
          "CTCB_SWEEP_TC_COOP": (["0"], "1"), "CTCB_SWEEP_TRACE": (["1"], "0"),
          "CTCB_CTC": (["auto", "warp", "pair", "par", "ckpt"], "pa"), "CTCB_LSTM": (["auto", "reread"], "reg"),
-         "CTCB_LSTM_PARTS": (["auto", "1", "2", "3", "17", "499", "500"], "501")}
+         "CTCB_LSTM_PARTS": (["auto", "1", "2", "3", "17", "499", "500"], "501"),
+         "CTCB_SWEEP_PARTS": (["auto", "1", "2", "3", "17", "499", "500"], "501")}
 
 
 def _ckpt_refuses():
@@ -133,6 +134,7 @@ def test_set_knob_takes_the_documented_values_only():
         assert lib.ctcb_debug_set_knob(name.encode(), None) == 0
     for v in ("0", "01", "-1", "+2", "2x", " 2", "4294967298"):     # the partition count is a plain decimal 1..500
         assert lib.ctcb_debug_set_knob(b"CTCB_LSTM_PARTS", v.encode()) == -1, v
+        assert lib.ctcb_debug_set_knob(b"CTCB_SWEEP_PARTS", v.encode()) == -1, v
     # a refused value leaves the table as it was
     assert lib.ctcb_debug_set_knob(b"CTCB_CTC", b"ckpt") == 0 and _ckpt_refuses()
     assert lib.ctcb_debug_set_knob(b"CTCB_CTC", b"pa") == -1 and _ckpt_refuses()
