@@ -309,7 +309,11 @@ size_t ctcb_brnn_forward_workspace_bytes(const ctcb_brnn_config *cfg, size_t *er
  * rescaled activations.  cell = 1 only: what = 3 the activated gates (G wide, the same buffer as what = 0 of that layer),
  * 4 / 5 c of the forward / backward direction (H wide).  subsample = k >= 2: the entries of maps >= L (and of their
  * temporal layers) are [Tmax'][B][width] with that call's Tmax' = ceil(Tmax / k); what = 6 is S, the stacked input of
- * map L, [Tmax'][B][k n] (`layer` is ignored). */
+ * map L, [Tmax'][B][k n] (`layer` is ignored).  what = 7 is the delta of affine map `layer` (1..numLayers+1), the
+ * buffer that map's weight and bias gradients read, [T][B][rows] with rows its output width (G at an LSTM layer):
+ * dz after layer normalisation, the gate gradients at an LSTM layer, the BPTT result at a uni-directional clipped-ReLU
+ * temporal layer.  CTCB_EINVAL where a later stage of the call overwrites it: a uni-directional clipped-ReLU temporal
+ * layer above the lowest two of its stack. */
 int ctcb_brnn_activation_offset(const ctcb_brnn_config *cfg, int what, int layer, size_t *offset, int32_t *width);
 
 /* With temporal layers, refuses (CTCB_EINVAL, with the planner's message) a config whose recurrent sweep the device
@@ -403,6 +407,23 @@ int ctcb_layernorm_forward_f32(const float *z, float *y, float *mu, float *rstd,
 int ctcb_layernorm_backward_f32(float *delta, const float *z, const float *mu, const float *rstd, const float *gamma,
                                 float *dgamma, float *dbeta, int64_t R, int H, int accumulate, void *workspace,
                                 size_t ws_bytes, void *stream);
+
+/* ---- the training step's reductions on their own: the launches a training call makes ----------------------------
+ * colsum : out[j] = sum over the R rows of the row-major R x n matrix delta (the bias gradients), or with accumulate
+ *          != 0 added into out.  workspace: 16-byte aligned, ctcb_colsum_workspace_bytes(R, n) bytes of partial sums
+ *          (CTCB_ENOMEM when shorter); 0 for R or n < 1.  Stage 1 sums row blocks in a fixed order, stage 2 adds the
+ *          blocks' partials in order, so the bits depend only on R, n, the inputs, the alignment of delta and the
+ *          device's SM count.  CTCB_EINVAL for R or n < 1, or more than 65535 row blocks of 128.
+ * ctcb_debug_colsum_plan: out (HOST, 4 int32) = {path: 1 wide (n % 4 == 0 and delta 16-byte aligned: each thread a
+ *          float4 column group, 4 rows per loop step) / 0 narrow (8 strided threads per column), column blocks,
+ *          rows per block (wide: R / (2 SMs / column blocks) within [128, 1024]; narrow: 1024), row blocks}.
+ * softmax_rows: p = softmax of each row of the row-major R x K matrix x, the forward-only probabilities of a
+ *          ctcb_brnn_cost_and_grad call (probs_out); one warp per row. */
+size_t ctcb_colsum_workspace_bytes(int64_t R, int n);
+int ctcb_colsum_f32(const float *delta, int64_t R, int n, float *out, int accumulate, void *workspace, size_t ws_bytes,
+                    void *stream);
+int ctcb_debug_colsum_plan(int64_t R, int n, const float *delta, int32_t *out);
+int ctcb_softmax_rows_f32(const float *x, float *p, int64_t R, int K, void *stream);
 
 /* ---- frame stacking on its own (subsample = k, above) ----------------------------------------------------------
  * x / d_out are time-major [Tmax][B][n], s_out / ds [ceil(Tmax / k)][B][k n], T_per_utt int32[B] (<= Tmax).

@@ -91,6 +91,10 @@ _PROTOS = {
     "ctcb_layernorm_forward_f32": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_int, c_vp]),
     "ctcb_layernorm_backward_f32": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_int, c_int, c_vp, c_sz,
                                             c_vp]),
+    "ctcb_colsum_workspace_bytes": (c_sz, [c_i64, c_int]),
+    "ctcb_colsum_f32": (c_int, [c_vp, c_i64, c_int, c_vp, c_int, c_vp, c_sz, c_vp]),
+    "ctcb_debug_colsum_plan": (c_int, [c_i64, c_int, c_vp, ctypes.POINTER(ctypes.c_int32)]),
+    "ctcb_softmax_rows_f32": (c_int, [c_vp, c_vp, c_i64, c_int, c_vp]),
     "ctcb_frame_stack_f32": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp]),
     "ctcb_frame_unstack_f32": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp]),
     "ctcb_debug_sweep_plan": (c_int, [c_int, c_int, c_int, ctypes.POINTER(ctypes.c_int32)]),

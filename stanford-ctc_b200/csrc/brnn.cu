@@ -145,26 +145,53 @@ __global__ void batch_stats_kernel(const float *__restrict__ cost, const int32_t
 }
 
 
+// The stage-1 grid of run_colsum: the wide kernel (n % 4 == 0 and a 16-byte aligned delta) over ncb column blocks of
+// bx threads and row blocks of rpb rows, or the narrow one over ncb blocks of 32 columns and row blocks of CS_ROWS rows
+struct ColsumPlan {
+    bool wide;
+    int ncb, bx;
+    int64_t rpb;
+    int nblk;
+};
+ColsumPlan colsum_plan(const float *delta, int64_t R, int n) {
+    ColsumPlan p{};
+    p.wide = n % 4 == 0 && (((uintptr_t)delta) & 15) == 0;
+    if (p.wide) {
+        const int n4 = n / 4;
+        p.bx = n4 >= 256 ? 256 : (n4 + 31) / 32 * 32;
+        p.ncb = (n4 + p.bx - 1) / p.bx;
+        p.rpb = R / (2 * num_sms() / p.ncb > 0 ? 2 * num_sms() / p.ncb : 1);     // ~2 blocks per SM
+        if (p.rpb < CS_ROWS_MIN) p.rpb = CS_ROWS_MIN;
+        if (p.rpb > CS_ROWS) p.rpb = CS_ROWS;
+    } else {
+        p.bx = 32;
+        p.ncb = (n + 31) / 32;
+        p.rpb = CS_ROWS;
+    }
+    p.nblk = (int)((R + p.rpb - 1) / p.rpb);
+    return p;
+}
+
 // both stages of the column sums of the row-major R x n matrix `delta` into out[n]; `partial` holds one row of n floats
 // per CS_ROWS_MIN rows of R
 int run_colsum(const float *delta, int64_t R, int n, float *partial, float *out, bool accumulate, cudaStream_t st) {
-    int nblk;
-    if (n % 4 == 0 && (((uintptr_t)delta) & 15) == 0) {
-        const int n4 = n / 4;
-        const int bx = n4 >= 256 ? 256 : (n4 + 31) / 32 * 32;
-        const int ncb = (n4 + bx - 1) / bx;
-        int64_t rpb = R / (2 * num_sms() / ncb > 0 ? 2 * num_sms() / ncb : 1);     // ~2 blocks per SM
-        if (rpb < CS_ROWS_MIN) rpb = CS_ROWS_MIN;
-        if (rpb > CS_ROWS) rpb = CS_ROWS;
-        nblk = (int)((R + rpb - 1) / rpb);
-        colsum_stage1_wide<<<dim3(ncb, nblk), bx, 0, st>>>((const float4 *)delta, R, n4, (int)rpb, (float4 *)partial);
-    } else {
-        nblk = (int)((R + CS_ROWS - 1) / CS_ROWS);
-        colsum_stage1<<<dim3((n + 31) / 32, nblk), dim3(32, 8), 0, st>>>(delta, R, n, partial);
-    }
+    const ColsumPlan p = colsum_plan(delta, R, n);
+    if (p.wide)
+        colsum_stage1_wide<<<dim3(p.ncb, p.nblk), p.bx, 0, st>>>((const float4 *)delta, R, n / 4, (int)p.rpb,
+                                                                (float4 *)partial);
+    else
+        colsum_stage1<<<dim3(p.ncb, p.nblk), dim3(32, 8), 0, st>>>(delta, R, n, partial);
     CTCB_LAUNCH_CHECK();
-    if (!accumulate) colsum_stage2<false><<<(n + 127) / 128, 128, 0, st>>>(partial, nblk, n, out);
-    else colsum_stage2<true><<<(n + 127) / 128, 128, 0, st>>>(partial, nblk, n, out);
+    if (!accumulate) colsum_stage2<false><<<(n + 127) / 128, 128, 0, st>>>(partial, p.nblk, n, out);
+    else colsum_stage2<true><<<(n + 127) / 128, 128, 0, st>>>(partial, p.nblk, n, out);
+    CTCB_LAUNCH_CHECK();
+    return CTCB_OK;
+}
+
+// the row softmax of the forward-only output: one warp per row, 8 rows per block
+int run_softmax_rows(const float *x, float *p, int64_t R, int K, cudaStream_t st) {
+    const int wpb = 8;
+    softmax_rows_kernel<<<(unsigned)((R + wpb - 1) / wpb), wpb * 32, 0, st>>>(x, p, R, K);
     CTCB_LAUNCH_CHECK();
     return CTCB_OK;
 }
@@ -879,12 +906,7 @@ static int brnn_forward(ctcb_brnn *h, const float *feats, const int32_t *T_per_u
             }
         }
     }
-    if (probs_out) {
-        const int64_t R = (int64_t)h->frames(N + 1, Tmax0) * B;
-        const int wpb = 8;
-        softmax_rows_kernel<<<(unsigned)((R + wpb - 1) / wpb), wpb * 32, 0, st>>>(m.X[N + 1], probs_out, R, K);
-        CTCB_LAUNCH_CHECK();
-    }
+    if (probs_out) TRY(run_softmax_rows(m.X[N + 1], probs_out, (int64_t)h->frames(N + 1, Tmax0) * B, K, st));
     return CTCB_OK;
 }
 
@@ -1239,14 +1261,72 @@ extern "C" int ctcb_brnn_set_dropout_utts(ctcb_brnn *h, int64_t first, int64_t s
 
 extern "C" size_t ctcb_brnn_sweep_workspace_bytes(int H, int B) { return 4096 + ctcb::sweep_tc_workspace_bytes(H, B); }
 
+// ---- the step's reductions on their own: the same launches as the training call makes ---------------------------
+extern "C" size_t ctcb_colsum_workspace_bytes(int64_t R, int n) {
+    if (R <= 0 || n <= 0) return 0;
+    return (size_t)((R + CS_ROWS_MIN - 1) / CS_ROWS_MIN) * (size_t)n * sizeof(float);
+}
+
+static int colsum_check(const char *fn, int64_t R, int n) {
+    if (R <= 0 || n <= 0) return set_error(CTCB_EINVAL, "%s: R = %lld, n = %d (need R >= 1, n >= 1)", fn, (long long)R, n);
+    if ((R + CS_ROWS_MIN - 1) / CS_ROWS_MIN > 65535)
+        return set_error(CTCB_EINVAL, "%s: R = %lld rows exceed %d row blocks of %d", fn, (long long)R, 65535, CS_ROWS_MIN);
+    return CTCB_OK;
+}
+
+extern "C" int ctcb_colsum_f32(const float *delta, int64_t R, int n, float *out, int accumulate, void *workspace,
+                               size_t ws_bytes, void *stream) {
+    if (int rc = colsum_check("ctcb_colsum_f32", R, n)) return rc;
+    if (!delta || !out || !workspace) return set_error(CTCB_EINVAL, "ctcb_colsum_f32: null pointer argument");
+    if (((uintptr_t)workspace) & 15) return set_error(CTCB_EINVAL, "ctcb_colsum_f32: workspace is not 16-byte aligned");
+    const size_t need = ctcb_colsum_workspace_bytes(R, n);
+    if (ws_bytes < need) return set_error(CTCB_ENOMEM, "ctcb_colsum_f32: workspace %zu < %zu bytes", ws_bytes, need);
+    return run_colsum(delta, R, n, (float *)workspace, out, accumulate != 0, (cudaStream_t)stream);
+}
+
+extern "C" int ctcb_debug_colsum_plan(int64_t R, int n, const float *delta, int32_t *out) {
+    if (int rc = colsum_check("ctcb_debug_colsum_plan", R, n)) return rc;
+    if (!out) return set_error(CTCB_EINVAL, "ctcb_debug_colsum_plan: null pointer argument");
+    const ColsumPlan p = colsum_plan(delta, R, n);
+    out[0] = p.wide ? 1 : 0;
+    out[1] = p.ncb;
+    out[2] = (int32_t)p.rpb;
+    out[3] = p.nblk;
+    return CTCB_OK;
+}
+
+extern "C" int ctcb_softmax_rows_f32(const float *x, float *p, int64_t R, int K, void *stream) {
+    if (!x || !p) return set_error(CTCB_EINVAL, "ctcb_softmax_rows_f32: null pointer argument");
+    if (R <= 0 || K <= 0 || (R + 7) / 8 > 0x7fffffff)
+        return set_error(CTCB_EINVAL, "ctcb_softmax_rows_f32: R = %lld, K = %d (need 1 <= R < 2^34, K >= 1)", (long long)R, K);
+    return run_softmax_rows(x, p, R, K, (cudaStream_t)stream);
+}
+
 // Test / diagnostic hook: where, inside the workspace, the activations of the LAST ctcb_brnn_cost_and_grad call lie
 // (time-major [Tmax][B][n] with that call's B and Tmax).  what = 0: output of affine map `layer` (1..numLayers+1; the
 // temporal layer's entry holds For + Back, the last one the logits), 1: For, 2: Back (temporal layer only; with
 // several, `layer` says which, and only a bi-directional stack has a Back of every layer).  Subsampled nets: entries of
-// maps >= L are [Tmax'][B][n]; what = 6: S, the stacked input of map L, k n wide.
+// maps >= L are [Tmax'][B][n]; what = 6: S, the stacked input of map L, k n wide.  what = 7: the delta of map `layer`,
+// the buffer its weight and bias gradients read (Step::delta), where no later stage of the call overwrites it.
 extern "C" int ctcb_brnn_activation_offset(const ctcb_brnn_config *cfg, int what, int layer, size_t *offset, int32_t *width) {
     if (!valid_cfg(cfg) || !offset) return set_error(CTCB_EINVAL, "ctcb_brnn_activation_offset: bad arguments");
     const WsLayout w = ws_layout(cfg);
+    if (what == 7) {
+        if (layer < 1 || layer > cfg->numLayers + 1)
+            return set_error(CTCB_EINVAL, "ctcb_brnn_activation_offset: layer %d", layer);
+        const int j = layer - eff_tl(cfg);
+        if (cfg->unidirectional && cfg->cell != 1 && is_temporal(cfg, layer)) {
+            // the BPTT result is the delta; layer j - 2 of the stack writes the same pair after it
+            if (j >= 2)
+                return set_error(CTCB_EINVAL, "ctcb_brnn_activation_offset: the delta of map %d is overwritten by the "
+                                 "call", layer);
+            *offset = w.dFor[j % 2];
+        } else {
+            *offset = w.D[layer];
+        }
+        if (width) *width = map_rows(cfg, layer);
+        return CTCB_OK;
+    }
     if (what == 6 && eff_k(cfg) > 1) {
         *offset = w.S;
         if (width) *width = map_cols(cfg, cfg->subsampleLayer);

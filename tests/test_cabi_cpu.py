@@ -102,6 +102,54 @@ def test_gemm_row_limit():
     assert b"rows exceed" in lib.ctcb_last_error()
 
 
+def test_step_reduction_entry_points_check_their_arguments():
+    """ctcb_colsum_f32, ctcb_debug_colsum_plan and ctcb_softmax_rows_f32 refuse bad arguments before any launch, and the
+    delta hook (what = 7) refuses the maps it cannot expose."""
+    import _ctcb
+    lib = _ctcb.lib
+    buf = (ctypes.c_float * 64)()
+    p = ctypes.addressof(buf)
+    aligned = (p + 15) // 16 * 16
+    assert lib.ctcb_colsum_workspace_bytes(1000, 5) == 8 * 5 * 4
+    assert lib.ctcb_colsum_workspace_bytes(0, 5) == 0 and lib.ctcb_colsum_workspace_bytes(5, 0) == 0
+    need = lib.ctcb_colsum_workspace_bytes(3, 4)
+    for args in ((None, 3, 4, p, 0, aligned, need), (p, 3, 4, None, 0, aligned, need), (p, 3, 4, p, 0, None, need),
+                 (p, 0, 4, p, 0, aligned, need), (p, -1, 4, p, 0, aligned, need), (p, 3, 0, p, 0, aligned, need),
+                 (p, 3, -4, p, 0, aligned, need), (p, 128 * 65535 + 1, 4, p, 0, aligned, 1 << 40),
+                 (p, 3, 4, p, 0, aligned + 4, need)):
+        assert lib.ctcb_colsum_f32(*args, None) == -1, args
+    assert lib.ctcb_colsum_f32(p, 3, 4, p, 1, aligned, need - 1, None) == -3
+    assert b"workspace" in lib.ctcb_last_error()
+    out = (ctypes.c_int32 * 4)()
+    assert lib.ctcb_debug_colsum_plan(0, 4, aligned, out) == -1
+    assert lib.ctcb_debug_colsum_plan(3, 0, aligned, out) == -1
+    assert lib.ctcb_debug_colsum_plan(3, 4, aligned, None) == -1
+    assert lib.ctcb_debug_colsum_plan(5, 64, aligned, out) == 0 and list(out)[0] == 1 and list(out)[2] == 128
+    assert lib.ctcb_debug_colsum_plan(5, 64, aligned + 4, out) == 0 and list(out) == [0, 2, 1024, 1]
+    assert lib.ctcb_debug_colsum_plan(5000, 35, aligned, out) == 0 and list(out) == [0, 2, 1024, 5]
+    for args in ((None, p, 3, 4), (p, None, 3, 4), (p, p, 0, 4), (p, p, -3, 4), (p, p, 3, 0), (p, p, 3, -1)):
+        assert lib.ctcb_softmax_rows_f32(*args, None) == -1, args
+    # the delta of map `layer`: 1..N+1 only, G wide at an LSTM layer, refused above the lowest two layers of a
+    # uni-directional clipped-ReLU stack (the pair they share is overwritten)
+    off, width = ctypes.c_size_t(), ctypes.c_int32()
+    hook = lambda cfg, layer: lib.ctcb_brnn_activation_offset(ctypes.byref(cfg), 7, layer, ctypes.byref(off),  # noqa: E731
+                                                              ctypes.byref(width))
+    bi = _ctcb.BrnnConfig(41, 62, 512, 2, 1, 200, 32, 30, 0.0, 20.0)
+    assert hook(bi, 0) == -1 and hook(bi, 4) == -1
+    assert [hook(bi, j) == 0 and width.value for j in (1, 2, 3)] == [512, 512, 62]
+    lstm = _ctcb.BrnnConfig(41, 62, 64, 2, 1, 200, 32, 30, 0.0, 20.0, 0, 1, 1)
+    assert hook(lstm, 1) == 0 and width.value == 2 * 4 * 64
+    uni3 = _ctcb.BrnnConfig(41, 62, 64, 4, 1, 200, 32, 30, 0.0, 20.0, 1, 3)
+    seen = set()
+    for j in (1, 2, 4, 5):
+        assert hook(uni3, j) == 0 and width.value == (62 if j == 5 else 64), j
+        seen.add(off.value)
+    assert len(seen) == 4
+    assert hook(uni3, 3) == -1 and b"overwritten" in lib.ctcb_last_error()
+    uni3_lstm = _ctcb.BrnnConfig(41, 62, 64, 4, 1, 200, 32, 30, 0.0, 20.0, 1, 3, 1)
+    assert hook(uni3_lstm, 3) == 0 and width.value == 4 * 64
+
+
 # The knobs of INTEGRATION.md section 4 that ctcb_debug_set_knob takes: every documented value, and a value outside them
 KNOBS = {"CTCB_GEMM": (["simt"], "s"), "CTCB_GEMM_TC_COPY": (["0", "1"], "2"), "CTCB_GEMM_TRACE": (["1"], "0"),
          "CTCB_SWEEP": (["auto", "barrier", "reread"], "b"), "CTCB_SWEEP_NB": ([str(n) for n in range(1, 9)], "9"),

@@ -85,7 +85,8 @@ def _ln_parts(R):
 
 
 @pytest.mark.parametrize("H,R", [(13, 1000), (64, 1000), (512, 1000), (1824, 1000), (2048, 1000), (64, 20000),
-                                 (70, 333), (8192, 40)])
+                                 (70, 333), (8192, 40), (3001, 1000), (4096, 1000), (1023, 1000), (8191, 40),
+                                 (2048, 5000)])
 def test_kernels_match_float64_of_their_inputs(H, R, cuda):
     torch = cuda
     from _ctcb import lib, check
