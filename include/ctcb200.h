@@ -288,7 +288,8 @@ int ctcb_brnn_tensor_info(const ctcb_brnn_config *cfg, int idx, int64_t *offset,
 size_t ctcb_brnn_workspace_bytes(const ctcb_brnn_config *cfg);
 /* Byte offset, inside the workspace, of a uint32 that the recurrent-sweep kernels set non-zero when an
  * inter-CTA wait timed out (results are then invalid; never a hang).  Callers that synchronise anyway
- * (e.g. for the per-step log line) should read it. */
+ * (e.g. for the per-step log line) should read it.  The value names the kernel whose wait timed out:
+ * 1 the generic sweep, 2 the cluster sweep, 3 the tensor-core sweep, 4 the LSTM sweep. */
 size_t ctcb_brnn_error_flag_offset(const ctcb_brnn_config *cfg);
 /* Workspace of a forward-only call (grads == NULL): two ping-pong activation slabs, For and Back (For only when
  * unidirectional, neither without a temporal layer), the split-K area of the forward contractions, the sweep

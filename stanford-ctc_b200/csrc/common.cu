@@ -73,8 +73,8 @@ static const KnobDef KNOBS[KNOB_COUNT] = {
     {"CTCB_SWEEP_TRACE", 0, {nullptr, "1"}},
     {"CTCB_CTC", 0, {"auto", "warp", "pair", "par", "ckpt"}},
     {"CTCB_LSTM", 0, {"auto", "reread"}},
-    {"CTCB_LSTM_PARTS", 0, {"auto"}, LSTM_MAX_PARTS},
-    {"CTCB_SWEEP_PARTS", 0, {"auto"}, SWEEP_MAX_PARTS},
+    {"CTCB_LSTM_PARTS", 0, {"auto"}, COOP_SWEEP_MAX_PARTS},
+    {"CTCB_SWEEP_PARTS", 0, {"auto"}, COOP_SWEEP_MAX_PARTS},
 };
 static int g_knob_initial[KNOB_COUNT], g_knob[KNOB_COUNT];     // what the environment said, what is in effect
 static std::once_flag g_knob_once;

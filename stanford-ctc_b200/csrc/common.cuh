@@ -45,11 +45,10 @@ int stream_priority_greatest();
 enum Knob { KNOB_GEMM, KNOB_GEMM_TC_COPY, KNOB_GEMM_TRACE, KNOB_SWEEP, KNOB_SWEEP_NB, KNOB_SWEEP_TC, KNOB_SWEEP_TC_CS,
             KNOB_SWEEP_TC_COOP, KNOB_SWEEP_TRACE, KNOB_CTC, KNOB_LSTM, KNOB_LSTM_PARTS, KNOB_SWEEP_PARTS, KNOB_COUNT };
 int knob(Knob k);
-// The most utterance partitions of an LSTM sweep: its barrier counters ([ndir][parts] words) share 4 KB of scratch with
-// the error flags.  CTCB_LSTM_PARTS takes auto or 1..LSTM_MAX_PARTS.
-constexpr int LSTM_MAX_PARTS = 500;
-// The same for the generic recurrent sweep (sweep.cu), whose counters take the same scratch: CTCB_SWEEP_PARTS.
-constexpr int SWEEP_MAX_PARTS = 500;
+// The most utterance partitions of a cooperative sweep (the generic and LSTM kernels, coop_sweep.cuh): their barrier
+// counters ([ndir][parts] words) share 4 KB of scratch with the 16 error words.  CTCB_SWEEP_PARTS and CTCB_LSTM_PARTS
+// take auto or 1..COOP_SWEEP_MAX_PARTS.
+constexpr int COOP_SWEEP_MAX_PARTS = 500;
 
 // Optional per-phase device timing (ctcb_profile_*): CUDA events recorded on the launching stream
 // around each phase of the step; off by default so the timed benchmark region carries no events.

@@ -25,14 +25,16 @@
 // exchanged through the output array in L2 (ld.global.cg), which has to be written anyway.
 //
 // Data layout: time-major [T][B][H] fp32, so one time step of all utterances is contiguous.
-#include "common.cuh"
+//
+// From coop_sweep.cuh, which the LSTM sweep (sweep_lstm.cu) shares: the block and tile sizes, the state-tile load, the
+// transposing butterfly, the partition's tiles, the bounded step barrier (a timeout sets the error flag to 1), and on
+// the host the partition planner, the KI dispatch and the cooperative launch.
+#include "coop_sweep.cuh"
 #include <stdlib.h>
 
 namespace ctcb {
 
-constexpr int SW_THREADS = 256;
 constexpr int SW_ROWS = 32;   // output units per CTA (4 per warp)
-constexpr int SW_NB = 8;      // utterances per inner tile
 
 struct SweepArgs {
     int mode;               // 0: forward recurrences, 1: BPTT
@@ -45,28 +47,17 @@ struct SweepArgs {
     float maxAct;
     int parts;              // utterance partitions (gridDim.y)
     int ndir;               // 2: forward and backward direction (gridDim.z); 1: forward in time only
-    unsigned int *counters; // [2 * parts], zeroed before launch
+    unsigned int *err;      // word 0 of the scratch: the error flag, cleared by the caller
+    unsigned int *counters; // [ndir * parts], zeroed before launch
 };
 
-__device__ __forceinline__ void domain_barrier(unsigned int *ctr, unsigned int target) {
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        __threadfence();
-        atomicAdd(ctr, 1u);
-        unsigned int v;
-        do {
-            asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(ctr) : "memory");
-        } while (v < target);
-    }
-    __syncthreads();
-}
-
-// KI > 0: H == 32*KI and the weights live in registers.  KI == 0: any H, weights re-read through L1/L2.
+// KI > 0: H == 32*KI and the weights live in registers.  KI == 0: any H, weights re-read through L1/L2, at three CTAs
+// per SM (at most 80 registers), which sets how wide a layer the device holds co-resident.
 template <int KI>
-__global__ void __launch_bounds__(SW_THREADS, 1) sweep_kernel(SweepArgs a) {
-    extern __shared__ __align__(16) float hs[];   // [SW_NB][Hp]
+__global__ void __launch_bounds__(COOP_THREADS, KI > 0 ? 1 : 3) sweep_kernel(SweepArgs a) {
+    extern __shared__ __align__(16) float hs[];   // [COOP_NB][Hp]
     const int H = a.H, B = a.B, T = a.T;
-    const int Hp = (H + 3) / 4 * 4 + 4;
+    const int Hp = coop_hp(H);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int dir = blockIdx.z;
     const int j0 = blockIdx.x * SW_ROWS + warp * 4;
@@ -86,13 +77,11 @@ __global__ void __launch_bounds__(SW_THREADS, 1) sweep_kernel(SweepArgs a) {
                 wreg[r][i] = (j < H) ? (bptt ? W[(int64_t)k * H + j] : W[(int64_t)j * H + k]) : 0.f;
             }
     }
-    // utterance range of this partition, in tiles of SW_NB
-    const int ntiles = (B + SW_NB - 1) / SW_NB;
-    const int tiles_per_part = (ntiles + a.parts - 1) / a.parts;
-    const int tile_beg = blockIdx.y * tiles_per_part;
-    const int tile_end = min(ntiles, tile_beg + tiles_per_part);
+    int tile_beg, tile_end;
+    coop_tile_range(B, a.parts, tile_beg, tile_end);
     unsigned int *ctr = a.counters + (dir * a.parts + blockIdx.y);
     const unsigned int nslices = gridDim.x;
+    bool dead = false;
 
     // lane -> (row r, utterance b) of the value it ends up owning after the transposing reduction
     const int orow = lane >> 3, ob = lane & 7;
@@ -102,7 +91,7 @@ __global__ void __launch_bounds__(SW_THREADS, 1) sweep_kernel(SweepArgs a) {
         const int t = ascending ? s : T - 1 - s;
         const int tprev = ascending ? t - 1 : t + 1;
         for (int tile = tile_beg; tile < tile_end; ++tile) {
-            const int b0 = tile * SW_NB;
+            const int b0 = tile * COOP_NB;
             const int b = b0 + ob;
             // issue the epilogue operands early: they do not depend on the recurrence
             float pre_v = 0.f, act_v = 0.f;
@@ -118,41 +107,26 @@ __global__ void __launch_bounds__(SW_THREADS, 1) sweep_kernel(SweepArgs a) {
 #pragma unroll
             for (int i = 0; i < 32; ++i) acc[i] = 0.f;
             if (s > 0) {
-                // previous state of this tile's utterances: [SW_NB][H] from L2 -> shared
-                const float *src = out + ((int64_t)tprev * B + b0) * H;
-                const int nb = min(SW_NB, B - b0);
-                if ((H & 3) == 0) {
-                    const int h4 = H >> 2;
-                    for (int idx = threadIdx.x; idx < nb * h4; idx += SW_THREADS) {
-                        const int bb = idx / h4, k4 = idx - bb * h4;
-                        const float4 v = __ldcg(reinterpret_cast<const float4 *>(src + (int64_t)bb * H) + k4);
-                        *reinterpret_cast<float4 *>(hs + bb * Hp + 4 * k4) = v;
-                    }
-                } else {
-                    for (int idx = threadIdx.x; idx < nb * H; idx += SW_THREADS) {
-                        const int bb = idx / H, k = idx - bb * H;
-                        hs[bb * Hp + k] = __ldcg(src + (int64_t)bb * H + k);
-                    }
-                }
-                for (int idx = threadIdx.x + nb * Hp; idx < SW_NB * Hp; idx += SW_THREADS) hs[idx] = 0.f;
+                // previous state of this tile's utterances from L2
+                coop_load_state(hs, Hp, out + ((int64_t)tprev * B + b0) * H, H, min(COOP_NB, B - b0), H);
                 __syncthreads();
                 if (KI > 0) {
 #pragma unroll
                     for (int i = 0; i < KI; ++i) {
-                        float hv[SW_NB];
+                        float hv[COOP_NB];
 #pragma unroll
-                        for (int bb = 0; bb < SW_NB; ++bb) hv[bb] = hs[bb * Hp + lane + 32 * i];
+                        for (int bb = 0; bb < COOP_NB; ++bb) hv[bb] = hs[bb * Hp + lane + 32 * i];
 #pragma unroll
                         for (int r = 0; r < 4; ++r)
 #pragma unroll
-                            for (int bb = 0; bb < SW_NB; ++bb)
+                            for (int bb = 0; bb < COOP_NB; ++bb)
                                 acc[r * 8 + bb] = fmaf(wreg[r][i], hv[bb], acc[r * 8 + bb]);
                     }
                 } else {
                     for (int k = lane; k < H; k += 32) {
-                        float hv[SW_NB], wv[4];
+                        float hv[COOP_NB], wv[4];
 #pragma unroll
-                        for (int bb = 0; bb < SW_NB; ++bb) hv[bb] = hs[bb * Hp + k];
+                        for (int bb = 0; bb < COOP_NB; ++bb) hv[bb] = hs[bb * Hp + k];
 #pragma unroll
                         for (int r = 0; r < 4; ++r) {
                             const int j = j0 + r;
@@ -161,21 +135,11 @@ __global__ void __launch_bounds__(SW_THREADS, 1) sweep_kernel(SweepArgs a) {
 #pragma unroll
                         for (int r = 0; r < 4; ++r)
 #pragma unroll
-                            for (int bb = 0; bb < SW_NB; ++bb)
+                            for (int bb = 0; bb < COOP_NB; ++bb)
                                 acc[r * 8 + bb] = fmaf(wv[r], hv[bb], acc[r * 8 + bb]);
                     }
                 }
-                // transposing butterfly: lane l ends with sum over lanes of acc[l]
-#pragma unroll
-                for (int off = 16, n = 32; off >= 1; off >>= 1, n >>= 1) {
-                    const bool up = (lane & off) != 0;
-#pragma unroll
-                    for (int i = 0; i < n / 2; ++i) {
-                        const float send = up ? acc[i] : acc[i + n / 2];
-                        const float keep = up ? acc[i + n / 2] : acc[i];
-                        acc[i] = keep + __shfl_xor_sync(0xffffffffu, send, off);
-                    }
-                }
+                coop_butterfly(acc, lane);
                 __syncthreads();   // hs is reused by the next tile
             }
             if (valid) {
@@ -190,33 +154,13 @@ __global__ void __launch_bounds__(SW_THREADS, 1) sweep_kernel(SweepArgs a) {
                 out[((int64_t)t * B + b) * H + oj] = v;
             }
         }
-        if (s + 1 < T) domain_barrier(ctr, nslices * (unsigned int)(s + 1));
+        if (s + 1 < T) coop_barrier(ctr, nslices * (unsigned int)(s + 1), a.err, 1u, dead);
     }
 }
 
 __global__ void add2_kernel(const float *__restrict__ x, const float *__restrict__ y, float *__restrict__ z, int64_t n) {
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) z[i] = x[i] + y[i];
-}
-
-// CTAs of the generic kernel one SM holds with this much dynamic shared memory (at most max_smem_optin())
-template <int KI>
-static int sweep_occupancy(size_t smem, int *per_sm) {
-    CTCB_CUDA_CHECK(cudaFuncSetAttribute(sweep_kernel<KI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    CTCB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(per_sm, sweep_kernel<KI>, SW_THREADS, smem));
-    return CTCB_OK;
-}
-
-template <int KI>
-static int launch_sweep(SweepArgs &a, int slices, const SweepPlan &p, cudaStream_t st) {
-    a.parts = p.groups;
-    a.counters += 16;     // words [0..15] are reserved for error flags, which the CALLER clears (once per step)
-    CTCB_CUDA_CHECK(cudaMemsetAsync(a.counters, 0, sizeof(unsigned int) * (a.ndir * a.parts), st));
-    dim3 grid(slices, a.parts, a.ndir);
-    void *params[] = {&a};
-    CTCB_CUDA_CHECK(cudaLaunchCooperativeKernel((void *)sweep_kernel<KI>, grid, dim3(SW_THREADS), params, p.smem, st));
-    count_launch();
-    return CTCB_OK;
 }
 
 bool sweep_tc_plan(int H, int B, int ndir, SweepPlan *p);
@@ -242,48 +186,22 @@ int select_sweep(int H, int B, int ndir, SweepPlan *p) {
     p->kernel = SWEEP_GENERIC;
     const bool reg = (H == 128 || H == 256 || H == 512 || H == 1024) && knob(KNOB_SWEEP) != 2;
     p->KI = reg ? H / 32 : 0;
-    const int Hp = (H + 3) / 4 * 4 + 4;
-    p->smem = (size_t)SW_NB * Hp * sizeof(float);
+    p->smem = coop_smem(H);
     if (p->smem > max_smem_optin())
         return set_error(CTCB_EINVAL, "recurrent sweep: layerSize %d needs %zu bytes of shared memory per CTA, device "
                          "allows %zu", H, p->smem, max_smem_optin());
-    int rc;
-    switch (p->KI) {
-        case 4: rc = sweep_occupancy<4>(p->smem, &p->per_sm); break;
-        case 8: rc = sweep_occupancy<8>(p->smem, &p->per_sm); break;
-        case 16: rc = sweep_occupancy<16>(p->smem, &p->per_sm); break;
-        case 32: rc = sweep_occupancy<32>(p->smem, &p->per_sm); break;
-        default: rc = sweep_occupancy<0>(p->smem, &p->per_sm); break;
-    }
+    const int rc = with_ki<4, 8, 16, 32>(p->KI, [&](auto ki) {
+        return coop_occupancy(sweep_kernel<decltype(ki)::value>, p->smem, &p->per_sm);
+    });
     if (rc != CTCB_OK) return rc;
-    const int capacity = p->per_sm * num_sms();
-    const int slices = (H + SW_ROWS - 1) / SW_ROWS;
-    if (ndir * slices > capacity)
-        return set_error(CTCB_EINVAL, "recurrent sweep: layerSize %d needs %d co-resident CTAs, device holds %d",
-                         H, ndir * slices, capacity);
-    const int ntiles = (B + SW_NB - 1) / SW_NB;
-    int parts = capacity / (ndir * slices);
-    if (knob(KNOB_SWEEP_PARTS)) {
-        if (knob(KNOB_SWEEP_PARTS) > parts)
-            return set_error(CTCB_EINVAL, "recurrent sweep: CTCB_SWEEP_PARTS=%d needs %d co-resident CTAs, device holds %d",
-                             knob(KNOB_SWEEP_PARTS), knob(KNOB_SWEEP_PARTS) * ndir * slices, capacity);
-        parts = knob(KNOB_SWEEP_PARTS);
-    }
-    if (parts > ntiles) parts = ntiles;
-    if (parts > SWEEP_MAX_PARTS) parts = SWEEP_MAX_PARTS;   // the counters region holds 1008 words
-    if (parts < 1) parts = 1;
-    p->groups = parts;
-    return CTCB_OK;
+    return coop_parts("recurrent sweep", H, p->per_sm, ndir, (H + SW_ROWS - 1) / SW_ROWS, B, knob(KNOB_SWEEP_PARTS),
+                      "CTCB_SWEEP_PARTS", &p->groups);
 }
 
 // ctcb_brnn_create's check that the device holds the ReLU sweep of a config at its largest batch (every plan that holds
-// maxB holds a smaller batch); without a device there is nothing to check against, and the launch checks again
+// maxB holds a smaller batch)
 int sweep_check(int H, int B, int ndir) {
-    int n = 0;
-    if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) {
-        (void)cudaGetLastError();
-        return CTCB_OK;
-    }
+    if (no_device()) return CTCB_OK;
     SweepPlan p;
     return select_sweep(H, B, ndir, &p);
 }
@@ -303,17 +221,13 @@ int run_sweep(int mode, int T, int B, int H, const int32_t *Tlen, const float *p
     SweepArgs a;
     a.mode = mode; a.T = T; a.B = B; a.H = H; a.Tlen = Tlen; a.pre = pre;
     a.W[0] = Wf; a.W[1] = Wb; a.out[0] = outF; a.out[1] = outB; a.act[0] = actF; a.act[1] = actB;
-    a.maxAct = maxAct; a.counters = counters; a.parts = 1;
+    a.maxAct = maxAct;
     a.ndir = Wb ? 2 : 1;
     if (!Wb) { a.W[1] = Wf; a.out[1] = outF; a.act[1] = actF; }   // never dereferenced: gridDim.z == 1
-    const int slices = (H + SW_ROWS - 1) / SW_ROWS;
-    switch (p.KI) {
-        case 4: return launch_sweep<4>(a, slices, p, st);
-        case 8: return launch_sweep<8>(a, slices, p, st);
-        case 16: return launch_sweep<16>(a, slices, p, st);
-        case 32: return launch_sweep<32>(a, slices, p, st);
-        default: return launch_sweep<0>(a, slices, p, st);
-    }
+    return with_ki<4, 8, 16, 32>(p.KI, [&](auto ki) {
+        return coop_launch(sweep_kernel<decltype(ki)::value>, a, counters, (H + SW_ROWS - 1) / SW_ROWS, p.groups, p.smem,
+                           st);
+    });
 }
 
 int run_add2(const float *x, const float *y, float *z, int64_t n, cudaStream_t st) {

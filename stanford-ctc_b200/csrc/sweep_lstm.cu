@@ -11,9 +11,12 @@
 // blocks), so after the transposing butterfly lane (r, b) holds gate r -- or, in BPTT, the part of dh that gate block r
 // contributes -- of utterance b, and the cell update is four shuffles inside the warp: no second exchange per step.
 // The state of the previous step (h, or the dz of all 4H rows in BPTT) is exchanged through L2, as the generic sweep
-// does, behind one counter barrier per step whose wait is bounded: a timeout sets the error flag and the sweep runs on
-// (results invalid, never a hang).  U lives in registers where the CTAs that hold it are co-resident (H = 64..1024 in
-// steps of powers of two, while ndir * H / 8 CTAs fit one per SM), else it is re-read through L1/L2.
+// does.  U lives in registers where the CTAs that hold it are co-resident (H = 64..1024 in steps of powers of two,
+// while ndir * H / 8 CTAs fit one per SM), else it is re-read through L1/L2.
+//
+// From coop_sweep.cuh, which the generic sweep shares: the block and tile sizes, the state-tile load, the transposing
+// butterfly, the partition's tiles, the bounded step barrier (a timeout sets the error flag to 4 and the sweep runs on),
+// and on the host the partition planner, the KI dispatch and the cooperative launch.
 //
 // The forward mode writes the activated gates over the pre-activations in place, c of every frame, and h into the
 // layer's For / Back; the BPTT mode reads those back and carries dc from step to step in a [B][H] scratch per direction.
@@ -23,13 +26,11 @@
 // unit.  BPTT: dc = dh o (1 - tanh^2 c) + p_o dz_o + carry, and the scratch carries f dc + p_i dz_i + p_f dz_f of the
 // step just finished instead of dc.  The peephole weight gradients are a separate reduction over dz and c
 // (lstm_peephole_grad below).
-#include "common.cuh"
+#include "coop_sweep.cuh"
 
 namespace ctcb {
 
-constexpr int LS_THREADS = 256;
 constexpr int LS_UNITS = 8;    // hidden units per CTA (one per warp, four gate rows each)
-constexpr int LS_NB = 8;       // utterances per inner tile
 
 struct LstmArgs {
     int mode;                  // 0: forward recurrences, 1: BPTT
@@ -54,57 +55,15 @@ struct LstmPeepArgs : LstmArgs {
 template <bool PEEP> struct LstmArgsOf { using type = LstmArgs; };
 template <> struct LstmArgsOf<true> { using type = LstmPeepArgs; };
 
-// The per-step barrier of the CTAs of one (direction, partition).  A wait longer than ~0.5 s sets the error flag and
-// gives up waiting for the rest of the sweep.
-__device__ __forceinline__ void lstm_barrier(unsigned int *ctr, unsigned int target, unsigned int *err, bool &dead) {
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        __threadfence();
-        atomicAdd(ctr, 1u);
-        if (!dead) {
-            const long long t0 = clock64();
-            while (true) {
-                unsigned int v;
-                asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(ctr) : "memory");
-                if (v >= target) break;
-                if (clock64() - t0 > 1000000000LL) {
-                    dead = true;
-                    atomicExch(err, 4u);
-                    break;
-                }
-            }
-        }
-    }
-    __syncthreads();
-}
-
-// [LS_NB][Hp] <- nb rows of H floats at src, src + pitch, ...; the rows beyond nb are zeroed
-__device__ __forceinline__ void lstm_load_state(float *hs, int Hp, const float *src, int64_t pitch, int nb, int H) {
-    if ((H & 3) == 0 && (pitch & 3) == 0 && (((uintptr_t)src) & 15) == 0) {
-        const int h4 = H >> 2;
-        for (int idx = threadIdx.x; idx < nb * h4; idx += LS_THREADS) {
-            const int bb = idx / h4, k4 = idx - bb * h4;
-            const float4 v = __ldcg(reinterpret_cast<const float4 *>(src + bb * pitch) + k4);
-            *reinterpret_cast<float4 *>(hs + bb * Hp + 4 * k4) = v;
-        }
-    } else {
-        for (int idx = threadIdx.x; idx < nb * H; idx += LS_THREADS) {
-            const int bb = idx / H, k = idx - bb * H;
-            hs[bb * Hp + k] = __ldcg(src + bb * pitch + k);
-        }
-    }
-    for (int idx = threadIdx.x + nb * Hp; idx < LS_NB * Hp; idx += LS_THREADS) hs[idx] = 0.f;
-}
-
 __device__ __forceinline__ float lstm_sigmoid(float z) { return 1.f / (1.f + expf(-z)); }
 
 // KI > 0: H == 32 KI and U lives in registers (one CTA per SM).  KI == 0: any H, U re-read (two CTAs per SM).
 template <int KI, bool PEEP>
-__global__ void __launch_bounds__(LS_THREADS, KI > 0 ? 1 : 2) lstm_sweep_kernel(typename LstmArgsOf<PEEP>::type a) {
-    extern __shared__ __align__(16) float hs[];   // [LS_NB][Hp]
+__global__ void __launch_bounds__(COOP_THREADS, KI > 0 ? 1 : 2) lstm_sweep_kernel(typename LstmArgsOf<PEEP>::type a) {
+    extern __shared__ __align__(16) float hs[];   // [COOP_NB][Hp]
     const int H = a.H, B = a.B, T = a.T;
     const int64_t G = (int64_t)a.ndir * 4 * H;
-    const int Hp = (H + 3) / 4 * 4 + 4;
+    const int Hp = coop_hp(H);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int dir = blockIdx.z;
     const int j = blockIdx.x * LS_UNITS + warp;     // this warp's hidden unit
@@ -122,10 +81,8 @@ __global__ void __launch_bounds__(LS_THREADS, KI > 0 ? 1 : 2) lstm_sweep_kernel(
                 wreg[r][i] = (j < H) ? (bptt ? U[(int64_t)(r * H + k) * H + j] : U[(int64_t)(r * H + j) * H + k]) : 0.f;
             }
     }
-    const int ntiles = (B + LS_NB - 1) / LS_NB;
-    const int tiles_per_part = (ntiles + a.parts - 1) / a.parts;
-    const int tile_beg = blockIdx.y * tiles_per_part;
-    const int tile_end = min(ntiles, tile_beg + tiles_per_part);
+    int tile_beg, tile_end;
+    coop_tile_range(B, a.parts, tile_beg, tile_end);
     unsigned int *ctr = a.counters + (dir * a.parts + blockIdx.y);
     const unsigned int nslices = gridDim.x;
     bool dead = false;
@@ -147,7 +104,7 @@ __global__ void __launch_bounds__(LS_THREADS, KI > 0 ? 1 : 2) lstm_sweep_kernel(
         const int tp = (dir == 0) ? t - 1 : t + 1;     // predecessor of t in the forward recurrence
         const int tn = (dir == 0) ? t + 1 : t - 1;     // its successor: the step BPTT came from
         for (int tile = tile_beg; tile < tile_end; ++tile) {
-            const int b0 = tile * LS_NB;
+            const int b0 = tile * COOP_NB;
             const int b = b0 + ob;
             const bool valid = (j < H) && (b < B);
             const int64_t go = ((int64_t)t * B + b) * G + gbase + (int64_t)orow * H + j;    // this lane's gate
@@ -161,67 +118,57 @@ __global__ void __launch_bounds__(LS_THREADS, KI > 0 ? 1 : 2) lstm_sweep_kernel(
 #pragma unroll
             for (int i = 0; i < 32; ++i) acc[i] = 0.f;
             if (s > 0) {
-                const int nb = min(LS_NB, B - b0);
+                const int nb = min(COOP_NB, B - b0);
                 if (!bptt) {       // U h_prev: the four gate rows of unit j
-                    lstm_load_state(hs, Hp, a.h[dir] + ((int64_t)tp * B + b0) * H, H, nb, H);
+                    coop_load_state(hs, Hp, a.h[dir] + ((int64_t)tp * B + b0) * H, H, nb, H);
                     __syncthreads();
                     if (KI > 0) {
 #pragma unroll
                         for (int i = 0; i < KI; ++i) {
-                            float hv[LS_NB];
+                            float hv[COOP_NB];
 #pragma unroll
-                            for (int bb = 0; bb < LS_NB; ++bb) hv[bb] = hs[bb * Hp + lane + 32 * i];
+                            for (int bb = 0; bb < COOP_NB; ++bb) hv[bb] = hs[bb * Hp + lane + 32 * i];
 #pragma unroll
                             for (int r = 0; r < 4; ++r)
 #pragma unroll
-                                for (int bb = 0; bb < LS_NB; ++bb) acc[r * 8 + bb] = fmaf(wreg[r][i], hv[bb], acc[r * 8 + bb]);
+                                for (int bb = 0; bb < COOP_NB; ++bb) acc[r * 8 + bb] = fmaf(wreg[r][i], hv[bb], acc[r * 8 + bb]);
                         }
                     } else if (j < H) {
                         for (int k = lane; k < H; k += 32) {
-                            float hv[LS_NB], wv[4];
+                            float hv[COOP_NB], wv[4];
 #pragma unroll
-                            for (int bb = 0; bb < LS_NB; ++bb) hv[bb] = hs[bb * Hp + k];
+                            for (int bb = 0; bb < COOP_NB; ++bb) hv[bb] = hs[bb * Hp + k];
 #pragma unroll
                             for (int r = 0; r < 4; ++r) wv[r] = __ldg(U + (int64_t)(r * H + j) * H + k);
 #pragma unroll
                             for (int r = 0; r < 4; ++r)
 #pragma unroll
-                                for (int bb = 0; bb < LS_NB; ++bb) acc[r * 8 + bb] = fmaf(wv[r], hv[bb], acc[r * 8 + bb]);
+                                for (int bb = 0; bb < COOP_NB; ++bb) acc[r * 8 + bb] = fmaf(wv[r], hv[bb], acc[r * 8 + bb]);
                         }
                     }
                     __syncthreads();   // hs is reused by the next tile
                 } else {           // U^T dz_next, one gate block r at a time: row r of the warp sums block r
 #pragma unroll
                     for (int r = 0; r < 4; ++r) {
-                        lstm_load_state(hs, Hp, a.dz + ((int64_t)tn * B + b0) * G + gbase + (int64_t)r * H, G, nb, H);
+                        coop_load_state(hs, Hp, a.dz + ((int64_t)tn * B + b0) * G + gbase + (int64_t)r * H, G, nb, H);
                         __syncthreads();
                         if (KI > 0) {
 #pragma unroll
                             for (int i = 0; i < KI; ++i)
 #pragma unroll
-                                for (int bb = 0; bb < LS_NB; ++bb)
+                                for (int bb = 0; bb < COOP_NB; ++bb)
                                     acc[r * 8 + bb] = fmaf(wreg[r][i], hs[bb * Hp + lane + 32 * i], acc[r * 8 + bb]);
                         } else if (j < H) {
                             for (int k = lane; k < H; k += 32) {
                                 const float wv = __ldg(U + (int64_t)(r * H + k) * H + j);
 #pragma unroll
-                                for (int bb = 0; bb < LS_NB; ++bb) acc[r * 8 + bb] = fmaf(wv, hs[bb * Hp + k], acc[r * 8 + bb]);
+                                for (int bb = 0; bb < COOP_NB; ++bb) acc[r * 8 + bb] = fmaf(wv, hs[bb * Hp + k], acc[r * 8 + bb]);
                             }
                         }
                         __syncthreads();
                     }
                 }
-                // transposing butterfly: lane l ends with the sum over lanes of acc[l]
-#pragma unroll
-                for (int off = 16, n = 32; off >= 1; off >>= 1, n >>= 1) {
-                    const bool up = (lane & off) != 0;
-#pragma unroll
-                    for (int i = 0; i < n / 2; ++i) {
-                        const float send = up ? acc[i] : acc[i + n / 2];
-                        const float keep = up ? acc[i + n / 2] : acc[i];
-                        acc[i] = keep + __shfl_xor_sync(0xffffffffu, send, off);
-                    }
-                }
+                coop_butterfly(acc, lane);
             }
             const bool live = valid && t < Tb;
             const int64_t hc = ((int64_t)t * B + b) * H + j;      // (t, b, j) in the [T][B][H] arrays
@@ -297,7 +244,7 @@ __global__ void __launch_bounds__(LS_THREADS, KI > 0 ? 1 : 2) lstm_sweep_kernel(
                 }
             }
         }
-        if (s + 1 < T) lstm_barrier(ctr, nslices * (unsigned int)(s + 1), a.err, dead);
+        if (s + 1 < T) coop_barrier(ctr, nslices * (unsigned int)(s + 1), a.err, 4u, dead);
     }
 }
 
@@ -308,26 +255,6 @@ struct LstmPlan {
     size_t smem;
 };
 
-template <int KI, bool PEEP>
-static int lstm_occupancy(size_t smem, int *per_sm) {
-    CTCB_CUDA_CHECK(cudaFuncSetAttribute(lstm_sweep_kernel<KI, PEEP>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)smem));
-    CTCB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(per_sm, lstm_sweep_kernel<KI, PEEP>, LS_THREADS, smem));
-    return CTCB_OK;
-}
-
-template <bool PEEP>
-static int lstm_occupancy_of(int KI, size_t smem, int *per_sm) {
-    switch (KI) {
-        case 2: return lstm_occupancy<2, PEEP>(smem, per_sm);
-        case 4: return lstm_occupancy<4, PEEP>(smem, per_sm);
-        case 8: return lstm_occupancy<8, PEEP>(smem, per_sm);
-        case 16: return lstm_occupancy<16, PEEP>(smem, per_sm);
-        case 32: return lstm_occupancy<32, PEEP>(smem, per_sm);
-        default: return lstm_occupancy<0, PEEP>(smem, per_sm);
-    }
-}
-
 // the plan of the kernel that runs: the peephole mode's occupancy is its own.  CTCB_LSTM=reread takes KI = 0 at any
 // H; CTCB_LSTM_PARTS forces the partition count, refused here, before any launch, where its CTAs cannot all be
 // co-resident.  A width whose shared memory exceeds the opt-in maximum is refused before the attribute call.
@@ -335,68 +262,26 @@ int lstm_plan(int H, int B, int ndir, bool peep, LstmPlan *p) {
     if (H <= 0 || B <= 0 || (ndir != 1 && ndir != 2))
         return set_error(CTCB_EINVAL, "LSTM sweep: bad sizes (H=%d, B=%d, ndir=%d)", H, B, ndir);
     const int slices = (H + LS_UNITS - 1) / LS_UNITS;
-    const int Hp = (H + 3) / 4 * 4 + 4;
-    p->smem = (size_t)LS_NB * Hp * sizeof(float);
+    p->smem = coop_smem(H);
     if (p->smem > max_smem_optin())
         return set_error(CTCB_EINVAL, "LSTM sweep: layerSize %d needs %zu bytes of shared memory per CTA, device allows "
                          "%zu", H, p->smem, max_smem_optin());
     const bool reg = (H == 64 || H == 128 || H == 256 || H == 512 || H == 1024) && knob(KNOB_LSTM) == 0;
-    int capacity = 0;
     for (p->KI = reg ? H / 32 : 0;; p->KI = 0) {   // U does not fit the register files the device holds: re-read it
-        const int rc = peep ? lstm_occupancy_of<true>(p->KI, p->smem, &p->per_sm)
-                            : lstm_occupancy_of<false>(p->KI, p->smem, &p->per_sm);
+        const int rc = with_ki<2, 4, 8, 16, 32>(p->KI, [&](auto ki) {
+            constexpr int KI = decltype(ki)::value;
+            return peep ? coop_occupancy(lstm_sweep_kernel<KI, true>, p->smem, &p->per_sm)
+                        : coop_occupancy(lstm_sweep_kernel<KI, false>, p->smem, &p->per_sm);
+        });
         if (rc != CTCB_OK) return rc;
-        capacity = p->per_sm * num_sms();
-        if (ndir * slices <= capacity) break;
-        if (p->KI == 0)
-            return set_error(CTCB_EINVAL, "LSTM sweep: layerSize %d needs %d co-resident CTAs, device holds %d", H,
-                             ndir * slices, capacity);
+        if (p->KI == 0 || ndir * slices <= p->per_sm * num_sms()) break;
     }
-    const int ntiles = (B + LS_NB - 1) / LS_NB;
-    int parts = capacity / (ndir * slices);
-    if (knob(KNOB_LSTM_PARTS)) {
-        if (knob(KNOB_LSTM_PARTS) > parts)
-            return set_error(CTCB_EINVAL, "LSTM sweep: CTCB_LSTM_PARTS=%d needs %d co-resident CTAs, device holds %d",
-                             knob(KNOB_LSTM_PARTS), knob(KNOB_LSTM_PARTS) * ndir * slices, capacity);
-        parts = knob(KNOB_LSTM_PARTS);
-    }
-    if (parts > ntiles) parts = ntiles;
-    if (parts > LSTM_MAX_PARTS) parts = LSTM_MAX_PARTS;
-    if (parts < 1) parts = 1;
-    p->parts = parts;
-    return CTCB_OK;
+    return coop_parts("LSTM sweep", H, p->per_sm, ndir, slices, B, knob(KNOB_LSTM_PARTS), "CTCB_LSTM_PARTS", &p->parts);
 }
 
-template <int KI, bool PEEP>
-static int lstm_launch(typename LstmArgsOf<PEEP>::type &a, int slices, const LstmPlan &p, cudaStream_t st) {
-    dim3 grid(slices, a.parts, a.ndir);
-    void *params[] = {&a};
-    CTCB_CUDA_CHECK(cudaLaunchCooperativeKernel((void *)lstm_sweep_kernel<KI, PEEP>, grid, dim3(LS_THREADS), params, p.smem,
-                                                st));
-    count_launch();
-    return CTCB_OK;
-}
-
-template <bool PEEP>
-static int lstm_launch_of(typename LstmArgsOf<PEEP>::type &a, int slices, const LstmPlan &p, cudaStream_t st) {
-    switch (p.KI) {
-        case 2: return lstm_launch<2, PEEP>(a, slices, p, st);
-        case 4: return lstm_launch<4, PEEP>(a, slices, p, st);
-        case 8: return lstm_launch<8, PEEP>(a, slices, p, st);
-        case 16: return lstm_launch<16, PEEP>(a, slices, p, st);
-        case 32: return lstm_launch<32, PEEP>(a, slices, p, st);
-        default: return lstm_launch<0, PEEP>(a, slices, p, st);
-    }
-}
-
-// ctcb_brnn_create's check that the device holds the sweep of a config; without a device there is nothing to check
-// against, and the launch checks again
+// ctcb_brnn_create's check that the device holds the sweep of a config
 int lstm_check(int H, int B, int ndir, bool peep) {
-    int n = 0;
-    if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) {
-        (void)cudaGetLastError();
-        return CTCB_OK;
-    }
+    if (no_device()) return CTCB_OK;
     LstmPlan p;
     return lstm_plan(H, B, ndir, peep, &p);
 }
@@ -419,14 +304,15 @@ int run_lstm_sweep(int mode, int T, int B, int H, const int32_t *Tlen, float *ga
     a.h[0] = hF; a.h[1] = Ub ? hB : hF;
     a.c[0] = cF; a.c[1] = Ub ? cB : cF;
     a.dh = dh; a.dz = dz; a.dc = dc;
-    a.parts = p.parts; a.ndir = ndir;
-    a.err = counters;
-    a.counters = counters + 16;     // words [0..15] are reserved for error flags
+    a.ndir = ndir;
     a.P[0] = Pf; a.P[1] = Ub ? Pb : Pf;
-    CTCB_CUDA_CHECK(cudaMemsetAsync(a.counters, 0, sizeof(unsigned int) * (ndir * p.parts), st));
     const int slices = (H + LS_UNITS - 1) / LS_UNITS;
-    if (peep) return lstm_launch_of<true>(a, slices, p, st);
-    return lstm_launch_of<false>(static_cast<LstmArgs &>(a), slices, p, st);
+    return with_ki<2, 4, 8, 16, 32>(p.KI, [&](auto ki) {
+        constexpr int KI = decltype(ki)::value;
+        return peep ? coop_launch(lstm_sweep_kernel<KI, true>, a, counters, slices, p.parts, p.smem, st)
+                    : coop_launch(lstm_sweep_kernel<KI, false>, static_cast<LstmArgs &>(a), counters, slices, p.parts,
+                                  p.smem, st);
+    });
 }
 
 // ---- the peephole weight gradients -----------------------------------------------------------------------------
@@ -572,10 +458,9 @@ extern "C" int ctcb_debug_lstm_plan(int H, int B, int ndir, int peephole, int32_
     ctcb::LstmPlan p;
     const int rc = ctcb::lstm_plan(H, B, ndir, peephole != 0, &p);
     if (rc != CTCB_OK) return rc;
-    const int ntiles = (B + ctcb::LS_NB - 1) / ctcb::LS_NB;
     out[0] = p.KI;
     out[1] = p.parts;
     out[2] = p.per_sm;
-    out[3] = (ntiles + p.parts - 1) / p.parts;
+    out[3] = (ctcb::coop_tiles(B) + p.parts - 1) / p.parts;
     return CTCB_OK;
 }
