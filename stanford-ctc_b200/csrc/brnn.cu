@@ -979,7 +979,9 @@ int Step::rec_weight_grads(int j) const {
     const int H = h->cfg.layerSize, iWtf = h->rec(j), iWtb = iWtf + 2;
     float *dFor = buf(w.dFor[j % 2]), *dBack = buf(w.dBack[j % 2]);
     CTCB_CUDA_CHECK(cudaEventRecord(h->ev_sweep, main));
+    TRY(stall(main, STALL_MAIN));
     CTCB_CUDA_CHECK(cudaStreamWaitEvent(side, h->ev_sweep, 0));
+    TRY(stall(side, STALL_SIDE));
     ProfScope ps("gemm_dw_rec", side);
     const int Tmax = T(h->tl + j);
     const int64_t R = this->R(h->tl + j);
@@ -1070,6 +1072,7 @@ int Step::backward() const {
             CTCB_CUDA_CHECK(cudaStreamWaitEvent(main, h->ev_pair[p], 0));
         // the deltas of maps side_top..i are complete here
         CTCB_CUDA_CHECK(cudaEventRecord(h->ev_delta[i], main));
+        TRY(stall(main, STALL_MAIN));
         {
         ProfScope ps("sweep_bptt", main);
         if (lstm)
@@ -1082,6 +1085,7 @@ int Step::backward() const {
                           buf(w.dBack[p]), m.For[j], m.Back[j], h->cfg.maxAct, m.counters, m.sweep, m.sweep_bytes, main));
         }
         CTCB_CUDA_CHECK(cudaStreamWaitEvent(side, h->ev_delta[i], 0));
+        TRY(stall(side, STALL_SIDE));
         for (; side_top >= i; --side_top) TRY(weight_grads(side_top, true));
         TRY(rec_weight_grads(j));
         if (!uni && !lstm) {
@@ -1172,6 +1176,7 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
         TRY(ensure_side_stream(h));
         CTCB_CUDA_CHECK(cudaEventRecord(h->ev_fork, caller));
         CTCB_CUDA_CHECK(cudaStreamWaitEvent(h->hi, h->ev_fork, 0));
+        TRY(stall(h->hi, STALL_MAIN));
         s.main = h->hi;
         s.side = h->side;
     }

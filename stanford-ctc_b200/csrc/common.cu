@@ -75,6 +75,8 @@ static const KnobDef KNOBS[KNOB_COUNT] = {
     {"CTCB_LSTM", 0, {"auto", "reread"}},
     {"CTCB_LSTM_PARTS", 0, {"auto"}, COOP_SWEEP_MAX_PARTS},
     {"CTCB_SWEEP_PARTS", 0, {"auto"}, COOP_SWEEP_MAX_PARTS},
+    {"CTCB_STALL", STALL_OFF, {"off", "main", "side"}},
+    {"CTCB_STALL_US", 2000, {}, STALL_MAX_US},
 };
 static int g_knob_initial[KNOB_COUNT], g_knob[KNOB_COUNT];     // what the environment said, what is in effect
 static std::once_flag g_knob_once;
@@ -105,6 +107,25 @@ static int *knob_table() {
 }
 
 int knob(Knob k) { return knob_table()[k]; }
+
+// One warp sleeping on %globaltimer until ns have passed; it writes nothing, and ns is clamped to the knob's maximum,
+// so the wait always ends.
+__global__ void stall_kernel(uint64_t ns) {
+    ns = ns < (uint64_t)STALL_MAX_US * 1000u ? ns : (uint64_t)STALL_MAX_US * 1000u;
+    uint64_t t0, t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
+    do {
+        __nanosleep(1000);
+        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    } while (t - t0 < ns);
+}
+
+int stall(cudaStream_t st, int which) {
+    if (which == STALL_OFF || knob(KNOB_STALL) != which) return CTCB_OK;
+    stall_kernel<<<1, 32, 0, st>>>((uint64_t)knob(KNOB_STALL_US) * 1000u);
+    CTCB_LAUNCH_CHECK();
+    return CTCB_OK;
+}
 
 static bool g_prof_on = false;
 struct ProfRec { std::string name; cudaEvent_t a, b; };

@@ -43,8 +43,15 @@ int stream_priority_greatest();
 // Debug / measurement overrides of the planners (INTEGRATION.md section 4): one table (common.cu), filled from the
 // environment at first use and changed by ctcb_debug_set_knob.  Planners read it through knob() on every planning call.
 enum Knob { KNOB_GEMM, KNOB_GEMM_TC_COPY, KNOB_GEMM_TRACE, KNOB_SWEEP, KNOB_SWEEP_NB, KNOB_SWEEP_TC, KNOB_SWEEP_TC_CS,
-            KNOB_SWEEP_TC_COOP, KNOB_SWEEP_TRACE, KNOB_CTC, KNOB_LSTM, KNOB_LSTM_PARTS, KNOB_SWEEP_PARTS, KNOB_COUNT };
+            KNOB_SWEEP_TC_COOP, KNOB_SWEEP_TRACE, KNOB_CTC, KNOB_LSTM, KNOB_LSTM_PARTS, KNOB_SWEEP_PARTS, KNOB_STALL,
+            KNOB_STALL_US, KNOB_COUNT };
 int knob(Knob k);
+// The schedule test's stall hook (CTCB_STALL, CTCB_STALL_US): stall(st, which) launches one warp that holds `st` for
+// CTCB_STALL_US microseconds when CTCB_STALL names `which`, and does nothing otherwise (off, the default, names neither).
+// The training step calls it right after each point where one of its streams releases or is released by the other.
+enum { STALL_OFF = 0, STALL_MAIN = 1, STALL_SIDE = 2 };
+constexpr int STALL_MAX_US = 100000;
+int stall(cudaStream_t st, int which);
 // The most utterance partitions of a cooperative sweep (the generic and LSTM kernels, coop_sweep.cuh): their barrier
 // counters ([ndir][parts] words) share 4 KB of scratch with the 16 error words.  CTCB_SWEEP_PARTS and CTCB_LSTM_PARTS
 // take auto or 1..COOP_SWEEP_MAX_PARTS.

@@ -157,7 +157,9 @@ KNOBS = {"CTCB_GEMM": (["simt"], "s"), "CTCB_GEMM_TC_COPY": (["0", "1"], "2"), "
          "CTCB_SWEEP_TC_COOP": (["0"], "1"), "CTCB_SWEEP_TRACE": (["1"], "0"),
          "CTCB_CTC": (["auto", "warp", "pair", "par", "ckpt"], "pa"), "CTCB_LSTM": (["auto", "reread"], "reg"),
          "CTCB_LSTM_PARTS": (["auto", "1", "2", "3", "17", "499", "500"], "501"),
-         "CTCB_SWEEP_PARTS": (["auto", "1", "2", "3", "17", "499", "500"], "501")}
+         "CTCB_SWEEP_PARTS": (["auto", "1", "2", "3", "17", "499", "500"], "501"),
+         "CTCB_STALL": (["off", "main", "side"], "both"),
+         "CTCB_STALL_US": (["1", "2", "500", "2000", "99999", "100000"], "100001")}
 
 
 def _ckpt_refuses():
@@ -183,6 +185,9 @@ def test_set_knob_takes_the_documented_values_only():
     for v in ("0", "01", "-1", "+2", "2x", " 2", "4294967298"):     # the partition count is a plain decimal 1..500
         assert lib.ctcb_debug_set_knob(b"CTCB_LSTM_PARTS", v.encode()) == -1, v
         assert lib.ctcb_debug_set_knob(b"CTCB_SWEEP_PARTS", v.encode()) == -1, v
+        assert lib.ctcb_debug_set_knob(b"CTCB_STALL_US", v.encode()) == -1, v     # and the stall 1..100000 us
+    for v in ("auto", "off", "main"):                                  # the stall length has no named value
+        assert lib.ctcb_debug_set_knob(b"CTCB_STALL_US", v.encode()) == -1, v
     # a refused value leaves the table as it was
     assert lib.ctcb_debug_set_knob(b"CTCB_CTC", b"ckpt") == 0 and _ckpt_refuses()
     assert lib.ctcb_debug_set_knob(b"CTCB_CTC", b"pa") == -1 and _ckpt_refuses()
