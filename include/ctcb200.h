@@ -191,6 +191,11 @@ typedef struct ctcb_brnn_config {
     int32_t peephole;      /* 0: off (so an initialiser without this member keeps its meaning); 1: peephole connections of
                             * the LSTM cell (below), which needs cell = 1; any other value, or 1 with cell = 0, makes the
                             * config invalid.  Without a temporal layer it lays out and launches nothing. */
+    int32_t maskFeatDim;   /* nu: 0 off (so an initialiser without this member keeps its meaning); nu > 0 lays the input
+                            * rows out as c = inputDim / nu frame slots of nu filter-bank bins for the SpecAugment masks
+                            * of ctcb_brnn_set_input_masks (below) and reserves their masked copy in the training
+                            * workspace.  Invalid: nu < 0, nu not dividing inputDim, an even c, or a layout whose bit sets
+                            * exceed the mask pass's 48 KB of shared memory (about inputDim + 64 > 393,000 bits). */
 } ctcb_brnn_config;
 
 /* Frame subsampling (subsample = k >= 2; not in the reference; cf. Deep Speech 2's striding and the frame stacking of
@@ -263,6 +268,7 @@ typedef struct ctcb_brnn ctcb_brnn; /* opaque; owns no device memory */
  * layerNorm = 1 appends [gamma_i, beta_i] of every normalised hidden layer i, in ascending i.
  * peephole = 1 then appends [P_f,j, dummy] [P_b,j, dummy] (unidirectional: [P_j, dummy]) of every temporal layer j in
  * ascending order, each P 3 x H. */
+/* maskFeatDim = nu > 0 adds no parameter. */
 int64_t ctcb_brnn_param_count(const ctcb_brnn_config *cfg);
 int ctcb_brnn_num_tensors(const ctcb_brnn_config *cfg);                    /* 2 * len(stack) */
 int ctcb_brnn_tensor_info(const ctcb_brnn_config *cfg, int idx, int64_t *offset, int32_t *rows, int32_t *cols);
@@ -284,7 +290,9 @@ int ctcb_brnn_tensor_info(const ctcb_brnn_config *cfg, int idx, int64_t *offset,
  * workspace.  With k <= 1 no offset moves and nothing is appended.
  * peephole = 1 (with a temporal layer) appends, behind everything else, the partial sums of the peephole weight
  * gradients, ctcb_lstm_peephole_grad_workspace_bytes(Tmax_l, maxB, layerSize, ndir) bytes for the frames Tmax_l of the
- * lowest temporal layer (maxT, or ceil(maxT / k) above the subsampling point).  The forward workspace does not grow. */
+ * lowest temporal layer (maxT, or ceil(maxT / k) above the subsampling point).  The forward workspace does not grow.
+ * maskFeatDim = nu > 0 appends, behind everything else, the masked copy of a call's features: maxT*maxB*inputDim floats
+ * rounded up to 256 bytes.  No other offset moves, and the forward workspace does not grow. */
 size_t ctcb_brnn_workspace_bytes(const ctcb_brnn_config *cfg);
 /* Byte offset, inside the workspace, of a uint32 that the recurrent-sweep kernels set non-zero when an
  * inter-CTA wait timed out (results are then invalid; never a hang).  Callers that synchronise anyway
@@ -386,13 +394,48 @@ int ctcb_brnn_apply_l2_f32(ctcb_brnn *h, const float *params, float *grads, void
 int ctcb_brnn_set_dropout(ctcb_brnn *h, float p, uint64_t seed, const int64_t *step);
 /* Utterance u of the following calls is minibatch utterance g = first + stride * u: rank + world * (u0 + u) for rank
  * `rank` of `world` (round-robin shards) and a micro-batch starting at position u0 of the rank's shard, so one call, a
- * micro-batched step and a data-parallel step draw the same mask for the same utterance.  Default (0, 1).  CTCB_EINVAL
- * for first < 0 or stride < 1.  Host-only. */
+ * micro-batched step and a data-parallel step draw the same mask for the same utterance.  The same g places the
+ * utterance for the input masks (ctcb_brnn_set_input_masks).  Default (0, 1).  CTCB_EINVAL for first < 0 or
+ * stride < 1.  Host-only. */
 int ctcb_brnn_set_dropout_utts(ctcb_brnn *h, int64_t first, int64_t stride);
 /* *step += 1 on `stream` (one thread); inside a capture it becomes part of the graph like any other launch.  The
  * counter is the optimisation step: the dropout mask and the adaptive optimisers (ctcb_adagrad_step_f32,
  * ctcb_adam_step_f32) read the same one, and sgd.SGD advances it once per step, so it equals SGD.it. */
 int ctcb_dropout_advance(int64_t *step, void *stream);
+
+/* ---- SpecAugment: frequency and time masks of the input features (Park et al., Interspeech 2019) --------------------
+ * Layout (maskFeatDim = nu > 0): row t' of utterance u holds c = inputDim / nu frame slots of nu bins each, frame-major
+ * (Kaldi splice-feats), c odd, h = (c - 1) / 2; slot j holds raw frame clamp(t' + j - h, 0, T_u - 1), so splicing
+ * repeats the edge frames.  c = 1 is features without splicing.
+ * Policy: m_F = freqMasks, F = freqWidth, m_T = timeMasks, T = timeWidth, p = timeRatio.  Minibatch utterance g (as
+ * ctcb_brnn_set_dropout_utts places it) at optimisation step s draws, for mask k = 0 .. m_F + m_T - 1, one block
+ *     (r0, r1, r2, r3) = Philox4x32-10(counter = (s mod 2^32, g mod 2^32, 0, k), key = (seed mod 2^32, seed >> 32))
+ * (k < 2^24, dropout's fourth counter word is >= 2^24, so the two can share a seed), and with 64-bit integer products:
+ *   k <  m_F: width w = (r0 (F + 1)) >> 32, start f0 = (r1 (nu - w + 1)) >> 32: bins [f0, f0 + w) are masked;
+ *   k >= m_F: W = min(T, floor(p T_u)) (the product in float64), w = (r0 (W + 1)) >> 32, t0 = (r1 (T_u - w + 1)) >> 32:
+ *             raw frames [t0, t0 + w) are masked.
+ * Element (t' < T_u, slot j, bin b) becomes +0.0 where b lies in a frequency band or its raw frame in a time band
+ * (bands may overlap); every other element, the padding rows t' >= T_u included, is copied bit for bit.
+ * Limits: m_F and m_T in 0..64, 0 <= F <= nu, T >= 0, p in [0, 1].
+ *
+ * ctcb_brnn_set_input_masks: every TRAINING call (grads != NULL) then writes the masked copy of feats into its workspace
+ * (maxT*maxB*inputDim floats behind everything else) with one pass on the main chain, and every stage reads that copy:
+ * map 1's contraction, the frame stacking when subsampleLayer = 1, map 1's weight gradient.  feats is never written, so
+ * a replayed step over one device batch does not mask twice and forward-only calls (grads == NULL, which never mask)
+ * see the original features.  step is the int64 DEVICE counter of ctcb_dropout_advance, read when the pass runs.  Both
+ * counts 0 (the default) disables it: the call reads feats and issues exactly the launches it does without.
+ * CTCB_EINVAL for values outside the limits, counts > 0 on a config with maskFeatDim = 0, or counts > 0 with a null
+ * step.  Host-only: no device work. */
+int ctcb_brnn_set_input_masks(ctcb_brnn *h, int freqMasks, int freqWidth, int timeMasks, int timeWidth,
+                              double timeRatio, uint64_t seed, const int64_t *step);
+/* The pass on its own, with the launch a training call makes: out = feats masked for the utterances g = first +
+ * stride * u, both [Tmax][B][inputDim] (out must not overlap feats), T_per_utt int32[B] (<= Tmax).  16-byte accesses
+ * where inputDim % 4 == 0 and both arrays are 16-byte aligned, else 4-byte ones.  With both counts 0 it copies and step
+ * may be NULL.  CTCB_EINVAL for a layout the config would refuse, a policy outside the limits, first < 0, stride < 1,
+ * B or Tmax < 1, or B * Tmax >= 2^31. */
+int ctcb_input_mask_f32(const float *feats, const int32_t *T_per_utt, int B, int Tmax, int inputDim, int featDim,
+                        int freqMasks, int freqWidth, int timeMasks, int timeWidth, double timeRatio, uint64_t seed,
+                        const int64_t *step, int64_t first, int64_t stride, float *out, void *stream);
 
 /* ---- layer normalisation on its own (layerNorm = 1, above) -----------------------------------------------------
  * Rows are [R][H] fp32, 1 <= H <= CTCB_LAYERNORM_MAX_H; with H % 4 == 0 every pointer must be 16-byte aligned.

@@ -31,6 +31,11 @@ int comm_allreduce_ranges(ctcb_comm *c, float *const *ptrs, const int64_t *count
 int comm_world(const ctcb_comm *c);
 int run_dropout(float *X, int64_t R, int B, int H, int layer, uint64_t seed, const int64_t *step, int64_t first,
                 int64_t stride, uint32_t thr, float scale, cudaStream_t st);
+const char *input_mask_layout_error(int D, int nu, char (&buf)[192]);
+const char *input_mask_policy_error(int nu, int mF, int F, int mT, int Tw, double p, char (&buf)[192]);
+int run_input_mask(const float *x, const int32_t *lens, int B, int Tmax, int D, int nu, int mF, int F, int mT, int Tw,
+                   double p, uint64_t seed, const int64_t *step, int64_t first, int64_t stride, float *y,
+                   cudaStream_t st);
 size_t lstm_carry_bytes(int H, int B);
 int run_lstm_sweep(int mode, int T, int B, int H, const int32_t *Tlen, float *gates, const float *Uf, const float *Ub,
                    const float *Pf, const float *Pb, float *hF, float *hB, float *cF, float *cB, const float *dh,
@@ -249,6 +254,13 @@ static const char *cfg_error(const ctcb_brnn_config *c, char (&buf)[192]) {
         if ((int64_t)k * n > 0x7fffffff || ((int64_t)c->maxT + k - 1) / k * k * c->maxB > 0x7fffffff)
             return say("subsample %d: %d x %d stacked columns or ceil(maxT / k) * k * maxB rows exceed 2^31 - 1", k, k, n);
     }
+    if (c->maskFeatDim < 0)
+        return say("maskFeatDim %d is negative (0: no input masks; nu > 0: nu filter-bank bins per frame slot)",
+                   c->maskFeatDim);
+    if (c->maskFeatDim > 0) {
+        char why[192];
+        if (const char *e = input_mask_layout_error(c->inputDim, c->maskFeatDim, why)) return say("maskFeatDim: %s", e);
+    }
     const bool ok = c->inputDim > 0 && c->outputDim > 1 && c->layerSize > 0 && c->numLayers >= 1 && c->numLayers <= 64 &&
                     c->maxT > 0 && c->maxB > 0 && c->maxLabels >= 0 && c->numTemporal >= 0 &&
                     // a stacked block must lie inside the hidden layers; k <= 1 keeps the silent "no temporal layer" rule below
@@ -446,6 +458,7 @@ struct WsLayout {
     // subsampling only (0 elsewhere): the stacked input S of map L, its delta dS (L >= 2), T'_u of the call
     size_t S, dS, lens;
     size_t peep_part;   // peephole nets only (0 elsewhere): the partial sums of the peephole weight gradients
+    size_t masked;      // maskFeatDim > 0 only (0 elsewhere): the masked copy of the call's features
     size_t total;
 };
 
@@ -534,6 +547,8 @@ WsLayout ws_layout(const ctcb_brnn_config *c) {
     }
     if (peep_tensors(c))     // the lowest temporal layer has the most rows
         w.peep_part = take(off, lstm_peephole_grad_bytes((int64_t)max_rows(c, tl), H, uni ? 1 : 2));
+    if (c->maskFeatDim > 0)     // read by map 1 (its contraction, the frame stacking, its weight gradient) all call long
+        w.masked = take(off, (size_t)c->maxT * c->maxB * c->inputDim * sizeof(float));
     w.total = off;
     return w;
 }
@@ -700,7 +715,13 @@ struct ctcb_brnn {
     const int64_t *drop_step = nullptr;     // the caller's device counter
     uint32_t drop_thr = 0;                  // keep iff Philox output >= drop_thr
     float drop_scale = 1.f;                 // 1 / (1 - p), rounded once; also the delta contraction's alpha
-    int64_t drop_first = 0, drop_stride = 1;
+    int64_t drop_first = 0, drop_stride = 1;     // the minibatch index of utterance u, for dropout and the input masks
+    // SpecAugment masks of the input features in training calls (ctcb_brnn_set_input_masks); mask_f + mask_t == 0: off
+    int mask_f = 0, mask_fw = 0, mask_t = 0, mask_tw = 0;
+    double mask_p = 1.0;
+    uint64_t mask_seed = 0;
+    const int64_t *mask_step = nullptr;
+    bool masks_on() const { return mask_f + mask_t > 0; }
 
     bool uni() const { return cfg.unidirectional != 0; }
     bool lstm() const { return cfg.cell == 1; }
@@ -1169,7 +1190,9 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
     FwdBufs m{};
     train_bufs(w, N, h->nt, ws, &m);
     const bool dp = (h->comm != nullptr) && comm_world(h->comm) > 1;
-    Step s{h, m, w, ws, feats, params, T_per_utt, grads, B, Tmax, first, last, h->drop_p > 0.f, dp,
+    // with input masks on, every stage of the call reads the masked copy in place of feats, which it never writes
+    const float *in = h->masks_on() ? (const float *)(ws + w.masked) : feats;
+    Step s{h, m, w, ws, in, params, T_per_utt, grads, B, Tmax, first, last, h->drop_p > 0.f, dp,
            caller, nullptr, caller};
     const bool overlap = (h->tl > 0);
     if (overlap) {     // fork: the main chain runs on h->hi until the join below
@@ -1180,7 +1203,13 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
         s.main = h->hi;
         s.side = h->side;
     }
-    TRY(brnn_forward(h, feats, T_per_utt, B, Tmax, params, probs_out, m, s.drop, s.main));
+    if (h->masks_on()) {     // the side stream reads the copy only behind events recorded on main after this
+        ProfScope ps("input_mask", s.main);
+        TRY(run_input_mask(feats, T_per_utt, B, Tmax, c.inputDim, c.maskFeatDim, h->mask_f, h->mask_fw, h->mask_t,
+                           h->mask_tw, h->mask_p, h->mask_seed, h->mask_step, h->drop_first, h->drop_stride,
+                           (float *)(ws + w.masked), s.main));
+    }
+    TRY(brnn_forward(h, in, T_per_utt, B, Tmax, params, probs_out, m, s.drop, s.main));
     {     // brnnet.py:161-175
     ProfScope ps("ctc", s.main);
     TRY(ctcb_ctc_loss_grad_f32(m.X[N + 1], 0, (int64_t)K, (int64_t)B * K, labels, label_off, s.lens(N + 1), B, s.T(N + 1), K,
@@ -1261,6 +1290,26 @@ extern "C" int ctcb_brnn_set_dropout_utts(ctcb_brnn *h, int64_t first, int64_t s
                          "stride >= 1)", (long long)first, (long long)stride);
     h->drop_first = first;
     h->drop_stride = stride;
+    return CTCB_OK;
+}
+
+extern "C" int ctcb_brnn_set_input_masks(ctcb_brnn *h, int freqMasks, int freqWidth, int timeMasks, int timeWidth,
+                                         double timeRatio, uint64_t seed, const int64_t *step) {
+    if (!h) return set_error(CTCB_EINVAL, "ctcb_brnn_set_input_masks: null handle");
+    char buf[192];
+    if (const char *why = input_mask_policy_error(h->cfg.maskFeatDim, freqMasks, freqWidth, timeMasks, timeWidth,
+                                                  timeRatio, buf))
+        return set_error(CTCB_EINVAL, "ctcb_brnn_set_input_masks: %s", why);
+    if (freqMasks + timeMasks > 0 && !step)
+        return set_error(CTCB_EINVAL, "ctcb_brnn_set_input_masks: %d frequency and %d time masks need a step counter",
+                         freqMasks, timeMasks);
+    h->mask_f = freqMasks;
+    h->mask_fw = freqWidth;
+    h->mask_t = timeMasks;
+    h->mask_tw = timeWidth;
+    h->mask_p = timeRatio;
+    h->mask_seed = seed;
+    h->mask_step = step;
     return CTCB_OK;
 }
 

@@ -32,6 +32,12 @@ single contiguous vector.  New, additive surface for the minibatch/data-parallel
     NNet(..., dropout=p, dropoutSeed=33)     inverted dropout on the ReLU hidden layers of training calls; the mask
                                                 of an utterance is drawn from (seed, the device counter dropoutStep,
                                                 layer, its index in the step's minibatch, frame, unit)
+    NNet(..., freqMasks=2, freqMaskWidth=15, timeMasks=2, timeMaskWidth=70, timeMaskRatio=0.2, featDim=41)
+                                             SpecAugment masks of the input features of training calls
+                                                (include/ctcb200.h: ctcb_brnn_set_input_masks): bands of the featDim
+                                                filter-bank bins of each spliced frame slot and spans of raw frames,
+                                                drawn from (seed dropoutSeed, the counter dropoutStep, the utterance's
+                                                index in the step's minibatch); featDim=None is inputDim (no splicing)
     costAndGradBatch(datas, labelss)         -> (costs[B], grad, skips[B])   host arrays in; more than maxUtts
                                                 utterances are accumulated over micro-batches
     costAndGradDevice(batch, first, last)    -> no host sync; see DeviceBatch
@@ -157,7 +163,8 @@ class NNet:
     def __init__(self, inputDim, outputDim, layerSize, numLayers, maxBatch,
                  train=True, temporalLayer=-1, reg=0.0, maxUtts=1, maxLabels=None,
                  allowTopTemporal=False, device=None, unidirectional=False, numTemporal=1, dropout=0.0,
-                 dropoutSeed=33, cell="relu", layerNorm=False, subsample=1, subsampleLayer=1, peephole=False):
+                 dropoutSeed=33, cell="relu", layerNorm=False, subsample=1, subsampleLayer=1, peephole=False,
+                 freqMasks=0, freqMaskWidth=0, timeMasks=0, timeMaskWidth=0, timeMaskRatio=1.0, featDim=None):
         torch = _ctcb.require_cuda()
         self._torch = torch
         self.dev = torch.device("cuda", torch.cuda.current_device() if device is None else device)
@@ -208,28 +215,41 @@ class NNet:
         self.layerNorm = bool(layerNorm)
         # 0 and 1: off; the config refuses k < 0 and an L outside 1..numLayers+1 with a message (ValueError)
         self.subsample, self.subsampleLayer = int(subsample), int(subsampleLayer)
+        # SpecAugment (include/ctcb200.h: ctcb_brnn_set_input_masks).  Only a net that masks lays its input out in
+        # frame slots of featDim bins and reserves the masked copy, so a net without masks keeps today's workspace.
+        self.freqMasks, self.freqMaskWidth = int(freqMasks), int(freqMaskWidth)
+        self.timeMasks, self.timeMaskWidth, self.timeMaskRatio = int(timeMasks), int(timeMaskWidth), float(timeMaskRatio)
+        self.inputMasks = self.freqMasks != 0 or self.timeMasks != 0      # negative counts: refused below
+        if featDim is not None and not self.inputMasks:
+            raise ValueError("featDim=%r is the layout of the input masks; it needs freqMasks or timeMasks > 0"
+                             % (featDim,))
+        self.featDim = (inputDim if featDim is None else int(featDim)) if self.inputMasks else None
         self._cfg = BrnnConfig(inputDim, outputDim, layerSize, numLayers, max(self.temporalLayer, 0), maxBatch,
                                maxUtts, self.maxLabels, float(reg), float(self.maxAct), int(self.unidirectional),
                                self.numTemporal, _ctcb.CELLS[cell], int(self.layerNorm), self.subsample,
-                               self.subsampleLayer, int(self.peephole))
+                               self.subsampleLayer, int(self.peephole), self.featDim or 0)
         self._h = ctypes.c_void_p()
         check(lib.ctcb_brnn_create(ctypes.byref(self._cfg), ctypes.byref(self._h)))
         self.stack = None
         self.grad = None
-        # Inverted dropout (include/ctcb200.h: ctcb_brnn_set_dropout).  The step counter lives on the device, so a CUDA
-        # graph of an SGD step reads its current value at every replay; sgd.SGD advances it once per step.
-        # dropoutShard = (rank, world) places this process's utterances in the step's minibatch (None: from
-        # torch.distributed).
+        # Inverted dropout (include/ctcb200.h: ctcb_brnn_set_dropout) and the input masks.  The step counter lives on the
+        # device, so a CUDA graph of an SGD step reads its current value at every replay; sgd.SGD advances it once per
+        # step.  The net owns it when either is on.  dropoutShard = (rank, world) places this process's utterances in
+        # the step's minibatch for both (None: from torch.distributed).
         self.dropout = float(dropout)
         self.dropoutSeed = int(dropoutSeed)
         self.dropoutStep = None
         self.dropoutShard = None
-        if self.dropout != 0.0:
-            if not 0.0 < self.dropout < 1.0:
-                raise ValueError("dropout=%r must be in [0, 1)" % (dropout,))
+        if self.dropout != 0.0 and not 0.0 < self.dropout < 1.0:
+            raise ValueError("dropout=%r must be in [0, 1)" % (dropout,))
+        if self.dropout != 0.0 or self.inputMasks:
             self.dropoutStep = torch.zeros(1, dtype=torch.int64, device=self.dev)
-            check(lib.ctcb_brnn_set_dropout(self._h, self.dropout, self.dropoutSeed & 0xFFFFFFFFFFFFFFFF,
-                                            ptr(self.dropoutStep)))
+        seed = self.dropoutSeed & 0xFFFFFFFFFFFFFFFF
+        if self.dropout != 0.0:
+            check(lib.ctcb_brnn_set_dropout(self._h, self.dropout, seed, ptr(self.dropoutStep)))
+        # called with counts 0 too, so that every value outside the limits is refused with the library's message
+        check(lib.ctcb_brnn_set_input_masks(self._h, self.freqMasks, self.freqMaskWidth, self.timeMasks,
+                                            self.timeMaskWidth, self.timeMaskRatio, seed, ptr(self.dropoutStep)))
 
     def __del__(self):
         h = getattr(self, "_h", None)
@@ -368,10 +388,10 @@ class NNet:
         the gradient and the statistics tail into what the earlier calls left; only the last=True call exchanges
         over the ranks and adds the L2 term.  `out` optionally names the (cost[B], skip[B]) device tensors to write
         (default: the net's own per-utterance buffers).  u0: position of the batch's first utterance in this rank's
-        shard of the step, which with the rank places each utterance in the minibatch for its dropout mask."""
+        shard of the step, which with the rank places each utterance in the minibatch for its dropout and input masks."""
         if not self.train:
             return self._forward_device(batch)
-        if self.dropout > 0.0:
+        if self.dropout > 0.0 or self.inputMasks:
             rank, world = self.dropoutShard or parallel.world_info()[1:]
             check(lib.ctcb_brnn_set_dropout_utts(self._h, rank + world * u0, world))
         B, Tmax = batch.B, batch.Tmax
@@ -567,7 +587,7 @@ class NNet:
     def check_grad(self, data, labels, epsilon=1e-3, maxChecks=10, verbose=True):
         """Finite-difference check on a small section of every weight matrix (brnnet.py:279-297).
         Returns the list of (analytic, numeric) pairs it printed.  costAndGrad never advances the dropout counter,
-        so every evaluation sees the same mask."""
+        so every evaluation sees the same dropout and input masks."""
         cost, grad, _ = self.costAndGrad(data, labels)
         out = []
         ana = [dw.clone() for dw, _ in grad]

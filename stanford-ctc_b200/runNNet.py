@@ -8,7 +8,8 @@ last_cost, sentinel, train.log), resume through --cfg_file with the step size re
 The implementation is organised differently: a declarative flag table, one RunDir helper that owns the
 side files, and separate train/evaluate phases.  Site paths of run_cfg.py / decoder_config.py became
 flags (--runDir, --outDir); new flags: --numTemporal, --cell, --peephole, --layerNorm, --subsample, --subsampleLayer, --batchSize, --maxUtts, --maxLabels,
---dropout, --optimizer, --beta1, --beta2, --epsilon, --quiet.  Under torchrun the same
+--dropout, --freqMasks, --freqMaskWidth, --timeMasks, --timeMaskWidth, --timeMaskRatio, --featDim, --optimizer,
+--beta1, --beta2, --epsilon, --quiet.  Under torchrun the same
 script trains data-parallel (one process per GPU, one NCCL all-reduce per step).
 """
 import argparse
@@ -63,6 +64,15 @@ FLAGS = [
     ("maxLabels", int, 511, "longest label sequence the buffers are sized for"),
     ("dropout", float, 0.0, "inverted dropout probability on the ReLU hidden layers while training (0 = off; "
                             "--test never drops)"),
+    ("freqMasks", int, 0, "SpecAugment while training: frequency masks per utterance and step, each a band of at most "
+                          "--freqMaskWidth filter-bank bins of every frame slot (0 = off; --test never masks; a cfg.json "
+                          "written without it has none)"),
+    ("freqMaskWidth", int, 0, "widest frequency mask, in bins (at most --featDim)"),
+    ("timeMasks", int, 0, "SpecAugment while training: time masks per utterance and step, each a span of raw frames"),
+    ("timeMaskWidth", int, 0, "widest time mask, in frames"),
+    ("timeMaskRatio", float, 1.0, "a time mask covers at most this fraction of the utterance's frames"),
+    ("featDim", int, None, "filter-bank bins per frame slot of the spliced input (e.g. 41 for --inputDim 41*15); "
+                           "default --inputDim, features without splicing"),
     ("optimizer", str, "nesterov", "update rule: nesterov (the reference's, with --momentum), adagrad or adam; --step "
                                    "is the step size of each and --anneal applies to it"),
     ("beta1", float, 0.9, "adam: decay of the first-moment estimate"),
@@ -209,7 +219,9 @@ def _train(opts, cfg, run_dir, log, rank, world):
                      maxUtts=utterance_capacity(opts, world),
                      maxLabels=min(opts.maxLabels, opts.maxUttLen), dropout=opts.dropout, cell=opts.cell,
                      layerNorm=opts.layerNorm, subsample=opts.subsample, subsampleLayer=opts.subsampleLayer,
-                     peephole=opts.peephole)
+                     peephole=opts.peephole, freqMasks=opts.freqMasks, freqMaskWidth=opts.freqMaskWidth,
+                     timeMasks=opts.timeMasks, timeMaskWidth=opts.timeMaskWidth, timeMaskRatio=opts.timeMaskRatio,
+                     featDim=opts.featDim)
     net.initParams()
     optimizer = sgd.SGD(net, opts.maxUttLen, alpha=opts.step, optimizer=opts.optimizer, momentum=opts.momentum,
                         batchSize=opts.batchSize, verbose=(rank == 0 and not opts.quiet), beta1=opts.beta1,
