@@ -196,6 +196,9 @@ typedef struct ctcb_brnn_config {
                             * of ctcb_brnn_set_input_masks (below) and reserves their masked copy in the training
                             * workspace.  Invalid: nu < 0, nu not dividing inputDim, an even c, or a layout whose bit sets
                             * exceed the mask pass's 48 KB of shared memory (about inputDim + 64 > 393,000 bits). */
+    int32_t weightNoise;   /* 0: off (so an initialiser without this member keeps its meaning); 1: reserves the noisy copy
+                            * of the parameters for the Gaussian weight noise of ctcb_brnn_set_weight_noise (below) in
+                            * the training workspace; any other value makes the config invalid. */
 } ctcb_brnn_config;
 
 /* Frame subsampling (subsample = k >= 2; not in the reference; cf. Deep Speech 2's striding and the frame stacking of
@@ -268,7 +271,7 @@ typedef struct ctcb_brnn ctcb_brnn; /* opaque; owns no device memory */
  * layerNorm = 1 appends [gamma_i, beta_i] of every normalised hidden layer i, in ascending i.
  * peephole = 1 then appends [P_f,j, dummy] [P_b,j, dummy] (unidirectional: [P_j, dummy]) of every temporal layer j in
  * ascending order, each P 3 x H. */
-/* maskFeatDim = nu > 0 adds no parameter. */
+/* maskFeatDim = nu > 0 adds no parameter, and neither does weightNoise = 1. */
 int64_t ctcb_brnn_param_count(const ctcb_brnn_config *cfg);
 int ctcb_brnn_num_tensors(const ctcb_brnn_config *cfg);                    /* 2 * len(stack) */
 int ctcb_brnn_tensor_info(const ctcb_brnn_config *cfg, int idx, int64_t *offset, int32_t *rows, int32_t *cols);
@@ -292,6 +295,8 @@ int ctcb_brnn_tensor_info(const ctcb_brnn_config *cfg, int idx, int64_t *offset,
  * gradients, ctcb_lstm_peephole_grad_workspace_bytes(Tmax_l, maxB, layerSize, ndir) bytes for the frames Tmax_l of the
  * lowest temporal layer (maxT, or ceil(maxT / k) above the subsampling point).  The forward workspace does not grow.
  * maskFeatDim = nu > 0 appends, behind everything else, the masked copy of a call's features: maxT*maxB*inputDim floats
+ * rounded up to 256 bytes.  No other offset moves, and the forward workspace does not grow.
+ * weightNoise = 1 appends, behind everything else, the noisy copy of the parameters: ctcb_brnn_param_count floats
  * rounded up to 256 bytes.  No other offset moves, and the forward workspace does not grow. */
 size_t ctcb_brnn_workspace_bytes(const ctcb_brnn_config *cfg);
 /* Byte offset, inside the workspace, of a uint32 that the recurrent-sweep kernels set non-zero when an
@@ -436,6 +441,39 @@ int ctcb_brnn_set_input_masks(ctcb_brnn *h, int freqMasks, int freqWidth, int ti
 int ctcb_input_mask_f32(const float *feats, const int32_t *T_per_utt, int B, int Tmax, int inputDim, int featDim,
                         int freqMasks, int freqWidth, int timeMasks, int timeWidth, double timeRatio, uint64_t seed,
                         const int64_t *step, int64_t first, int64_t stride, float *out, void *stream);
+
+/* ---- Gaussian weight noise (Graves, Mohamed & Hinton, ICASSP 2013; Graves & Jaitly, ICML 2014) -----------------------
+ * Noised tensors: the ones L2 regularisation sees, the even tensors 0 .. nreg - 1 of the flat vector -- W of every
+ * affine map and every recurrent matrix (the clipped-ReLU Wtf / Wtb / Wt, the LSTM U).  Biases, the dummies, the
+ * layer-norm [gamma, beta] and the peephole P are used as they are.
+ * Draw: at optimisation step s, element e of a noised matrix (e its offset in the flat vector; every tensor is 16-byte
+ * aligned, so the quad q = e / 4 never straddles two tensors), j = e % 4:
+ *     (r0, r1, r2, r3) = Philox4x32-10(counter = (s mod 2^32, q mod 2^32, 1, 0), key = (seed mod 2^32, seed >> 32))
+ *     (a, b) = (r0, r1) for j in {0, 1}, (r2, r3) for j in {2, 3}
+ *     u1 = (a + 1) 2^-32,  u2 = b 2^-32,  rho = sqrt(-2 ln u1)                 (float64)
+ *     z = rho cos(2 pi u2) for even j, rho sin(2 pi u2) for odd j              (float64)
+ *     w' = w + float32(sigma z)                                                (sigma z rounded once, a float32 add)
+ * Every other element, the alignment gaps included, is copied bit for bit.  The three draws of a seed never meet:
+ * dropout's fourth counter word is (layer << 24) | .. >= 2^24, SpecAugment's third word is 0, this rule's third word
+ * is 1 and its fourth 0.
+ * One draw per step: the noise does not depend on the utterance, the rank or the micro-batch, so a batch of B
+ * utterances shares one noisy net (at one utterance per step, the reference's schedule, that is noise per sequence).
+ *
+ * ctcb_brnn_set_weight_noise: with sigma > 0 every TRAINING call (grads != NULL) writes w' into its workspace (behind
+ * everything else, with weightNoise = 1) with one pass at the start of the main chain, and every stage that reads a
+ * weight reads that copy: the forward contractions, the recurrent sweeps, the delta contractions.  The gradient is
+ * that of the returned cost, evaluated at w'.  The L2 term (reg w in the gradient, reg/2 |w|^2 in regcost) and the
+ * data-parallel exchange see the CLEAN params, and params is never written, so an update applies to the clean w (with
+ * Nesterov the noise sits on the look-ahead point the caller passes).  Every training call forms the copy from params,
+ * so the micro-batches of one step see the same bits.  step is the int64 DEVICE counter of ctcb_dropout_advance, read
+ * when the pass runs.  Forward-only calls (grads == NULL) never add noise.  sigma = 0 (the default) disables it: the
+ * call reads params and issues exactly the launches it does without.  CTCB_EINVAL for sigma negative, NaN or
+ * infinite, sigma > 0 on a config with weightNoise = 0, or sigma > 0 with a null step.  Host-only: no device work. */
+int ctcb_brnn_set_weight_noise(ctcb_brnn *h, float sigma, uint64_t seed, const int64_t *step);
+/* The pass on its own, with the launch a training call makes under the handle's settings: out = params with the
+ * noise of the current step (ctcb_brnn_param_count floats each; out must not overlap params).  With sigma = 0 it
+ * copies.  16-byte accesses where both are 16-byte aligned, else 4-byte ones. */
+int ctcb_brnn_weight_noise_f32(ctcb_brnn *h, const float *params, float *out, void *stream);
 
 /* ---- layer normalisation on its own (layerNorm = 1, above) -----------------------------------------------------
  * Rows are [R][H] fp32, 1 <= H <= CTCB_LAYERNORM_MAX_H; with H % 4 == 0 every pointer must be 16-byte aligned.

@@ -30,7 +30,8 @@ class BrnnConfig(ctypes.Structure):
                 ("maxB", ctypes.c_int32), ("maxLabels", ctypes.c_int32), ("reg", ctypes.c_float),
                 ("maxAct", ctypes.c_float), ("unidirectional", ctypes.c_int32), ("numTemporal", ctypes.c_int32),
                 ("cell", ctypes.c_int32), ("layerNorm", ctypes.c_int32), ("subsample", ctypes.c_int32),
-                ("subsampleLayer", ctypes.c_int32), ("peephole", ctypes.c_int32), ("maskFeatDim", ctypes.c_int32)]
+                ("subsampleLayer", ctypes.c_int32), ("peephole", ctypes.c_int32), ("maskFeatDim", ctypes.c_int32),
+                ("weightNoise", ctypes.c_int32)]
 
 
 _PROTOS = {
@@ -106,6 +107,8 @@ _PROTOS = {
     "ctcb_brnn_set_input_masks": (c_int, [c_vp, c_int, c_int, c_int, c_int, ctypes.c_double, ctypes.c_uint64, c_vp]),
     "ctcb_input_mask_f32": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, ctypes.c_double,
                                     ctypes.c_uint64, c_vp, c_i64, c_i64, c_vp, c_vp]),
+    "ctcb_brnn_set_weight_noise": (c_int, [c_vp, c_f32, ctypes.c_uint64, c_vp]),
+    "ctcb_brnn_weight_noise_f32": (c_int, [c_vp, c_vp, c_vp, c_vp]),
     "ctcb_comm_get_unique_id": (c_int, [c_vp]),
     "ctcb_comm_create": (c_int, [c_vp, c_int, c_int, ctypes.POINTER(c_vp)]),
     "ctcb_comm_destroy": (None, [c_vp]),

@@ -36,6 +36,8 @@ const char *input_mask_policy_error(int nu, int mF, int F, int mT, int Tw, doubl
 int run_input_mask(const float *x, const int32_t *lens, int B, int Tmax, int D, int nu, int mF, int F, int mT, int Tw,
                    double p, uint64_t seed, const int64_t *step, int64_t first, int64_t stride, float *y,
                    cudaStream_t st);
+int run_weight_noise(const float *w, float *y, int64_t n, const int64_t *lo, const int64_t *hi, int nr, float sigma,
+                     uint64_t seed, const int64_t *step, cudaStream_t st);
 size_t lstm_carry_bytes(int H, int B);
 int run_lstm_sweep(int mode, int T, int B, int H, const int32_t *Tlen, float *gates, const float *Uf, const float *Ub,
                    const float *Pf, const float *Pb, float *hF, float *hB, float *cF, float *cB, const float *dh,
@@ -261,6 +263,8 @@ static const char *cfg_error(const ctcb_brnn_config *c, char (&buf)[192]) {
         char why[192];
         if (const char *e = input_mask_layout_error(c->inputDim, c->maskFeatDim, why)) return say("maskFeatDim: %s", e);
     }
+    if (c->weightNoise != 0 && c->weightNoise != 1)
+        return say("weightNoise %d is neither 0 (off) nor 1 (reserve the noisy copy of the parameters)", c->weightNoise);
     const bool ok = c->inputDim > 0 && c->outputDim > 1 && c->layerSize > 0 && c->numLayers >= 1 && c->numLayers <= 64 &&
                     c->maxT > 0 && c->maxB > 0 && c->maxLabels >= 0 && c->numTemporal >= 0 &&
                     // a stacked block must lie inside the hidden layers; k <= 1 keeps the silent "no temporal layer" rule below
@@ -459,6 +463,7 @@ struct WsLayout {
     size_t S, dS, lens;
     size_t peep_part;   // peephole nets only (0 elsewhere): the partial sums of the peephole weight gradients
     size_t masked;      // maskFeatDim > 0 only (0 elsewhere): the masked copy of the call's features
+    size_t noisy;       // weightNoise = 1 only (0 elsewhere): the noisy copy of the parameters
     size_t total;
 };
 
@@ -549,6 +554,8 @@ WsLayout ws_layout(const ctcb_brnn_config *c) {
         w.peep_part = take(off, lstm_peephole_grad_bytes((int64_t)max_rows(c, tl), H, uni ? 1 : 2));
     if (c->maskFeatDim > 0)     // read by map 1 (its contraction, the frame stacking, its weight gradient) all call long
         w.masked = take(off, (size_t)c->maxT * c->maxB * c->inputDim * sizeof(float));
+    if (c->weightNoise == 1)     // read by every stage that reads a weight, all call long
+        w.noisy = take(off, (size_t)ctcb_brnn_param_count(c) * sizeof(float));
     w.total = off;
     return w;
 }
@@ -722,6 +729,14 @@ struct ctcb_brnn {
     uint64_t mask_seed = 0;
     const int64_t *mask_step = nullptr;
     bool masks_on() const { return mask_f + mask_t > 0; }
+    // Gaussian weight noise in training calls (ctcb_brnn_set_weight_noise); noise_sigma == 0: off.  noise_lo / hi: the
+    // element ranges of the noised matrices, the even tensors below net.nreg.
+    float noise_sigma = 0.f;
+    uint64_t noise_seed = 0;
+    const int64_t *noise_step = nullptr;
+    int noise_n = 0;
+    int64_t noise_lo[(2 * 65 + 4 * 64) / 2], noise_hi[(2 * 65 + 4 * 64) / 2];
+    bool noise_on() const { return noise_sigma > 0.f; }
 
     bool uni() const { return cfg.unidirectional != 0; }
     bool lstm() const { return cfg.cell == 1; }
@@ -786,6 +801,11 @@ extern "C" int ctcb_brnn_create(const ctcb_brnn_config *cfg, ctcb_brnn **out) {
         }
     }
     net_table(cfg, &h->net);
+    for (int idx = 0; idx < h->net.nreg; idx += 2) {     // the matrices ctcb_brnn_apply_l2_f32 regularises
+        const NetTable::Tensor &t = h->net.t[idx];
+        h->noise_lo[h->noise_n] = t.off;
+        h->noise_hi[h->noise_n++] = t.off + (int64_t)t.rows * t.cols;
+    }
     *out = h;
     return CTCB_OK;
 }
@@ -936,13 +956,14 @@ namespace {
 // workspace `ws` for what only the backward half uses, the call's arguments.  `main` carries the forward pass, the
 // CTC, the delta chain and the sweeps, `side` the weight gradients of the layers at and above the lowest temporal
 // layer; `caller` is the stream the call was given, which `main` is forked from and both are joined into.  Without a
-// temporal layer main == caller and there is no side stream.
+// temporal layer main == caller and there is no side stream.  `params` is what every stage reads (the noisy copy with
+// weight noise on), `clean` the caller's vector, which only the L2 term reads.
 struct Step {
     ctcb_brnn *h;
     const FwdBufs &m;
     const WsLayout &w;
     char *ws;
-    const float *feats, *params;
+    const float *feats, *params, *clean;
     const int32_t *T_per_utt;
     float *grads;
     int B, Tmax;            // Tmax of the input; map i runs on T(i) frames
@@ -1135,11 +1156,11 @@ int Step::finish(float *stats, float *regcost_out) const {
         set_scalar_kernel<<<1, 1, 0, caller>>>(regcost_out, 0.f);
         CTCB_LAUNCH_CHECK();
     }
-    if (!h->defer_l2) TRY(ctcb_brnn_apply_l2_f32(h, params, grads, caller));
+    if (!h->defer_l2) TRY(ctcb_brnn_apply_l2_f32(h, clean, grads, caller));
     if (regcost_out && reg > 0.f)
         for (int idx = 0; idx < h->net.nreg; idx += 2) {     // the same weight matrices
             const NetTable::Tensor &t = h->net.t[idx];
-            TRY(run_sumsq(params + t.off, (int64_t)t.rows * t.cols, regcost_out, 0.5f * reg, 1, ws + w.l2_scratch, caller));
+            TRY(run_sumsq(clean + t.off, (int64_t)t.rows * t.cols, regcost_out, 0.5f * reg, 1, ws + w.l2_scratch, caller));
         }
     return CTCB_OK;
 }
@@ -1192,7 +1213,9 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
     const bool dp = (h->comm != nullptr) && comm_world(h->comm) > 1;
     // with input masks on, every stage of the call reads the masked copy in place of feats, which it never writes
     const float *in = h->masks_on() ? (const float *)(ws + w.masked) : feats;
-    Step s{h, m, w, ws, in, params, T_per_utt, grads, B, Tmax, first, last, h->drop_p > 0.f, dp,
+    // with weight noise on, every stage reads the noisy copy in place of params; the L2 term reads params
+    const float *wts = h->noise_on() ? (const float *)(ws + w.noisy) : params;
+    Step s{h, m, w, ws, in, wts, params, T_per_utt, grads, B, Tmax, first, last, h->drop_p > 0.f, dp,
            caller, nullptr, caller};
     const bool overlap = (h->tl > 0);
     if (overlap) {     // fork: the main chain runs on h->hi until the join below
@@ -1209,7 +1232,12 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
                            h->mask_tw, h->mask_p, h->mask_seed, h->mask_step, h->drop_first, h->drop_stride,
                            (float *)(ws + w.masked), s.main));
     }
-    TRY(brnn_forward(h, in, T_per_utt, B, Tmax, params, probs_out, m, s.drop, s.main));
+    if (h->noise_on()) {     // the side stream reads no weight; it meets main only behind events recorded after this
+        ProfScope ps("weight_noise", s.main);
+        TRY(run_weight_noise(params, (float *)(ws + w.noisy), h->net.params, h->noise_lo, h->noise_hi, h->noise_n,
+                             h->noise_sigma, h->noise_seed, h->noise_step, s.main));
+    }
+    TRY(brnn_forward(h, in, T_per_utt, B, Tmax, wts, probs_out, m, s.drop, s.main));
     {     // brnnet.py:161-175
     ProfScope ps("ctc", s.main);
     TRY(ctcb_ctc_loss_grad_f32(m.X[N + 1], 0, (int64_t)K, (int64_t)B * K, labels, label_off, s.lens(N + 1), B, s.T(N + 1), K,
@@ -1311,6 +1339,35 @@ extern "C" int ctcb_brnn_set_input_masks(ctcb_brnn *h, int freqMasks, int freqWi
     h->mask_seed = seed;
     h->mask_step = step;
     return CTCB_OK;
+}
+
+extern "C" int ctcb_brnn_set_weight_noise(ctcb_brnn *h, float sigma, uint64_t seed, const int64_t *step) {
+    if (!h) return set_error(CTCB_EINVAL, "ctcb_brnn_set_weight_noise: null handle");
+    if (!(sigma >= 0.f && sigma <= 3.4028235e38f))
+        return set_error(CTCB_EINVAL, "ctcb_brnn_set_weight_noise: sigma = %g is not a finite value >= 0", (double)sigma);
+    if (sigma > 0.f && h->cfg.weightNoise != 1)
+        return set_error(CTCB_EINVAL, "ctcb_brnn_set_weight_noise: sigma = %g needs the noisy copy (weightNoise = 1 in "
+                         "the config)", (double)sigma);
+    if (sigma > 0.f && !step)
+        return set_error(CTCB_EINVAL, "ctcb_brnn_set_weight_noise: sigma = %g needs a step counter", (double)sigma);
+    h->noise_sigma = sigma;
+    h->noise_seed = seed;
+    h->noise_step = step;
+    return CTCB_OK;
+}
+
+extern "C" int ctcb_brnn_weight_noise_f32(ctcb_brnn *h, const float *params, float *out, void *stream) {
+    if (!h || !params || !out) return set_error(CTCB_EINVAL, "ctcb_brnn_weight_noise_f32: null pointer argument");
+    const int64_t n = h->net.params;
+    if (params < out + n && out < params + n)
+        return set_error(CTCB_EINVAL, "ctcb_brnn_weight_noise_f32: out overlaps params");
+    if (!h->noise_on()) {
+        CTCB_CUDA_CHECK(cudaMemcpyAsync(out, params, (size_t)n * sizeof(float), cudaMemcpyDeviceToDevice,
+                                        (cudaStream_t)stream));
+        return CTCB_OK;
+    }
+    return run_weight_noise(params, out, n, h->noise_lo, h->noise_hi, h->noise_n, h->noise_sigma, h->noise_seed,
+                            h->noise_step, (cudaStream_t)stream);
 }
 
 extern "C" size_t ctcb_brnn_sweep_workspace_bytes(int H, int B) { return 4096 + ctcb::sweep_tc_workspace_bytes(H, B); }

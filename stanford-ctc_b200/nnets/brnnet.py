@@ -38,6 +38,10 @@ single contiguous vector.  New, additive surface for the minibatch/data-parallel
                                                 filter-bank bins of each spliced frame slot and spans of raw frames,
                                                 drawn from (seed dropoutSeed, the counter dropoutStep, the utterance's
                                                 index in the step's minibatch); featDim=None is inputDim (no splicing)
+    NNet(..., weightNoise=sigma)             Gaussian noise of standard deviation sigma on the weight matrices of
+                                                training calls (include/ctcb200.h: ctcb_brnn_set_weight_noise): one
+                                                draw per step from (seed dropoutSeed, the counter dropoutStep, the
+                                                element's offset); the L2 term and the update see the clean weights
     costAndGradBatch(datas, labelss)         -> (costs[B], grad, skips[B])   host arrays in; more than maxUtts
                                                 utterances are accumulated over micro-batches
     costAndGradDevice(batch, first, last)    -> no host sync; see DeviceBatch
@@ -164,7 +168,8 @@ class NNet:
                  train=True, temporalLayer=-1, reg=0.0, maxUtts=1, maxLabels=None,
                  allowTopTemporal=False, device=None, unidirectional=False, numTemporal=1, dropout=0.0,
                  dropoutSeed=33, cell="relu", layerNorm=False, subsample=1, subsampleLayer=1, peephole=False,
-                 freqMasks=0, freqMaskWidth=0, timeMasks=0, timeMaskWidth=0, timeMaskRatio=1.0, featDim=None):
+                 freqMasks=0, freqMaskWidth=0, timeMasks=0, timeMaskWidth=0, timeMaskRatio=1.0, featDim=None,
+                 weightNoise=0.0):
         torch = _ctcb.require_cuda()
         self._torch = torch
         self.dev = torch.device("cuda", torch.cuda.current_device() if device is None else device)
@@ -224,25 +229,32 @@ class NNet:
             raise ValueError("featDim=%r is the layout of the input masks; it needs freqMasks or timeMasks > 0"
                              % (featDim,))
         self.featDim = (inputDim if featDim is None else int(featDim)) if self.inputMasks else None
+        # Gaussian weight noise (include/ctcb200.h: ctcb_brnn_set_weight_noise).  Only a net with sigma > 0 reserves
+        # the noisy copy of the parameters, so a net without noise keeps today's workspace.
+        self.weightNoise = float(weightNoise)
+        if not (np.isfinite(self.weightNoise) and self.weightNoise >= 0.0):
+            raise ValueError("weightNoise=%r must be a finite standard deviation >= 0" % (weightNoise,))
         self._cfg = BrnnConfig(inputDim, outputDim, layerSize, numLayers, max(self.temporalLayer, 0), maxBatch,
                                maxUtts, self.maxLabels, float(reg), float(self.maxAct), int(self.unidirectional),
                                self.numTemporal, _ctcb.CELLS[cell], int(self.layerNorm), self.subsample,
-                               self.subsampleLayer, int(self.peephole), self.featDim or 0)
+                               self.subsampleLayer, int(self.peephole), self.featDim or 0,
+                               int(self.weightNoise > 0.0))
         self._h = ctypes.c_void_p()
         check(lib.ctcb_brnn_create(ctypes.byref(self._cfg), ctypes.byref(self._h)))
         self.stack = None
         self.grad = None
-        # Inverted dropout (include/ctcb200.h: ctcb_brnn_set_dropout) and the input masks.  The step counter lives on the
-        # device, so a CUDA graph of an SGD step reads its current value at every replay; sgd.SGD advances it once per
-        # step.  The net owns it when either is on.  dropoutShard = (rank, world) places this process's utterances in
-        # the step's minibatch for both (None: from torch.distributed).
+        # Inverted dropout (include/ctcb200.h: ctcb_brnn_set_dropout), the input masks and the weight noise.  The step
+        # counter lives on the device, so a CUDA graph of an SGD step reads its current value at every replay; sgd.SGD
+        # advances it once per step.  The net owns it when any of them is on.  dropoutShard = (rank, world) places
+        # this process's utterances in the step's minibatch for dropout and the masks (None: from torch.distributed).
+        # The weight noise is one draw per step, the same on every rank.
         self.dropout = float(dropout)
         self.dropoutSeed = int(dropoutSeed)
         self.dropoutStep = None
         self.dropoutShard = None
         if self.dropout != 0.0 and not 0.0 < self.dropout < 1.0:
             raise ValueError("dropout=%r must be in [0, 1)" % (dropout,))
-        if self.dropout != 0.0 or self.inputMasks:
+        if self.dropout != 0.0 or self.inputMasks or self.weightNoise > 0.0:
             self.dropoutStep = torch.zeros(1, dtype=torch.int64, device=self.dev)
         seed = self.dropoutSeed & 0xFFFFFFFFFFFFFFFF
         if self.dropout != 0.0:
@@ -250,6 +262,8 @@ class NNet:
         # called with counts 0 too, so that every value outside the limits is refused with the library's message
         check(lib.ctcb_brnn_set_input_masks(self._h, self.freqMasks, self.freqMaskWidth, self.timeMasks,
                                             self.timeMaskWidth, self.timeMaskRatio, seed, ptr(self.dropoutStep)))
+        if self.weightNoise > 0.0:
+            check(lib.ctcb_brnn_set_weight_noise(self._h, self.weightNoise, seed, ptr(self.dropoutStep)))
 
     def __del__(self):
         h = getattr(self, "_h", None)
@@ -587,7 +601,8 @@ class NNet:
     def check_grad(self, data, labels, epsilon=1e-3, maxChecks=10, verbose=True):
         """Finite-difference check on a small section of every weight matrix (brnnet.py:279-297).
         Returns the list of (analytic, numeric) pairs it printed.  costAndGrad never advances the dropout counter,
-        so every evaluation sees the same dropout and input masks."""
+        so every evaluation sees the same dropout and input masks and the same weight noise (which does not depend on
+        the weights' values)."""
         cost, grad, _ = self.costAndGrad(data, labels)
         out = []
         ana = [dw.clone() for dw, _ in grad]

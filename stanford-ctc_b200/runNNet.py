@@ -8,7 +8,8 @@ last_cost, sentinel, train.log), resume through --cfg_file with the step size re
 The implementation is organised differently: a declarative flag table, one RunDir helper that owns the
 side files, and separate train/evaluate phases.  Site paths of run_cfg.py / decoder_config.py became
 flags (--runDir, --outDir); new flags: --numTemporal, --cell, --peephole, --layerNorm, --subsample, --subsampleLayer, --batchSize, --maxUtts, --maxLabels,
---dropout, --freqMasks, --freqMaskWidth, --timeMasks, --timeMaskWidth, --timeMaskRatio, --featDim, --optimizer,
+--dropout, --freqMasks, --freqMaskWidth, --timeMasks, --timeMaskWidth, --timeMaskRatio, --featDim, --weightNoise,
+--optimizer,
 --beta1, --beta2, --epsilon, --quiet.  Under torchrun the same
 script trains data-parallel (one process per GPU, one NCCL all-reduce per step).
 """
@@ -73,6 +74,9 @@ FLAGS = [
     ("timeMaskRatio", float, 1.0, "a time mask covers at most this fraction of the utterance's frames"),
     ("featDim", int, None, "filter-bank bins per frame slot of the spliced input (e.g. 41 for --inputDim 41*15); "
                            "default --inputDim, features without splicing"),
+    ("weightNoise", float, 0.0, "standard deviation of the Gaussian noise added to the weight matrices while training, "
+                                "one draw per step (0 = off; --test never adds noise; a cfg.json written without it "
+                                "has none)"),
     ("optimizer", str, "nesterov", "update rule: nesterov (the reference's, with --momentum), adagrad or adam; --step "
                                    "is the step size of each and --anneal applies to it"),
     ("beta1", float, 0.9, "adam: decay of the first-moment estimate"),
@@ -221,7 +225,7 @@ def _train(opts, cfg, run_dir, log, rank, world):
                      layerNorm=opts.layerNorm, subsample=opts.subsample, subsampleLayer=opts.subsampleLayer,
                      peephole=opts.peephole, freqMasks=opts.freqMasks, freqMaskWidth=opts.freqMaskWidth,
                      timeMasks=opts.timeMasks, timeMaskWidth=opts.timeMaskWidth, timeMaskRatio=opts.timeMaskRatio,
-                     featDim=opts.featDim)
+                     featDim=opts.featDim, weightNoise=opts.weightNoise)
     net.initParams()
     optimizer = sgd.SGD(net, opts.maxUttLen, alpha=opts.step, optimizer=opts.optimizer, momentum=opts.momentum,
                         batchSize=opts.batchSize, verbose=(rank == 0 and not opts.quiet), beta1=opts.beta1,
