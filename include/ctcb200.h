@@ -199,6 +199,9 @@ typedef struct ctcb_brnn_config {
     int32_t weightNoise;   /* 0: off (so an initialiser without this member keeps its meaning); 1: reserves the noisy copy
                             * of the parameters for the Gaussian weight noise of ctcb_brnn_set_weight_noise (below) in
                             * the training workspace; any other value makes the config invalid. */
+    int32_t zoneout;       /* 0: off (so an initialiser without this member keeps its meaning); 1: zoneout of the LSTM
+                            * cell's state (below) with the probabilities of ctcb_brnn_set_zoneout, which needs cell = 1;
+                            * any other value, or 1 with cell = 0, makes the config invalid. */
 } ctcb_brnn_config;
 
 /* Frame subsampling (subsample = k >= 2; not in the reference; cf. Deep Speech 2's striding and the frame stacking of
@@ -261,6 +264,36 @@ typedef struct ctcb_brnn_config {
  * [gamma, beta] pairs included), so no other offset and not the early all-reduce range moves; the peephole gradients
  * travel with the exchange at the end of the step.  P is not L2-regularised; the dummies get a zero gradient. */
 
+/* Zoneout (zoneout = 1 with cell = 1; not in the reference; Krueger et al., ICLR 2017).  For each LSTM temporal layer i
+ * (its hidden-layer index, 1..numLayers) and direction d (0 forward in time, 1 backward), time in the direction's own
+ * order (the backward direction mirrored, as above), frames at the layer's own rate, and the two probabilities z_c, z_h
+ * in [0, 1) of ctcb_brnn_set_zoneout:
+ *     c~_t = f_t c_{t-1} + i_t g_t;   c_t = lambda_c,t c_{t-1} + (1 - lambda_c,t) c~_t
+ *     h~_t = o_t tanh(c_t);           h_t = lambda_h,t h_{t-1} + (1 - lambda_h,t) h~_t
+ *   c and h are 0 before the first frame and at every frame t >= T_u, as without zoneout; with peepholes i and f see
+ *   the zoned c_{t-1} and o the zoned c_t.  The layer's output is h_f + h_b (uni-directional h_f) of the zoned h, and
+ *   the c buffers hold the zoned c.
+ * Training calls (grads != NULL) draw lambda in {0, 1} for unit j of frame t of minibatch utterance g (as
+ * ctcb_brnn_set_dropout_utts places it; t the frame index 0..T-1 at the layer's rate, in either direction) at step s:
+ *     (r0, r1, r2, r3) = Philox4x32-10(counter = (s mod 2^32, g mod 2^32, t, (i << 24) | (d << 23) | j),
+ *                                      key = (seed mod 2^32, seed >> 32))
+ *     lambda_c = 1 iff r0 < floor(z_c 2^32),  lambda_h = 1 iff r1 < floor(z_h 2^32)     (the products in float64)
+ *   and lambda = 1 is a select: the kept value has exactly the bytes of c_{t-1} or h_{t-1}.  The counter never meets
+ *   the other draws of a seed: dropout's fourth word carries a non-temporal layer's index in its top 8 bits, this
+ *   rule's a temporal one's; SpecAugment's fourth word is < 2^24 and this rule's >= 2^24 (i >= 1); weight noise's
+ *   fourth word is 0.
+ * Forward-only calls (grads == NULL) use the expectation, lambda_c = z_c and lambda_h = z_h in float32:
+ *   c_t = fmaf(z_c, c_{t-1}, (1 - z_c) c~_t), h_t likewise.  So with a probability > 0 a forward-only call's probs_out
+ *   is not a training call's (ctcb_brnn_forward_workspace_bytes); at z_c = z_h = 0 nothing changes.
+ * BPTT (training calls; "next" = t + 1 in the direction's order):
+ *     dh_t  = delta_t + U^T dz_next + lambda_h,next dh_next;   dh~_t = (1 - lambda_h,t) dh_t
+ *     dz_o  = dh~_t tanh(c_t) o(1-o)
+ *     dc_t  = dh~_t o (1 - tanh^2 c_t) [+ p_o dz_o] + (lambda_c,next + (1 - lambda_c,next) f_next) dc_next
+ *             [+ p_i dz_i,next + p_f dz_f,next];   dc~_t = (1 - lambda_c,t) dc_t
+ *     dz_i = dc~_t g i(1-i);  dz_f = dc~_t c_{t-1} f(1-f);  dz_g = dc~_t i(1-g^2)
+ *   dU, dW, db, delta_{i-1} and dP are unchanged and read the zoned h and c.  At lambda = 0 every formula is the cell
+ *   above.  No tensor is added and the flat vector does not change. */
+
 typedef struct ctcb_brnn ctcb_brnn; /* opaque; owns no device memory */
 
 /* Flat parameter vector layout: the reference's `stack` order (brnnet.py:38-41,66-72):
@@ -271,7 +304,7 @@ typedef struct ctcb_brnn ctcb_brnn; /* opaque; owns no device memory */
  * layerNorm = 1 appends [gamma_i, beta_i] of every normalised hidden layer i, in ascending i.
  * peephole = 1 then appends [P_f,j, dummy] [P_b,j, dummy] (unidirectional: [P_j, dummy]) of every temporal layer j in
  * ascending order, each P 3 x H. */
-/* maskFeatDim = nu > 0 adds no parameter, and neither does weightNoise = 1. */
+/* maskFeatDim = nu > 0 adds no parameter, and neither do weightNoise = 1 and zoneout = 1. */
 int64_t ctcb_brnn_param_count(const ctcb_brnn_config *cfg);
 int ctcb_brnn_num_tensors(const ctcb_brnn_config *cfg);                    /* 2 * len(stack) */
 int ctcb_brnn_tensor_info(const ctcb_brnn_config *cfg, int idx, int64_t *offset, int32_t *rows, int32_t *cols);
@@ -297,7 +330,9 @@ int ctcb_brnn_tensor_info(const ctcb_brnn_config *cfg, int idx, int64_t *offset,
  * maskFeatDim = nu > 0 appends, behind everything else, the masked copy of a call's features: maxT*maxB*inputDim floats
  * rounded up to 256 bytes.  No other offset moves, and the forward workspace does not grow.
  * weightNoise = 1 appends, behind everything else, the noisy copy of the parameters: ctcb_brnn_param_count floats
- * rounded up to 256 bytes.  No other offset moves, and the forward workspace does not grow. */
+ * rounded up to 256 bytes.  No other offset moves, and the forward workspace does not grow.
+ * zoneout = 1 (with a temporal layer) appends, behind everything else, the BPTT sweep's dh carry: 2*maxB*layerSize
+ * floats rounded up to 256 bytes.  No other offset moves, and the forward workspace does not grow. */
 size_t ctcb_brnn_workspace_bytes(const ctcb_brnn_config *cfg);
 /* Byte offset, inside the workspace, of a uint32 that the recurrent-sweep kernels set non-zero when an
  * inter-CTA wait timed out (results are then invalid; never a hang).  Callers that synchronise anyway
@@ -310,7 +345,8 @@ size_t ctcb_brnn_error_flag_offset(const ctcb_brnn_config *cfg);
  * byte offset of the sweep error flag inside it (same meaning as ctcb_brnn_error_flag_offset).  0 for an invalid
  * config.  A forward-only call always uses this layout, in any workspace of at least this size (the training size
  * included), and launches the same kernels with the same plans as a training call of the same B and Tmax, so its
- * probs_out is bit-identical to that call's. */
+ * probs_out is bit-identical to that call's -- except under zoneout probabilities > 0, where a forward-only call runs
+ * the expectation cell and a training call the drawn masks (zoneout, above). */
 size_t ctcb_brnn_forward_workspace_bytes(const ctcb_brnn_config *cfg, size_t *error_flag_offset);
 
 /* Diagnostic hook (used by the parity tests): byte offset inside the workspace of the activations the LAST
@@ -475,6 +511,16 @@ int ctcb_brnn_set_weight_noise(ctcb_brnn *h, float sigma, uint64_t seed, const i
  * copies.  16-byte accesses where both are 16-byte aligned, else 4-byte ones. */
 int ctcb_brnn_weight_noise_f32(ctcb_brnn *h, const float *params, float *out, void *stream);
 
+/* ---- zoneout of the LSTM cell's state (zoneout = 1, above) ----------------------------------------------------------
+ * ctcb_brnn_set_zoneout: zc and zh are the probabilities z_c and z_h of every LSTM layer; training calls draw the masks
+ * with seed and the int64 DEVICE counter step (ctcb_dropout_advance's), read when each sweep runs, so the micro-batches
+ * of one step, its shards (ctcb_brnn_set_dropout_utts) and a replayed graph draw the same masks.  Forward-only calls use
+ * the expectation.  zc = zh = 0 (the default) disables it: every call issues exactly the launches and bits it does
+ * without.  CTCB_EINVAL for a value outside [0, 1) (NaN included), or a value > 0 on a config with zoneout = 0.  step
+ * may be NULL for forward-only use; a training call with a value > 0 and a NULL step then returns CTCB_EINVAL before it
+ * launches anything.  Host-only: no device work. */
+int ctcb_brnn_set_zoneout(ctcb_brnn *h, float zc, float zh, uint64_t seed, const int64_t *step);
+
 /* ---- layer normalisation on its own (layerNorm = 1, above) -----------------------------------------------------
  * Rows are [R][H] fp32, 1 <= H <= CTCB_LAYERNORM_MAX_H; with H % 4 == 0 every pointer must be 16-byte aligned.
  * forward : y = relu(gamma (z - mu) rstd + beta) per row; y may alias z; mu / rstd (R floats each) receive the row
@@ -549,6 +595,17 @@ int ctcb_lstm_sweep_f32(int mode, int T, int B, int H, const int32_t *T_per_utt,
 int ctcb_lstm_sweep_peephole_f32(int mode, int T, int B, int H, const int32_t *T_per_utt, float *gates, const float *Uf,
                                  const float *Ub, const float *Pf, const float *Pb, float *hF, float *hB, float *cF,
                                  float *cB, const float *dh, float *dz, void *scratch, size_t scratch_bytes, void *stream);
+/* The same with zoneout (zoneout = 1, above), with peephole connections when Pf != NULL.  train != 0 draws the masks of
+ * (seed, *step, g = first + stride * b, t, layer, direction, j), train == 0 uses the expectation; mode 1 runs the BPTT
+ * above with those lambdas (with train == 0, lambda = z).  hF / hB are read in mode 0 (h_{t-1}).  The BPTT carries
+ * lambda_h dh in a second [ndir][B][H] area: scratch is ctcb_lstm_sweep_zoneout_workspace_bytes(H, B) bytes.
+ * CTCB_EINVAL for zc or zh outside [0, 1), train with a NULL step, first < 0, stride < 1 or layer outside 1..255. */
+size_t ctcb_lstm_sweep_zoneout_workspace_bytes(int H, int B);
+int ctcb_lstm_sweep_zoneout_f32(int mode, int T, int B, int H, const int32_t *T_per_utt, float *gates, const float *Uf,
+                                const float *Ub, const float *Pf, const float *Pb, float *hF, float *hB, float *cF,
+                                float *cB, const float *dh, float *dz, float zc, float zh, int train, uint64_t seed,
+                                const int64_t *step, int64_t first, int64_t stride, int layer, void *scratch,
+                                size_t scratch_bytes, void *stream);
 /* The peephole weight gradients of one LSTM layer: dz [T][B][G] as mode 1 of the sweep wrote it, cF / cB [T][B][H] as
  * mode 0 did (cB == NULL: one direction, G = 4H, dPb ignored); dPf / dPb [3][H] receive dp_i, dp_f, dp_o, or with
  * accumulate != 0 have them added.  workspace: ctcb_lstm_peephole_grad_workspace_bytes(T, B, H, ndir) bytes of partial
@@ -562,6 +619,8 @@ int ctcb_lstm_peephole_grad_f32(int T, int B, int H, const float *dz, const floa
  * last partitions may get fewer, or none)}; or the error the sweep call and ctcb_brnn_create return for a width, or a
  * forced partition count, the device cannot hold. */
 int ctcb_debug_lstm_plan(int H, int B, int ndir, int peephole, int32_t *out);
+/* The same for the zoneout kernels (ctcb_lstm_sweep_zoneout_f32), whose occupancy is their own. */
+int ctcb_debug_lstm_zoneout_plan(int H, int B, int ndir, int peephole, int32_t *out);
 /* 1 when the recurrences of a (layerSize H, B utterances, bi-directional) step run on the tensor-core kernel. */
 int ctcb_sweep_uses_tensor_cores(int H, int B);
 /* The plan ctcb_brnn_sweep_f32 launches for (H, B, ndir = 2 bi-directional / 1 forward in time only) on the current

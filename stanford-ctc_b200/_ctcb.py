@@ -31,7 +31,7 @@ class BrnnConfig(ctypes.Structure):
                 ("maxAct", ctypes.c_float), ("unidirectional", ctypes.c_int32), ("numTemporal", ctypes.c_int32),
                 ("cell", ctypes.c_int32), ("layerNorm", ctypes.c_int32), ("subsample", ctypes.c_int32),
                 ("subsampleLayer", ctypes.c_int32), ("peephole", ctypes.c_int32), ("maskFeatDim", ctypes.c_int32),
-                ("weightNoise", ctypes.c_int32)]
+                ("weightNoise", ctypes.c_int32), ("zoneout", ctypes.c_int32)]
 
 
 _PROTOS = {
@@ -88,6 +88,12 @@ _PROTOS = {
     "ctcb_lstm_peephole_grad_workspace_bytes": (c_sz, [c_int, c_int, c_int, c_int]),
     "ctcb_lstm_peephole_grad_f32": (c_int, [c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_sz, c_vp]),
     "ctcb_debug_lstm_plan": (c_int, [c_int, c_int, c_int, c_int, ctypes.POINTER(ctypes.c_int32)]),
+    "ctcb_debug_lstm_zoneout_plan": (c_int, [c_int, c_int, c_int, c_int, ctypes.POINTER(ctypes.c_int32)]),
+    "ctcb_lstm_sweep_zoneout_workspace_bytes": (c_sz, [c_int, c_int]),
+    "ctcb_lstm_sweep_zoneout_f32": (c_int, [c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                            c_vp, c_vp, c_vp, c_vp, c_f32, c_f32, c_int, ctypes.c_uint64, c_vp, c_i64,
+                                            c_i64, c_int, c_vp, c_sz, c_vp]),
+    "ctcb_brnn_set_zoneout": (c_int, [c_vp, c_f32, c_f32, ctypes.c_uint64, c_vp]),
     "ctcb_layernorm_workspace_bytes": (c_sz, [c_i64, c_int]),
     "ctcb_layernorm_forward_f32": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_int, c_vp]),
     "ctcb_layernorm_backward_f32": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_int, c_int, c_vp, c_sz,

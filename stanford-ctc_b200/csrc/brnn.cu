@@ -41,8 +41,8 @@ int run_weight_noise(const float *w, float *y, int64_t n, const int64_t *lo, con
 size_t lstm_carry_bytes(int H, int B);
 int run_lstm_sweep(int mode, int T, int B, int H, const int32_t *Tlen, float *gates, const float *Uf, const float *Ub,
                    const float *Pf, const float *Pb, float *hF, float *hB, float *cF, float *cB, const float *dh,
-                   float *dz, unsigned int *counters, float *dc, cudaStream_t st);
-int lstm_check(int H, int B, int ndir, bool peep);
+                   float *dz, unsigned int *counters, float *dc, const LstmZoneout *zo, cudaStream_t st);
+int lstm_check(int H, int B, int ndir, bool peep, bool zo);
 int sweep_check(int H, int B, int ndir);
 size_t lstm_peephole_grad_bytes(int64_t R, int H, int ndir);
 int run_lstm_peephole_grad(int T, int B, int H, const float *dz, const float *cF, const float *cB, float *dPf,
@@ -265,6 +265,10 @@ static const char *cfg_error(const ctcb_brnn_config *c, char (&buf)[192]) {
     }
     if (c->weightNoise != 0 && c->weightNoise != 1)
         return say("weightNoise %d is neither 0 (off) nor 1 (reserve the noisy copy of the parameters)", c->weightNoise);
+    if (c->zoneout != 0 && c->zoneout != 1)
+        return say("zoneout %d is neither 0 (off) nor 1 (zoneout of the LSTM cell's state)", c->zoneout);
+    if (c->zoneout == 1 && c->cell != 1)
+        return say("zoneout 1 needs the LSTM cell (cell 1); cell is %d", c->cell);
     const bool ok = c->inputDim > 0 && c->outputDim > 1 && c->layerSize > 0 && c->numLayers >= 1 && c->numLayers <= 64 &&
                     c->maxT > 0 && c->maxB > 0 && c->maxLabels >= 0 && c->numTemporal >= 0 &&
                     // a stacked block must lie inside the hidden layers; k <= 1 keeps the silent "no temporal layer" rule below
@@ -464,6 +468,7 @@ struct WsLayout {
     size_t peep_part;   // peephole nets only (0 elsewhere): the partial sums of the peephole weight gradients
     size_t masked;      // maskFeatDim > 0 only (0 elsewhere): the masked copy of the call's features
     size_t noisy;       // weightNoise = 1 only (0 elsewhere): the noisy copy of the parameters
+    size_t zo_dh;       // zoneout nets only (0 elsewhere): the BPTT sweep's dh carry
     size_t total;
 };
 
@@ -556,6 +561,8 @@ WsLayout ws_layout(const ctcb_brnn_config *c) {
         w.masked = take(off, (size_t)c->maxT * c->maxB * c->inputDim * sizeof(float));
     if (c->weightNoise == 1)     // read by every stage that reads a weight, all call long
         w.noisy = take(off, (size_t)ctcb_brnn_param_count(c) * sizeof(float));
+    if (c->zoneout == 1 && nt)
+        w.zo_dh = take(off, lstm_carry_bytes(H, c->maxB));
     w.total = off;
     return w;
 }
@@ -737,6 +744,15 @@ struct ctcb_brnn {
     int noise_n = 0;
     int64_t noise_lo[(2 * 65 + 4 * 64) / 2], noise_hi[(2 * 65 + 4 * 64) / 2];
     bool noise_on() const { return noise_sigma > 0.f; }
+    // zoneout of the LSTM layers (ctcb_brnn_set_zoneout); zo_c == zo_h == 0: off, the sweeps without it run
+    float zo_c = 0.f, zo_h = 0.f;
+    uint64_t zo_seed = 0;
+    const int64_t *zo_step = nullptr;
+    bool zo_on() const { return zo_c > 0.f || zo_h > 0.f; }
+    // the settings of temporal layer i's sweep: the masks in a training call, the expectation in a forward-only one
+    LstmZoneout zoneout(int i, bool train, float *dhc) const {
+        return LstmZoneout{zo_c, zo_h, train, zo_seed, zo_step, drop_first, drop_stride, i, dhc};
+    }
 
     bool uni() const { return cfg.unidirectional != 0; }
     bool lstm() const { return cfg.cell == 1; }
@@ -791,8 +807,11 @@ extern "C" int ctcb_brnn_create(const ctcb_brnn_config *cfg, ctcb_brnn **out) {
     h->nt = eff_nt(cfg);
     if (h->nt) {      // a width or batch whose sweep the device cannot hold co-resident
         const int ndir = cfg->unidirectional ? 1 : 2;
-        const int rc = cfg->cell == 1 ? lstm_check(cfg->layerSize, cfg->maxB, ndir, cfg->peephole == 1)
-                                      : sweep_check(cfg->layerSize, cfg->maxB, ndir);
+        // zoneout = 1: the zoneout kernels too, which run whenever a probability is > 0
+        int rc = cfg->cell == 1 ? lstm_check(cfg->layerSize, cfg->maxB, ndir, cfg->peephole == 1, false)
+                                : sweep_check(cfg->layerSize, cfg->maxB, ndir);
+        if (rc == CTCB_OK && cfg->zoneout == 1)
+            rc = lstm_check(cfg->layerSize, cfg->maxB, ndir, cfg->peephole == 1, true);
         if (rc != CTCB_OK) {
             char why[512];
             snprintf(why, sizeof(why), "%s", ctcb_last_error());
@@ -881,7 +900,8 @@ static int brnn_reduce_rest(ctcb_brnn *h, float *grads, float *stats, cudaStream
 // gradients and the ReLU mask of the delta contraction all read the dropped activations.
 // With subsampling, map L first stacks its input into S (and T'_u into m.lens); maps L and above run on Tmax' frames.
 static int brnn_forward(ctcb_brnn *h, const float *feats, const int32_t *T_per_utt, int B, int Tmax0,
-                        const float *params, float *probs_out, const FwdBufs &m, bool drop, cudaStream_t st) {
+                        const float *params, float *probs_out, const FwdBufs &m, bool train, bool drop,
+                        cudaStream_t st) {
     const ctcb_brnn_config &c = h->cfg;
     const int N = c.numLayers, H = c.layerSize, K = c.outputDim;
     const bool uni = h->uni();
@@ -923,11 +943,12 @@ static int brnn_forward(ctcb_brnn *h, const float *feats, const int32_t *T_per_u
             const int j = i - h->tl, iU = h->rec(j), iP = h->peep_idx(j);
             const float *Pf = h->peep() ? h->tensor(params, iP) : nullptr;
             const float *Pb = h->peep() && !uni ? h->tensor(params, iP + 2) : nullptr;
+            const LstmZoneout zo = h->zoneout(i, train, nullptr);
             {
             ProfScope ps("sweep_fwd", st);
             TRY(run_lstm_sweep(0, Tmax, B, H, Tlen, m.X[i], h->tensor(params, iU),
                                uni ? nullptr : h->tensor(params, iU + 2), Pf, Pb, m.For[j], m.Back[j], m.Cf[j], m.Cb[j],
-                               nullptr, nullptr, m.counters, (float *)m.sweep, st));
+                               nullptr, nullptr, m.counters, (float *)m.sweep, h->zo_on() ? &zo : nullptr, st));
             }
             if (!uni) {
                 ProfScope ps("elementwise", st);
@@ -1117,12 +1138,13 @@ int Step::backward() const {
         TRY(stall(main, STALL_MAIN));
         {
         ProfScope ps("sweep_bptt", main);
-        if (lstm)
+        if (lstm) {
+            const LstmZoneout zo = h->zoneout(i, true, buf(w.zo_dh));
             TRY(run_lstm_sweep(1, T(i), B, H, lens(i), m.X[i], P(iWtf), uni ? nullptr : P(iWtf + 2),
                                h->peep() ? P(h->peep_idx(j)) : nullptr,
                                h->peep() && !uni ? P(h->peep_idx(j) + 2) : nullptr, nullptr, nullptr, m.Cf[j], m.Cb[j],
-                               doth, buf(w.D[i]), m.counters, (float *)m.sweep, main));
-        else
+                               doth, buf(w.D[i]), m.counters, (float *)m.sweep, h->zo_on() ? &zo : nullptr, main));
+        } else
             TRY(run_sweep(1, T(i), B, H, lens(i), doth, P(iWtf), uni ? nullptr : P(iWtf + 2), buf(w.dFor[p]),
                           buf(w.dBack[p]), m.For[j], m.Back[j], h->cfg.maxAct, m.counters, m.sweep, m.sweep_bytes, main));
         }
@@ -1188,6 +1210,9 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
         return set_error(CTCB_EINVAL, "ctcb_brnn_cost_and_grad: training mode needs labels and cost/skip outputs");
     if (!train && !probs_out)
         return set_error(CTCB_EINVAL, "ctcb_brnn_cost_and_grad: forward-only mode needs probs_out");
+    if (train && h->zo_on() && !h->zo_step)
+        return set_error(CTCB_EINVAL, "ctcb_brnn_cost_and_grad: zoneout (zc = %g, zh = %g) in a training call needs a "
+                         "step counter (ctcb_brnn_set_zoneout)", (double)h->zo_c, (double)h->zo_h);
     const cudaStream_t caller = (cudaStream_t)stream;
     char *ws = (char *)workspace;
     const int N = c.numLayers, K = c.outputDim;
@@ -1202,7 +1227,7 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
             return set_error(CTCB_ENOMEM, "ctcb_brnn_cost_and_grad: workspace %zu < %zu bytes", ws_bytes, h->fwd.total);
         FwdBufs m{};
         fwd_bufs(h->fwd, N, h->nt, ws, &m);
-        return brnn_forward(h, feats, T_per_utt, B, Tmax, params, probs_out, m, false, caller);
+        return brnn_forward(h, feats, T_per_utt, B, Tmax, params, probs_out, m, false, false, caller);
     }
     // planned on every call: the contraction planners' overrides may change under a live handle (common.cuh)
     const WsLayout w = ws_layout(&c);
@@ -1237,7 +1262,7 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
         TRY(run_weight_noise(params, (float *)(ws + w.noisy), h->net.params, h->noise_lo, h->noise_hi, h->noise_n,
                              h->noise_sigma, h->noise_seed, h->noise_step, s.main));
     }
-    TRY(brnn_forward(h, in, T_per_utt, B, Tmax, wts, probs_out, m, s.drop, s.main));
+    TRY(brnn_forward(h, in, T_per_utt, B, Tmax, wts, probs_out, m, true, s.drop, s.main));
     {     // brnnet.py:161-175
     ProfScope ps("ctc", s.main);
     TRY(ctcb_ctc_loss_grad_f32(m.X[N + 1], 0, (int64_t)K, (int64_t)B * K, labels, label_off, s.lens(N + 1), B, s.T(N + 1), K,
@@ -1353,6 +1378,21 @@ extern "C" int ctcb_brnn_set_weight_noise(ctcb_brnn *h, float sigma, uint64_t se
     h->noise_sigma = sigma;
     h->noise_seed = seed;
     h->noise_step = step;
+    return CTCB_OK;
+}
+
+extern "C" int ctcb_brnn_set_zoneout(ctcb_brnn *h, float zc, float zh, uint64_t seed, const int64_t *step) {
+    if (!h) return set_error(CTCB_EINVAL, "ctcb_brnn_set_zoneout: null handle");
+    if (!(zc >= 0.f && zc < 1.f) || !(zh >= 0.f && zh < 1.f))
+        return set_error(CTCB_EINVAL, "ctcb_brnn_set_zoneout: zc = %g, zh = %g (need both in [0, 1))", (double)zc,
+                         (double)zh);
+    if ((zc > 0.f || zh > 0.f) && h->cfg.zoneout != 1)
+        return set_error(CTCB_EINVAL, "ctcb_brnn_set_zoneout: zc = %g, zh = %g need zoneout = 1 in the config",
+                         (double)zc, (double)zh);
+    h->zo_c = zc;
+    h->zo_h = zh;
+    h->zo_seed = seed;
+    h->zo_step = step;
     return CTCB_OK;
 }
 

@@ -109,4 +109,16 @@ void gemm_simt_plan(int M, int N, int K, const float *A, int64_t lda, const floa
 // Both contraction kernels put 128-row output tiles on gridDim.y (at most 65,535): the largest M they take.
 constexpr int GEMM_MAX_M = 128 * 65535;
 
+// The zoneout settings of one LSTM sweep launch (include/ctcb200.h: zoneout = 1); run_lstm_sweep (sweep_lstm.cu) takes
+// a null pointer for the cell without zoneout.
+struct LstmZoneout {
+    float zc, zh;
+    bool train;                // masks drawn from (seed, *step, g, t, layer, dir, j); else the expectation, lambda = z
+    uint64_t seed;
+    const int64_t *step;       // device counter, read by the kernel (training mode)
+    int64_t first, stride;     // utterance b of the call is minibatch utterance first + stride b
+    int layer;                 // hidden-layer index of the temporal layer, 1..255
+    float *dhc;                // BPTT: the [ndir][B][H] dh carry
+};
+
 }  // namespace ctcb

@@ -26,7 +26,16 @@
 // unit.  BPTT: dc = dh o (1 - tanh^2 c) + p_o dz_o + carry, and the scratch carries f dc + p_i dz_i + p_f dz_f of the
 // step just finished instead of dc.  The peephole weight gradients are a separate reduction over dz and c
 // (lstm_peephole_grad below).
+//
+// Zoneout mode (ZO, include/ctcb200.h: zoneout = 1), composed with either: after the cell update c_t and h_t each keep
+// the previous step's value where their mask says so (a select, so a kept value has the bytes of c_{t-1} / h_{t-1}),
+// or, in expectation mode, become the z-weighted blend.  The masks are one Philox block per (t, b, j), drawn by every
+// lane of the warp for its utterance ob, and are drawn again in BPTT rather than stored: the draw is a few dozen
+// integer instructions per step and lane, a stored mask would be a pass, a buffer and a load per step.  BPTT carries
+// lambda_h dh in a second [ndir][B][H] scratch and, as PEEP does, the whole dc_{t+1} term of dc_t in the first.
 #include "coop_sweep.cuh"
+#include <cmath>
+#include <curand_philox4x32_x.h>
 
 namespace ctcb {
 
@@ -52,14 +61,31 @@ struct LstmArgs {
 struct LstmPeepArgs : LstmArgs {
     const float *P[2];
 };
-template <bool PEEP> struct LstmArgsOf { using type = LstmArgs; };
-template <> struct LstmArgsOf<true> { using type = LstmPeepArgs; };
+// zoneout mode: the probabilities, the draw and the dh carry (P is null without peepholes)
+struct LstmZoArgs : LstmPeepArgs {
+    float *dhc;                // mode 1: [ndir][B][H] carry, lambda_h dh of the step just finished
+    int train;                 // 1: masks drawn from Philox; 0: the expectation, lambda = z
+    float zc, zh;              // expectation mode
+    uint32_t thr_c, thr_h;     // training mode: keep iff r < thr
+    uint2 key;
+    const int64_t *step;       // training mode: the device step counter
+    int64_t first, stride;     // utterance b of the call is minibatch utterance first + stride b
+    int layer;                 // the hidden-layer index of the temporal layer, 1..255
+};
+template <bool PEEP, bool ZO> struct LstmArgsOf { using type = LstmArgs; };
+template <> struct LstmArgsOf<true, false> { using type = LstmPeepArgs; };
+template <bool PEEP> struct LstmArgsOf<PEEP, true> { using type = LstmZoArgs; };
 
 __device__ __forceinline__ float lstm_sigmoid(float z) { return 1.f / (1.f + expf(-z)); }
 
+// zoneout of one state value: training mode selects prev where the mask keeps it, expectation mode blends with lambda = z
+__device__ __forceinline__ float zone(const LstmZoArgs &a, bool keep, float z, float prev, float cur) {
+    return a.train ? (keep ? prev : cur) : fmaf(z, prev, (1.f - z) * cur);
+}
+
 // KI > 0: H == 32 KI and U lives in registers (one CTA per SM).  KI == 0: any H, U re-read (two CTAs per SM).
-template <int KI, bool PEEP>
-__global__ void __launch_bounds__(COOP_THREADS, KI > 0 ? 1 : 2) lstm_sweep_kernel(typename LstmArgsOf<PEEP>::type a) {
+template <int KI, bool PEEP, bool ZO>
+__global__ void __launch_bounds__(COOP_THREADS, KI > 0 ? 1 : 2) lstm_sweep_kernel(typename LstmArgsOf<PEEP, ZO>::type a) {
     extern __shared__ __align__(16) float hs[];   // [COOP_NB][Hp]
     const int H = a.H, B = a.B, T = a.T;
     const int64_t G = (int64_t)a.ndir * 4 * H;
@@ -97,6 +123,10 @@ __global__ void __launch_bounds__(COOP_THREADS, KI > 0 ? 1 : 2) lstm_sweep_kerne
             pf = __ldg(P + H + j);
             po = __ldg(P + 2 * H + j);
         }
+    }
+    uint32_t s32 = 0;
+    if constexpr (ZO) {
+        if (a.train) s32 = (uint32_t)__ldg(a.step);
     }
 
     for (int s = 0; s < T; ++s) {
@@ -172,6 +202,17 @@ __global__ void __launch_bounds__(COOP_THREADS, KI > 0 ? 1 : 2) lstm_sweep_kerne
             }
             const bool live = valid && t < Tb;
             const int64_t hc = ((int64_t)t * B + b) * H + j;      // (t, b, j) in the [T][B][H] arrays
+            bool kc = false, kh = false;     // zoneout, training mode: c_t / h_t keep the previous step's value
+            if constexpr (ZO) {
+                if (a.train && valid) {
+                    const uint32_t g = (uint32_t)(a.first + a.stride * b);
+                    const uint4 r = curand_Philox4x32_10(
+                        make_uint4(s32, g, (uint32_t)t, ((uint32_t)a.layer << 24) | ((uint32_t)dir << 23) | (uint32_t)j),
+                        a.key);
+                    kc = r.x < a.thr_c;
+                    kh = r.y < a.thr_h;
+                }
+            }
             if (!bptt && PEEP) {
                 // c_prev of utterance b from the lane that wrote it, to the four gate lanes of b
                 const float cp0 = (valid && orow == 0 && live && s > 0) ? a.c[dir][((int64_t)tp * B + b) * H + j] : 0.f;
@@ -182,13 +223,15 @@ __global__ void __launch_bounds__(COOP_THREADS, KI > 0 ? 1 : 2) lstm_sweep_kerne
                 float act = (orow == 2) ? tanhf(z) : lstm_sigmoid(z);
                 const float gi = __shfl_sync(0xffffffffu, act, ob), gf = __shfl_sync(0xffffffffu, act, 8 + ob);
                 const float gg = __shfl_sync(0xffffffffu, act, 16 + ob);
-                const float cn = fmaf(gf, cp, gi * gg);
+                float cn = fmaf(gf, cp, gi * gg);
+                if constexpr (ZO) cn = zone(a, kc, a.zc, cp, cn);
                 if (orow == 3) act = lstm_sigmoid(fmaf(po, cn, z));
                 const float gO = __shfl_sync(0xffffffffu, act, 24 + ob);
                 if (valid) {
                     a.gates[go] = live ? act : 0.f;
                     if (orow == 0) {
-                        const float hn = gO * tanhf(cn);
+                        float hn = gO * tanhf(cn);
+                        if constexpr (ZO) hn = zone(a, kh, a.zh, (live && s > 0) ? a.h[dir][((int64_t)tp * B + b) * H + j] : 0.f, hn);
                         a.c[dir][hc] = live ? cn : 0.f;
                         a.h[dir][hc] = live ? hn : 0.f;
                     }
@@ -202,8 +245,10 @@ __global__ void __launch_bounds__(COOP_THREADS, KI > 0 ? 1 : 2) lstm_sweep_kerne
                     a.gates[go] = live ? act : 0.f;
                     if (orow == 0) {
                         const float cp = (live && s > 0) ? a.c[dir][((int64_t)tp * B + b) * H + j] : 0.f;
-                        const float cn = fmaf(gf, cp, gi * gg);
-                        const float hn = gO * tanhf(cn);
+                        float cn = fmaf(gf, cp, gi * gg);
+                        if constexpr (ZO) cn = zone(a, kc, a.zc, cp, cn);
+                        float hn = gO * tanhf(cn);
+                        if constexpr (ZO) hn = zone(a, kh, a.zh, (live && s > 0) ? a.h[dir][((int64_t)tp * B + b) * H + j] : 0.f, hn);
                         a.c[dir][hc] = live ? cn : 0.f;
                         a.h[dir][hc] = live ? hn : 0.f;
                     }
@@ -213,7 +258,41 @@ __global__ void __launch_bounds__(COOP_THREADS, KI > 0 ? 1 : 2) lstm_sweep_kerne
                 const float p2 = __shfl_sync(0xffffffffu, acc[0], 16 + ob), p3 = __shfl_sync(0xffffffffu, acc[0], 24 + ob);
                 const float gi = __shfl_sync(0xffffffffu, gv, ob), gf = __shfl_sync(0xffffffffu, gv, 8 + ob);
                 const float gg = __shfl_sync(0xffffffffu, gv, 16 + ob), gO = __shfl_sync(0xffffffffu, gv, 24 + ob);
-                if (valid && orow == 0) {
+                if constexpr (ZO) {
+                    if (valid && orow == 0) {
+                        float *dcp = a.dc + ((int64_t)dir * B + b) * H + j;
+                        float *dhp = a.dhc + ((int64_t)dir * B + b) * H + j;
+                        // hcar: lambda_h dh, -0 where nothing is carried (x + -0 is x, bit for bit, for every x)
+                        float dzi = 0.f, dzf = 0.f, dzg = 0.f, dzo = 0.f, dct = 0.f, hcar = -0.f;
+                        if (live) {
+                            float dh = __ldg(a.dh + hc) + ((p0 + p1) + (p2 + p3));
+                            const bool has_prev = (tp >= 0 && tp < T), has_next = (s > 0);
+                            if (has_next) dh += *dhp;
+                            const float ct = a.c[dir][hc], tc = tanhf(ct);
+                            const float cp = has_prev ? a.c[dir][((int64_t)tp * B + b) * H + j] : 0.f;
+                            const float dht = a.train ? (kh ? 0.f : dh) : (1.f - a.zh) * dh;     // d h~_t
+                            dzo = dht * tc * (gO * (1.f - gO));
+                            const float carry = has_next ? *dcp : 0.f;
+                            if constexpr (PEEP) dct = fmaf(po, dzo, dht * gO * (1.f - tc * tc)) + carry;
+                            else dct = dht * gO * (1.f - tc * tc) + carry;
+                            const float dcc = a.train ? (kc ? 0.f : dct) : (1.f - a.zc) * dct;     // d c~_t
+                            dzi = dcc * gg * (gi * (1.f - gi));
+                            dzf = dcc * cp * (gf * (1.f - gf));
+                            dzg = dcc * gi * (1.f - gg * gg);
+                            hcar = a.train ? (kh ? dh : -0.f) : a.zh * dh;
+                        }
+                        // the whole dc_t term of dc_{t-1}: (lambda_c + (1 - lambda_c) f) dc [+ p_i dz_i + p_f dz_f]
+                        const float fz = a.train ? (kc ? 1.f : gf) : fmaf(1.f - a.zc, gf, a.zc);
+                        if constexpr (PEEP) *dcp = (a.train && kc) ? dct : fmaf(fz, dct, fmaf(pi, dzi, pf * dzf));
+                        else *dcp = (a.train && kc) ? dct : fz * dct;
+                        *dhp = hcar;
+                        float *dzp = a.dz + ((int64_t)t * B + b) * G + gbase + j;
+                        dzp[0] = dzi;
+                        dzp[H] = dzf;
+                        dzp[2 * H] = dzg;
+                        dzp[3 * H] = dzo;
+                    }
+                } else if (valid && orow == 0) {
                     float *dcp = a.dc + ((int64_t)dir * B + b) * H + j;
                     float dzi = 0.f, dzf = 0.f, dzg = 0.f, dzo = 0.f, dct = 0.f;
                     if (live) {
@@ -255,10 +334,10 @@ struct LstmPlan {
     size_t smem;
 };
 
-// the plan of the kernel that runs: the peephole mode's occupancy is its own.  CTCB_LSTM=reread takes KI = 0 at any
+// the plan of the kernel that runs: the peephole and zoneout modes' occupancy is their own.  CTCB_LSTM=reread takes KI = 0 at any
 // H; CTCB_LSTM_PARTS forces the partition count, refused here, before any launch, where its CTAs cannot all be
 // co-resident.  A width whose shared memory exceeds the opt-in maximum is refused before the attribute call.
-int lstm_plan(int H, int B, int ndir, bool peep, LstmPlan *p) {
+int lstm_plan(int H, int B, int ndir, bool peep, bool zo, LstmPlan *p) {
     if (H <= 0 || B <= 0 || (ndir != 1 && ndir != 2))
         return set_error(CTCB_EINVAL, "LSTM sweep: bad sizes (H=%d, B=%d, ndir=%d)", H, B, ndir);
     const int slices = (H + LS_UNITS - 1) / LS_UNITS;
@@ -270,8 +349,11 @@ int lstm_plan(int H, int B, int ndir, bool peep, LstmPlan *p) {
     for (p->KI = reg ? H / 32 : 0;; p->KI = 0) {   // U does not fit the register files the device holds: re-read it
         const int rc = with_ki<2, 4, 8, 16, 32>(p->KI, [&](auto ki) {
             constexpr int KI = decltype(ki)::value;
-            return peep ? coop_occupancy(lstm_sweep_kernel<KI, true>, p->smem, &p->per_sm)
-                        : coop_occupancy(lstm_sweep_kernel<KI, false>, p->smem, &p->per_sm);
+            if (zo)
+                return peep ? coop_occupancy(lstm_sweep_kernel<KI, true, true>, p->smem, &p->per_sm)
+                            : coop_occupancy(lstm_sweep_kernel<KI, false, true>, p->smem, &p->per_sm);
+            return peep ? coop_occupancy(lstm_sweep_kernel<KI, true, false>, p->smem, &p->per_sm)
+                        : coop_occupancy(lstm_sweep_kernel<KI, false, false>, p->smem, &p->per_sm);
         });
         if (rc != CTCB_OK) return rc;
         if (p->KI == 0 || ndir * slices <= p->per_sm * num_sms()) break;
@@ -280,25 +362,29 @@ int lstm_plan(int H, int B, int ndir, bool peep, LstmPlan *p) {
 }
 
 // ctcb_brnn_create's check that the device holds the sweep of a config
-int lstm_check(int H, int B, int ndir, bool peep) {
+int lstm_check(int H, int B, int ndir, bool peep, bool zo) {
     if (no_device()) return CTCB_OK;
     LstmPlan p;
-    return lstm_plan(H, B, ndir, peep, &p);
+    return lstm_plan(H, B, ndir, peep, zo, &p);
 }
 
 size_t lstm_carry_bytes(int H, int B) { return align_up((size_t)2 * B * H * sizeof(float), 256); }
 
+// keep iff r < floor(z 2^32), the product in float64; z in [0, 1) keeps it below 2^32
+uint32_t zoneout_threshold(float z) { return (uint32_t)std::floor((double)z * 4294967296.0); }
+
 // counters: 4096 bytes of device scratch (word 0 = error flag, cleared by the caller); dc: lstm_carry_bytes(H, B).
-// Pf (and Pb with Ub) non-null: the peephole mode.
+// Pf (and Pb with Ub) non-null: the peephole mode.  zo non-null: the zoneout mode (its dhc another
+// lstm_carry_bytes(H, B) in mode 1).
 int run_lstm_sweep(int mode, int T, int B, int H, const int32_t *Tlen, float *gates, const float *Uf, const float *Ub,
                    const float *Pf, const float *Pb, float *hF, float *hB, float *cF, float *cB, const float *dh,
-                   float *dz, unsigned int *counters, float *dc, cudaStream_t st) {
+                   float *dz, unsigned int *counters, float *dc, const LstmZoneout *zo, cudaStream_t st) {
     LstmPlan p;
     const int ndir = Ub ? 2 : 1;
     const bool peep = (Pf != nullptr);
-    const int rc = lstm_plan(H, B, ndir, peep, &p);
+    const int rc = lstm_plan(H, B, ndir, peep, zo != nullptr, &p);
     if (rc != CTCB_OK) return rc;
-    LstmPeepArgs a;
+    LstmZoArgs a;
     a.mode = mode; a.T = T; a.B = B; a.H = H; a.Tlen = Tlen; a.gates = gates;
     a.U[0] = Uf; a.U[1] = Ub ? Ub : Uf;
     a.h[0] = hF; a.h[1] = Ub ? hB : hF;
@@ -306,12 +392,29 @@ int run_lstm_sweep(int mode, int T, int B, int H, const int32_t *Tlen, float *ga
     a.dh = dh; a.dz = dz; a.dc = dc;
     a.ndir = ndir;
     a.P[0] = Pf; a.P[1] = Ub ? Pb : Pf;
+    if (zo) {
+        a.dhc = zo->dhc;
+        a.train = zo->train ? 1 : 0;
+        a.zc = zo->zc;
+        a.zh = zo->zh;
+        a.thr_c = zoneout_threshold(zo->zc);
+        a.thr_h = zoneout_threshold(zo->zh);
+        a.key = make_uint2((uint32_t)zo->seed, (uint32_t)(zo->seed >> 32));
+        a.step = zo->step;
+        a.first = zo->first;
+        a.stride = zo->stride;
+        a.layer = zo->layer;
+    }
     const int slices = (H + LS_UNITS - 1) / LS_UNITS;
     return with_ki<2, 4, 8, 16, 32>(p.KI, [&](auto ki) {
         constexpr int KI = decltype(ki)::value;
-        return peep ? coop_launch(lstm_sweep_kernel<KI, true>, a, counters, slices, p.parts, p.smem, st)
-                    : coop_launch(lstm_sweep_kernel<KI, false>, static_cast<LstmArgs &>(a), counters, slices, p.parts,
-                                  p.smem, st);
+        if (zo)
+            return peep ? coop_launch(lstm_sweep_kernel<KI, true, true>, a, counters, slices, p.parts, p.smem, st)
+                        : coop_launch(lstm_sweep_kernel<KI, false, true>, a, counters, slices, p.parts, p.smem, st);
+        return peep ? coop_launch(lstm_sweep_kernel<KI, true, false>, static_cast<LstmPeepArgs &>(a), counters, slices,
+                                  p.parts, p.smem, st)
+                    : coop_launch(lstm_sweep_kernel<KI, false, false>, static_cast<LstmArgs &>(a), counters, slices,
+                                  p.parts, p.smem, st);
     });
 }
 
@@ -397,30 +500,37 @@ extern "C" size_t ctcb_lstm_sweep_workspace_bytes(int H, int B) {
     return 4096 + ctcb::lstm_carry_bytes(H, B);
 }
 
+extern "C" size_t ctcb_lstm_sweep_zoneout_workspace_bytes(int H, int B) {
+    if (H <= 0 || B <= 0) return 0;
+    return 4096 + 2 * ctcb::lstm_carry_bytes(H, B);
+}
+
+// zo non-null: the zoneout mode, whose dh carry follows the dc carry in scratch
 static int lstm_sweep_entry(const char *name, int mode, int T, int B, int H, const int32_t *T_per_utt, float *gates,
                             const float *Uf, const float *Ub, const float *Pf, const float *Pb, float *hF, float *hB,
-                            float *cF, float *cB, const float *dh, float *dz, void *scratch, size_t scratch_bytes,
-                            void *stream) {
+                            float *cF, float *cB, const float *dh, float *dz, ctcb::LstmZoneout *zo, void *scratch,
+                            size_t scratch_bytes, void *stream) {
     using namespace ctcb;
     if (!T_per_utt || !gates || !Uf || !cF || !scratch || (mode == 0 && !hF) || (mode == 1 && (!dh || !dz)) ||
         (Ub && (!cB || (mode == 0 && !hB))))
         return set_error(CTCB_EINVAL, "%s: null pointer argument", name);
     if (T <= 0 || B <= 0 || H <= 0 || (mode != 0 && mode != 1))
         return set_error(CTCB_EINVAL, "%s: bad sizes", name);
-    const size_t need = ctcb_lstm_sweep_workspace_bytes(H, B);
+    const size_t need = zo ? ctcb_lstm_sweep_zoneout_workspace_bytes(H, B) : ctcb_lstm_sweep_workspace_bytes(H, B);
     if (scratch_bytes < need || (((uintptr_t)scratch) & 255))
         return set_error(CTCB_ENOMEM, "%s: scratch of %zu bytes (256-byte aligned) needed, got %zu", name, need,
                          scratch_bytes);
+    if (zo) zo->dhc = (float *)((char *)scratch + 4096 + lstm_carry_bytes(H, B));
     CTCB_CUDA_CHECK(cudaMemsetAsync(scratch, 0, 16 * sizeof(unsigned int), (cudaStream_t)stream));   // error flag
     return run_lstm_sweep(mode, T, B, H, T_per_utt, gates, Uf, Ub, Pf, Pb, hF, hB, cF, cB, dh, dz,
-                          (unsigned int *)scratch, (float *)((char *)scratch + 4096), (cudaStream_t)stream);
+                          (unsigned int *)scratch, (float *)((char *)scratch + 4096), zo, (cudaStream_t)stream);
 }
 
 extern "C" int ctcb_lstm_sweep_f32(int mode, int T, int B, int H, const int32_t *T_per_utt, float *gates,
                                    const float *Uf, const float *Ub, float *hF, float *hB, float *cF, float *cB,
                                    const float *dh, float *dz, void *scratch, size_t scratch_bytes, void *stream) {
     return lstm_sweep_entry("ctcb_lstm_sweep_f32", mode, T, B, H, T_per_utt, gates, Uf, Ub, nullptr, nullptr, hF, hB,
-                            cF, cB, dh, dz, scratch, scratch_bytes, stream);
+                            cF, cB, dh, dz, nullptr, scratch, scratch_bytes, stream);
 }
 
 extern "C" int ctcb_lstm_sweep_peephole_f32(int mode, int T, int B, int H, const int32_t *T_per_utt, float *gates,
@@ -429,7 +539,27 @@ extern "C" int ctcb_lstm_sweep_peephole_f32(int mode, int T, int B, int H, const
                                             void *scratch, size_t scratch_bytes, void *stream) {
     if (!Pf || (Ub && !Pb)) return ctcb::set_error(CTCB_EINVAL, "ctcb_lstm_sweep_peephole_f32: null pointer argument");
     return lstm_sweep_entry("ctcb_lstm_sweep_peephole_f32", mode, T, B, H, T_per_utt, gates, Uf, Ub, Pf, Pb, hF, hB,
-                            cF, cB, dh, dz, scratch, scratch_bytes, stream);
+                            cF, cB, dh, dz, nullptr, scratch, scratch_bytes, stream);
+}
+
+extern "C" int ctcb_lstm_sweep_zoneout_f32(int mode, int T, int B, int H, const int32_t *T_per_utt, float *gates,
+                                           const float *Uf, const float *Ub, const float *Pf, const float *Pb,
+                                           float *hF, float *hB, float *cF, float *cB, const float *dh, float *dz,
+                                           float zc, float zh, int train, uint64_t seed, const int64_t *step,
+                                           int64_t first, int64_t stride, int layer, void *scratch,
+                                           size_t scratch_bytes, void *stream) {
+    using namespace ctcb;
+    const char *name = "ctcb_lstm_sweep_zoneout_f32";
+    if (Pf && Ub && !Pb) return set_error(CTCB_EINVAL, "%s: null pointer argument", name);
+    if (!(zc >= 0.f && zc < 1.f) || !(zh >= 0.f && zh < 1.f))
+        return set_error(CTCB_EINVAL, "%s: zc = %g, zh = %g (need both in [0, 1))", name, (double)zc, (double)zh);
+    if (train && !step) return set_error(CTCB_EINVAL, "%s: training mode needs a step counter", name);
+    if (first < 0 || stride < 1 || layer < 1 || layer > 255)
+        return set_error(CTCB_EINVAL, "%s: first = %lld, stride = %lld, layer = %d (need first >= 0, stride >= 1, "
+                         "1 <= layer <= 255)", name, (long long)first, (long long)stride, layer);
+    LstmZoneout zo{zc, zh, train != 0, seed, step, first, stride, layer, nullptr};
+    return lstm_sweep_entry(name, mode, T, B, H, T_per_utt, gates, Uf, Ub, Pf, Pf ? Pb : nullptr, hF, hB, cF, cB, dh,
+                            dz, &zo, scratch, scratch_bytes, stream);
 }
 
 extern "C" size_t ctcb_lstm_peephole_grad_workspace_bytes(int T, int B, int H, int ndir) {
@@ -453,14 +583,22 @@ extern "C" int ctcb_lstm_peephole_grad_f32(int T, int B, int H, const float *dz,
                                   (cudaStream_t)stream);
 }
 
-extern "C" int ctcb_debug_lstm_plan(int H, int B, int ndir, int peephole, int32_t *out) {
+static int debug_lstm_plan(int H, int B, int ndir, bool peep, bool zo, int32_t *out) {
     if (!out) return ctcb::set_error(CTCB_EINVAL, "ctcb_debug_lstm_plan: null output");
     ctcb::LstmPlan p;
-    const int rc = ctcb::lstm_plan(H, B, ndir, peephole != 0, &p);
+    const int rc = ctcb::lstm_plan(H, B, ndir, peep, zo, &p);
     if (rc != CTCB_OK) return rc;
     out[0] = p.KI;
     out[1] = p.parts;
     out[2] = p.per_sm;
     out[3] = (ctcb::coop_tiles(B) + p.parts - 1) / p.parts;
     return CTCB_OK;
+}
+
+extern "C" int ctcb_debug_lstm_plan(int H, int B, int ndir, int peephole, int32_t *out) {
+    return debug_lstm_plan(H, B, ndir, peephole != 0, false, out);
+}
+
+extern "C" int ctcb_debug_lstm_zoneout_plan(int H, int B, int ndir, int peephole, int32_t *out) {
+    return debug_lstm_plan(H, B, ndir, peephole != 0, true, out);
 }

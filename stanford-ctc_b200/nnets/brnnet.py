@@ -42,6 +42,12 @@ single contiguous vector.  New, additive surface for the minibatch/data-parallel
                                                 training calls (include/ctcb200.h: ctcb_brnn_set_weight_noise): one
                                                 draw per step from (seed dropoutSeed, the counter dropoutStep, the
                                                 element's offset); the L2 term and the update see the clean weights
+    NNet(..., cell='lstm', zoneoutCell=zc, zoneoutHidden=zh)
+                                             zoneout of every LSTM layer's c and h (include/ctcb200.h: zoneout):
+                                                training calls keep each unit's previous c / h with probability zc /
+                                                zh, drawn from (seed dropoutSeed, the counter dropoutStep, the
+                                                utterance's index, the frame, the layer, the unit); forward-only calls
+                                                use the expectation, so a net for testing needs the trained values
     costAndGradBatch(datas, labelss)         -> (costs[B], grad, skips[B])   host arrays in; more than maxUtts
                                                 utterances are accumulated over micro-batches
     costAndGradDevice(batch, first, last)    -> no host sync; see DeviceBatch
@@ -169,7 +175,7 @@ class NNet:
                  allowTopTemporal=False, device=None, unidirectional=False, numTemporal=1, dropout=0.0,
                  dropoutSeed=33, cell="relu", layerNorm=False, subsample=1, subsampleLayer=1, peephole=False,
                  freqMasks=0, freqMaskWidth=0, timeMasks=0, timeMaskWidth=0, timeMaskRatio=1.0, featDim=None,
-                 weightNoise=0.0):
+                 weightNoise=0.0, zoneoutCell=0.0, zoneoutHidden=0.0):
         torch = _ctcb.require_cuda()
         self._torch = torch
         self.dev = torch.device("cuda", torch.cuda.current_device() if device is None else device)
@@ -234,11 +240,20 @@ class NNet:
         self.weightNoise = float(weightNoise)
         if not (np.isfinite(self.weightNoise) and self.weightNoise >= 0.0):
             raise ValueError("weightNoise=%r must be a finite standard deviation >= 0" % (weightNoise,))
+        # Zoneout of the LSTM state (include/ctcb200.h: ctcb_brnn_set_zoneout).  Only a net with a probability > 0
+        # reserves the dh carry, so a net without zoneout keeps today's workspace.
+        self.zoneoutCell, self.zoneoutHidden = float(zoneoutCell), float(zoneoutHidden)
+        for name, z in (("zoneoutCell", self.zoneoutCell), ("zoneoutHidden", self.zoneoutHidden)):
+            if not 0.0 <= z < 1.0:
+                raise ValueError("%s=%r must be in [0, 1)" % (name, z))
+        self.zoneout = self.zoneoutCell > 0.0 or self.zoneoutHidden > 0.0
+        if self.zoneout and cell != "lstm":
+            raise ValueError("zoneoutCell / zoneoutHidden > 0 need cell='lstm'; cell is %r" % (cell,))
         self._cfg = BrnnConfig(inputDim, outputDim, layerSize, numLayers, max(self.temporalLayer, 0), maxBatch,
                                maxUtts, self.maxLabels, float(reg), float(self.maxAct), int(self.unidirectional),
                                self.numTemporal, _ctcb.CELLS[cell], int(self.layerNorm), self.subsample,
                                self.subsampleLayer, int(self.peephole), self.featDim or 0,
-                               int(self.weightNoise > 0.0))
+                               int(self.weightNoise > 0.0), int(self.zoneout))
         self._h = ctypes.c_void_p()
         check(lib.ctcb_brnn_create(ctypes.byref(self._cfg), ctypes.byref(self._h)))
         self.stack = None
@@ -247,14 +262,14 @@ class NNet:
         # counter lives on the device, so a CUDA graph of an SGD step reads its current value at every replay; sgd.SGD
         # advances it once per step.  The net owns it when any of them is on.  dropoutShard = (rank, world) places
         # this process's utterances in the step's minibatch for dropout and the masks (None: from torch.distributed).
-        # The weight noise is one draw per step, the same on every rank.
+        # The weight noise is one draw per step, the same on every rank; zoneout's masks are placed like dropout's.
         self.dropout = float(dropout)
         self.dropoutSeed = int(dropoutSeed)
         self.dropoutStep = None
         self.dropoutShard = None
         if self.dropout != 0.0 and not 0.0 < self.dropout < 1.0:
             raise ValueError("dropout=%r must be in [0, 1)" % (dropout,))
-        if self.dropout != 0.0 or self.inputMasks or self.weightNoise > 0.0:
+        if self.dropout != 0.0 or self.inputMasks or self.weightNoise > 0.0 or self.zoneout:
             self.dropoutStep = torch.zeros(1, dtype=torch.int64, device=self.dev)
         seed = self.dropoutSeed & 0xFFFFFFFFFFFFFFFF
         if self.dropout != 0.0:
@@ -264,6 +279,9 @@ class NNet:
                                             self.timeMaskWidth, self.timeMaskRatio, seed, ptr(self.dropoutStep)))
         if self.weightNoise > 0.0:
             check(lib.ctcb_brnn_set_weight_noise(self._h, self.weightNoise, seed, ptr(self.dropoutStep)))
+        if self.zoneout:
+            check(lib.ctcb_brnn_set_zoneout(self._h, self.zoneoutCell, self.zoneoutHidden, seed,
+                                            ptr(self.dropoutStep)))
 
     def __del__(self):
         h = getattr(self, "_h", None)
@@ -402,10 +420,11 @@ class NNet:
         the gradient and the statistics tail into what the earlier calls left; only the last=True call exchanges
         over the ranks and adds the L2 term.  `out` optionally names the (cost[B], skip[B]) device tensors to write
         (default: the net's own per-utterance buffers).  u0: position of the batch's first utterance in this rank's
-        shard of the step, which with the rank places each utterance in the minibatch for its dropout and input masks."""
+        shard of the step, which with the rank places each utterance in the minibatch for its dropout, input and zoneout
+        masks."""
         if not self.train:
             return self._forward_device(batch)
-        if self.dropout > 0.0 or self.inputMasks:
+        if self.dropout > 0.0 or self.inputMasks or self.zoneout:
             rank, world = self.dropoutShard or parallel.world_info()[1:]
             check(lib.ctcb_brnn_set_dropout_utts(self._h, rank + world * u0, world))
         B, Tmax = batch.B, batch.Tmax

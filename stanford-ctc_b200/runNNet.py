@@ -9,6 +9,7 @@ The implementation is organised differently: a declarative flag table, one RunDi
 side files, and separate train/evaluate phases.  Site paths of run_cfg.py / decoder_config.py became
 flags (--runDir, --outDir); new flags: --numTemporal, --cell, --peephole, --layerNorm, --subsample, --subsampleLayer, --batchSize, --maxUtts, --maxLabels,
 --dropout, --freqMasks, --freqMaskWidth, --timeMasks, --timeMaskWidth, --timeMaskRatio, --featDim, --weightNoise,
+--zoneoutCell, --zoneoutHidden,
 --optimizer,
 --beta1, --beta2, --epsilon, --quiet.  Under torchrun the same
 script trains data-parallel (one process per GPU, one NCCL all-reduce per step).
@@ -77,6 +78,10 @@ FLAGS = [
     ("weightNoise", float, 0.0, "standard deviation of the Gaussian noise added to the weight matrices while training, "
                                 "one draw per step (0 = off; --test never adds noise; a cfg.json written without it "
                                 "has none)"),
+    ("zoneoutCell", float, 0.0, "zoneout probability of the LSTM cell state c while training (needs --cell lstm; "
+                                "0 = off; --test runs the expectation cell with the trained value; a cfg.json "
+                                "written without it has none)"),
+    ("zoneoutHidden", float, 0.0, "zoneout probability of the LSTM output h, as --zoneoutCell"),
     ("optimizer", str, "nesterov", "update rule: nesterov (the reference's, with --momentum), adagrad or adam; --step "
                                    "is the step size of each and --anneal applies to it"),
     ("beta1", float, 0.9, "adam: decay of the first-moment estimate"),
@@ -225,7 +230,8 @@ def _train(opts, cfg, run_dir, log, rank, world):
                      layerNorm=opts.layerNorm, subsample=opts.subsample, subsampleLayer=opts.subsampleLayer,
                      peephole=opts.peephole, freqMasks=opts.freqMasks, freqMaskWidth=opts.freqMaskWidth,
                      timeMasks=opts.timeMasks, timeMaskWidth=opts.timeMaskWidth, timeMaskRatio=opts.timeMaskRatio,
-                     featDim=opts.featDim, weightNoise=opts.weightNoise)
+                     featDim=opts.featDim, weightNoise=opts.weightNoise, zoneoutCell=opts.zoneoutCell,
+                     zoneoutHidden=opts.zoneoutHidden)
     net.initParams()
     optimizer = sgd.SGD(net, opts.maxUttLen, alpha=opts.step, optimizer=opts.optimizer, momentum=opts.momentum,
                         batchSize=opts.batchSize, verbose=(rank == 0 and not opts.quiet), beta1=opts.beta1,
@@ -289,7 +295,8 @@ def test(opts, rank=0, world=1):
     net = rnnet.NNet(trained.inputDim, trained.outputDim, trained.layerSize, trained.numLayers, trained.maxUttLen,
                      temporalLayer=trained.temporalLayer, train=False, maxUtts=max(1, opts.maxUtts),
                      numTemporal=trained.numTemporal, cell=trained.cell, layerNorm=trained.layerNorm,
-                     subsample=trained.subsample, subsampleLayer=trained.subsampleLayer, peephole=trained.peephole)
+                     subsample=trained.subsample, subsampleLayer=trained.subsampleLayer, peephole=trained.peephole,
+                     zoneoutCell=trained.zoneoutCell, zoneoutHidden=trained.zoneoutHidden)
     net.initParams()
     with open(trained.in_file, "rb") as fid:
         pickle.load(fid)                              # optimiser state: not needed here

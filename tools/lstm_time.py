@@ -6,9 +6,10 @@ over whole optimisation steps (sgd.SGD.step_device: CUDA graph replay, host pack
 does it), the arms alternated over two rounds after a warm-up; then one eager pass per arm with the per-phase events
 of ctcb_profile_* gives the two sweeps alone (sweep_fwd, sweep_bptt) and the rest of the step.  The card's name, power
 limit and clock are read in the same run.  Prints one JSON object (and writes it to --out).  With --peephole the two
-arms are the LSTM net without and with peephole connections (peephole=True), and the ratio is theirs.
+arms are the LSTM net without and with peephole connections (peephole=True), and the ratio is theirs.  With --zoneout
+the two arms are the LSTM net without and with zoneout (zoneoutCell=0.15, zoneoutHidden=0.05).
 
-    python tools/lstm_time.py [--steps 5] [--warmup 4] [--shapes c2,c3] [--peephole] [--out FILE]
+    python tools/lstm_time.py [--steps 5] [--warmup 4] [--shapes c2,c3] [--peephole | --zoneout] [--out FILE]
 """
 import argparse
 import ctypes
@@ -29,12 +30,13 @@ SHAPES = {
 }
 
 
-def make_opt(c, cell, peephole=False):
+def make_opt(c, cell, peephole=False, zoneout=False):
     import nnets.brnnet as rnnet
     import sgd
     np.random.seed(33)
+    z = dict(zoneoutCell=0.15, zoneoutHidden=0.05) if zoneout else {}
     nn = rnnet.NNet(c["D"], c["K"], c["H"], c["N"], c["T"], temporalLayer=c["tl"], maxUtts=c["B"], maxLabels=c["L"],
-                    cell=cell, peephole=peephole)
+                    cell=cell, peephole=peephole, **z)
     nn.initParams()
     opt = sgd.SGD(nn, c["T"], alpha=1e-5, momentum=0.9, batchSize=c["B"], verbose=False)
     opt.it = 11                      # past the momentum warm-up: one step shape
@@ -47,6 +49,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=4)
     ap.add_argument("--shapes", default="c2,c3")
     ap.add_argument("--peephole", action="store_true", help="time LSTM with peepholes against LSTM without")
+    ap.add_argument("--zoneout", action="store_true", help="time LSTM with zoneout against LSTM without")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     import torch
@@ -61,8 +64,12 @@ def main():
         datas, labels = make_batch(c, c["B"], seed=33)
         out = {}
         with torch.cuda.stream(stream):
-            kinds = {"lstm": ("lstm", False), "lstm_peephole": ("lstm", True)} if args.peephole else \
-                {"relu": ("relu", False), "lstm": ("lstm", False)}
+            if args.zoneout:
+                kinds = {"lstm": ("lstm", False, False), "lstm_zoneout": ("lstm", False, True)}
+            elif args.peephole:
+                kinds = {"lstm": ("lstm", False), "lstm_peephole": ("lstm", True)}
+            else:
+                kinds = {"relu": ("relu", False), "lstm": ("lstm", False)}
             arms = {arm: make_opt(c, *kind) for arm, kind in kinds.items()}
             for cell, (nn, opt) in arms.items():
                 for _ in range(args.warmup):
@@ -73,7 +80,9 @@ def main():
                     rec[cell].append(time_steps(torch, opt, datas, labels, args.steps))
             for cell, (nn, opt) in arms.items():
                 plan = (ctypes.c_int32 * 4)()
-                if cell != "relu":
+                if cell == "lstm_zoneout":
+                    lib.ctcb_debug_lstm_zoneout_plan(c["H"], c["B"], 2, 0, plan)
+                elif cell != "relu":
                     lib.ctcb_debug_lstm_plan(c["H"], c["B"], 2, int(kinds[cell][1]), plan)
                 out[cell] = dict(ms_per_step_device=[round(r[0], 3) for r in rec[cell]],
                                  ms_per_step_wall=[round(r[1], 3) for r in rec[cell]],
