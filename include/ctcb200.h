@@ -54,8 +54,11 @@ int ctcb_profile_report(char *buf, size_t cap);
  * nll_out   : float32[B]  -log p(labels | acts)     (ctc_fast.pyx:152)
  * skip_out  : int32[B]    1 where a frame normaliser was 0 (ctc_fast.pyx:147-149), and 1 where the scaled trellis
  *             lost mass to float64 underflow (forward and backward log-likelihoods more than 1e-4 nats apart: long
- *             utterances with unaligned outputs, where the reference returns a wrong loss and gradient)
- * workspace : ctcb_ctc_workspace_bytes(B, Tmax, max_labels) bytes of device scratch.  That size never decreases with B,
+ *             utterances with unaligned outputs, where the reference returns a wrong loss and gradient), and,
+ *             checked on the device before any row is read, where utterance u is malformed: a label count
+ *             label_off[u+1] - label_off[u] below 0 or above max_labels, or a label outside [0, K).  A malformed
+ *             utterance is skipped exactly as one with T_per_utt = 0: the same nll, a zero gradient on all Tmax rows.
+ * workspace: ctcb_ctc_workspace_bytes(B, Tmax, max_labels) bytes of device scratch.  That size never decreases with B,
  *             Tmax or max_labels, so a buffer sized for the largest call serves every smaller one: one fp64 trellis
  *             plane of Tmax x 64P doubles (P = pairs per lane, 1..16 by max_labels) per utterance, two per utterance
  *             for the first 256 (the frame-parallel kernel spills alpha and beta), i.e. max(B, 2 min(B, 256)) planes.

@@ -95,8 +95,10 @@ def ctc_loss(params, seq, blank=0):
     seq = np.ascontiguousarray(seq)
     if seq.dtype != np.int32 or seq.ndim != 1:
         raise ValueError("Buffer dtype mismatch, expected 'int' but got '%s'" % seq.dtype)
-    torch = _ctcb.require_cuda()
     K, T = params.shape
+    if seq.size and (seq.min() < 0 or seq.max() >= K):
+        raise IndexError("label sequence out of range [0, %d)" % K)     # the reference would read out of bounds
+    torch = _ctcb.require_cuda()
     L = int(seq.shape[0])
     dev = torch.device("cuda", torch.cuda.current_device())
     b = _single_utterance_buffers(torch, dev, T, K, L)

@@ -68,13 +68,28 @@ from _ctcb import lib, check, ptr, BrnnConfig
 CTC_MAX_LABELS = 511      # CTCB_CTC_MAX_LABELS
 
 
+def utterance_labels(u, labels, maxLabels, K):
+    """The label sequence of utterance u as int32, refused with a ValueError when the net cannot train on it: more than
+    maxLabels labels, or a label outside [0, K) (an alignment file numbered 1..K, say).  The CTC kernel would skip such
+    an utterance on the device without a word; here training stops at it."""
+    l = np.asarray(labels, dtype=np.int32).reshape(-1)
+    if l.shape[0] > maxLabels:
+        raise ValueError("utterance %d has %d labels; this net was built for at most maxLabels=%d"
+                         % (u, l.shape[0], maxLabels))
+    bad = np.flatnonzero((l < 0) | (l >= K))
+    if bad.size:
+        raise ValueError("utterance %d has the label %d at position %d; this net has %d output classes, labels 0..%d"
+                         % (u, int(l[bad[0]]), int(bad[0]), K, K - 1))
+    return l
+
+
 class DeviceBatch(object):
     """A minibatch staged for the device: pinned host staging buffers + device tensors.
-    feats is time-major [Tmax][B][inputDim]."""
+    feats is time-major [Tmax][B][inputDim]; labels lie in [0, K)."""
 
-    def __init__(self, torch, dev, maxT, maxB, inputDim, maxLabels):
+    def __init__(self, torch, dev, maxT, maxB, inputDim, maxLabels, K):
         self.maxT, self.maxB, self.D = maxT, maxB, inputDim
-        self.maxLabels = maxLabels
+        self.maxLabels, self.K = maxLabels, K
         self.h_feats = torch.zeros(maxT * maxB * inputDim, dtype=torch.float32).pin_memory()
         self.h_lens = torch.zeros(maxB, dtype=torch.int32).pin_memory()
         self.h_labels = torch.zeros(max(1, maxB * maxLabels), dtype=torch.int32).pin_memory()
@@ -115,10 +130,7 @@ class DeviceBatch(object):
         if labelss is not None:
             n = 0
             for u, l in enumerate(labelss):
-                l = np.asarray(l, dtype=np.int32).reshape(-1)
-                if l.shape[0] > self.maxLabels:
-                    raise ValueError("utterance %d has %d labels; this net was built for at most maxLabels=%d"
-                                     % (u, l.shape[0], self.maxLabels))
+                l = utterance_labels(u, l, self.maxLabels, self.K)
                 lab[n:n + l.shape[0]] = l
                 n += l.shape[0]
                 off[u + 1] = n
@@ -357,7 +369,8 @@ class NNet:
         # call reports its flag in the statistics tail); set by the sweep kernels on a wait timeout
         self._errflag = self._ws[fwd_off.value:fwd_off.value + 4].view(torch.int32)
         self._fwd_host = None       # pinned probabilities + error flag of one forward micro-batch (forwardBatch)
-        self._batch = DeviceBatch(torch, self.dev, self.maxBatch, self.maxUtts, self.inputDim, self.maxLabels)
+        self._batch = DeviceBatch(torch, self.dev, self.maxBatch, self.maxUtts, self.inputDim, self.maxLabels,
+                                  self.outputDim)
         self._batch_alt = None      # second staging buffer, created on first use by SGD.run's prefetch
         # per-utterance outputs: cost (float32) and skip (int32) share one buffer -> one D2H copy reads both
         self._out = torch.zeros(2 * self.maxUtts, dtype=torch.float32, device=self.dev)
@@ -378,7 +391,7 @@ class NNet:
         current (SGD.run packs minibatch i+1 into it while the device still works on minibatch i)."""
         if self._batch_alt is None:
             self._batch_alt = DeviceBatch(self._torch, self.dev, self.maxBatch, self.maxUtts, self.inputDim,
-                                          self.maxLabels)
+                                          self.maxLabels, self.outputDim)
         self._batch, self._batch_alt = self._batch_alt, self._batch
         return self._batch
 
