@@ -205,7 +205,34 @@ typedef struct ctcb_brnn_config {
     int32_t zoneout;       /* 0: off (so an initialiser without this member keeps its meaning); 1: zoneout of the LSTM
                             * cell's state (below) with the probabilities of ctcb_brnn_set_zoneout, which needs cell = 1;
                             * any other value, or 1 with cell = 0, makes the config invalid. */
+    int32_t interLayer;    /* m: 0 off (so an initialiser without this member keeps its meaning); 1 <= m <= numLayers - 1
+                            * adds the intermediate CTC loss of hidden layer m to training calls (below); any other value
+                            * makes the config invalid. */
+    float interWeight;     /* lambda of the intermediate CTC loss: ignored with interLayer = 0; with interLayer > 0 a
+                            * value that is not finite and > 0 makes the config invalid. */
 } ctcb_brnn_config;
+
+/* Intermediate CTC loss (interLayer = m >= 1; not in the reference; Lee & Watanabe, "Intermediate Loss Regularization
+ * for CTC-based Speech Recognition", ICASSP 2021, after the hierarchical CTC of Fernandez et al. 2007 and Sanabria &
+ * Metze, SLT 2018).  N = numLayers, K = outputDim, lambda = interWeight.  X_m is hidden layer m's output as map m + 1
+ * sees it (dropped, normalised, For + Back at a bi-directional temporal layer, h_f + h_b at an LSTM layer), on T_m
+ * frames: T_u, or T'_u = ceil(T_u / k) when m >= subsampleLayer.  The head is the net's own output map, as in ESPnet's
+ * InterCTC; it adds no parameter, so the flat vector, checkpoints and forward-only calls are those of the net without it.
+ *   Forward (training calls only): A = X_m W_{N+1}^T + b_{N+1}, [T_m][B][K]; nll_aux[u] is the CTC loss of softmax(A)
+ *   against utterance u's labels over its T_m frames, with the blank, maxLabels and skip rules of the main CTC.
+ *   Objective: cost = nll_main + lambda nll_aux per utterance.  Lee & Watanabe's (1 - w) L + w L_inter is this objective
+ *   with lambda = w / (1 - w) and the step size scaled by (1 - w); this form leaves the gradient of the top of the net
+ *   as it is without the loss.
+ *   Backward: D_aux = lambda d(nll_aux)/dA (the CTC gradient scaled in place, once, so that the two contractions and the
+ *   column sums below read the same values); dW_{N+1} += D_aux^T X_m and db_{N+1} += the column sums of D_aux; the
+ *   incoming delta of layer m gains D_aux W_{N+1}, under the ReLU mask and dropout's alpha of the delta from map m + 1,
+ *   added before layer normalisation's backward or the BPTT sweep reads it (behind the unstacking when map m + 1 reads
+ *   stacked frames: the term is at layer m's own rate).
+ *   Each CTC skips on its own: an utterance the intermediate CTC skips gets no gradient from it and adds nothing to its
+ *   sums.  cost_out, skip_out and the first four floats of stats_out keep their meaning (the main CTC's).
+ * Forward-only calls (grads == NULL) never run the head: probs_out and the forward workspace are those of the net
+ * without it.  Invalid configs: m outside 0..N-1, lambda not finite and > 0 with m > 0, and m > 0 with subsample >= 2
+ * at subsampleLayer = N + 1 (W_{N+1} then reads k H columns and cannot take X_m). */
 
 /* Frame subsampling (subsample = k >= 2; not in the reference; cf. Deep Speech 2's striding and the frame stacking of
  * pyramidal and low-frame-rate CTC models).  Affine map L = subsampleLayer reads k consecutive frames of layer L - 1
@@ -307,7 +334,7 @@ typedef struct ctcb_brnn ctcb_brnn; /* opaque; owns no device memory */
  * layerNorm = 1 appends [gamma_i, beta_i] of every normalised hidden layer i, in ascending i.
  * peephole = 1 then appends [P_f,j, dummy] [P_b,j, dummy] (unidirectional: [P_j, dummy]) of every temporal layer j in
  * ascending order, each P 3 x H. */
-/* maskFeatDim = nu > 0 adds no parameter, and neither do weightNoise = 1 and zoneout = 1. */
+/* maskFeatDim = nu > 0 adds no parameter, and neither do weightNoise = 1, zoneout = 1 and interLayer > 0. */
 int64_t ctcb_brnn_param_count(const ctcb_brnn_config *cfg);
 int ctcb_brnn_num_tensors(const ctcb_brnn_config *cfg);                    /* 2 * len(stack) */
 int ctcb_brnn_tensor_info(const ctcb_brnn_config *cfg, int idx, int64_t *offset, int32_t *rows, int32_t *cols);
@@ -335,7 +362,12 @@ int ctcb_brnn_tensor_info(const ctcb_brnn_config *cfg, int idx, int64_t *offset,
  * weightNoise = 1 appends, behind everything else, the noisy copy of the parameters: ctcb_brnn_param_count floats
  * rounded up to 256 bytes.  No other offset moves, and the forward workspace does not grow.
  * zoneout = 1 (with a temporal layer) appends, behind everything else, the BPTT sweep's dh carry: 2*maxB*layerSize
- * floats rounded up to 256 bytes.  No other offset moves, and the forward workspace does not grow. */
+ * floats rounded up to 256 bytes.  No other offset moves, and the forward workspace does not grow.
+ * interLayer = m >= 1 appends, behind everything else, with R_m = T_m maxB (T_m = maxT, or ceil(maxT / k) when
+ * m >= subsampleLayer), each area rounded up to 256 bytes: A and D_aux (R_m * outputDim floats each), the intermediate
+ * nll (maxB floats) and skips (maxB int32), and, only where the intermediate CTC runs on more frames than the main one
+ * (m < subsampleLayer with k >= 2), its own CTC area of ctcb_ctc_workspace_bytes(maxB, maxT, maxLabels) bytes; otherwise
+ * it shares the main CTC's area.  No other offset moves, and the forward workspace does not grow. */
 size_t ctcb_brnn_workspace_bytes(const ctcb_brnn_config *cfg);
 /* Byte offset, inside the workspace, of a uint32 that the recurrent-sweep kernels set non-zero when an
  * inter-CTA wait timed out (results are then invalid; never a hang).  Callers that synchronise anyway
@@ -366,7 +398,9 @@ size_t ctcb_brnn_forward_workspace_bytes(const ctcb_brnn_config *cfg, size_t *er
  * buffer that map's weight and bias gradients read, [T][B][rows] with rows its output width (G at an LSTM layer):
  * dz after layer normalisation, the gate gradients at an LSTM layer, the BPTT result at a uni-directional clipped-ReLU
  * temporal layer.  CTCB_EINVAL where a later stage of the call overwrites it: a uni-directional clipped-ReLU temporal
- * layer above the lowest two of its stack. */
+ * layer above the lowest two of its stack.  interLayer = m >= 1 only (`layer` is ignored): what = 8 the intermediate
+ * logits A, 9 D_aux = lambda d(nll_aux)/dA (both [T_m][B][outputDim]), 10 the intermediate nll (float32[B]), 11 its
+ * skips (int32[B]). */
 int ctcb_brnn_activation_offset(const ctcb_brnn_config *cfg, int what, int layer, size_t *offset, int32_t *width);
 
 /* With temporal layers, refuses (CTCB_EINVAL, with the planner's message) a config whose recurrent sweep the device
@@ -384,7 +418,9 @@ void ctcb_brnn_destroy(ctcb_brnn *h);
  *             brnnet.py:171-173; that mode needs only ctcb_brnn_forward_workspace_bytes of workspace)
  * stats_out : optional device float[4] = {number of non-skipped utterances, sum of their nll,
  *             number skipped, sweep error flag (see ctcb_brnn_error_flag_offset)}.  Callers place it directly behind the flat gradient so that the
- *             data-parallel all-reduce of the gradient carries it along.
+ *             data-parallel all-reduce of the gradient carries it along.  With interLayer > 0 it is float[6]: those
+ *             four, then the sum of the intermediate nll over the utterances its CTC kept and the number it skipped,
+ *             summed over micro-batches and ranks as the first four are.
  */
 int ctcb_brnn_cost_and_grad(ctcb_brnn *h, const float *feats, const int32_t *T_per_utt,
                             const int32_t *labels, const int32_t *label_off, int B, int Tmax,

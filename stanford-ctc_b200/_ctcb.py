@@ -31,7 +31,8 @@ class BrnnConfig(ctypes.Structure):
                 ("maxAct", ctypes.c_float), ("unidirectional", ctypes.c_int32), ("numTemporal", ctypes.c_int32),
                 ("cell", ctypes.c_int32), ("layerNorm", ctypes.c_int32), ("subsample", ctypes.c_int32),
                 ("subsampleLayer", ctypes.c_int32), ("peephole", ctypes.c_int32), ("maskFeatDim", ctypes.c_int32),
-                ("weightNoise", ctypes.c_int32), ("zoneout", ctypes.c_int32)]
+                ("weightNoise", ctypes.c_int32), ("zoneout", ctypes.c_int32), ("interLayer", ctypes.c_int32),
+                ("interWeight", ctypes.c_float)]
 
 
 _PROTOS = {

@@ -151,6 +151,27 @@ __global__ void batch_stats_kernel(const float *__restrict__ cost, const int32_t
     }
 }
 
+// the intermediate CTC's pair of the statistics tail: stats[0] += the sum of its nll over the utterances it kept,
+// stats[1] += the number it skipped (= with ACC false); one warp
+template <bool ACC>
+__global__ void inter_stats_kernel(const float *__restrict__ cost, const int32_t *__restrict__ skip, int B, float *stats) {
+    float cs = 0.f, ns = 0.f;
+    for (int u = threadIdx.x; u < B; u += 32) {
+        if (skip[u]) ns += 1.f;
+        else cs += cost[u];
+    }
+    cs = warp_sum(cs); ns = warp_sum(ns);
+    if (threadIdx.x == 0) {
+        if (ACC) { cs += stats[0]; ns += stats[1]; }
+        stats[0] = cs; stats[1] = ns;
+    }
+}
+
+// x[0..n) *= s in place (the intermediate loss's weight on its CTC gradient)
+__global__ void scale_kernel(float *__restrict__ x, int64_t n, float s) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+        x[i] *= s;
+}
 
 // The stage-1 grid of run_colsum: the wide kernel (n % 4 == 0 and a 16-byte aligned delta) over ncb column blocks of
 // bx threads and row blocks of rpb rows, or the narrow one over ncb blocks of 32 columns and row blocks of CS_ROWS rows
@@ -207,6 +228,20 @@ int run_batch_stats(const float *cost, const int32_t *skip, int B, float *stats,
                     bool accumulate, cudaStream_t st) {
     if (!accumulate) batch_stats_kernel<false><<<1, 32, 0, st>>>(cost, skip, B, stats, errflag);
     else batch_stats_kernel<true><<<1, 32, 0, st>>>(cost, skip, B, stats, errflag);
+    CTCB_LAUNCH_CHECK();
+    return CTCB_OK;
+}
+
+int run_inter_stats(const float *cost, const int32_t *skip, int B, float *stats, bool accumulate, cudaStream_t st) {
+    if (!accumulate) inter_stats_kernel<false><<<1, 32, 0, st>>>(cost, skip, B, stats);
+    else inter_stats_kernel<true><<<1, 32, 0, st>>>(cost, skip, B, stats);
+    CTCB_LAUNCH_CHECK();
+    return CTCB_OK;
+}
+
+int run_scale(float *x, int64_t n, float s, cudaStream_t st) {
+    const int64_t blocks = (n + 255) / 256;
+    scale_kernel<<<(unsigned)(blocks < 4 * num_sms() ? blocks : 4 * num_sms()), 256, 0, st>>>(x, n, s);
     CTCB_LAUNCH_CHECK();
     return CTCB_OK;
 }
@@ -269,6 +304,18 @@ static const char *cfg_error(const ctcb_brnn_config *c, char (&buf)[192]) {
         return say("zoneout %d is neither 0 (off) nor 1 (zoneout of the LSTM cell's state)", c->zoneout);
     if (c->zoneout == 1 && c->cell != 1)
         return say("zoneout 1 needs the LSTM cell (cell 1); cell is %d", c->cell);
+    if (c->interLayer != 0) {
+        if (c->interLayer < 1 || c->interLayer > c->numLayers - 1)
+            return say("interLayer %d is not one of the hidden layers 1..%d (numLayers - 1) an intermediate CTC loss "
+                       "can read (0: off)", c->interLayer, c->numLayers - 1);
+        if (!(c->interWeight > 0.f && c->interWeight <= 3.4028235e38f))
+            return say("interWeight %g of the intermediate CTC loss at layer %d is not a finite value > 0",
+                       (double)c->interWeight, c->interLayer);
+        if (c->subsample >= 2 && c->subsampleLayer == c->numLayers + 1)
+            return say("interLayer %d with subsample %d at subsampleLayer %d (numLayers + 1): the output map then "
+                       "reads %d stacked frames and cannot take one layer's output", c->interLayer, c->subsample,
+                       c->subsampleLayer, c->subsample);
+    }
     const bool ok = c->inputDim > 0 && c->outputDim > 1 && c->layerSize > 0 && c->numLayers >= 1 && c->numLayers <= 64 &&
                     c->maxT > 0 && c->maxB > 0 && c->maxLabels >= 0 && c->numTemporal >= 0 &&
                     // a stacked block must lie inside the hidden layers; k <= 1 keeps the silent "no temporal layer" rule below
@@ -469,6 +516,9 @@ struct WsLayout {
     size_t masked;      // maskFeatDim > 0 only (0 elsewhere): the masked copy of the call's features
     size_t noisy;       // weightNoise = 1 only (0 elsewhere): the noisy copy of the parameters
     size_t zo_dh;       // zoneout nets only (0 elsewhere): the BPTT sweep's dh carry
+    // interLayer > 0 only (0 elsewhere): the intermediate logits A and D_aux, its nll and skips, and the CTC area it
+    // uses (the main one's, unless it runs on more frames)
+    size_t inter_A, inter_D, inter_nll, inter_skip, inter_ctc, inter_ctc_bytes;
     size_t total;
 };
 
@@ -563,6 +613,17 @@ WsLayout ws_layout(const ctcb_brnn_config *c) {
         w.noisy = take(off, (size_t)ctcb_brnn_param_count(c) * sizeof(float));
     if (c->zoneout == 1 && nt)
         w.zo_dh = take(off, lstm_carry_bytes(H, c->maxB));
+    if (c->interLayer > 0) {
+        const size_t Rm = max_rows(c, c->interLayer), K = (size_t)c->outputDim;
+        w.inter_A = take(off, Rm * K * sizeof(float));
+        w.inter_D = take(off, Rm * K * sizeof(float));
+        w.inter_nll = take(off, (size_t)c->maxB * sizeof(float));
+        w.inter_skip = take(off, (size_t)c->maxB * sizeof(int32_t));
+        w.inter_ctc = w.ctc;
+        w.inter_ctc_bytes = w.ctc_bytes;
+        if (Rm > max_rows(c, N + 1))     // below the subsampling point: maxT frames, the main CTC has fewer
+            w.inter_ctc = take(off, ctcb_ctc_workspace_bytes(c->maxB, c->maxT, c->maxLabels), &w.inter_ctc_bytes);
+    }
     w.total = off;
     return w;
 }
@@ -756,6 +817,8 @@ struct ctcb_brnn {
 
     bool uni() const { return cfg.unidirectional != 0; }
     bool lstm() const { return cfg.cell == 1; }
+    int inter() const { return cfg.interLayer; }     // the layer of the intermediate CTC loss, 0 without
+    int stats_floats() const { return inter() ? 6 : 4; }     // of stats_out
     bool peep() const { return cfg.peephole == 1; }
     int peep_idx(int j) const { return peep_index(&cfg, j); }
     bool temporal(int i) const { return nt > 0 && i >= tl && i < tl + nt; }
@@ -888,8 +951,9 @@ static int brnn_reduce_rest(ctcb_brnn *h, float *grads, float *stats, cudaStream
     int k = 0;
     ptrs[k] = grads; cnt[k] = lo; ++k;
     const bool tail_adjacent = (stats == grads + P);
-    ptrs[k] = grads + hi; cnt[k] = P - hi + (stats && tail_adjacent ? 4 : 0); ++k;
-    if (stats && !tail_adjacent) { ptrs[k] = stats; cnt[k] = 4; ++k; }
+    const int ns = h->stats_floats();
+    ptrs[k] = grads + hi; cnt[k] = P - hi + (stats && tail_adjacent ? ns : 0); ++k;
+    if (stats && !tail_adjacent) { ptrs[k] = stats; cnt[k] = ns; ++k; }
     return comm_allreduce_ranges(h->comm, ptrs, cnt, k, st);
 }
 
@@ -1028,6 +1092,16 @@ int Step::weight_grads(int i, bool on_side) const {
     ProfScope ps("colsum", st);
     TRY(run_colsum(delta(i), R(i + 1), n_out, buf(on_side ? w.colsum2 : w.colsum), G(2 * i + 1), !first, st));
     }
+    // the intermediate loss's share of W_{N+1} and b_{N+1}: added behind the main one on the same stream, so ahead of
+    // the early exchange, whose range holds them.  The side stream gets here behind ev_delta, which main records after
+    // the intermediate CTC.
+    if (i == h->cfg.numLayers && h->inter()) {
+        const int mi = h->inter(), K = h->cfg.outputDim, H = h->cfg.layerSize;
+        ProfScope ps("inter_ctc_dw", st);
+        TRY(ctcb_gemm_f32(1, 0, K, H, (int)R(mi), 1.f, buf(w.inter_D), K, h->act(m, mi), H, 1.f, G(2 * i), H, nullptr,
+                          0, nullptr, on_side ? ws + w.gemm2 : m.gemm, on_side ? w.gemm2_bytes : m.gemm_bytes, st));
+        TRY(run_colsum(buf(w.inter_D), R(mi), K, buf(on_side ? w.colsum2 : w.colsum), G(2 * i + 1), true, st));
+    }
     if (h->uni() && h->temporal(i + 1) && !h->lstm() && i + 1 - h->tl >= 2)  // the last read of the pair of uni-directional layer i + 1
         CTCB_CUDA_CHECK(cudaEventRecord(h->ev_pair[(i + 1 - h->tl) % 2], side));
     // every gradient tensor of the layers >= tl is now queued on the side stream: sum that contiguous range over
@@ -1121,6 +1195,12 @@ int Step::backward() const {
         if (stacked) {
             ProfScope ps("subsample", main);
             TRY(run_frame_unstack(buf(w.dS), T_per_utt, T(i), B, n, h->k(), doth, main));
+        }
+        if (i == h->inter()) {     // + D_aux W_{N+1}, at layer i's own rate, under the same mask and alpha
+            ProfScope ps("inter_ctc_delta", main);
+            TRY(ctcb_gemm_f32(0, 0, (int)R, n, h->cfg.outputDim, alpha, buf(w.inter_D), h->cfg.outputDim, P(2 * N), n,
+                              1.f, doth, n, nullptr, 0, h->temporal(i) ? nullptr : h->act(m, i), m.gemm, m.gemm_bytes,
+                              main));
         }
         if (h->normed(i)) {     // g -> dz in place, before anything reads D[i]; dgamma / dbeta of the layer
             const int ig = ln_index(&h->cfg, i);
@@ -1268,9 +1348,24 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
     TRY(ctcb_ctc_loss_grad_f32(m.X[N + 1], 0, (int64_t)K, (int64_t)B * K, labels, label_off, s.lens(N + 1), B, s.T(N + 1), K,
                                c.maxLabels, 0, s.buf(w.D[N + 1]), cost_out, skip_out, ws + w.ctc, w.ctc_bytes, s.main));
     }
+    float *inter_nll = h->inter() ? s.buf(w.inter_nll) : nullptr;
+    int32_t *inter_skip = h->inter() ? (int32_t *)(ws + w.inter_skip) : nullptr;
+    if (h->inter()) {     // A = X_m W_{N+1}^T + b_{N+1}, its CTC, and D_aux = lambda dnll/dA scaled in place: the two
+                          // contractions and the column sums of the backward pass then read the same values
+        const int mi = h->inter(), H = c.layerSize;
+        float *A = s.buf(w.inter_A), *Da = s.buf(w.inter_D);
+        ProfScope ps("inter_ctc", s.main);
+        TRY(ctcb_gemm_f32(0, 1, (int)s.R(mi), K, H, 1.f, h->act(m, mi), H, s.P(2 * N), H, 0.f, A, K, s.P(2 * N + 1), 0,
+                          nullptr, m.gemm, m.gemm_bytes, s.main));
+        TRY(ctcb_ctc_loss_grad_f32(A, 0, (int64_t)K, (int64_t)B * K, labels, label_off, s.lens(mi), B, s.T(mi), K,
+                                   c.maxLabels, 0, Da, inter_nll, inter_skip, ws + w.inter_ctc, w.inter_ctc_bytes,
+                                   s.main));
+        TRY(run_scale(Da, s.R(mi) * K, c.interWeight, s.main));
+    }
     TRY(s.backward());
     if (stats_out)     // after both sweeps, so that the tail carries the error flag of either
         TRY(run_batch_stats(cost_out, skip_out, B, stats_out, m.counters, !first, s.main));
+    if (stats_out && h->inter()) TRY(run_inter_stats(inter_nll, inter_skip, B, stats_out + 4, !first, s.main));
     if (overlap) {     // join: every gradient tensor is complete on the caller's stream from here on
         CTCB_CUDA_CHECK(cudaEventRecord(h->ev_side, h->side));
         CTCB_CUDA_CHECK(cudaEventRecord(h->ev_hi, h->hi));
@@ -1459,9 +1554,18 @@ extern "C" int ctcb_softmax_rows_f32(const float *x, float *p, int64_t R, int K,
 // several, `layer` says which, and only a bi-directional stack has a Back of every layer).  Subsampled nets: entries of
 // maps >= L are [Tmax'][B][n]; what = 6: S, the stacked input of map L, k n wide.  what = 7: the delta of map `layer`,
 // the buffer its weight and bias gradients read (Step::delta), where no later stage of the call overwrites it.
+// what = 8..11 (interLayer > 0): the intermediate logits A, D_aux, the intermediate nll and skips.
 extern "C" int ctcb_brnn_activation_offset(const ctcb_brnn_config *cfg, int what, int layer, size_t *offset, int32_t *width) {
     if (!valid_cfg(cfg) || !offset) return set_error(CTCB_EINVAL, "ctcb_brnn_activation_offset: bad arguments");
     const WsLayout w = ws_layout(cfg);
+    if (what >= 8 && what <= 11) {     // the intermediate CTC loss: A, D_aux, nll, skips
+        if (cfg->interLayer <= 0)
+            return set_error(CTCB_EINVAL, "ctcb_brnn_activation_offset: nothing of kind %d without interLayer", what);
+        const size_t at[4] = {w.inter_A, w.inter_D, w.inter_nll, w.inter_skip};
+        *offset = at[what - 8];
+        if (width) *width = what <= 9 ? cfg->outputDim : 1;
+        return CTCB_OK;
+    }
     if (what == 7) {
         if (layer < 1 || layer > cfg->numLayers + 1)
             return set_error(CTCB_EINVAL, "ctcb_brnn_activation_offset: layer %d", layer);

@@ -48,6 +48,12 @@ single contiguous vector.  New, additive surface for the minibatch/data-parallel
                                                 zh, drawn from (seed dropoutSeed, the counter dropoutStep, the
                                                 utterance's index, the frame, the layer, the unit); forward-only calls
                                                 use the expectation, so a net for testing needs the trained values
+    NNet(..., interLayer=m, interWeight=lam) an intermediate CTC loss (include/ctcb200.h: interLayer): hidden layer m's
+                                                output through the net's own output map W_{N+1}, b_{N+1}, scored by a
+                                                second CTC; training calls differentiate main + lam * that loss, and
+                                                costAndGrad returns it.  No parameter is added and forward-only calls do
+                                                not change; interCosts / interSkips hold the last batch's per-utterance
+                                                intermediate nll and skips
     costAndGradBatch(datas, labelss)         -> (costs[B], grad, skips[B])   host arrays in; more than maxUtts
                                                 utterances are accumulated over micro-batches
     costAndGradDevice(batch, first, last)    -> no host sync; see DeviceBatch
@@ -187,7 +193,14 @@ class NNet:
                  allowTopTemporal=False, device=None, unidirectional=False, numTemporal=1, dropout=0.0,
                  dropoutSeed=33, cell="relu", layerNorm=False, subsample=1, subsampleLayer=1, peephole=False,
                  freqMasks=0, freqMaskWidth=0, timeMasks=0, timeMaskWidth=0, timeMaskRatio=1.0, featDim=None,
-                 weightNoise=0.0, zoneoutCell=0.0, zoneoutHidden=0.0):
+                 weightNoise=0.0, zoneoutCell=0.0, zoneoutHidden=0.0, interLayer=0, interWeight=0.0):
+        # The intermediate CTC loss (include/ctcb200.h: interLayer).  The library refuses a layer outside
+        # 1..numLayers-1 and a subsampled output map, with its message; a layer and a weight come only together.
+        self.interLayer, self.interWeight = int(interLayer), float(interWeight)
+        if self.interLayer != 0 and not (np.isfinite(self.interWeight) and self.interWeight > 0.0):
+            raise ValueError("interLayer=%d needs a finite interWeight > 0; interWeight is %r" % (interLayer, interWeight))
+        if self.interLayer == 0 and self.interWeight != 0.0:
+            raise ValueError("interWeight=%r weighs the intermediate CTC loss; it needs interLayer >= 1" % (interWeight,))
         torch = _ctcb.require_cuda()
         self._torch = torch
         self.dev = torch.device("cuda", torch.cuda.current_device() if device is None else device)
@@ -265,7 +278,7 @@ class NNet:
                                maxUtts, self.maxLabels, float(reg), float(self.maxAct), int(self.unidirectional),
                                self.numTemporal, _ctcb.CELLS[cell], int(self.layerNorm), self.subsample,
                                self.subsampleLayer, int(self.peephole), self.featDim or 0,
-                               int(self.weightNoise > 0.0), int(self.zoneout))
+                               int(self.weightNoise > 0.0), int(self.zoneout), self.interLayer, self.interWeight)
         self._h = ctypes.c_void_p()
         check(lib.ctcb_brnn_create(ctypes.byref(self._cfg), ctypes.byref(self._h)))
         self.stack = None
@@ -347,15 +360,20 @@ class NNet:
         for (w, b), (hw, hb) in zip(self.stack, host):
             w.copy_(torch.from_numpy(hw.astype(np.float32)))
             b.copy_(torch.from_numpy(hb.astype(np.float32)))
+        # the floats of the statistics tail: 4, and 6 with the intermediate CTC loss (its nll sum and skip count)
+        self.statsFloats = 6 if self.interLayer else 4
         if self.train:
             # flat gradient + a 4-float tail {n_valid, sum nll, n_skipped, sweep error flag} that rides along in the
             # data-parallel all-reduce (see include/ctcb200.h: stats_out), + 4 local floats {gnorm^2, regcost, -, -}:
-            # the 8 floats behind the gradient are the step's log record, read back with ONE 32-byte copy
+            # the 8 floats behind the gradient are the step's log record, read back with ONE 32-byte copy.  With the
+            # intermediate CTC loss the tail has its two floats too and the record is
+            # {n_valid, sum nll, n_skipped, flag, sum intermediate nll, n_skipped by it, gnorm^2, regcost}.
+            ns = self.statsFloats
             self.grads_ext = torch.zeros(self.nparams + 8, dtype=torch.float32, device=self.dev)
             self.grads = self.grads_ext[:self.nparams]
-            self.stats = self.grads_ext[self.nparams:self.nparams + 4]
+            self.stats = self.grads_ext[self.nparams:self.nparams + ns]
             self.record = self.grads_ext[self.nparams:self.nparams + 8]
-            self._gnorm2 = self.grads_ext[self.nparams + 4:self.nparams + 5]
+            self._gnorm2 = self.grads_ext[self.nparams + ns:self.nparams + ns + 1]
             self.grad = self._views(self.grads)
         else:
             self.grads = None
@@ -377,7 +395,7 @@ class NNet:
         self._cost = self._out[:self.maxUtts]
         self._skip = self._out[self.maxUtts:].view(torch.int32)
         if self.train:
-            self._regcost = self.grads_ext[self.nparams + 5:self.nparams + 6]
+            self._regcost = self.grads_ext[self.nparams + self.statsFloats + 1:self.nparams + self.statsFloats + 2]
         else:
             self._regcost = torch.zeros(1, dtype=torch.float32, device=self.dev)
         self._out_host = torch.zeros(2 * self.maxUtts, dtype=torch.float32).pin_memory()
@@ -385,6 +403,14 @@ class NNet:
         self._rec_host = torch.zeros(8, dtype=torch.float32).pin_memory()
         self._probs = None
         self._comm = None
+        self.interCosts = self.interSkips = None      # the intermediate nll and skips of the last costAndGradBatch
+        self._inter_all = None      # their device copies, for a step of several micro-batches
+        if self.interLayer and self.train:
+            off = ctypes.c_size_t()
+            check(lib.ctcb_brnn_activation_offset(ctypes.byref(self._cfg), 10, 0, ctypes.byref(off), None))
+            self._inter_nll = self._ws[off.value:off.value + 4 * self.maxUtts].view(torch.float32)
+            check(lib.ctcb_brnn_activation_offset(ctypes.byref(self._cfg), 11, 0, ctypes.byref(off), None))
+            self._inter_skip = self._ws[off.value:off.value + 4 * self.maxUtts].view(torch.float32)
 
     def swap_batches(self):
         """Double buffering of the staging area: returns the buffer that is NOT the current one and makes it
@@ -478,11 +504,13 @@ class NNet:
             return self._cost_and_grad_accumulated(datas, labelss)
         self._batch.pack(datas, labelss).upload()
         self.costAndGradDevice(self._batch)
+        self._keep_inter(B, 0, B)
         # two pinned D2H copies on the stream (no kernels, no allocation), one synchronisation
         self._out_host.copy_(self._out, non_blocking=True)
         self._rec_host.copy_(self.record, non_blocking=True)
         self._torch.cuda.current_stream().synchronize()
         self._read_record()
+        self._read_inter(B)
         out = self._out_host.numpy()
         costs = out[:B].astype(np.float64)
         skips = out[self.maxUtts:self.maxUtts + B].view(np.int32) != 0
@@ -492,7 +520,25 @@ class NNet:
         rec = self._rec_host.numpy()
         if rec[3] != 0:
             raise RuntimeError("recurrent sweep: inter-CTA wait timed out (flag %d); results are invalid" % int(rec[3]))
-        self.regcost = float(rec[5])
+        self.regcost = float(rec[self.statsFloats + 1])
+
+    def _keep_inter(self, B, u0, n):
+        """With the intermediate CTC loss: enqueue the copy of the last call's n intermediate nll and skips to
+        positions u0.. of the step's B (the workspace holds one call's only)."""
+        if not self.interLayer:
+            return
+        torch = self._torch
+        if self._inter_all is None or self._inter_all.numel() < 2 * B:
+            self._inter_all = torch.zeros(2 * B, dtype=torch.float32, device=self.dev)
+        self._inter_all[u0:u0 + n].copy_(self._inter_nll[:n])
+        self._inter_all[B + u0:B + u0 + n].copy_(self._inter_skip[:n])
+
+    def _read_inter(self, B):
+        if not self.interLayer:
+            return
+        out = self._inter_all[:2 * B].cpu().numpy()
+        self.interCosts = out[:B].astype(np.float64)
+        self.interSkips = out[B:2 * B].view(np.int32) != 0
 
     def _cost_and_grad_accumulated(self, datas, labelss):
         torch = self._torch
@@ -512,12 +558,14 @@ class NNet:
             n = len(idx)
             self.costAndGradDevice(batch, first=(k == 0), last=(k == len(pieces) - 1),
                                    out=(cost_all[u0:u0 + n], skip_all[u0:u0 + n]), u0=u0)
+            self._keep_inter(B, u0, n)
             u0 += n
         host = self._out_all_host[:2 * B]
         host.copy_(self._out_all[:2 * B], non_blocking=True)
         self._rec_host.copy_(self.record, non_blocking=True)
         torch.cuda.current_stream().synchronize()
         self._read_record()
+        self._read_inter(B)
         out = host.numpy()
         costs = out[:B].astype(np.float64)
         skips = out[B:2 * B].view(np.int32) != 0
@@ -525,7 +573,9 @@ class NNet:
 
     def costAndGrad(self, data, labels=None, sentence=None):
         """Reference signature (brnnet.py:117): data is inputDim x T float32; returns (cost, grad, skip)
-        when training, else the K x T float32 softmax outputs (K x ceil(T / k) with subsample=k)."""
+        when training, else the K x T float32 softmax outputs (K x ceil(T / k) with subsample=k).  With the
+        intermediate CTC loss the cost is the objective the gradient is of, main + interWeight * intermediate nll
+        (the latter left out where its CTC skips); skip is the main CTC's."""
         T = data.shape[1]
         self.setViews(T)
         if not self.train:
@@ -538,6 +588,8 @@ class NNet:
             return out
         costs, grad, skips = self.costAndGradBatch([data], [labels])
         cost = float(costs[0])
+        if self.interLayer and not self.interSkips[0]:      # the objective the gradient is of
+            cost = cost + float(np.float32(self.interWeight)) * float(self.interCosts[0])
         if self.reg > 0:
             cost = cost + self.regcost          # brnnet.py:177-183
         return cost, grad, bool(skips[0])

@@ -9,7 +9,7 @@ The implementation is organised differently: a declarative flag table, one RunDi
 side files, and separate train/evaluate phases.  Site paths of run_cfg.py / decoder_config.py became
 flags (--runDir, --outDir); new flags: --numTemporal, --cell, --peephole, --layerNorm, --subsample, --subsampleLayer, --batchSize, --maxUtts, --maxLabels,
 --dropout, --freqMasks, --freqMaskWidth, --timeMasks, --timeMaskWidth, --timeMaskRatio, --featDim, --weightNoise,
---zoneoutCell, --zoneoutHidden,
+--zoneoutCell, --zoneoutHidden, --interLayer, --interWeight,
 --optimizer,
 --beta1, --beta2, --epsilon, --quiet.  Under torchrun the same
 script trains data-parallel (one process per GPU, one NCCL all-reduce per step).
@@ -82,6 +82,11 @@ FLAGS = [
                                 "0 = off; --test runs the expectation cell with the trained value; a cfg.json "
                                 "written without it has none)"),
     ("zoneoutHidden", float, 0.0, "zoneout probability of the LSTM output h, as --zoneoutCell"),
+    ("interLayer", int, 0, "intermediate CTC loss while training: hidden layer m (1..numLayers-1) through the output "
+                           "map, scored against the same labels (0 = off; --test ignores it; a cfg.json written "
+                           "without it has none)"),
+    ("interWeight", float, 0.0, "lambda of the intermediate CTC loss: the objective is main + lambda * intermediate "
+                                "(Lee & Watanabe's weight w is lambda = w / (1 - w) at (1 - w) times the step size)"),
     ("optimizer", str, "nesterov", "update rule: nesterov (the reference's, with --momentum), adagrad or adam; --step "
                                    "is the step size of each and --anneal applies to it"),
     ("beta1", float, 0.9, "adam: decay of the first-moment estimate"),
@@ -231,7 +236,7 @@ def _train(opts, cfg, run_dir, log, rank, world):
                      peephole=opts.peephole, freqMasks=opts.freqMasks, freqMaskWidth=opts.freqMaskWidth,
                      timeMasks=opts.timeMasks, timeMaskWidth=opts.timeMaskWidth, timeMaskRatio=opts.timeMaskRatio,
                      featDim=opts.featDim, weightNoise=opts.weightNoise, zoneoutCell=opts.zoneoutCell,
-                     zoneoutHidden=opts.zoneoutHidden)
+                     zoneoutHidden=opts.zoneoutHidden, interLayer=opts.interLayer, interWeight=opts.interWeight)
     net.initParams()
     optimizer = sgd.SGD(net, opts.maxUttLen, alpha=opts.step, optimizer=opts.optimizer, momentum=opts.momentum,
                         batchSize=opts.batchSize, verbose=(rank == 0 and not opts.quiet), beta1=opts.beta1,

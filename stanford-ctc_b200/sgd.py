@@ -105,7 +105,8 @@ class SGD:
             self._step = torch.zeros(1, dtype=torch.int64, device=model.dev)
         self._gnorm2 = model._gnorm2          # lives in the 8-float record behind the flat gradient
         self._scratch = torch.zeros(8192, dtype=torch.uint8, device=model.dev)
-        # per-step log record {n_valid, sum nll, n_skipped, sweep error flag, gnorm^2, regcost, -, -}: the 8 floats behind
+        # per-step log record {n_valid, sum nll, n_skipped, sweep error flag, gnorm^2, regcost, -, -} (with the
+        # intermediate CTC loss its two sums sit before gnorm^2: nnets.brnnet.NNet.statsFloats): the 8 floats behind
         # the flat gradient, copied to pinned host memory on the stream right behind the step (one 32-byte D2H copy,
         # no kernel) and read one step later (two slots alternate)
         self._log_host = [torch.zeros(8, dtype=torch.float32).pin_memory() for _ in range(2)]
@@ -317,8 +318,9 @@ class SGD:
         if host[3] != 0:       # summed over ranks with the rest of the tail: every rank raises together
             raise RuntimeError("recurrent sweep: inter-CTA wait timed out (flag %d); results are invalid" % int(host[3]))
         nvalid, costsum = float(host[0]), float(host[1])
-        gnorm = float(np.sqrt(host[4]))
-        m.regcost = float(host[5])
+        ns = getattr(m, "statsFloats", 4)        # the tail's floats; gnorm^2 and regcost follow it
+        gnorm = float(np.sqrt(host[ns]))
+        m.regcost = float(host[ns + 1])
         if nvalid == 0:
             logging.info("SKIPPING: Keys=%s" % (",".join(str(k) for k in prep["used"])))
             return
@@ -337,8 +339,14 @@ class SGD:
                 else:
                     self.regcost.append(rc)
         if self.verbose and rank == 0:
-            print("Iter %d : Cost=%.4f, ExpCost=%.4f, GradNorm=%.4f, SeqLen=%d, NumFrames=%d."
-                  % (prep["it"], cost, self.expcost[-1] if self.expcost else float('nan'), gnorm,
+            # with the intermediate CTC loss: its mean nll over the utterances its CTC kept (not in ExpCost, which
+            # stays the main CTC's so that runs with and without it compare)
+            inter = ""
+            if ns == 6:
+                kept = float(host[0]) + float(host[2]) - float(host[5])
+                inter = ", InterCost=%.4f" % (float(host[4]) / kept if kept > 0 else float("nan"))
+            print("Iter %d : Cost=%.4f%s, ExpCost=%.4f, GradNorm=%.4f, SeqLen=%d, NumFrames=%d."
+                  % (prep["it"], cost, inter, self.expcost[-1] if self.expcost else float('nan'), gnorm,
                      prep["nlab"], prep["nframes"]))
 
     def run(self, data_dict, alis, keys, sizes):
