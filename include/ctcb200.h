@@ -210,6 +210,9 @@ typedef struct ctcb_brnn_config {
                             * makes the config invalid. */
     float interWeight;     /* lambda of the intermediate CTC loss: ignored with interLayer = 0; with interLayer > 0 a
                             * value that is not finite and > 0 makes the config invalid. */
+    int32_t selfCondition; /* 0: off (so an initialiser without this member keeps its meaning); 1: self-conditioned CTC
+                            * (below), which needs interLayer >= 1; any other value, or 1 with interLayer = 0, makes the
+                            * config invalid. */
 } ctcb_brnn_config;
 
 /* Intermediate CTC loss (interLayer = m >= 1; not in the reference; Lee & Watanabe, "Intermediate Loss Regularization
@@ -230,9 +233,27 @@ typedef struct ctcb_brnn_config {
  *   stacked frames: the term is at layer m's own rate).
  *   Each CTC skips on its own: an utterance the intermediate CTC skips gets no gradient from it and adds nothing to its
  *   sums.  cost_out, skip_out and the first four floats of stats_out keep their meaning (the main CTC's).
- * Forward-only calls (grads == NULL) never run the head: probs_out and the forward workspace are those of the net
- * without it.  Invalid configs: m outside 0..N-1, lambda not finite and > 0 with m > 0, and m > 0 with subsample >= 2
- * at subsampleLayer = N + 1 (W_{N+1} then reads k H columns and cannot take X_m). */
+ * Forward-only calls (grads == NULL) never run the head, unless selfCondition = 1 (below): probs_out and the forward
+ * workspace are those of the net without it.  Invalid configs: m outside 0..N-1, lambda not finite and > 0 with m > 0, and m > 0 with subsample >= 2
+ * at subsampleLayer = N + 1 (W_{N+1} then reads k H columns and cannot take X_m).
+ *
+ * Self-conditioned CTC (selfCondition = 1 with interLayer = m; not in the reference; Nozaki & Komatsu, "Relaxing the
+ * Conditional Independence Assumption of CTC-based ASR by Conditioning on Intermediate Predictions", Interspeech 2021;
+ * ESPnet's interctc_use_conditioning).  H = layerSize.  The intermediate posteriors are projected back to the layer's
+ * width and added to its output, so the layers above condition on a first guess at the labels.  Parameters W_c (H x K)
+ * and b_c (H), behind every other tensor of the flat vector (below).
+ *   Forward (training and forward-only calls): A = X_m W_{N+1}^T + b_{N+1} (as above); P = softmax(A) per row (float32,
+ *   the row-softmax kernel); X'_m = X_m + P W_c^T + b_c.  Map m + 1 reads X'_m in place of X_m, and so does the frame
+ *   stacking when m + 1 = subsampleLayer.  The intermediate CTC still scores A.  X_m keeps every other role: the ReLU
+ *   and dropout mask of layer m's delta and the head's input.  A training call writes X'_m into a buffer of its own,
+ *   a forward-only call over X_m in place, with the same launches and plans, so probs_out stays bit-identical.
+ *   Backward: D'_m = dL/dX'_m is the delta contraction of map m + 1 (after any unstacking), without the mask and with
+ *   alpha = 1.  dP = D'_m W_c; dA = P (dP - sum_k P_k dP_k) + D_aux (ctcb_softmax_rows_backward_f32); dW_c = D'_m^T P,
+ *   db_c = the column sums of D'_m; dW_{N+1} += dA^T X_m and db_{N+1} += the column sums of dA (in place of the D_aux
+ *   term above); the delta of layer m is alpha [X_m > 0] (D'_m + dA W_{N+1}), the mask and alpha at a ReLU layer only,
+ *   and layer normalisation's backward or the BPTT sweep read it as they read the delta without conditioning.
+ *   W_c and b_c start at 0 (a new net is the InterCTC net), are not L2-regularised and get no weight noise.  The
+ *   objective is still nll_main + lambda nll_aux. */
 
 /* Frame subsampling (subsample = k >= 2; not in the reference; cf. Deep Speech 2's striding and the frame stacking of
  * pyramidal and low-frame-rate CTC models).  Affine map L = subsampleLayer reads k consecutive frames of layer L - 1
@@ -333,7 +354,9 @@ typedef struct ctcb_brnn ctcb_brnn; /* opaque; owns no device memory */
  * [Wtf_j,dummy] [Wtb_j,dummy] (unidirectional: [Wt_j,dummy]); for k = 1 this is the layout above.
  * layerNorm = 1 appends [gamma_i, beta_i] of every normalised hidden layer i, in ascending i.
  * peephole = 1 then appends [P_f,j, dummy] [P_b,j, dummy] (unidirectional: [P_j, dummy]) of every temporal layer j in
- * ascending order, each P 3 x H. */
+ * ascending order, each P 3 x H.
+ * selfCondition = 1 then appends [W_c, b_c], W_c layerSize x outputDim and b_c layerSize x 1, behind everything else;
+ * like [gamma, beta] and P they lie behind the range L2 regularisation and weight noise see. */
 /* maskFeatDim = nu > 0 adds no parameter, and neither do weightNoise = 1, zoneout = 1 and interLayer > 0. */
 int64_t ctcb_brnn_param_count(const ctcb_brnn_config *cfg);
 int ctcb_brnn_num_tensors(const ctcb_brnn_config *cfg);                    /* 2 * len(stack) */
@@ -367,7 +390,12 @@ int ctcb_brnn_tensor_info(const ctcb_brnn_config *cfg, int idx, int64_t *offset,
  * m >= subsampleLayer), each area rounded up to 256 bytes: A and D_aux (R_m * outputDim floats each), the intermediate
  * nll (maxB floats) and skips (maxB int32), and, only where the intermediate CTC runs on more frames than the main one
  * (m < subsampleLayer with k >= 2), its own CTC area of ctcb_ctc_workspace_bytes(maxB, maxT, maxLabels) bytes; otherwise
- * it shares the main CTC's area.  No other offset moves, and the forward workspace does not grow. */
+ * it shares the main CTC's area.  No other offset moves, and the forward workspace does not grow.
+ * selfCondition = 1 appends, behind those, X'_m (R_m * layerSize floats), P and dA (R_m * outputDim floats each), each
+ * rounded up to 256 bytes.  No other offset moves, except that with weightNoise = 1 the noisy copy holds W_c and b_c
+ * too (it is ctcb_brnn_param_count floats) and what lies behind it moves by as much.  The forward workspace appends A and P (R_m * outputDim floats each,
+ * rounded up to 256 bytes), and its split-K area also covers the A and conditioning contractions at every R <= R_m
+ * (within the training area), so that they take the plans of a training call. */
 size_t ctcb_brnn_workspace_bytes(const ctcb_brnn_config *cfg);
 /* Byte offset, inside the workspace, of a uint32 that the recurrent-sweep kernels set non-zero when an
  * inter-CTA wait timed out (results are then invalid; never a hang).  Callers that synchronise anyway
@@ -400,7 +428,8 @@ size_t ctcb_brnn_forward_workspace_bytes(const ctcb_brnn_config *cfg, size_t *er
  * temporal layer.  CTCB_EINVAL where a later stage of the call overwrites it: a uni-directional clipped-ReLU temporal
  * layer above the lowest two of its stack.  interLayer = m >= 1 only (`layer` is ignored): what = 8 the intermediate
  * logits A, 9 D_aux = lambda d(nll_aux)/dA (both [T_m][B][outputDim]), 10 the intermediate nll (float32[B]), 11 its
- * skips (int32[B]). */
+ * skips (int32[B]).  selfCondition = 1 only (`layer` is ignored): what = 12 X'_m (layerSize wide), 13 P, 14 dA (both
+ * outputDim wide), all [T_m][B][width]. */
 int ctcb_brnn_activation_offset(const ctcb_brnn_config *cfg, int what, int layer, size_t *offset, int32_t *width);
 
 /* With temporal layers, refuses (CTCB_EINVAL, with the planner's message) a config whose recurrent sweep the device
@@ -585,12 +614,17 @@ int ctcb_layernorm_backward_f32(float *delta, const float *z, const float *mu, c
  *          float4 column group, 4 rows per loop step) / 0 narrow (8 strided threads per column), column blocks,
  *          rows per block (wide: R / (2 SMs / column blocks) within [128, 1024]; narrow: 1024), row blocks}.
  * softmax_rows: p = softmax of each row of the row-major R x K matrix x, the forward-only probabilities of a
- *          ctcb_brnn_cost_and_grad call (probs_out); one warp per row. */
+ *          ctcb_brnn_cost_and_grad call (probs_out); one warp per row.
+ * softmax_rows_backward: out = p (dp - sum_k p_k dp_k) + add per row of the row-major R x K matrices, the gradient of a
+ *          row softmax p with respect to its logits given dp = dL/dp, plus add (may be NULL); out may alias dp.  The
+ *          dA of self-conditioned CTC (selfCondition, above); one warp per row.  Argument checks as softmax_rows. */
 size_t ctcb_colsum_workspace_bytes(int64_t R, int n);
 int ctcb_colsum_f32(const float *delta, int64_t R, int n, float *out, int accumulate, void *workspace, size_t ws_bytes,
                     void *stream);
 int ctcb_debug_colsum_plan(int64_t R, int n, const float *delta, int32_t *out);
 int ctcb_softmax_rows_f32(const float *x, float *p, int64_t R, int K, void *stream);
+int ctcb_softmax_rows_backward_f32(const float *p, const float *dp, const float *add, float *out, int64_t R, int K,
+                                   void *stream);
 
 /* ---- frame stacking on its own (subsample = k, above) ----------------------------------------------------------
  * x / d_out are time-major [Tmax][B][n], s_out / ds [ceil(Tmax / k)][B][k n], T_per_utt int32[B] (<= Tmax).

@@ -32,7 +32,7 @@ class BrnnConfig(ctypes.Structure):
                 ("cell", ctypes.c_int32), ("layerNorm", ctypes.c_int32), ("subsample", ctypes.c_int32),
                 ("subsampleLayer", ctypes.c_int32), ("peephole", ctypes.c_int32), ("maskFeatDim", ctypes.c_int32),
                 ("weightNoise", ctypes.c_int32), ("zoneout", ctypes.c_int32), ("interLayer", ctypes.c_int32),
-                ("interWeight", ctypes.c_float)]
+                ("interWeight", ctypes.c_float), ("selfCondition", ctypes.c_int32)]
 
 
 _PROTOS = {
@@ -103,6 +103,7 @@ _PROTOS = {
     "ctcb_colsum_f32": (c_int, [c_vp, c_i64, c_int, c_vp, c_int, c_vp, c_sz, c_vp]),
     "ctcb_debug_colsum_plan": (c_int, [c_i64, c_int, c_vp, ctypes.POINTER(ctypes.c_int32)]),
     "ctcb_softmax_rows_f32": (c_int, [c_vp, c_vp, c_i64, c_int, c_vp]),
+    "ctcb_softmax_rows_backward_f32": (c_int, [c_vp, c_vp, c_vp, c_vp, c_i64, c_int, c_vp]),
     "ctcb_frame_stack_f32": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp]),
     "ctcb_frame_unstack_f32": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp]),
     "ctcb_debug_sweep_plan": (c_int, [c_int, c_int, c_int, ctypes.POINTER(ctypes.c_int32)]),

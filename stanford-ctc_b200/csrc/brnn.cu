@@ -130,6 +130,23 @@ __global__ void softmax_rows_kernel(const float *__restrict__ x, float *__restri
     for (int k = lane; k < K; k += 32) p[row * K + k] = expf(xr[k] - m) * inv;
 }
 
+// out = p (dp - sum_k p_k dp_k) + add per row: the backward of the row softmax (self-conditioned CTC's dA); one warp per
+// row.  out may alias dp: each lane reads its elements of dp before the warp sum and writes only those after it.
+__global__ void softmax_rows_backward_kernel(const float *__restrict__ p, const float *dp, const float *__restrict__ add,
+                                             float *out, int64_t R, int K) {
+    const int lane = threadIdx.x & 31;
+    const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (row >= R) return;
+    const float *pr = p + row * K, *dr = dp + row * K;
+    float s = 0.f;
+    for (int k = lane; k < K; k += 32) s = fmaf(pr[k], dr[k], s);
+    s = warp_sum(s);
+    for (int k = lane; k < K; k += 32) {
+        const float v = pr[k] * (dr[k] - s);
+        out[row * K + k] = add ? v + add[row * K + k] : v;
+    }
+}
+
 __global__ void set_scalar_kernel(float *p, float v) { *p = v; }
 
 // stats = {#non-skipped, sum of their nll, #skipped, sweep error flag}; one warp.  The flag rides in the data-parallel
@@ -220,6 +237,15 @@ int run_colsum(const float *delta, int64_t R, int n, float *partial, float *out,
 int run_softmax_rows(const float *x, float *p, int64_t R, int K, cudaStream_t st) {
     const int wpb = 8;
     softmax_rows_kernel<<<(unsigned)((R + wpb - 1) / wpb), wpb * 32, 0, st>>>(x, p, R, K);
+    CTCB_LAUNCH_CHECK();
+    return CTCB_OK;
+}
+
+// its backward, in the same grid
+int run_softmax_rows_backward(const float *p, const float *dp, const float *add, float *out, int64_t R, int K,
+                              cudaStream_t st) {
+    const int wpb = 8;
+    softmax_rows_backward_kernel<<<(unsigned)((R + wpb - 1) / wpb), wpb * 32, 0, st>>>(p, dp, add, out, R, K);
     CTCB_LAUNCH_CHECK();
     return CTCB_OK;
 }
@@ -316,6 +342,12 @@ static const char *cfg_error(const ctcb_brnn_config *c, char (&buf)[192]) {
                        "reads %d stacked frames and cannot take one layer's output", c->interLayer, c->subsample,
                        c->subsampleLayer, c->subsample);
     }
+    if (c->selfCondition != 0 && c->selfCondition != 1)
+        return say("selfCondition %d is neither 0 (off) nor 1 (condition the layers above interLayer on its posteriors)",
+                   c->selfCondition);
+    if (c->selfCondition == 1 && c->interLayer == 0)
+        return "selfCondition 1 conditions on the intermediate CTC's posteriors and needs interLayer >= 1; interLayer "
+               "is 0";
     const bool ok = c->inputDim > 0 && c->outputDim > 1 && c->layerSize > 0 && c->numLayers >= 1 && c->numLayers <= 64 &&
                     c->maxT > 0 && c->maxB > 0 && c->maxLabels >= 0 && c->numTemporal >= 0 &&
                     // a stacked block must lie inside the hidden layers; k <= 1 keeps the silent "no temporal layer" rule below
@@ -392,24 +424,27 @@ static int peep_index(const ctcb_brnn_config *c, int j) {
     return ln_index(c, c->numLayers + 1) + j * (c->unidirectional ? 2 : 4);
 }
 
+// the [W_c, b_c] entry of a self-conditioned net, behind everything else; 0 without
+static int cond_tensors(const ctcb_brnn_config *c) { return c->selfCondition == 1 ? 2 : 0; }
+
 extern "C" int ctcb_brnn_num_tensors(const ctcb_brnn_config *cfg) {
     if (!valid_cfg(cfg)) return 0;
     int n = base_tensors(cfg);
     for (int i = 1; i <= cfg->numLayers; ++i) n += 2 * is_normed(cfg, i);
-    return n + peep_tensors(cfg);
+    return n + peep_tensors(cfg) + cond_tensors(cfg);
 }
 
 namespace {
 // The flat parameter (and gradient) vector of a valid config: W and b of every affine map, then per temporal layer its
 // recurrent matrices, each followed by the reference's `dummy` bias (brnnet.py:60-72), then [gamma, beta] of every
-// layer-normalised hidden layer, then [P, dummy] of every direction of every peephole LSTM layer; every tensor 16-byte
-// aligned.
+// layer-normalised hidden layer, then [P, dummy] of every direction of every peephole LSTM layer, then [W_c, b_c] of a
+// self-conditioned net; every tensor 16-byte aligned.
 struct NetTable {
     struct Tensor { int64_t off; int32_t rows, cols; };
     int n;
-    int nreg;       // tensors 0 .. nreg-1 are the ones L2 regularisation sees (its even ones): all but the LN pairs and
-                    // the peephole entries
-    Tensor t[2 * 65 + 4 * 64 + 2 * 64 + 4 * 64];
+    int nreg;       // tensors 0 .. nreg-1 are the ones L2 regularisation sees (its even ones): all but the LN pairs,
+                    // the peephole entries and the conditioning entry
+    Tensor t[2 * 65 + 4 * 64 + 2 * 64 + 4 * 64 + 2];
     int64_t params;
     // The gradients that a data-parallel step sums over the ranks early, on the side stream next to the BPTT sweep: the
     // contiguous range from W of the lowest temporal layer to the end of b of layer N+1; empty (at `params`) without a
@@ -421,11 +456,14 @@ void net_table(const ctcb_brnn_config *c, NetTable *nt) {
     const int nl = c->numLayers + 1;
     nt->n = ctcb_brnn_num_tensors(c);
     nt->nreg = base_tensors(c);
-    const int peep0 = nt->n - peep_tensors(c);
+    const int cond0 = nt->n - cond_tensors(c), peep0 = cond0 - peep_tensors(c);
     int64_t off = 0;
     for (int t = 0; t < nt->n; ++t) {
         int r, cc;
-        if (t >= peep0) {           // P (rows i, f, o) of one direction, or its dummy
+        if (t >= cond0) {           // W_c (H x K) or b_c (H x 1)
+            r = c->layerSize;
+            cc = t == cond0 ? c->outputDim : 1;
+        } else if (t >= peep0) {           // P (rows i, f, o) of one direction, or its dummy
             r = (t - peep0) % 2 == 0 ? 3 : 1;
             cc = (t - peep0) % 2 == 0 ? c->layerSize : 1;
         } else if (t >= nt->nreg) {        // gamma or beta of a normalised layer
@@ -519,6 +557,7 @@ struct WsLayout {
     // interLayer > 0 only (0 elsewhere): the intermediate logits A and D_aux, its nll and skips, and the CTC area it
     // uses (the main one's, unless it runs on more frames)
     size_t inter_A, inter_D, inter_nll, inter_skip, inter_ctc, inter_ctc_bytes;
+    size_t cond_X, cond_P, cond_dA;     // selfCondition = 1 only (0 elsewhere): X'_m, P and dA
     size_t total;
 };
 
@@ -624,6 +663,12 @@ WsLayout ws_layout(const ctcb_brnn_config *c) {
         if (Rm > max_rows(c, N + 1))     // below the subsampling point: maxT frames, the main CTC has fewer
             w.inter_ctc = take(off, ctcb_ctc_workspace_bytes(c->maxB, c->maxT, c->maxLabels), &w.inter_ctc_bytes);
     }
+    if (c->selfCondition == 1) {
+        const size_t Rm = max_rows(c, c->interLayer);
+        w.cond_X = take(off, Rm * H * sizeof(float));
+        w.cond_P = take(off, Rm * c->outputDim * sizeof(float));
+        w.cond_dA = take(off, Rm * c->outputDim * sizeof(float));
+    }
     w.total = off;
     return w;
 }
@@ -642,6 +687,7 @@ struct FwdLayout {
     size_t Cf, Cb, Out;     // LSTM layers: c of each direction and the bi-directional output, shared as For / Back are
     SweepWs sweep;      // as in ws_layout: the same sweep plan
     size_t S, lens;     // subsampling only: the stacked input of map L and T'_u
+    size_t cond_A, cond_P;      // selfCondition = 1 only: the intermediate logits A and P
     size_t total;
 };
 
@@ -676,15 +722,20 @@ FwdLayout fwd_layout(const ctcb_brnn_config *c) {
     // fall back here too).  The need changes with R only at multiples of the row tile and grows with R once
     // num_sms() row tiles are exceeded (the split counts are then fixed), so those multiples and R itself bound it.
     // Each map's own rows bound its R (R' from map L up).
+    // A self-conditioned net's A and conditioning contractions (R_m x K x H, R_m x H x K) are covered the same way.
     size_t g = 0;
-    for (int i = 0; i <= N; ++i) {
-        const int Rint = (int)max_rows(c, i + 1);
+    auto cover = [&](int Rint, int n_out, int n_in) {
         const int Mtop = (Rint < GEMM_ROW_TILE * num_sms()) ? Rint : GEMM_ROW_TILE * num_sms();
         for (int M = GEMM_ROW_TILE; ; M += GEMM_ROW_TILE) {
-            const size_t b = ctcb_gemm_workspace_bytes(M <= Mtop ? M : Rint, map_rows(c, i + 1), map_cols(c, i + 1));
+            const size_t b = ctcb_gemm_workspace_bytes(M <= Mtop ? M : Rint, n_out, n_in);
             if (b > g) g = b;
             if (M > Mtop) break;
         }
+    };
+    for (int i = 0; i <= N; ++i) cover((int)max_rows(c, i + 1), map_rows(c, i + 1), map_cols(c, i + 1));
+    if (c->selfCondition == 1) {
+        cover((int)max_rows(c, c->interLayer), c->outputDim, H);
+        cover((int)max_rows(c, c->interLayer), H, c->outputDim);
     }
     const size_t train_area = ws_layout(c).gemm_bytes;
     f.gemm = take(off, g < train_area ? g : train_area, &f.gemm_bytes);
@@ -692,6 +743,11 @@ FwdLayout fwd_layout(const ctcb_brnn_config *c) {
     if (eff_k(c) > 1) {     // the slabs ping-pong, and map L - 1 wrote the one map L does not
         f.S = take(off, stacked_bytes(c));
         f.lens = take(off, (size_t)c->maxB * sizeof(int32_t));
+    }
+    if (c->selfCondition == 1) {
+        const size_t RmK = max_rows(c, c->interLayer) * c->outputDim * sizeof(float);
+        f.cond_A = take(off, RmK);
+        f.cond_P = take(off, RmK);
     }
     f.total = off;
     return f;
@@ -712,6 +768,9 @@ struct FwdBufs {
     size_t sweep_bytes;
     float *S;           // subsampling: the stacked input of map L, and T'_u of the call; else null
     int32_t *lens;
+    // selfCondition = 1: the intermediate logits A, P, and X'_m (a copy of X_m in a training call; null in a forward-only
+    // one, which conditions X_m in place); else null
+    float *A, *Pc, *Xc;
 };
 
 void fwd_bufs(const FwdLayout &f, int N, int nt, char *ws, FwdBufs *m) {
@@ -730,6 +789,9 @@ void fwd_bufs(const FwdLayout &f, int N, int nt, char *ws, FwdBufs *m) {
     m->sweep_bytes = f.sweep.scratch_bytes;
     m->S = f.S ? (float *)(ws + f.S) : nullptr;
     m->lens = f.S ? (int32_t *)(ws + f.lens) : nullptr;
+    m->A = f.cond_A ? (float *)(ws + f.cond_A) : nullptr;
+    m->Pc = f.cond_A ? (float *)(ws + f.cond_P) : nullptr;
+    m->Xc = nullptr;
 }
 void train_bufs(const WsLayout &w, int N, int nt, char *ws, FwdBufs *m) {
     for (int i = 1; i <= N + 1; ++i) m->X[i] = (float *)(ws + w.X[i]);
@@ -752,6 +814,9 @@ void train_bufs(const WsLayout &w, int N, int nt, char *ws, FwdBufs *m) {
     m->sweep_bytes = w.sweep.scratch_bytes;
     m->S = w.S ? (float *)(ws + w.S) : nullptr;
     m->lens = w.S ? (int32_t *)(ws + w.lens) : nullptr;
+    m->A = w.cond_X ? (float *)(ws + w.inter_A) : nullptr;
+    m->Pc = w.cond_X ? (float *)(ws + w.cond_P) : nullptr;
+    m->Xc = w.cond_X ? (float *)(ws + w.cond_X) : nullptr;
 }
 }  // namespace
 
@@ -774,6 +839,8 @@ struct ctcb_brnn {
     // the two dFor/dBack pairs that stacked temporal layers alternate: ev_pair[p] is recorded on the side stream after
     // its last read of pair p, and the BPTT sweep that writes pair p next waits for it
     cudaEvent_t ev_pair[2] = {};
+    // selfCondition = 1 with a temporal layer above the conditioned one: dA is complete on main (Step::backward)
+    cudaEvent_t ev_cond = nullptr;
     bool side_ready = false;
     // data-parallel callers sum the gradient over ranks first and add reg*W ONCE afterwards (ctcb_brnn_apply_l2_f32);
     // the L2 cost is still reported by every call
@@ -819,6 +886,11 @@ struct ctcb_brnn {
     bool lstm() const { return cfg.cell == 1; }
     int inter() const { return cfg.interLayer; }     // the layer of the intermediate CTC loss, 0 without
     int stats_floats() const { return inter() ? 6 : 4; }     // of stats_out
+    int cond() const { return cfg.selfCondition == 1 ? cfg.interLayer : 0; }     // the conditioned layer m, 0 without
+    // The early exchange of the data-parallel step (brnn_reduce_early) holds W_{N+1}, b_{N+1}.  A self-conditioned net
+    // whose m lies below the lowest temporal layer adds its share of them on main only after the side stream's last
+    // weight gradients, so it exchanges the whole gradient at the end instead.
+    bool early() const { return tl > 0 && !(cond() && cond() < tl); }
     bool peep() const { return cfg.peephole == 1; }
     int peep_idx(int j) const { return peep_index(&cfg, j); }
     bool temporal(int i) const { return nt > 0 && i >= tl && i < tl + nt; }
@@ -839,6 +911,10 @@ struct ctcb_brnn {
         if (!temporal(i)) return m.X[i];
         return uni() ? m.For[i - tl] : lstm() ? m.Out[i - tl] : m.X[i];
     }
+    // what map i + 1 (its contraction, the frame stacking, its weight gradient) reads of layer i: X'_m at the conditioned
+    // layer of a training call, else act() (a forward-only call conditions act() in place)
+    const float *next_in(const FwdBufs &m, int i) const { return (i == cond() && m.Xc) ? m.Xc : act(m, i); }
+    int cond_idx() const { return net.n - 2; }     // flat-vector index of W_c; b_c is the next tensor
 };
 
 extern "C" size_t ctcb_brnn_workspace_bytes(const ctcb_brnn_config *cfg) {
@@ -902,6 +978,7 @@ extern "C" void ctcb_brnn_destroy(ctcb_brnn *h) {
         cudaEventDestroy(h->ev_sweep);
         cudaEventDestroy(h->ev_side);
         for (int p = 0; p < 2; ++p) cudaEventDestroy(h->ev_pair[p]);
+        if (h->ev_cond) cudaEventDestroy(h->ev_cond);
     }
     delete h;
 }
@@ -918,6 +995,7 @@ static int ensure_side_stream(ctcb_brnn *h) {
     CTCB_CUDA_CHECK(cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming));
     CTCB_CUDA_CHECK(cudaEventCreateWithFlags(&h->ev_hi, cudaEventDisableTiming));
     for (int p = 0; p < 2; ++p) CTCB_CUDA_CHECK(cudaEventCreateWithFlags(&h->ev_pair[p], cudaEventDisableTiming));
+    if (h->cond()) CTCB_CUDA_CHECK(cudaEventCreateWithFlags(&h->ev_cond, cudaEventDisableTiming));
     h->side_ready = true;
     return CTCB_OK;
 }
@@ -945,7 +1023,7 @@ static int brnn_reduce_early(ctcb_brnn *h, float *grads, cudaStream_t st) {
 
 // The part of the flat gradient that was NOT summed early, plus the statistics tail, in one grouped NCCL launch.
 static int brnn_reduce_rest(ctcb_brnn *h, float *grads, float *stats, cudaStream_t st) {
-    const int64_t P = h->net.params, lo = h->net.early_lo, hi = h->net.early_hi;
+    const int64_t P = h->net.params, lo = h->early() ? h->net.early_lo : P, hi = h->early() ? h->net.early_hi : P;
     float *ptrs[3];
     int64_t cnt[3];
     int k = 0;
@@ -972,7 +1050,7 @@ static int brnn_forward(ctcb_brnn *h, const float *feats, const int32_t *T_per_u
     // the sweep kernels' error flag (word 0) is cleared once per call, so a forward-sweep timeout survives the BPTT sweep
     CTCB_CUDA_CHECK(cudaMemsetAsync(m.counters, 0, 16 * sizeof(unsigned int), st));
     for (int i = 1; i <= N + 1; ++i) {
-        const float *in = (i == 1) ? feats : h->act(m, i - 1);
+        const float *in = (i == 1) ? feats : h->next_in(m, i - 1);
         const int relu = (i <= N && !h->temporal(i)) ? 1 : 0;
         const int n_out = h->rows(i), n_in = h->cols(i);
         const int Tmax = h->frames(i, Tmax0);
@@ -1031,6 +1109,20 @@ static int brnn_forward(ctcb_brnn *h, const float *feats, const int32_t *T_per_u
                 TRY(run_add2(m.For[j], m.Back[j], m.X[i], R * H, st));     // brnnet.py:153
             }
         }
+        if (i == h->cond()) {     // A, P = softmax(A), X'_m = X_m + P W_c^T + b_c (include/ctcb200.h: selfCondition)
+            const float *Wc = h->tensor(params, h->cond_idx()), *bc = h->tensor(params, h->cond_idx() + 1);
+            float *Xm = h->act(m, i);
+            ProfScope ps("self_cond", st);
+            TRY(ctcb_gemm_f32(0, 1, (int)R, K, H, 1.f, Xm, H, h->tensor(params, 2 * N), H, 0.f, m.A, K,
+                              h->tensor(params, 2 * N + 1), 0, nullptr, m.gemm, m.gemm_bytes, st));
+            TRY(run_softmax_rows(m.A, m.Pc, R, K, st));
+            if (m.Xc) {     // a training call keeps X_m (the masks, the head, the BPTT) and conditions a copy
+                CTCB_CUDA_CHECK(cudaMemcpyAsync(m.Xc, Xm, (size_t)R * H * sizeof(float), cudaMemcpyDeviceToDevice, st));
+                Xm = m.Xc;
+            }
+            TRY(ctcb_gemm_f32(0, 1, (int)R, H, K, 1.f, m.Pc, K, Wc, K, 1.f, Xm, H, bc, 0, nullptr, m.gemm, m.gemm_bytes,
+                              st));
+        }
     }
     if (probs_out) TRY(run_softmax_rows(m.X[N + 1], probs_out, (int64_t)h->frames(N + 1, Tmax0) * B, K, st));
     return CTCB_OK;
@@ -1070,6 +1162,8 @@ struct Step {
         return buf((h->uni() && h->temporal(i + 1) && !h->lstm()) ? w.dFor[(i + 1 - h->tl) % 2] : w.D[i + 1]);
     }
     int weight_grads(int i, bool on_side) const;
+    int head_grads(bool on_side) const;
+    int cond_backward(int i, float *doth, float alpha) const;
     int rec_weight_grads(int j) const;
     int backward() const;
     int finish(float *stats, float *regcost_out) const;
@@ -1079,7 +1173,7 @@ struct Step {
 // the weight and bias gradients of map i, on the side stream or in the main chain, where its delta is complete
 int Step::weight_grads(int i, bool on_side) const {
     const cudaStream_t st = on_side ? side : main;
-    const float *Xi = h->stacked(i + 1) ? m.S : (i == 0) ? feats : h->act(m, i);
+    const float *Xi = h->stacked(i + 1) ? m.S : (i == 0) ? feats : h->next_in(m, i);
     const int n_out = h->rows(i + 1), n_in = h->cols(i + 1);
     // dW = delta^T . X_i   (brnnet.py:196); dW_L = delta^T . S
     {
@@ -1094,20 +1188,60 @@ int Step::weight_grads(int i, bool on_side) const {
     }
     // the intermediate loss's share of W_{N+1} and b_{N+1}: added behind the main one on the same stream, so ahead of
     // the early exchange, whose range holds them.  The side stream gets here behind ev_delta, which main records after
-    // the intermediate CTC.
-    if (i == h->cfg.numLayers && h->inter()) {
-        const int mi = h->inter(), K = h->cfg.outputDim, H = h->cfg.layerSize;
-        ProfScope ps("inter_ctc_dw", st);
-        TRY(ctcb_gemm_f32(1, 0, K, H, (int)R(mi), 1.f, buf(w.inter_D), K, h->act(m, mi), H, 1.f, G(2 * i), H, nullptr,
-                          0, nullptr, on_side ? ws + w.gemm2 : m.gemm, on_side ? w.gemm2_bytes : m.gemm_bytes, st));
-        TRY(run_colsum(buf(w.inter_D), R(mi), K, buf(on_side ? w.colsum2 : w.colsum), G(2 * i + 1), true, st));
-    }
+    // the intermediate CTC (and, self-conditioned with m at or above the highest temporal layer, after layer m's stage,
+    // which completes dA).  A self-conditioned net with m below the highest temporal layer adds it at layer m
+    // (Step::cond_backward).
+    if (i == h->cfg.numLayers && h->inter() && (!h->cond() || (h->tl > 0 && h->cond() >= h->tl + h->nt - 1)))
+        TRY(head_grads(on_side));
     if (h->uni() && h->temporal(i + 1) && !h->lstm() && i + 1 - h->tl >= 2)  // the last read of the pair of uni-directional layer i + 1
         CTCB_CUDA_CHECK(cudaEventRecord(h->ev_pair[(i + 1 - h->tl) % 2], side));
     // every gradient tensor of the layers >= tl is now queued on the side stream: sum that contiguous range over
     // the ranks there, next to the BPTT sweep on the main stream
-    if (dp && last && on_side && i == h->tl) TRY(brnn_reduce_early(h, grads, side));
+    if (dp && last && on_side && i == h->tl && h->early()) TRY(brnn_reduce_early(h, grads, side));
     return CTCB_OK;
+}
+
+// dW_{N+1} += D^T X_m, db_{N+1} += the column sums of D, behind the main term: D = D_aux, or dA when self-conditioned
+int Step::head_grads(bool on_side) const {
+    const cudaStream_t st = on_side ? side : main;
+    const int N = h->cfg.numLayers, mi = h->inter(), K = h->cfg.outputDim, H = h->cfg.layerSize;
+    const float *D = buf(h->cond() ? w.cond_dA : w.inter_D);
+    ProfScope ps("inter_ctc_dw", st);
+    TRY(ctcb_gemm_f32(1, 0, K, H, (int)R(mi), 1.f, D, K, h->act(m, mi), H, 1.f, G(2 * N), H, nullptr, 0, nullptr,
+                      on_side ? ws + w.gemm2 : m.gemm, on_side ? w.gemm2_bytes : m.gemm_bytes, st));
+    TRY(run_colsum(D, R(mi), K, buf(on_side ? w.colsum2 : w.colsum), G(2 * N + 1), true, st));
+    return CTCB_OK;
+}
+
+// Self-conditioned layer i = m (include/ctcb200.h: selfCondition), on main: doth holds D'_m, the unmasked delta of map
+// m + 1 at layer m's rate.  dP = D'_m W_c into the dA buffer, dW_c and db_c (before doth is overwritten), dA in place,
+// then doth = alpha [X_m > 0] (D'_m + dA W_{N+1}).  Where dA's share of W_{N+1}, b_{N+1} goes, so that it lands behind
+// weight_grads(N)'s writes and ahead of the early exchange: inside weight_grads(N) when m is at or above the highest
+// temporal layer; on main here without a temporal layer; otherwise on the side stream here, behind ev_cond (host order
+// puts it after weight_grads(N), enqueued in an earlier iteration, and ahead of this iteration's weight gradients and
+// the early exchange, which early() drops when m is below the lowest temporal layer).
+int Step::cond_backward(int i, float *doth, float alpha) const {
+    const int N = h->cfg.numLayers, K = h->cfg.outputDim, H = h->cfg.layerSize, ic = h->cond_idx();
+    const int64_t Rm = R(i);
+    float *dA = buf(w.cond_dA);
+    {
+    ProfScope ps("self_cond_bwd", main);
+    TRY(ctcb_gemm_f32(0, 0, (int)Rm, K, H, 1.f, doth, H, P(ic), K, 0.f, dA, K, nullptr, 0, nullptr, m.gemm,
+                      m.gemm_bytes, main));
+    TRY(ctcb_gemm_f32(1, 0, H, K, (int)Rm, 1.f, doth, H, m.Pc, K, beta_g(), G(ic), K, nullptr, 0, nullptr, m.gemm,
+                      m.gemm_bytes, main));
+    TRY(run_colsum(doth, Rm, H, buf(w.colsum), G(ic + 1), !first, main));
+    TRY(run_softmax_rows_backward(m.Pc, dA, buf(w.inter_D), dA, Rm, K, main));
+    TRY(ctcb_gemm_f32(0, 0, (int)Rm, H, K, alpha, dA, K, P(2 * N), H, alpha, doth, H, nullptr, 0,
+                      h->temporal(i) ? nullptr : h->act(m, i), m.gemm, m.gemm_bytes, main));
+    }
+    if (h->tl == 0) return head_grads(false);
+    if (i >= h->tl + h->nt - 1) return CTCB_OK;
+    CTCB_CUDA_CHECK(cudaEventRecord(h->ev_cond, main));
+    TRY(stall(main, STALL_MAIN));
+    CTCB_CUDA_CHECK(cudaStreamWaitEvent(side, h->ev_cond, 0));
+    TRY(stall(side, STALL_SIDE));
+    return head_grads(true);
 }
 
 // The recurrent weight gradients of temporal layer j (brnnet.py:227-230), behind its BPTT sweep: independent of the
@@ -1185,18 +1319,22 @@ int Step::backward() const {
         // layer's X_i is 0 at every dropped unit, so the same mask removes those; the kept ones were scaled by
         // drop_scale in the forward pass, and so is their delta, through alpha.  S holds X_i stacked, and 0 at the
         // padding frames, whose delta is 0 either way.
-        const float *mask = h->temporal(i) ? nullptr : stacked ? m.S : h->act(m, i);
+        // The self-conditioned layer takes D'_m without the mask and alpha, which cond_backward applies.
+        const bool cond = (i == h->cond());
+        const float *mask = (h->temporal(i) || cond) ? nullptr : stacked ? m.S : h->act(m, i);
         const float alpha = (drop && !h->temporal(i)) ? h->drop_scale : 1.f;
         {
         ProfScope ps("gemm_delta", main);
-        TRY(ctcb_gemm_f32(0, 0, (int)this->R(i + 1), n_in, n_out, alpha, delta(i), n_out, P(2 * i), n_in, 0.f,
-                          stacked ? buf(w.dS) : doth, n_in, nullptr, 0, mask, m.gemm, m.gemm_bytes, main));
+        TRY(ctcb_gemm_f32(0, 0, (int)this->R(i + 1), n_in, n_out, cond ? 1.f : alpha, delta(i), n_out, P(2 * i), n_in,
+                          0.f, stacked ? buf(w.dS) : doth, n_in, nullptr, 0, mask, m.gemm, m.gemm_bytes, main));
         }
         if (stacked) {
             ProfScope ps("subsample", main);
             TRY(run_frame_unstack(buf(w.dS), T_per_utt, T(i), B, n, h->k(), doth, main));
         }
-        if (i == h->inter()) {     // + D_aux W_{N+1}, at layer i's own rate, under the same mask and alpha
+        if (cond) {
+            TRY(cond_backward(i, doth, alpha));
+        } else if (i == h->inter()) {     // + D_aux W_{N+1}, at layer i's own rate, under the same mask and alpha
             ProfScope ps("inter_ctc_delta", main);
             TRY(ctcb_gemm_f32(0, 0, (int)R, n, h->cfg.outputDim, alpha, buf(w.inter_D), h->cfg.outputDim, P(2 * N), n,
                               1.f, doth, n, nullptr, 0, h->temporal(i) ? nullptr : h->act(m, i), m.gemm, m.gemm_bytes,
@@ -1355,8 +1493,9 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
         const int mi = h->inter(), H = c.layerSize;
         float *A = s.buf(w.inter_A), *Da = s.buf(w.inter_D);
         ProfScope ps("inter_ctc", s.main);
-        TRY(ctcb_gemm_f32(0, 1, (int)s.R(mi), K, H, 1.f, h->act(m, mi), H, s.P(2 * N), H, 0.f, A, K, s.P(2 * N + 1), 0,
-                          nullptr, m.gemm, m.gemm_bytes, s.main));
+        if (!h->cond())     // a self-conditioned net computed A in the forward pass
+            TRY(ctcb_gemm_f32(0, 1, (int)s.R(mi), K, H, 1.f, h->act(m, mi), H, s.P(2 * N), H, 0.f, A, K, s.P(2 * N + 1),
+                              0, nullptr, m.gemm, m.gemm_bytes, s.main));
         TRY(ctcb_ctc_loss_grad_f32(A, 0, (int64_t)K, (int64_t)B * K, labels, label_off, s.lens(mi), B, s.T(mi), K,
                                    c.maxLabels, 0, Da, inter_nll, inter_skip, ws + w.inter_ctc, w.inter_ctc_bytes,
                                    s.main));
@@ -1413,7 +1552,7 @@ extern "C" int ctcb_brnn_set_comm(ctcb_brnn *h, ctcb_comm *comm) {
 extern "C" int ctcb_brnn_exchange_only(ctcb_brnn *h, const float *params, float *grads, float *stats_out, void *stream) {
     if (!h || !params || !grads) return set_error(CTCB_EINVAL, "ctcb_brnn_exchange_only: null pointer argument");
     if (!h->comm || comm_world(h->comm) <= 1) return CTCB_OK;
-    if (h->tl > 0) TRY(brnn_reduce_early(h, grads, (cudaStream_t)stream));
+    if (h->early()) TRY(brnn_reduce_early(h, grads, (cudaStream_t)stream));
     TRY(brnn_reduce_rest(h, grads, stats_out, (cudaStream_t)stream));
     return h->defer_l2 ? CTCB_OK : ctcb_brnn_apply_l2_f32(h, params, grads, stream);
 }
@@ -1548,13 +1687,23 @@ extern "C" int ctcb_softmax_rows_f32(const float *x, float *p, int64_t R, int K,
     return run_softmax_rows(x, p, R, K, (cudaStream_t)stream);
 }
 
+extern "C" int ctcb_softmax_rows_backward_f32(const float *p, const float *dp, const float *add, float *out, int64_t R,
+                                              int K, void *stream) {
+    if (!p || !dp || !out) return set_error(CTCB_EINVAL, "ctcb_softmax_rows_backward_f32: null pointer argument");
+    if (R <= 0 || K <= 0 || (R + 7) / 8 > 0x7fffffff)
+        return set_error(CTCB_EINVAL, "ctcb_softmax_rows_backward_f32: R = %lld, K = %d (need 1 <= R < 2^34, K >= 1)",
+                         (long long)R, K);
+    return run_softmax_rows_backward(p, dp, add, out, R, K, (cudaStream_t)stream);
+}
+
 // Test / diagnostic hook: where, inside the workspace, the activations of the LAST ctcb_brnn_cost_and_grad call lie
 // (time-major [Tmax][B][n] with that call's B and Tmax).  what = 0: output of affine map `layer` (1..numLayers+1; the
 // temporal layer's entry holds For + Back, the last one the logits), 1: For, 2: Back (temporal layer only; with
 // several, `layer` says which, and only a bi-directional stack has a Back of every layer).  Subsampled nets: entries of
 // maps >= L are [Tmax'][B][n]; what = 6: S, the stacked input of map L, k n wide.  what = 7: the delta of map `layer`,
 // the buffer its weight and bias gradients read (Step::delta), where no later stage of the call overwrites it.
-// what = 8..11 (interLayer > 0): the intermediate logits A, D_aux, the intermediate nll and skips.
+// what = 8..11 (interLayer > 0): the intermediate logits A, D_aux, the intermediate nll and skips.  what = 12..14
+// (selfCondition = 1): X'_m, P, dA.
 extern "C" int ctcb_brnn_activation_offset(const ctcb_brnn_config *cfg, int what, int layer, size_t *offset, int32_t *width) {
     if (!valid_cfg(cfg) || !offset) return set_error(CTCB_EINVAL, "ctcb_brnn_activation_offset: bad arguments");
     const WsLayout w = ws_layout(cfg);
@@ -1564,6 +1713,14 @@ extern "C" int ctcb_brnn_activation_offset(const ctcb_brnn_config *cfg, int what
         const size_t at[4] = {w.inter_A, w.inter_D, w.inter_nll, w.inter_skip};
         *offset = at[what - 8];
         if (width) *width = what <= 9 ? cfg->outputDim : 1;
+        return CTCB_OK;
+    }
+    if (what >= 12 && what <= 14) {     // self-conditioned CTC: X'_m, P, dA
+        if (cfg->selfCondition != 1)
+            return set_error(CTCB_EINVAL, "ctcb_brnn_activation_offset: nothing of kind %d without selfCondition", what);
+        const size_t at[3] = {w.cond_X, w.cond_P, w.cond_dA};
+        *offset = at[what - 12];
+        if (width) *width = what == 12 ? cfg->layerSize : cfg->outputDim;
         return CTCB_OK;
     }
     if (what == 7) {

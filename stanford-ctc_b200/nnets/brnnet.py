@@ -54,6 +54,12 @@ single contiguous vector.  New, additive surface for the minibatch/data-parallel
                                                 costAndGrad returns it.  No parameter is added and forward-only calls do
                                                 not change; interCosts / interSkips hold the last batch's per-utterance
                                                 intermediate nll and skips
+    NNet(..., interLayer=m, interWeight=lam, selfCondition=True)
+                                             self-conditioned CTC (include/ctcb200.h: selfCondition): the intermediate
+                                                posteriors P = softmax(A) are projected back, X_m + W_c P + b_c, and
+                                                the layers above read that, in training and forward-only calls alike;
+                                                one [W_c (H x K), b_c (H x 1)] pair appended to `stack` behind
+                                                everything else, both 0 at start (the net starts as the InterCTC net)
     costAndGradBatch(datas, labelss)         -> (costs[B], grad, skips[B])   host arrays in; more than maxUtts
                                                 utterances are accumulated over micro-batches
     costAndGradDevice(batch, first, last)    -> no host sync; see DeviceBatch
@@ -169,6 +175,15 @@ def check_ln_pairs(got, want, n_ln, what):
                          % (what, got, n_ln, want, "without" if got < want else "with more"))
 
 
+def check_cond_pairs(got, want, selfCondition, what):
+    """A checkpoint of the other self-conditioning setting has the [W_c, b_c] pair more or fewer, which zip() would
+    leave unset or drop."""
+    if got != want:
+        raise ValueError("the checkpoint's %s has %d tensors where this net (selfCondition=%s) has %d: a checkpoint of a "
+                         "net %s self-conditioned CTC, or of another shape"
+                         % (what, 2 * got, selfCondition, 2 * want, "with" if got > want else "without"))
+
+
 def check_peephole_pairs(got, want, peephole, what):
     """An LSTM net loads only a checkpoint with its own number of [W, b] pairs: one of the other peephole setting has
     [P, dummy] pairs more or fewer, which zip() would leave unset or drop."""
@@ -193,7 +208,8 @@ class NNet:
                  allowTopTemporal=False, device=None, unidirectional=False, numTemporal=1, dropout=0.0,
                  dropoutSeed=33, cell="relu", layerNorm=False, subsample=1, subsampleLayer=1, peephole=False,
                  freqMasks=0, freqMaskWidth=0, timeMasks=0, timeMaskWidth=0, timeMaskRatio=1.0, featDim=None,
-                 weightNoise=0.0, zoneoutCell=0.0, zoneoutHidden=0.0, interLayer=0, interWeight=0.0):
+                 weightNoise=0.0, zoneoutCell=0.0, zoneoutHidden=0.0, interLayer=0, interWeight=0.0,
+                 selfCondition=False):
         # The intermediate CTC loss (include/ctcb200.h: interLayer).  The library refuses a layer outside
         # 1..numLayers-1 and a subsampled output map, with its message; a layer and a weight come only together.
         self.interLayer, self.interWeight = int(interLayer), float(interWeight)
@@ -201,6 +217,9 @@ class NNet:
             raise ValueError("interLayer=%d needs a finite interWeight > 0; interWeight is %r" % (interLayer, interWeight))
         if self.interLayer == 0 and self.interWeight != 0.0:
             raise ValueError("interWeight=%r weighs the intermediate CTC loss; it needs interLayer >= 1" % (interWeight,))
+        self.selfCondition = bool(selfCondition)
+        if self.selfCondition and self.interLayer == 0:
+            raise ValueError("selfCondition=True conditions on the intermediate CTC's posteriors; it needs interLayer >= 1")
         torch = _ctcb.require_cuda()
         self._torch = torch
         self.dev = torch.device("cuda", torch.cuda.current_device() if device is None else device)
@@ -278,7 +297,8 @@ class NNet:
                                maxUtts, self.maxLabels, float(reg), float(self.maxAct), int(self.unidirectional),
                                self.numTemporal, _ctcb.CELLS[cell], int(self.layerNorm), self.subsample,
                                self.subsampleLayer, int(self.peephole), self.featDim or 0,
-                               int(self.weightNoise > 0.0), int(self.zoneout), self.interLayer, self.interWeight)
+                               int(self.weightNoise > 0.0), int(self.zoneout), self.interLayer, self.interWeight,
+                               int(self.selfCondition))
         self._h = ctypes.c_void_p()
         check(lib.ctcb_brnn_create(ctypes.byref(self._cfg), ctypes.byref(self._h)))
         self.stack = None
@@ -353,6 +373,9 @@ class NNet:
         # [P, dummy] of every direction of every peephole LSTM layer, behind those: P = 0 without a draw, so the net starts
         # out as the same net without peepholes
         host += [[np.zeros((3, H)), np.zeros((1, 1))] for _ in range(self.peepholeEntries())]
+        # [W_c, b_c] of self-conditioned CTC, behind those: 0 without a draw, so the net starts as the InterCTC net
+        if self.selfCondition:
+            host.append([np.zeros((H, self.outputDim)), np.zeros((H, 1))])
 
         self.nparams = int(lib.ctcb_brnn_param_count(ctypes.byref(self._cfg)))
         self.params = torch.zeros(self.nparams, dtype=torch.float32, device=self.dev)
@@ -665,7 +688,12 @@ class NNet:
 
     def check_pair_count(self, got, views, what):
         """A checkpoint's `what` (a list of [w, b]) has as many pairs as this net's: a layer-norm net refuses one with
-        other [gamma, beta] pairs, an LSTM net one of the other peephole setting."""
+        other [gamma, beta] pairs, an LSTM net one of the other peephole setting, a self-conditioned net one without
+        [W_c, b_c], and any net one with a trailing [W_c, b_c] it does not have."""
+        H, K = self.layerSize, self.outputDim
+        cond_tail = (len(got) == len(views) + 1 and np.shape(got[-1][0]) == (H, K) and np.size(got[-1][1]) == H)
+        if self.selfCondition or cond_tail:
+            check_cond_pairs(len(got), len(views), self.selfCondition, what)
         if self.cell == "lstm" and self.numTemporal:
             check_peephole_pairs(len(got), len(views), self.peephole, what)
         if self.layerNorm:

@@ -9,7 +9,7 @@ The implementation is organised differently: a declarative flag table, one RunDi
 side files, and separate train/evaluate phases.  Site paths of run_cfg.py / decoder_config.py became
 flags (--runDir, --outDir); new flags: --numTemporal, --cell, --peephole, --layerNorm, --subsample, --subsampleLayer, --batchSize, --maxUtts, --maxLabels,
 --dropout, --freqMasks, --freqMaskWidth, --timeMasks, --timeMaskWidth, --timeMaskRatio, --featDim, --weightNoise,
---zoneoutCell, --zoneoutHidden, --interLayer, --interWeight,
+--zoneoutCell, --zoneoutHidden, --interLayer, --interWeight, --selfCondition,
 --optimizer,
 --beta1, --beta2, --epsilon, --quiet.  Under torchrun the same
 script trains data-parallel (one process per GPU, one NCCL all-reduce per step).
@@ -83,10 +83,13 @@ FLAGS = [
                                 "written without it has none)"),
     ("zoneoutHidden", float, 0.0, "zoneout probability of the LSTM output h, as --zoneoutCell"),
     ("interLayer", int, 0, "intermediate CTC loss while training: hidden layer m (1..numLayers-1) through the output "
-                           "map, scored against the same labels (0 = off; --test ignores it; a cfg.json written "
-                           "without it has none)"),
+                           "map, scored against the same labels (0 = off; --test ignores it without "
+                           "--selfCondition; a cfg.json written without it has none)"),
     ("interWeight", float, 0.0, "lambda of the intermediate CTC loss: the objective is main + lambda * intermediate "
                                 "(Lee & Watanabe's weight w is lambda = w / (1 - w) at (1 - w) times the step size)"),
+    ("selfCondition", None, False, "self-conditioned CTC (needs --interLayer): the intermediate posteriors, projected "
+                                   "back to the layer's width, are added to layer m's output, in training and in --test "
+                                   "alike; a cfg.json written without it has none"),
     ("optimizer", str, "nesterov", "update rule: nesterov (the reference's, with --momentum), adagrad or adam; --step "
                                    "is the step size of each and --anneal applies to it"),
     ("beta1", float, 0.9, "adam: decay of the first-moment estimate"),
@@ -236,7 +239,8 @@ def _train(opts, cfg, run_dir, log, rank, world):
                      peephole=opts.peephole, freqMasks=opts.freqMasks, freqMaskWidth=opts.freqMaskWidth,
                      timeMasks=opts.timeMasks, timeMaskWidth=opts.timeMaskWidth, timeMaskRatio=opts.timeMaskRatio,
                      featDim=opts.featDim, weightNoise=opts.weightNoise, zoneoutCell=opts.zoneoutCell,
-                     zoneoutHidden=opts.zoneoutHidden, interLayer=opts.interLayer, interWeight=opts.interWeight)
+                     zoneoutHidden=opts.zoneoutHidden, interLayer=opts.interLayer, interWeight=opts.interWeight,
+                     selfCondition=opts.selfCondition)
     net.initParams()
     optimizer = sgd.SGD(net, opts.maxUttLen, alpha=opts.step, optimizer=opts.optimizer, momentum=opts.momentum,
                         batchSize=opts.batchSize, verbose=(rank == 0 and not opts.quiet), beta1=opts.beta1,
@@ -297,11 +301,14 @@ def test(opts, rank=0, world=1):
     the files (parallel.rank_files)."""
     trained = trained_config(opts.cfg_file)
     logging.getLogger().info("Running on %s" % get_hostname())
+    # the intermediate CTC loss only trains, unless the net conditions its upper layers on it
+    cond = dict(interLayer=trained.interLayer, interWeight=trained.interWeight,
+                selfCondition=True) if trained.selfCondition else {}
     net = rnnet.NNet(trained.inputDim, trained.outputDim, trained.layerSize, trained.numLayers, trained.maxUttLen,
                      temporalLayer=trained.temporalLayer, train=False, maxUtts=max(1, opts.maxUtts),
                      numTemporal=trained.numTemporal, cell=trained.cell, layerNorm=trained.layerNorm,
                      subsample=trained.subsample, subsampleLayer=trained.subsampleLayer, peephole=trained.peephole,
-                     zoneoutCell=trained.zoneoutCell, zoneoutHidden=trained.zoneoutHidden)
+                     zoneoutCell=trained.zoneoutCell, zoneoutHidden=trained.zoneoutHidden, **cond)
     net.initParams()
     with open(trained.in_file, "rb") as fid:
         pickle.load(fid)                              # optimiser state: not needed here
