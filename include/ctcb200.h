@@ -429,7 +429,12 @@ size_t ctcb_brnn_forward_workspace_bytes(const ctcb_brnn_config *cfg, size_t *er
  * layer above the lowest two of its stack.  interLayer = m >= 1 only (`layer` is ignored): what = 8 the intermediate
  * logits A, 9 D_aux = lambda d(nll_aux)/dA (both [T_m][B][outputDim]), 10 the intermediate nll (float32[B]), 11 its
  * skips (int32[B]).  selfCondition = 1 only (`layer` is ignored): what = 12 X'_m (layerSize wide), 13 P, 14 dA (both
- * outputDim wide), all [T_m][B][width]. */
+ * outputDim wide), all [T_m][B][width].  A layer-normalised hidden layer `layer` only: what = 15 its z, the
+ * contraction's output before the normalisation (layerSize wide), 16 / 17 its row statistics Mu / Rstd (width 1), all
+ * [T][B][width] at that layer's rate.  maskFeatDim > 0 only (`layer` is ignored): what = 18 the masked copy of the
+ * features that every stage of a call with input masks on reads, [Tmax][B][inputDim].  weightNoise = 1 only (`layer`
+ * is ignored): what = 19 the noisy copy of the flat parameter vector that every stage of a call with noise on reads,
+ * *width = ctcb_brnn_param_count floats.  Each of 15..19 is CTCB_EINVAL where its feature is off. */
 int ctcb_brnn_activation_offset(const ctcb_brnn_config *cfg, int what, int layer, size_t *offset, int32_t *width);
 
 /* With temporal layers, refuses (CTCB_EINVAL, with the planner's message) a config whose recurrent sweep the device

@@ -1703,7 +1703,8 @@ extern "C" int ctcb_softmax_rows_backward_f32(const float *p, const float *dp, c
 // maps >= L are [Tmax'][B][n]; what = 6: S, the stacked input of map L, k n wide.  what = 7: the delta of map `layer`,
 // the buffer its weight and bias gradients read (Step::delta), where no later stage of the call overwrites it.
 // what = 8..11 (interLayer > 0): the intermediate logits A, D_aux, the intermediate nll and skips.  what = 12..14
-// (selfCondition = 1): X'_m, P, dA.
+// (selfCondition = 1): X'_m, P, dA.  what = 15..17 (layer-normalised layer `layer`): z, Mu, Rstd.  what = 18
+// (maskFeatDim > 0): the masked feature copy; 19 (weightNoise = 1): the noisy parameter copy.
 extern "C" int ctcb_brnn_activation_offset(const ctcb_brnn_config *cfg, int what, int layer, size_t *offset, int32_t *width) {
     if (!valid_cfg(cfg) || !offset) return set_error(CTCB_EINVAL, "ctcb_brnn_activation_offset: bad arguments");
     const WsLayout w = ws_layout(cfg);
@@ -1721,6 +1722,28 @@ extern "C" int ctcb_brnn_activation_offset(const ctcb_brnn_config *cfg, int what
         const size_t at[3] = {w.cond_X, w.cond_P, w.cond_dA};
         *offset = at[what - 12];
         if (width) *width = what == 12 ? cfg->layerSize : cfg->outputDim;
+        return CTCB_OK;
+    }
+    if (what >= 15 && what <= 17) {     // a layer-normalised layer: z, Mu, Rstd
+        if (layer < 1 || layer > cfg->numLayers || !is_normed(cfg, layer))
+            return set_error(CTCB_EINVAL, "ctcb_brnn_activation_offset: layer %d is not layer-normalised", layer);
+        const size_t at[3] = {w.Z[layer], w.Mu[layer], w.Rstd[layer]};
+        *offset = at[what - 15];
+        if (width) *width = what == 15 ? cfg->layerSize : 1;
+        return CTCB_OK;
+    }
+    if (what == 18) {     // the masked copy of the features, [Tmax][B][inputDim]
+        if (cfg->maskFeatDim <= 0)
+            return set_error(CTCB_EINVAL, "ctcb_brnn_activation_offset: no masked feature copy without maskFeatDim");
+        *offset = w.masked;
+        if (width) *width = cfg->inputDim;
+        return CTCB_OK;
+    }
+    if (what == 19) {     // the noisy copy of the flat parameter vector
+        if (cfg->weightNoise != 1)
+            return set_error(CTCB_EINVAL, "ctcb_brnn_activation_offset: no noisy parameter copy without weightNoise");
+        *offset = w.noisy;
+        if (width) *width = (int32_t)ctcb_brnn_param_count(cfg);
         return CTCB_OK;
     }
     if (what == 7) {

@@ -190,7 +190,8 @@ __global__ void __launch_bounds__(256) ln_backward_kernel(float *__restrict__ d,
 #pragma unroll
             for (int c = 0; c < 4; ++c) {
                 const float gg = get(g[k], c), x = get(xh[k], c);
-                put(o, c, rs * (gg * get(ga[k], c) - a - x * b));
+                // + 0: a zero row of g (a padded frame) gives +0.0, where a negative gamma would leave -0.0
+                put(o, c, rs * (gg * get(ga[k], c) - a - x * b) + 0.f);
                 put(ag[k], c, fmaf(gg, x, get(ag[k], c)));
                 put(ab[k], c, get(ab[k], c) + gg);
             }

@@ -147,7 +147,7 @@ def test_kernels_match_float64_of_their_inputs(H, R, cuda):
     bb = 2 * (D + 4) * U32 * np.abs(g64).sum(axis=0, keepdims=True)
     r_dz = max(_ratio(np.abs(out[acc][0] - dz64), bound_dz) for acc in (0, 1))
     assert np.array_equal(out[0][0], out[1][0])
-    assert not np.any(out[0][0][2::11])                 # zero delta rows stay zero
+    assert not out[0][0][2::11].view(np.uint32).any()     # zero delta rows stay +0.0, whatever the sign of gamma
     r_dg = _ratio(np.abs(out[0][1] - dgam64), bg)
     r_db = _ratio(np.abs(out[0][2] - dbet64), bb)
     r_dg_acc = _ratio(np.abs(out[1][1] - (dgam64 + prev_g)), bg + U32 * np.abs(dgam64 + prev_g))
