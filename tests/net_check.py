@@ -3,8 +3,8 @@
 compare() reads what the device left behind -- per-utterance costs and skips, the gradient, and every activation
 array ctcb_brnn_activation_offset exposes -- and runs one loop over the utterances: the oracle's own forward and
 back-propagation (its own float64 masks), and its back-propagation through the device's own activations (the device's
-masks), each summed over the utterances with reg * W added once.  It returns plain numbers; the tests decide which
-bounds apply."""
+masks, and X'_m and P of a self-conditioned net), each summed over the utterances under Net.costAndGradBatch's rule
+with reg * W added once.  It returns plain numbers; the tests decide which bounds apply."""
 import ctypes
 
 import numpy as np
@@ -33,17 +33,19 @@ def bits(t):
 
 def workspace_activations(nn, B, Tmax):
     """{(what, layer): float32 [T][B][width]} of every array the activation hook exposes for nn's last call of B
-    utterances of at most Tmax frames (what 0 X, 1 For / h_f, 2 Back / h_b, 3 gates, 4 c_f, 5 c_b, 6 S), each at its
-    map's own frame count: ceil(Tmax / k) from map L = subsampleLayer up."""
+    utterances of at most Tmax frames (what 0 X, 1 For / h_f, 2 Back / h_b, 3 gates, 4 c_f, 5 c_b, 6 S, and with
+    selfCondition 12 X'_m and 13 P), each at its map's own frame count: ceil(Tmax / k) from map L = subsampleLayer up
+    (X'_m and P at layer m's)."""
     from _ctcb import lib
     off, width = ctypes.c_size_t(), ctypes.c_int32()
     out = {}
-    for what in range(7):
+    for what in list(range(7)) + ([12, 13] if nn.selfCondition else []):
         for layer in range(nn.numLayers + 2):
             if lib.ctcb_brnn_activation_offset(ctypes.byref(nn._cfg), what, layer, ctypes.byref(off),
                                                ctypes.byref(width)) != 0:
                 continue
-            T = nn.frames(Tmax) if what == 6 or (nn.subsample > 1 and layer >= nn.subsampleLayer) else Tmax
+            rate = nn.interLayer if what >= 12 else layer
+            T = nn.frames(Tmax) if what == 6 or (nn.subsample > 1 and rate >= nn.subsampleLayer) else Tmax
             n = T * B * width.value
             out[what, layer] = nn._ws[off.value:off.value + 4 * n].view(nn._torch.float32).cpu().numpy() \
                 .reshape(T, B, width.value)
@@ -58,6 +60,9 @@ def compare(nn, oracle, datas, labelss, lens, utts=None):
       skips        the device's skips; skips_own / skips_given the oracle's on its own and on the device's activations
       cost_own     largest relative error of the device's costs against the oracle's own (non-skipped utterances)
       cost_given   the same against the oracle's costs on the device's activations
+      inter_cost, inter_skips, inter_skips_own (interLayer only)
+                   largest relative error of the device's intermediate nll against the oracle's own (utterances the
+                   device's intermediate CTC keeps), the device's intermediate skips and the oracle's own
       fwd          {kind: largest relmax over the utterances}: X (list, layers 1..N+1, each layer's output: For of a
                    uni-directional clipped-ReLU layer, h_f + h_b of an LSTM layer), For and Back (clipped-ReLU), gates,
                    h and c (LSTM), S (subsampling)
@@ -77,7 +82,7 @@ def compare(nn, oracle, datas, labelss, lens, utts=None):
     reg, oracle.reg = oracle.reg, 0.0
     own = [[np.zeros_like(w), np.zeros_like(b)] for w, b in oracle.stack]
     given = [[np.zeros_like(w), np.zeros_like(b)] for w, b in oracle.stack]
-    c_own, c_given, s_own, s_given = [], [], [], []
+    c_own, c_given, s_own, s_given, i_own, i_skip = [], [], [], [], [], []
     fwd = dict(X=[0.0] * (N + 1))
     kinds = (["h", "c", "gates"] if lstm else ["For"] + ([] if oracle.unidirectional else ["Back"])) if temporal else []
     fwd.update((kind, 0.0) for kind in kinds + (["S"] if k > 1 else []))
@@ -111,17 +116,22 @@ def compare(nn, oracle, datas, labelss, lens, utts=None):
                 fwd["X"][i - 1] = max(fwd["X"][i - 1], relmax(act, hActs[i]))
             if k > 1:
                 fwd["S"] = max(fwd["S"], relmax(acts[6, 0][:frames(lens[u], k), u].T, stack_frames(hActs[L - 1], k)))
+            cond = None
+            if oracle.selfCondition:
+                Tm = frames(lens[u], k) if oracle.interLayer >= L > 0 else lens[u]
+                cond = (acts[12, 0][:Tm, u].T, acts[13, 0][:Tm, u].T)
             for path, tot, c_, s_ in (((hActs, o_temp, probs), own, c_own, s_own), (None, given, c_given, s_given)):
                 if path is None:
-                    c, g, s = oracle.costAndGradGiven(d, l, g_acts, g_temp)
+                    c, g, s = oracle.costAndGradGiven(d, l, g_acts, g_temp, cond=cond)
                 else:
                     c, g, s = oracle.costAndGrad(d, l, _given=path)
+                    i_own.append(oracle.interCost)
+                    i_skip.append(oracle.interSkip)
                 c_.append(c)
                 s_.append(bool(s))
-                if not s:
-                    for (tw, tb), (gw, gb) in zip(tot, g):
-                        tw += gw
-                        tb += gb
+                for (tw, tb), (gw, gb) in zip(tot, g):     # a main skip adds the intermediate gradient alone
+                    tw += gw
+                    tb += gb
     finally:
         oracle.reg = reg
     for tot in (own, given):
@@ -140,9 +150,13 @@ def compare(nn, oracle, datas, labelss, lens, utts=None):
         grad_given.append(rel(x, y))
         grad_elem.append(relmax(x, y))
         grad_plain.append(rel(x, z))
-    ok = ~skips
-    cost_err = lambda ref: float(np.max(np.abs(costs[ok] - np.array(ref)[ok]) / np.abs(np.array(ref)[ok]))) \
+    cost_err = lambda got, ref, ok: float(np.max(np.abs(got[ok] - np.array(ref)[ok]) / np.abs(np.array(ref)[ok]))) \
         if ok.any() else 0.0     # noqa: E731
-    return dict(acts=acts, skips=skips, skips_own=np.array(s_own), skips_given=np.array(s_given),
-                cost_own=cost_err(c_own), cost_given=cost_err(c_given), fwd=fwd, grad_given=grad_given,
-                grad_given_elem=grad_elem, grad_plain=grad_plain)
+    out = dict(acts=acts, skips=skips, skips_own=np.array(s_own), skips_given=np.array(s_given),
+               cost_own=cost_err(costs, c_own, ~skips), cost_given=cost_err(costs, c_given, ~skips), fwd=fwd,
+               grad_given=grad_given, grad_given_elem=grad_elem, grad_plain=grad_plain)
+    if oracle.interLayer:
+        iskips = np.asarray(nn.interSkips[:B], dtype=bool)
+        out.update(inter_cost=cost_err(np.asarray(nn.interCosts[:B], np.float64), i_own, ~iskips), inter_skips=iskips,
+                   inter_skips_own=np.array(i_skip))
+    return out

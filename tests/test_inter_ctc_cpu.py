@@ -1,15 +1,13 @@
 """CPU tests of the intermediate CTC loss (ctcb_brnn_config.interLayer): the float64 restatement
-(tests/inter_ctc_oracle.InterNet) against central differences of its objective and, at interLayer = 0, against Net bit
-for bit; the config and NNet refusals; the exact workspace growth; the runNNet flags."""
+(tests/net_oracle.Net) against central differences of its objective, its intermediate term against the head net's loss,
+each CTC skipping on its own; the config and NNet refusals; the exact workspace growth; the runNNet flags."""
 import ctypes
 
 import numpy as np
 import pytest
 
 import recipes
-from inter_ctc_oracle import InterNet
 from net_oracle import Net
-from peephole_oracle import PeepholeNet
 
 D, K, H = 5, 6, 6
 NETS = {
@@ -25,21 +23,18 @@ NETS = {
 }
 
 
-def _net(name, lam=0.7, round_f32=False, reg=1e-3, cls=InterNet, **extra):
+def _net(name, lam=0.7, round_f32=False, reg=1e-3):
     c = dict(NETS[name])
     N, tl, m = c.pop("N"), c.pop("tl"), c.pop("m")
-    kw = dict(temporalLayer=tl, reg=reg, round_f32=round_f32, dropoutSeed=5, **c)
-    if cls is InterNet:
-        kw.update(interLayer=m if lam else 0, interWeight=lam)
-    elif cls is Net:
-        kw.pop("peephole", None)
+    kw = dict(temporalLayer=tl, reg=reg, round_f32=round_f32, dropoutSeed=5, interLayer=m if lam else 0,
+              interWeight=lam, **c)
     np.random.seed(11)
-    net = cls(D, K, H, N, 40, **kw, **extra)
+    net = Net(D, K, H, N, 40, **kw)
     net.initParams()
     rng = np.random.RandomState(6)
     for w, b in net.stack[:N + 1]:     # no hidden unit sits exactly on its ReLU kink where a column of X is all 0
         b[...] = rng.uniform(-0.1, 0.1, b.shape)
-    if getattr(net, "peephole", False):
+    if net.peephole:
         rng = np.random.RandomState(4)
         for k in range(len(net.stack) - net.entries(), len(net.stack)):
             net.stack[k][0][...] = rng.uniform(-0.5, 0.5, net.stack[k][0].shape)
@@ -95,28 +90,6 @@ def test_intermediate_term_is_the_head_nets_loss_and_reaches_only_the_head(name)
     assert not np.array_equal(g1[with_.numLayers][0], g0[with_.numLayers][0])
 
 
-@pytest.mark.parametrize("name", [n for n in NETS if not NETS[n].get("peephole")])
-def test_off_is_net_bit_for_bit(name):
-    off = _net(name, lam=0.0, round_f32=True)
-    ref = _net(name, round_f32=True, cls=Net)
-    data, labels = _data()
-    c0, g0, s0 = off.costAndGrad(data, labels)
-    c1, g1, s1 = ref.costAndGrad(data, labels)
-    assert c0 == c1 and s0 == s1
-    for (a, b), (x, y) in zip(g0, g1):
-        assert np.array_equal(a, x) and np.array_equal(b, y)
-    assert np.array_equal(off.forward(data)[2], ref.forward(data)[2])
-
-
-def test_off_is_peephole_net_bit_for_bit():
-    off = _net("lstm_peep_k2_m_temporal", lam=0.0, round_f32=True)
-    ref = _net("lstm_peep_k2_m_temporal", round_f32=True, cls=PeepholeNet)
-    data, labels = _data()
-    c0, g0, _ = off.costAndGrad(data, labels)
-    c1, g1, _ = ref.costAndGrad(data, labels)
-    assert c0 == c1 and all(np.array_equal(a, x) and np.array_equal(b, y) for (a, b), (x, y) in zip(g0, g1))
-
-
 def test_each_ctc_skips_on_its_own():
     """Below the subsampling point the intermediate CTC has T frames where the main one has ceil(T / 2): five equal
     labels need nine frames, so the main CTC alone skips that utterance, which still gets the intermediate gradient."""
@@ -134,7 +107,7 @@ def test_oracle_refusals():
                dict(interLayer=3, interWeight=0.5), dict(interLayer=-1, interWeight=0.5),
                dict(interLayer=1, interWeight=0.5, subsample=2, subsampleLayer=4)):
         with pytest.raises(ValueError):
-            InterNet(D, K, H, 3, 20, temporalLayer=2, **kw)
+            Net(D, K, H, 3, 20, temporalLayer=2, **kw)
 
 
 # ------------------------------------------------------------------------------------------------------- C ABI

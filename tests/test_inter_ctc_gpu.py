@@ -1,6 +1,6 @@
 """GPU tests of the intermediate CTC loss (ctcb_brnn_config.interLayer) on one H100.
 
-Whole nets against tests/inter_ctc_oracle.InterNet (tests/net_check.py): the per-utterance intermediate nll and every
+Whole nets against tests/net_oracle.Net (tests/net_check.py): the per-utterance intermediate nll and every
 gradient tensor.  Then the two CTCs skipping on their own, the statistics tail, micro-batches and emulated shards,
 graph replay and forced stalls bit for bit, forward-only probabilities bit for bit with the net without the loss,
 checkpoints in both directions, check_grad, the SGD log line and runNNet.  Each comparison prints its measured numbers
@@ -12,8 +12,8 @@ import numpy as np
 import pytest
 
 import recipes
-from inter_ctc_oracle import InterNet
 from net_check import bits as _bits, compare, rel as _rel
+from net_oracle import Net
 from recipes import knobs  # noqa: F401  (fixture)
 
 pytestmark = pytest.mark.gpu
@@ -48,7 +48,7 @@ def _gpu_net(c, B, reg=0.0, lam=LAM, train=True):
 
 
 def _oracle(c, reg, lam=LAM):
-    return InterNet(D, K, c["H"], c["N"], c["T"], **_kwargs(c, reg, lam))
+    return Net(D, K, c["H"], c["N"], c["T"], **_kwargs(c, reg, lam))
 
 
 def _batch(c, seed=5):
@@ -88,20 +88,18 @@ def _pair(c, B, reg):
 
 @pytest.mark.parametrize("name", list(NETS))
 def test_net_matches_float64_oracle(name, cuda):
-    """The device's training call against InterNet: the main costs, the intermediate nll of every utterance, and every
-    gradient tensor against the back-propagation through the device's own activations."""
+    """The device's training call against the float64 net: the main costs, the intermediate nll of every utterance,
+    and every gradient tensor against the back-propagation through the device's own activations."""
     import torch
     c = NETS[name]
     lens, (datas, labelss) = _batch(c)
     nn, on = _pair(c, c["B"], 1e-3)
     nn.costAndGradBatch(datas, labelss)
     torch.cuda.synchronize()
-    icost, iskip = nn.interCosts.copy(), nn.interSkips.copy()
     r = compare(nn, on, datas, labelss, lens)
-    on.costAndGradBatch(datas, labelss)
     assert np.array_equal(r["skips"], r["skips_own"]) and not r["skips"].any()
-    assert np.array_equal(iskip, on.interSkips) and not iskip.any()
-    inter = float(np.max(np.abs(icost - on.interCosts) / np.abs(on.interCosts)))
+    assert np.array_equal(r["inter_skips"], r["inter_skips_own"]) and not r["inter_skips"].any()
+    inter = r["inter_cost"]
     grad_err = r["grad_given"]
     print(json.dumps({"inter_ctc_net_" + name: dict(cost=r["cost_own"], inter_cost=inter,
                                                     grad_given_frob_max=max(grad_err),

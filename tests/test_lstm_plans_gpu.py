@@ -13,7 +13,7 @@ Forward: every output x (gates, c, h) satisfies |x - x64| <= C_FWD u S, u = 2^-2
 from the GPU's own state of the step before and S the sum of the magnitudes of the terms that make x (1 + |pre| +
 |U| |h_prev| (+ |p| |c|) for a gate, |f c_prev| + |i g| for c, |o| for h); and where z is exact (h_prev = 0) the
 activation alone, |a - a64| <= C_ACT u |a64|, which is what sees a less accurate exp or tanh at large |z|.  BPTT: dz
-against the float64 BPTT of the GPU's own forward activations (net_oracle / peephole_oracle), |dz - dz64| <= C_BPTT u S
+against the float64 BPTT of the GPU's own forward activations (net_oracle), |dz - dz64| <= C_BPTT u S
 with S = max |dz64| of that utterance and direction, no floor: the bound is scale-free, and exact linearity in dh
 (below) is what makes that sound.  Exact: padded frames 0 (outputs start as NaN), NaN guard bands around gates, h, c,
 dz and the scratch unchanged, the error flag 0, a rerun gives the same bytes, dh 2^-20 gives dz 2^-20 where no dz
@@ -28,7 +28,6 @@ import numpy as np
 import pytest
 
 import net_oracle
-import peephole_oracle
 from recipes import knobs  # noqa: F401  (fixture)
 
 pytestmark = pytest.mark.gpu
@@ -238,11 +237,9 @@ def _check_bptt(r, sw):
             blk = slice(d * 4 * H, (d + 1) * 4 * H)
             g = r["gates"][:Tu, u, blk].T.astype(np.float64)
             c, h = r["c"][d][:Tu, u].T.astype(np.float64), r["h"][d][:Tu, u].T.astype(np.float64)
-            if sw.Ps is None:
-                dz64 = net_oracle.lstm_direction_bptt(dh, g, c, h, Us[d], reverse=(d == 1))[0]
-            else:
-                dz64 = peephole_oracle.lstm_direction_bptt(dh, g, c, h, Us[d], reverse=(d == 1),
-                                                           peephole=sw.Ps[d].astype(np.float64))[0]
+            P = np.zeros((3, H)) if sw.Ps is None else sw.Ps[d].astype(np.float64)
+            zero = np.zeros((H, Tu))     # no zoneout
+            dz64 = net_oracle.lstm_direction_bptt(dh, g, c, h, Us[d], d == 1, P, zero, zero)[0]
             S = float(np.max(np.abs(dz64)))
             assert S > 0.0, "utterance %d direction %d has no gradient to compare" % (u, d)
             worst = max(worst, float(np.max(np.abs(r["dz"][:Tu, u, blk].T - dz64))) / (U32 * S))

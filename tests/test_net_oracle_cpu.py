@@ -1,6 +1,8 @@
 """CPU tests of the float64 restatement of the net (tests/net_oracle.py): with every feature off it is the pinned oracle
 (oracle/brnn_oracle.py), it draws the library's tensor table, its gradient is the central difference of its cost for
-every feature (stacked, uni-directional, DNN, dropout, LSTM, layer norm, subsampling), and back-propagation through
+every feature (stacked, uni-directional, DNN, dropout, LSTM, layer norm, subsampling) and for nets that combine
+peepholes, zoneout and the intermediate or self-conditioned CTC (each feature alone is in its own CPU file), and
+back-propagation through
 given activations is the same as through its own; its LSTM cell and normalisation are torch's and its subsampled
 nets torch autograd's.  No compute call is made on a device here."""
 import ctypes
@@ -127,9 +129,10 @@ def _gradcheck_one(net, seed, probes):
 
 
 def _gradcheck_batch(net, lens, nlabs, rng_seed, scale=1.0, every_pair_entry=False):
-    """A ragged batch, reg > 0, weights times `scale` and gamma, beta moved off 1, 0: 3 entries of every tensor (every
-    entry of the [gamma, beta] pairs with every_pair_entry, one more in each sub-frame block of W_L) against the central
-    difference of the summed cost, |analytic - numeric| <= 1e-6 max(1, |numeric|)."""
+    """A ragged batch, reg > 0, weights times `scale`, gamma, beta moved off 1, 0 and P, W_c, b_c off 0: 3 entries of
+    every tensor (every entry of the tensors behind the recurrent ones with every_pair_entry, one more in each sub-frame
+    block of W_L) against the central difference of the summed objective (main + lambda intermediate),
+    |analytic - numeric| <= 1e-6 max(1, |numeric|)."""
     np.random.seed(11)
     net.initParams()
     for w, _ in net.stack:
@@ -139,14 +142,23 @@ def _gradcheck_batch(net, lens, nlabs, rng_seed, scale=1.0, every_pair_entry=Fal
         gamma, beta = net.stack[net.ln_index(i)]
         gamma += 0.3 * rng.randn(*gamma.shape)
         beta += 0.3 * rng.randn(*beta.shape)
+    for w, b in net.stack[net.peep_index(0, 0):]:      # [P, dummy] and [W_c, b_c], behind the [gamma, beta] pairs
+        w[...] = rng.uniform(-0.5, 0.5, w.shape)
+        if b.shape != (1, 1):
+            b[...] = rng.uniform(-0.1, 0.1, b.shape)
     datas, labels = recipes.synth_batch(net.inputDim, net.outputDim, lens, nlabs, seed=3)
     _, grad, skips = net.costAndGradBatch(datas, labels)
-    assert not skips.any()
+    assert not skips.any() and not (net.interLayer and net.interSkips.any())
     N = net.numLayers
     base = N + 1 + net.numTemporal * net.nrec
     if net.layerNorm:
-        assert len(net.stack) - base == len(net.normedLayers()) > 0
-    f = lambda: net.costAndGradBatch(datas, labels)[0].sum() + net.regcost        # noqa: E731
+        assert len(net.stack) - base == len(net.normedLayers()) + net.entries() + net.selfCondition
+        assert len(net.normedLayers()) > 0
+
+    def f():
+        costs = net.costAndGradBatch(datas, labels)[0]
+        inter = net.lam() * net.interCosts.sum() if net.interLayer else 0.0
+        return costs.sum() + net.regcost + inter
     for ti, (w, b) in enumerate(net.stack):
         for x, gx in ((w, grad[ti][0]), (b, grad[ti][1])):
             if N < ti < base and x is b:        # the recurrent matrices' dummies take no part
@@ -212,6 +224,19 @@ def _subsampled(name, **kw):
 
 for _name in SUBSAMPLE:
     FD["subsample_" + _name] = (_subsampled(_name), dict(recipe="batch", lens=LENS, nlabs=NLABS, rng_seed=2))
+# feature combinations: every tensor, P, W_c and b_c in full
+FD["combo_bi_lstm_peep_zoneout_selfcond_ln_drop"] = (
+    dict(dims=(5, 6, 6, 3, 13), temporalLayer=2, cell="lstm", peephole=True, zoneoutCell=0.3, zoneoutHidden=0.2,
+         interLayer=2, interWeight=0.7, selfCondition=True, layerNorm=True, dropout=0.3, dropoutSeed=5),
+    dict(recipe="batch", lens=LENS, nlabs=NLABS, rng_seed=2, every_pair_entry=True))
+FD["combo_uni_lstm_zoneout_inter_sub_below"] = (
+    dict(dims=(5, 6, 6, 4, 13), temporalLayer=2, numTemporal=2, unidirectional=True, cell="lstm", zoneoutCell=0.3,
+         zoneoutHidden=0.2, interLayer=2, interWeight=0.7, subsample=2, subsampleLayer=1, dropoutSeed=5),
+    dict(recipe="batch", lens=LENS, nlabs=NLABS, rng_seed=2, every_pair_entry=True))
+FD["combo_bi_lstm_peep_zoneout_k2_selfcond_top"] = (
+    dict(dims=(5, 6, 6, 4, 13), temporalLayer=2, numTemporal=2, cell="lstm", peephole=True, zoneoutCell=0.2,
+         zoneoutHidden=0.3, interLayer=3, interWeight=0.5, selfCondition=True, dropout=0.2, dropoutSeed=5),
+    dict(recipe="batch", lens=LENS, nlabs=NLABS, rng_seed=2, every_pair_entry=True))
 
 
 @pytest.mark.parametrize("name", list(FD))
@@ -285,10 +310,11 @@ def test_oracle_matches_torch_lstm(uni):
         loss.backward()
         pre = W.dot(x) + b[:, None]
         dz_all = []
+        plain = (np.zeros((3, H)), np.zeros((H, T)), np.zeros((H, T)))     # no peepholes, no zoneout
         for d in range(ndir):
-            gates, c, h = lstm_direction(pre[d * 4 * H:(d + 1) * 4 * H], Us[d], reverse=(d == 1))
+            gates, c, h = lstm_direction(pre[d * 4 * H:(d + 1) * 4 * H], Us[d], d == 1, *plain)
             np.testing.assert_allclose(h, out[d * H:(d + 1) * H].detach().numpy(), rtol=1e-12, atol=1e-13)
-            dz, dU = lstm_direction_bptt(Rw, gates, c, h, Us[d], reverse=(d == 1))
+            dz, dU, _ = lstm_direction_bptt(Rw, gates, c, h, Us[d], d == 1, *plain)
             np.testing.assert_allclose(dU, getattr(lstm, "weight_hh_l0" + sfx[d]).grad.numpy(), rtol=1e-10, atol=1e-12)
             dz_all.append(dz)
         dz = np.concatenate(dz_all)

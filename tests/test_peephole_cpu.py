@@ -1,5 +1,5 @@
 """CPU tests of the peephole connections of the LSTM cell (ctcb_brnn_config.peephole = 1): the float64 restatement
-(tests/peephole_oracle.py) with P = 0 is tests/net_oracle.py's net without peepholes, bit for bit; with P drawn
+(tests/net_oracle.py) with peepholes and P = 0 is its net without peepholes, bit for bit; with P drawn
 non-zero it agrees with an independent torch-autograd restatement of the cell and with central differences on every
 tensor; peephole = 0 answers
 every config query as before; the config contract and the tensor table of peephole = 1; runNNet's flag."""
@@ -11,8 +11,7 @@ import pytest
 
 import config_matrix
 import recipes
-from net_oracle import Net
-from peephole_oracle import PeepholeNet, lstm_direction, lstm_direction_bptt
+from net_oracle import Net, lstm_direction, lstm_direction_bptt
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
@@ -37,7 +36,7 @@ def test_zero_peepholes_are_the_cell_without_them(kw):
     nets = []
     for peep in (False, True):
         np.random.seed(4)
-        n = (PeepholeNet if peep else Net)(7, 5, 6, 3, 9, cell="lstm", reg=1e-3, round_f32=False, **kw)
+        n = Net(7, 5, 6, 3, 9, cell="lstm", reg=1e-3, round_f32=False, peephole=peep, **kw)
         n.initParams()
         nets.append(n)
     off, on = nets
@@ -94,9 +93,10 @@ def test_oracle_cell_matches_torch_autograd(reverse):
         P = rng.uniform(-0.5, 0.5, (3, H))
         R = rng.randn(H, T)
         h_t, dpre, dU_t, dP_t = _torch_peephole_direction(pre, U, P, reverse, R)
-        gates, c, h = lstm_direction(pre, U, reverse, peephole=P)
+        zero = np.zeros((H, T))     # no zoneout
+        gates, c, h = lstm_direction(pre, U, reverse, P, zero, zero)
         np.testing.assert_allclose(h, h_t, rtol=1e-12, atol=1e-14)
-        dz, dU, dP = lstm_direction_bptt(R, gates, c, h, U, reverse, peephole=P)
+        dz, dU, dP = lstm_direction_bptt(R, gates, c, h, U, reverse, P, zero, zero)
         np.testing.assert_allclose(dz, dpre, rtol=1e-10, atol=1e-13)
         np.testing.assert_allclose(dU, dU_t, rtol=1e-10, atol=1e-13)
         np.testing.assert_allclose(dP, dP_t, rtol=1e-10, atol=1e-13)
@@ -133,7 +133,7 @@ def test_oracle_gradient_matches_central_differences(name):
     """P drawn non-zero, reg > 0, weights twice the initial scale, biases off 0: 3 entries of every tensor (every entry
     of every P) against the central difference of the summed cost, |analytic - numeric| <= 1e-6 max(1, |numeric|)."""
     kw, lens = dict(FD[name][0]), FD[name][1]
-    net = PeepholeNet(*kw.pop("dims"), reg=1e-3, round_f32=False, cell="lstm", **kw)
+    net = Net(*kw.pop("dims"), reg=1e-3, round_f32=False, cell="lstm", peephole=True, **kw)
     np.random.seed(11)
     net.initParams()
     for w, _ in net.stack:
@@ -166,7 +166,7 @@ def test_oracle_gradient_matches_central_differences(name):
 def test_back_propagation_through_given_activations_is_the_same():
     """costAndGradGiven on the net's own activations = costAndGrad, bit for bit, with non-zero P."""
     np.random.seed(2)
-    nn = PeepholeNet(7, 5, 12, 4, 9, temporalLayer=2, numTemporal=2, cell="lstm", round_f32=False)
+    nn = Net(7, 5, 12, 4, 9, temporalLayer=2, numTemporal=2, cell="lstm", peephole=True, round_f32=False)
     nn.initParams()
     _draw_p(nn, 4)
     data = np.random.RandomState(1).randn(7, 9)
@@ -182,7 +182,7 @@ def test_back_propagation_through_given_activations_is_the_same():
 
 def test_oracle_refuses_peepholes_without_the_lstm_cell():
     with pytest.raises(ValueError, match="peephole.*cell='lstm'.*'relu'"):
-        PeepholeNet(7, 5, 6, 3, 9, temporalLayer=2)
+        Net(7, 5, 6, 3, 9, temporalLayer=2, peephole=True)
 
 
 # ------------------------------------------------------------------------------------------- the config contract

@@ -2,7 +2,7 @@
 
 The sweep alone in peephole mode (ctcb_lstm_sweep_peephole_f32), on every plan, and the peephole weight gradients
 alone (ctcb_lstm_peephole_grad_f32) are tests/test_lstm_plans_gpu.py.  Here the whole net against
-peephole_oracle.PeepholeNet (tests/net_check.py) with P drawn non-zero, and micro-batches, shards, graph
+tests/net_oracle.Net (tests/net_check.py) with P drawn non-zero, and micro-batches, shards, graph
 replay, forward-only probabilities, runNNet and checkpoints.  Each comparison prints its measured numbers as one JSON
 line (pytest -s)."""
 import json
@@ -14,7 +14,7 @@ import pytest
 
 import recipes
 from net_check import bits as _bits, compare, rel as _rel
-from peephole_oracle import PeepholeNet
+from net_oracle import Net
 
 pytestmark = pytest.mark.gpu
 COST_TOL, FWD_TOL, GRAD_TOL = 1e-4, 1e-4, 1e-4
@@ -34,7 +34,7 @@ NETS = {
 
 
 def _kwargs(c, reg=0.0):
-    """The keyword arguments of nnets.brnnet.NNet and peephole_oracle.PeepholeNet that make net c."""
+    """The keyword arguments of nnets.brnnet.NNet and net_oracle.Net that make net c."""
     k, L = c.get("sub", (1, 1))
     return dict(temporalLayer=c["tl"], numTemporal=c["k"], reg=reg, unidirectional=bool(c.get("uni")), cell="lstm",
                 peephole=True, layerNorm=bool(c.get("ln")), dropout=c.get("p", 0.0), dropoutSeed=5, subsample=k,
@@ -85,7 +85,7 @@ def test_peephole_net_matches_float64_oracle(name, cuda):
     nn = _gpu_net(c, B, reg=reg)
     nn.initParams()
     np.random.seed(21)
-    on = PeepholeNet(D, K, H, N, c["T"], **_kwargs(c, reg))
+    on = Net(D, K, H, N, c["T"], **_kwargs(c, reg))
     on.initParams()
     for (w, b), (ow, ob) in zip(nn.stack, on.stack):        # the same draws, shapes and order, P = 0
         assert np.array_equal(w.cpu().numpy(), ow.astype(np.float32)) and tuple(b.shape) == ob.shape
@@ -118,7 +118,7 @@ def test_forward_only_probs_are_bit_identical_to_a_training_call(cuda):
         np.random.seed(3)
         nn = _gpu_net(c, c["B"])
         nn.initParams()
-        on = PeepholeNet(D, K, c["H"], c["N"], c["T"], **_kwargs(c))
+        on = Net(D, K, c["H"], c["N"], c["T"], **_kwargs(c))
         np.random.seed(3)
         on.initParams()
         _set_p(nn, on)

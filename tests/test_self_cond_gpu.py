@@ -1,11 +1,10 @@
 """GPU tests of self-conditioned CTC (ctcb_brnn_config.selfCondition) on one H100.
 
 The row-softmax backward kernel against float64; the InterCTC test's nine whole nets with random non-zero W_c, b_c
-against tests/self_cond_oracle.SelfCondNet; at W_c = b_c = 0 the InterCTC net; forward-only probabilities bit for bit
+against tests/net_oracle.Net; at W_c = b_c = 0 the InterCTC net; forward-only probabilities bit for bit
 with a training call's; micro-batches and emulated shards, forced stalls and graph replay for m below, at and above
 the lowest temporal layer; two ranks over NCCL (skipped with fewer than 2 GPUs); checkpoints, check_grad and runNNet.
 Each comparison prints its measured numbers as one JSON line (pytest -s)."""
-import ctypes
 import json
 import os
 import pickle
@@ -18,7 +17,7 @@ import pytest
 import recipes
 from net_check import bits as _bits, compare, rel as _rel
 from recipes import knobs  # noqa: F401  (fixture)
-from self_cond_oracle import SelfCondNet
+from net_oracle import Net
 from test_inter_ctc_gpu import NETS, D, K, LAM, _batch, _kwargs, _ragged
 
 pytestmark = pytest.mark.gpu
@@ -87,7 +86,7 @@ def _pair(c, B, reg, wc=True):
     nn = _gpu_net(c, B, reg=reg)
     nn.initParams()
     np.random.seed(21)
-    on = SelfCondNet(D, K, c["H"], c["N"], c["T"], selfCondition=True, **_kwargs(c, reg))
+    on = Net(D, K, c["H"], c["N"], c["T"], selfCondition=True, **_kwargs(c, reg))
     on.initParams()
     if c.get("peep"):
         n = nn.peepholeEntries()
@@ -104,22 +103,9 @@ def _pair(c, B, reg, wc=True):
     return nn, on
 
 
-def _ws(nn, what, T, B):
-    """[T][B][width] float32 of kind `what` of the net's last training call."""
-    from _ctcb import lib
-    off, width = ctypes.c_size_t(), ctypes.c_int32()
-    assert lib.ctcb_brnn_activation_offset(ctypes.byref(nn._cfg), what, 0, ctypes.byref(off), ctypes.byref(width)) == 0
-    n = T * B * width.value
-    return nn._ws[off.value:off.value + 4 * n].view(nn._torch.float32).cpu().numpy().reshape(T, B, width.value)
-
-
-def _cond_frames(nn, T):
-    return nn.frames(T) if nn.subsample > 1 and nn.interLayer >= nn.subsampleLayer else T
-
-
 @pytest.mark.parametrize("name", list(NETS))
 def test_net_matches_float64_oracle(name, cuda):
-    """The device's training call against SelfCondNet: the main costs, the intermediate nll of every utterance, and
+    """The device's training call against the float64 net: the main costs, the intermediate nll of every utterance, and
     every gradient tensor (W_c and b_c included) against the back-propagation through the device's own activations,
     X'_m and P."""
     import torch
@@ -128,17 +114,10 @@ def test_net_matches_float64_oracle(name, cuda):
     nn, on = _pair(c, c["B"], 1e-3)
     nn.costAndGradBatch(datas, labelss)
     torch.cuda.synchronize()
-    icost, iskip = nn.interCosts.copy(), nn.interSkips.copy()
-    B, Tm = len(datas), _cond_frames(nn, max(lens))
-    Xp, P = _ws(nn, 12, Tm, B), _ws(nn, 13, Tm, B)
-    fr = [_cond_frames(nn, n) for n in lens]
-    on.givenCond = {u: (Xp[:fr[u], u].T, P[:fr[u], u].T) for u in range(B)}
     r = compare(nn, on, datas, labelss, lens)
-    on.givenCond = None
-    on.costAndGradBatch(datas, labelss)
     assert np.array_equal(r["skips"], r["skips_own"]) and not r["skips"].any()
-    assert np.array_equal(iskip, on.interSkips) and not iskip.any()
-    inter = float(np.max(np.abs(icost - on.interCosts) / np.abs(on.interCosts)))
+    assert np.array_equal(r["inter_skips"], r["inter_skips_own"]) and not r["inter_skips"].any()
+    inter = r["inter_cost"]
     grad_err = r["grad_given"]
     print(json.dumps({"self_cond_net_" + name: dict(cost=r["cost_own"], inter_cost=inter,
                                                     grad_given_frob_max=max(grad_err),

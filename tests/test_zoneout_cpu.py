@@ -1,7 +1,6 @@
-"""CPU tests of zoneout on the LSTM cell: the mask restatement (tests/zoneout_oracle.py) against a plain loop, its keep
-rates, its counters against the other draws of a seed, the float64 cell against Net / PeepholeNet at z = 0, against a
-torch-autograd restatement and against central differences, and the C ABI's config, setter, workspace and runNNet
-contract (no device work)."""
+"""CPU tests of zoneout on the LSTM cell: the mask restatement (tests/net_oracle.py) against a plain loop, its keep
+rates, its counters against the other draws of a seed, the float64 cell against a torch-autograd restatement and
+against central differences, and the C ABI's config, setter, workspace and runNNet contract (no device work)."""
 import ctypes
 
 import numpy as np
@@ -9,9 +8,7 @@ import pytest
 import torch
 from scipy import stats
 
-import zoneout_oracle as zo
-from net_oracle import Net, philox4x32_10
-from peephole_oracle import PeepholeNet
+from net_oracle import Net, lstm_direction, lstm_direction_bptt, philox4x32_10, zoneout_masks, zoneout_threshold
 
 
 def _loop_masks(zc, zh, seed, step, layer, d, g, T, H):
@@ -34,7 +31,7 @@ def _loop_masks(zc, zh, seed, step, layer, d, g, T, H):
 ])
 def test_restatement_equals_a_plain_loop(case):
     zc, zh, seed, step, layer, d, g, T, H = case
-    lc, lh = zo.masks(zc, zh, seed, step, layer, d, g, T, H)
+    lc, lh = zoneout_masks(zc, zh, seed, step, layer, d, g, T, H)
     wc, wh = _loop_masks(zc, zh, seed, step, layer, d, g, T, H)
     assert np.array_equal(lc, wc) and np.array_equal(lh, wh)
 
@@ -42,12 +39,12 @@ def test_restatement_equals_a_plain_loop(case):
 @pytest.mark.parametrize("z", [0.05, 0.15, 0.5, 0.9])
 def test_keep_rates_follow_their_binomial_law(z):
     """The kept count of 200 x 256 units is Binomial(n, floor(z 2^32) / 2^32): a two-sided 1e-6 test, per word."""
-    lc, lh = zo.masks(z, z, 7, 3, 2, 1, 5, 200, 256)
-    p = zo.threshold(z) / 2.0 ** 32
+    lc, lh = zoneout_masks(z, z, 7, 3, 2, 1, 5, 200, 256)
+    p = zoneout_threshold(z) / 2.0 ** 32
     for m in (lc, lh):
         assert stats.binomtest(int(m.sum()), m.size, p).pvalue > 1e-6
     assert 0.0 < np.mean(lc != lh) < 1.0 or z == 0.0        # the two words are separate draws
-    lc0, lh0 = zo.masks(0.0, 0.0, 7, 3, 2, 1, 5, 50, 64)
+    lc0, lh0 = zoneout_masks(0.0, 0.0, 7, 3, 2, 1, 5, 50, 64)
     assert not lc0.any() and not lh0.any()
 
 
@@ -84,37 +81,17 @@ def _data(T=9, seed=3, L=3):
     return rng.randn(D, T).astype(np.float32).astype(np.float64), rng.randint(1, K, size=L).astype(np.int32)
 
 
-def _nets(name, peephole, round_f32=True, **z):
+def _net(name, peephole, round_f32=True, **z):
     kw = dict(NETS[name], cell="lstm", reg=1e-3, dropoutSeed=5, round_f32=round_f32)
     np.random.seed(4)
-    base = PeepholeNet(D, K, 6, 4, 20, peephole=True, **kw) if peephole else Net(D, K, 6, 4, 20, **kw)
-    base.initParams()
-    np.random.seed(4)
-    net = zo.ZoneoutNet(D, K, 6, 4, 20, peephole=peephole, **kw, **z)
+    net = Net(D, K, 6, 4, 20, peephole=peephole, **kw, **z)
     net.initParams()
     if peephole:
         rng = np.random.RandomState(8)
         for k in range(len(net.stack) - net.entries(), len(net.stack), 2):
-            base.stack[k][0][...] = net.stack[k][0][...] = rng.uniform(-0.5, 0.5, net.stack[k][0].shape)
-    for n in (base, net):
-        n.dropoutStep, n.utt = 2, 1
-    return base, net
-
-
-@pytest.mark.parametrize("peephole", [False, True])
-@pytest.mark.parametrize("name", list(NETS))
-def test_zero_probabilities_equal_the_plain_and_peephole_oracles_bit_for_bit(name, peephole):
-    base, net = _nets(name, peephole)
-    data, labels = _data()
-    for expectation in (False, True):
-        net.expectation = expectation
-        h0, t0, p0 = base.forward(data)
-        h1, t1, p1 = net.forward(data)
-        assert all(np.array_equal(a, b) for a, b in zip(h0, h1)) and np.array_equal(p0, p1)
-        c0, g0, _ = base.costAndGrad(data, labels)
-        c1, g1, _ = net.costAndGrad(data, labels)
-        assert c0 == c1
-        assert all(np.array_equal(a, b) for x, y in zip(g0, g1) for a, b in zip(x, y))
+            net.stack[k][0][...] = rng.uniform(-0.5, 0.5, net.stack[k][0].shape)
+    net.dropoutStep, net.utt = 2, 1
+    return net
 
 
 def _torch_direction(P, U, reverse, peep, lc, lh):
@@ -149,15 +126,16 @@ def test_cell_matches_torch_autograd_and_central_differences(mode, peephole, rev
     P = rng.randn(4 * H, T)
     U = rng.uniform(-0.6, 0.6, (4 * H, H))
     peep = rng.uniform(-0.5, 0.5, (3, H)) if peephole else None
+    p64 = peep if peephole else np.zeros((3, H))     # the oracle's cell without peepholes: P = 0
     if mode == "masks":
-        lc, lh = zo.masks(0.4, 0.3, 9, 1, 2, int(reverse), 3, T, H)
+        lc, lh = zoneout_masks(0.4, 0.3, 9, 1, 2, int(reverse), 3, T, H)
         lc, lh = lc.T.astype(np.float64), lh.T.astype(np.float64)
         assert lc.any() and lh.any() and not lc.all() and not lh.all()
     else:
         lc, lh = np.full((H, T), 0.4), np.full((H, T), 0.3)
     w = rng.randn(H, T)
-    gates, c, h = zo.lstm_direction(P, U, reverse, peep, lc, lh)
-    dz, dU, dP = zo.lstm_direction_bptt(w, gates, c, h, U, reverse, peep, lc, lh)
+    gates, c, h = lstm_direction(P, U, reverse, p64, lc, lh)
+    dz, dU, dP = lstm_direction_bptt(w, gates, c, h, U, reverse, p64, lc, lh)
     tP, tU = torch.tensor(P, requires_grad=True), torch.tensor(U, requires_grad=True)
     tpeep = torch.tensor(peep, requires_grad=True) if peephole else None
     th = _torch_direction(tP, tU, reverse, tpeep, torch.tensor(lc), torch.tensor(lh))
@@ -169,15 +147,15 @@ def test_cell_matches_torch_autograd_and_central_differences(mode, peephole, rev
         assert np.allclose(tpeep.grad.numpy(), dP, rtol=1e-9, atol=1e-12)
 
     def loss(P_, U_, peep_):
-        return float(np.sum(w * zo.lstm_direction(P_, U_, reverse, peep_, lc, lh)[2]))
+        return float(np.sum(w * lstm_direction(P_, U_, reverse, peep_, lc, lh)[2]))
     eps = 1e-6
     for arr, grad in ((P, dz), (U, dU)) + (((peep, dP),) if peephole else ()):
         for idx in [(0, 0), (arr.shape[0] - 1, arr.shape[1] - 1), (arr.shape[0] // 2, 1)]:
             old = arr[idx]
             arr[idx] = old + eps
-            up = loss(P, U, peep)
+            up = loss(P, U, p64)
             arr[idx] = old - eps
-            dn = loss(P, U, peep)
+            dn = loss(P, U, p64)
             arr[idx] = old
             assert abs((up - dn) / (2 * eps) - grad[idx]) <= 1e-6 * max(1.0, abs(grad[idx]))
 
@@ -185,7 +163,7 @@ def test_cell_matches_torch_autograd_and_central_differences(mode, peephole, rev
 def test_whole_net_central_differences():
     """The net's gradient (masks drawn, peepholes, two stacked layers) against central differences of its cost on
     every tensor."""
-    _, net = _nets("bi_k2_ln_drop_sub", True, round_f32=False, zoneoutCell=0.3, zoneoutHidden=0.2)
+    net = _net("bi_k2_ln_drop_sub", True, round_f32=False, zoneoutCell=0.3, zoneoutHidden=0.2)
     data, labels = _data()
     cost, grad, skip = net.costAndGrad(data, labels)
     assert not skip
@@ -207,11 +185,11 @@ def test_whole_net_central_differences():
 def test_oracle_refuses_what_nnet_refuses():
     for bad in (-0.1, 1.0, float("nan")):
         with pytest.raises(ValueError):
-            zo.ZoneoutNet(D, K, 6, 3, 20, temporalLayer=2, cell="lstm", zoneoutCell=bad)
+            Net(D, K, 6, 3, 20, temporalLayer=2, cell="lstm", zoneoutCell=bad)
         with pytest.raises(ValueError):
-            zo.ZoneoutNet(D, K, 6, 3, 20, temporalLayer=2, cell="lstm", zoneoutHidden=bad)
+            Net(D, K, 6, 3, 20, temporalLayer=2, cell="lstm", zoneoutHidden=bad)
     with pytest.raises(ValueError):
-        zo.ZoneoutNet(D, K, 6, 3, 20, temporalLayer=2, cell="relu", zoneoutCell=0.1)
+        Net(D, K, 6, 3, 20, temporalLayer=2, cell="relu", zoneoutCell=0.1)
 
 
 # ------------------------------------------------------------------------------------------------------- C ABI

@@ -3,7 +3,7 @@
 The sweep alone (ctcb_lstm_sweep_zoneout_f32) on every plan, with and without peepholes, in training and expectation
 mode, against a float64 step from its own previous state, and its exact properties: a kept value has the bytes of the
 previous one, z = 0 gives the plain (and peephole) sweep's bytes, the bytes do not depend on the plan, the error flag
-stays 0.  Then whole nets against tests/zoneout_oracle.ZoneoutNet (tests/net_check.py), micro-batches, emulated shards,
+stays 0.  Then whole nets against tests/net_oracle.Net (tests/net_check.py), micro-batches, emulated shards,
 graph replay and resume bit for bit, forward-only probabilities against the expectation oracle, check_grad, forced
 stalls and runNNet.  Each comparison prints its measured numbers as one JSON line (pytest -s)."""
 import ctypes
@@ -15,8 +15,8 @@ import pytest
 
 import recipes
 from net_check import bits as _bits, compare, rel as _rel
+from net_oracle import Net, lstm_direction_bptt, zoneout_masks
 from recipes import knobs  # noqa: F401  (fixture)
-import zoneout_oracle as zo
 
 pytestmark = pytest.mark.gpu
 
@@ -84,7 +84,7 @@ class Sweep:
         """[T][H] float64 lambdas of utterance b, direction d."""
         if not train:
             return (np.full((self.T, self.H), float(np.float32(zc))), np.full((self.T, self.H), float(np.float32(zh))))
-        lc, lh = zo.masks(zc, zh, 77, 5, layer, d, first + stride * b, self.T, self.H)
+        lc, lh = zoneout_masks(zc, zh, 77, 5, layer, d, first + stride * b, self.T, self.H)
         return lc.astype(np.float64), lh.astype(np.float64)
 
 
@@ -135,10 +135,11 @@ def _bptt_error(sw, gates, h, c, dz, zc, zh, train):
             Tb = sw.lens[b]
             lc, lh = sw.lambdas(zc, zh, train, d, b)
             g = gates[:Tb, b, d * 4 * H:(d + 1) * 4 * H].T.astype(np.float64)
-            want, _, _ = zo.lstm_direction_bptt(sw.dh[:Tb, b].T.astype(np.float64), g,
-                                                c[d][:Tb, b].T.astype(np.float64), h[d][:Tb, b].T.astype(np.float64),
-                                                sw.U[d].astype(np.float64), d == 1,
-                                                sw.P[d].astype(np.float64) if sw.P else None, lc[:Tb].T, lh[:Tb].T)
+            want, _, _ = lstm_direction_bptt(sw.dh[:Tb, b].T.astype(np.float64), g,
+                                             c[d][:Tb, b].T.astype(np.float64), h[d][:Tb, b].T.astype(np.float64),
+                                             sw.U[d].astype(np.float64), d == 1,
+                                             sw.P[d].astype(np.float64) if sw.P else np.zeros((3, H)), lc[:Tb].T,
+                                             lh[:Tb].T)
             got = dz[:Tb, b, d * 4 * H:(d + 1) * 4 * H].T
             err = max(err, float(np.max(np.abs(got - want))))
             scale = max(scale, float(np.max(np.abs(want))))
@@ -238,8 +239,7 @@ def _gpu_net(c, B, reg=0.0, train=True, z=(ZC, ZH)):
 
 
 def _oracle(c, reg, z=(ZC, ZH)):
-    kw = _kwargs(c, reg, z)
-    return zo.ZoneoutNet(D, K, c["H"], c["N"], c["T"], **kw)
+    return Net(D, K, c["H"], c["N"], c["T"], **_kwargs(c, reg, z))
 
 
 def _batch(c, seed=5):
@@ -267,7 +267,7 @@ def _set_p(nn, on, seed=8):
 
 @pytest.mark.parametrize("name", list(NETS))
 def test_zoneout_net_matches_float64_oracle(name, cuda):
-    """The device's training call against ZoneoutNet with the same masks (and the same dropout masks)."""
+    """The device's training call against the float64 net with the same masks (and the same dropout masks)."""
     import torch
     c = NETS[name]
     lens, (datas, labelss) = _batch(c)
