@@ -179,12 +179,16 @@ def _sig(z):
     return 1.0 / (1.0 + np.exp(-z))
 
 
-def _check_forward(r, sw):
+def _check_forward(r, sw, lc=None, lh=None):
     """Largest |x - x64| / (u S) of the gates, c and h over the live frames, the step vectorised over the batch; and
-    where z is exact (h_prev = 0: z = pre, plus p c_prev = 0 for i and f) the activation alone, |a - a64| / (u |a64|)."""
+    where z is exact (h_prev = 0: z = pre, plus p c_prev = 0 for i and f) the activation alone, |a - a64| / (u |a64|).
+    Zoneout: lc, lh are per direction [T][B][H] lambdas (0 by default), c64 = lc c_prev + (1 - lc)(f c_prev + i g) with
+    |lc c_prev| in S, h64 likewise; "kept" says whether every c and h with lambda = 1 has the bytes of the one before."""
     H, T, nd = sw.H, sw.T, sw.ndir
     live = np.arange(T)[:, None] < sw.lens[None, :]
     ratio = dict(gates=0.0, c=0.0, h=0.0, act_exact=0.0)
+    if lc is not None:
+        ratio["kept"] = True
     exact_rows = slice(0, 3 * H) if sw.Ps is not None else slice(0, 4 * H)     # peephole o: z_o + p_o c_t rounds
     for d in range(nd):
         blk = slice(d * 4 * H, (d + 1) * 4 * H)
@@ -216,17 +220,25 @@ def _check_forward(r, sw):
                 a, b = gt[ex, exact_rows], a64[ex, exact_rows]
                 ratio["act_exact"] = max(ratio["act_exact"], float(np.max(np.abs(a - b) / (U32 * np.abs(b) + 1e-300))))
             i_, f_, g_, o_ = gt[:, :H], gt[:, H:2 * H], gt[:, 2 * H:3 * H], gt[:, 3 * H:]
-            c64 = f_ * cpt + i_ * g_
-            Sc = np.abs(f_ * cpt) + np.abs(i_ * g_) + 1e-30
+            lct = np.zeros_like(ct) if lc is None else np.asarray(lc[d][t, m], np.float64)
+            lht = np.zeros_like(ct) if lh is None else np.asarray(lh[d][t, m], np.float64)
+            c64 = lct * cpt + (1.0 - lct) * (f_ * cpt + i_ * g_)
+            Sc = np.abs(lct * cpt) + np.abs(f_ * cpt) + np.abs(i_ * g_) + 1e-30
             ratio["c"] = max(ratio["c"], float(np.max(np.abs(ct - c64) / (U32 * Sc))))
-            h64 = o_ * np.tanh(ct)
-            ratio["h"] = max(ratio["h"], float(np.max(np.abs(h[t, m] - h64) / (U32 * (np.abs(o_) + 1e-30)))))
+            h64 = lht * hp[t, m] + (1.0 - lht) * o_ * np.tanh(ct)
+            Sh = np.abs(lht * hp[t, m]) + np.abs(o_) + 1e-30
+            ratio["h"] = max(ratio["h"], float(np.max(np.abs(h[t, m] - h64) / (U32 * Sh))))
+            src = t - 1 if d == 0 else t + 1
+            if lc is not None and 0 <= src < T:
+                for lam, x in ((lct, r["c"][d]), (lht, r["h"][d])):
+                    k = lam == 1.0
+                    ratio["kept"] &= bool(np.array_equal(x[t, m][k].view(np.uint32), x[src, m][k].view(np.uint32)))
     return ratio
 
 
-def _check_bptt(r, sw):
+def _check_bptt(r, sw, lc=None, lh=None):
     """Largest |dz - dz64| / (u max |dz64|) per (utterance, direction), dz64 the float64 BPTT of the GPU's own forward
-    activations."""
+    activations (through the zoneout lambdas lc, lh of _check_forward, 0 by default)."""
     H, nd = sw.H, sw.ndir
     Us = [u.astype(np.float64) for u in sw.Us]
     worst = 0.0
@@ -238,8 +250,9 @@ def _check_bptt(r, sw):
             g = r["gates"][:Tu, u, blk].T.astype(np.float64)
             c, h = r["c"][d][:Tu, u].T.astype(np.float64), r["h"][d][:Tu, u].T.astype(np.float64)
             P = np.zeros((3, H)) if sw.Ps is None else sw.Ps[d].astype(np.float64)
-            zero = np.zeros((H, Tu))     # no zoneout
-            dz64 = net_oracle.lstm_direction_bptt(dh, g, c, h, Us[d], d == 1, P, zero, zero)[0]
+            zero = np.zeros((H, Tu))
+            lam = [zero if x is None else np.asarray(x[d][:Tu, u], np.float64).T for x in (lc, lh)]
+            dz64 = net_oracle.lstm_direction_bptt(dh, g, c, h, Us[d], d == 1, P, *lam)[0]
             S = float(np.max(np.abs(dz64)))
             assert S > 0.0, "utterance %d direction %d has no gradient to compare" % (u, d)
             worst = max(worst, float(np.max(np.abs(r["dz"][:Tu, u, blk].T - dz64))) / (U32 * S))

@@ -36,6 +36,7 @@ U = 2.0 ** -24
 C_COLSUM = 0.2
 # A priori (module docstring); the largest ratio measured on an H100 80GB HBM3 at 700 W is 0.49 of it.
 C_SOFTMAX = 2.0
+NEG = 10.0                     # a wrong wiring must exceed the bound at least this many times
 H100_SMS = 132
 GUARD = 64                     # floats of NaN around every output
 WS_GUARD = 4096                # bytes of 0xA5 behind every workspace
@@ -247,6 +248,9 @@ NETS = {
                                                   subsampleLayer=2)),
     "bi_sub3_L3_dropout": dict(H=44, N=3, K=27, kw=dict(temporalLayer=2, subsample=3, subsampleLayer=3,
                                                          dropout=0.1)),
+    # the recurrent and peephole gradients of both directions through the zoneout sweep's BPTT
+    "lstm_bi_peep_zoneout": dict(H=32, N=3, K=28, kw=dict(temporalLayer=2, cell="lstm", peephole=True,
+                                                          zoneoutCell=0.2, zoneoutHidden=0.15)),
 }
 MAXT, MAXB = 40, 7
 
@@ -311,9 +315,11 @@ def _gemm_plan(M, N, K, a_ptr, lda, b_ptr, ldb):
     return dict(zip(GEMM_FIELDS, list(out)))
 
 
-def _check_maps(nn, batch, lens, prev=None):
-    """Every map's padded delta frames, db and dW against the call's own delta and input.  prev: the flat gradient
-    (float32, NumPy) the call added onto, or None for a CTCB_PART_FIRST call.  Returns {map: ratios}."""
+def _check_maps(nn, batch, lens, prev=None, neg=None):
+    """Every map's padded delta frames, db and dW against the call's own delta and input, and the recurrent (and
+    peephole) gradients of every LSTM layer and of the lowest two of a uni-directional ReLU stack (rec_grads).  prev:
+    the flat gradient (float32, NumPy) the call added onto, or None for a CTCB_PART_FIRST call.  neg collects the
+    negative controls.  Returns {map: ratios}."""
     B, N = batch.B, nn.numLayers
     grads = nn.grads.cpu().numpy()
     out = {}
@@ -361,6 +367,140 @@ def _check_maps(nn, batch, lens, prev=None):
         r_b = _ratio(np.abs(db - want_b), bound_b)
         out[j] = dict(R=R, rows=rows, cols=cols, colsum=cplan, gemm_kernel=gplan["kernel"], L=L, dW=r_w, db=r_b)
         assert r_w <= 1.0 and r_b <= 1.0, (j, out[j])
+    for j in range(nn.numTemporal):      # the recurrent gradients, where the delta they read survives the call
+        if nn.cell == "relu" and not (nn.unidirectional and j < 2):
+            continue
+        r = _rec_from_hooks(nn, batch, lens, j, grads, prev, neg)
+        out["rec%d" % (nn.temporalLayer + j)] = r
+        assert max(v for k, v in r.items() if not k.startswith("kernel")) <= 1.0, (j, r)
+    return out
+
+
+def _rec_from_hooks(nn, batch, lens, j, grads, prev, neg):
+    """rec_grads of temporal layer tl + j from what the call left: dz (LSTM) or dFor (uni-directional ReLU, j < 2),
+    For / Back and Cf / Cb."""
+    i = nn.temporalLayer + j
+    reduced = nn.subsample > 1 and i >= nn.subsampleLayer
+    T = nn.frames(batch.Tmax) if reduced else batch.Tmax
+    Tu = [nn.frames(t) if reduced else t for t in lens]
+    B, H = batch.B, nn.layerSize
+    ndir = 1 if nn.unidirectional else 2
+    dd = _ws_array(nn, _hook(nn, 7, i)[0], T, B, nn._map_rows(i))
+    d = dd.cpu().numpy()
+    hd = [_ws_array(nn, _hook(nn, 1 + q, i)[0], T, B, H) for q in range(ndir)]
+    hs = [x.cpu().numpy() for x in hd]
+    if nn.cell == "lstm":
+        M = 4 * H
+        dzs = [d[:, :, q * M:(q + 1) * M] for q in range(ndir)]
+        cs = [_ws_array(nn, _hook(nn, 4 + q, i)[0], T, B, H).cpu().numpy() for q in range(ndir)]
+        ldz = ndir * M
+        ptrs = (dd.data_ptr() + 4 * B * ldz, dd.data_ptr() + 4 * M, hd[0].data_ptr(),
+                hd[-1].data_ptr() + 4 * B * H, ldz)
+    else:
+        dzs, cs = [d], None
+        ptrs = (dd.data_ptr() + 4 * B * H, None, hd[0].data_ptr(), None, H)
+    return rec_grads(nn, j, T, Tu, dzs, hs, cs, ptrs, grads, prev, neg)
+
+
+def _grad_view(nn, grads, idx, part=0):
+    """float64 copy of tensor stack[idx][part] of the flat float32 gradient `grads` (NumPy)."""
+    v = nn.grad[idx][part]
+    o = (v.data_ptr() - nn.grads.data_ptr()) // 4
+    return grads[o:o + v.numel()].reshape(tuple(v.shape))
+
+
+def _pairs(T, Tu, d):
+    """[T][B] weights of the frames t whose dz direction d pairs with h of frame t - 1 (d = 0) or t + 1 (d = 1) in
+    its own utterance: 0 where that frame lies outside [0, T_u)."""
+    t = np.arange(T)[:, None]
+    Tu = np.asarray(Tu)[None, :]
+    return ((t < Tu) & (t >= 1) if d == 0 else (t + 1 < Tu)).astype(np.float64)
+
+
+def _shift(x, d):
+    """x [T][B][n] moved one frame: y[t] = x[t - 1] (d = 0) or x[t + 1] (d = 1), 0 beyond the ends."""
+    y = np.zeros(x.shape)
+    if d == 0:
+        y[1:] = x[:-1]
+    else:
+        y[:-1] = x[1:]
+    return y
+
+
+def peep_idx(nn, j, d):
+    """Index into nn.stack of [P, dummy] of direction d of temporal layer tl + j."""
+    ndir = 1 if nn.unidirectional else 2
+    return len(nn.stack) - (1 if nn.selfCondition else 0) - nn.peepholeEntries() + j * ndir + d
+
+
+def rec_grads(nn, j, T, Tu, dzs, hs, cs, ptrs, grads, prev=None, neg=None):
+    """Ratios of the recurrent weight gradients of temporal layer tl + j (dU, or Wtf / Wtb) and of its peephole
+    gradients to float64 of the float32 deltas dzs and states hs, cs (per direction [T][B][.], direction 1 reversed in
+    time), each direction paired with its own shift within each utterance's length T_u.  The contraction: the bound of
+    test_gemm_plans_gpu.py at each problem's plan, as test_gemm_pair_plans takes it (ptrs: the step's A0, A1, B0, B1
+    and the pitch of A); dP: the bound of test_peephole_grad_matches_float64.  prev: the flat gradient the call added
+    onto (None for CTCB_PART_FIRST).  One frame: the recurrent gradients are exactly +0.0 in a first part and keep
+    their bytes in an accumulating one.  neg collects the negative controls: direction 1 unshifted, dp_o with c_prev,
+    beta = 0 where the call accumulates."""
+    ndir = len(dzs)
+    H = hs[0].shape[2]
+    B = hs[0].shape[1]
+    M = dzs[0].shape[2]
+    base = nn.numLayers + 1 + j * ndir
+    out = {}
+    neg = {} if neg is None else neg
+    lda = ptrs[4]
+    for d in range(ndir):
+        w = _pairs(T, Tu, d)[:, :, None]
+        A = (dzs[d].astype(np.float64) * w).reshape(T * B, M)
+        Bm = _shift(hs[d].astype(np.float64), d).reshape(T * B, H)
+        P, S = A.T @ Bm, np.abs(A).T @ np.abs(Bm)
+        got = _grad_view(nn, grads, base + d).astype(np.float64)
+        pw = None if prev is None else _grad_view(nn, prev, base + d).astype(np.float64)
+        if T == 1:                       # no recurrence: a memset in a first part, untouched in an accumulating one
+            want = np.zeros_like(got) if pw is None else pw
+            out["dU%d" % d] = 0.0 if np.array_equal(got.astype(np.float32).view(np.uint32),
+                                                     want.astype(np.float32).view(np.uint32)) else float("inf")
+        else:
+            a_ptr, b_ptr = (ptrs[0], ptrs[2]) if d == 0 else (ptrs[1], ptrs[3])
+            plan = _gemm_plan(M, H, (T - 1) * B, a_ptr, lda, b_ptr, H)
+            c0, c1 = GEMM_BOUNDS[plan["kernel"]]
+            k = (c0 + c1 * gemm_chain(plan, (T - 1) * B)) * U
+            if pw is not None and pw.any():      # (after a part of one-frame utterances dU is 0)
+                neg.setdefault("beta_0_accumulating", []).append(_ratio(np.abs(got - P), k * (S + np.abs(pw))))
+                P, S = P + pw, S + np.abs(pw)
+            out["dU%d" % d] = _ratio(np.abs(got - P), k * S)
+            out["kernel%d" % d] = plan["kernel"]
+            if d == 1:
+                wrong = dzs[d].astype(np.float64).reshape(T * B, M).T @ hs[d].astype(np.float64).reshape(T * B, H)
+                neg.setdefault("direction_1_unshifted", []).append(_ratio(np.abs(got - wrong - (0 if pw is None else pw)),
+                                                                          k * S))
+        if not nn.peephole:
+            continue
+        dz = dzs[d].astype(np.float64)
+        live = (np.arange(T)[:, None] < np.asarray(Tu)[None, :])[:, :, None]
+        c = cs[d].astype(np.float64) * live
+        cp = _shift(c, d) * _pairs(T, Tu, d)[:, :, None]
+        terms = [dz[:, :, :H] * cp, dz[:, :, H:2 * H] * cp, dz[:, :, 3 * H:] * c]
+        want = np.stack([x.sum(axis=(0, 1)) for x in terms])
+        S = np.stack([np.abs(x).sum(axis=(0, 1)) for x in terms])
+        K = 128 + 8 + -(-(T * B) // 1024) + 1
+        bound = K * U * S
+        ip = peep_idx(nn, j, d)
+        got = _grad_view(nn, grads, ip).astype(np.float64)
+        if prev is not None:
+            pp = _grad_view(nn, prev, ip).astype(np.float64)
+            neg.setdefault("beta_0_accumulating", []).append(_ratio(np.abs(got - want), bound + U * np.abs(want + pp)))
+            want = want + pp
+            bound = bound + U * np.abs(want)
+        out["dP%d" % d] = _ratio(np.abs(got - want), bound)
+        wrong = want.copy()
+        wrong[2] += (dz[:, :, 3 * H:] * (cp - c)).sum(axis=(0, 1))
+        neg.setdefault("dp_o_with_c_prev", []).append(_ratio(np.abs(got - wrong), bound))
+        if d == 1:
+            wrong = want.copy()
+            wrong[:2] += np.stack([(dz[:, :, q * H:(q + 1) * H] * (c - cp)).sum(axis=(0, 1)) for q in range(2)])
+            neg.setdefault("direction_1_unshifted", []).append(_ratio(np.abs(got - wrong), bound))
     return out
 
 
@@ -382,7 +522,7 @@ def test_every_map_gradient_from_the_step_delta(name, cuda):
     c = NETS[name]
     nn = _net(c)
     nn.grads.fill_(float("nan"))                      # CTCB_PART_FIRST must overwrite every tensor
-    rep = {}
+    rep, neg = {}, {}
     prev = None
     u0 = 0
     for part, seed in enumerate((41, 42)):
@@ -391,7 +531,7 @@ def test_every_map_gradient_from_the_step_delta(name, cuda):
         nn.costAndGradDevice(batch, want_probs=True, first=part == 0, last=part == 1, u0=u0)
         u0 += batch.B
         torch.cuda.synchronize()
-        rep[part] = _check_maps(nn, batch, lens, prev)
+        rep[part] = _check_maps(nn, batch, lens, prev, neg)
         # the probabilities the call wrote are the softmax of the logits it left behind, bit for bit
         T = nn.frames(batch.Tmax)
         off, K = _hook(nn, 0, nn.numLayers + 1)
@@ -406,7 +546,44 @@ def test_every_map_gradient_from_the_step_delta(name, cuda):
     dummies = [nn.grad[p][1] for p in range(nmaps, nmaps + nn.numTemporal * ndir)]
     dummies += [nn.grad[-1 - q][1] for q in range(nn.peepholeEntries())]
     assert all(bool((d == 0).all()) for d in dummies), "a dummy bias has a gradient"
-    print(json.dumps({"step_maps_" + name: {"first": rep[0], "accumulate": rep[1]}}))
+    negs = {k: min(v) for k, v in neg.items()}
+    print(json.dumps({"step_maps_" + name: {"first": rep[0], "accumulate": rep[1], "negative_controls": negs}}))
+    assert all(v >= NEG for v in negs.values()), negs
+
+
+def _one_frame_batch(c, seed):
+    """MAXB utterances of one frame and one label each."""
+    lens = [1] * MAXB
+    return lens, recipes.synth_batch(D_IN, c["K"], lens, [1] * MAXB, seed=seed)
+
+
+@pytest.mark.parametrize("name", [n for n, c in NETS.items() if c["kw"].get("temporalLayer")])
+def test_one_frame_micro_batches(name, cuda):
+    """A micro-batch whose utterances are all one frame long (Tmax = 1: no recurrence): as a first part every recurrent
+    gradient is exactly +0.0; after a part of full-length utterances, as an accumulating part, the recurrent gradients
+    keep their bytes and dP adds the dz_o c term alone; every map's gradients meet part (c)'s bounds throughout."""
+    torch = cuda
+    c = NETS[name]
+    nn = _net(c)
+    nn.grads.fill_(float("nan"))
+    rep, neg = {}, {}
+    prev = None
+    u0 = 0
+    for part, (kind, seed) in enumerate((("ones", 44), ("full", 41), ("ones", 45))):
+        lens, (datas, labelss) = (_one_frame_batch if kind == "ones" else _batches)(c, seed)
+        batch = nn.swap_batches().pack(datas, labelss).upload()
+        nn.costAndGradDevice(batch, first=part == 0, last=part == 2, u0=u0)
+        u0 += batch.B
+        torch.cuda.synchronize()
+        assert (batch.Tmax == 1) == (kind == "ones")
+        rep[part] = _check_maps(nn, batch, lens, prev, neg)
+        prev = nn.grads.cpu().numpy().copy()
+    ndir = 1 if nn.unidirectional else 2
+    rec = [_grad_view(nn, prev, nn.numLayers + 1 + q) for q in range(nn.numTemporal * ndir)]
+    negs = {k: min(v) for k, v in neg.items()}
+    print(json.dumps({"step_one_frame_" + name: dict(parts=rep, negative_controls=negs)}))
+    assert all(v >= NEG for v in negs.values()), negs
+    assert all(np.isfinite(x).all() for x in rec)
 
 
 # ------------------------------------------------------------------------------------------------ d. the tail

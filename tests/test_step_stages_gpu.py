@@ -33,12 +33,19 @@ self-conditioning, weight noise, SpecAugment masks, zoneout and widths that reac
            step's delta bit for bit;
   D_aux    against lambda times the float64 CTC gradient of the step's own A over the frames of layer m (bound of
            test_ctc_plans_gpu.py at the step's plan, plus one rounding for lambda).
-Not checked inside the step: the LSTM sweep and its BPTT (gates, c, h, peephole, zoneout masks), and with them the
-conditioned delta at an LSTM layer m; their kernels have element-wise tests of their own (test_lstm_plans_gpu.py,
-test_zoneout_gpu.py), and nets with them run every other stage here.
+  LSTM     the pre-activation recomputed at the step's plan and checked; the standalone sweep (plain, peephole or
+           zoneout, U and P as the step read them, the layer's own lengths, zoneout's layer i, step and utterance
+           numbering) from it on fresh buffers equals the step's gates, h and c bit for bit, which are checked against a
+           float64 step from the step's own state (C_FWD, C_ACT of test_lstm_plans_gpu.py, with the lambdas); padded
+           frames +0.0; the map above reads For + Back bit for bit; dh (+ D_aux W_{N+1}, or D'_m + dA W_{N+1} at the
+           conditioned layer) recomputed and checked, the standalone BPTT from it equal to the step's dz bit for bit,
+           and dz against net_oracle.lstm_direction_bptt (C_BPTT);
+  recurrent every temporal layer's dU, or Wtf / Wtb, and dP (rec_grads of test_step_reductions_gpu.py), from the dz,
+           dFor / dBack the call left or the BPTT recomputed (top-down where a uni-directional pair was reused).
 Negative controls: the reference with a plausible wrong wiring (alpha omitted, the D_aux term dropped, X_m for X'_m,
 the raw features, the clean parameters, gamma omitted, the dropout draw of the next step, the full-rate lengths at a
-reduced layer m) must exceed the same bound at least 10 times on the same arrays.
+reduced layer m, the other direction's U, the clean U, P omitted, the zoneout draw of the next step or numbered by u,
+direction 1 unshifted, dp_o from c_prev) must exceed the same bound at least 10 times on the same arrays.
 Each net prints its ratios as one JSON line (pytest -s); the ledger test asserts which paths were reached."""
 import ctypes
 import json
@@ -50,13 +57,17 @@ from test_gemm_plans_gpu import BOUNDS as GEMM_BOUNDS, _chain as gemm_chain
 from net_oracle import keep_mask
 from test_ctc_plans_gpu import BOUNDS as CTC_BOUNDS, _plan as ctc_plan
 from test_layernorm_gpu import C_FWD as C_LN, _fwd64 as ln_fwd64
+from net_oracle import zoneout_masks
+from test_lstm_plans_gpu import C_ACT, C_BPTT, C_FWD, _check_bptt, _check_forward
 from test_sweep_gpu import MAXACT, _bound as sweep_bound, _plan as sweep_plan, _steps as sweep_steps
-from test_step_reductions_gpu import (C_SOFTMAX, D_IN, MAXB, MAXT, NETS as MAP_NETS, U, _batches, _colsum_bound,
-                                      _colsum_plan, _gemm_plan, _hook, _ratio, _softmax_check, _ws_array)
+from test_step_reductions_gpu import (C_SOFTMAX, D_IN, MAXB, MAXT, NEG, NETS as MAP_NETS, U, _batches, _colsum_bound,
+                                      _colsum_plan, _gemm_plan, _hook, _ratio, _rec_from_hooks, _softmax_check,
+                                      _ws_array, peep_idx, rec_grads)
 
 pytestmark = pytest.mark.gpu
-NEG = 10.0                 # a wrong wiring must exceed the bound at least this many times
-STEP = 5                   # the step counter of every call: dropout draws from it
+STEP = 5                   # the step counter of every call: dropout, zoneout and weight noise draw from it
+SHARD = (1, 2)             # the call's utterances are minibatch entries FIRST + STRIDE u (an emulated rank 1 of 2)
+FIRST, STRIDE = SHARD
 NETS = dict(MAP_NETS)
 NETS.update({
     # the intermediate CTC at a ReLU layer with layer norm and dropout, and at a temporal layer
@@ -87,22 +98,42 @@ NETS.update({
     # the stacked map reads k H = 512 columns over about 140 rows: the tensor-core contraction splits over K
     "uni_h256_sub2_splitk": dict(H=256, N=3, K=33, kw=dict(temporalLayer=2, unidirectional=True, subsample=2,
                                                           subsampleLayer=2)),
+    # the tensor-core ReLU sweep; the LSTM sweep with U in registers (KI = 32)
+    "bi_relu_h1024": dict(H=1024, N=2, K=30, kw=dict(temporalLayer=1)),
+    "lstm_uni_h1024": dict(H=1024, N=2, K=30, kw=dict(temporalLayer=1, cell="lstm", unidirectional=True)),
+    # dh of an LSTM layer with the D_aux term; a dh pair used by layers j and j + 2; reduced lengths; the noisy U
+    "lstm_inter": dict(H=32, N=3, K=28, kw=dict(temporalLayer=2, cell="lstm", interLayer=2, interWeight=0.4)),
+    "lstm_uni_stack3_peep": dict(H=33, N=4, K=28, kw=dict(temporalLayer=1, numTemporal=3, cell="lstm",
+                                                          unidirectional=True, peephole=True)),
+    "lstm_sub_above": dict(H=32, N=4, K=28, kw=dict(temporalLayer=3, cell="lstm", subsample=2, subsampleLayer=2)),
+    "lstm_noise_peep": dict(H=32, N=3, K=28, kw=dict(temporalLayer=2, cell="lstm", peephole=True, weightNoise=0.05)),
 })
-LEDGER = dict(kernels={}, splitk=set(), stages=set(), sweeps=set(), missing={})
+LEDGER = dict(kernels={}, splitk=set(), stages=set(), sweeps=set(), lstm_ki=set(), missing={}, rec={})
 # the stage kinds every feature must reach somewhere in the table
 WANT_STAGES = {
     "fwd_map", "fwd_logits", "fwd_stack", "ln_fwd", "ln_stats", "dropout", "delta", "delta_unstack", "ln_bwd",
     "inter_A", "inter_delta", "cond_A", "cond_P", "cond_X", "cond_Dm", "cond_dP", "cond_dA", "cond_delta", "cond_dWc",
     "cond_dbc", "head_dW", "head_db", "maps_dW", "maps_db", "masked_input", "noisy_params", "padding", "sweep_fwd",
-    "bptt_dh", "bptt", "D_aux",
+    "bptt_dh", "bptt", "D_aux", "lstm_pre", "lstm_sweep", "lstm_bptt", "lstm_dh", "lstm_out", "rec_dW", "peep_dP",
+    "cond_dh_lstm",
 }
 
 
 def _want(nn):
     """The stage kinds a net must reach, by its features."""
     w = {"fwd_map", "fwd_logits", "delta", "maps_dW", "maps_db", "padding"}
+    if nn.numTemporal:
+        w.add("rec_dW")
     if nn.numTemporal and nn.cell == "relu":
         w |= {"sweep_fwd", "bptt_dh"}
+    if nn.numTemporal and nn.cell == "lstm":
+        w |= {"lstm_pre", "lstm_sweep", "lstm_bptt"}
+        if any(_temporal(nn, i) and i != _cond(nn) for i in range(1, nn.numLayers + 1)):
+            w.add("lstm_dh")
+        if nn.peephole:
+            w.add("peep_dP")
+        if nn.selfCondition and _temporal(nn, nn.interLayer):
+            w.add("cond_dh_lstm")
     if nn.subsample > 1:
         w.add("fwd_stack")
     if nn.layerNorm:
@@ -133,6 +164,9 @@ def _net(c):
     if nn.selfCondition:                  # W_c, b_c off 0, so X'_m differs from X_m
         nn.stack[-1][0].copy_(torch.from_numpy(rng.uniform(-0.4, 0.4, tuple(nn.stack[-1][0].shape)).astype(np.float32)))
         nn.stack[-1][1].copy_(torch.from_numpy(rng.uniform(-0.1, 0.1, tuple(nn.stack[-1][1].shape)).astype(np.float32)))
+    for k in range(nn.peepholeEntries()):     # peepholes off 0, so an omitted P shows
+        pk = nn.stack[len(nn.stack) - (1 if nn.selfCondition else 0) - nn.peepholeEntries() + k][0]
+        pk.copy_(torch.from_numpy(rng.uniform(-0.5, 0.5, tuple(pk.shape)).astype(np.float32)))
     for i in nn.normedLayers():           # gamma off 1 and beta off 0, so a missing gamma or beta shows
         g, be = nn.stack[_ln_idx(nn, i)]
         g.copy_(torch.from_numpy((1.0 + 0.5 * rng.randn(*g.shape)).astype(np.float32)))
@@ -163,6 +197,9 @@ class Call:
 
     def __init__(self, nn, batch, lens, labels):
         self.nn, self.batch, self.B, self.lens, self.labels = nn, batch, batch.B, lens, labels
+        self.grads = nn.grads.cpu().numpy()
+        self.rdelta = {}           # map j: (device, host) of its delta, recomputed where the call overwrote it
+        self.rec_done = set()      # the temporal layers whose recurrent gradients were checked
 
     def T(self, i):
         return self.nn.frames(self.batch.Tmax) if _reduced(self.nn, i) else self.batch.Tmax
@@ -256,7 +293,8 @@ def _cmp(got, want, bound, relu=False, mask=None):
     return _ratio(np.abs(got - want), bound)
 
 
-def _recompute(ta, tb, M, N, K, alpha, a, lda, b, ldb, beta=0.0, c0=None, mask=None, step_plan=None, bias=None):
+def _recompute(ta, tb, M, N, K, alpha, a, lda, b, ldb, beta=0.0, c0=None, mask=None, step_plan=None, bias=None,
+               relu=False):
     """ctcb_gemm_f32 into fresh 256-byte-aligned scratch (C0 copied in when beta != 0), at the plan of the step's call."""
     import _ctcb
     import torch
@@ -267,7 +305,7 @@ def _recompute(ta, tb, M, N, K, alpha, a, lda, b, ldb, beta=0.0, c0=None, mask=N
     assert _plan(ta, tb, M, N, K, a, lda, b, ldb) == step_plan
     wsb = int(lib.ctcb_gemm_workspace_bytes(M, N, K))
     ws = torch.zeros(max(wsb, 16), dtype=torch.uint8, device="cuda")
-    check(lib.ctcb_gemm_f32(ta, tb, M, N, K, alpha, a, lda, b, ldb, beta, out.data_ptr(), N, bias, 0,
+    check(lib.ctcb_gemm_f32(ta, tb, M, N, K, alpha, a, lda, b, ldb, beta, out.data_ptr(), N, bias, int(relu),
                             None if mask is None else mask, ws.data_ptr(), wsb, _ctcb.current_stream()))
     torch.cuda.synchronize()
     return out, out.cpu().numpy().reshape(M, N)
@@ -297,9 +335,11 @@ def _unstack(dS, T, B, n, k, Tu):
 
 # ------------------------------------------------------------------------------------------------ sweeps and the CTC
 def _keep(nn, i, c, step):
-    """[T*B][H] keep mask of hidden layer i of the call's utterances (g = u) at `step`, as the device draws it."""
+    """[T*B][H] keep mask of hidden layer i of the call's utterances (g = FIRST + STRIDE u) at `step`, as the device
+    draws it."""
     T, H = c.T(i), nn.layerSize
-    k = np.stack([keep_mask(nn.dropout, nn.dropoutSeed, step, i, u, T, H) for u in range(c.B)], axis=1)
+    k = np.stack([keep_mask(nn.dropout, nn.dropoutSeed, step, i, FIRST + STRIDE * u, T, H) for u in range(c.B)],
+                 axis=1)
     return k.reshape(T * c.B, H)
 
 
@@ -347,68 +387,260 @@ def _relu_sweep_fwd(c, i, pre, rep):
     LEDGER["stages"].add("sweep_fwd")
 
 
-def _relu_bptt(c, i, rep, neg):
-    """dh of ReLU temporal layer i (delta_{i+1} W_{i+1}, unstacked, + D_aux W_{N+1} at interLayer), recomputed at the
-    step's plans and checked; then the BPTT from it: the uni-directional result in place, the bi-directional one
-    recomputed with ctcb_brnn_sweep_f32 and equal, as For + Back, to the step's delta bit for bit."""
-    import _ctcb
+def _dh(c, i, rep, neg):
+    """(device dh, host dh [R][H]) of temporal layer i: delta_{i+1} W_{i+1} (the step's delta of map i + 1, or the one
+    recomputed above where the call overwrote it), unstacked below map L, + D_aux W_{N+1} at interLayer, recomputed at
+    the step's plans and checked; None where the delta of map i + 1 is not known."""
     import torch
-    from _ctcb import lib, check
     nn = c.nn
     N, B, H, K = nn.numLayers, c.B, nn.layerSize, nn.outputDim
     T, R = c.T(i), c.R(i)
-    if _hook(nn, 7, i + 1) is None:
-        return
-    dd, d = c.ws(7, i + 1, c.T(i + 1))
+    if _hook(nn, 7, i + 1) is not None:
+        dd, d = c.ws(7, i + 1, c.T(i + 1))
+    elif i + 1 in c.rdelta:
+        dd, d = c.rdelta[i + 1]
+    else:
+        return None
     n_out = d.shape[1]
     W, Wp = c.tensor(i, 0)
     n_in = W.shape[1]
     R1 = c.R(i + 1)
     plan = _plan(0, 0, R1, n_in, n_out, dd.data_ptr(), n_out, Wp, n_in)
     cb = _note("delta", plan, n_out)
-    _, dh = _recompute(0, 0, R1, n_in, n_out, 1.0, dd.data_ptr(), n_out, Wp, n_in, step_plan=plan)
+    dh_d, dh = _recompute(0, 0, R1, n_in, n_out, 1.0, dd.data_ptr(), n_out, Wp, n_in, step_plan=plan)
     P, S = _mm(d, W)
     bound = cb * U * S
     if nn.subsample > 1 and i + 1 == nn.subsampleLayer:
         dh, P, bound = (_unstack(a, T, B, H, nn.subsample, c.Tu(i)) for a in (dh, P, bound))
+        dh_d = torch.from_numpy(np.ascontiguousarray(dh, np.float32).reshape(-1)).cuda()
         LEDGER["stages"].add("delta_unstack")
     if i == nn.interLayer:
         Dd, Da = c.ws(9, 0, T)
         Wo, Wop = c.tensor(N, 0)
         plan2 = _plan(0, 0, R, H, K, Dd.data_ptr(), K, Wop, H)
         cb2 = _note("inter_delta", plan2, K)
-        _, dh2 = _recompute(0, 0, R, H, K, 1.0, Dd.data_ptr(), K, Wop, H, beta=1.0, c0=dh, step_plan=plan2)
+        dh_d, dh2 = _recompute(0, 0, R, H, K, 1.0, Dd.data_ptr(), K, Wop, H, beta=1.0, c0=dh, step_plan=plan2)
         P2, S2 = _mm(Da, Wo)
         bound = bound + cb2 * U * (S2 + np.abs(P))
         neg.setdefault("D_aux_dropped", []).append(_ratio(np.abs(dh2 - P), bound))
         P, dh = P + P2, dh2
         LEDGER["stages"].add("inter_delta")
-    rep["bptt_dh%d" % i] = _ratio(np.abs(dh - P), bound)
-    LEDGER["stages"].add("bptt_dh")
+    kind = "lstm_dh" if nn.cell == "lstm" else "bptt_dh"
+    rep["%s%d" % (kind, i)] = _ratio(np.abs(dh - P), bound)
+    LEDGER["stages"].add(kind)
+    return dh_d, dh
+
+
+def _relu_bptt(c, i, rep, neg):
+    """The BPTT of ReLU temporal layer i from its dh (_dh): the uni-directional result in place where the call left it,
+    else recomputed with ctcb_brnn_sweep_f32 (and then the delta of map i for the layer below); the bi-directional one
+    recomputed and equal, as For + Back, to the step's delta bit for bit.  Then the recurrent gradients from it."""
+    import _ctcb
+    import torch
+    from _ctcb import lib, check
+    nn = c.nn
+    B, H = c.B, nn.layerSize
+    T, R = c.T(i), c.R(i)
+    got = _dh(c, i, rep, neg)
+    if got is None:
+        return
+    dh_d, dh = got
     Wr = _rec(c, i)
     acts = [c.ws(1, i, T)[1]] + ([] if nn.unidirectional else [c.ws(2, i, T)[1]])
-    if nn.unidirectional:
-        if _hook(nn, 7, i) is None:
-            return                               # a later layer of the stack wrote the pair
-        dF = [c.ws(7, i, T)[1]]
+    if nn.unidirectional and _hook(nn, 7, i) is not None:
+        dd = c.ws(7, i, T)
+        dF, ptrs = [dd[1]], (dd[0].data_ptr() + 4 * B * H, None, c.ws(1, i, T)[0].data_ptr(), None, H)
     else:
-        f32 = lambda a: torch.from_numpy(np.ascontiguousarray(a, np.float32).reshape(-1)).cuda()   # noqa: E731
-        dh_d = f32(dh)
-        outs = [torch.zeros(R * H, dtype=torch.float32, device="cuda") for _ in range(2)]
+        outs = [torch.zeros(R * H, dtype=torch.float32, device="cuda") for _ in range(len(Wr))]
         lens_d = torch.tensor(c.Tu(i), dtype=torch.int32, device="cuda")
         wsb = int(lib.ctcb_brnn_sweep_workspace_bytes(H, B))
         scr = torch.zeros(wsb, dtype=torch.uint8, device="cuda")
-        check(lib.ctcb_brnn_sweep_f32(1, T, B, H, lens_d.data_ptr(), dh_d.data_ptr(), Wr[0][1], Wr[1][1],
-                                      outs[0].data_ptr(), outs[1].data_ptr(), c.ws(1, i, T)[0].data_ptr(),
-                                      c.ws(2, i, T)[0].data_ptr(), MAXACT, scr.data_ptr(), wsb,
-                                      _ctcb.current_stream()))
+        bi = not nn.unidirectional
+        check(lib.ctcb_brnn_sweep_f32(1, T, B, H, lens_d.data_ptr(), dh_d.data_ptr(), Wr[0][1],
+                                      Wr[1][1] if bi else None, outs[0].data_ptr(), outs[1].data_ptr() if bi else None,
+                                      c.ws(1, i, T)[0].data_ptr(), c.ws(2, i, T)[0].data_ptr() if bi else None,
+                                      MAXACT, scr.data_ptr(), wsb, _ctcb.current_stream()))
         torch.cuda.synchronize()
         dF = [o.cpu().numpy().reshape(R, H) for o in outs]
-        got = c.ws(7, i, T)[1]
-        assert np.array_equal(got.view(np.uint32), (dF[0] + dF[1]).view(np.uint32)), \
-            "the delta of map %d is not the BPTT of its recomputed dh" % i
+        if bi:
+            got = c.ws(7, i, T)[1]
+            assert np.array_equal(got.view(np.uint32), (dF[0] + dF[1]).view(np.uint32)), \
+                "the delta of map %d is not the BPTT of its recomputed dh" % i
+            ptrs = (outs[0].data_ptr() + 4 * B * H, outs[1].data_ptr(), c.ws(1, i, T)[0].data_ptr(),
+                    c.ws(2, i, T)[0].data_ptr() + 4 * B * H, H)
+        else:                                    # a later layer of the stack wrote the pair: the delta of map i
+            c.rdelta[i] = (outs[0], dF[0])
+            ptrs = (outs[0].data_ptr() + 4 * B * H, None, c.ws(1, i, T)[0].data_ptr(), None, H)
     rep["bptt%d" % i] = _sweep_ratio(c, i, dF, dh, [w for w, _ in Wr], acts)
     LEDGER["stages"].add("bptt")
+    r = lambda a: np.asarray(a).reshape(T, B, H)      # noqa: E731
+    _rec_check(c, i, rec_grads(nn, i - nn.temporalLayer, T, c.Tu(i), [r(x) for x in dF], [r(a) for a in acts], None,
+                               ptrs, c.grads, None, neg), rep)
+
+
+def _rec_check(c, i, out, rep):
+    rep["rec%d" % i] = {k: v for k, v in out.items() if not k.startswith("kernel")}
+    LEDGER["stages"].add("rec_dW")
+    if any(k.startswith("dP") for k in out):
+        LEDGER["stages"].add("peep_dP")
+    c.rec_done.add(i)
+
+
+# ------------------------------------------------------------------------------------------------ LSTM layers
+def _lstm_sweep(c, i, mode, gates, hs, cs, dh=None, dz=None):
+    """ctcb_lstm_sweep_f32 / _peephole_f32 / _zoneout_f32, as the net calls for, on device buffers: mode 0 the forward
+    from pre-activations in `gates`, mode 1 the BPTT from dh into dz; U and P as the step read them."""
+    import _ctcb
+    import torch
+    from _ctcb import lib, check
+    nn = c.nn
+    T, B, H = c.T(i), c.B, nn.layerSize
+    j = i - nn.temporalLayer
+    nd = len(hs)
+    Us = [p for _, p in _rec(c, i)]
+    Ps = [c.tensor(peep_idx(nn, j, d), 0)[1] for d in range(nd)] if nn.peephole else [None, None]
+    lens = torch.tensor(c.Tu(i), dtype=torch.int32, device="cuda")
+    p = lambda t: None if t is None else t.data_ptr()      # noqa: E731
+    two = lambda xs: (p(xs[0]), p(xs[1]) if nd == 2 else None)     # noqa: E731
+    Uf, Ub = Us[0], Us[1] if nd == 2 else None
+    Pf, Pb = Ps[0], Ps[1] if nd == 2 else None
+    hF, hB = two(hs) if mode == 0 else (None, None)
+    cF, cB = two(cs)
+    st = _ctcb.current_stream()
+    if nn.zoneout:
+        n = int(lib.ctcb_lstm_sweep_zoneout_workspace_bytes(H, B))
+        ws = torch.zeros(n, dtype=torch.uint8, device="cuda")
+        rc = lib.ctcb_lstm_sweep_zoneout_f32(mode, T, B, H, p(lens), p(gates), Uf, Ub, Pf, Pb, hF, hB, cF, cB, p(dh),
+                                             p(dz), nn.zoneoutCell, nn.zoneoutHidden, 1,
+                                             nn.dropoutSeed & 0xFFFFFFFFFFFFFFFF, p(nn.dropoutStep), FIRST, STRIDE, i,
+                                             p(ws), n, st)
+    else:
+        n = int(lib.ctcb_lstm_sweep_workspace_bytes(H, B))
+        ws = torch.zeros(n, dtype=torch.uint8, device="cuda")
+        if nn.peephole:
+            rc = lib.ctcb_lstm_sweep_peephole_f32(mode, T, B, H, p(lens), p(gates), Uf, Ub, Pf, Pb, hF, hB, cF, cB,
+                                                  p(dh), p(dz), p(ws), n, st)
+        else:
+            rc = lib.ctcb_lstm_sweep_f32(mode, T, B, H, p(lens), p(gates), Uf, Ub, hF, hB, cF, cB, p(dh), p(dz), p(ws),
+                                         n, st)
+    check(rc)
+    torch.cuda.synchronize()
+    assert int(ws[:4].view(torch.int32).item()) == 0, "the LSTM sweep set its error flag"
+
+
+class _Prob:
+    """What _check_forward / _check_bptt of test_lstm_plans_gpu.py read of a sweep problem."""
+
+    def __init__(self, c, i, pre, Us, Ps, dh=None):
+        nn = c.nn
+        self.H, self.T, self.B = nn.layerSize, c.T(i), c.B
+        self.ndir = len(Us)
+        self.lens = np.asarray(c.Tu(i))
+        self.pre = pre.reshape(self.T, self.B, -1)
+        self.Us, self.Ps = Us, Ps
+        self.dh = None if dh is None else dh.reshape(self.T, self.B, self.H)
+
+
+def _lambdas(c, i, step=STEP, numbered=None):
+    """Per direction [T][B][H] lambda_c, lambda_h of layer i as the device draws them (None without zoneout); numbered:
+    the minibatch index of utterance u (FIRST + STRIDE u by default)."""
+    nn = c.nn
+    if not nn.zoneout:
+        return None, None
+    T, H = c.T(i), nn.layerSize
+    g = numbered or (lambda u: FIRST + STRIDE * u)
+    nd = 1 if nn.unidirectional else 2
+    m = [[zoneout_masks(nn.zoneoutCell, nn.zoneoutHidden, nn.dropoutSeed, step, i, d, g(u), T, H) for u in range(c.B)]
+         for d in range(nd)]
+    return ([np.stack([x[0] for x in md], axis=1).astype(np.float64) for md in m],
+            [np.stack([x[1] for x in md], axis=1).astype(np.float64) for md in m])
+
+
+def _lstm_state(c, i):
+    """The step's gates (device, host [T][B][G]), h and c per direction (device, host [T][B][H])."""
+    nn = c.nn
+    T, B, H = c.T(i), c.B, nn.layerSize
+    nd = 1 if nn.unidirectional else 2
+    g = c.ws(3, i, T)
+    hs = [c.ws(1 + d, i, T) for d in range(nd)]
+    cs = [c.ws(4 + d, i, T) for d in range(nd)]
+    sh = lambda x: x[1].reshape(T, B, -1)      # noqa: E731
+    return g, [sh(x) for x in hs], [sh(x) for x in cs], hs, cs, sh(g)
+
+
+def _lstm_forward(c, i, pre_d, pre, rep, neg):
+    """LSTM layer i from the pre-activation the map wrote (recomputed, as the gates overwrote it): the forward sweep on
+    fresh buffers equals the step's gates, h and c bit for bit; those against a float64 step from the step's own state
+    of the step before (C_FWD, C_ACT), with zoneout's lambdas and kept values; padded frames +0.0."""
+    import torch
+    nn = c.nn
+    T, B, H = c.T(i), c.B, nn.layerSize
+    nd = 1 if nn.unidirectional else 2
+    j = i - nn.temporalLayer
+    plan = (ctypes.c_int32 * 4)()
+    from _ctcb import lib
+    debug = lib.ctcb_debug_lstm_zoneout_plan if nn.zoneout else lib.ctcb_debug_lstm_plan
+    assert debug(H, B, nd, int(nn.peephole), plan) == 0
+    LEDGER["lstm_ki"].add(int(plan[0]))
+    gates = pre_d.clone()
+    hs = [torch.zeros(T * B * H, dtype=torch.float32, device="cuda") for _ in range(nd)]
+    cs = [torch.zeros(T * B * H, dtype=torch.float32, device="cuda") for _ in range(nd)]
+    _lstm_sweep(c, i, 0, gates, hs, cs)
+    _, sh, sc, _, _, sg = _lstm_state(c, i)
+    for name, a, b in [("gates", gates, sg)] + [("h%d" % d, hs[d], sh[d]) for d in range(nd)] + \
+            [("c%d" % d, cs[d], sc[d]) for d in range(nd)]:
+        assert np.array_equal(a.cpu().numpy().view(np.uint32), b.reshape(-1).view(np.uint32)), \
+            "layer %d: the sweep of the recomputed pre-activation gives other %s than the step" % (i, name)
+    for u, t in enumerate(c.Tu(i)):
+        assert not any(x[t:, u].view(np.uint32).any() for x in [sg] + sh + sc), "a padded frame of layer %d" % i
+    LEDGER["stages"].add("lstm_sweep")
+    U_ = [w for w, _ in _rec(c, i)]
+    P_ = [c.tensor(peep_idx(nn, j, d), 0)[0] for d in range(nd)] if nn.peephole else None
+    r = dict(gates=sg, h=sh, c=sc)
+    lc, lh = _lambdas(c, i)
+    f = _check_forward(r, _Prob(c, i, pre, U_, P_), lc, lh)
+    rep["lstm_fwd%d" % i] = dict(gates=f["gates"] / C_FWD, c=f["c"] / C_FWD, h=f["h"] / C_FWD,
+                                 act=f["act_exact"] / C_ACT)
+    if lc is not None:
+        assert f["kept"], "layer %d: a kept c or h does not carry the previous value's bytes" % i
+    worst = lambda g: max(g["gates"], g["c"], g["h"]) / C_FWD      # noqa: E731
+    if nd == 2:
+        neg.setdefault("other_direction_U", []).append(
+            _check_forward(r, _Prob(c, i, pre, U_[::-1], P_), lc, lh)["gates"] / C_FWD)
+    if nn.weightNoise > 0.0:
+        clean = [c.tensor(nn.numLayers + 1 + j * nd + d, 0, noisy=False)[0] for d in range(nd)]
+        neg.setdefault("clean_U", []).append(_check_forward(r, _Prob(c, i, pre, clean, P_), lc, lh)["gates"] / C_FWD)
+    if nn.peephole:
+        neg.setdefault("P_omitted", []).append(_check_forward(r, _Prob(c, i, pre, U_, None), lc, lh)["gates"] / C_FWD)
+    if lc is not None:
+        neg.setdefault("zoneout_draw_of_next_step", []).append(
+            worst(_check_forward(r, _Prob(c, i, pre, U_, P_), *_lambdas(c, i, STEP + 1))))
+        neg.setdefault("zoneout_numbered_by_u", []).append(
+            worst(_check_forward(r, _Prob(c, i, pre, U_, P_), *_lambdas(c, i, numbered=lambda u: u))))
+
+
+def _lstm_bptt(c, i, dh_d, dh, rep, neg):
+    """The BPTT of LSTM layer i from its dh: the standalone sweep (mode 1) from the step's gates and c gives the step's
+    dz (the delta of map i) bit for bit; dz against net_oracle.lstm_direction_bptt of the step's own activations
+    (C_BPTT, the lambdas included); then the recurrent and peephole gradients from it."""
+    import torch
+    nn = c.nn
+    T, B, H = c.T(i), c.B, nn.layerSize
+    nd = 1 if nn.unidirectional else 2
+    j = i - nn.temporalLayer
+    g, sh, sc, hd, cd, sg = _lstm_state(c, i)
+    dz = torch.zeros(T * B * nd * 4 * H, dtype=torch.float32, device="cuda")
+    _lstm_sweep(c, i, 1, g[0].clone(), [None] * nd, [x[0].clone() for x in cd], dh=dh_d, dz=dz)
+    got = c.ws(7, i, T)[1]
+    assert np.array_equal(dz.cpu().numpy().view(np.uint32), got.reshape(-1).view(np.uint32)), \
+        "the delta of map %d is not the LSTM BPTT of its recomputed dh" % i
+    U_ = [w for w, _ in _rec(c, i)]
+    P_ = [c.tensor(peep_idx(nn, j, d), 0)[0] for d in range(nd)] if nn.peephole else None
+    r = dict(gates=sg, h=sh, c=sc, dz=got.reshape(T, B, -1))
+    lc, lh = _lambdas(c, i)
+    rep["lstm_bptt%d" % i] = _check_bptt(r, _Prob(c, i, sg, U_, P_, dh), lc, lh) / C_BPTT
+    LEDGER["stages"].add("lstm_bptt")
+    _rec_check(c, i, _rec_from_hooks(nn, c.batch, c.lens, j, c.grads, None, neg), rep)
 
 
 def _daux(c, rep, neg):
@@ -519,10 +751,28 @@ def _forward(c, rep, neg):
             LEDGER["stages"].add("fwd_map")
             _relu_sweep_fwd(c, i, pre, rep)
             continue
-        if _temporal(nn, i):
-            rep["fwd_map%d" % i] = "overwritten"      # the LSTM gates now hold X_i
+        if _temporal(nn, i):                          # the gates overwrote the pre-activation: recompute it
+            pre_d, pre = _recompute(0, 1, R, n_out, n_in, 1.0, xp, n_in, Wp, n_in, step_plan=plan,
+                                    bias=nn.stack[i - 1][1].data_ptr() if nn.weightNoise == 0.0 else
+                                    _noisy_ptr(c, i - 1, 1))
+            rep["fwd_map%d" % i] = _cmp(pre, P, bound)
+            LEDGER["stages"].update(("fwd_map", "lstm_pre"))
+            _lstm_forward(c, i, pre_d, pre, rep, neg)
             continue
         _, X = c.ws(0, i, c.T(i))
+        below = i - 1
+        if _temporal(nn, below) and nn.cell == "lstm" and not nn.unidirectional and below != _cond(nn) and \
+                not (nn.subsample > 1 and i == nn.subsampleLayer) and not (nn.dropout > 0.0 and relu):
+            # map i read Out = For + Back: the same contraction of For + Back in float32 gives its bytes
+            import torch
+            out_d = torch.from_numpy(np.ascontiguousarray(x, np.float32).reshape(-1)).cuda()
+            _, again = _recompute(0, 1, R, n_out, n_in, 1.0, out_d.data_ptr(), n_in, Wp, n_in, step_plan=plan,
+                                  bias=nn.stack[i - 1][1].data_ptr() if nn.weightNoise == 0.0 else
+                                  _noisy_ptr(c, i - 1, 1), relu=relu and not _normed(nn, i))
+            mine = c.ws(15, i, c.T(i))[1] if _normed(nn, i) else X
+            assert np.array_equal(again.view(np.uint32), mine.view(np.uint32)), \
+                "map %d did not read For + Back of LSTM layer %d" % (i, below)
+            LEDGER["stages"].add("lstm_out")
         if nn.dropout > 0.0 and relu:
             keep = _keep(nn, i, c, STEP)
             assert not X[~keep].view(np.uint32).any(), "layer %d: a dropped entry is not +0.0" % i
@@ -607,11 +857,14 @@ def _backward(c, rep, neg):
             assert not d[t:, u].view(np.uint32).any(), "map %d: a padded frame of the delta is not +0.0" % j
         LEDGER["stages"].add("padding")
     for i in range(N, 0, -1):
-        if _temporal(nn, i):
-            if nn.cell == "relu" and i != _cond(nn):
+        if _temporal(nn, i) and i != _cond(nn):
+            if nn.cell == "relu":
                 _relu_bptt(c, i, rep, neg)
-            if i != _cond(nn):
-                continue                         # LSTM layers: not checked inside the step (DESIGN.md section 4)
+            else:
+                got = _dh(c, i, rep, neg)
+                if got is not None:
+                    _lstm_bptt(c, i, *got, rep, neg)
+            continue
         hd = _hook(nn, 7, i + 1)
         if hd is None:
             continue
@@ -731,6 +984,13 @@ def _cond_backward(c, rep, neg, m, dd, d, W, Wp, alpha):
         if alpha != 1.0:
             neg.setdefault("alpha_omitted", []).append(_cmp(got, want / alpha, bound, mask=xm))
         LEDGER["stages"].add("cond_delta")
+    elif nn.cell == "lstm":                     # dh = D'_m + dA W_{N+1}, no mask: the BPTT starts from it
+        dh_d, dh = _recompute(0, 0, R, H, K, 1.0, dAd.data_ptr(), K, Wop, H, beta=1.0, c0=Dm, step_plan=plan_d)
+        P3, S3 = _mm(dA, Wo)
+        rep["cond_dh_lstm"] = _cmp(dh, P3 + Dm.astype(np.float64), cbd * U * (S3 + np.abs(Dm)))
+        neg.setdefault("D_aux_dropped", []).append(_cmp(dh, Dm.astype(np.float64), cbd * U * (S3 + np.abs(Dm))))
+        LEDGER["stages"].add("cond_dh_lstm")
+        _lstm_bptt(c, m, dh_d, dh, rep, neg)
     # dW_c = D'_m^T P (beta 0 in a first call), db_c = column sums of D'_m
     gW = nn.grad[len(nn.stack) - 1][0].cpu().numpy()
     gb = nn.grad[len(nn.stack) - 1][1].cpu().numpy().reshape(-1)
@@ -792,6 +1052,7 @@ def test_every_stage_of_the_step_from_its_own_inputs(name, cuda):
     nn = _net(c)
     lens, (datas, labelss) = _batches(c, 41)
     batch = nn.swap_batches().pack(datas, labelss).upload()
+    nn.dropoutShard = SHARD
     nn.costAndGradDevice(batch, want_probs=True)
     torch.cuda.synchronize()
     call = Call(nn, batch, lens, labelss)
@@ -806,8 +1067,10 @@ def test_every_stage_of_the_step_from_its_own_inputs(name, cuda):
     finally:
         LEDGER["missing"][name] = sorted(_want(nn) - LEDGER["stages"])
         LEDGER["stages"] |= reached
+    LEDGER["rec"][name] = sorted(_rec_missing(call))
     ratios = [v for v in rep.values() if isinstance(v, float)]
     ratios += [v[k] for v in rep.values() if isinstance(v, dict) for k in ("ratio", "dW", "db") if k in v]
+    ratios += [x for k, v in rep.items() if k.startswith(("rec", "lstm_fwd")) for x in v.values()]
     negs = {k: min(v) for k, v in neg.items() if v and all(x is not None for x in v)}
     print(json.dumps({"step_stages_" + name: dict(stages=rep, negative_controls=negs)}))
     assert max(ratios) <= 1.0, {k: v for k, v in rep.items() if (v if isinstance(v, float) else 0) > 1.0 or
@@ -826,22 +1089,43 @@ def test_every_stage_of_the_step_from_its_own_inputs(name, cuda):
         assert "gamma_omitted" in negs
     if kw.get("interLayer") and kw.get("subsample", 1) > 1 and kw["interLayer"] >= kw["subsampleLayer"]:
         assert "full_rate_lens" in negs
+    if kw.get("cell") == "lstm" and not kw.get("unidirectional"):
+        assert "other_direction_U" in negs
+    if kw.get("cell") == "lstm" and kw.get("weightNoise"):
+        assert "clean_U" in negs
+    if kw.get("peephole"):
+        assert "P_omitted" in negs and "dp_o_with_c_prev" in negs
+    if kw.get("zoneoutCell"):
+        assert "zoneout_draw_of_next_step" in negs and "zoneout_numbered_by_u" in negs
+    if kw.get("temporalLayer") and not kw.get("unidirectional"):
+        assert "direction_1_unshifted" in negs
+    if kw.get("cell") == "lstm" and kw.get("interLayer") == kw.get("temporalLayer"):
+        assert "D_aux_dropped" in negs
     assert not LEDGER["missing"][name], LEDGER["missing"][name]
+    assert not LEDGER["rec"][name], "no recurrent gradient check at layers %s" % LEDGER["rec"][name]
+
+
+def _rec_missing(call):
+    """The temporal layers of the call's net whose recurrent gradients were not checked."""
+    nn = call.nn
+    return {i for i in range(1, nn.numLayers + 1) if _temporal(nn, i)} - call.rec_done
 
 
 def test_every_path_was_reached(cuda):
     """Both contraction kernels in the forward maps, the deltas, the weight gradients and the head / conditioning
-    contractions; split-K in a forward map (the stacked map of uni_h256_sub2_splitk); both sweep families the table's
-    widths reach (the generic and the cluster kernel); every stage kind, and every net the stage kinds of its
-    features."""
+    contractions; split-K in a forward map (the stacked map of uni_h256_sub2_splitk); all three ReLU sweep families
+    (generic, cluster, tensor-core at H = 1024); the LSTM sweep with U in registers and re-read; every stage kind,
+    every net the stage kinds of its features, and every temporal layer its recurrent gradients."""
     missing = sorted(WANT_STAGES - LEDGER["stages"])
     kernels = {k: sorted(v) for k, v in LEDGER["kernels"].items()}
     print(json.dumps({"step_stages_ledger": dict(kernels=kernels, splitk=sorted(LEDGER["splitk"]),
-                                                 sweeps=sorted(LEDGER["sweeps"]),
+                                                 sweeps=sorted(LEDGER["sweeps"]), lstm_ki=sorted(LEDGER["lstm_ki"]),
                                                  stages=sorted(LEDGER["stages"]))}))
     assert not missing, missing
     for kind in ("fwd", "delta", "dW", "head", "cond"):
         assert LEDGER["kernels"].get(kind) == {0, 1}, (kind, kernels)
     assert "fwd" in LEDGER["splitk"], LEDGER["splitk"]
-    assert {"generic", "cluster"} <= LEDGER["sweeps"], LEDGER["sweeps"]
+    assert {"generic", "cluster", "tensor-core"} <= LEDGER["sweeps"], LEDGER["sweeps"]
+    assert 0 in LEDGER["lstm_ki"] and LEDGER["lstm_ki"] - {0}, LEDGER["lstm_ki"]
     assert len(LEDGER["missing"]) == len(NETS) and not any(LEDGER["missing"].values()), LEDGER["missing"]
+    assert len(LEDGER["rec"]) == len(NETS) and not any(LEDGER["rec"].values()), LEDGER["rec"]

@@ -160,6 +160,57 @@ def test_cell_matches_torch_autograd_and_central_differences(mode, peephole, rev
             assert abs((up - dn) / (2 * eps) - grad[idx]) <= 1e-6 * max(1.0, abs(grad[idx]))
 
 
+@pytest.mark.parametrize("peephole", [False, True])
+def test_elementwise_check_accepts_the_rounded_oracle_and_rejects_a_flipped_lambda(peephole):
+    """_check_forward / _check_bptt of test_lstm_plans_gpu.py with lambdas, the bounds the GPU's zoneout sweep is held
+    to: net_oracle.lstm_direction's gates, c, h and its BPTT's dz, each rounded to float32, meet C_FWD and C_BPTT; the
+    same arrays checked with one lambda_c, or one lambda_h, flipped at a frame where that changes c or h exceed them."""
+    from test_lstm_plans_gpu import C_BPTT, C_FWD, _check_bptt, _check_forward
+    H, T, B, nd = 6, 7, 3, 2
+    rng = np.random.RandomState(5 + peephole)
+    lens = np.array([T, 4, 1], np.int32)
+    f32 = lambda a: np.asarray(a, np.float32)           # noqa: E731
+    pre = f32(rng.uniform(-1.5, 1.5, (T, B, nd * 4 * H)))
+    Us = [f32(rng.uniform(-0.8, 0.8, (4 * H, H))) for _ in range(nd)]
+    Ps = [f32(rng.uniform(-0.5, 0.5, (3, H))) for _ in range(nd)] if peephole else None
+    dh = f32(rng.randn(T, B, H))
+    lc = [np.zeros((T, B, H)) for _ in range(nd)]
+    lh = [np.zeros((T, B, H)) for _ in range(nd)]
+    r = dict(gates=np.zeros((T, B, nd * 4 * H), np.float32), c=[np.zeros((T, B, H), np.float32) for _ in range(nd)],
+             h=[np.zeros((T, B, H), np.float32) for _ in range(nd)], dz=np.zeros((T, B, nd * 4 * H), np.float32))
+    for d in range(nd):
+        blk = slice(d * 4 * H, (d + 1) * 4 * H)
+        p64 = Ps[d].astype(np.float64) if peephole else np.zeros((3, H))
+        for u, Tu in enumerate(lens):
+            a, b = zoneout_masks(0.4, 0.3, 9, 1, 2, d, u, Tu, H)
+            lc[d][:Tu, u], lh[d][:Tu, u] = a, b
+            P = pre[:Tu, u, blk].T.astype(np.float64)
+            g, c, h = lstm_direction(P, Us[d].astype(np.float64), d == 1, p64, lc[d][:Tu, u].T, lh[d][:Tu, u].T)
+            dz = lstm_direction_bptt(dh[:Tu, u].T.astype(np.float64), g, c, h, Us[d].astype(np.float64), d == 1, p64,
+                                     lc[d][:Tu, u].T, lh[d][:Tu, u].T)[0]
+            r["gates"][:Tu, u, blk], r["c"][d][:Tu, u], r["h"][d][:Tu, u] = f32(g.T), f32(c.T), f32(h.T)
+            r["dz"][:Tu, u, blk] = f32(dz.T)
+
+    class Problem:
+        pass
+    sw = Problem()
+    sw.H, sw.T, sw.B, sw.ndir, sw.lens, sw.pre, sw.Us, sw.Ps, sw.dh = H, T, B, nd, lens, pre, Us, Ps, dh
+    fwd, dz = _check_forward(r, sw, lc, lh), _check_bptt(r, sw, lc, lh)
+    assert fwd["gates"] <= C_FWD and fwd["c"] <= C_FWD and fwd["h"] <= C_FWD and fwd["kept"], fwd
+    assert dz <= C_BPTT, dz
+    # a frame of utterance 0, direction 0, where the new c (h) is far from the one it would keep
+    c0, h0 = r["c"][0][:, 0].astype(np.float64), r["h"][0][:, 0].astype(np.float64)
+    for lam, x, key in ((lc, c0, "c"), (lh, h0, "h")):
+        gap = np.abs(x[2:] - x[1:-1])
+        t, j = np.unravel_index(int(np.argmax(gap)), gap.shape)
+        t += 2
+        flipped = [a.copy() for a in lam]
+        flipped[0][t, 0, j] = 1.0 - flipped[0][t, 0, j]
+        args = (flipped, lh) if key == "c" else (lc, flipped)
+        assert _check_forward(r, sw, *args)[key] > 10 * C_FWD, key
+        assert _check_bptt(r, sw, *args) > C_BPTT, key
+
+
 def test_whole_net_central_differences():
     """The net's gradient (masks drawn, peepholes, two stacked layers) against central differences of its cost on
     every tensor."""

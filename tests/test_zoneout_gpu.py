@@ -1,7 +1,8 @@
 """GPU tests of zoneout on the LSTM cell (ctcb_brnn_config.zoneout = 1) on one H100.
 
 The sweep alone (ctcb_lstm_sweep_zoneout_f32) on every plan, with and without peepholes, in training and expectation
-mode, against a float64 step from its own previous state, and its exact properties: a kept value has the bytes of the
+mode, against a float64 step from its own previous state under the element-wise bounds C_FWD / C_ACT / C_BPTT of
+test_lstm_plans_gpu.py (the lambdas in c64, h64 and the float64 BPTT), and its exact properties: a kept value has the bytes of the
 previous one, z = 0 gives the plain (and peephole) sweep's bytes, the bytes do not depend on the plan, the error flag
 stays 0.  Then whole nets against tests/net_oracle.Net (tests/net_check.py), micro-batches, emulated shards,
 graph replay and resume bit for bit, forward-only probabilities against the expectation oracle, check_grad, forced
@@ -15,8 +16,9 @@ import pytest
 
 import recipes
 from net_check import bits as _bits, compare, rel as _rel
-from net_oracle import Net, lstm_direction_bptt, zoneout_masks
+from net_oracle import Net, zoneout_masks
 from recipes import knobs  # noqa: F401  (fixture)
+from test_lstm_plans_gpu import C_ACT, C_BPTT, C_FWD, _check_bptt, _check_forward
 
 pytestmark = pytest.mark.gpu
 
@@ -88,63 +90,18 @@ class Sweep:
         return lc.astype(np.float64), lh.astype(np.float64)
 
 
-def _sig(x):
-    return 1.0 / (1.0 + np.exp(-x))
+class _Problem:
+    """The view of a Sweep that _check_forward / _check_bptt of test_lstm_plans_gpu.py read."""
+
+    def __init__(self, sw):
+        self.H, self.T, self.B, self.ndir = sw.H, sw.T, sw.B, sw.ndir
+        self.lens, self.pre, self.Us, self.Ps, self.dh = np.asarray(sw.lens), sw.pre, sw.U, sw.P, sw.dh
 
 
-def _step_errors(sw, gates, h, c, zc, zh, train):
-    """Largest error of c and h over every live frame against a float64 step from the device's own previous state,
-    relative to the largest |c| / |h|; and whether every kept value has the previous value's bytes."""
-    H, T = sw.H, sw.T
-    ec = eh = 0.0
-    kept_ok = True
-    for d in range(sw.ndir):
-        U = sw.U[d].astype(np.float64)
-        for b in range(sw.B):
-            Tb = sw.lens[b]
-            lc, lh = sw.lambdas(zc, zh, train, d, b)
-            order = range(Tb) if d == 0 else range(Tb - 1, -1, -1)
-            for n, t in enumerate(order):
-                tp = t - 1 if d == 0 else t + 1
-                cp = c[d][tp, b].astype(np.float64) if n else np.zeros(H)
-                hp = h[d][tp, b].astype(np.float64) if n else np.zeros(H)
-                z = sw.pre[t, b, d * 4 * H:(d + 1) * 4 * H].astype(np.float64) + U.dot(hp)
-                pe = sw.P[d].astype(np.float64) if sw.P else np.zeros((3, H))
-                i, f, g = _sig(z[:H] + pe[0] * cp), _sig(z[H:2 * H] + pe[1] * cp), np.tanh(z[2 * H:3 * H])
-                cn = lc[t] * cp + (1 - lc[t]) * (f * cp + i * g)
-                o = _sig(z[3 * H:] + pe[2] * cn)
-                hn = lh[t] * hp + (1 - lh[t]) * o * np.tanh(cn)
-                ec = max(ec, float(np.max(np.abs(c[d][t, b] - cn))))
-                eh = max(eh, float(np.max(np.abs(h[d][t, b] - hn))))
-                if train and n:
-                    kc, kh = lc[t] > 0, lh[t] > 0
-                    kept_ok &= np.array_equal(c[d][t, b][kc].view(np.uint32), c[d][tp, b][kc].view(np.uint32))
-                    kept_ok &= np.array_equal(h[d][t, b][kh].view(np.uint32), h[d][tp, b][kh].view(np.uint32))
-            assert not np.any(c[d][Tb:, b]) and not np.any(h[d][Tb:, b])
-    sc = max(float(np.max(np.abs(x))) for x in c)
-    sh = max(float(np.max(np.abs(x))) for x in h)
-    return ec / sc, eh / sh, kept_ok
-
-
-def _bptt_error(sw, gates, h, c, dz, zc, zh, train):
-    """Largest element-wise error of dz against the float64 BPTT through the device's own activations."""
-    H = sw.H
-    err, scale = 0.0, 0.0
-    for d in range(sw.ndir):
-        for b in range(sw.B):
-            Tb = sw.lens[b]
-            lc, lh = sw.lambdas(zc, zh, train, d, b)
-            g = gates[:Tb, b, d * 4 * H:(d + 1) * 4 * H].T.astype(np.float64)
-            want, _, _ = lstm_direction_bptt(sw.dh[:Tb, b].T.astype(np.float64), g,
-                                             c[d][:Tb, b].T.astype(np.float64), h[d][:Tb, b].T.astype(np.float64),
-                                             sw.U[d].astype(np.float64), d == 1,
-                                             sw.P[d].astype(np.float64) if sw.P else np.zeros((3, H)), lc[:Tb].T,
-                                             lh[:Tb].T)
-            got = dz[:Tb, b, d * 4 * H:(d + 1) * 4 * H].T
-            err = max(err, float(np.max(np.abs(got - want))))
-            scale = max(scale, float(np.max(np.abs(want))))
-            assert not np.any(dz[Tb:, b, d * 4 * H:(d + 1) * 4 * H])
-    return err / max(scale, 1e-30)
+def _lambdas(sw, zc, zh, train):
+    """Per direction [T][B][H] lambda_c and lambda_h of every utterance."""
+    lam = [[sw.lambdas(zc, zh, train, d, b) for b in range(sw.B)] for d in range(sw.ndir)]
+    return ([np.stack([x[0] for x in per], axis=1) for per in lam], [np.stack([x[1] for x in per], axis=1) for per in lam])
 
 
 PLANS = [("auto", None), ("reread", None), ("auto", 1), ("reread", 2)]
@@ -155,7 +112,6 @@ SWEEPS = {
     "h1024_bi": dict(T=12, B=5, H=1024, ndir=2),
     "h1024_uni": dict(T=12, B=9, H=1024, ndir=1),        # KI = 32: U in registers
 }
-STEP_TOL, BPTT_TOL = 2e-5, 1e-4
 
 
 def _plan(knobs, lstm, parts):
@@ -180,12 +136,17 @@ def test_sweep_on_every_plan_against_float64(name, peep, knobs, cuda):
             zc, zh = 0.3, 0.2
             gates, h, cc, dz, err = sw.run(zc, zh, train)
             assert err == 0
-            e_c, e_h, kept = _step_errors(sw, gates, h, cc, zc, zh, train)
-            e_dz = _bptt_error(sw, gates, h, cc, dz, zc, zh, train)
+            r = dict(gates=gates, h=h, c=cc, dz=dz)
+            lc, lh = _lambdas(sw, zc, zh, train)
+            fwd = _check_forward(r, _Problem(sw), lc, lh)
+            e_dz = _check_bptt(r, _Problem(sw), lc, lh)
             key = "%s_%s_%s" % (lstm, parts, "train" if train else "expect")
-            out[key] = dict(KI=int(plan[0]), parts=int(plan[1]), c=e_c, h=e_h, dz=e_dz)
-            assert kept
-            assert e_c <= STEP_TOL and e_h <= STEP_TOL and e_dz <= BPTT_TOL, out[key]
+            out[key] = dict(KI=int(plan[0]), parts=int(plan[1]), dz=e_dz, **fwd)
+            for b, Tb in enumerate(sw.lens):
+                assert not any(np.any(x[Tb:, b]) for x in [gates, dz] + h + cc), "a padded frame is not 0"
+            assert fwd["kept"], out[key]
+            assert fwd["gates"] <= C_FWD and fwd["c"] <= C_FWD and fwd["h"] <= C_FWD, out[key]
+            assert fwd["act_exact"] <= C_ACT and e_dz <= C_BPTT, out[key]
             b = [x.view(np.uint32).tobytes() for x in [gates, dz] + h + cc]
             if train in ref_bits:
                 assert b == ref_bits[train], "the bits depend on the plan: " + key
