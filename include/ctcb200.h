@@ -129,6 +129,18 @@ int ctcb_gemm_pair_f32(int transA, int transB, int M, int N, int K, float alpha,
  *   ceil(K / splits) rounded up to a multiple of 16.  M <= 0 or N <= 0 reports {0, .., 0, 1}. */
 int ctcb_debug_gemm_plan(int transA, int transB, int M, int N, int K, const float *A, int64_t lda,
                          const float *B, int64_t ldb, int problems, int32_t *out);
+/* The same three in TF32 mode (ctcb_brnn_config.tf32, below): same arguments and workspace; a shape that goes to the
+ * FFMA kernel runs it, with ctcb_gemm_f32's bits, and the plan entry reports it.  The TF32 plans keep the default's
+ * BN, K splits and operand paths; their ring stages are their own. */
+int ctcb_gemm_tf32(int transA, int transB, int M, int N, int K, float alpha,
+                   const float *A, int64_t lda, const float *B, int64_t ldb, float beta,
+                   float *C, int64_t ldc, const float *bias, int relu, const float *mask_src,
+                   void *workspace, size_t ws_bytes, void *stream);
+int ctcb_gemm_pair_tf32(int transA, int transB, int M, int N, int K, float alpha,
+                        const float *A0, const float *A1, int64_t lda, const float *B0, const float *B1, int64_t ldb,
+                        float beta, float *C0, float *C1, int64_t ldc, void *workspace, size_t ws_bytes, void *stream);
+int ctcb_debug_gemm_plan_tf32(int transA, int transB, int M, int N, int K, const float *A, int64_t lda,
+                              const float *B, int64_t ldb, int problems, int32_t *out);
 
 /* Debug hook: set one planner knob of INTEGRATION.md section 4 in this process, e.g. ("CTCB_CTC", "ckpt") or
  * ("CTCB_SWEEP_TC_CS", "2").  value uses the environment's syntax; value == NULL restores what the environment said at
@@ -213,7 +225,21 @@ typedef struct ctcb_brnn_config {
     int32_t selfCondition; /* 0: off (so an initialiser without this member keeps its meaning); 1: self-conditioned CTC
                             * (below), which needs interLayer >= 1; any other value, or 1 with interLayer = 0, makes the
                             * config invalid. */
+    int32_t tf32;          /* 0: off (so an initialiser without this member keeps its meaning); 1: every tensor-core
+                            * contraction and sweep of the net's training and forward-only calls runs in TF32 mode
+                            * (below); any other value makes the config invalid. */
 } ctcb_brnn_config;
+
+/* TF32 mode (tf32 = 1, ctcb_gemm_tf32, ctcb_brnn_sweep_tf32; not in the reference).  By default every product on the
+ * tensor cores is fp32-faithful: each operand is split into two TF32 parts and a product costs three MMAs (3xTF32).
+ * In TF32 mode every product that runs on the tensor cores reads each operand rounded to the nearest TF32 value, ties
+ * away from zero (cvt.rna.tf32.f32: the low 13 mantissa bits become zero), and is ONE .tf32 MMA accumulated in fp32, as
+ * PyTorch's allow_tf32 does.  The K splits (no accumulator chain longer than K = 2048) and the deterministic split-K
+ * reduce are those of the default, and so are the workspace sizes and offsets: ctcb_gemm_workspace_bytes,
+ * ctcb_brnn_sweep_workspace_bytes, ctcb_brnn_workspace_bytes and ctcb_brnn_forward_workspace_bytes do not depend on
+ * the mode.  The exact FFMA kernels keep their bits in either mode: the small contractions (ctcb_debug_gemm_plan
+ * kernel 0), the cluster and generic ReLU sweeps (H <= 512), the LSTM sweeps, the CTC, layer normalisation and the
+ * optimisers.  No parameter changes, so checkpoints are the same in both modes. */
 
 /* Intermediate CTC loss (interLayer = m >= 1; not in the reference; Lee & Watanabe, "Intermediate Loss Regularization
  * for CTC-based Speech Recognition", ICASSP 2021, after the hierarchical CTC of Fernandez et al. 2007 and Sanabria &
@@ -657,6 +683,12 @@ size_t ctcb_brnn_sweep_workspace_bytes(int H, int B);
 int ctcb_brnn_sweep_f32(int mode, int T, int B, int H, const int32_t *T_per_utt, const float *pre,
                         const float *Wf, const float *Wb, float *outF, float *outB, const float *actF,
                         const float *actB, float maxAct, void *scratch, size_t scratch_bytes, void *stream);
+/* The same in TF32 mode (ctcb_brnn_config.tf32, above), same arguments and scratch: the tensor-core kernel rounds W
+ * (W^T) and each step's state to TF32 and runs one MMA per product; S_t itself stays the exact fp32 output of the
+ * step.  The cluster and generic kernels run as ctcb_brnn_sweep_f32, with its bits. */
+int ctcb_brnn_sweep_tf32(int mode, int T, int B, int H, const int32_t *T_per_utt, const float *pre,
+                         const float *Wf, const float *Wb, float *outF, float *outB, const float *actF,
+                         const float *actB, float maxAct, void *scratch, size_t scratch_bytes, void *stream);
 /* The LSTM recurrences of one temporal layer on their own (cell = 1).  Time-major arrays; G = 8H with Ub, 4H without.
  * mode 0: gates [T][B][G] holds pre = W x + b on entry and the activated gates i, f, g, o (0 at padded frames) on
  *   return; hF / hB [T][B][H] receive h, cF / cB [T][B][H] receive c.
@@ -712,6 +744,8 @@ int ctcb_sweep_uses_tensor_cores(int H, int B);
  * plan the device cannot hold: CTCB_EINVAL for a width whose shared memory or co-resident CTAs exceed the device, or a
  * forced partition count it cannot hold co-resident. */
 int ctcb_debug_sweep_plan(int H, int B, int ndir, int32_t *out);
+/* The plan ctcb_brnn_sweep_tf32 launches, in the same form. */
+int ctcb_debug_sweep_plan_tf32(int H, int B, int ndir, int32_t *out);
 
 /* ---- optimiser (replaces sgd.SGD.run arithmetic, ctc_fast/sgd.py:91-161, and
  *      NNet.updateParams, brnnet.py:251-256) --------------------------------------------------- */

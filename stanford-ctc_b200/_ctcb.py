@@ -32,7 +32,7 @@ class BrnnConfig(ctypes.Structure):
                 ("cell", ctypes.c_int32), ("layerNorm", ctypes.c_int32), ("subsample", ctypes.c_int32),
                 ("subsampleLayer", ctypes.c_int32), ("peephole", ctypes.c_int32), ("maskFeatDim", ctypes.c_int32),
                 ("weightNoise", ctypes.c_int32), ("zoneout", ctypes.c_int32), ("interLayer", ctypes.c_int32),
-                ("interWeight", ctypes.c_float), ("selfCondition", ctypes.c_int32)]
+                ("interWeight", ctypes.c_float), ("selfCondition", ctypes.c_int32), ("tf32", ctypes.c_int32)]
 
 
 _PROTOS = {
@@ -57,6 +57,12 @@ _PROTOS = {
                                    c_f32, c_vp, c_vp, c_i64, c_vp, c_sz, c_vp]),
     "ctcb_debug_gemm_plan": (c_int, [c_int, c_int, c_int, c_int, c_int, c_vp, c_i64, c_vp, c_i64, c_int,
                                      ctypes.POINTER(ctypes.c_int32)]),
+    "ctcb_gemm_tf32": (c_int, [c_int, c_int, c_int, c_int, c_int, c_f32, c_vp, c_i64, c_vp, c_i64, c_f32, c_vp,
+                               c_i64, c_vp, c_int, c_vp, c_vp, c_sz, c_vp]),
+    "ctcb_gemm_pair_tf32": (c_int, [c_int, c_int, c_int, c_int, c_int, c_f32, c_vp, c_vp, c_i64, c_vp, c_vp, c_i64,
+                                    c_f32, c_vp, c_vp, c_i64, c_vp, c_sz, c_vp]),
+    "ctcb_debug_gemm_plan_tf32": (c_int, [c_int, c_int, c_int, c_int, c_int, c_vp, c_i64, c_vp, c_i64, c_int,
+                                          ctypes.POINTER(ctypes.c_int32)]),
     "ctcb_debug_set_knob": (c_int, [ctypes.c_char_p, ctypes.c_char_p]),
     "ctcb_debug_gemm_trace": (c_int, [c_vp]),
     "ctcb_debug_set_ctc_kernel": (c_int, [c_int]),
@@ -79,6 +85,8 @@ _PROTOS = {
                                              c_vp, c_vp, c_vp, c_int, c_vp, c_sz, c_vp]),
     "ctcb_brnn_sweep_f32": (c_int, [c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_f32,
                                     c_vp, c_sz, c_vp]),
+    "ctcb_brnn_sweep_tf32": (c_int, [c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                     c_f32, c_vp, c_sz, c_vp]),
     "ctcb_brnn_sweep_workspace_bytes": (c_sz, [c_int, c_int]),
     "ctcb_sweep_uses_tensor_cores": (c_int, [c_int, c_int]),
     "ctcb_lstm_sweep_workspace_bytes": (c_sz, [c_int, c_int]),
@@ -107,6 +115,7 @@ _PROTOS = {
     "ctcb_frame_stack_f32": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp]),
     "ctcb_frame_unstack_f32": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp]),
     "ctcb_debug_sweep_plan": (c_int, [c_int, c_int, c_int, ctypes.POINTER(ctypes.c_int32)]),
+    "ctcb_debug_sweep_plan_tf32": (c_int, [c_int, c_int, c_int, ctypes.POINTER(ctypes.c_int32)]),
     "ctcb_brnn_set_deferred_l2": (c_int, [c_vp, c_int]),
     "ctcb_brnn_apply_l2_f32": (c_int, [c_vp, c_vp, c_vp, c_vp]),
     "ctcb_brnn_set_dropout": (c_int, [c_vp, c_f32, ctypes.c_uint64, c_vp]),

@@ -348,6 +348,8 @@ static const char *cfg_error(const ctcb_brnn_config *c, char (&buf)[192]) {
     if (c->selfCondition == 1 && c->interLayer == 0)
         return "selfCondition 1 conditions on the intermediate CTC's posteriors and needs interLayer >= 1; interLayer "
                "is 0";
+    if (c->tf32 != 0 && c->tf32 != 1)
+        return say("tf32 %d is neither 0 (off) nor 1 (the tensor-core contractions and sweeps in TF32 mode)", c->tf32);
     const bool ok = c->inputDim > 0 && c->outputDim > 1 && c->layerSize > 0 && c->numLayers >= 1 && c->numLayers <= 64 &&
                     c->maxT > 0 && c->maxB > 0 && c->maxLabels >= 0 && c->numTemporal >= 0 &&
                     // a stacked block must lie inside the hidden layers; k <= 1 keeps the silent "no temporal layer" rule below
@@ -946,6 +948,7 @@ extern "C" int ctcb_brnn_create(const ctcb_brnn_config *cfg, ctcb_brnn **out) {
     h->nt = eff_nt(cfg);
     if (h->nt) {      // a width or batch whose sweep the device cannot hold co-resident
         const int ndir = cfg->unidirectional ? 1 : 2;
+        Tf32Scope tf32(cfg->tf32);
         // zoneout = 1: the zoneout kernels too, which run whenever a probability is > 0
         int rc = cfg->cell == 1 ? lstm_check(cfg->layerSize, cfg->maxB, ndir, cfg->peephole == 1, false)
                                 : sweep_check(cfg->layerSize, cfg->maxB, ndir);
@@ -1012,6 +1015,14 @@ extern "C" int ctcb_brnn_sweep_f32(int mode, int T, int B, int H, const int32_t 
     if (scratch_bytes < 4096) return set_error(CTCB_ENOMEM, "ctcb_brnn_sweep_f32: scratch %zu < 4096 bytes", scratch_bytes);
     return run_sweep(mode, T, B, H, T_per_utt, pre, Wf, Wb, outF, outB, actF, actB, maxAct,
                      (unsigned int *)scratch, (char *)scratch + 4096, scratch_bytes - 4096, (cudaStream_t)stream);
+}
+
+extern "C" int ctcb_brnn_sweep_tf32(int mode, int T, int B, int H, const int32_t *T_per_utt, const float *pre,
+                                    const float *Wf, const float *Wb, float *outF, float *outB, const float *actF,
+                                    const float *actB, float maxAct, void *scratch, size_t scratch_bytes, void *stream) {
+    Tf32Scope tf32(1);
+    return ctcb_brnn_sweep_f32(mode, T, B, H, T_per_utt, pre, Wf, Wb, outF, outB, actF, actB, maxAct, scratch,
+                               scratch_bytes, stream);
 }
 
 // ---- the data-parallel exchange: the early range of the net table, then everything else --------------------
@@ -1420,6 +1431,7 @@ extern "C" int ctcb_brnn_cost_and_grad_part(ctcb_brnn *h, const float *feats, co
         return set_error(CTCB_EINVAL, "ctcb_brnn_cost_and_grad_part: unknown flags 0x%x", flags);
     const bool first = (flags & CTCB_PART_FIRST) != 0, last = (flags & CTCB_PART_LAST) != 0;
     const ctcb_brnn_config &c = h->cfg;
+    Tf32Scope tf32(c.tf32);     // every contraction and sweep this call plans, training or forward-only
     if (B <= 0 || B > c.maxB || Tmax <= 0 || Tmax > c.maxT)
         return set_error(CTCB_EINVAL, "ctcb_brnn_cost_and_grad: batch %d x %d frames exceeds the configured %d x %d",
                          B, Tmax, c.maxB, c.maxT);

@@ -108,6 +108,11 @@ static int *knob_table() {
 
 int knob(Knob k) { return knob_table()[k]; }
 
+static thread_local int g_tf32 = 0;
+int tf32_mode() { return g_tf32; }
+Tf32Scope::Tf32Scope(int on) : prev(g_tf32) { g_tf32 = on ? 1 : 0; }
+Tf32Scope::~Tf32Scope() { g_tf32 = prev; }
+
 // One warp sleeping on %globaltimer until ns have passed; it writes nothing, and ns is clamped to the knob's maximum,
 // so the wait always ends.
 __global__ void stall_kernel(uint64_t ns) {

@@ -46,6 +46,15 @@ enum Knob { KNOB_GEMM, KNOB_GEMM_TC_COPY, KNOB_GEMM_TRACE, KNOB_SWEEP, KNOB_SWEE
             KNOB_SWEEP_TC_COOP, KNOB_SWEEP_TRACE, KNOB_CTC, KNOB_LSTM, KNOB_LSTM_PARTS, KNOB_SWEEP_PARTS, KNOB_STALL,
             KNOB_STALL_US, KNOB_COUNT };
 int knob(Knob k);
+// TF32 mode (include/ctcb200.h: ctcb_brnn_config.tf32): the tensor-core contraction and sweep planners take the TF32
+// kernels while a Tf32Scope(1) is alive on the calling thread.  A net's calls and the *_tf32 entry points open one
+// around their launches; everything else plans the fp32-faithful kernels.
+int tf32_mode();
+struct Tf32Scope {
+    int prev;
+    explicit Tf32Scope(int on);
+    ~Tf32Scope();
+};
 // The schedule test's stall hook (CTCB_STALL, CTCB_STALL_US): stall(st, which) launches one warp that holds `st` for
 // CTCB_STALL_US microseconds when CTCB_STALL names `which`, and does nothing otherwise (off, the default, names neither).
 // The training step calls it right after each point where one of its streams releases or is released by the other.
@@ -93,6 +102,7 @@ struct SweepPlan {
     uint32_t stage_bytes;   // tensor-core: bytes per ring stage
     size_t smem;            // dynamic shared memory per CTA
     int per_sm;             // generic: CTAs of the kernel one SM holds
+    int tf32;               // tensor-core: TF32 mode (tf32_mode() when planned)
 };
 int select_sweep(int H, int B, int ndir, SweepPlan *p);
 

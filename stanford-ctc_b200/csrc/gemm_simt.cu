@@ -367,3 +367,20 @@ extern "C" int ctcb_gemm_pair_f32(int transA, int transB, int M, int N, int K, f
     return ctcb_gemm_f32(transA, transB, M, N, K, alpha, A1, lda, B1, ldb, beta, C1, ldc, nullptr, 0, nullptr,
                          workspace, ws_bytes, stream);
 }
+
+// TF32 mode (include/ctcb200.h): the same calls with the planners in TF32 mode
+extern "C" int ctcb_gemm_tf32(int transA, int transB, int M, int N, int K, float alpha, const float *A, int64_t lda,
+                              const float *B, int64_t ldb, float beta, float *C, int64_t ldc, const float *bias,
+                              int relu, const float *mask_src, void *workspace, size_t ws_bytes, void *stream) {
+    Tf32Scope tf32(1);
+    return ctcb_gemm_f32(transA, transB, M, N, K, alpha, A, lda, B, ldb, beta, C, ldc, bias, relu, mask_src, workspace,
+                         ws_bytes, stream);
+}
+extern "C" int ctcb_gemm_pair_tf32(int transA, int transB, int M, int N, int K, float alpha, const float *A0,
+                                   const float *A1, int64_t lda, const float *B0, const float *B1, int64_t ldb,
+                                   float beta, float *C0, float *C1, int64_t ldc, void *workspace, size_t ws_bytes,
+                                   void *stream) {
+    Tf32Scope tf32(1);
+    return ctcb_gemm_pair_f32(transA, transB, M, N, K, alpha, A0, A1, lda, B0, B1, ldb, beta, C0, C1, ldc, workspace,
+                              ws_bytes, stream);
+}

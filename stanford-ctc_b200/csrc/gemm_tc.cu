@@ -29,6 +29,17 @@
 // Each product sees the same hi and lo values and the MMAs run in the same order whichever way an operand arrives, so
 // the results do not depend on the operand path.
 // Two problems of the same shape (the two recurrent weight gradients) can share one launch and one split-K reduce.
+//
+// TF32 mode (include/ctcb200.h; gemm_tc_tf32_kernel, planned while a Tf32Scope is on): each operand is rounded to the
+// nearest TF32 value (cvt.rna) instead of split, and a product is ONE MMA.  The consumers round their A fragments in
+// registers; the producer rewrites B's value slot rounded (in place when K-major, in the transpose when MN-major), so
+// no low half is written and a K-major B needs no second slot: the ring takes as many of these smaller stages as fit
+// in the fp32-faithful ring's shared memory (tc_tf32_stages).  Copied operands stay exact in the workspace and are
+// rounded in the ring like the others (rounding is idempotent).  BN, the K splits, the operand paths, the pair
+// decision and the workspace are the fp32-faithful plan's.  With a third of the MMAs a k-block is no longer bound by
+// the tensor pipe: on an H100 the traced k-block period falls from about 1920 to 1270 SM clocks (K-major 48000 x
+// 2048 x 2048), of which the MMA issue is about 375; the rest is the operand stream (32 KB per CTA per k-block, about
+// 6.6 TB/s from L2 over the 132 SMs), DESIGN.md section 6.
 #include "common.cuh"
 #include "wgmma.cuh"
 #include <cuda.h>
@@ -148,6 +159,19 @@ struct TcTile {
             for (int q = 0; q < Q; ++q) reinterpret_cast<float4 *>(lo)[threadIdx.x + 128 * q] = tc_lo4(v[q]);
         }
     }
+    // TF32 mode: the value slot `hi` receives the values rounded to TF32 (in place when K-major), and `lo` only serves
+    // as the MN-major landing area.
+    static __device__ __forceinline__ void store_rna(uint8_t *hi, const float4 (&v)[Q]) {
+        if (MN) {
+            const int r = threadIdx.x % ROWS, c0 = threadIdx.x / ROWS;
+#pragma unroll
+            for (int q = 0; q < Q; ++q)
+                *reinterpret_cast<float4 *>(hi + r * 128 + (((c0 + (128 / ROWS) * q) ^ (r & 7)) << 4)) = tf32_rna4(v[q]);
+        } else {
+#pragma unroll
+            for (int q = 0; q < Q; ++q) reinterpret_cast<float4 *>(hi)[threadIdx.x + 128 * q] = tf32_rna4(v[q]);
+        }
+    }
 };
 
 // The consumers' A fragments (WgmmaTf32Rs) of one k-block, read from the A slot and split in registers: hi[4 kk + i] is
@@ -167,7 +191,8 @@ template <bool A_MN>
 __device__ __forceinline__ int tc_tile_row(int cw, int q, int g, int h) {
     return A_MN ? 64 * cw + 32 * (q >> 1) + 8 * (q & 1) + 4 * h + 16 * (g >> 2) + (g & 3) : 64 * cw + 16 * q + g + 8 * h;
 }
-template <bool A_MN>
+// TF32 = true: hi receives the values rounded to TF32 instead, and lo is not written.
+template <bool A_MN, bool TF32>
 __device__ __forceinline__ void tc_load_split_a(uint32_t sA, int cw, int q, int g, int t, uint32_t (&hi)[16],
                                                 uint32_t (&lo)[16]) {
     // offsets of k-step kk, register i: the swizzle bits (4..6) are XORed in, the rest added
@@ -181,21 +206,32 @@ __device__ __forceinline__ void tc_load_split_a(uint32_t sA, int cw, int q, int 
                                     : ((p ^ ((2 * kk + (i >> 1)) << 4)) + (i & 1) * 1024);
             uint32_t x;
             asm volatile("ld.shared.b32 %0, [%1];" : "=r"(x) : "r"(a));
-            hi[4 * kk + i] = x;
-            lo[4 * kk + i] = __float_as_uint(__fsub_rn(__uint_as_float(x), __uint_as_float(x & 0xffffe000u)));
+            if (TF32) {
+                hi[4 * kk + i] = tf32_rna(__uint_as_float(x));
+            } else {
+                hi[4 * kk + i] = x;
+                lo[4 * kk + i] = __float_as_uint(__fsub_rn(__uint_as_float(x), __uint_as_float(x & 0xffffe000u)));
+            }
         }
     }
 }
 
-// A stage holds [A value | B value | B low half], each tile 1024-byte aligned.  A_MN / B_MN: the operand is MN-major in
-// global memory (A: four swizzled 32-row boxes, see tc_load_split_a; B: its TMA box lands in the low-half slot, see TcTile).
-template <int BN, int STAGES, bool A_MN, bool B_MN>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmB0,
-               const __grid_constant__ CUtensorMap tmA1, const __grid_constant__ CUtensorMap tmB1, GemmTcArgs g) {
+// Bytes of one ring stage: [A value | B value | B low half], each tile 1024-byte aligned.  TF32 mode has no low half;
+// the slot stays only as the landing area of an MN-major B.
+template <int BN, bool B_MN, bool TF32>
+__host__ __device__ constexpr uint32_t tc_stage_bytes() {
+    return TC_BM * TC_BK * 4 + ((TF32 && !B_MN) ? 1 : 2) * BN * TC_BK * 4;
+}
+
+// A_MN / B_MN: the operand is MN-major in global memory (A: four swizzled 32-row boxes, see tc_load_split_a; B: its TMA
+// box lands in the low-half slot, see TcTile).  TF32: one MMA of the operands rounded to TF32 per k8 step (the kernel
+// gemm_tc_tf32_kernel), else three of their hi and lo parts (gemm_tc_kernel).
+template <int BN, int STAGES, bool A_MN, bool B_MN, bool TF32>
+__device__ __forceinline__ void gemm_tc_body(const CUtensorMap &tmA0, const CUtensorMap &tmB0, const CUtensorMap &tmA1,
+                                             const CUtensorMap &tmB1, const GemmTcArgs &g) {
     constexpr uint32_t A_BYTES = TC_BM * TC_BK * 4, B_BYTES = BN * TC_BK * 4;
     constexpr uint32_t B_OFF = A_BYTES;
-    constexpr uint32_t STAGE_BYTES = B_OFF + 2 * B_BYTES;
+    constexpr uint32_t STAGE_BYTES = tc_stage_bytes<BN, B_MN, TF32>();
     extern __shared__ __align__(1024) uint8_t tc_smem[];
     // 1024-byte alignment is required by SWIZZLE_128B: align manually (dynamic smem base is only 16B-aligned by contract)
     uint8_t *base = (uint8_t *)(((uintptr_t)tc_smem + 1023) & ~(uintptr_t)1023);
@@ -243,7 +279,10 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__
                 float4 vb[TcTile<BN, B_MN>::Q];    // every load first, then every store
                 TcTile<BN, B_MN>::load(st + B_OFF, st + B_OFF + B_BYTES, vb);
                 if (B_MN) asm volatile("bar.sync 1, 128;" ::: "memory");   // the producer warpgroup only
-                TcTile<BN, B_MN>::store(st + B_OFF, st + B_OFF + B_BYTES, vb);
+                if (TF32)
+                    TcTile<BN, B_MN>::store_rna(st + B_OFF, vb);
+                else
+                    TcTile<BN, B_MN>::store(st + B_OFF, st + B_OFF + B_BYTES, vb);
                 asm volatile("fence.proxy.async.shared::cta;" ::: "memory");    // generic writes -> tensor-core (async) proxy
                 __syncwarp();
                 if (lane == 0) tc_mbar_arrive(tc_smem_u32(&ready[s]));
@@ -287,15 +326,19 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__
         tc_mbar_wait(tc_smem_u32(&full[s]), (uint32_t)(use & 1));       // (complete by now) the TMA writes these loads read
         if (threadIdx.x == 128) TC_STAMP(i, 3);
         const uint32_t sa = tc_smem_u32(base + s * STAGE_BYTES);
-        tc_load_split_a<A_MN>(sa, cw, q, lane >> 2, lane & 3, ah, al);
+        tc_load_split_a<A_MN, TF32>(sa, cw, q, lane >> 2, lane & 3, ah, al);
         const uint64_t dB = wg_desc(sa + B_OFF), dBl = wg_desc(sa + B_OFF + B_BYTES);
         wg_fence();
 #pragma unroll
         for (int k8 = 0; k8 < TC_BK / 8; ++k8) {
             const uint64_t adv = (uint64_t)((k8 * 32) >> 4);
-            WgmmaTf32Rs<BN>::mma(acc, al + 4 * k8, dB + adv, (i > 0 || k8 > 0) ? 1u : 0u);   // lo . hi
-            WgmmaTf32Rs<BN>::mma(acc, ah + 4 * k8, dBl + adv, 1u);                            // hi . lo
-            WgmmaTf32Rs<BN>::mma(acc, ah + 4 * k8, dB + adv, 1u);                             // hi . hi
+            if (TF32) {
+                WgmmaTf32Rs<BN>::mma(acc, ah + 4 * k8, dB + adv, (i > 0 || k8 > 0) ? 1u : 0u);   // rna . rna
+            } else {
+                WgmmaTf32Rs<BN>::mma(acc, al + 4 * k8, dB + adv, (i > 0 || k8 > 0) ? 1u : 0u);   // lo . hi
+                WgmmaTf32Rs<BN>::mma(acc, ah + 4 * k8, dBl + adv, 1u);                            // hi . lo
+                WgmmaTf32Rs<BN>::mma(acc, ah + 4 * k8, dB + adv, 1u);                             // hi . hi
+            }
         }
         wg_commit();
         if (threadIdx.x == 128) TC_STAMP(i, 4);
@@ -327,6 +370,19 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__
             }
         }
     }
+}
+
+template <int BN, int STAGES, bool A_MN, bool B_MN>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmB0,
+               const __grid_constant__ CUtensorMap tmA1, const __grid_constant__ CUtensorMap tmB1, GemmTcArgs g) {
+    gemm_tc_body<BN, STAGES, A_MN, B_MN, false>(tmA0, tmB0, tmA1, tmB1, g);
+}
+template <int BN, int STAGES, bool A_MN, bool B_MN>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+gemm_tc_tf32_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmB0,
+                    const __grid_constant__ CUtensorMap tmA1, const __grid_constant__ CUtensorMap tmB1, GemmTcArgs g) {
+    gemm_tc_body<BN, STAGES, A_MN, B_MN, true>(tmA0, tmB0, tmA1, tmB1, g);
 }
 
 // ---------------------------------------------------------------------------------- prep kernels
@@ -481,7 +537,16 @@ static int tc_operand_path(bool mn_major, const float *p, int64_t ld) {
 
 struct GemmTcPlan {
     int BN, stages, splits, kb_per_split, ctas, a_path, b_path, problems;
+    int tf32;    // TF32 mode (tf32_mode() when planned): gemm_tc_tf32_kernel
 };
+
+// The ring depth of a plan.  TF32 mode: as many of its smaller stages as fit in the shared memory of the fp32-faithful
+// ring, so both modes hold one CTA per SM alike.
+template <int BN, int STAGES>
+constexpr int tc_tf32_stages(bool b_mn) {
+    return (int)(STAGES * tc_stage_bytes<BN, false, false>() /
+                 (b_mn ? tc_stage_bytes<BN, true, true>() : tc_stage_bytes<BN, false, true>()));
+}
 
 // The one place that decides how a tensor-core contraction runs: the launcher (run_gemm_tc, run_gemm_tc_pair) and
 // ctcb_debug_gemm_plan both call it.  problems = 2 asks for a pair in one launch; a pair with an operand that needs a
@@ -492,6 +557,11 @@ static void gemm_tc_plan(int transA, int transB, int M, int N, int K, const floa
     p->stages = p->BN == 64 ? 4 : 3;     // 192 KB of ring either way: 4 stages of 48 KB (64-wide) or 3 of 64 KB
     p->a_path = tc_operand_path(transA != 0, A, lda);
     p->b_path = tc_operand_path(transB == 0, B, ldb);
+    p->tf32 = tf32_mode();
+    if (p->tf32) {
+        const bool bm = p->b_path == TC_PATH_MN;
+        p->stages = p->BN == 64 ? tc_tf32_stages<64, 4>(bm) : tc_tf32_stages<128, 3>(bm);
+    }
     p->problems = (problems == 2 && p->a_path != TC_PATH_COPY && p->b_path != TC_PATH_COPY) ? 2 : 1;
     const int tiles = ((M + TC_BM - 1) / TC_BM) * ((N + p->BN - 1) / p->BN);
     const int nkb = (K + TC_BK - 1) / TC_BK;
@@ -523,13 +593,16 @@ size_t gemm_tc_pair_workspace_bytes(int M, int N, int K) {
     return pair > single ? pair : single;
 }
 
-template <int BN, int STAGES, bool A_MN, bool B_MN>
+template <int BN, int STAGES, bool A_MN, bool B_MN, bool TF32>
 static int launch_tc(const CUtensorMap *tA, const CUtensorMap *tB, const GemmTcArgs &g, int ctas_z, cudaStream_t st) {
-    constexpr size_t smem = (size_t)STAGES * (TC_BM * TC_BK * 4 + 2 * BN * TC_BK * 4) + 3 * STAGES * 8 + 1024;
+    constexpr size_t smem = (size_t)STAGES * tc_stage_bytes<BN, B_MN, TF32>() + 3 * STAGES * 8 + 1024;
     static_assert(smem <= 227 * 1024, "stage ring exceeds the shared memory of a block");
-    CTCB_CUDA_CHECK(cudaFuncSetAttribute((gemm_tc_kernel<BN, STAGES, A_MN, B_MN>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    void (*kernel)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, GemmTcArgs);
+    if constexpr (TF32) kernel = gemm_tc_tf32_kernel<BN, STAGES, A_MN, B_MN>;
+    else kernel = gemm_tc_kernel<BN, STAGES, A_MN, B_MN>;
+    CTCB_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     dim3 grid((g.N + BN - 1) / BN, (g.M + TC_BM - 1) / TC_BM, ctas_z);
-    gemm_tc_kernel<BN, STAGES, A_MN, B_MN><<<grid, TC_THREADS, smem, st>>>(tA[0], tB[0], tA[1], tB[1], g);
+    kernel<<<grid, TC_THREADS, smem, st>>>(tA[0], tB[0], tA[1], tB[1], g);
     CTCB_LAUNCH_CHECK();
     return CTCB_OK;
 }
@@ -539,10 +612,17 @@ static int launch_tc_paths(const GemmTcPlan &p, const CUtensorMap *tA, const CUt
                            cudaStream_t st) {
     const int z = p.problems * p.splits;
     const bool am = p.a_path == TC_PATH_MN, bm = p.b_path == TC_PATH_MN;
-    if (am && bm) return launch_tc<BN, STAGES, true, true>(tA, tB, g, z, st);
-    if (am) return launch_tc<BN, STAGES, true, false>(tA, tB, g, z, st);
-    if (bm) return launch_tc<BN, STAGES, false, true>(tA, tB, g, z, st);
-    return launch_tc<BN, STAGES, false, false>(tA, tB, g, z, st);
+    if (p.tf32) {
+        constexpr int SK = tc_tf32_stages<BN, STAGES>(false), SM = tc_tf32_stages<BN, STAGES>(true);
+        if (am && bm) return launch_tc<BN, SM, true, true, true>(tA, tB, g, z, st);
+        if (am) return launch_tc<BN, SK, true, false, true>(tA, tB, g, z, st);
+        if (bm) return launch_tc<BN, SM, false, true, true>(tA, tB, g, z, st);
+        return launch_tc<BN, SK, false, false, true>(tA, tB, g, z, st);
+    }
+    if (am && bm) return launch_tc<BN, STAGES, true, true, false>(tA, tB, g, z, st);
+    if (am) return launch_tc<BN, STAGES, true, false, false>(tA, tB, g, z, st);
+    if (bm) return launch_tc<BN, STAGES, false, true, false>(tA, tB, g, z, st);
+    return launch_tc<BN, STAGES, false, false, false>(tA, tB, g, z, st);
 }
 
 // One launch (and, with splits, one reduce) of p.problems problems that share shape, pitches, alpha and beta.
@@ -655,6 +735,12 @@ extern "C" int ctcb_debug_gemm_plan(int transA, int transB, int M, int N, int K,
     const int32_t v[8] = {1, p.BN, p.stages, p.splits, p.ctas, p.a_path, p.b_path, p.problems};
     for (int i = 0; i < 8; ++i) out[i] = v[i];
     return CTCB_OK;
+}
+
+extern "C" int ctcb_debug_gemm_plan_tf32(int transA, int transB, int M, int N, int K, const float *A, int64_t lda,
+                                         const float *B, int64_t ldb, int problems, int32_t *out) {
+    ctcb::Tf32Scope tf32(1);
+    return ctcb_debug_gemm_plan(transA, transB, M, N, K, A, lda, B, ldb, problems, out);
 }
 
 // Diagnostic: the per-k-block clock stamps of CTA (0,0,0) of the last tensor-core GEMM (CTCB_GEMM_TRACE=1):

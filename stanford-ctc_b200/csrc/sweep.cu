@@ -252,6 +252,11 @@ extern "C" int ctcb_debug_sweep_plan(int H, int B, int ndir, int32_t *out) {
     return CTCB_OK;
 }
 
+extern "C" int ctcb_debug_sweep_plan_tf32(int H, int B, int ndir, int32_t *out) {
+    ctcb::Tf32Scope tf32(1);
+    return ctcb_debug_sweep_plan(H, B, ndir, out);
+}
+
 extern "C" int ctcb_sweep_uses_tensor_cores(int H, int B) {
     ctcb::SweepPlan p;
     return (ctcb::select_sweep(H, B, 2, &p) == CTCB_OK && p.kernel == ctcb::SWEEP_TC) ? 1 : 0;

@@ -22,6 +22,13 @@
 //   * W is streamed from L2 every step (hi + lo of both directions: 16 MB at H = 1024, 64 MB at H = 2048, against the
 //     50 MB L2 of an H100); the stream is hidden behind the MMAs whenever the batch is large enough.
 // Scratch: the (hi, lo) stacks of W (W^T for BPTT) for both directions and the two-slot ring of state low halves.
+//
+// TF32 mode (include/ctcb200.h; sweep_tc_tf32_kernel, planned while a Tf32Scope is on): the prep kernel writes W (W^T)
+// rounded to the nearest TF32 value as one plane of the stack, the epilogue writes the rounded state into the ring's
+// low-half plane (S_t in HBM stays the exact fp32 output), a stage holds one plane of each operand and a k8 step is ONE
+// MMA.  Half the stage bytes give the ring twice the stages (up to 8) in the same shared memory; W's stream from L2
+// halves.  The cluster K-slice reduction, the clip / mask epilogue, the counter barrier, the plan's CS, NS and NP and
+// the scratch are the fp32-faithful kernel's.
 #include "common.cuh"
 #include "wgmma.cuh"
 #include <cuda.h>
@@ -134,16 +141,17 @@ __device__ __forceinline__ void stc_consumer_sync() { asm volatile("bar.sync 1, 
 //                   DSMEM, epilogue (state, its low half for the next step, one counter arrival per CTA).
 // There is no generic-proxy write into the operand ring: both halves of both operands arrive by TMA.
 // ---------------------------------------------------------------------------------------------------
-template <int NP>
-__global__ void __launch_bounds__(STC_THREADS, 1)
-sweep_tc_kernel(const __grid_constant__ CUtensorMap tmW0, const __grid_constant__ CUtensorMap tmW1,
-                const __grid_constant__ CUtensorMap tmR0, const __grid_constant__ CUtensorMap tmR1, SweepTcArgs a) {
+// TF32 = true (sweep_tc_tf32_kernel): W's stack and the ring hold one plane of values rounded to TF32 each (the ring's
+// in the low-half plane), a stage holds [W | state], and a k8 step is one MMA.
+template <int NP, bool TF32>
+__device__ __forceinline__ void sweep_tc_body(const CUtensorMap &tmW0, const CUtensorMap &tmW1, const CUtensorMap &tmR0,
+                                              const CUtensorMap &tmR1, const SweepTcArgs &a) {
     extern __shared__ __align__(1024) uint8_t stc_smem[];
     uint8_t *base = (uint8_t *)(((uintptr_t)stc_smem + 1023) & ~(uintptr_t)1023);
     const int STAGES = a.stages;
     const uint32_t stage_bytes = a.stage_bytes;
     constexpr uint32_t B_BYTES = (uint32_t)NP * 128u;
-    constexpr uint32_t s_off = 2 * STC_A_BYTES;                      // where the state tiles sit inside a stage
+    constexpr uint32_t s_off = (TF32 ? 1 : 2) * STC_A_BYTES;         // where the state tiles sit inside a stage
     uint8_t *after_ring = base + (size_t)STAGES * stage_bytes;
     // the partial product [NP][128] has a region of its own when it fits (then W tiles of the NEXT step may land in
     // the ring while peers still read this CTA's partial); otherwise it aliases the ring and nothing is prefetched
@@ -195,9 +203,9 @@ sweep_tc_kernel(const __grid_constant__ CUtensorMap tmW0, const __grid_constant_
     auto issue_W = [&](uint32_t g) {
         const int st = (int)(g % (uint32_t)STAGES);
         const uint32_t fb = stc_smem_u32(&fullW[st]);
-        stc_mbar_expect_tx(fb, 2 * STC_A_BYTES);
+        stc_mbar_expect_tx(fb, (TF32 ? 1 : 2) * STC_A_BYTES);
         const int i = (int)(g % (uint32_t)nkb);
-        stc_tma_3d(stc_smem_u32(base + (size_t)st * stage_bytes), tmW, fb, (rank * nkb + i) * STC_BK, m0, 0);   // both planes
+        stc_tma_3d(stc_smem_u32(base + (size_t)st * stage_bytes), tmW, fb, (rank * nkb + i) * STC_BK, m0, 0);   // every plane
     };
 
     for (int s = 0; s < T; ++s) {
@@ -253,8 +261,8 @@ sweep_tc_kernel(const __grid_constant__ CUtensorMap tmW0, const __grid_constant_
                     const int kc = (rank * nkb + (int)(g % (uint32_t)nkb)) * STC_BK;
                     if (leader) {
                         if (need_w) issue_W(g);
-                        stc_mbar_expect_tx(fb, 2 * B_BYTES);
-                        stc_tma_4d(sdst, tmR, fb, kc, b_lo, 0, (s - 1) & 1);
+                        stc_mbar_expect_tx(fb, (TF32 ? 1 : 2) * B_BYTES);
+                        stc_tma_4d(sdst, tmR, fb, kc, b_lo, TF32 ? 1 : 0, (s - 1) & 1);
                     }
                     __syncwarp();
                 }
@@ -292,9 +300,13 @@ sweep_tc_kernel(const __grid_constant__ CUtensorMap tmW0, const __grid_constant_
 #pragma unroll
                     for (int k8 = 0; k8 < STC_BK / 8; ++k8) {
                         const uint64_t adv = (uint64_t)((k8 * 32) >> 4);
-                        WgmmaTf32<NP>::mma(acc, dAl + adv, dB + adv, (g > g0 || k8 > 0) ? 1u : 0u);   // lo . hi
-                        WgmmaTf32<NP>::mma(acc, dA + adv, dBl + adv, 1u);                           // hi . lo
-                        WgmmaTf32<NP>::mma(acc, dA + adv, dB + adv, 1u);                            // hi . hi
+                        if (TF32) {
+                            WgmmaTf32<NP>::mma(acc, dA + adv, dB + adv, (g > g0 || k8 > 0) ? 1u : 0u);   // rna . rna
+                        } else {
+                            WgmmaTf32<NP>::mma(acc, dAl + adv, dB + adv, (g > g0 || k8 > 0) ? 1u : 0u);   // lo . hi
+                            WgmmaTf32<NP>::mma(acc, dA + adv, dBl + adv, 1u);                           // hi . lo
+                            WgmmaTf32<NP>::mma(acc, dA + adv, dB + adv, 1u);                            // hi . hi
+                        }
                     }
                     wg_commit();
                     // the previous job's MMAs are complete once at most this one is outstanding: release its slot
@@ -353,7 +365,9 @@ sweep_tc_kernel(const __grid_constant__ CUtensorMap tmW0, const __grid_constant_
                 }
                 if (t >= Tb[ci]) v = make_float4(0.f, 0.f, 0.f, 0.f);
                 *reinterpret_cast<float4 *>(out + ((int64_t)t * B + b) * H + j4) = v;
-                if (s + 1 < T) {      // the next step's B operands: v again (same tensor map as its low half) and the low half
+                if (s + 1 < T && TF32) {      // the next step's B operand: v rounded to TF32
+                    *reinterpret_cast<float4 *>(ring_s + (int64_t)(B + b) * H + j4) = tf32_rna4(v);
+                } else if (s + 1 < T) {      // the next step's B operands: v again (same tensor map as its low half) and the low half
                     *reinterpret_cast<float4 *>(ring_s + (int64_t)b * H + j4) = v;
                     float4 lo;
                     lo.x = v.x - __uint_as_float(__float_as_uint(v.x) & 0xffffe000u);
@@ -382,9 +396,24 @@ sweep_tc_kernel(const __grid_constant__ CUtensorMap tmW0, const __grid_constant_
     stc_cluster_sync();
 }
 
+template <int NP>
+__global__ void __launch_bounds__(STC_THREADS, 1)
+sweep_tc_kernel(const __grid_constant__ CUtensorMap tmW0, const __grid_constant__ CUtensorMap tmW1,
+                const __grid_constant__ CUtensorMap tmR0, const __grid_constant__ CUtensorMap tmR1, SweepTcArgs a) {
+    sweep_tc_body<NP, false>(tmW0, tmW1, tmR0, tmR1, a);
+}
+template <int NP>
+__global__ void __launch_bounds__(STC_THREADS, 1)
+sweep_tc_tf32_kernel(const __grid_constant__ CUtensorMap tmW0, const __grid_constant__ CUtensorMap tmW1,
+                     const __grid_constant__ CUtensorMap tmR0, const __grid_constant__ CUtensorMap tmR1, SweepTcArgs a) {
+    sweep_tc_body<NP, true>(tmW0, tmW1, tmR0, tmR1, a);
+}
+
 // Operand preparation, once per launch: out[0] = W (or W^T for BPTT), out[1] = its low half x - tf32(x); both H x H
-// row-major, stacked so that ONE 3-D TMA box fetches the hi and the lo tile of a k-block.
-__global__ void stc_prep_kernel(const float *__restrict__ w, float *__restrict__ stack, int H, int transpose) {
+// row-major, stacked so that ONE 3-D TMA box fetches the hi and the lo tile of a k-block.  TF32 mode
+// (stc_prep_tf32_kernel): out[0] = W (or W^T) rounded to TF32, and no out[1].
+template <bool TF32>
+__device__ __forceinline__ void stc_prep(const float *__restrict__ w, float *__restrict__ stack, int H, int transpose) {
     __shared__ float tile[32][33];
     const int c0 = blockIdx.x * 32, r0 = blockIdx.y * 32;
     float *hi = stack, *lo = stack + (size_t)H * H;
@@ -394,17 +423,31 @@ __global__ void stc_prep_kernel(const float *__restrict__ w, float *__restrict__
         for (int i = threadIdx.y; i < 32; i += 8) {
             const float v = tile[threadIdx.x][i];
             const int64_t o = (int64_t)(c0 + i) * H + r0 + threadIdx.x;
-            hi[o] = v;
-            lo[o] = v - __uint_as_float(__float_as_uint(v) & 0xffffe000u);
+            if (TF32) {
+                hi[o] = __uint_as_float(tf32_rna(v));
+            } else {
+                hi[o] = v;
+                lo[o] = v - __uint_as_float(__float_as_uint(v) & 0xffffe000u);
+            }
         }
     } else {
         for (int i = threadIdx.y; i < 32; i += 8) {
             const int64_t o = (int64_t)(r0 + i) * H + c0 + threadIdx.x;
             const float v = w[o];
-            hi[o] = v;
-            lo[o] = v - __uint_as_float(__float_as_uint(v) & 0xffffe000u);
+            if (TF32) {
+                hi[o] = __uint_as_float(tf32_rna(v));
+            } else {
+                hi[o] = v;
+                lo[o] = v - __uint_as_float(__float_as_uint(v) & 0xffffe000u);
+            }
         }
     }
+}
+__global__ void stc_prep_kernel(const float *__restrict__ w, float *__restrict__ stack, int H, int transpose) {
+    stc_prep<false>(w, stack, H, transpose);
+}
+__global__ void stc_prep_tf32_kernel(const float *__restrict__ w, float *__restrict__ stack, int H, int transpose) {
+    stc_prep<true>(w, stack, H, transpose);
 }
 
 // ---------------------------------------------------------------------------------- host side
@@ -470,12 +513,14 @@ static bool stc_plan_cs(int H, int B, int ndir, int cs, SweepPlan *p) {
     p->cs = cs;
     p->groups = (B + Npad - 1) / Npad;       // drop splits that would be empty
     p->np = Npad;
+    p->tf32 = tf32_mode();
     const size_t partial_bytes = (size_t)Npad * 512;
-    p->stage_bytes = 2 * STC_A_BYTES + 2 * (uint32_t)Npad * 128u;
+    // TF32 mode: one plane of each operand per stage, so about twice the stages in the same shared memory
+    p->stage_bytes = (p->tf32 ? 1 : 2) * (STC_A_BYTES + (uint32_t)Npad * 128u);
     // own region for the partial when at least two ring stages still fit beside it
     p->partial_own = (STC_SMEM_MAX >= partial_bytes + 2 * (size_t)p->stage_bytes) ? 1 : 0;
     int stages = (int)((STC_SMEM_MAX - (p->partial_own ? partial_bytes : 0)) / p->stage_bytes);
-    if (stages > 6) stages = 6;
+    if (stages > (p->tf32 ? 8 : 6)) stages = p->tf32 ? 8 : 6;     // the kernel has barriers for 8
     if (stages < 2) return false;
     if (!p->partial_own && (size_t)stages * p->stage_bytes < partial_bytes) return false;    // the ring must hold the aliased partial
     p->stages = stages;
@@ -504,23 +549,31 @@ size_t sweep_tc_workspace_bytes(int H, int B) {
     return stc_ws_stack_bytes(H) + stc_ws_ring_bytes(H, B) + STC_TRACE_STEPS * 16 * 8 + 1024;
 }
 
-template <int NP>
+template <int NP, bool TF32>
 static cudaError_t stc_launch(cudaLaunchConfig_t *cfg, const CUtensorMap *tmW, const CUtensorMap *tmR, const SweepTcArgs &a) {
-    cudaError_t e = cudaFuncSetAttribute(sweep_tc_kernel<NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg->dynamicSmemBytes);
+    void (*kernel)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, SweepTcArgs);
+    if constexpr (TF32) kernel = sweep_tc_tf32_kernel<NP>;
+    else kernel = sweep_tc_kernel<NP>;
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg->dynamicSmemBytes);
     if (e != cudaSuccess) return e;
-    return cudaLaunchKernelEx(cfg, sweep_tc_kernel<NP>, tmW[0], tmW[1], tmR[0], tmR[1], a);
+    return cudaLaunchKernelEx(cfg, kernel, tmW[0], tmW[1], tmR[0], tmR[1], a);
 }
+template <bool TF32>
 static cudaError_t stc_launch_np(int np, cudaLaunchConfig_t *cfg, const CUtensorMap *tmW, const CUtensorMap *tmR, const SweepTcArgs &a) {
     switch (np) {
-        case 32: return stc_launch<32>(cfg, tmW, tmR, a);
-        case 64: return stc_launch<64>(cfg, tmW, tmR, a);
-        case 96: return stc_launch<96>(cfg, tmW, tmR, a);
-        case 128: return stc_launch<128>(cfg, tmW, tmR, a);
-        case 160: return stc_launch<160>(cfg, tmW, tmR, a);
-        case 192: return stc_launch<192>(cfg, tmW, tmR, a);
-        case 224: return stc_launch<224>(cfg, tmW, tmR, a);
-        default: return stc_launch<256>(cfg, tmW, tmR, a);
+        case 32: return stc_launch<32, TF32>(cfg, tmW, tmR, a);
+        case 64: return stc_launch<64, TF32>(cfg, tmW, tmR, a);
+        case 96: return stc_launch<96, TF32>(cfg, tmW, tmR, a);
+        case 128: return stc_launch<128, TF32>(cfg, tmW, tmR, a);
+        case 160: return stc_launch<160, TF32>(cfg, tmW, tmR, a);
+        case 192: return stc_launch<192, TF32>(cfg, tmW, tmR, a);
+        case 224: return stc_launch<224, TF32>(cfg, tmW, tmR, a);
+        default: return stc_launch<256, TF32>(cfg, tmW, tmR, a);
     }
+}
+static cudaError_t stc_launch_plan(const SweepPlan &p, cudaLaunchConfig_t *cfg, const CUtensorMap *tmW, const CUtensorMap *tmR,
+                                   const SweepTcArgs &a) {
+    return p.tf32 ? stc_launch_np<true>(p.np, cfg, tmW, tmR, a) : stc_launch_np<false>(p.np, cfg, tmW, tmR, a);
 }
 
 // the tensor-core plan for (H, B, ndir), when this kernel applies
@@ -539,7 +592,10 @@ int run_sweep_tc(const SweepPlan &p, int mode, int T, int B, int H, const int32_
     float *ring = (float *)((char *)ws + stc_ws_stack_bytes(H));
     const float *Wd[2] = {Wf, Wb ? Wb : Wf};
     for (int d = 0; d < ndir; ++d) {
-        stc_prep_kernel<<<dim3(H / 32, H / 32), dim3(32, 8), 0, st>>>(Wd[d], stack + (size_t)d * 2 * H * H, H, mode == 1 ? 1 : 0);
+        if (p.tf32)
+            stc_prep_tf32_kernel<<<dim3(H / 32, H / 32), dim3(32, 8), 0, st>>>(Wd[d], stack + (size_t)d * 2 * H * H, H, mode == 1);
+        else
+            stc_prep_kernel<<<dim3(H / 32, H / 32), dim3(32, 8), 0, st>>>(Wd[d], stack + (size_t)d * 2 * H * H, H, mode == 1 ? 1 : 0);
         CTCB_LAUNCH_CHECK();
     }
     float *outs[2] = {outF, Wb ? outB : outF};
@@ -547,9 +603,9 @@ int run_sweep_tc(const SweepPlan &p, int mode, int T, int B, int H, const int32_
     for (int d = 0; d < 2; ++d) {
         const int dd = (d < ndir) ? d : 0;
         {
-            cuuint64_t dims[3] = {(cuuint64_t)H, (cuuint64_t)H, 2};
+            cuuint64_t dims[3] = {(cuuint64_t)H, (cuuint64_t)H, p.tf32 ? 1u : 2u};
             cuuint64_t strides[2] = {(cuuint64_t)H * sizeof(float), (cuuint64_t)H * H * sizeof(float)};
-            cuuint32_t box[3] = {(cuuint32_t)STC_BK, (cuuint32_t)STC_BM, 2};
+            cuuint32_t box[3] = {(cuuint32_t)STC_BK, (cuuint32_t)STC_BM, p.tf32 ? 1u : 2u};
             cuuint32_t es[3] = {1, 1, 1};
             CUresult r = enc(&tmW[d], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, (void *)(stack + (size_t)dd * 2 * H * H), dims, strides, box, es,
                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -559,7 +615,7 @@ int run_sweep_tc(const SweepPlan &p, int mode, int T, int B, int H, const int32_
         {
             cuuint64_t dims[4] = {(cuuint64_t)H, (cuuint64_t)B, 2, 2};
             cuuint64_t strides[3] = {(cuuint64_t)H * sizeof(float), (cuuint64_t)B * H * sizeof(float), (cuuint64_t)2 * B * H * sizeof(float)};
-            cuuint32_t box[4] = {(cuuint32_t)STC_BK, (cuuint32_t)p.np, 2, 1};
+            cuuint32_t box[4] = {(cuuint32_t)STC_BK, (cuuint32_t)p.np, p.tf32 ? 1u : 2u, 1};   // TF32: the rounded plane
             cuuint32_t es[4] = {1, 1, 1, 1};
             CUresult r = enc(&tmR[d], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void *)(ring + (size_t)dd * 4 * B * H), dims, strides, box, es,
                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
@@ -591,14 +647,14 @@ int run_sweep_tc(const SweepPlan &p, int mode, int T, int B, int H, const int32_
     static int coop = -1;     // does this driver accept cluster + cooperative together?  Learned at the first such launch
     if (knob(KNOB_SWEEP_TC_COOP) && coop != 0) {     // CTCB_SWEEP_TC_COOP=0: plain cluster launch
         cfg.numAttrs = 2;
-        cudaError_t e = stc_launch_np(p.np, &cfg, tmW, tmR, a);
+        cudaError_t e = stc_launch_plan(p, &cfg, tmW, tmR, a);
         if (e == cudaSuccess) { coop = 1; count_launch(); return CTCB_OK; }
         cudaGetLastError();
         if (coop == 1) return set_error(CTCB_ECUDA, "sweep_tc: launch failed: %s", cudaGetErrorString(e));
         coop = 0;
     }
     cfg.numAttrs = 1;         // grid <= one wave of clusters by construction (stc_plan)
-    CTCB_CUDA_CHECK(stc_launch_np(p.np, &cfg, tmW, tmR, a));
+    CTCB_CUDA_CHECK(stc_launch_plan(p, &cfg, tmW, tmR, a));
     count_launch();
     return CTCB_OK;
 }

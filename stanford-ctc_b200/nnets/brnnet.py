@@ -60,6 +60,11 @@ single contiguous vector.  New, additive surface for the minibatch/data-parallel
                                                 the layers above read that, in training and forward-only calls alike;
                                                 one [W_c (H x K), b_c (H x 1)] pair appended to `stack` behind
                                                 everything else, both 0 at start (the net starts as the InterCTC net)
+    NNet(..., tf32=True)                     TF32 mode (include/ctcb200.h: tf32): every tensor-core contraction and
+                                                sweep of training and forward-only calls reads its operands rounded
+                                                to TF32 and runs one MMA per product instead of three, as PyTorch's
+                                                allow_tf32; no parameter or workspace changes, so checkpoints load
+                                                in either mode
     costAndGradBatch(datas, labelss)         -> (costs[B], grad, skips[B])   host arrays in; more than maxUtts
                                                 utterances are accumulated over micro-batches
     costAndGradDevice(batch, first, last)    -> no host sync; see DeviceBatch
@@ -209,7 +214,7 @@ class NNet:
                  dropoutSeed=33, cell="relu", layerNorm=False, subsample=1, subsampleLayer=1, peephole=False,
                  freqMasks=0, freqMaskWidth=0, timeMasks=0, timeMaskWidth=0, timeMaskRatio=1.0, featDim=None,
                  weightNoise=0.0, zoneoutCell=0.0, zoneoutHidden=0.0, interLayer=0, interWeight=0.0,
-                 selfCondition=False):
+                 selfCondition=False, tf32=False):
         # The intermediate CTC loss (include/ctcb200.h: interLayer).  The library refuses a layer outside
         # 1..numLayers-1 and a subsampled output map, with its message; a layer and a weight come only together.
         self.interLayer, self.interWeight = int(interLayer), float(interWeight)
@@ -220,6 +225,7 @@ class NNet:
         self.selfCondition = bool(selfCondition)
         if self.selfCondition and self.interLayer == 0:
             raise ValueError("selfCondition=True conditions on the intermediate CTC's posteriors; it needs interLayer >= 1")
+        self.tf32 = bool(tf32)
         torch = _ctcb.require_cuda()
         self._torch = torch
         self.dev = torch.device("cuda", torch.cuda.current_device() if device is None else device)
@@ -298,7 +304,7 @@ class NNet:
                                self.numTemporal, _ctcb.CELLS[cell], int(self.layerNorm), self.subsample,
                                self.subsampleLayer, int(self.peephole), self.featDim or 0,
                                int(self.weightNoise > 0.0), int(self.zoneout), self.interLayer, self.interWeight,
-                               int(self.selfCondition))
+                               int(self.selfCondition), int(self.tf32))
         self._h = ctypes.c_void_p()
         check(lib.ctcb_brnn_create(ctypes.byref(self._cfg), ctypes.byref(self._h)))
         self.stack = None

@@ -11,7 +11,7 @@ h[:,t] = clip(pre[:,t] + Wt.h[:,t-1], 0, 20) (rnnet.py:112-116), BPTT rnnet.py:1
 term in this class.  layerNorm=True normalises the ReLU hidden layers.  subsample=k runs map subsampleLayer and above at 1/k
 of the frame rate; costAndGrad(train=False) best-path decodes those ceil(T / k) frames.  cell='lstm' makes the temporal layers uni-directional LSTMs (peephole=True adds their peephole connections).  numTemporal=k stacks k such layers (stack ends with [Wt_1, dummy] .. [Wt_k, dummy]).  initParams, updateParams, toFile, fromFile, check_grad and the minibatch additions
 (maxUtts, costAndGradBatch, costAndGradDevice, dropout, the input masks, the weight noise, zoneout, the intermediate CTC
-loss interLayer / interWeight and its selfCondition) are inherited.
+loss interLayer / interWeight and its selfCondition, TF32 mode tf32) are inherited.
 """
 import numpy as np
 
@@ -26,7 +26,7 @@ class NNet(brnnet.NNet):
                  allowTopTemporal=False, dropout=0.0, dropoutSeed=33, cell="relu", layerNorm=False, subsample=1,
                  subsampleLayer=1, peephole=False, freqMasks=0, freqMaskWidth=0, timeMasks=0, timeMaskWidth=0,
                  timeMaskRatio=1.0, featDim=None, weightNoise=0.0, zoneoutCell=0.0, zoneoutHidden=0.0, interLayer=0,
-                 interWeight=0.0, selfCondition=False):
+                 interWeight=0.0, selfCondition=False, tf32=False):
         brnnet.NNet.__init__(self, inputDim, outputDim, layerSize, numLayers, maxBatch, train=train,
                              temporalLayer=temporalLayer, reg=0.0, maxUtts=maxUtts, maxLabels=maxLabels,
                              allowTopTemporal=allowTopTemporal, device=device, unidirectional=True,
@@ -36,7 +36,7 @@ class NNet(brnnet.NNet):
                              timeMaskWidth=timeMaskWidth, timeMaskRatio=timeMaskRatio, featDim=featDim,
                              weightNoise=weightNoise, zoneoutCell=zoneoutCell, zoneoutHidden=zoneoutHidden,
                              interLayer=interLayer, interWeight=interWeight,
-                             selfCondition=selfCondition)
+                             selfCondition=selfCondition, tf32=tf32)
 
     def costAndGrad(self, data, labels=None):
         if not self.train:

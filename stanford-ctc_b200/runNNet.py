@@ -9,7 +9,7 @@ The implementation is organised differently: a declarative flag table, one RunDi
 side files, and separate train/evaluate phases.  Site paths of run_cfg.py / decoder_config.py became
 flags (--runDir, --outDir); new flags: --numTemporal, --cell, --peephole, --layerNorm, --subsample, --subsampleLayer, --batchSize, --maxUtts, --maxLabels,
 --dropout, --freqMasks, --freqMaskWidth, --timeMasks, --timeMaskWidth, --timeMaskRatio, --featDim, --weightNoise,
---zoneoutCell, --zoneoutHidden, --interLayer, --interWeight, --selfCondition,
+--zoneoutCell, --zoneoutHidden, --interLayer, --interWeight, --selfCondition, --tf32,
 --optimizer,
 --beta1, --beta2, --epsilon, --quiet.  Under torchrun the same
 script trains data-parallel (one process per GPU, one NCCL all-reduce per step).
@@ -90,6 +90,9 @@ FLAGS = [
     ("selfCondition", None, False, "self-conditioned CTC (needs --interLayer): the intermediate posteriors, projected "
                                    "back to the layer's width, are added to layer m's output, in training and in --test "
                                    "alike; a cfg.json written without it has none"),
+    ("tf32", None, False, "TF32 mode: the tensor-core contractions and sweeps read their operands rounded to TF32 and "
+                          "run one MMA per product instead of three (PyTorch's allow_tf32), in training and in --test "
+                          "alike; checkpoints are the same in both modes; a cfg.json written without it is off"),
     ("optimizer", str, "nesterov", "update rule: nesterov (the reference's, with --momentum), adagrad or adam; --step "
                                    "is the step size of each and --anneal applies to it"),
     ("beta1", float, 0.9, "adam: decay of the first-moment estimate"),
@@ -240,7 +243,7 @@ def _train(opts, cfg, run_dir, log, rank, world):
                      timeMasks=opts.timeMasks, timeMaskWidth=opts.timeMaskWidth, timeMaskRatio=opts.timeMaskRatio,
                      featDim=opts.featDim, weightNoise=opts.weightNoise, zoneoutCell=opts.zoneoutCell,
                      zoneoutHidden=opts.zoneoutHidden, interLayer=opts.interLayer, interWeight=opts.interWeight,
-                     selfCondition=opts.selfCondition)
+                     selfCondition=opts.selfCondition, tf32=opts.tf32)
     net.initParams()
     optimizer = sgd.SGD(net, opts.maxUttLen, alpha=opts.step, optimizer=opts.optimizer, momentum=opts.momentum,
                         batchSize=opts.batchSize, verbose=(rank == 0 and not opts.quiet), beta1=opts.beta1,
@@ -308,7 +311,7 @@ def test(opts, rank=0, world=1):
                      temporalLayer=trained.temporalLayer, train=False, maxUtts=max(1, opts.maxUtts),
                      numTemporal=trained.numTemporal, cell=trained.cell, layerNorm=trained.layerNorm,
                      subsample=trained.subsample, subsampleLayer=trained.subsampleLayer, peephole=trained.peephole,
-                     zoneoutCell=trained.zoneoutCell, zoneoutHidden=trained.zoneoutHidden, **cond)
+                     zoneoutCell=trained.zoneoutCell, zoneoutHidden=trained.zoneoutHidden, tf32=trained.tf32, **cond)
     net.initParams()
     with open(trained.in_file, "rb") as fid:
         pickle.load(fid)                              # optimiser state: not needed here
