@@ -539,8 +539,9 @@ int ctcb_brnn_set_dropout(ctcb_brnn *h, float p, uint64_t seed, const int64_t *s
  * stride < 1.  Host-only. */
 int ctcb_brnn_set_dropout_utts(ctcb_brnn *h, int64_t first, int64_t stride);
 /* *step += 1 on `stream` (one thread); inside a capture it becomes part of the graph like any other launch.  The
- * counter is the optimisation step: the dropout mask and the adaptive optimisers (ctcb_adagrad_step_f32,
- * ctcb_adam_step_f32) read the same one, and sgd.SGD advances it once per step, so it equals SGD.it. */
+ * counter is the optimisation step: the dropout mask, the adaptive optimisers (ctcb_adagrad_step_f32,
+ * ctcb_adam_step_f32) and the weight average (ctcb_ema_update_f32) read the same one, and sgd.SGD advances it once per
+ * step, so it equals SGD.it. */
 int ctcb_dropout_advance(int64_t *step, void *stream);
 
 /* ---- SpecAugment: frequency and time masks of the input features (Park et al., Interspeech 2019) --------------------
@@ -777,6 +778,19 @@ int ctcb_adagrad_step_f32(float *w, float *r, const float *g, int64_t n, float a
 int ctcb_adam_step_f32(float *w, float *m, float *v, const float *g, int64_t n, float alpha, float beta1,
                        float beta2, float eps, float max_gnorm, const float *gnorm2, const float *n_valid,
                        const int64_t *step, void *stream);
+/* Exponential moving average of the weights (Polyak averaging while it warms up), one pass over the flat vector, run
+ * after the rule's update on the w it just wrote (Nesterov: the clean weight, the look-ahead undone).  With decay d in
+ * [0, 1) and t = max(1, *step), the int64 at `step` (DEVICE memory: the counter of ctcb_dropout_advance) read when the
+ * kernel runs:
+ *   d_t = min(d, 1 - 1/t)      (float64, rounded to float32 once)
+ *   avg = fmaf(d_t, avg - w, w)   element-wise in float32, i.e. avg = w + d_t (avg - w)
+ * At t = 1, d_t = 0 and avg becomes a copy of w bit for bit.  While 1 - 1/t < d, avg is the plain mean of the iterates
+ * w_1 .. w_t; after that an EMA of decay d (d = 0.9999: the mean of the first 10 000 steps, then the EMA).  When n_valid
+ * (optional device float) reads 0, avg is left bit for bit unchanged; the caller still advances the counter.  12 B per
+ * parameter.  Checked on the host before any launch: n <= 0 is a no-op; CTCB_EINVAL for a null avg, w or step, and for
+ * a decay that is NaN or outside [0, 1). */
+int ctcb_ema_update_f32(float *avg, const float *w, int64_t n, float decay, const float *n_valid, const int64_t *step,
+                        void *stream);
 
 /* ---- CUDA graphs: replay one optimisation step (the reference issues ~16(N+3)+8(T-1) launches per utterance,
  *      sgd.py:91-161 + brnnet.py:117-249; this library ~40 per minibatch) as ONE graph launch -----------------------

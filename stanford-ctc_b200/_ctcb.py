@@ -144,6 +144,7 @@ _PROTOS = {
     "ctcb_adagrad_step_f32": (c_int, [c_vp, c_vp, c_vp, c_i64, c_f32, c_f32, c_vp, c_vp, c_vp, c_vp]),
     "ctcb_adam_step_f32": (c_int, [c_vp, c_vp, c_vp, c_vp, c_i64, c_f32, c_f32, c_f32, c_f32, c_f32, c_vp, c_vp, c_vp,
                                    c_vp]),
+    "ctcb_ema_update_f32": (c_int, [c_vp, c_vp, c_i64, c_f32, c_vp, c_vp, c_vp]),
 }
 
 EXPORTS = sorted(_PROTOS)

@@ -7,7 +7,8 @@
 //   ctc_fast/sgd.py:161 and nnets/brnnet.py:251-256 (w += v)
 // with one axpy, one two-stage sum of squares and one fused update kernel; the clip scale is
 // computed on the device from the reduced norm, so the step never synchronises with the host.
-// AdaGrad (ctc_fast/sgd.py:143-158) and Adam, not in the reference's working code, are one fused kernel each.
+// AdaGrad (ctc_fast/sgd.py:143-158) and Adam, not in the reference's working code, are one fused kernel each; the
+// exponential moving average of the weights is one more pass behind whichever rule ran.
 #include <cmath>
 #include "common.cuh"
 
@@ -125,6 +126,24 @@ __global__ void adam_kernel(float *__restrict__ w, float *__restrict__ m, float 
     }
 }
 
+// The weight average (include/ctcb200.h: ctcb_ema_update_f32), launched after the rule's kernel on the w it wrote:
+// a <- fmaf(d_t, a - w, w),  d_t = min(d, 1 - 1/t)                                                  12 B per parameter
+// d_t = 0 (t <= 1) is a plain copy, so a becomes w bit for bit whatever a held (-0.0, infinities and NaN included).
+__global__ void ema_kernel(float *__restrict__ a, const float *__restrict__ w, int64_t n, float decay,
+                           const float *__restrict__ n_valid, const int64_t *__restrict__ step) {
+    if (n_valid != nullptr && n_valid[0] == 0.f) return;
+    const float d = (float)fmin((double)decay, 1.0 - 1.0 / step_number(step));
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    if (d == 0.f) {
+        for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) a[i] = w[i];
+        return;
+    }
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+        const float wi = w[i];
+        a[i] = fmaf(d, a[i] - wi, wi);
+    }
+}
+
 static int ew_blocks(int64_t n) {
     int64_t b = (n + 1023) / 1024;
     const int cap = 8 * num_sms();
@@ -203,6 +222,18 @@ extern "C" int ctcb_adam_step_f32(float *w, float *m, float *v, const float *g, 
     ProfScope ps("sgd", (cudaStream_t)stream);
     adam_kernel<<<ew_blocks(n), 256, 0, (cudaStream_t)stream>>>(w, m, v, g, n, alpha, beta1, beta2, eps, max_gnorm,
                                                                 gnorm2, n_valid, step);
+    CTCB_LAUNCH_CHECK();
+    return CTCB_OK;
+}
+
+extern "C" int ctcb_ema_update_f32(float *avg, const float *w, int64_t n, float decay, const float *n_valid,
+                                   const int64_t *step, void *stream) {
+    if (n <= 0) return CTCB_OK;
+    if (!avg || !w || !step) return set_error(CTCB_EINVAL, "ctcb_ema_update_f32: null pointer");
+    if (!valid_beta(decay))
+        return set_error(CTCB_EINVAL, "ctcb_ema_update_f32: decay=%g must be in [0, 1)", (double)decay);
+    ProfScope ps("sgd", (cudaStream_t)stream);
+    ema_kernel<<<ew_blocks(n), 256, 0, (cudaStream_t)stream>>>(avg, w, n, decay, n_valid, step);
     CTCB_LAUNCH_CHECK();
     return CTCB_OK;
 }

@@ -11,7 +11,8 @@ flags (--runDir, --outDir); new flags: --numTemporal, --cell, --peephole, --laye
 --dropout, --freqMasks, --freqMaskWidth, --timeMasks, --timeMaskWidth, --timeMaskRatio, --featDim, --weightNoise,
 --zoneoutCell, --zoneoutHidden, --interLayer, --interWeight, --selfCondition, --tf32,
 --optimizer,
---beta1, --beta2, --epsilon, --quiet.  Under torchrun the same
+--beta1, --beta2, --epsilon, --emaDecay, --lastWeights, --quiet.  With --emaDecay, params.pk holds a third pickle,
+the weight average in the stack's format.  Under torchrun the same
 script trains data-parallel (one process per GPU, one NCCL all-reduce per step).
 """
 import argparse
@@ -98,6 +99,12 @@ FLAGS = [
     ("beta1", float, 0.9, "adam: decay of the first-moment estimate"),
     ("beta2", float, 0.999, "adam: decay of the second-moment estimate"),
     ("epsilon", float, 1e-8, "adam: added to the square root of the second moment"),
+    ("emaDecay", float, 0.0, "decay d in [0, 1) of an exponential moving average of the weights, updated every step "
+                             "(the mean of the iterates until step 1/(1-d), then the EMA); checkpoints carry it as a "
+                             "third pickle of params.pk and --test writes the arks from it (0 = off; a cfg.json written "
+                             "without it has none)"),
+    ("lastWeights", None, False, "--test of a run trained with --emaDecay: write the arks from the last weights, not "
+                                 "from the average (taken from the command line, not from cfg.json)"),
     ("runDir", str, "./runs", "parent of the time-stamped run directory"),
     ("outDir", str, None, "--test: directory for the likelihood arks"),
     ("quiet", None, False, "no console logging / per-iteration prints"),
@@ -170,9 +177,12 @@ class RunDir(object):
             fid.write(str(value))
 
     def checkpoint(self, optimizer, net, suffix=""):
-        with open(self.file("params.pk") + suffix, "wb") as fid:     # two pickles back to back
+        # two pickles back to back, the SGD state and the stack; with a weight average, the average as a third
+        with open(self.file("params.pk") + suffix, "wb") as fid:
             optimizer.toFile(fid)
             net.toFile(fid)
+            if optimizer.average is not None:
+                optimizer.averageToFile(fid)
 
 
 def _attach_logging(run, rank, quiet):
@@ -216,7 +226,7 @@ def run(args=None):
     cfg["output_dir"] = out_dir
     cfg["in_file"] = cfg["out_file"] = os.path.join(out_dir, "params.pk")
     if cli.test:                                      # these come from the command line, not the stored config
-        for key in ("dataDir", "numFiles", "startFile", "outDir", "maxUtts"):
+        for key in ("dataDir", "numFiles", "startFile", "outDir", "maxUtts", "lastWeights"):
             cfg[key] = getattr(cli, key)
 
     run_dir = RunDir(out_dir)
@@ -247,17 +257,19 @@ def _train(opts, cfg, run_dir, log, rank, world):
     net.initParams()
     optimizer = sgd.SGD(net, opts.maxUttLen, alpha=opts.step, optimizer=opts.optimizer, momentum=opts.momentum,
                         batchSize=opts.batchSize, verbose=(rank == 0 and not opts.quiet), beta1=opts.beta1,
-                        beta2=opts.beta2, epsilon=opts.epsilon)
+                        beta2=opts.beta2, epsilon=opts.epsilon, emaDecay=opts.emaDecay)
     cfg["param_count"] = net.paramCount()
     if rank == 0:
         dump_config(cfg, opts.cfg_file)
 
     first_epoch = run_dir.read_int("epoch", -1) + 1
-    if os.path.exists(opts.in_file):                  # resume: optimiser state, then the stack
+    if os.path.exists(opts.in_file):                  # resume: optimiser state, then the stack (then the average)
         with open(opts.in_file, "rb") as fid:
             optimizer.fromFile(fid)
             optimizer.alpha = optimizer.alpha / (opts.anneal ** first_epoch)
             net.fromFile(fid)
+            if optimizer.average is not None:
+                optimizer.averageFromFile(fid)
 
     for epoch in range(first_epoch, opts.epochs):
         order = np.random.permutation(opts.numFiles) + 1
@@ -301,7 +313,8 @@ def test(opts, rank=0, world=1):
     """Forward-only pass of a trained model over data files; writes Kaldi arks + pickles
     (runNNet.py:208-237, analysis-utils/writeLikelihoods.py).  --maxUtts utterances per forward call (0: one, the
     reference's loop); rank `rank` of `world` processes (run() passes them under torchrun) writes its own share of
-    the files (parallel.rank_files)."""
+    the files (parallel.rank_files).  A model trained with --emaDecay writes the arks from its weight average (the
+    third pickle of params.pk), or from its last weights with --lastWeights."""
     trained = trained_config(opts.cfg_file)
     logging.getLogger().info("Running on %s" % get_hostname())
     # the intermediate CTC loss only trains, unless the net conditions its upper layers on it
@@ -316,6 +329,8 @@ def test(opts, rank=0, world=1):
     with open(trained.in_file, "rb") as fid:
         pickle.load(fid)                              # optimiser state: not needed here
         net.fromFile(fid)
+        if trained.emaDecay > 0.0 and not getattr(opts, "lastWeights", False):
+            net.fromFile(fid)                         # the average, in the stack's format
     loader = dl.DataLoader(opts.dataDir, trained.rawDim, trained.inputDim, opts.alisDir or opts.dataDir)
     out_dir = getattr(opts, "outDir", None) or os.path.join(opts.output_dir, "ctc_loglikes")
     os.makedirs(out_dir, exist_ok=True)

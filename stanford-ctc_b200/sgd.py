@@ -20,6 +20,10 @@ sgd.py:24-26,143-158, state `gradt`) or 'adam' (state `moment1`, `moment2`; beta
 in include/ctcb200.h.  The adaptive rules read the step number t from the same device counter (allocated here when
 the net has no dropout), so graph replays see the current step.  The states follow the flat vector, so a net with
 layer normalisation simply has its [gamma, beta] pairs in them too.
+`emaDecay` = d in (0, 1) keeps an exponential moving average of the weights on the device, `average` (a [W, b]
+FlatList of one flat vector, filled with the net's weights when the SGD is built): after each update,
+a <- w + d_t (a - w) with d_t = min(d, 1 - 1/t) for the same counter t (ctcb_ema_update_f32), so it is the mean of the
+iterates until 1 - 1/t reaches d and an EMA after that.  0 (the default) keeps no average and launches nothing for it.
 """
 import logging
 import pickle
@@ -59,9 +63,11 @@ class SGD:
 
     def __init__(self, model, maxBatch, alpha=1e-2, optimizer='nesterov',
                  momentum=0.9, maxGradNorm=1500, batchSize=1, verbose=True, bucketPool=16,
-                 beta1=0.9, beta2=0.999, epsilon=1e-8):
+                 beta1=0.9, beta2=0.999, epsilon=1e-8, emaDecay=0.0):
         if optimizer not in OPTIMIZERS:          # ctc/sgd.py:27
             raise ValueError("optimizer=%r: one of %s" % (optimizer, ", ".join(sorted(OPTIMIZERS))))
+        if not 0.0 <= emaDecay < 1.0:            # NaN too
+            raise ValueError("emaDecay=%r must be in [0, 1)" % (emaDecay,))
         if optimizer == "adam":
             for name, beta in (("beta1", beta1), ("beta2", beta2)):
                 if not 0.0 <= beta < 1.0:
@@ -98,10 +104,18 @@ class SGD:
             self._flat[name] = torch.zeros(model.nparams, dtype=torch.float32, device=model.dev)
             setattr(self, name, FlatList(model._views(self._flat[name]), self._flat[name]))
         self._vflat = self._flat.get("velocity")
+        # the weight average, started from the net's current weights so that a first step that is skipped still
+        # leaves weights in it
+        self.emaDecay = float(emaDecay)
+        self._avg, self.average = None, None
+        if self.emaDecay > 0.0:
+            self._avg = model.params.clone()
+            self.average = FlatList(model._views(self._avg), self._avg)
         # the optimisation step on the device: the dropout counter when the net has one, else one of our own where the
-        # rule reads t (a Nesterov step on a net without dropout needs none and launches nothing for it)
+        # rule or the average reads t (a Nesterov step on a net without dropout and without an average needs none and
+        # launches nothing for it)
         self._step = model.dropoutStep
-        if self._step is None and optimizer != "nesterov":
+        if self._step is None and (optimizer != "nesterov" or self._avg is not None):
             self._step = torch.zeros(1, dtype=torch.int64, device=model.dev)
         self._gnorm2 = model._gnorm2          # lives in the 8-float record behind the flat gradient
         self._scratch = torch.zeros(8192, dtype=torch.uint8, device=model.dev)
@@ -128,7 +142,6 @@ class SGD:
         pickle.dump([self.it, self.costt, self.expcost, pack_state(self.optimizer, pairs)], fid)
 
     def fromFile(self, fid):
-        torch = self._torch
         try:
             params = pickle.load(fid)
         except UnicodeDecodeError:
@@ -148,9 +161,30 @@ class SGD:
         if self._step is not None:      # a resumed run draws the masks and takes the steps an uninterrupted one would
             self._step.fill_(int(it))
         for name, stack in states.items():
-            for (w, b), (wi, bi) in zip(getattr(self, name), stack):
-                w.copy_(torch.from_numpy(np.ascontiguousarray(wi, dtype=np.float32).reshape(tuple(w.shape))))
-                b.copy_(torch.from_numpy(np.ascontiguousarray(bi, dtype=np.float32).reshape(tuple(b.shape))))
+            self._copy_pairs(getattr(self, name), stack)
+
+    def _copy_pairs(self, views, stack):
+        torch = self._torch
+        for (w, b), (wi, bi) in zip(views, stack):
+            w.copy_(torch.from_numpy(np.ascontiguousarray(wi, dtype=np.float32).reshape(tuple(w.shape))))
+            b.copy_(torch.from_numpy(np.ascontiguousarray(bi, dtype=np.float32).reshape(tuple(b.shape))))
+
+    def averageToFile(self, fid):
+        """The weight average in NNet.toFile's format (a pickled list of [w, b] host arrays), so that NNet.fromFile
+        loads it as a net's weights.  runNNet writes it as the third pickle of params.pk."""
+        pickle.dump([[w.cpu().numpy(), b.cpu().numpy()] for w, b in self.average], fid)
+
+    def averageFromFile(self, fid):
+        """Reads averageToFile's pickle into the average.  At the end of the file (a checkpoint written without an
+        average) the average starts again from the net's current weights."""
+        try:
+            stack = pickle.load(fid)
+        except EOFError:
+            self._avg.copy_(self.model.params)
+            return
+        self.model.check_pair_count(stack, self.average, "weight average")
+        self.model.check_shapes(stack, self.average, "weight average")
+        self._copy_pairs(self.average, stack)
 
     # ------------------------------------------------------------------ one optimisation step
     def step_device(self, batch, mom):
@@ -164,7 +198,7 @@ class SGD:
             return self._step_eager(batch, mom)
         import ctypes
         key = (id(batch), batch.B, batch.Tmax, float(mom), float(self.alpha), float(self.maxGNorm), stream,
-               self.optimizer, float(self.beta1), float(self.beta2), float(self.epsilon))
+               self.optimizer, float(self.beta1), float(self.beta2), float(self.epsilon), self.emaDecay)
         g = self._graphs.get(key)
         if g is None:
             seen = self._graph_seen.get(key, 0)
@@ -198,8 +232,9 @@ class SGD:
             check(lib.ctcb_axpy_f32(ptr(m.params), ptr(self._vflat), float(mom), m.nparams, stream))
 
     def _update(self, mom, stream):
-        """Global norm of the (reduced) gradient, then the rule's fused clip and update; a step whose utterances were
-        all skipped (n_valid = 0, the first float of m.stats) changes nothing but Nesterov's undo of the look-ahead."""
+        """Global norm of the (reduced) gradient, then the rule's fused clip and update, then the weight average; a step
+        whose utterances were all skipped (n_valid = 0, the first float of m.stats) changes nothing but Nesterov's undo
+        of the look-ahead."""
         m = self.model
         # gnorm over all parameters as one vector                       sgd.py:103-107
         check(lib.ctcb_sumsq_f32(ptr(m.grads), m.nparams, ptr(self._gnorm2), ptr(self._scratch), stream))
@@ -217,6 +252,9 @@ class SGD:
                                          ptr(m.grads), m.nparams, float(self.alpha), float(self.beta1),
                                          float(self.beta2), float(self.epsilon), float(self.maxGNorm),
                                          ptr(self._gnorm2), ptr(m.stats), ptr(self._step), stream))
+        if self._avg is not None:
+            check(lib.ctcb_ema_update_f32(ptr(self._avg), ptr(m.params), m.nparams, self.emaDecay, ptr(m.stats),
+                                          ptr(self._step), stream))
 
     def _step_eager(self, batch, mom):
         m = self.model
